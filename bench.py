@@ -1,7 +1,8 @@
 #!/usr/bin/env python
 """bench.py -- separated-audio-seconds per second of the Conv-TasNet path (forward + SI-SDR/PIT loss).
 
-    python bench.py --gpus N --steps K --warmup W            # our sm_100a path (one process per GPU under torchrun)
+    python bench.py --gpus N --steps K --warmup W            # our sm_90a path (one process per GPU under torchrun)
+    python bench.py --steps K --dump-outputs DIR             # also write the last timed step's outputs as DIR/<name>.npy
     python bench.py --impl reference --steps K --warmup W    # the reference algorithm on the host CPU cores (oracle port)
     python bench.py --config cfg4                            # DPRNN-TasNet (segment / overlap-add path), its own line
     python bench.py --train [--n-sources 3 --batch 8]        # the training step alone, its own line
@@ -59,7 +60,11 @@ def parse():
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--no-train-block", action="store_true")
     ap.add_argument("--train", action="store_true", help="time the TRAINING step only; prints its own line")
+    ap.add_argument("--dump-outputs", default=None, metavar="DIR",
+                    help="after the timed steps, write what the last timed step returned (estimates, loss, permutation) as DIR/<name>.npy")
     a = ap.parse_args()
+    if a.dump_outputs and a.train:
+        ap.error("--dump-outputs records the forward benchmark's outputs; it does not apply to --train")
     d = {"cfg2": (32, 4.0, 8000, 2), "cfg3": (8, 4.0, 8000, 3), "cfg4": (16, 4.0, 8000, 2), "cfg5": (16, 8.0, 16000, 4)}[a.config]
     a.batch = a.batch if a.batch is not None else d[0]
     a.seconds = a.seconds if a.seconds is not None else d[1]
@@ -74,11 +79,11 @@ def peaks():
         p = json.load(open(path))
         return dict(hbm=p["hbm_gbs"], bf16_burst=p["bf16_tflops"], bf16_sustained=p.get("bf16_tflops_sustained", p["bf16_tflops"]),
                     source="measured (MEASURED_PEAKS.json)")
-    return dict(hbm=6650.0, bf16_burst=1590.0, bf16_sustained=1400.0, source="fallback (B200_PROFILING.md)")
+    return dict(hbm=3350.0, bf16_burst=989.0, bf16_sustained=989.0, source="NVIDIA H100 SXM data sheet (dense, 700 W)")
 
 
 class ClockSampler:
-    """nvidia-smi clocks / throttle reasons DURING the timed region (B200_PROFILING.md recipe)."""
+    """nvidia-smi clocks / throttle reasons DURING the timed region."""
     Q = ("clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.hw_slowdown,clocks_event_reasons.hw_thermal_slowdown,"
          "clocks_event_reasons.sw_thermal_slowdown,clocks_event_reasons.sw_power_cap")
 
@@ -244,6 +249,33 @@ def cuda_time(fn, steps, torch, D, dev, sampler=None):
     return D.max_over_ranks(ms_local, dev), ms_local, ret
 
 
+DUMP_LIMIT = 64 << 20
+
+
+def dump_outputs(path, last):
+    """Writes the arrays the timed path handed its caller in its last step: the separated estimates (B, S, T) as float32 and
+    the PIT loss and permutation as float64, one DIR/<name>.npy each (8.2 MB at cfg2; the inputs are seeded, so two builds run
+    with the same arguments can be compared output for output).  Estimates larger than the 64 MB budget are replaced by a fixed,
+    seeded sample: estimates_sample.npy (float32) and the flat indices it was taken at, estimates_sample_index.npy (float64)."""
+    import numpy as np
+    os.makedirs(path, exist_ok=True)
+    for name, t in last.items():
+        a = t.detach().cpu().numpy()
+        if name != "estimates":
+            np.save(os.path.join(path, name + ".npy"), a.astype(np.float64))
+            continue
+        a = a.astype(np.float32)
+        if a.nbytes <= DUMP_LIMIT - (1 << 20):
+            np.save(os.path.join(path, name + ".npy"), a)
+            continue
+        k = (DUMP_LIMIT - (1 << 20)) // 12          # float32 value + float64 index per sampled element
+        stride = -(-a.size // k)
+        start = int(np.random.default_rng(111).integers(stride))
+        idx = np.arange(start, a.size, stride, dtype=np.int64)
+        np.save(os.path.join(path, name + "_sample.npy"), a.reshape(-1)[idx])
+        np.save(os.path.join(path, name + "_sample_index.npy"), idx.astype(np.float64))
+
+
 def build_convtasnet(args, dev, torch, S):
     from ctn_b200.models.conv_tasnet import ConvTasNet
     torch.manual_seed(111)  # reference default seed (train.sh:59); default init = the reference's default init
@@ -394,9 +426,13 @@ def main():
     out_h = torch.empty(B, S, T).pin_memory()
     mixture_d, sources_d = mixture_h.to(dev), sources_h.to(dev)
 
+    last = {}
+
     def step_resident():
         out = model(mixture_d)
-        return crit(out, sources_d)
+        loss, perm = crit(out, sources_d)
+        last.update(estimates=out, loss=loss, perm=perm)
+        return loss, perm
 
     if args.config == "cfg4":
         loss_pin = torch.empty(1).pin_memory()
@@ -432,6 +468,8 @@ def main():
         N.ctn_profile_enable(0)
         with ClockSampler(local_rank) as clk:
             ms, ms_local, _ = cuda_time(step_resident, args.steps, torch, D, dev)
+        if args.dump_outputs and rank == 0:
+            dump_outputs(args.dump_outputs, last)
         # ---- timed: end to end ----------------------------------------------------------------------------------
         for _ in range(2):
             step_e2e()
@@ -510,7 +548,7 @@ def main():
         roof["step"] = {"ms": ms / args.steps, "moved_bytes_model": step_bytes,
                         "hbm_frac_on_moved_bytes": step_bytes / (ms / args.steps * 1e-3) / 1e9 / pk["hbm"]}
     else:
-        # cfg4: the step is 12 bi-LSTM + projection calls (tcgen05 kernel, csrc/ctn_lstm.cu) plus HBM-bound glue (segment, overlap-add,
+        # cfg4: the step is 12 bi-LSTM + projection calls (csrc/ctn_lstm.cu) plus HBM-bound glue (segment, overlap-add,
         # gLN + residual + path swap).  Dominant kernel = the LSTM: timed alone here at the intra-chunk shape of the step.
         from ctn_b200.models import dprnn as dprnn_mod
         F_, K_, P_, H_ = CFG4["sep_bottleneck_channels"], CFG4["sep_chunk_size"], CFG4["sep_hop_size"], CFG4["sep_hidden_channels"]
@@ -547,11 +585,11 @@ def main():
                         ms_lib, _, _ = cuda_time(step_resident, 2, torch, D, dev)
                 finally:
                     dprnn_mod.NATIVE_LSTM = True
-            roof = {"kernel": "k_bilstm_pair (bi-LSTM recurrence + 2H->F projection, 2-CTA clusters, h in tensor memory; 12 calls per step)",
-                    "bound": "tensor", "achieved": ach, "peak": tf32_peak, "unit": "TFLOP/s", "frac": ach / tf32_peak, "traffic": None,
+            roof = {"kernel": "k_bilstm (bi-LSTM recurrence + 2H->F projection, 3xTF32 wgmma; 12 calls per step)",
+                    "bound": "tensor", "achieved": ach, "peak": pk["bf16_sustained"] / 2, "unit": "TFLOP/s", "frac": ach / (pk["bf16_sustained"] / 2), "traffic": None,
                     "ms_per_call": ms_lstm, "algorithmic_flops_per_call": flops,
-                    "peak_note": "fp16 dense = bf16_tflops_sustained of measured (MEASURED_PEAKS.json); algorithmic flops (the 3-pass hi/lo split issues "
-                                 "3x that); a recurrence: 250 dependent steps per call, " + str(4 * ((B * Sn + 127) // 128)) + " CTAs",
+                    "peak_note": f"TF32 dense = bf16_tflops_sustained/2 of {pk['source']}; algorithmic flops (the 3-pass hi/lo split issues 3x that); "
+                                 "a recurrence: 250 dependent steps per call",
                     "glue_bytes_per_step": glue_bytes, "glue_ideal_ms_at_peak": glue_bytes / (pk["hbm"] * 1e9) * 1e3,
                     "library_lstm_ms_per_step": (ms_lib / 2 if ms_lib == ms_lib else None), "native_lstm_ms_per_step": ms / args.steps,
                     "note": "library_lstm_ms_per_step = the same step with cuDNN's LSTM (IEEE fp32, as parity with the reference needs) + a library GEMM"}
@@ -562,8 +600,8 @@ def main():
         "metric": METRIC if args.config == "cfg2" else METRIC.replace("Conv-TasNet 2spk 4s@8kHz", workload_config(args, world)["workload"].split(",")[0]),
         "value": value, "unit": "audio-sec/s", "n_gpus": world, "steps": args.steps, "warmup": max(args.warmup, 3),
         "ms_per_step": ms / args.steps, "higher_is_better": True, "scaling": "weak", "vs_baseline": None,
-        "dtype": {"fp32": "f32 (CUDA-core FFMA)", "tf32x3": "f32 via 3xTF32 split on tcgen05, fp32 accumulate", "tf32": "tf32 (single pass), fp32 accumulate",
-                  "f16x3": "f32 via 3xFP16 split on tcgen05 (kind::f16), fp32 accumulate"}[math_name],
+        "dtype": {"fp32": "f32 (CUDA-core FFMA)", "tf32x3": "f32 via 3xTF32 split on wgmma, fp32 accumulate", "tf32": "tf32 (single pass), fp32 accumulate",
+                  "f16x3": "f32 via 3xFP16 split on wgmma (f16), fp32 accumulate"}[math_name],
         "data": "synthetic", "config": workload_config(args, world),
         "detail": {"math": math_name, "parallelism": f"batch shards x{world}, no data-path collective in the forward",
                    "value_timing": "CUDA events, stage timers off, max over ranks"},

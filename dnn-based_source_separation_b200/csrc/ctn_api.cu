@@ -103,12 +103,12 @@ struct Carver {
 struct TcnWs {
   double* stats;  // [2*RX][B][2]
   std::vector<FoldedConv> folds;  // per block, (Bc+Sc) rows
-  std::vector<float*> wimg1, wimg2;  // per block: tcgen05 weight images of the two pointwise convs (math != fp32)
+  std::vector<float*> wimg1, wimg2;  // per block: tensor-core weight images of the two pointwise convs (math != fp32)
   std::vector<float*> rblk;          // per block: raw [out;skip] contraction output r_i (B, Bc+Sc, pitch), kept for the
                                      // deferred skip reduction (the skip accumulator is written once, at the end)
   float *x, *skip, *h, *u, *outraw;
   void* causal_ws;  // causal (cLN) models: scratch of the un-fused pipeline (ctn_causal.cu)
-  float* xalt;  // second residual-stream buffer (tcgen05 modes ping-pong x between blocks: the update is fused into pw1)
+  float* xalt;  // second residual-stream buffer (tensor-core modes ping-pong x between blocks: the update is fused into pw1)
   // fp16-piece mode: activation envelope (ctn_act_scales)
   std::vector<float*> dwp;  // per block: packed depthwise parameters [ceil16(H)][8]
   float* scales;            // [2*RX + 1] power-of-two operand scales (+ 3*RX floats of scratch)
@@ -169,7 +169,6 @@ static void carve_tcn(Carver& cv, const ctn_config_t* c, int B, int pitch, TcnWs
 
 static int pw_dispatch(const PwArgs& a, int pro, int epi, int math, cudaStream_t st) {
   if (math == CTN_MATH_FP32) return ctn_pw_simt(a, pro, epi, st);
-  if (math == CTN_MATH_F16X3 && ctn_pw_tma_supported(a, pro, epi)) return ctn_pw_tma(a, pro, epi, st);
   return ctn_pw_umma(a, pro, epi, math, st);
 }
 
@@ -184,7 +183,7 @@ static int run_tcn(const ctn_config_t* c, const ctn_block_params_t* blocks, TcnW
   const int R = c->num_blocks, X = c->num_layers, Bc = c->bottleneck, H = c->hidden, Sc = c->skip;
   if (c->causal)  // cLN: cumulative statistics -> un-fused pipeline in the reference's operation order
     return ctn_causal_tcn(c, blocks, ws->x, ws->skip, ws->h, ws->u, B, frames, pitch, ws->causal_ws, st);
-  // weight preparation for all blocks: gLN2 folding, then (tcgen05 modes) the swizzled hi/lo operand images
+  // weight preparation for all blocks: gLN2 folding, then (tensor-core modes) the swizzled hi/lo operand images
   {
     StageTimer tm(CTN_ST_PREP, st);
     std::vector<FoldJob> fj;
@@ -239,7 +238,7 @@ static int run_tcn(const ctn_config_t* c, const ctn_block_params_t* blocks, TcnW
       // K_A: h = PReLU(W1 x + b1), stats1
       PwArgs a;
       memset(&a, 0, sizeof(a));
-      // tcgen05 modes: the residual stream ping-pongs between ws->x and ws->xalt; block i >= 1 applies block i-1's
+      // tensor-core modes: the residual stream ping-pongs between ws->x and ws->xalt; block i >= 1 applies block i-1's
       // update x += rstd2*r[:Bc] + c inside its own producer (PRO_RES) -- no separate finishing pass over x
       const bool fuse_res = c->math != CTN_MATH_FP32;
       float* xbuf[2] = {ws->x + go * Bc, ws->xalt + go * Bc};
@@ -263,7 +262,7 @@ static int run_tcn(const ctn_config_t* c, const ctn_block_params_t* blocks, TcnW
         a.res_stats = ws->stats + (size_t)(2 * (i - 1) + 1) * B * 2 + 2 * g0; a.res_n = (double)H * (double)frames; a.res_eps = c->eps_tcn;
         a.res_x_out = hooks ? hooks->x_keep[i] : xbuf[i & 1];
       }
-      if (hooks && !(c->math == CTN_MATH_F16X3 && ctn_pw_tma_supported(a, pro1, EPI_H))) return CTN_EUNSUPPORTED;
+      if (hooks && c->math != CTN_MATH_F16X3) return CTN_EUNSUPPORTED;
       { StageTimer tm(CTN_ST_PW1, st); CTN_TRY(pw_dispatch(a, pro1, EPI_H, c->math, st)); }
       const int Mt = has_out ? Bc + Sc : Sc;
       float* rb = ws->rblk[i] + go * Mt;
@@ -272,7 +271,7 @@ static int run_tcn(const ctn_config_t* c, const ctn_block_params_t* blocks, TcnW
       // stand-alone depthwise stage
       const bool dw_fusable = c->sep_kernel == 3 && (dilation == 1 || dilation == 2 || dilation % 4 == 0);
       if (c->math != CTN_MATH_FP32 && dw_fusable) {
-        // K_BC fused (tcgen05): the producer warps compute u = PReLU(dwconv(gLN1(h))) (+stats2) on the fly and feed
+        // K_BC fused (tensor-core modes): the producer warps compute u = PReLU(dwconv(gLN1(h))) (+stats2) on the fly and feed
         // it straight to the tensor core; u never touches HBM.  r = [Wo;Ws] diag(gamma2) u
         StageTimer tm(CTN_ST_PW2, st);
         memset(&a, 0, sizeof(a));
@@ -283,7 +282,7 @@ static int run_tcn(const ctn_config_t* c, const ctn_block_params_t* blocks, TcnW
         if (scaled) { a.act_scale = ws->scales + 2 * i + 1; a.dw_params = ws->dwp[i]; }
         if (hooks) {
           a.dw_in_slope = p.prelu1; a.dw_u_pre_out = hooks->upre[i];
-          if (!(c->math == CTN_MATH_F16X3 && ctn_pw_tma_supported(a, PRO_DW, EPI_RAW))) return CTN_EUNSUPPORTED;
+          if (c->math != CTN_MATH_F16X3) return CTN_EUNSUPPORTED;
         }
         CTN_TRY(pw_dispatch(a, PRO_DW, EPI_RAW, c->math, st));
       } else {
@@ -322,7 +321,7 @@ static int run_tcn(const ctn_config_t* c, const ctn_block_params_t* blocks, TcnW
   if (x_final) {
     const int n = R * X;
     float* xbuf[2] = {ws->x, ws->xalt};
-    float* xl = (c->math != CTN_MATH_FP32) ? xbuf[(n - 1) & 1] : ws->x;  // x_{n-1} (tcgen05 modes defer every update to the next block)
+    float* xl = (c->math != CTN_MATH_FP32) ? xbuf[(n - 1) & 1] : ws->x;  // x_{n-1} (tensor-core modes defer every update to the next block)
     if (c->math != CTN_MATH_FP32 && blocks[n - 1].out_w)
       CTN_TRY(ctn_finish_fwd(ws->rblk[n - 1], ws->folds[n - 1], ws->stats + (size_t)(2 * (n - 1) + 1) * B * 2, (double)H * (double)frames,
                              c->eps_tcn, xl, ws->skip, B, Bc, Sc, 1, 2 /* x rows only */, frames, pitch, st));
@@ -571,11 +570,11 @@ static int run_separator(const ctn_config_t* c, const ctn_params_t* p, ModelWs* 
   if (dec && !mask_out && mask_math == CTN_MATH_F16X3 && c->kernel_size == 16 && c->stride == 8) {
     PwArgs f = a;
     f.D = dec->out; f.dec_w = p->dec_w; f.dec_crop_left = dec->crop_left; f.dec_T_out = dec->T_out;
-    if (ctn_pw_tma_supported(f, PRO_PRELU, EPI_MASKDEC)) {
+    if (ctn_pw_maskdec_supported(f, mask_math)) {
       StageTimer tm(CTN_ST_MASK, st);
       cudaError_t e = cudaMemsetAsync(dec->out, 0, sizeof(float) * (size_t)B * S * dec->T_out, st);  // tile seams are red.add'ed
       if (e != cudaSuccess) return (int)e;
-      CTN_TRY(ctn_pw_tma(f, PRO_PRELU, EPI_MASKDEC, st));
+      CTN_TRY(ctn_pw_umma(f, PRO_PRELU, EPI_MASKDEC, mask_math, st));
       dec->fused = true;
       return CTN_OK;
     }
@@ -827,6 +826,6 @@ extern "C" int ctn_debug_pointwise(const float* A, const float* W, float* D, int
   float* wimg = (float*)(((uintptr_t)workspace + 255) & ~(uintptr_t)255);
   CTN_TRY(ctn_umma_build_wimg(W, M, K, math, wimg, st));
   a.wimg = wimg;
-  if (dbg) { a.dbg_idesc = dbg[0]; a.dbg_lbo_a = dbg[1]; a.dbg_sbo_a = dbg[2]; a.dbg_sbo_w = dbg[3]; }
+  if (dbg && (dbg[0] | dbg[1] | dbg[2] | dbg[3])) return CTN_EUNSUPPORTED;  // the wgmma kernels take no descriptor overrides
   return ctn_pw_umma(a, PRO_NONE, epi, math, st);
 }

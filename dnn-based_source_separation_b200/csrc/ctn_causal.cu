@@ -6,7 +6,7 @@
 //   h = PReLU(W1 x + b1)  [contraction, fused bias+PReLU epilogue]   -> cLN1 (step sums -> scan -> apply, in place)
 //   u = PReLU(dwconv_causal(h) + bd)                                  -> cLN2
 //   r = [Wo; Ws] u  [contraction]   ;   x += r[:Bc] + bo ; skip += r[Bc:] + bs
-// The contractions are the same tcgen05 / FFMA kernels as everywhere else; the rest are streaming kernels (HBM-bound).
+// The contractions are the same wgmma / FFMA kernels as everywhere else; the rest are streaming kernels (HBM-bound).
 // Note: the reference's own cLN cannot run on CUDA (its frame counter is built on the CPU, norm.py:83), so this path has
 // no GPU baseline in the reference at all.
 #include <string.h>

@@ -1,4 +1,4 @@
-// Shared device/host helpers for the Conv-TasNet sm_100a kernels.
+// Shared device/host helpers for the Conv-TasNet sm_90a kernels.
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>

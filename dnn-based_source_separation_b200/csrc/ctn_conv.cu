@@ -1,7 +1,7 @@
 // Plain depthwise-separable convolution of src/modules/conv.py:13-29 (DepthwiseSeparableConv1d: depthwise Conv1d(groups = C,
 // kernel K, stride, padding, dilation, bias) followed by a pointwise 1x1 Conv1d with bias).  Not on Conv-TasNet's hot path
 // (SURVEY.md 8a row a11'); exposed for API completeness.  The depthwise stage is an HBM-bound streaming kernel; the pointwise
-// stage reuses the dense-contraction kernels of the path (tcgen05 or FFMA, selected by `math`) on the padded layout.
+// stage reuses the dense-contraction kernels of the path (wgmma or FFMA, selected by `math`) on the padded layout.
 #include <string.h>
 #include "ctn_internal.h"
 

@@ -1,4 +1,4 @@
-// Depthwise-stage math shared by the fused depthwise + pointwise producers (ctn_umma.cu, ctn_pwtma.cu).
+// Depthwise-stage math shared by the fused depthwise + pointwise producers (ctn_umma.cu).
 #pragma once
 #include "ctn_common.cuh"
 
@@ -17,18 +17,10 @@ __device__ __forceinline__ float4 dw_channel(const float4 q0, const float4 q1, c
   constexpr int i2 = DCLS == 4 ? 8 : (DCLS == 2 ? 6 : 5);
   float o[4];
   if (INTERIOR) {
-    // packed fp32 (FFMA2): two time steps per instruction
     const float a0 = gsc * w0, a1 = gsc * w1, a2 = gsc * w2;
     const float cst = fmaf(gsh, (w0 + w1) + w2, bd);
-    const float2 A0 = make_float2(a0, a0), A1 = make_float2(a1, a1), A2 = make_float2(a2, a2), C = make_float2(cst, cst);
 #pragma unroll
-    for (int e = 0; e < 4; e += 2) {
-      float2 r = __ffma2_rn(A0, make_float2(win[i0 + e], win[i0 + e + 1]), C);
-      r = __ffma2_rn(A1, make_float2(win[i1 + e], win[i1 + e + 1]), r);
-      r = __ffma2_rn(A2, make_float2(win[i2 + e], win[i2 + e + 1]), r);
-      o[e] = r.x;
-      o[e + 1] = r.y;
-    }
+    for (int e = 0; e < 4; ++e) o[e] = fmaf(a2, win[i2 + e], fmaf(a1, win[i1 + e], fmaf(a0, win[i0 + e], cst)));
   } else {
 #pragma unroll
     for (int e = 0; e < 4; ++e) {
@@ -54,10 +46,10 @@ __device__ __forceinline__ float4 dw_channel(const float4 q0, const float4 q1, c
     if (!INTERIOR && (tbase + e >= frames || !cvalid)) u = 0.f;
     o[e] = u;
   }
-  const float2 u01 = make_float2(o[0], o[1]), u23 = make_float2(o[2], o[3]);
-  ls = __fadd2_rn(ls, __fadd2_rn(u01, u23));
-  lss = __ffma2_rn(u01, u01, lss);
-  lss = __ffma2_rn(u23, u23, lss);
+  ls.x += o[0] + o[2];
+  ls.y += o[1] + o[3];
+  lss.x = fmaf(o[2], o[2], fmaf(o[0], o[0], lss.x));
+  lss.y = fmaf(o[3], o[3], fmaf(o[1], o[1], lss.y));
   return make_float4(o[0], o[1], o[2], o[3]);
 }
 

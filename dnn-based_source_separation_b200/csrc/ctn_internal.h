@@ -25,7 +25,7 @@ struct PwArgs {
   int B, M, K, frames, pitch;
   // prologue
   const float* pro_slope;  // PRO_PRELU / PRO_DW: PReLU slope (1)
-  // PRO_DW (tcgen05 path): A is h (B,K,pitch); the producer computes u = PReLU(dwconv3(gLN1(h)) + bd) on the fly
+  // PRO_DW (tensor-core path): A is h (B,K,pitch); the producer computes u = PReLU(dwconv3(gLN1(h)) + bd) on the fly
   const float* dw_norm_g;  // (K) gLN1 gamma
   const float* dw_norm_b;  // (K) gLN1 beta
   const float* dw_w;       // (K,3) depthwise taps
@@ -43,16 +43,16 @@ struct PwArgs {
   double n_in;             // EPI_HEAD: element count of a gLN group of the input
   float eps;               // EPI_HEAD
   double* stats_out;       // EPI_H: (B,2) += (sum, sumsq) over valid outputs
-  int store_pre;           // EPI_H (tcgen05 path only): store W A + bias (pre-activation) instead of PReLU(.); stats unchanged
+  int store_pre;           // EPI_H (tensor-core path only): store W A + bias (pre-activation) instead of PReLU(.); stats unchanged
   const float* wenc;       // EPI_MASK: encoder output (B, Nb, pitch)
   int Nb;                  // EPI_MASK: n_basis
   float* mask_out;         // EPI_MASK: optional raw mask output (B, M, pitch)
   int mask_logits;         // EPI_MASK: 1 = store the LOGITS (W A + bias) to D, no sigmoid, no w product (softmax masks take a second pass)
-  // EPI_MASKDEC (TMA-fed kernel): mask 1x1 + sigmoid + w*mask + transposed-conv decoder + crop in one epilogue; w_hat is never
+  // EPI_MASKDEC: mask 1x1 + sigmoid + w*mask + transposed-conv decoder + crop in one epilogue; w_hat is never
   // materialised.  D = estimates (B, M/Nb, dec_T_out) contiguous, ZERO-initialised by the caller (tile seams are red.add'ed)
   const float* dec_w;      // (Nb, 1, 16) decoder basis, kernel 16 / stride 8
   int dec_crop_left, dec_T_out;
-  // PRO_RES (tcgen05 path): the operand is the UPDATED residual stream  x_new = A + rstd*res_r[:K] + (v1 - mean*rstd*v2)
+  // PRO_RES (tensor-core path): the operand is the UPDATED residual stream  x_new = A + rstd*res_r[:K] + (v1 - mean*rstd*v2)
   // (the deferred gLN2 of the previous block); CTAs with n-tile 0 also store x_new to res_x_out (ping-pong buffer).
   const float* res_r;       // (B, res_Mt, pitch) raw [out;skip] contraction of the previous block; rows [0,K) are used
   int res_Mt;
@@ -62,27 +62,28 @@ struct PwArgs {
   double res_n;
   float res_eps;
   float* res_x_out;         // (B, K, pitch)
-  // tcgen05 path only
+  // tensor-core path only
   const float* wimg;       // pre-swizzled hi/lo weight images (ctn_umma_build_wimg)
   // fp16-piece mode: power-of-two scale of the activation operand (device scalar, nullable = 1), chosen per forward from a
   // bound on |operand| derived from the weights alone (ctn_act_scales) so that fp16 can never saturate; undone in the epilogue
   const float* act_scale;
-  const float* dw_params;  // PRO_DW, TMA-fed kernel: packed per-channel parameters [ceil16(K)][8] (ctn_act_scales)
-  // PRO_DW, training forward (TMA-fed kernel): A holds the PRE-activation h_pre = W1 x + b1 (the backward needs it), the producer
+  const float* dw_params;  // PRO_DW: packed per-channel parameters [ceil16(K)][8] (ctn_act_scales)
+  // PRO_DW, training forward : A holds the PRE-activation h_pre = W1 x + b1 (the backward needs it), the producer
   // applies PReLU(dw_in_slope) on load; the depthwise pre-activation u_pre is stored to dw_u_pre_out (B, K, pitch)
   const float* dw_in_slope;
   float* dw_u_pre_out;
-  uint32_t dbg_idesc, dbg_lbo_a, dbg_sbo_a, dbg_sbo_w;  // 0 = defaults (descriptor probing from the debug entry)
 };
 
 // fp32 CUDA-core path (ctn_tcn_simt.cu)
 int ctn_pw_simt(const PwArgs& a, int pro, int epi, cudaStream_t st);
-// tcgen05 path (ctn_umma.cu); math = CTN_MATH_TF32X3 / CTN_MATH_TF32
+// wgmma tensor-core path (ctn_umma.cu); math = CTN_MATH_TF32X3 / CTN_MATH_TF32 / CTN_MATH_F16X3
 int ctn_pw_umma(const PwArgs& a, int pro, int epi, int math, cudaStream_t st);
+// EPI_MASKDEC (PRO_PRELU) applies to this contraction: fp16-piece mode, n_basis a multiple of 128, decoder kernel 16 / stride 8 (caller)
+int ctn_pw_maskdec_supported(const PwArgs& a, int math);
 size_t ctn_umma_wimg_bytes(int M, int K, int math);
 int ctn_umma_build_wimg(const float* W, int M, int K, int math, float* wimg, cudaStream_t st);
 
-// tcgen05 weight gradient of a 1x1 conv (ctn_wgrad_umma.cu): dW (M,K) += sum_{b,t} dY[b][m][t] X[b][k][t]; rows
+// wgmma weight gradient of a 1x1 conv (ctn_wgrad_umma.cu): dW (M,K) += sum_{b,t} dY[b][m][t] X[b][k][t]; rows
 // [0,split_row) -> dWa, rest -> dWb (nullable).  dW must be zero-initialised by the caller (split-K partials are added).
 int ctn_wgrad_umma(const float* dy, size_t dy_bs, const float* x, size_t x_bs, float* dWa, float* dWb, int split_row, int M,
                    int K, int B, int frames, int pitch, int math, cudaStream_t st);
@@ -96,10 +97,6 @@ struct WimgJob { const float* W; float* wimg; int M, K; };
 #define CTN_MAX_JOBS 48
 int ctn_fold_batch(const FoldJob* jobs, int n, cudaStream_t st);
 int ctn_umma_build_wimg_batch(const WimgJob* jobs, int n, int math, cudaStream_t st);
-
-// TMA-fed tcgen05 kernels of the fp16-piece mode (ctn_pwtma.cu): pw1 (PRO_RES / PRO_NONE + EPI_H) and pw2 (PRO_DW + EPI_RAW)
-int ctn_pw_tma_supported(const PwArgs& a, int pro, int epi);
-int ctn_pw_tma(const PwArgs& a, int pro, int epi, cudaStream_t st);
 
 // Activation envelope of the fp16-piece mode.  Per residual block i the two operands that meet the tensor core as fp16
 // pieces are x_i (pw1) and u_i (fused depthwise output, pw2); the mask contraction sees PReLU(skip sum).  From the weights

@@ -1,4 +1,4 @@
-// CUDA-core (exact fp32 FFMA) implementation of the TCN stages + the stages shared with the tcgen05 path
+// CUDA-core (exact fp32 FFMA) implementation of the TCN stages + the stages shared with the wgmma path
 // (weight folding, depthwise stage, finishing, pitch copies).
 //
 // Per ResidualBlock1d (src/models/tdcn.py:107-147 + 177-196), with d = dilation:

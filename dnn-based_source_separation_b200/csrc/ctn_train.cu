@@ -3,7 +3,7 @@
 // (egs/wsj0-mix/common/src/driver.py:146-150) for the modules of src/models/conv_tasnet.py, src/models/tdcn.py,
 // src/models/filterbank.py and src/modules/norm.py.
 //
-// Structure (first cut: correctness and full coverage; the dense contractions already run on the tcgen05 kernels):
+// Structure (first cut: correctness and full coverage; the dense contractions already run on the wgmma kernels):
 //   * every 1x1 convolution, forward or data-gradient (W^T dY), is ONE call of the pointwise contraction kernels of the
 //     inference path (ctn_pw_umma / ctn_pw_simt, raw epilogue) -- 3xTF32 on the tensor cores by default;
 //   * weight gradients dW = sum_{b,t} dY X^T reduce over B*frames (128 k at cfg2): a split-K FFMA kernel (k_wgrad,
@@ -912,7 +912,7 @@ extern "C" int ctn_convtasnet_fwd_train(const ctn_config_t* c, const ctn_params_
   const double nH = (double)H * (double)frames;
   // un-normalised operands (x_i, skip sum) without operand scales: tf32 pieces (8-bit exponent) in the fp16-piece mode
   const int fmath = c->math == CTN_MATH_F16X3 ? CTN_MATH_TF32X3 : c->math;
-  // fp16-piece mode: the TCN runs through the SAME fused TMA-fed kernels as inference (pw1 with the residual update fused,
+  // fp16-piece mode: the TCN runs through the SAME fused kernels as inference (pw1 with the residual update fused,
   // depthwise producer feeding the [out;skip] contraction), which additionally leave x_i, W1 x + b1 and the depthwise
   // pre-activation behind for the backward -- 2 launches per block instead of 7, no u / gLN2(u) round trips
   bool fused = false;

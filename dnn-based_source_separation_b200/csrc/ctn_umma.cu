@@ -1,25 +1,20 @@
-// tcgen05 (5th-gen tensor core) implementation of the dense 1x1 "pointwise" contractions of the Conv-TasNet path.
+// Hopper (sm_90a) wgmma implementation of the dense 1x1 "pointwise" contractions of the Conv-TasNet path.
 //
 //   D[b][n][t] = epi( sum_k W[n][k] * pro(A[b][k][t]) )        A: (B,K,pitch) fp32, time contiguous
 //
-// Orientation: TIME runs along the UMMA M dimension (TMEM lanes), output channels along N (TMEM columns):
-//   * the activation operand is consumed as an MN-major (time-contiguous) SWIZZLE_128B_BASE32B shared-memory tile, i.e. the
-//     (channels, time) tensor is used as it lies in HBM -- no transposition anywhere;
-//   * the weight operand is K-major (PyTorch (out,in,1) layout), pre-arranged once per forward into the exact
-//     swizzled shared-memory image so that one 1-D bulk async copy (TMA engine) brings a 32-channel slab in;
-//   * the epilogue reads a TMEM lane = one time step per thread, so every global store of a warp is a contiguous
-//     128-byte row segment of D.
-// fp32-parity numerics: x = hi + lo with 11-bit pieces, D = A_hi W_hi + A_lo W_hi + A_hi W_lo accumulated in fp32 in TMEM
-// (the dropped lo*lo term is ~2^-22 relative).  Pieces are TF32 ("3xTF32", kind::tf32) or FP16 ("3xFP16", kind::f16: twice
-// the tensor rate, half the shared memory per stage; weights pre-scaled per 16-row group, see wimg_f16_group) -- template
-// parameter F16.  The layouts described here are the TF32 ones; the FP16 ones are next to the code that stages them.
+// A CTA computes one tile of 128 time steps x 128 output channels.  Orientation: TIME runs along the wgmma M dimension
+// (two warpgroups of 64 rows each), output channels along N = 128:
+//   * the activation operand is formed by the CTA's own threads (global -> registers -> prologue -> hi/lo split) and stored
+//     K-major (rows of one time step, 32 input channels per slab) in the same swizzled layout as the weights;
+//   * the weight operand is K-major (PyTorch (out,in,1) layout), pre-arranged once per forward into the exact swizzled
+//     shared-memory image of a slab, so that one 1-D bulk async copy (TMA engine) brings a 32-channel slab in;
+//   * the accumulator stays in registers; the fused epilogue runs on it directly.
+// fp32-parity numerics: x = hi + lo with 11-bit pieces, D = A_hi W_hi + A_lo W_hi + A_hi W_lo accumulated in fp32 (the dropped
+// lo*lo term is ~2^-22 relative).  Pieces are TF32 ("3xTF32", SWIZZLE_128B rows of 32 x 4 B) or FP16 ("3xFP16", SWIZZLE_64B
+// rows of 32 x 2 B, twice the tensor rate, weights pre-scaled per 16-row group, see wimg_f16_group) -- template parameter F16.
 //
-// One persistent CTA per SM, warp-specialised:
-//   warps 0-3   epilogue  (TMEM -> registers -> fused epilogue -> coalesced global stores)
-//   warp  4     TMEM allocator + single-thread tcgen05.mma issuer
-//   warps 5-12  producers (global -> registers -> prologue + hi/lo split -> swizzled st.shared; one thread also issues
-//               the bulk copies of the weight slabs)
-// Pipelines: smem ring (full/empty mbarriers, tcgen05.commit frees a stage) and a 2-deep TMEM accumulator ring.
+// Pipeline: two shared-memory stages.  While the tensor core works on slab ks (wgmma is asynchronous), all 256 threads load
+// and stage slab ks + 1 and one thread issues the bulk copy of its weights.
 #include "ctn_internal.h"
 #include "ctn_umma_ptx.cuh"
 #include "ctn_dw_math.cuh"
@@ -29,604 +24,340 @@
 
 namespace {
 
-constexpr int TM = 128;       // time steps per tile (UMMA M)
-#ifndef CTN_KS
-#define CTN_KS 32
-#endif
-constexpr int KS = CTN_KS;    // input channels per smem slab.  32: 128-byte weight rows (SWIZZLE_128B), 2-3 stages;
-                              // 16: 64-byte rows (SWIZZLE_64B), 4-6 stages -- measured SLOWER (per-slab handshakes dominate)
-constexpr int A_BYTES = TM * KS * 4;  // 8 KB per precision
-constexpr int MAX_STAGES = 8;
-constexpr uint32_t W_LAYOUT = KS == 32 ? 2u : 4u;    // UMMA layout type of the weight operand (SWIZZLE_128B / SWIZZLE_64B)
-constexpr uint32_t W_SBO = KS == 32 ? 1024u : 512u;  // bytes between 8-row groups of the weight image
-constexpr int NUM_THREADS_DW = 21 * 32;   // PRO_DW kernels: 4 epilogue + 1 MMA + 16 producer warps (2 channels each)
-constexpr int NUM_THREADS_E8 = 17 * 32;   // other kernels: 4 + 1 + 8 producer warps + a second epilogue warpgroup (13-16)
-constexpr int NUM_THREADS_RES = 25 * 32;  // PRO_RES kernels (CTN_RES_WARPS16): 4 + 1 + 16 producer warps + second epilogue warpgroup (21-24)
-constexpr int F16_MAX_ROWS = 2048;  // fp16-piece mode: padded output channels whose scales fit the shared-memory table
-constexpr int SMEM_HEADER = 2048 + F16_MAX_ROWS * 4;  // barriers + tmem pointer, the epilogue parameter row, the fp16-mode output scales
-constexpr int SMEM_SCALES = 2048;   // byte offset of float[F16_MAX_ROWS]: power-of-two scale of every padded output channel of the
-                                    // contraction (F16 kernels), loaded ONCE per CTA (a per-item staging put a global-load latency
-                                    // on the epilogue's critical path: +0.9 us per item, 0.5 ms per step)
-constexpr int SMEM_PARAMS = 1024;   // byte offset of float[256] inside the header
+constexpr int TM = 128;        // time steps per tile (2 warpgroups x wgmma M = 64)
+constexpr int KS = 32;         // input channels per smem slab (128-byte tf32 rows / 64-byte fp16 rows)
+constexpr int NT = 128;        // output channels per tile (wgmma N)
+constexpr int THREADS = 256;   // 8 warps: warp w stages channels [4w, 4w+4) of every slab, lane l time steps [4l, 4l+4)
+constexpr int CPW = 4;         // channels of a slab per warp
+constexpr int STAGES = 2;
+constexpr int SMEM_HEADER = 1024;   // mbarriers
+constexpr int F16_MAX_ROWS = 2048;  // fp16-piece mode: padded output channels of one contraction (see eff_math)
 
-struct UmmaArgs {
+struct TcArgs {
   PwArgs a;
-  const float* wimg;  // [n_tiles][k_slabs][NPASS][n_tile*32] swizzled images
-  const float* oscale;  // fp16-piece mode: [n_tiles*n_tile] per-output-channel scale 2^-e (stored behind the images)
-  int n_tile, n_tiles, k_slabs, t_tiles, num_items, stages;
-  uint32_t stage_bytes, w_bytes;  // w_bytes: bytes per precision of a weight slab (n_tile*128)
-  uint32_t idesc, lbo_a, sbo_a, lbo_w, sbo_w, a_layout, w_layout;
-  int cluster, tiles_total, cluster_items, wsplit;  // 2 = CTA pair (cta_group::2 MMA, each CTA stages half of the weight slab); B*t_tiles; n_tiles*ceil(tiles/cluster)
-  uint32_t dbg;  // CTN_UMMA_DBG bits: 1 = no epilogue stores, 2 = no activation loads, 4 = no weight copies, 8 = no MMA
+  const float* wimg;    // [n_tiles][k_slabs][NPREC][NT*KS] swizzled images
+  const float* oscale;  // fp16-piece mode: [n_tiles*NT] per-output-channel scale 2^-e (stored behind the images)
+  int n_tiles, k_slabs, t_tiles;
+  int nt_per_cta;  // n-tiles a CTA walks back to back: 1, or all n-tiles of one source (EPI_MASKDEC)
 };
 
-// producer warps per prologue: the depthwise producer always runs 16; the residual-update producer (pw1, the second
-// largest kernel, latency-bound: 47 % issue-active) can run 8 or 16 -- compile-time switch CTN_RES_WARPS16
-#ifndef CTN_RES_WARPS16
-#define CTN_RES_WARPS16 0  // measured: 16 warps (72 registers) 3.66 ms vs 3.28 ms with 8 warps (96 registers) at cfg2
-#endif
-template <int PRO> struct Roles {
-  static constexpr int PROD_WARPS = (PRO == PRO_DW || (PRO == PRO_RES && CTN_RES_WARPS16)) ? 16 : 8;
-  static constexpr int EGROUPS = PRO == PRO_DW ? 1 : 2;
-  static constexpr int THREADS = (4 + 1 + PROD_WARPS + 4 * (EGROUPS - 1)) * 32;
-};
-static_assert(Roles<PRO_DW>::THREADS == NUM_THREADS_DW && Roles<PRO_NONE>::THREADS == NUM_THREADS_E8, "role layout");
-
-// debug timeline (CTN_UMMA_DBG bit 128): CTA 0 records globaltimer stamps per role and slab
-__device__ unsigned long long g_timeline[3 * 4096];
-__device__ __forceinline__ unsigned long long gtime() {
-  unsigned long long t;
-  asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t));
-  return t;
-}
-
-struct __align__(8) SmemHeader {
-  uint64_t full[MAX_STAGES];
-  uint64_t empty[MAX_STAGES];
-  uint64_t tfull[2];
-  uint64_t tempty[2];
-  uint32_t tmem_base;
-};
-
-template <int DCLS, bool INTERIOR, int CPW>
-__device__ __forceinline__ void dw_slab(const PwArgs& a, int b, int ks, int pw, int tbase, float2 mr1, float pslope, bool skip_loads,
-                                        bool prefetch_next, float4 (&v)[CPW], float2& dls, float2& dlss) {
+// u = PReLU(dwconv3(gLN1(h)) + bd) for this thread's 4 time steps of the CPW channels of warp pw in slab ks.
+// TRAIN: A holds the pre-activation of h; PReLU(dw_in_slope) is applied on load and the depthwise pre-activation goes to pre[].
+template <int DCLS, bool INTERIOR, bool TRAIN>
+__device__ __forceinline__ void dw_slab(const PwArgs& a, int b, int ks, int pw, int tbase, float2 mr1, float pslope, float4 (&v)[CPW],
+                                        float4 (&pre)[CPW], float2& dls, float2& dlss) {
   const int d = a.dw_dilation, pl = a.dw_pad_left;
   const int step = DCLS == 4 ? d : 4;
   const int first = DCLS == 4 ? tbase - pl : tbase - 4;
-  float4 q[CPW][3];
-  float pg[CPW], pb[CPW], pbd[CPW], pw0[CPW], pw1[CPW], pw2[CPW];
+  const float islope = TRAIN ? __ldg(a.dw_in_slope) : 0.f;
 #pragma unroll
   for (int j = 0; j < CPW; ++j) {
     const int c = ks * KS + pw * CPW + j;
     const int cc = INTERIOR ? c : (c < a.K ? c : a.K - 1);
     const float* hr = a.A + ((size_t)b * a.K + cc) * a.pitch;
+    float4 q[3];
 #pragma unroll
     for (int k = 0; k < 3; ++k) {
       int ts = first + k * step;
       if (!INTERIOR) ts = ts < 0 ? 0 : (ts > a.pitch - 4 ? a.pitch - 4 : ts);
-      q[j][k] = skip_loads ? make_float4(1.f, 2.f, 3.f, 4.f) : __ldg(reinterpret_cast<const float4*>(hr + ts));
+      q[k] = __ldg(reinterpret_cast<const float4*>(hr + ts));
+      if (TRAIN) { q[k].x = prelu_f(q[k].x, islope); q[k].y = prelu_f(q[k].y, islope); q[k].z = prelu_f(q[k].z, islope); q[k].w = prelu_f(q[k].w, islope); }
     }
-    pg[j] = __ldg(a.dw_norm_g + cc); pb[j] = __ldg(a.dw_norm_b + cc); pbd[j] = __ldg(a.dw_b + cc);
-    pw0[j] = __ldg(a.dw_w + cc * 3); pw1[j] = __ldg(a.dw_w + cc * 3 + 1); pw2[j] = __ldg(a.dw_w + cc * 3 + 2);
-  }
-  if (prefetch_next && INTERIOR) {
-    // pull the next slab's rows towards the SM while this slab is being computed (no register cost)
-#pragma unroll
-    for (int j = 0; j < CPW; ++j) {
-      const float* hr = a.A + ((size_t)b * a.K + (ks + 1) * KS + pw * CPW + j) * a.pitch;
-#pragma unroll
-      for (int k = 0; k < 3; ++k) asm volatile("prefetch.global.L2 [%0];" ::"l"(hr + first + k * step));
-    }
-  }
-#pragma unroll
-  for (int j = 0; j < CPW; ++j) {
-    const int c = ks * KS + pw * CPW + j;
-    const float gsc = pg[j] * mr1.y, gsh = pb[j] - mr1.x * mr1.y * pg[j];
-    v[j] = dw_channel<DCLS, INTERIOR>(q[j][0], q[j][1], q[j][2], gsc, gsh, pw0[j], pw1[j], pw2[j], pbd[j], pslope, first, step,
-                                      tbase, a.frames, c < a.K, dls, dlss);
+    const float pg = __ldg(a.dw_norm_g + cc), pb = __ldg(a.dw_norm_b + cc), pbd = __ldg(a.dw_b + cc);
+    const float w0 = __ldg(a.dw_w + cc * 3), w1 = __ldg(a.dw_w + cc * 3 + 1), w2 = __ldg(a.dw_w + cc * 3 + 2);
+    const float gsc = pg * mr1.y, gsh = pb - mr1.x * mr1.y * pg;
+    v[j] = dw_channel<DCLS, INTERIOR, TRAIN>(q[0], q[1], q[2], gsc, gsh, w0, w1, w2, pbd, pslope, first, step, tbase, a.frames, c < a.K,
+                                             dls, dlss, &pre[j]);
   }
 }
 
-// PAIR: the kernel runs as clusters of 2 CTAs driving cta_group::2 MMAs.  It is a template parameter (not a run-time
-// flag) because a kernel that contains cta_group::2 instructions can only be launched with an even cluster size.
-// F16: operands are staged as fp16 hi/lo pieces (kind::f16, "3xFP16"): A MN-major SWIZZLE_128B (atoms of 64 time steps x 8
-// channels), W K-major SWIZZLE_64B (rows of 32 channels = 64 bytes) -- both pinned on hardware by tools/umma_unit_f16.cu.
-// Half the shared-memory bytes per stage (4-deep ring at N = 256) and half the tensor-pipe time of the TF32 split.
-template <int PRO, int EPI, int NPASS, bool PAIR, bool F16>
-__global__ void __launch_bounds__(Roles<PRO>::THREADS, 1) k_pw_umma(const UmmaArgs g) {
-  constexpr int NPREC = NPASS == 3 ? 2 : 1;  // precisions staged per operand (hi [, lo])
-  constexpr int A_BYTES = F16 ? TM * KS * 2 : TM * KS * 4;  // bytes of one precision of the activation slab (shadows the tf32 constant)
-  static_assert(!F16 || (NPASS == 3 && !PAIR), "fp16 operands: 3-pass split, single-CTA only");
-  constexpr int EGROUPS = Roles<PRO>::EGROUPS;  // epilogue warpgroups (each covers all 128 TMEM lanes)
-  constexpr int PROD_WARPS = Roles<PRO>::PROD_WARPS;
-  constexpr int CPW = KS / PROD_WARPS;            // channels of a slab per producer warp (2 or 4)
+// F16 kernels fit two CTAs per SM (66 KB of shared memory each): measured 27.0 vs 36.7 ms per cfg2 step with one (H100 SXM, 700 W),
+// despite a few spilled registers under the 128-register cap.  The tf32 kernels need 130 KB, so one CTA per SM and no cap.
+template <int PRO, int EPI, int NPASS, bool F16, bool TRAIN>
+__global__ void __launch_bounds__(THREADS, F16 ? 2 : 1) k_pw_wgmma(const TcArgs g) {
+  constexpr int NPREC = NPASS == 3 ? 2 : 1;                   // precisions staged per operand (hi [, lo])
+  constexpr uint32_t ROWB = F16 ? 64u : 128u;                 // bytes of one operand row (32 channels)
+  constexpr uint32_t A_BYTES = TM * ROWB, W_BYTES = NT * ROWB;  // one precision of a slab
+  constexpr uint32_t STAGE_BYTES = NPREC * (A_BYTES + W_BYTES);
+  constexpr uint32_t LAYOUT = F16 ? ptx::SW64 : ptx::SW128;
   extern __shared__ uint8_t smem_raw[];
   const uint32_t raw = ptx::smem_u32(smem_raw);
-  const uint32_t base = (raw + 1023u) & ~1023u;  // SWIZZLE_128B atoms need 1024-byte alignment
+  const uint32_t base = (raw + 1023u) & ~1023u;  // swizzle atoms need 1024-byte alignment
   uint8_t* smem = smem_raw + (base - raw);
-  SmemHeader* hdr = reinterpret_cast<SmemHeader*>(smem);
+  uint64_t* wbar = reinterpret_cast<uint64_t*>(smem);
   const uint32_t stage0 = base + SMEM_HEADER;
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, wg = warp >> 2;
   const PwArgs& a = g.a;
-  constexpr bool pair = PAIR;  // CTA pair: cta_group::2 MMA (M = 256), each CTA stages its time tile and HALF of the weights
+
+  // item -> (group of output-channel tiles, time tile, sample); the groups of one time tile are adjacent (activations shared in L2)
+  const int n_groups = g.n_tiles / g.nt_per_cta;
+  const int ngrp = (int)blockIdx.x % n_groups;
+  const int tt = ((int)blockIdx.x / n_groups) % g.t_tiles;
+  const int b = (int)blockIdx.x / (n_groups * g.t_tiles);
+  // EPI_MASKDEC: decoder partial sums of the tile, [frame][tap], accumulated over the n-tiles of the source
+  float* dacc = reinterpret_cast<float*>(smem + SMEM_HEADER + STAGES * STAGE_BYTES);
 
   if (threadIdx.x == 0) {
-    for (int s = 0; s < g.stages; ++s) {
-      // pair mode: the peer's producers fill the PEER's full[s]; its relay warp forwards one arrival to the leader's
-      ptx::mbar_init(ptx::smem_u32(&hdr->full[s]), PROD_WARPS + 1 + ((pair && ptx::cluster_ctarank() == 0) ? 1 : 0));
-      ptx::mbar_init(ptx::smem_u32(&hdr->empty[s]), 1);
-    }
-    for (int i = 0; i < 2; ++i) {
-      ptx::mbar_init(ptx::smem_u32(&hdr->tfull[i]), 1);
-      ptx::mbar_init(ptx::smem_u32(&hdr->tempty[i]), pair ? 2 * 4 * EGROUPS : 128 * EGROUPS);
-    }
+    for (int s = 0; s < STAGES; ++s) ptx::mbar_init(ptx::smem_u32(&wbar[s]), 1);
     ptx::fence_mbar_init();
   }
-  if (warp == 4) {
-    if constexpr (pair) ptx::tmem_alloc2(ptx::smem_u32(&hdr->tmem_base), 512);
-    else ptx::tmem_alloc(ptx::smem_u32(&hdr->tmem_base), 512);
-  }
+  __syncthreads();
+
   // fp16 pieces: power-of-two scale of the activation operand (|operand| * act_s <= 2^15 by construction, ctn_act_scales),
   // undone together with the weight-group scales in the epilogue
   float act_s = 1.f;
-  if constexpr (F16) {
-    if (a.act_scale) act_s = __ldg(a.act_scale);
-    const float inv = 1.f / act_s;
-    float* ssc_all = reinterpret_cast<float*>(smem + SMEM_SCALES);
-    for (int i = threadIdx.x; i < g.n_tiles * g.n_tile; i += blockDim.x) ssc_all[i] = __ldg(g.oscale + i) * inv;
+  if (F16 && a.act_scale) act_s = __ldg(a.act_scale);
+  float pslope = 0.f;
+  if (PRO == PRO_PRELU || PRO == PRO_DW) pslope = __ldg(a.pro_slope);
+  const int tbase = tt * TM + lane * 4;  // first of this thread's 4 time steps
+  float2 mr1 = make_float2(0.f, 1.f), mr_res = make_float2(0.f, 1.f);
+  if (PRO == PRO_DW) mr1 = gln_mean_rstd(a.dw_stats_in + 2 * b, (double)a.K * (double)a.frames, a.dw_eps);
+  if (PRO == PRO_RES) mr_res = gln_mean_rstd(a.res_stats + 2 * b, a.res_n, a.res_eps);
+  int dcls = 4;
+  bool dw_interior = false;
+  if (PRO == PRO_DW) {
+    const int d = a.dw_dilation;
+    dcls = d >= 4 ? 4 : d;
+    const int reach = d >= 4 ? d : 4;  // furthest sample touched on either side of the tile
+    dw_interior = (tt * TM - reach >= 0) && (tt * TM + TM - 1 + reach + 3 < a.frames) && (a.K % KS == 0) && (a.dw_pad_left == d);
   }
-  ptx::tc_fence_before();
-  __syncthreads();
-  ptx::tc_fence_after();
-  const uint32_t tmem_base = hdr->tmem_base;
-  if (pair) ptx::cluster_sync_all();  // barriers of every CTA initialised before any remote arrive / multicast
+  const float* Ab = a.A + (size_t)b * a.K * a.pitch + tbase;
+  if (EPI == EPI_MASKDEC)
+    for (int i = threadIdx.x; i < TM * 16; i += THREADS) dacc[i] = 0.f;
 
-  // Work decomposition.  A cluster of C CTAs walks the same sequence of cluster items J = cidx + it * num_clusters;
-  // J -> (weight tile nt = J % n_tiles, tile group J / n_tiles); CTA rank r of the cluster takes time tile
-  // L = group * C + r -> (b, tt).  All CTAs of a cluster therefore need the SAME weight slabs at the same step, of which
-  // each CTA of a pair stages one half; ranks whose L falls off the end run a dummy item (no loads, no stores).
-  const int crank = pair ? (int)ptx::cluster_ctarank() : 0;
-  const int cidx = (int)blockIdx.x / g.cluster, num_clusters = (int)gridDim.x / g.cluster;
-  const int items_per_cta = (g.cluster_items - cidx + num_clusters - 1) / num_clusters;
-  auto decode = [&](int it2, int& nt2, int& tt2, int& b2) -> bool {
-    const int J = cidx + it2 * num_clusters;
-    nt2 = J % g.n_tiles;
-    const int L = (J / g.n_tiles) * g.cluster + crank;
-    tt2 = L % g.t_tiles;
-    b2 = L / g.t_tiles;
-    if (L >= g.tiles_total) { tt2 = 0; b2 = 0; return false; }
-    return true;
-  };
-
-  if (warp >= 5 && warp < 5 + PROD_WARPS) {
-    // ===================================== PRODUCERS ========================================================
-    const int p = threadIdx.x - 160;  // 0 .. 32*PROD_WARPS-1
-    const int pw = p >> 5;            // producer warp: rows pw*CPW .. pw*CPW+CPW-1 of the slab
-    float pslope = 0.f;
-    if (PRO == PRO_PRELU || PRO == PRO_DW) pslope = a.pro_slope[0];
-    int s = 0;
-    uint32_t ph = 0;
-    // activation loads of slab (it2, ks2): issued ONE SLAB AHEAD of their use (register double buffer), across item
-    // boundaries, so that the global-load latency overlaps the split/store work and the barrier waits
-    auto load_A = [&](int it2, int ks2, float4 (&dst)[CPW], float4 (&dstr)[CPW]) {
-      int nt2, tt2, b2;
-      const bool live2 = decode(it2, nt2, tt2, b2);
-      const float* Ab2 = a.A + (size_t)b2 * a.K * a.pitch + (size_t)tt2 * TM + lane * 4;
+  for (int ntl = 0; ntl < g.nt_per_cta; ++ntl) {
+  const int nt = ngrp * g.nt_per_cta + ntl;
+  const int n0 = nt * NT;
+  const uint8_t* wsrc = reinterpret_cast<const uint8_t*>(g.wimg) + (size_t)nt * g.k_slabs * NPREC * W_BYTES;
+  float2 dls = make_float2(0.f, 0.f), dlss = make_float2(0.f, 0.f);
+  float acc[64];
 #pragma unroll
-      for (int j = 0; j < CPW; ++j) {
-        const int k = ks2 * KS + pw * CPW + j;
-        dst[j] = (k < a.K && live2 && !(g.dbg & 2u)) ? __ldg(reinterpret_cast<const float4*>(Ab2 + (size_t)k * a.pitch))
-                                             : make_float4(0.f, 0.f, 0.f, 0.f);
+  for (int i = 0; i < 64; ++i) acc[i] = 0.f;
+
+  for (int ks = 0; ks < g.k_slabs; ++ks) {
+    const int gk = ntl * g.k_slabs + ks;  // slab counter of the CTA: stage and mbarrier phase
+    const int s = gk & 1;
+    const uint32_t st_base = stage0 + (uint32_t)s * STAGE_BYTES;
+    // the stage was last read by the MMAs of slab ks - 2, complete in both warpgroups (wait + barrier at the end of ks - 1)
+    if (threadIdx.x == 0) {
+      const uint32_t fb = ptx::smem_u32(&wbar[s]);
+      ptx::mbar_arrive_expect_tx(fb, NPREC * W_BYTES);
+      ptx::bulk_g2s(st_base + NPREC * A_BYTES, wsrc + (size_t)ks * NPREC * W_BYTES, NPREC * W_BYTES, fb);
+    }
+    float4 v[CPW];
+    if (PRO == PRO_DW) {
+      float4 pre[CPW];
+      if (dw_interior) {
+        if (dcls == 4) dw_slab<4, true, TRAIN>(a, b, ks, warp, tbase, mr1, pslope, v, pre, dls, dlss);
+        else if (dcls == 2) dw_slab<2, true, TRAIN>(a, b, ks, warp, tbase, mr1, pslope, v, pre, dls, dlss);
+        else dw_slab<1, true, TRAIN>(a, b, ks, warp, tbase, mr1, pslope, v, pre, dls, dlss);
+      } else {
+        if (dcls == 4) dw_slab<4, false, TRAIN>(a, b, ks, warp, tbase, mr1, pslope, v, pre, dls, dlss);
+        else if (dcls == 2) dw_slab<2, false, TRAIN>(a, b, ks, warp, tbase, mr1, pslope, v, pre, dls, dlss);
+        else dw_slab<1, false, TRAIN>(a, b, ks, warp, tbase, mr1, pslope, v, pre, dls, dlss);
       }
-      if (PRO == PRO_RES) {
-        const float* Rb2 = a.res_r + (size_t)b2 * a.res_Mt * a.pitch + (size_t)tt2 * TM + lane * 4;
+      if (TRAIN && nt == 0) {
 #pragma unroll
         for (int j = 0; j < CPW; ++j) {
-          const int k = ks2 * KS + pw * CPW + j;
-          dstr[j] = (k < a.K && live2) ? __ldg(reinterpret_cast<const float4*>(Rb2 + (size_t)k * a.pitch)) : make_float4(0.f, 0.f, 0.f, 0.f);
+          const int k = ks * KS + warp * CPW + j;
+          if (k < a.K) *reinterpret_cast<float4*>(a.dw_u_pre_out + ((size_t)b * a.K + k) * a.pitch + tbase) = pre[j];
         }
       }
-    };
-    float4 vnext[CPW], rnext[CPW];
-    if (PRO != PRO_DW && items_per_cta > 0) load_A(0, 0, vnext, rnext);
-    for (int it = 0; it < items_per_cta; ++it) {
-      int nt, tt, b;
-      const bool live = decode(it, nt, tt, b);
-      const uint8_t* wsrc = reinterpret_cast<const uint8_t*>(g.wimg) + (size_t)nt * g.k_slabs * NPREC * g.w_bytes;
-      // PRO_DW: per-sample gLN1 statistics of h (the A operand)
-      float2 mr1 = make_float2(0.f, 1.f);
-      float2 dls = make_float2(0.f, 0.f), dlss = make_float2(0.f, 0.f);
-      if (PRO == PRO_DW) mr1 = gln_mean_rstd(a.dw_stats_in + 2 * b, (double)a.K * (double)a.frames, a.dw_eps);
-      float2 mr_res = make_float2(0.f, 1.f);
-      if (PRO == PRO_RES) mr_res = gln_mean_rstd(a.res_stats + 2 * b, a.res_n, a.res_eps);
-      const int tbase = tt * TM + lane * 4;  // first of this thread's 4 time steps
-      int dcls = 4;
-      bool dw_interior = false;
-      if (PRO == PRO_DW) {
-        const int d = a.dw_dilation;
-        dcls = d >= 4 ? 4 : d;
-        const int reach = d >= 4 ? d : 4;  // furthest sample touched on either side of the tile
-        dw_interior = (tt * TM - reach >= 0) && (tt * TM + TM - 1 + reach + 3 < a.frames) && (a.K % KS == 0) &&
-                      (a.dw_pad_left == d);
+    } else {
+#pragma unroll
+      for (int j = 0; j < CPW; ++j) {
+        const int k = ks * KS + warp * CPW + j;
+        v[j] = k < a.K ? __ldg(reinterpret_cast<const float4*>(Ab + (size_t)k * a.pitch)) : make_float4(0.f, 0.f, 0.f, 0.f);
       }
-      for (int ks = 0; ks < g.k_slabs; ++ks) {
-        float4 v[CPW];
-        if (PRO != PRO_DW) {
+      if (PRO == PRO_RES) {
+        // x_new = x + rstd2*r + (v1 - mean2*rstd2*v2): the previous block's residual update, applied on the fly;
+        // the n-tile-0 CTA of each time tile also writes x_new for the block after next
+        const float* Rb = a.res_r + (size_t)b * a.res_Mt * a.pitch + tbase;
 #pragma unroll
-          for (int j = 0; j < CPW; ++j) v[j] = vnext[j];
-          if (PRO == PRO_RES) {
-            // x_new = x + rstd2*r + (v1 - mean2*rstd2*v2): the previous block's residual update, applied on the fly;
-            // the n-tile-0 CTA of each time tile also writes x_new for the block after next
-#pragma unroll
-            for (int j = 0; j < CPW; ++j) {
-              const int k = ks * KS + pw * CPW + j;
-              const int kc = k < a.K ? k : a.K - 1;
-              const float cst = __ldg(a.res_v1 + kc) - mr_res.x * mr_res.y * __ldg(a.res_v2 + kc);
-              float4 xn;
-              xn.x = fmaf(mr_res.y, rnext[j].x, v[j].x + cst); xn.y = fmaf(mr_res.y, rnext[j].y, v[j].y + cst);
-              xn.z = fmaf(mr_res.y, rnext[j].z, v[j].z + cst); xn.w = fmaf(mr_res.y, rnext[j].w, v[j].w + cst);
-              if (tbase + 0 >= a.frames) xn.x = 0.f;
-              if (tbase + 1 >= a.frames) xn.y = 0.f;
-              if (tbase + 2 >= a.frames) xn.z = 0.f;
-              if (tbase + 3 >= a.frames) xn.w = 0.f;
-              if (k >= a.K || !live) xn = make_float4(0.f, 0.f, 0.f, 0.f);
-              v[j] = xn;
-              if (nt == 0 && live && k < a.K)
-                *reinterpret_cast<float4*>(a.res_x_out + ((size_t)b * a.K + k) * a.pitch + tbase) = xn;
-            }
-          }
-          const int ks_n = ks + 1 < g.k_slabs ? ks + 1 : 0;
-          const int it_n = ks + 1 < g.k_slabs ? it : it + 1;
-          if (it_n < items_per_cta) load_A(it_n, ks_n, vnext, rnext);
-        } else {
-          // u[c][t] = PReLU( sum_k wd[c][k] * hn[c][t + k*d - pl] + bd[c] ), hn = gLN1(h) inside [0,frames), 0 outside.
-          // All 12 128-bit loads of the slab (4 channels x 3 taps) are issued before any arithmetic.  The branch below is
-          // uniform over the CTA (depends on the item only).
-          const bool skipl = (g.dbg & 2u) != 0;
-          const bool pfn = (ks + 1 < g.k_slabs) && !(g.dbg & 16u);
-          if (!live) {
-#pragma unroll
-            for (int j = 0; j < CPW; ++j) v[j] = make_float4(0.f, 0.f, 0.f, 0.f);
-          } else if (dw_interior) {
-            if (dcls == 4) dw_slab<4, true, CPW>(a, b, ks, pw, tbase, mr1, pslope, skipl, pfn, v, dls, dlss);
-            else if (dcls == 2) dw_slab<2, true, CPW>(a, b, ks, pw, tbase, mr1, pslope, skipl, pfn, v, dls, dlss);
-            else dw_slab<1, true, CPW>(a, b, ks, pw, tbase, mr1, pslope, skipl, pfn, v, dls, dlss);
-          } else {
-            if (dcls == 4) dw_slab<4, false, CPW>(a, b, ks, pw, tbase, mr1, pslope, skipl, pfn, v, dls, dlss);
-            else if (dcls == 2) dw_slab<2, false, CPW>(a, b, ks, pw, tbase, mr1, pslope, skipl, pfn, v, dls, dlss);
-            else dw_slab<1, false, CPW>(a, b, ks, pw, tbase, mr1, pslope, skipl, pfn, v, dls, dlss);
-          }
+        for (int j = 0; j < CPW; ++j) {
+          const int k = ks * KS + warp * CPW + j;
+          const int kc = k < a.K ? k : a.K - 1;
+          const float4 r = k < a.K ? __ldg(reinterpret_cast<const float4*>(Rb + (size_t)k * a.pitch)) : make_float4(0.f, 0.f, 0.f, 0.f);
+          const float cst = __ldg(a.res_v1 + kc) - mr_res.x * mr_res.y * __ldg(a.res_v2 + kc);
+          float4 xn;
+          xn.x = fmaf(mr_res.y, r.x, v[j].x + cst); xn.y = fmaf(mr_res.y, r.y, v[j].y + cst);
+          xn.z = fmaf(mr_res.y, r.z, v[j].z + cst); xn.w = fmaf(mr_res.y, r.w, v[j].w + cst);
+          if (tbase + 0 >= a.frames) xn.x = 0.f;
+          if (tbase + 1 >= a.frames) xn.y = 0.f;
+          if (tbase + 2 >= a.frames) xn.z = 0.f;
+          if (tbase + 3 >= a.frames) xn.w = 0.f;
+          if (k >= a.K) xn = make_float4(0.f, 0.f, 0.f, 0.f);
+          v[j] = xn;
+          if (nt == 0 && k < a.K) *reinterpret_cast<float4*>(a.res_x_out + ((size_t)b * a.K + k) * a.pitch + tbase) = xn;
         }
-        const bool tl = (g.dbg & 128u) && blockIdx.x == 0 && p == 0 && (it * g.k_slabs + ks) < 1024;
-        if (tl) g_timeline[(it * g.k_slabs + ks) * 4 + 0] = gtime();
-        ptx::mbar_wait(ptx::smem_u32(&hdr->empty[s]), ph ^ 1u);
-        if (tl) g_timeline[(it * g.k_slabs + ks) * 4 + 1] = gtime();
-        const uint32_t st_base = stage0 + (uint32_t)s * g.stage_bytes;
-        if (p == 0) {
-          const uint32_t fb = ptx::smem_u32(&hdr->full[s]);
-          if (g.dbg & 4u) {
-            ptx::mbar_arrive(fb);
-          } else if (!pair) {
-            ptx::mbar_arrive_expect_tx(fb, NPREC * g.w_bytes);
-            const uint32_t chunk = NPREC * g.w_bytes / (uint32_t)g.wsplit;  // several requests in flight per slab
-            for (int c = 0; c < g.wsplit; ++c)
-              ptx::bulk_g2s(st_base + NPREC * A_BYTES + c * chunk, wsrc + (size_t)ks * NPREC * g.w_bytes + (size_t)c * chunk, chunk, fb);
-          } else {
-            // pair mode: this CTA stages rows [crank*n_tile/2, +n_tile/2) of the slab (a contiguous half of the hi image and
-            // of the lo image); the copy completes on this CTA's own full[s].
-            const uint32_t half = g.w_bytes / 2;
-            const uint32_t lb = fb;
-            ptx::mbar_arrive_expect_tx(lb, NPREC * half);
-            const uint8_t* src = wsrc + (size_t)ks * NPREC * g.w_bytes + (size_t)crank * half;
-#pragma unroll
-            for (int pr = 0; pr < NPREC; ++pr)
-              ptx::bulk_g2s(st_base + NPREC * A_BYTES + pr * half, src + (size_t)pr * g.w_bytes, half, lb);
-          }
-        }
-#pragma unroll
-        for (int j = 0; j < ((g.dbg & 64u) ? 0 : CPW); ++j) {
-          const int kl = pw * CPW + j;  // 0..KS-1 within the slab
-          const int kg = kl >> 2, r = kl & 3;
-          // MN-major tf32 needs SWIZZLE_128B_BASE32B (the only MN-major layout the tensor core accepts for 32-bit
-          // operands; pinned on hardware with tools/umma_unit.cu): atoms of 4 channel rows x 128 B (32 time steps),
-          // 32-byte chunks XOR (row & 3); atoms along time 512 B apart (LBO), 4-channel groups 2048 B apart (SBO).
-          const uint32_t off = (uint32_t)kg * 2048u + (uint32_t)(lane >> 3) * 512u + (uint32_t)r * 128u +
-                               (uint32_t)(((((lane & 7) >> 1) ^ r) << 5) | ((lane & 1) << 4));
-          float4 x = v[j];
-          if (PRO == PRO_PRELU) {
-            x.x = prelu_f(x.x, pslope); x.y = prelu_f(x.y, pslope); x.z = prelu_f(x.z, pslope); x.w = prelu_f(x.w, pslope);
-          }
-          if constexpr (F16) {
-            x.x *= act_s; x.y *= act_s; x.z *= act_s; x.w *= act_s;
-            // MN-major 16-bit SWIZZLE_128B: atoms of 64 time steps x 8 channels (1024 B): channel row r = kl & 7 at r*128 B,
-            // 16-byte chunks (8 time steps) XOR r; time atoms 1024 B apart (LBO), 8-channel groups 2048 B apart (SBO)
-            const uint32_t r8 = (uint32_t)(kl & 7);
-            const uint32_t off16 = (uint32_t)(kl >> 3) * 2048u + (uint32_t)(lane >> 4) * 1024u + r8 * 128u +
-                                   (((uint32_t)((lane & 15) >> 1) ^ r8) << 4) + (uint32_t)(lane & 1) * 8u;
-            uint2 h2, l2;
-            ptx::split_f16x2(x.x, x.y, h2.x, l2.x);
-            ptx::split_f16x2(x.z, x.w, h2.y, l2.y);
-            *reinterpret_cast<uint2*>(smem + SMEM_HEADER + (size_t)s * g.stage_bytes + off16) = h2;
-            *reinterpret_cast<uint2*>(smem + SMEM_HEADER + (size_t)s * g.stage_bytes + A_BYTES + off16) = l2;
-          } else {
-          float4 hi, lo;
-          hi.x = ptx::hi_tf32(x.x); hi.y = ptx::hi_tf32(x.y); hi.z = ptx::hi_tf32(x.z); hi.w = ptx::hi_tf32(x.w);
-          {  // lo = x - hi (exact), two elements per FADD2
-            const float2 l01 = __fadd2_rn(make_float2(x.x, x.y), make_float2(-hi.x, -hi.y));
-            const float2 l23 = __fadd2_rn(make_float2(x.z, x.w), make_float2(-hi.z, -hi.w));
-            lo = make_float4(l01.x, l01.y, l23.x, l23.y);
-          }
-          *reinterpret_cast<float4*>(smem + SMEM_HEADER + (size_t)s * g.stage_bytes + off) = hi;
-          if (NPASS == 3) *reinterpret_cast<float4*>(smem + SMEM_HEADER + (size_t)s * g.stage_bytes + A_BYTES + off) = lo;
-          }
-        }
-        ptx::fence_proxy_async_smem();
-        __syncwarp();
-        if (lane == 0) ptx::mbar_arrive(ptx::smem_u32(&hdr->full[s]));
-        if (tl) g_timeline[(it * g.k_slabs + ks) * 4 + 2] = gtime();
-        if (++s == g.stages) { s = 0; ph ^= 1u; }
       }
-      if (PRO == PRO_DW && nt == 0 && live) {
-        const double sd = warp_sum_d((double)dls.x + (double)dls.y), ssd = warp_sum_d((double)dlss.x + (double)dlss.y);
-        if (lane == 0) { atomicAdd(&a.dw_stats_out[2 * b], sd); atomicAdd(&a.dw_stats_out[2 * b + 1], ssd); }
-      }
-    }
-  } else if (warp == 4) {
-    // ===================================== MMA ISSUER =======================================================
-    // The whole warp walks the loop converged; one elected lane issues.  The stage-free commit of slab q is issued
-    // AFTER the first MMA of slab q+1 (same item), so the tensor pipe always has work queued while the thread is busy
-    // with the commit / barrier bookkeeping.
-    if (!pair || crank == 0) {  // pair mode: only the leader CTA issues (its MMAs span both CTAs' TMEM and smem)
-      int s = 0;
-      uint32_t ph = 0;
-      const bool leader = ptx::elect_one();
-      const uint32_t w_lo_off = (pair ? g.w_bytes / 2 : g.w_bytes) >> 4;
-      // descriptor templates: only the 14-bit start-address field changes
-      const uint64_t da_t = ptx::make_smem_desc(0, g.lbo_a, g.sbo_a, g.a_layout);
-      const uint64_t dw_t = ptx::make_smem_desc(0, g.lbo_w, g.sbo_w, g.w_layout);
-      for (int it = 0; it < items_per_cta; ++it) {
-        const int acc = it & 1;
-        if (pair) ptx::mbar_wait_cluster(ptx::smem_u32(&hdr->tempty[acc]), ((uint32_t)(it >> 1) & 1u) ^ 1u);
-        else ptx::mbar_wait(ptx::smem_u32(&hdr->tempty[acc]), ((uint32_t)(it >> 1) & 1u) ^ 1u);
-        ptx::tc_fence_after();
-        const uint32_t d_tmem = tmem_base + (uint32_t)acc * 256u;
-        int prev_s = -1;
-        for (int ks = 0; ks < g.k_slabs; ++ks) {
-          const bool tl = (g.dbg & 128u) && blockIdx.x == 0 && lane == 0 && (it * g.k_slabs + ks) < 1024;
-          if (tl) g_timeline[4096 + (it * g.k_slabs + ks) * 4 + 0] = gtime();
-          if (pair) ptx::mbar_wait_cluster(ptx::smem_u32(&hdr->full[s]), ph);
-          else ptx::mbar_wait(ptx::smem_u32(&hdr->full[s]), ph);
-          if (tl) g_timeline[4096 + (it * g.k_slabs + ks) * 4 + 1] = gtime();
-          ptx::tc_fence_after();
-          const uint32_t st_base = stage0 + (uint32_t)s * g.stage_bytes;
-          const uint32_t a_hi = st_base >> 4, a_lo = (st_base + A_BYTES) >> 4;
-          const uint32_t w_hi = (st_base + NPREC * A_BYTES) >> 4, w_lo = w_hi + w_lo_off;
-          if (leader) {
-            auto commit = [&](uint64_t* bar) {
-              if constexpr (pair) ptx::mma2_commit_multicast(ptx::smem_u32(bar), (uint16_t)3u);  // same barrier in both CTAs
-              else ptx::mma_commit(ptx::smem_u32(bar));
-            };
-            auto mma = [&](uint64_t da, uint64_t dw, uint32_t accum) {
-              if constexpr (pair) ptx::mma2_tf32(d_tmem, da, dw, g.idesc, accum);
-              else if constexpr (F16) ptx::mma_f16(d_tmem, da, dw, g.idesc, accum);
-              else ptx::mma_tf32(d_tmem, da, dw, g.idesc, accum);
-            };
+      if (PRO == PRO_PRELU) {
 #pragma unroll
-            // per instruction: 8 channels (tf32) or 16 (fp16); either way the A start address advances by 4096 B (two channel
-            // groups) and the W start address by 32 B
-            for (int kk = 0; kk < (F16 ? KS / 16 : KS / 8); ++kk) {
-              if (g.dbg & 8u) break;
-              const uint64_t da_hi = da_t | (uint64_t)(a_hi + kk * 256), dw_hi = dw_t | (uint64_t)(w_hi + kk * 2);
-              mma(da_hi, dw_hi, (ks | kk) ? 1u : 0u);
-              if (kk == 0 && prev_s >= 0) commit(&hdr->empty[prev_s]);  // previous slab's stage (its MMAs are queued ahead)
-              if (NPASS == 3) {
-                const uint64_t da_lo = da_t | (uint64_t)(a_lo + kk * 256), dw_lo = dw_t | (uint64_t)(w_lo + kk * 2);
-                mma(da_lo, dw_hi, 1u);
-                mma(da_hi, dw_lo, 1u);
-              }
-            }
-            if ((g.dbg & 8u) && prev_s >= 0) commit(&hdr->empty[prev_s]);
-            if (ks == g.k_slabs - 1) {
-              commit(&hdr->empty[s]);     // last slab of the item: free its stage right away
-              commit(&hdr->tfull[acc]);   // accumulator ready for the epilogue
-            }
-          }
-          __syncwarp();
-          if (tl) g_timeline[4096 + (it * g.k_slabs + ks) * 4 + 2] = gtime();
-          prev_s = s;
-          if (++s == g.stages) { s = 0; ph ^= 1u; }
+        for (int j = 0; j < CPW; ++j) {
+          v[j].x = prelu_f(v[j].x, pslope); v[j].y = prelu_f(v[j].y, pslope);
+          v[j].z = prelu_f(v[j].z, pslope); v[j].w = prelu_f(v[j].w, pslope);
         }
       }
     }
-    else {
-      // peer CTA of a pair: this warp has no MMAs to issue; it forwards "my stage s is full" (the peer's local full[s]:
-      // its producer warps + its half of the weight slab) to the leader's full[s] with ONE cluster-scope arrival per
-      // slab, which keeps remote arrivals and cluster-scope releases off the producers' path
-      int s = 0;
-      uint32_t ph = 0;
-      for (int it = 0; it < items_per_cta; ++it)
-        for (int ks = 0; ks < g.k_slabs; ++ks) {
-          ptx::mbar_wait(ptx::smem_u32(&hdr->full[s]), ph);
-          if (lane == 0) ptx::mbar_arrive_remote(ptx::smem_u32(&hdr->full[s]), 0);
-          __syncwarp();
-          if (++s == g.stages) { s = 0; ph ^= 1u; }
-        }
-    }
-    __syncwarp();
-  } else {
-    // ===================================== EPILOGUE =========================================================
-    // thread = one time step (TMEM lane); columns = output channels.  Per-channel parameters of the tile are staged
-    // in shared memory once per item; TMEM is read in 16-column chunks, double buffered so that the next tcgen05.ld is
-    // in flight while the current chunk is transformed and stored (one coalesced 128-byte row segment per warp-store).
-    float eslope = 0.f;
-    if (EPI == EPI_H) eslope = a.slope[0];
-    const bool store_pre = EPI == EPI_H && a.store_pre != 0;  // training forward: keep the PRE-activation, statistics of PReLU(.)
-    float* sp = reinterpret_cast<float*>(smem + SMEM_PARAMS);  // [256] per-channel epilogue parameter
-    const int egroup = (EGROUPS == 2 && warp >= 5 + PROD_WARPS) ? 1 : 0;                     // second warpgroup handles the upper half of the columns
-    const int te = (warp & 3) * 32 + lane;                     // time step within the tile == TMEM lane
-    const int tid_e = egroup * 128 + te;
-    for (int it = 0; it < items_per_cta; ++it) {
-      int nt, tt, b;
-      const bool live = decode(it, nt, tt, b);
-      const int acc = it & 1;
-      const int t = tt * TM + te;
-      const bool tvalid = t < a.frames;
-      const int n0 = nt * g.n_tile;
-      const int nvalid = live ? min(g.n_tile, a.M - n0) : 0;  // dummy item: nothing to read, store or count
-      float mscale = 1.f;
-      {
-        // stage the per-channel parameter: EPI_HEAD: v1 - mean*rstd*v2 (deferred gLN shift); EPI_H / EPI_MASK: bias
-        float2 mr = make_float2(0.f, 1.f);
-        if (EPI == EPI_HEAD) { mr = gln_mean_rstd(a.stats_in + 2 * b, a.n_in, a.eps); mscale = mr.y; }
-        asm volatile("bar.sync 1, %0;" ::"n"(128 * EGROUPS) : "memory");  // previous item's readers are done with sp
-        for (int i = tid_e; i < g.n_tile; i += 128 * EGROUPS) {
-          float pv = 0.f;
-          if (i < nvalid) {
-            if (EPI == EPI_HEAD) pv = __ldg(a.v1 + n0 + i) - mr.x * mr.y * __ldg(a.v2 + n0 + i);
-            if (EPI == EPI_H || EPI == EPI_MASK) pv = __ldg(a.bias + n0 + i);
-          }
-          sp[i] = pv;
-        }
-        asm volatile("bar.sync 1, %0;" ::"n"(128 * EGROUPS) : "memory");
-      }
-      const bool tle = (g.dbg & 128u) && blockIdx.x == 0 && threadIdx.x == 0 && it < 1024;
-      if (tle) g_timeline[8192 + it * 4 + 0] = gtime();
-      ptx::mbar_wait(ptx::smem_u32(&hdr->tfull[acc]), (uint32_t)(it >> 1) & 1u);
-      if (tle) g_timeline[8192 + it * 4 + 1] = gtime();
-      ptx::tc_fence_after();
-      const uint32_t taddr = tmem_base + (uint32_t)acc * 256u + ((uint32_t)((warp & 3) * 32) << 16);
-      float* Dp = a.D + ((size_t)b * a.M + n0) * a.pitch + t;
-      float* Mp = (EPI == EPI_MASK && a.mask_out) ? a.mask_out + ((size_t)b * a.M + n0) * a.pitch + t : nullptr;
-      const float* Wp = (EPI == EPI_MASK) ? a.wenc + (size_t)b * a.Nb * a.pitch + t : nullptr;
-      const int nb0 = (EPI == EPI_MASK) ? n0 % a.Nb : 0;
-      float ls = 0.f, lss = 0.f;
-      const int ncols_all = (nvalid + 15) & ~15;
-      const int csplit = EGROUPS == 2 ? ((ncols_all / 2 + 15) & ~15) : ncols_all;  // group 0: [0,csplit), group 1: rest
-      const int cbeg = egroup == 0 ? 0 : csplit;
-      const int ncols = egroup == 0 ? csplit : ncols_all;
-
-      const bool do_store = !(g.dbg & 1u);
-      const bool tile_full = tt * TM + TM <= a.frames;  // every time step of this tile is a real frame
-      auto process = [&](const uint32_t (&buf)[16], int c0) {
-        float wv[16];
-        if (EPI == EPI_MASK) {
+    // K-major store: row = time step, this warp's 4 channels are 4 adjacent elements of the row
+    uint8_t* sa = smem + SMEM_HEADER + (size_t)s * STAGE_BYTES;
 #pragma unroll
-          for (int j = 0; j < 16; ++j) {
-            int nn = nb0 + c0 + j;
-            while (nn >= a.Nb) nn -= a.Nb;
-            wv[j] = (c0 + j < nvalid) ? __ldg(Wp + (size_t)nn * a.pitch) : 0.f;
-          }
-        }
-        float* q = Dp + (size_t)c0 * a.pitch;
-        float* qm = Mp ? Mp + (size_t)c0 * a.pitch : nullptr;
-        const bool full = (c0 + 16 <= nvalid) && tile_full && do_store;  // warp-uniform
-        // F16: the 16 output channels of a chunk share one power-of-two weight scale (wimg_f16_rows scales 16-row groups)
-        float osc = 1.f;
-        if constexpr (F16) osc = reinterpret_cast<const float*>(smem + SMEM_SCALES)[n0 + c0];
-        float o[16], mk[16];
-        // per-channel parameters are fetched 4 columns at a time (8 live registers instead of 32: the epilogue shares the
-        // register budget of the producers)
+    for (int e = 0; e < 4; ++e) {
+      const int t = lane * 4 + e;
+      float x[CPW];
 #pragma unroll
-        for (int j4 = 0; j4 < 4; ++j4) {
-          const float4 p4 = *reinterpret_cast<const float4*>(sp + c0 + j4 * 4);
-          const float pvv[4] = {p4.x, p4.y, p4.z, p4.w};
-#pragma unroll
-          for (int jj = 0; jj < 4; ++jj) {
-            const int j = j4 * 4 + jj;
-            float v = __uint_as_float(buf[j]);
-            mk[j] = 0.f;
-            // F16: v * osc undoes the power-of-two row scaling of the weights (exact), folded into the bias FMA
-            if (EPI == EPI_RAW && F16) v *= osc;
-            if (EPI == EPI_HEAD) v = F16 ? fmaf(mscale * osc, v, pvv[jj]) : fmaf(mscale, v, pvv[jj]);
-            if (EPI == EPI_H) {
-              const float pre = F16 ? fmaf(v, osc, pvv[jj]) : v + pvv[jj];
-              const float act = prelu_f(pre, eslope);
-              v = store_pre ? pre : act;
-              if (full) { ls += act; lss = fmaf(act, act, lss); }  // gLN statistics are always those of PReLU(.)
-            }
-            if (EPI == EPI_MASK) {
-              const float logit = F16 ? fmaf(v, osc, pvv[jj]) : v + pvv[jj];
-              if (a.mask_logits) {  // softmax masks: the normalisation over all S*N channels is a second pass (ctn_softmax_mask)
-                mk[j] = logit;
-                v = logit;
-              } else {
-                mk[j] = __fdividef(1.f, 1.f + __expf(-logit));
-                v = mk[j] * wv[j];
-              }
-            }
-            o[j] = v;
-          }
-        }
-        if (full) {
-#pragma unroll
-          for (int j = 0; j < 16; ++j) {
-            *q = o[j];
-            q += a.pitch;
-          }
-          if (EPI == EPI_MASK && qm) {
-#pragma unroll
-            for (int j = 0; j < 16; ++j) { *qm = mk[j]; qm += a.pitch; }
-          }
-        } else {
-#pragma unroll
-          for (int j = 0; j < 16; ++j) {
-            const float v = tvalid ? o[j] : 0.f;
-            if (c0 + j < nvalid) {
-              if (do_store) {
-                q[(size_t)j * a.pitch] = v;
-                if (EPI == EPI_MASK && qm) qm[(size_t)j * a.pitch] = tvalid ? mk[j] : 0.f;
-              }
-              if (EPI == EPI_H) { const float sv = store_pre ? prelu_f(v, eslope) : v; ls += sv; lss = fmaf(sv, sv, lss); }
-            }
-          }
-        }
-      };
-
-      uint32_t bufA[16], bufB[16];
-      if (cbeg < ncols && !(g.dbg & 32u)) ptx::tmem_ld16(taddr + (uint32_t)cbeg, bufA);
-      for (int c0 = cbeg; c0 < ((g.dbg & 32u) ? 0 : ncols); c0 += 32) {
-        ptx::tmem_ld_wait();
-        if (c0 + 16 < ncols) ptx::tmem_ld16(taddr + (uint32_t)(c0 + 16), bufB);
-        process(bufA, c0);
-        ptx::tmem_ld_wait();
-        if (c0 + 32 < ncols) ptx::tmem_ld16(taddr + (uint32_t)(c0 + 32), bufA);
-        if (c0 + 16 < ncols) process(bufB, c0 + 16);
-      }
-      ptx::tc_fence_before();
-      if (pair) {  // one arrival per warp, on the LEADER's barrier (its MMA warp overwrites both CTAs' accumulators)
-        __syncwarp();
-        if (lane == 0) {
-          if (crank == 0) ptx::mbar_arrive(ptx::smem_u32(&hdr->tempty[acc]));
-          else ptx::mbar_arrive_remote(ptx::smem_u32(&hdr->tempty[acc]), 0);
-        }
+      for (int j = 0; j < CPW; ++j) x[j] = e == 0 ? v[j].x : e == 1 ? v[j].y : e == 2 ? v[j].z : v[j].w;
+      if (F16) {
+        // SWIZZLE_64B: rows of 64 B, 16-byte chunk (8 channels) index XOR (row / 2) % 4
+        const uint32_t off = (uint32_t)t * 64u + (((uint32_t)(warp >> 1) ^ (uint32_t)((t >> 1) & 3)) << 4) + (uint32_t)(warp & 1) * 8u;
+        uint2 h2, l2;
+        ptx::split_f16x2(x[0] * act_s, x[1] * act_s, h2.x, l2.x);
+        ptx::split_f16x2(x[2] * act_s, x[3] * act_s, h2.y, l2.y);
+        *reinterpret_cast<uint2*>(sa + off) = h2;
+        *reinterpret_cast<uint2*>(sa + A_BYTES + off) = l2;
       } else {
-        ptx::mbar_arrive(ptx::smem_u32(&hdr->tempty[acc]));
+        // SWIZZLE_128B: rows of 128 B, 16-byte chunk (4 channels) index XOR row % 8
+        const uint32_t off = (uint32_t)t * 128u + (((uint32_t)warp ^ (uint32_t)(t & 7)) << 4);
+        float4 hi, lo;
+        hi.x = ptx::hi_tf32(x[0]); hi.y = ptx::hi_tf32(x[1]); hi.z = ptx::hi_tf32(x[2]); hi.w = ptx::hi_tf32(x[3]);
+        lo.x = x[0] - hi.x; lo.y = x[1] - hi.y; lo.z = x[2] - hi.z; lo.w = x[3] - hi.w;
+        *reinterpret_cast<float4*>(sa + off) = hi;
+        if (NPASS == 3) *reinterpret_cast<float4*>(sa + A_BYTES + off) = lo;
       }
-      if (tle) g_timeline[8192 + it * 4 + 2] = gtime();
-      if (EPI == EPI_H) {
-        double s = warp_sum_d((double)ls), ss = warp_sum_d((double)lss);
-        if (lane == 0) { atomicAdd(&a.stats_out[2 * b], s); atomicAdd(&a.stats_out[2 * b + 1], ss); }
+    }
+    ptx::fence_proxy_async_smem();
+    __syncthreads();
+    ptx::mbar_wait(ptx::smem_u32(&wbar[s]), (uint32_t)(gk >> 1) & 1u);
+    const uint32_t a_hi = st_base + (uint32_t)wg * 64u * ROWB, a_lo = a_hi + A_BYTES;
+    const uint32_t w_hi = st_base + NPREC * A_BYTES, w_lo = w_hi + W_BYTES;
+    ptx::wg_fence();
+#pragma unroll
+    for (int kk = 0; kk < (F16 ? KS / 16 : KS / 8); ++kk) {  // 32 bytes of the rows per instruction
+      const uint64_t dah = ptx::wg_desc(a_hi + kk * 32, 8 * ROWB, LAYOUT), dwh = ptx::wg_desc(w_hi + kk * 32, 8 * ROWB, LAYOUT);
+      if (F16) ptx::wg_mma_f16(acc, dah, dwh); else ptx::wg_mma_tf32(acc, dah, dwh);
+      if (NPASS == 3) {
+        const uint64_t dal = ptx::wg_desc(a_lo + kk * 32, 8 * ROWB, LAYOUT), dwl = ptx::wg_desc(w_lo + kk * 32, 8 * ROWB, LAYOUT);
+        if (F16) { ptx::wg_mma_f16(acc, dal, dwh); ptx::wg_mma_f16(acc, dah, dwl); }
+        else { ptx::wg_mma_tf32(acc, dal, dwh); ptx::wg_mma_tf32(acc, dah, dwl); }
       }
+    }
+    ptx::wg_commit();
+    ptx::wg_wait<1>();  // the MMAs of slab ks - 1 are done: its stage may be refilled
+    __syncthreads();
+  }
+  ptx::wg_wait<0>();
+
+  if (PRO == PRO_DW && nt == 0) {
+    const double sd = warp_sum_d((double)dls.x + (double)dls.y), ssd = warp_sum_d((double)dlss.x + (double)dlss.y);
+    if (lane == 0) { atomicAdd(&a.dw_stats_out[2 * b], sd); atomicAdd(&a.dw_stats_out[2 * b + 1], ssd); }
+  }
+
+  // ===================================== EPILOGUE (on the accumulator fragment) =====================================
+  float eslope = 0.f;
+  if (EPI == EPI_H) eslope = __ldg(a.slope);
+  const bool store_pre = EPI == EPI_H && a.store_pre != 0;  // training forward: keep the PRE-activation, statistics of PReLU(.)
+  float2 mr = make_float2(0.f, 1.f);
+  if (EPI == EPI_HEAD) mr = gln_mean_rstd(a.stats_in + 2 * b, a.n_in, a.eps);
+  const float inv_act = 1.f / act_s;
+  const int row0 = wg * 64 + (warp & 3) * 16 + (lane >> 2);
+  float ls = 0.f, lss = 0.f;
+  float dpart[2][16];  // EPI_MASKDEC: sum over this thread's columns of w_hat[n][t] * Dec[n][k], rows row0 and row0 + 8
+#pragma unroll
+  for (int k = 0; k < 32; ++k) dpart[k >> 4][k & 15] = 0.f;
+#pragma unroll
+  for (int i = 0; i < 64; ++i) {
+    const int row = row0 + 8 * ((i >> 1) & 1);
+    const int n = n0 + 8 * (i >> 2) + 2 * (lane & 3) + (i & 1);
+    const int t = tt * TM + row;
+    if (n >= a.M) continue;
+    const bool tvalid = t < a.frames;
+    // F16: v * osc undoes the power-of-two row scaling of the weights and the activation scale (exact)
+    const float osc = F16 ? __ldg(g.oscale + n) * inv_act : 1.f;
+    float v = acc[i];
+    float* q = a.D + ((size_t)b * a.M + n) * a.pitch + t;
+    if (EPI == EPI_RAW) {
+      if (F16) v *= osc;
+    } else if (EPI == EPI_HEAD) {
+      const float pv = __ldg(a.v1 + n) - mr.x * mr.y * __ldg(a.v2 + n);
+      v = F16 ? fmaf(mr.y * osc, v, pv) : fmaf(mr.y, v, pv);
+    } else if (EPI == EPI_H) {
+      const float pre = F16 ? fmaf(v, osc, __ldg(a.bias + n)) : v + __ldg(a.bias + n);
+      const float act = prelu_f(pre, eslope);
+      v = store_pre ? pre : act;
+      if (tvalid) { ls += act; lss = fmaf(act, act, lss); }  // gLN statistics are always those of PReLU(.)
+    } else if (EPI == EPI_MASK) {
+      const float logit = F16 ? fmaf(v, osc, __ldg(a.bias + n)) : v + __ldg(a.bias + n);
+      float mk;
+      if (a.mask_logits) {  // softmax masks: the normalisation over all S*N channels is a second pass (ctn_softmax_mask)
+        mk = logit;
+        v = logit;
+      } else {
+        mk = __fdividef(1.f, 1.f + __expf(-logit));
+        v = tvalid ? mk * __ldg(a.wenc + ((size_t)b * a.Nb + n % a.Nb) * a.pitch + t) : 0.f;
+      }
+      if (a.mask_out) a.mask_out[((size_t)b * a.M + n) * a.pitch + t] = tvalid ? mk : 0.f;
+    } else if (EPI == EPI_MASKDEC) {
+      // w_hat[n][t] = w[n][t] * sigmoid(logit), contracted on the spot with the decoder basis (ConvTranspose1d(N, 1, 16, stride 8),
+      // filterbank.py:245-247): frame t contributes w_hat[n][t] * Dec[n][k] to sample 8 t + k
+      const float logit = F16 ? fmaf(v, osc, __ldg(a.bias + n)) : v + __ldg(a.bias + n);
+      const float o = tvalid ? __fdividef(__ldg(a.wenc + ((size_t)b * a.Nb + n % a.Nb) * a.pitch + t), 1.f + __expf(-logit)) : 0.f;
+      const float4* dr = reinterpret_cast<const float4*>(a.dec_w + (size_t)(n % a.Nb) * 16);
+#pragma unroll
+      for (int q4 = 0; q4 < 4; ++q4) {
+        const float4 d4 = __ldg(dr + q4);
+        float* dp = dpart[(i >> 1) & 1] + 4 * q4;
+        dp[0] = fmaf(o, d4.x, dp[0]); dp[1] = fmaf(o, d4.y, dp[1]); dp[2] = fmaf(o, d4.z, dp[2]); dp[3] = fmaf(o, d4.w, dp[3]);
+      }
+      continue;
+    }
+    *q = tvalid ? v : 0.f;
+  }
+  if (EPI == EPI_H) {
+    const double s = warp_sum_d((double)ls), ss = warp_sum_d((double)lss);
+    if (lane == 0) { atomicAdd(&a.stats_out[2 * b], s); atomicAdd(&a.stats_out[2 * b + 1], ss); }
+  }
+  if (EPI == EPI_MASKDEC) {
+    // the 4 lanes of a quad hold the same two frames: reduce over them, lane 0 of the quad adds the frame's 16 taps to the tile sums
+#pragma unroll
+    for (int k = 0; k < 32; ++k) {
+      float v = dpart[k >> 4][k & 15];
+      v += __shfl_xor_sync(0xffffffffu, v, 1);
+      v += __shfl_xor_sync(0xffffffffu, v, 2);
+      dpart[k >> 4][k & 15] = v;
+    }
+    if ((lane & 3) == 0) {
+#pragma unroll
+      for (int k = 0; k < 32; ++k) dacc[(row0 + 8 * (k >> 4)) * 16 + (k & 15)] += dpart[k >> 4][k & 15];
     }
   }
-  ptx::tc_fence_before();
-  __syncthreads();
-  ptx::tc_fence_after();
-  if (pair) ptx::cluster_sync_all();  // nobody exits while a peer may still multicast into it / arrive on it
-  if (warp == 4) {
-    if constexpr (pair) ptx::tmem_dealloc2(tmem_base, 512);
-    else ptx::tmem_dealloc(tmem_base, 512);
+  }  // n-tiles of the CTA
+
+  if (EPI == EPI_MASKDEC) {
+    // sample 8 f + k of the tile = taps k < 8 of frame f + taps 8 + k of frame f - 1, then the crop (conv_tasnet.py:169).  The first 8
+    // samples also receive the previous tile's last frame and the 8 samples after the tile belong to the next tile's first frame:
+    // those are added to the zero-initialised output with red.add, exactly two operands each, so the result is order-independent.
+    __syncthreads();
+    const int src = ngrp, S = a.M / a.Nb;
+    float* yo = a.D + ((size_t)b * S + src) * (size_t)a.dec_T_out;
+    const long long base = 8LL * tt * TM - a.dec_crop_left;
+    for (int sidx = threadIdx.x; sidx < 8 * TM + 8; sidx += THREADS) {
+      const int f = sidx >> 3, k = sidx & 7;
+      float v = 0.f;
+      if (f < TM) v += dacc[f * 16 + k];
+      if (f >= 1) v += dacc[(f - 1) * 16 + 8 + k];
+      const long long tau = base + sidx;
+      if (tau < 0 || tau >= a.dec_T_out) continue;
+      if (sidx < 8 || sidx >= 8 * TM) atomicAdd(yo + tau, v);
+      else yo[tau] = v;
+    }
   }
 }
 
 // ---- weight images ---------------------------------------------------------------------------------------------
-// K-major SWIZZLE_64B image of an (n_tile x KS=16) weight slab: rows of 64 B (16 k), 8-row groups of 512 B (SBO),
-// 16-byte chunk index XOR ((row >> 1) & 3).  Float offset of element (row nl, k kl):
+// K-major SWIZZLE_128B image of an (n_tile x KS=32) tf32 weight slab: rows of 128 B, 8-row groups of 1024 B, 16-byte chunk
+// index XOR (row & 7).  Float offset of element (row nl, k kl):
 __host__ __device__ __forceinline__ int wimg_offset(int nl, int kl) {
-  if (KS == 32)  // SWIZZLE_128B: rows of 128 B, 8-row groups of 1024 B, chunk index XOR (row & 7)
-    return (nl >> 3) * 256 + (nl & 7) * 32 + ((((kl >> 2) ^ (nl & 7)) << 2) | (kl & 3));
-  return (nl >> 3) * 128 + (nl & 7) * 16 + ((((kl >> 2) ^ ((nl >> 1) & 3)) << 2) | (kl & 3));
+  return (nl >> 3) * 256 + (nl & 7) * 32 + ((((kl >> 2) ^ (nl & 7)) << 2) | (kl & 3));
 }
 
 // grid (k_slabs, n_tiles), block 256: builds the image(s) of one weight slab.
@@ -705,7 +436,7 @@ struct WimgJobs { WimgJob j[CTN_MAX_JOBS]; };
 // grid (max k_slabs * max n_tiles, jobs): one block per (slab, n-tile) of one job
 __global__ void __launch_bounds__(256) k_build_wimg_batch(const WimgJobs jobs, int nprec) {
   const WimgJob& jb = jobs.j[blockIdx.y];
-  const int n_tile = jb.M >= 256 ? 256 : ((jb.M + 15) / 16) * 16;
+  const int n_tile = NT;
   const int n_tiles = (jb.M + n_tile - 1) / n_tile, k_slabs = (jb.K + KS - 1) / KS;
   const size_t per = (size_t)n_tile * KS;
   for (int blk = blockIdx.x; blk < n_tiles * k_slabs; blk += gridDim.x) {
@@ -727,7 +458,7 @@ __global__ void __launch_bounds__(256) k_build_wimg_batch(const WimgJobs jobs, i
 __global__ void __launch_bounds__(512) k_build_wimg_batch_f16(const WimgJobs jobs) {
   __shared__ float smax[16];
   const WimgJob& jb = jobs.j[blockIdx.y];
-  const int n_tile = jb.M >= 256 ? 256 : ((jb.M + 15) / 16) * 16;
+  const int n_tile = NT;
   const int n_tiles = (jb.M + n_tile - 1) / n_tile, k_slabs = (jb.K + KS - 1) / KS;
   const int groups = n_tile / 16;
   __half* img = reinterpret_cast<__half*>(jb.wimg);
@@ -736,97 +467,68 @@ __global__ void __launch_bounds__(512) k_build_wimg_batch_f16(const WimgJobs job
     wimg_f16_group(jb.W, jb.M, jb.K, n_tile, k_slabs, blk / groups, blk % groups, img, oscale, smax);
 }
 
-int pick_n_tile(int M);
-// the fp16-piece mode keeps one scale per padded output channel in shared memory: contractions with more than
-// F16_MAX_ROWS padded output channels use the tf32 pieces instead (images and kernel are chosen by the same rule)
+// the fp16-piece mode keeps one scale per padded output channel: contractions with more than F16_MAX_ROWS padded output
+// channels use the tf32 pieces instead (images and kernel are chosen by the same rule)
 int eff_math(int M, int math) {
   if (math != CTN_MATH_F16X3) return math;
-  const int n_tile = pick_n_tile(M);
-  return ((M + n_tile - 1) / n_tile) * n_tile > F16_MAX_ROWS ? CTN_MATH_TF32X3 : math;
+  return ((M + NT - 1) / NT) * NT > F16_MAX_ROWS ? CTN_MATH_TF32X3 : math;
 }
 
-int pick_n_tile(int M) {
-  static const char* env_nt = getenv("CTN_UMMA_NTILE");
-  if (env_nt && atoi(env_nt) >= 16 && atoi(env_nt) <= 256 && atoi(env_nt) % 16 == 0 && M >= atoi(env_nt)) return atoi(env_nt);
-  if (M >= 256) return 256;
-  return ((M + 15) / 16) * 16;
-}
-
-int g_num_sms[CTN_MAX_DEVICES] = {0};  // per device ordinal
-int num_sms() {
-  const int dev = ctn_current_device();
-  if (g_num_sms[dev] == 0) {
-    cudaDeviceGetAttribute(&g_num_sms[dev], cudaDevAttrMultiProcessorCount, dev);
-    if (g_num_sms[dev] <= 0) g_num_sms[dev] = 148;
-  }
-  return g_num_sms[dev];
-}
-
-template <int PRO, int EPI, int NPASS, bool PAIR, bool F16>
-int launch(const UmmaArgs& g, size_t smem, int grid, cudaStream_t st) {
-  constexpr int NT = Roles<PRO>::THREADS;
+template <int PRO, int EPI, int NPASS, bool F16, bool TRAIN>
+int launch(const TcArgs& g, cudaStream_t st) {
+  constexpr int NPREC = NPASS == 3 ? 2 : 1;
+  constexpr size_t smem = SMEM_HEADER + 1024 + (size_t)STAGES * NPREC * (TM + NT) * (F16 ? 64 : 128) + (EPI == EPI_MASKDEC ? TM * 16 * 4 : 0);
   static bool attr_done[CTN_MAX_DEVICES] = {false};  // the opt-in is per device (context)
   const int dev = ctn_current_device();
   if (!attr_done[dev]) {
-    cudaError_t e = cudaFuncSetAttribute(k_pw_umma<PRO, EPI, NPASS, PAIR, F16>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024);
+    cudaError_t e = cudaFuncSetAttribute(k_pw_wgmma<PRO, EPI, NPASS, F16, TRAIN>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
     if (e != cudaSuccess) return (int)e;
     attr_done[dev] = true;
   }
-  if (PAIR) {
-    cudaLaunchConfig_t cfg;
-    memset(&cfg, 0, sizeof(cfg));
-    cfg.gridDim = dim3(grid);
-    cfg.blockDim = dim3(NT);
-    cfg.dynamicSmemBytes = smem;
-    cfg.stream = st;
-    cudaLaunchAttribute attr[1];
-    attr[0].id = cudaLaunchAttributeClusterDimension;
-    attr[0].val.clusterDim.x = 2;
-    attr[0].val.clusterDim.y = 1;
-    attr[0].val.clusterDim.z = 1;
-    cfg.attrs = attr;
-    cfg.numAttrs = 1;
-    cudaError_t e = cudaLaunchKernelEx(&cfg, k_pw_umma<PRO, EPI, NPASS, PAIR, F16>, g);
-    if (e != cudaSuccess) return (int)e;
-  } else {
-    k_pw_umma<PRO, EPI, NPASS, PAIR, F16><<<grid, NT, smem, st>>>(g);
-  }
+  const long long grid = (long long)g.a.B * g.t_tiles * (g.n_tiles / g.nt_per_cta);
+  if (grid > 0x7fffffffLL) return CTN_EUNSUPPORTED;
+  k_pw_wgmma<PRO, EPI, NPASS, F16, TRAIN><<<(unsigned)grid, THREADS, smem, st>>>(g);
   CTN_COUNT_LAUNCH();
   CTN_RETURN_IF_CUDA_ERR();
   return CTN_OK;
 }
 
+template <int PRO, int EPI, bool TRAIN = false>
+int launch_math(const TcArgs& g, int math, cudaStream_t st) {
+  if (math == CTN_MATH_F16X3) return launch<PRO, EPI, 3, true, TRAIN>(g, st);
+  if (math == CTN_MATH_TF32) return launch<PRO, EPI, 1, false, TRAIN>(g, st);
+  return launch<PRO, EPI, 3, false, TRAIN>(g, st);
+}
+
 }  // namespace
 
+// the tensor-core (hi/lo split) numeric modes are built
 extern "C" int ctn_has_tcgen05(void) { return 1; }
 
-// debug: copy the timeline of the last CTN_UMMA_DBG&128 launch (3 regions x 4096 stamps) to the host
+// the wgmma kernels record no timeline
 extern "C" int ctn_debug_timeline(unsigned long long* host, int n) {
   if (!host || n <= 0 || n > 3 * 4096) return CTN_EINVAL;
-  cudaError_t e = cudaMemcpyFromSymbol(host, g_timeline, sizeof(unsigned long long) * n);
-  return e == cudaSuccess ? CTN_OK : (int)e;
+  return CTN_EUNSUPPORTED;
 }
 
 size_t ctn_umma_wimg_bytes(int M, int K, int math) {
   const int nprec = math == CTN_MATH_TF32 ? 1 : 2;
-  const int n_tile = pick_n_tile(M);
-  const int n_tiles = (M + n_tile - 1) / n_tile, k_slabs = (K + KS - 1) / KS;
+  const int n_tiles = (M + NT - 1) / NT, k_slabs = (K + KS - 1) / KS;
   // fp16 images are half the size but carry the per-channel scale array behind them; the tf32x3 size + scales covers both
-  return (size_t)n_tiles * k_slabs * nprec * n_tile * KS * sizeof(float) + (size_t)n_tiles * n_tile * sizeof(float) + 256;
+  return (size_t)n_tiles * k_slabs * nprec * NT * KS * sizeof(float) + (size_t)n_tiles * NT * sizeof(float) + 256;
 }
 
 int ctn_umma_build_wimg(const float* W, int M, int K, int math, float* wimg, cudaStream_t st) {
   math = eff_math(M, math);
   const int nprec = math == CTN_MATH_TF32 ? 1 : 2;  // hi [, lo]
-  const int n_tile = pick_n_tile(M);
-  const int n_tiles = (M + n_tile - 1) / n_tile, k_slabs = (K + KS - 1) / KS;
+  const int n_tiles = (M + NT - 1) / NT, k_slabs = (K + KS - 1) / KS;
   if (math == CTN_MATH_F16X3) {
-    k_build_wimg_f16<<<dim3(n_tile / 16, n_tiles), 512, 0, st>>>(W, M, K, n_tile, k_slabs, n_tiles, wimg);
+    k_build_wimg_f16<<<dim3(NT / 16, n_tiles), 512, 0, st>>>(W, M, K, NT, k_slabs, n_tiles, wimg);
     CTN_COUNT_LAUNCH();
     CTN_RETURN_IF_CUDA_ERR();
     return CTN_OK;
   }
-  k_build_wimg<<<dim3(k_slabs, n_tiles), 256, 0, st>>>(W, M, K, n_tile, k_slabs, nprec, wimg);
+  k_build_wimg<<<dim3(k_slabs, n_tiles), 256, 0, st>>>(W, M, K, NT, k_slabs, nprec, wimg);
   CTN_COUNT_LAUNCH();
   CTN_RETURN_IF_CUDA_ERR();
   return CTN_OK;
@@ -836,7 +538,7 @@ int ctn_umma_build_wimg_batch(const WimgJob* jobs, int n, int math, cudaStream_t
   const int nprec = math == CTN_MATH_TF32 ? 1 : 2;
   bool uniform = true;
   for (int i = 0; i < n; ++i) uniform = uniform && eff_math(jobs[i].M, math) == math;
-  if (getenv("CTN_UMMA_NTILE") || !uniform) {  // debug override changes the tiling: fall back to per-job launches
+  if (!uniform) {
     for (int i = 0; i < n; ++i) CTN_TRY(ctn_umma_build_wimg(jobs[i].W, jobs[i].M, jobs[i].K, math, jobs[i].wimg, st));
     return CTN_OK;
   }
@@ -846,8 +548,7 @@ int ctn_umma_build_wimg_batch(const WimgJob* jobs, int n, int math, cudaStream_t
     int maxb = 1;
     for (int i = 0; i < m; ++i) {
       wj.j[i] = jobs[i0 + i];
-      const int n_tile = pick_n_tile(jobs[i0 + i].M);
-      const int blocks = ((jobs[i0 + i].M + n_tile - 1) / n_tile) * ((jobs[i0 + i].K + KS - 1) / KS);
+      const int blocks = ((jobs[i0 + i].M + NT - 1) / NT) * ((jobs[i0 + i].K + KS - 1) / KS);
       if (blocks > maxb) maxb = blocks;
     }
     if (math == CTN_MATH_F16X3) k_build_wimg_batch_f16<<<dim3(64, m), 512, 0, st>>>(wj);
@@ -858,84 +559,39 @@ int ctn_umma_build_wimg_batch(const WimgJob* jobs, int n, int math, cudaStream_t
   return CTN_OK;
 }
 
-#define NPREC_HOST(m) ((m) == CTN_MATH_TF32 ? 1u : 2u)
+// fused mask + decoder epilogue: fp16-piece mode, whole n-tiles per source, decoder basis (Nb, 1, 16) with kernel 16 / stride 8
+int ctn_pw_maskdec_supported(const PwArgs& a, int math) {
+  return eff_math(a.M, math) == CTN_MATH_F16X3 && a.dec_w && a.Nb > 0 && a.Nb % NT == 0 && a.M % a.Nb == 0 &&
+         (((uintptr_t)a.dec_w) & 15) == 0;
+}
+
 int ctn_pw_umma(const PwArgs& a, int pro, int epi, int math, cudaStream_t st) {
   if (!a.wimg) return CTN_EINVAL;
   math = eff_math(a.M, math);
   if (a.pitch % TM != 0) return CTN_EALIGN;
   if ((((uintptr_t)a.A) | ((uintptr_t)a.wimg)) & 15) return CTN_EALIGN;
-  UmmaArgs g;
+  TcArgs g;
   g.a = a;
   g.wimg = a.wimg;
-  g.n_tile = pick_n_tile(a.M);
-  g.n_tiles = (a.M + g.n_tile - 1) / g.n_tile;
+  g.n_tiles = (a.M + NT - 1) / NT;
   g.k_slabs = (a.K + KS - 1) / KS;
   g.t_tiles = a.pitch / TM;
-  g.num_items = a.B * g.t_tiles * g.n_tiles;
-  const int nprec = math == CTN_MATH_TF32 ? 1 : 2;
-  const bool f16 = math == CTN_MATH_F16X3;
-  const uint32_t a_bytes = f16 ? (uint32_t)(TM * KS * 2) : (uint32_t)A_BYTES;
-  g.w_bytes = (uint32_t)g.n_tile * (uint32_t)(KS * (f16 ? 2 : 4));
-  static const char* env_dbg = getenv("CTN_UMMA_DBG");
-  g.dbg = env_dbg ? (uint32_t)atoi(env_dbg) : 0u;
-  int grid = num_sms();
-  static const char* env_grid = getenv("CTN_UMMA_GRID");
-  if (env_grid && atoi(env_grid) > 0) grid = atoi(env_grid);
-  // CTA pairs (cluster of 2, tcgen05 cta_group::2; opt-in with CTN_UMMA_CLUSTER=2): one MMA covers two time tiles
-  // (M = 256) and each CTA stages only HALF of the weight slab, so a stage shrinks from 96 KB to 64 KB (3xTF32, n_tile
-  // 256) and the ring gets 3 stages instead of 2.  Parity-green on B200, but measured perf-neutral on cfg2 (10.59 vs
-  // 10.56 ms/step): with MMA-only (3.9 ms) and producer-only (4.2 ms) floors this close, the third stage does not buy
-  // overlap yet, so the simpler 1-CTA kernel stays the default (DESIGN.md section 6).
-  static const char* env_cl = getenv("CTN_UMMA_CLUSTER");
-  int cluster = env_cl ? atoi(env_cl) : 1;
-  if (cluster != 1 && cluster != 2) cluster = 1;
-  if (f16) cluster = 1;  // fp16 operands: single-CTA kernel only
-  g.tiles_total = a.B * g.t_tiles;
-  static const char* env_pm = getenv("CTN_UMMA_PAIR_MIN_N");
-  const int pair_min_n = env_pm ? atoi(env_pm) : 64;  // N = 64 / 256 are the pair shapes pinned by tools/umma_unit2.cu
-  if (cluster == 2 && (grid % 2 != 0 || g.tiles_total < 2 || g.n_tile % 32 != 0 || g.n_tile < pair_min_n)) cluster = 1;
-  g.cluster = cluster;
-  const uint32_t w_stage = cluster == 2 ? g.w_bytes / 2 : g.w_bytes;
-  g.stage_bytes = (uint32_t)nprec * (a_bytes + w_stage);
-  const size_t budget = 227 * 1024 - SMEM_HEADER - 1024;
-  int stages = (int)(budget / g.stage_bytes);
-  if (stages > MAX_STAGES) stages = MAX_STAGES;
-  static const char* env_st = getenv("CTN_UMMA_STAGES");
-  if (env_st && atoi(env_st) >= 1 && atoi(env_st) < stages) stages = atoi(env_st);
-  if (stages < 1) return CTN_EUNSUPPORTED;
-  g.stages = stages;
-  g.oscale = nullptr;
-  if (f16) {
-    g.oscale = reinterpret_cast<const float*>(reinterpret_cast<const uint8_t*>(a.wimg) + wimg_f16_image_bytes(g.n_tile, g.n_tiles, g.k_slabs));
-    g.idesc = ptx::make_idesc_f16(TM, g.n_tile, /*A MN-major*/ 1, /*B K-major*/ 0);
-    g.lbo_a = 1024u; g.sbo_a = 2048u; g.a_layout = 2u;  // 64-time-step atoms adjacent, 8-channel groups 2048 B apart
-    g.lbo_w = 16u; g.sbo_w = 512u; g.w_layout = 4u;      // SWIZZLE_64B rows of 32 k
-  } else {
-    g.idesc = a.dbg_idesc ? a.dbg_idesc : ptx::make_idesc_tf32(cluster == 2 ? 2 * TM : TM, g.n_tile, /*A MN-major*/ 1, /*B K-major*/ 0);
-    g.lbo_a = a.dbg_lbo_a ? a.dbg_lbo_a : 512u;   // between 32-time-step atoms
-    g.sbo_a = a.dbg_sbo_a ? a.dbg_sbo_a : 2048u;  // between 4-channel groups
-    g.lbo_w = 16u;                                 // unused for swizzled K-major
-    g.sbo_w = a.dbg_sbo_w ? a.dbg_sbo_w : W_SBO;  // between 8-row (output channel) groups
-    g.a_layout = 1u; g.w_layout = W_LAYOUT;
+  g.oscale = math == CTN_MATH_F16X3
+                 ? reinterpret_cast<const float*>(reinterpret_cast<const uint8_t*>(a.wimg) + wimg_f16_image_bytes(NT, g.n_tiles, g.k_slabs))
+                 : nullptr;
+  g.nt_per_cta = 1;
+  const bool train_dw = pro == PRO_DW && a.dw_u_pre_out != nullptr;
+  if (pro == PRO_NONE && epi == EPI_RAW) return launch_math<PRO_NONE, EPI_RAW>(g, math, st);
+  if (pro == PRO_DW && epi == EPI_RAW)
+    return train_dw ? launch_math<PRO_DW, EPI_RAW, true>(g, math, st) : launch_math<PRO_DW, EPI_RAW>(g, math, st);
+  if (pro == PRO_NONE && epi == EPI_HEAD) return launch_math<PRO_NONE, EPI_HEAD>(g, math, st);
+  if (pro == PRO_NONE && epi == EPI_H) return launch_math<PRO_NONE, EPI_H>(g, math, st);
+  if (pro == PRO_RES && epi == EPI_H) return launch_math<PRO_RES, EPI_H>(g, math, st);
+  if (pro == PRO_PRELU && epi == EPI_MASK) return launch_math<PRO_PRELU, EPI_MASK>(g, math, st);
+  if (pro == PRO_PRELU && epi == EPI_MASKDEC) {
+    if (!ctn_pw_maskdec_supported(a, math)) return CTN_EUNSUPPORTED;
+    g.nt_per_cta = a.Nb / NT;  // one CTA per (sample, time tile, source): the decoder sums over the source's channels
+    return launch<PRO_PRELU, EPI_MASKDEC, 3, true, false>(g, st);
   }
-  const size_t smem = SMEM_HEADER + 1024 + (size_t)stages * g.stage_bytes;
-  static const char* env_ws = getenv("CTN_UMMA_WSPLIT");
-  g.wsplit = env_ws ? atoi(env_ws) : 1;
-  if (g.wsplit < 1 || g.wsplit > 16 || ((NPREC_HOST(math) * g.w_bytes / g.wsplit) % 16) != 0) g.wsplit = 1;
-  g.cluster_items = g.n_tiles * ((g.tiles_total + cluster - 1) / cluster);
-  const int max_grid = g.cluster_items * cluster;
-  if (grid > max_grid) grid = max_grid;
-#define UM_LAUNCH(P, E)                                                                   \
-  if (pro == P && epi == E)                                                               \
-    return f16 ? launch<P, E, 3, false, true>(g, smem, grid, st)                                                                  \
-           : nprec == 2 ? (cluster == 2 ? launch<P, E, 3, true, false>(g, smem, grid, st) : launch<P, E, 3, false, false>(g, smem, grid, st)) \
-                        : (cluster == 2 ? launch<P, E, 1, true, false>(g, smem, grid, st) : launch<P, E, 1, false, false>(g, smem, grid, st));
-  UM_LAUNCH(PRO_NONE, EPI_RAW)
-  UM_LAUNCH(PRO_DW, EPI_RAW)
-  UM_LAUNCH(PRO_NONE, EPI_HEAD)
-  UM_LAUNCH(PRO_NONE, EPI_H)
-  UM_LAUNCH(PRO_RES, EPI_H)
-  UM_LAUNCH(PRO_PRELU, EPI_MASK)
-#undef UM_LAUNCH
   return CTN_EUNSUPPORTED;
 }

@@ -1,5 +1,5 @@
-// Raw PTX wrappers for the Blackwell (sm_100a) features the pointwise kernels use: mbarrier, 1-D bulk async copy
-// (TMA engine, UBLKCP), tcgen05 alloc / mma / commit / ld, proxy fences.  No CUTLASS dependency.
+// Raw PTX wrappers for the Hopper (sm_90a) features the tensor-core kernels use: mbarrier, 1-D bulk async copy (TMA
+// engine), clusters / distributed shared memory, wgmma, proxy fences.  No CUTLASS dependency.
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -32,7 +32,7 @@ __device__ __forceinline__ void mbar_wait(uint32_t bar, uint32_t parity) {
 }
 
 // ---- async proxy -----------------------------------------------------------------------------------------------
-// generic-proxy st.shared writes -> visible to the async proxy (tcgen05.mma operand reads)
+// generic-proxy st.shared writes -> visible to the async proxy (wgmma operand reads, bulk copies)
 __device__ __forceinline__ void fence_proxy_async_smem() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
 
 // 1-D bulk copy global -> shared, completion on an mbarrier (complete_tx::bytes).  size % 16 == 0, 16-byte aligned.
@@ -51,7 +51,7 @@ __device__ __forceinline__ void bulk_g2s_multicast(uint32_t dst_smem, const void
 }
 
 // one lane of a converged warp (elect.sync): code under this predicate is known single-threaded to the compiler, so
-// uniform-datapath instructions (tcgen05.mma / commit) are emitted without per-instruction election loops
+// uniform-datapath instructions are emitted without per-instruction election loops
 __device__ __forceinline__ bool elect_one() {
   uint32_t pred = 0;
   asm volatile(
@@ -101,7 +101,7 @@ __device__ __forceinline__ void mbar_wait_cluster(uint32_t bar, uint32_t parity)
 
 // bulk copy from this CTA's shared memory into the SAME offsets of CTA `rank` of the cluster (distributed shared memory), completing
 // on the mbarrier at `bar` (CTA-relative address) in that CTA: the transfer runs in the async proxy on both sides, so the
-// receiver's tcgen05.mma may read the data right after its mbarrier wait.  16-byte aligned, size % 16 == 0.
+// receiver's wgmma may read the data right after its mbarrier wait.  16-byte aligned, size % 16 == 0.
 __device__ __forceinline__ void bulk_s2peer(uint32_t dst_smem, uint32_t src_smem, uint32_t bytes, uint32_t bar, uint32_t rank) {
   asm volatile(
       "{\n\t"
@@ -124,125 +124,29 @@ __device__ __forceinline__ void st_peer_v4(uint32_t local_addr, uint32_t rank, u
       : "memory");
 }
 
-// ---- tcgen05 ---------------------------------------------------------------------------------------------------
-__device__ __forceinline__ void tmem_alloc(uint32_t smem_dst, uint32_t ncols) {  // whole warp
-  asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_dst), "r"(ncols) : "memory");
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr, uint32_t ncols) {  // whole warp (the allocating one)
-  asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
-}
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
+// ---- wgmma (Hopper warpgroup MMA) -----------------------------------------------------------------------------------
+// D (64 x 128, fp32, registers of the 128 threads of a warpgroup) += A (64 x K, shared memory) * B (128 x K, shared memory)^T.
+// Both operands K-major.  Accumulator fragment of thread (warp w of the group, lane l), register i:
+//   row = 16 w + l / 4 + 8 ((i / 2) % 2),  column = 8 (i / 4) + 2 (l % 4) + i % 2.
+__device__ __forceinline__ void wg_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wg_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void wg_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory"); }
 
-// D[tmem] (+)= A[smem desc] * B[smem desc]^T, kind::tf32, issued by ONE thread
-__device__ __forceinline__ void mma_tf32(uint32_t tmem_d, uint64_t desc_a, uint64_t desc_b, uint32_t idesc, uint32_t accumulate) {
+__device__ __forceinline__ void wg_mma_tf32(float (&d)[64], uint64_t da, uint64_t db) {
   asm volatile(
-      "{\n\t"
-      ".reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::tf32 [%0], %1, %2, %3, p;\n\t"
-      "}" ::"r"(tmem_d), "l"(desc_a), "l"(desc_b), "r"(idesc), "r"(accumulate)
-      : "memory");
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, 1, 0;\n\twgmma.mma_async.sync.aligned.m64n128k8.f32.tf32.tf32 "
+      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, %64, %65, p, 1, 1;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+      : "l"(da), "l"(db));
 }
-// same with fp16 operands (K = 16 per instruction, twice the rate of kind::tf32)
-__device__ __forceinline__ void mma_f16(uint32_t tmem_d, uint64_t desc_a, uint64_t desc_b, uint32_t idesc, uint32_t accumulate) {
+__device__ __forceinline__ void wg_mma_f16(float (&d)[64], uint64_t da, uint64_t db) {
   asm volatile(
-      "{\n\t"
-      ".reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t"
-      "}" ::"r"(tmem_d), "l"(desc_a), "l"(desc_b), "r"(idesc), "r"(accumulate)
-      : "memory");
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, 1, 0;\n\twgmma.mma_async.sync.aligned.m64n128k16.f32.f16.f16 "
+      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, %64, %65, p, 1, 1, 0, 0;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+      : "l"(da), "l"(db));
 }
-// arrive on an mbarrier when all previously issued tcgen05.mma of this thread have completed
-__device__ __forceinline__ void mma_commit(uint32_t bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(bar) : "memory");
-}
-
-// same, arriving on the barrier at this CTA-relative offset in every CTA of cta_mask
-__device__ __forceinline__ void mma_commit_multicast(uint32_t bar, uint16_t cta_mask) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;" ::"r"(bar),
-               "h"(cta_mask)
-               : "memory");
-}
-
-// ---- 2-CTA (cta_group::2) forms: one MMA spans a CTA pair (M = 256), each CTA stages its 128 rows of A and its half
-// of B; allocation / deallocation are executed by the same warp index in BOTH CTAs (verified with tools/umma_unit2.cu)
-__device__ __forceinline__ void tmem_alloc2(uint32_t smem_dst, uint32_t ncols) {
-  asm volatile("tcgen05.alloc.cta_group::2.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_dst), "r"(ncols) : "memory");
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::2.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc2(uint32_t taddr, uint32_t ncols) {
-  asm volatile("tcgen05.dealloc.cta_group::2.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
-}
-__device__ __forceinline__ void mma2_tf32(uint32_t tmem_d, uint64_t desc_a, uint64_t desc_b, uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n\t"
-      ".reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::2.kind::tf32 [%0], %1, %2, %3, p;\n\t"
-      "}" ::"r"(tmem_d), "l"(desc_a), "l"(desc_b), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-__device__ __forceinline__ void mma2_f16(uint32_t tmem_d, uint64_t desc_a, uint64_t desc_b, uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n\t"
-      ".reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::2.kind::f16 [%0], %1, %2, %3, p;\n\t"
-      "}" ::"r"(tmem_d), "l"(desc_a), "l"(desc_b), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-__device__ __forceinline__ void mma2_commit_multicast(uint32_t bar, uint16_t cta_mask) {
-  asm volatile("tcgen05.commit.cta_group::2.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;" ::"r"(bar),
-               "h"(cta_mask)
-               : "memory");
-}
-
-// 32 lanes x 32 columns of fp32: thread i of the warp receives columns [col, col+32) of TMEM lane (base_lane + i)
-__device__ __forceinline__ void tmem_ld32(uint32_t taddr, uint32_t (&v)[32]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-      : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7]), "=r"(v[8]),
-        "=r"(v[9]), "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]), "=r"(v[14]), "=r"(v[15]), "=r"(v[16]),
-        "=r"(v[17]), "=r"(v[18]), "=r"(v[19]), "=r"(v[20]), "=r"(v[21]), "=r"(v[22]), "=r"(v[23]), "=r"(v[24]),
-        "=r"(v[25]), "=r"(v[26]), "=r"(v[27]), "=r"(v[28]), "=r"(v[29]), "=r"(v[30]), "=r"(v[31])
-      : "r"(taddr)
-      : "memory");
-}
-__device__ __forceinline__ void tmem_ld16(uint32_t taddr, uint32_t (&v)[16]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x16.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];"
-      : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7]), "=r"(v[8]),
-        "=r"(v[9]), "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]), "=r"(v[14]), "=r"(v[15])
-      : "r"(taddr)
-      : "memory");
-}
-__device__ __forceinline__ void tmem_ld_wait() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
-
-// ---- A operand in tensor memory ("ts" form) ------------------------------------------------------------------------
-// D[tmem] (+)= A[tmem] * B[smem desc]^T, kind::f16.  A: lane = row m, 32-bit column j = {A[m][2j] (low half), A[m][2j+1]}; one
-// instruction consumes 8 columns (K = 16).  Layout verified on B200 with tools/umma_unit_ts.cu.
-__device__ __forceinline__ void mma_f16_ts(uint32_t tmem_d, uint32_t tmem_a, uint64_t desc_b, uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n\t"
-      ".reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], [%1], %2, %3, p;\n\t"
-      "}" ::"r"(tmem_d), "r"(tmem_a), "l"(desc_b), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-// thread i of the warp writes 8 consecutive 32-bit columns of TMEM lane (base_lane + i)
-__device__ __forceinline__ void tmem_st8(uint32_t taddr, const uint32_t (&v)[8]) {
-  asm volatile("tcgen05.st.sync.aligned.32x32b.x8.b32 [%0], {%1, %2, %3, %4, %5, %6, %7, %8};" ::"r"(taddr), "r"(v[0]), "r"(v[1]),
-               "r"(v[2]), "r"(v[3]), "r"(v[4]), "r"(v[5]), "r"(v[6]), "r"(v[7])
-               : "memory");
-}
-__device__ __forceinline__ void tmem_st_wait() { asm volatile("tcgen05.wait::st.sync.aligned;" ::: "memory"); }
 
 // round-to-nearest fp32 -> tf32 (result is an fp32 bit pattern with the low 13 mantissa bits cleared)
 __device__ __forceinline__ float to_tf32(float x) {
@@ -271,34 +175,14 @@ __device__ __forceinline__ void split_f16x2(float x0, float x1, uint32_t& hi, ui
 __device__ __forceinline__ float hi_tf32(float x) { return __uint_as_float((__float_as_uint(x) + 0x1000u) & 0xffffe000u); }
 
 // ---- descriptors -------------------------------------------------------------------------------------------------
-// Shared-memory matrix descriptor (sm_100 "version 1"), SWIZZLE_128B canonical layouts:
-//   bits [0,14) start address >> 4 | [16,30) leading byte offset >> 4 | [32,46) stride byte offset >> 4
-//   [46,48) version = 1 | [49,52) base offset = 0 | [61,64) layout type (2 = SWIZZLE_128B)
-//   layout types: 2 = SWIZZLE_128B (16-byte chunks XOR row%8; K-major tf32 and all 16-bit operands),
-//                 1 = SWIZZLE_128B_BASE32B (32-byte chunks XOR row%4) -- the ONLY layout the hardware accepts for
-//                     MN-major 32-bit (tf32) operands (measured: SWIZZLE_128B MN-major tf32 returns zeros).
-__host__ __device__ __forceinline__ uint64_t make_smem_desc(uint32_t smem_addr, uint32_t lbo_bytes, uint32_t sbo_bytes,
-                                                            uint32_t layout_type = 2) {
-  uint64_t d = 0;
-  d |= (uint64_t)((smem_addr >> 4) & 0x3FFF);
-  d |= (uint64_t)((lbo_bytes >> 4) & 0x3FFF) << 16;
-  d |= (uint64_t)((sbo_bytes >> 4) & 0x3FFF) << 32;
-  d |= (uint64_t)1 << 46;
-  d |= (uint64_t)layout_type << 61;
-  return d;
-}
-// Instruction descriptor for kind::tf32, fp32 accumulate, M = 128:
-//   [4,6) c_format = 1 (F32) | [7,10) a_format = 2 (TF32) | [10,13) b_format = 2 | [15] a_major | [16] b_major
-//   [17,23) N >> 3 | [24,29) M >> 4
-__host__ __device__ __forceinline__ uint32_t make_idesc_tf32(int M, int N, int a_mn_major, int b_mn_major) {
-  return (1u << 4) | (2u << 7) | (2u << 10) | ((uint32_t)a_mn_major << 15) | ((uint32_t)b_mn_major << 16) |
-         ((uint32_t)(N >> 3) << 17) | ((uint32_t)(M >> 4) << 24);
-}
-
-// kind::f16 with F16 inputs (a_format = b_format = 0), fp32 accumulate
-__host__ __device__ __forceinline__ uint32_t make_idesc_f16(int M, int N, int a_mn_major, int b_mn_major) {
-  return (1u << 4) | ((uint32_t)a_mn_major << 15) | ((uint32_t)b_mn_major << 16) | ((uint32_t)(N >> 3) << 17) |
-         ((uint32_t)(M >> 4) << 24);
+// sm_90 shared-memory matrix descriptor of a K-major operand in a swizzled canonical layout:
+//   bits [0,14) start address >> 4 | [16,30) leading byte offset >> 4 (unused by swizzled K-major layouts) |
+//   [32,46) stride byte offset >> 4 = bytes between 8-row groups | [62,64) layout: 1 = SWIZZLE_128B, 2 = SWIZZLE_64B.
+// Rows are 128 B (SWIZZLE_128B: 16-byte chunk index XOR row % 8) or 64 B (SWIZZLE_64B: chunk index XOR (row / 2) % 4); the
+// start address of the k-th 32-byte column step is base + 32 k.
+constexpr uint32_t SW128 = 1u, SW64 = 2u;
+__device__ __forceinline__ uint64_t wg_desc(uint32_t smem_addr, uint32_t sbo_bytes, uint32_t layout) {
+  return (uint64_t)((smem_addr & 0x3FFFFu) >> 4) | ((uint64_t)1 << 16) | ((uint64_t)(sbo_bytes >> 4) << 32) | ((uint64_t)layout << 62);
 }
 
 }  // namespace ptx

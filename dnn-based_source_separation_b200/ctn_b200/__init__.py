@@ -1,4 +1,4 @@
-"""ctn_b200 -- B200-native Conv-TasNet separation path (sm_100a CUDA behind the reference's class API).
+"""ctn_b200 -- H100-native Conv-TasNet separation path (sm_90a CUDA behind the reference's class API).
 
     from ctn_b200.models.conv_tasnet import ConvTasNet
     from ctn_b200.criterion.sdr import NegSISDR
@@ -14,7 +14,7 @@ __version__ = "0.1.0"
 
 
 def set_default_math(mode: str) -> None:
-    """'f16x3' (tcgen05 3-pass fp16 split, fp32-parity; the default when the tcgen05 family is built), 'tf32x3' (3-pass TF32 split),
+    """'f16x3' (wgmma 3-pass fp16 split, fp32-parity; the default when the tensor-core family is built), 'tf32x3' (3-pass TF32 split),
     'tf32' (single pass, looser tolerance) or 'fp32' (CUDA-core FFMA).  One switch for every model class (ConvTasNet, DPRNNTasNet,
     stand-alone TimeDilatedConvNet / Separator): it lives in models.tdcn.DEFAULT_MATH."""
     from .models import tdcn

@@ -16,7 +16,7 @@ LIB_PATH = os.environ.get("CTN_B200_LIB", os.path.join(os.path.dirname(_HERE), "
 
 if not os.path.exists(LIB_PATH):
     raise ImportError(
-        f"{LIB_PATH} not found: build the sm_100a extension first "
+        f"{LIB_PATH} not found: build the sm_90a extension first "
         "(python -c 'import __graft_entry__ as g; g.build()' or dnn-based_source_separation_b200/csrc/build.sh). "
         "There is no CPU fallback.")
 
@@ -151,7 +151,7 @@ def require_cuda(*tensors: torch.Tensor) -> torch.device:
         if t is None:
             continue
         if not t.is_cuda:
-            raise RuntimeError("ctn_b200 runs on CUDA (sm_100a) tensors only; there is no CPU fallback")
+            raise RuntimeError("ctn_b200 runs on CUDA (sm_90a) tensors only; there is no CPU fallback")
         if t.dtype != torch.float32:
             raise TypeError(f"ctn_b200 computes in float32, got {t.dtype}")
         if dev is None:

@@ -1,4 +1,4 @@
-"""SDR-family criteria on sm_100a kernels, mirroring src/criterion/sdr.py: ``sdr`` / ``SDR`` / ``NegSDR`` (:6-110), ``sisdr``
+"""SDR-family criteria on sm_90a kernels, mirroring src/criterion/sdr.py: ``sdr`` / ``SDR`` / ``NegSDR`` (:6-110), ``sisdr``
 (:122-139), ``SISDR`` (:141-185), ``NegSISDR`` (:187-231), ``ClippedSISDR`` / ``ClippedNegSISDR`` (:233-327).
 Inputs (batch_size, T), (batch_size, n_sources, T) or (batch_size, n_sources, n_mics, T).  ``sisdr`` is differentiable w.r.t. its
 input; ``sdr`` is forward only (evaluation metric)."""
@@ -43,7 +43,7 @@ def sdr(input, target, eps=EPS):
     if input.shape != target.shape:
         raise ValueError("input and target must have the same shape")
     if torch.is_grad_enabled() and (input.requires_grad or target.requires_grad):
-        raise NotImplementedError("sdr() is forward only on the sm_100a path (train with sisdr / NegSISDR)")
+        raise NotImplementedError("sdr() is forward only on the sm_90a path (train with sisdr / NegSISDR)")
     x, t = input.contiguous(), target.contiguous()
     dev = N.require_cuda(x, t)
     T = x.shape[-1]

@@ -1,4 +1,4 @@
-"""Conv-TasNet on hand-written sm_100a kernels, behind the reference's class API.
+"""Conv-TasNet on hand-written sm_90a kernels, behind the reference's class API.
 
 Mirrors src/models/conv_tasnet.py of the reference: ``ConvTasNet`` (:16-320; constructor :57-66, forward :116-119,
 extract_latent :121-171, get_config :173-198, build_model :199-236) and ``Separator`` (:322-378).  Module tree and
@@ -293,7 +293,7 @@ class ConvTasNet(nn.Module):
         synchronises the stream before reading them."""
         dev = self.encoder.conv1d.weight.device
         if dev.type != "cuda":
-            raise RuntimeError("ctn_b200 runs on CUDA (sm_100a) only; there is no CPU fallback")
+            raise RuntimeError("ctn_b200 runs on CUDA (sm_90a) only; there is no CPU fallback")
         B, _, T = mixture_host.shape
         key = (B, T, dev)
         st = getattr(self, "_host_state", None)

@@ -5,8 +5,8 @@
 
 What runs where: the dual-path state lives CHANNELS-LAST, (batch, D1, D2, features) -- already the batch_first tensor the
 path's LSTM consumes, so none of the reference's permute().contiguous() copies exist.  For num_features / hidden_channels in
-{32, 64, 128} (cfg4: 64 / 128) the bi-LSTM recurrence AND the 2H -> F Linear run in one tcgen05 kernel with h resident in tensor
-memory (``ctn_bilstm_proj_fwd``, csrc/ctn_lstm.cu): the (batch*D1, D2, 2H) LSTM output is never written.  gLN statistics,
+{32, 64, 128} (cfg4: 64 / 128) the bi-LSTM recurrence AND the 2H -> F Linear run in one native wgmma kernel (3xTF32)
+(``ctn_bilstm_proj_fwd``, csrc/ctn_lstm.cu): the (batch*D1, D2, 2H) LSTM output is never written.  gLN statistics,
 normalisation, the sum of the two directions' partial projections + bias, the residual add and the intra <-> inter layout swap are
 one more native call (``ctn_dprnn_norm_res2_fwd``).  Other sizes fall back to cuDNN's LSTM (IEEE fp32) + a library GEMM +
 ``ctn_dprnn_norm_res_fwd``; ``NATIVE_LSTM = False`` forces that path (it is the A/B baseline of bench.py --config cfg4).
@@ -25,7 +25,7 @@ from .transform import ctn_dprnn_norm_res_fwd
 EPS = 1e-12
 
 
-NATIVE_LSTM = True  # tcgen05 recurrence (csrc/ctn_lstm.cu) where the sizes allow; False = cuDNN + library GEMM everywhere
+NATIVE_LSTM = True  # native recurrence (csrc/ctn_lstm.cu) where the sizes allow; False = cuDNN + library GEMM everywhere
 LSTM_TF32 = False  # cuDNN's RNN path defaults to TF32 tensor-core math (1e-3 relative): off = fp32 parity with the reference
 
 
@@ -70,11 +70,11 @@ class _ChunkRNN(nn.Module):
         if rnn_type != 'lstm':
             raise NotImplementedError("Not support {}.".format(rnn_type))
         if causal_rnn:
-            raise NotImplementedError("causal DPRNN (uni-directional inter-chunk LSTM + cLN) is outside the sm_100a path")
+            raise NotImplementedError("causal DPRNN (uni-directional inter-chunk LSTM + cLN) is outside the sm_90a path")
         self.rnn = choose_rnn(rnn_type, input_size=num_features, hidden_size=hidden_channels, batch_first=True, bidirectional=True)
         self.fc = nn.Linear(2 * hidden_channels, num_features)
         if not norm:
-            raise NotImplementedError("norm=False is outside the sm_100a path")
+            raise NotImplementedError("norm=False is outside the sm_90a path")
         self.norm1d = choose_layer_norm('gLN', num_features, causal=False, eps=eps)
         self.eps = eps
 

@@ -2,9 +2,9 @@
 
 Same constructors, ``forward`` / ``extract_latent`` / ``get_config`` / ``build_model`` and the same ``state_dict`` keys as the
 reference, so its checkpoints load with ``load_state_dict``.  Forward = encoder kernel (+ gLN statistics) -> gLN folded
-into the bottleneck 1x1 (tcgen05) -> pad + Segment1d straight into the channels-last dual-path layout -> B x (intra, inter)
+into the bottleneck 1x1 (wgmma) -> pad + Segment1d straight into the channels-last dual-path layout -> B x (intra, inter)
 blocks (cuDNN LSTM + library GEMM between native gLN / residual / layout-swap calls, see dprnn.py) -> OverlapAdd1d + crop ->
-PReLU + mask 1x1 + sigmoid + w * mask (tcgen05) -> transposed-conv decoder + crop.
+PReLU + mask 1x1 + sigmoid + w * mask (wgmma) -> transposed-conv decoder + crop.
 Envelope: trainable bases, monaural 3-D input, non-causal, rnn_type='lstm', sigmoid mask; forward only.
 """
 import ctypes as C
@@ -33,7 +33,7 @@ class Separator(nn.Module):
         self.chunk_size, self.hop_size = chunk_size, hop_size
         self.norm, self.eps = norm, eps
         if causal:
-            raise NotImplementedError("causal DPRNN-TasNet (cLN, uni-directional inter-chunk LSTM) is outside the sm_100a path")
+            raise NotImplementedError("causal DPRNN-TasNet (cLN, uni-directional inter-chunk LSTM) is outside the sm_90a path")
         self.norm1d = choose_layer_norm('gLN', num_features, causal=False, eps=eps)
         self.bottleneck_conv1d = nn.Conv1d(num_features, bottleneck_channels, kernel_size=1, stride=1)
         self.segment1d = Segment1d(chunk_size, hop_size)
@@ -44,7 +44,7 @@ class Separator(nn.Module):
         if mask_nonlinear == 'sigmoid':
             pass
         elif mask_nonlinear == 'softmax':
-            raise NotImplementedError("mask_nonlinear='softmax' is outside the sm_100a kernel envelope")
+            raise NotImplementedError("mask_nonlinear='softmax' is outside the sm_90a kernel envelope")
         else:
             raise ValueError("Cannot support {}".format(mask_nonlinear))
         self.math = None
@@ -128,7 +128,7 @@ class DPRNNTasNet(nn.Module):
             assert input.size(1) == 1, "input.size() is expected (?, 1, ?), but given {}".format(input.size())
         elif n_dim == 4:
             assert input.size(1) == 1, "input.size() is expected (?, 1, ?, ?), but given {}".format(input.size())
-            raise NotImplementedError("multichannel (4-D) input is outside the sm_100a kernel envelope")
+            raise NotImplementedError("multichannel (4-D) input is outside the sm_90a kernel envelope")
         else:
             raise ValueError("Not support {} dimension input".format(n_dim))
         if torch.is_grad_enabled() and any(p.requires_grad for p in self.parameters()):

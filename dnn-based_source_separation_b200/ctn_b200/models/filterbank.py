@@ -1,4 +1,4 @@
-"""Trainable encoder / decoder filterbanks on sm_100a kernels.
+"""Trainable encoder / decoder filterbanks on sm_90a kernels.
 
 Mirrors ``Encoder`` (src/models/filterbank.py:205-235) and ``Decoder`` (:237-251) of the reference: same constructor,
 same ``conv1d.weight`` / ``conv_transpose1d.weight`` parameters, same forward shapes.  The nn.Conv1d /
@@ -15,7 +15,7 @@ class Encoder(nn.Module):
     def __init__(self, in_channels, n_basis, kernel_size=16, stride=8, nonlinear=None):
         super().__init__()
         if in_channels < 1 or in_channels > 64:
-            raise NotImplementedError("in_channels={} is outside the sm_100a path (1 .. 64)".format(in_channels))
+            raise NotImplementedError("in_channels={} is outside the sm_90a path (1 .. 64)".format(in_channels))
         self.in_channels, self.n_basis = in_channels, n_basis
         self.kernel_size, self.stride = kernel_size, stride
         self.conv1d = nn.Conv1d(in_channels, n_basis, kernel_size=kernel_size, stride=stride, bias=False)
@@ -58,7 +58,7 @@ class Decoder(nn.Module):
     def __init__(self, n_basis, out_channels, kernel_size=16, stride=8):
         super().__init__()
         if out_channels < 1 or out_channels > 64:
-            raise NotImplementedError("out_channels={} is outside the sm_100a path (1 .. 64)".format(out_channels))
+            raise NotImplementedError("out_channels={} is outside the sm_90a path (1 .. 64)".format(out_channels))
         self.n_basis, self.out_channels = n_basis, out_channels
         self.kernel_size, self.stride = kernel_size, stride
         self.conv_transpose1d = nn.ConvTranspose1d(n_basis, out_channels, kernel_size=kernel_size, stride=stride, bias=False)
@@ -72,7 +72,7 @@ class Decoder(nn.Module):
         BS, _, frames = x.shape
         L, S = self.kernel_size, self.stride
         if L % S != 0:
-            raise NotImplementedError("kernel_size % stride != 0 is outside the sm_100a decoder envelope")
+            raise NotImplementedError("kernel_size % stride != 0 is outside the sm_90a decoder envelope")
         T_out = (frames - 1) * S + L
         y = torch.empty(BS, self.out_channels, T_out, dtype=torch.float32, device=dev)
         if self.out_channels > 1:

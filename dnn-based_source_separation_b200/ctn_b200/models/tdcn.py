@@ -1,4 +1,4 @@
-"""Time-dilated convolutional network (the Conv-TasNet separator core) on sm_100a kernels.
+"""Time-dilated convolutional network (the Conv-TasNet separator core) on sm_90a kernels.
 
 Mirrors src/models/tdcn.py of the reference -- ``TimeDilatedConvNet`` (:13-41), ``TimeDilatedConvBlock1d`` (:43-75),
 ``ResidualBlock1d`` (:77-147), ``DepthwiseSeparableConv1d`` (:149-196): same constructors, same module tree and
@@ -21,7 +21,7 @@ from .. import _native as N
 from ..utils.tasnet import choose_layer_norm
 
 EPS = 1e-12
-DEFAULT_MATH = None  # None -> 'f16x3' when the tcgen05 family is built, else 'fp32'
+DEFAULT_MATH = None  # None -> 'f16x3' when the tensor-core family is built, else 'fp32'
 
 
 def resolve_math(mode=None):
@@ -57,7 +57,7 @@ class DepthwiseSeparableConv1d(nn.Module):
         self.skip_pointwise_conv1d = nn.Conv1d(in_channels, skip_channels, kernel_size=1, stride=1)
 
     def forward(self, input):
-        raise NotImplementedError("DepthwiseSeparableConv1d is fused into TimeDilatedConvNet.forward on the sm_100a path")
+        raise NotImplementedError("DepthwiseSeparableConv1d is fused into TimeDilatedConvNet.forward on the sm_90a path")
 
 
 class ResidualBlock1d(nn.Module):
@@ -67,7 +67,7 @@ class ResidualBlock1d(nn.Module):
                  separable=False, causal=True, nonlinear=None, norm=True, dual_head=True, eps=EPS):
         super().__init__()
         if not separable:
-            raise NotImplementedError("separable=False is outside the sm_100a kernel envelope")
+            raise NotImplementedError("separable=False is outside the sm_90a kernel envelope")
         self.kernel_size, self.stride, self.dilation = kernel_size, stride, dilation
         self.separable, self.causal, self.norm, self.dual_head = separable, causal, norm, dual_head
         self.bottleneck_conv1d = nn.Conv1d(num_features, hidden_channels, kernel_size=1, stride=1)
@@ -105,7 +105,7 @@ class TimeDilatedConvBlock1d(nn.Module):
                  separable=False, causal=True, nonlinear=None, norm=True, dual_head=True, eps=EPS):
         super().__init__()
         if not dilated:
-            raise NotImplementedError("dilated=False is outside the sm_100a kernel envelope")
+            raise NotImplementedError("dilated=False is outside the sm_90a kernel envelope")
         self.num_layers = num_layers
         net = []
         for idx in range(num_layers):
@@ -179,7 +179,7 @@ class TimeDilatedConvNet(nn.Module):
                  dilated=True, separable=False, causal=True, nonlinear=None, norm=True, eps=EPS):
         super().__init__()
         if nonlinear != 'prelu' or not norm:
-            raise NotImplementedError("the sm_100a TCN requires nonlinear='prelu' and norm=True")
+            raise NotImplementedError("the sm_90a TCN requires nonlinear='prelu' and norm=True")
         self.num_features, self.hidden_channels, self.skip_channels = num_features, hidden_channels, skip_channels
         self.kernel_size, self.num_blocks, self.num_layers = kernel_size, num_blocks, num_layers
         self.dilated, self.separable, self.causal, self.eps = dilated, separable, causal, eps

@@ -1,4 +1,4 @@
-"""Segment1d / OverlapAdd1d on sm_100a gather / scatter kernels (csrc/ctn_dprnn.cu).
+"""Segment1d / OverlapAdd1d on sm_90a gather / scatter kernels (csrc/ctn_dprnn.cu).
 
 Mirrors src/models/transform.py:6-65 of the reference (same constructors, same shapes): ``Segment1d`` turns
 (batch, features, frames) into (batch, features, S, chunk_size) with S = (frames - chunk_size) // hop_size + 1,

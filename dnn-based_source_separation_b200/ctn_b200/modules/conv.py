@@ -25,7 +25,7 @@ class DepthwiseSeparableConv1d(nn.Module):
         if input.dim() != 3 or input.size(1) != self.depthwise_conv1d.in_channels:
             raise ValueError("input.size() is expected (?, {}, ?), but given {}".format(self.depthwise_conv1d.in_channels, tuple(input.size())))
         if torch.is_grad_enabled() and (input.requires_grad or any(p.requires_grad for p in self.parameters())):
-            raise NotImplementedError("modules.conv.DepthwiseSeparableConv1d is inference-only on the sm_100a path: call under torch.no_grad()")
+            raise NotImplementedError("modules.conv.DepthwiseSeparableConv1d is inference-only on the sm_90a path: call under torch.no_grad()")
         x = input.contiguous()
         dev = N.require_cuda(x)
         B, Cc, T = x.shape

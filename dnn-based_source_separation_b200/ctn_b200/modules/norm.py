@@ -1,4 +1,4 @@
-"""Layer norms of the Conv-TasNet path, computed by sm_100a kernels.
+"""Layer norms of the Conv-TasNet path, computed by sm_90a kernels.
 
 Mirrors src/modules/norm.py of the reference: ``GlobalLayerNorm`` (:11-35, a GroupNorm(1, C) -> state_dict keys
 ``norm.weight`` / ``norm.bias``) and ``CumulativeLayerNorm1d`` (:42-101, parameters ``gamma`` / ``beta`` of shape

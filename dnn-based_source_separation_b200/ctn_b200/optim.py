@@ -21,7 +21,7 @@ class FlatClipAdam:
             raise ValueError("no trainable parameters")
         dev = self.params[0].device
         if dev.type != "cuda":
-            raise RuntimeError("ctn_b200 runs on CUDA (sm_100a) only; there is no CPU fallback")
+            raise RuntimeError("ctn_b200 runs on CUDA (sm_90a) only; there is no CPU fallback")
         self.dev, self.betas, self.eps, self.weight_decay = dev, betas, eps, weight_decay
         self.max_norm = 0.0 if max_norm is None else float(max_norm)
         self.lr = torch.full((1,), float(lr), dtype=torch.float32, device=dev)

@@ -12,5 +12,5 @@ def choose_layer_norm(name, num_features, causal=False, eps=EPS, **kwargs):
             raise ValueError("Global Layer Normalization is NOT causal.")
         return GlobalLayerNorm(num_features, eps=eps)
     if name in ('BN', 'batch', 'batch_norm'):
-        raise NotImplementedError("BatchNorm is outside the sm_100a Conv-TasNet path (only 'gLN' / 'cLN').")
+        raise NotImplementedError("BatchNorm is outside the sm_90a Conv-TasNet path (only 'gLN' / 'cLN').")
     raise NotImplementedError("Not support {} layer normalization.".format(name))

@@ -1,4 +1,4 @@
-/* ctn_b200.h -- C ABI of the B200-native Conv-TasNet separation path.
+/* ctn_b200.h -- C ABI of the H100-native (sm_90a) Conv-TasNet separation path.
  *
  * The reference (tky823/DNN-based_source_separation) has NO native/FFI layer: the path sits behind
  * Python nn.Module classes (SURVEY.md section 8b).  This header is therefore the boundary a maintainer would
@@ -40,9 +40,9 @@ enum ctn_status {
 /* numeric mode of the dense 1x1 contractions */
 enum ctn_math {
   CTN_MATH_FP32 = 0,   /* CUDA-core FFMA, exact fp32 products (verification mode)          */
-  CTN_MATH_TF32X3 = 1, /* tcgen05 kind::tf32, 3-pass hi/lo split, fp32 accumulate (default) */
-  CTN_MATH_TF32 = 2,   /* tcgen05 kind::tf32 single pass (fast mode, looser tolerance)      */
-  CTN_MATH_F16X3 = 3   /* tcgen05 kind::f16, 3-pass fp16 hi/lo split (11-bit pieces like TF32, twice the MMA rate), fp32
+  CTN_MATH_TF32X3 = 1, /* wgmma tf32, 3-pass hi/lo split, fp32 accumulate (default)      */
+  CTN_MATH_TF32 = 2,   /* wgmma tf32 single pass (fast mode, looser tolerance)           */
+  CTN_MATH_F16X3 = 3   /* wgmma f16, 3-pass fp16 hi/lo split (11-bit pieces like TF32, twice the MMA rate), fp32
                           accumulate; default of the Python classes.  Weight rows are rescaled by powers of two inside the
                           library (any magnitude is fine); activations must stay below 65504 in magnitude (conversion
                           saturates beyond) -- always true behind the normalisations of this network; the separator head
@@ -105,7 +105,7 @@ typedef struct ctn_params {
 /* ---- introspection ------------------------------------------------------------------------- */
 int ctn_version(void);
 const char* ctn_strerror(int status);
-/* 1 if the tcgen05 (sm_100a) kernel family is compiled in */
+/* 1 if the tensor-core (wgmma, sm_90a) kernel family is compiled in */
 int ctn_has_tcgen05(void);
 
 /* ---- geometry helpers (host only) ----------------------------------------------------------
@@ -187,7 +187,7 @@ int ctn_overlap_add_fwd(const float* Z, float* y, int B, int F, int S, int chunk
 int ctn_dprnn_norm_res_fwd(const float* Y, const float* R, const float* gamma, const float* beta, float* out, int B, int D1, int D2,
                            int F, float eps, int swap, double* scratch, ctn_stream_t stream);
 /* Bidirectional LSTM + the 2H -> F Linear of a dual-path block, src/models/dprnn.py:85-87 / 138-139 (nn.LSTM(batch_first,
- * bidirectional) followed by nn.Linear), on tcgen05 with h resident in tensor memory (csrc/ctn_lstm.cu).
+ * bidirectional) followed by nn.Linear), on wgmma, 3xTF32 (csrc/ctn_lstm.cu).
  * z (NSEQ,T,F) fp32, batch_first; w[8] = host array of device pointers in torch.nn.LSTM order: weight_ih_l0 (4H,F), weight_hh_l0
  * (4H,H), bias_ih_l0, bias_hh_l0 (4H), then the four *_reverse tensors; gate order i,f,g,o; zero initial state.
  * w_fc (Fo,2H) nullable.  P (2,NSEQ,T,Fo): partial projections W_fc[:, dir*H:(dir+1)*H] h_dir WITHOUT the Linear's bias -- the
@@ -196,7 +196,7 @@ int ctn_dprnn_norm_res_fwd(const float* Y, const float* R, const float* gamma, c
  * (ctn_bilstm_supported); workspace >= ctn_bilstm_workspace_bytes(F,H,Fo), 256-byte aligned.  z_absmax (nullable): device word holding
  * the bit pattern of max|z| (the fp16 operand scale of x is derived from it); null = measured here with one more pass over z. */
 int ctn_bilstm_supported(int F, int H, int Fo);
-int ctn_debug_lstm_timeline(unsigned long long* out, int n); /* debug: cycle stamps of one CTA (CTN_LSTM_DBG=16), tools/lstm_time.py */
+int ctn_debug_lstm_timeline(unsigned long long* out, int n); /* debug hook: returns CTN_EUNSUPPORTED (no timeline is recorded) */
 size_t ctn_bilstm_workspace_bytes(int F, int H, int Fo);
 int ctn_bilstm_proj_fwd(const float* z, int NSEQ, int T, int F, int H, const float* const* w, const float* w_fc, int Fo, float* P,
                         float* hout, const unsigned* z_absmax, void* workspace, size_t workspace_bytes, ctn_stream_t stream);
@@ -288,15 +288,14 @@ int ctn_clip_adam_step(const int32_t* chunk_table, int n_chunks, float* const* p
                        float weight_decay, float max_norm, float* norm_out, ctn_stream_t stream);
 
 /* Test hook: ONE pointwise (1x1) contraction D[b][m][t] = epi(sum_k W[m][k] A[b][k][t]) in the selected numeric mode,
- * so tests can compare the tcgen05 kernels with the FFMA kernels operand by operand.  A (B,K,pitch), D (B,M,pitch),
+ * so tests can compare the wgmma kernels with the FFMA kernels operand by operand.  A (B,K,pitch), D (B,M,pitch),
  * pitch % 128 == 0.  epi: 0 = raw, 2 = +bias, PReLU(slope), (sum,sumsq) -> stats_out.  dbg (nullable): 4 words
- * {idesc, lbo_a, sbo_a, sbo_w} overriding the UMMA descriptors (0 = default).  workspace: >= 4*M*K*2 + 64 KiB bytes. */
+ * kept for ABI compatibility; the wgmma kernels take no descriptor overrides, so any non-zero word -> CTN_EUNSUPPORTED.  workspace: >= 4*M*K*2 + 64 KiB bytes. */
 int ctn_debug_pointwise(const float* A, const float* W, float* D, int B, int M, int K, int frames, int pitch,
                         const float* bias, const float* slope, double* stats_out, int epi, int math,
                         const uint32_t* dbg, void* workspace, size_t workspace_bytes, ctn_stream_t stream);
 
-/* Test hook: globaltimer stamps recorded by CTA 0 of the last tcgen05 pointwise launch when the environment variable
- * CTN_UMMA_DBG has bit 128 set: [0,4096) producer, [4096,8192) MMA issuer, [8192,12288) epilogue (4 words per step). */
+/* Debug hook kept for ABI stability: the wgmma pointwise kernels record no timeline, so it returns CTN_EUNSUPPORTED. */
 int ctn_debug_timeline(unsigned long long* host, int n);
 
 /* number of kernel launches the last ctn_* call on this thread enqueued (for bench.py's gpu_launches) */

@@ -248,8 +248,8 @@ def module_cases():
     loss, pattern = crit(inp, tgt)
     rec["pit_selftest"] = {"input": inp, "target": tgt, "loss": loss, "pattern": pattern}
     for S in (2, 3, 4):
-        e = torch.randn(5, S, 3000, generator=g)
-        t = torch.randn(5, S, 3000, generator=g)
+        e = torch.randn(5, S, 1000, generator=g)
+        t = torch.randn(5, S, 1000, generator=g)
         # make some estimates close to permuted targets so the permutation is non-trivial
         perm = torch.randperm(S, generator=g)
         e = 0.3 * e + t[:, perm]

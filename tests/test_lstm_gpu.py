@@ -1,4 +1,4 @@
-"""GPU parity of the tcgen05 bi-LSTM + projection kernel (``ctn_bilstm_proj_fwd``, csrc/ctn_lstm.cu; ``-m gpu``).
+"""GPU parity of the native bi-LSTM + projection kernel (``ctn_bilstm_proj_fwd``, csrc/ctn_lstm.cu; ``-m gpu``).
 
 Oracle: the reference's recurrence is torch.nn.LSTM on the CPU (src/models/dprnn.py:60, 85 / 114-120, 138), restated in
 oracle/dprnn_oracle.py::_bilstm; here it is evaluated in fp64 as ground truth and in fp32 (the reference's own precision) to
@@ -64,7 +64,7 @@ def _ref(z, sd, dtype):
                                             (32, 64, 64, 260, 5)])
 def test_bilstm_vs_fp64_oracle(Fi, H, Fo, NSEQ, T):
     if not N.ctn_bilstm_supported(Fi, H, Fo):
-        pytest.skip("no tcgen05")
+        pytest.skip("shape outside the native LSTM envelope")
     sd = _weights(Fi, H, Fo, seed=NSEQ + T)
     z = torch.randn(NSEQ, T, Fi, generator=torch.Generator().manual_seed(T)) * 1.5
     h, P = _run(z, sd, H, Fo)
@@ -107,7 +107,7 @@ def test_bilstm_operand_scales(xscale, wscale, atol):
     that are not saturated see it)"""
     Fi, H, Fo, NSEQ, T = 64, 128, 64, 140, 12
     if not N.ctn_bilstm_supported(Fi, H, Fo):
-        pytest.skip("no tcgen05")
+        pytest.skip("shape outside the native LSTM envelope")
     sd = _weights(Fi, H, Fo, seed=3, wscale=wscale)
     z = torch.randn(NSEQ, T, Fi, generator=torch.Generator().manual_seed(4)) * xscale
     h, P = _run(z, sd, H, Fo)
@@ -120,7 +120,7 @@ def test_bilstm_operand_scales(xscale, wscale, atol):
 def test_bilstm_outputs_optional_and_errors():
     Fi, H, Fo = 64, 128, 64
     if not N.ctn_bilstm_supported(Fi, H, Fo):
-        pytest.skip("no tcgen05")
+        pytest.skip("shape outside the native LSTM envelope")
     sd = _weights(Fi, H, Fo, seed=9)
     z = torch.randn(33, 7, Fi, generator=torch.Generator().manual_seed(1))
     h_only, _ = _run(z, sd, H, Fo, want_p=False)
@@ -140,7 +140,7 @@ def test_bilstm_outputs_optional_and_errors():
 
 
 def test_dprnn_stack_native_vs_cudnn_and_oracle():
-    """DPRNN.forward at the cfg4 feature sizes (F = 64, H = 128): tcgen05 recurrence vs the cuDNN fallback vs the CPU oracle"""
+    """DPRNN.forward at the cfg4 feature sizes (F = 64, H = 128): native recurrence vs the cuDNN recurrence vs the CPU oracle"""
     cfg = DO.DPRNNConfig(n_basis=16, kernel_size=4, sep_hidden_channels=128, sep_bottleneck_channels=64, sep_chunk_size=50, sep_hop_size=25,
                          sep_num_blocks=2)
     sd = DO.synth_state_dict(cfg, seed=7)

@@ -1,11 +1,11 @@
-"""GPU parity tests (run on the B200 box with ``-m gpu``).  Every check goes through the Python mirror of the
+"""GPU parity tests (run on an H100 with ``-m gpu``).  Every check goes through the Python mirror of the
 reference API -> ctypes -> C ABI (libctn_b200.so) -> sm_100a kernels, and is compared against
   (a) golden vectors minted from the unmodified reference (tests/golden/*.pt), and
   (b) the CPU oracle (oracle/convtasnet_oracle.py) on the same seeded inputs.
 
 Tolerances (SURVEY.md 8c: the reference's own fp32-vs-fp64 noise is 1.3e-6 abs on outputs of |max| 1.3, and its
 8-thread vs 1-thread fp32 results differ by 1e-5):
-  * model outputs, fp32-parity modes ('fp32' FFMA and 'tf32x3' tcgen05 split):  rtol 1e-4, atol 2e-5
+  * model outputs, fp32-parity modes ('fp32' FFMA and 'tf32x3' wgmma split):  rtol 1e-4, atol 2e-5
   * PIT permutation indices: bit-exact;  loss: 1e-4 dB absolute
   * single-pass 'tf32' fast mode: rtol 2e-2, atol 5e-3 (stated, looser)
 """
@@ -406,7 +406,7 @@ def test_host_buffer_entry_point():
     assert torch.equal(perm_h, perm.cpu()) and abs(float(loss_h) - float(loss)) < 1e-5
 
 
-@pytest.mark.skipif(not N.ctn_has_tcgen05(), reason="tcgen05 family not built")
+@pytest.mark.skipif(not N.ctn_has_tcgen05(), reason="tensor-core family not built")
 def test_tf32_fast_mode_stated_tolerance(golden_dir):
     rec = _load(golden_dir, "paper_3spk_short")
     cfg = O.OracleConfig(**rec["cfg"])
@@ -451,7 +451,7 @@ def test_forward_and_loss_are_cuda_graph_capturable():
             assert torch.equal(perm_g, perm_e)
 
 
-@pytest.mark.skipif(not N.ctn_has_tcgen05(), reason="tcgen05 family not built")
+@pytest.mark.skipif(not N.ctn_has_tcgen05(), reason="tensor-core family not built")
 @pytest.mark.parametrize("mode", ["tf32x3", "f16x3"])
 def test_split_modes_are_robust_to_weight_magnitudes(mode):
     """The fp16-piece mode rescales every weight row by a power of two (ctn_umma.cu: wimg_f16_rows), so tiny (gamma-folded)
@@ -483,7 +483,7 @@ def _scaled_paperish(seed=91):
     return cfg, O.synth_state_dict(cfg, seed=seed)
 
 
-@pytest.mark.skipif(not N.ctn_has_tcgen05(), reason="tcgen05 family not built")
+@pytest.mark.skipif(not N.ctn_has_tcgen05(), reason="tensor-core family not built")
 @pytest.mark.parametrize("mode", ["tf32x3", "f16x3"])
 @pytest.mark.parametrize("scale", [1e-4, 1e3])
 def test_split_modes_are_robust_to_input_scale(mode, scale):
@@ -499,7 +499,7 @@ def test_split_modes_are_robust_to_input_scale(mode, scale):
     torch.testing.assert_close(out.cpu(), ref, rtol=RTOL, atol=ATOL * max(1e-30, float(ref.abs().max())))
 
 
-@pytest.mark.skipif(not N.ctn_has_tcgen05(), reason="tcgen05 family not built")
+@pytest.mark.skipif(not N.ctn_has_tcgen05(), reason="tensor-core family not built")
 @pytest.mark.parametrize("mode", ["tf32x3", "f16x3"])
 @pytest.mark.parametrize("mag", [1e-3, 1e4])
 def test_split_modes_are_robust_to_residual_and_skip_magnitude(mode, mag):
@@ -521,7 +521,7 @@ def test_split_modes_are_robust_to_residual_and_skip_magnitude(mode, mag):
     torch.testing.assert_close(out.cpu(), ref, rtol=RTOL, atol=ATOL * max(1.0, float(ref.abs().max())))
 
 
-@pytest.mark.skipif(not N.ctn_has_tcgen05(), reason="tcgen05 family not built")
+@pytest.mark.skipif(not N.ctn_has_tcgen05(), reason="tensor-core family not built")
 @pytest.mark.parametrize("T,S", [(8000, 2), (8003, 3), (1031, 2)])
 def test_fused_mask_decoder_matches_unfused_and_oracle(T, S):
     """forward() runs the fused mask 1x1 + sigmoid + w*mask + ConvTranspose1d + crop epilogue (w_hat never materialised, fp16-piece
@@ -547,7 +547,7 @@ def test_fused_mask_decoder_matches_unfused_and_oracle(T, S):
 
 
 def test_reference_checkpoint_runs_on_the_kernels(golden_dir):
-    """reference trainer checkpoint (tests/golden/ref_ckpt_tiny_gln.pth) -> build_model -> sm_100a forward == the golden output the
+    """reference trainer checkpoint (tests/golden/ref_ckpt_tiny_gln.pth) -> build_model -> sm_90a forward == the golden output the
     reference itself produced with those weights (tiny_gln)."""
     rec = _load(golden_dir, "tiny_gln")
     model = ConvTasNet.build_model(os.path.join(golden_dir, "ref_ckpt_tiny_gln.pth"), load_state_dict=True).cuda().eval()

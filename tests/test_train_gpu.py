@@ -163,9 +163,8 @@ def _oracle_grads64(cfg, sd, mixture, sources):
 # x 512 channels with ~1e4-fold cancellation, which amplifies every rounding error of the data gradients by that factor, and the
 # per-tensor noise is heavy-tailed (7e-8 ... 1e-1).  A second fp32 implementation therefore cannot agree with the reference's fp32
 # numbers to 2e-4 at this size; what is asserted is the distance to the fp64 answer:
-#   * whole gradient: ||g - g64||_2 / ||g64||_2 <= L2MAX[mode]   (the quantity SGD / Adam see).  Measured on B200: 1.5e-3 for the
-#     tcgen05 modes = 2.5x the reference's own fp32 (their 3-pass tf32 split carries 22-bit operands: products are 2^-21 relative
-#     instead of 2^-24), 1.2e-3 against the reference's fp64 fixture;
+#   * whole gradient: ||g - g64||_2 / ||g64||_2 <= L2MAX[mode]   (the quantity SGD / Adam see).  The tensor-core modes sit above
+#     the reference's own fp32 (their 3-pass split carries 22-bit operands: products are 2^-21 relative instead of 2^-24);
 #   * every tensor: max |g - g64| <= PER[mode] * scale(k), scale(k) = the largest |g64| entry among the tensors of the same role (all
 #     48 PReLU-slope gradients, all 24 depthwise weights, ...: a scalar that happens to be ~0 is judged against its peers) -- a
 #     structural check (a missing term or a wrong tile shows up at O(0.1 .. 1)); measured worst 1.2e-2.
@@ -204,7 +203,7 @@ def _check_grads_vs_fp64(named_grads, g64max, g64, noise32, mode):
 @pytest.mark.parametrize("S", [2, 3])
 def test_paper_size_gradients_vs_oracle_autograd(mode, S):
     """BASELINE hyper-parameters (N=512 L=16 B=128 H=512 Sc=128 X=8 R=3; cfg2 = 2 speakers, cfg3 = 3 speakers), batch 2,
-    T = 8000: the tcgen05 weight-gradient kernel runs its 4 M-tiles / K = 512 shapes and the split-K red.add path.  All 343
+    T = 8000: the wgmma weight-gradient kernel runs its 4 M-tiles / K = 512 shapes and the split-K red.add path.  All 343
     gradient tensors against torch autograd over the oracle IN FP64 (egs/wsj0-mix/common/src/driver.py:146-150), tolerance
     anchored on the fp32 oracle's own distance to fp64 (see _check_grads_vs_fp64)."""
     cfg = O.OracleConfig(causal=False, n_sources=S, **PAPER)
