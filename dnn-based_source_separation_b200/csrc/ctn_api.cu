@@ -1,5 +1,4 @@
 // extern "C" entry points + host-side orchestration of the Conv-TasNet forward (see include/ctn_b200.h).
-#include <stdlib.h>
 #include <string.h>
 #include <vector>
 #include "ctn_internal.h"
@@ -84,22 +83,6 @@ extern "C" int ctn_frames(int T, int kernel_size, int stride, int* pad_left, int
 
 extern "C" int ctn_pitch(int frames) { return frames <= 0 ? CTN_EINVAL : ctn_round_up(frames, CTN_TILE_T); }
 
-// ------------------------------------------------------------------------------------------------
-// workspace carving
-// ------------------------------------------------------------------------------------------------
-struct Carver {
-  char* base;
-  size_t off;
-  explicit Carver(void* b) : base((char*)b), off(0) {}
-  template <typename T>
-  T* take(size_t count) {
-    off = (off + 255) & ~(size_t)255;
-    T* p = base ? (T*)(base + off) : nullptr;
-    off += count * sizeof(T);
-    return p;
-  }
-};
-
 struct TcnWs {
   double* stats;  // [2*RX][B][2]
   std::vector<FoldedConv> folds;  // per block, (Bc+Sc) rows
@@ -141,8 +124,8 @@ static void carve_tcn(Carver& cv, const ctn_config_t* c, int B, int pitch, TcnWs
     ws->folds[i].v2 = cv.take<float>(Mt);
     ws->folds[i].vb = cv.take<float>(Mt);
     if (c->math != CTN_MATH_FP32) {
-      ws->wimg1[i] = cv.take<float>(ctn_umma_wimg_bytes(c->hidden, c->bottleneck, c->math) / sizeof(float));
-      ws->wimg2[i] = cv.take<float>(ctn_umma_wimg_bytes(Mt, c->hidden, c->math) / sizeof(float));
+      ws->wimg1[i] = cv.take<float>(ctn_pw_wimg_bytes(c->hidden, c->bottleneck, c->math) / sizeof(float));
+      ws->wimg2[i] = cv.take<float>(ctn_pw_wimg_bytes(Mt, c->hidden, c->math) / sizeof(float));
     }
   }
   ws->dwp.assign(RX, nullptr);
@@ -167,22 +150,20 @@ static void carve_tcn(Carver& cv, const ctn_config_t* c, int B, int pitch, TcnWs
   }
 }
 
-static int pw_dispatch(const PwArgs& a, int pro, int epi, int math, cudaStream_t st) {
-  if (math == CTN_MATH_FP32) return ctn_pw_simt(a, pro, epi, st);
-  return ctn_pw_umma(a, pro, epi, math, st);
-}
-
 // TCN over ws->x (padded layout) -> ws->skip.  stats region must be zeroed by the caller.
 // dil (nullable): explicit dilation per block (ctn_tcn_blocks_fwd); default 2^layer (dilated=True, tdcn.py:52-54).
 // x_final (nullable): receives a pointer to the residual stream AFTER the last block (x_n), updated in the workspace.
-// hooks (nullable): TRAINING forward through the fused kernels -- block i reads its input from x_keep[i] (x_keep[0] = the head's
-// output, filled by the caller) and leaves x_{i+1} in x_keep[i+1]; pw1 stores the PRE-activation W1 x + b1 in hpre[i], the fused
-// depthwise producer applies PReLU on load and stores its own pre-activation in upre[i] (what ctn_convtasnet_bwd consumes).
+// hooks (nullable, f16x3 mode only, see ctn_tcn_train_fwd): TRAINING forward through the fused kernels -- block i reads its input
+// from x_keep[i] (x_keep[0] = the head's output, filled by the caller) and leaves x_{i+1} in x_keep[i+1]; pw1 stores the
+// PRE-activation W1 x + b1 in hpre[i], the fused depthwise producer applies PReLU on load and stores its own pre-activation in
+// upre[i] (what ctn_convtasnet_bwd consumes).
 static int run_tcn(const ctn_config_t* c, const ctn_block_params_t* blocks, TcnWs* ws, int B, int frames, int pitch,
                    cudaStream_t st, const int* dil = nullptr, float** x_final = nullptr, const TcnTrainHooks* hooks = nullptr) {
   const int R = c->num_blocks, X = c->num_layers, Bc = c->bottleneck, H = c->hidden, Sc = c->skip;
   if (c->causal)  // cLN: cumulative statistics -> un-fused pipeline in the reference's operation order
     return ctn_causal_tcn(c, blocks, ws->x, ws->skip, ws->h, ws->u, B, frames, pitch, ws->causal_ws, st);
+  // fp16-piece mode: every contraction of the stack gets an operand scale (ctn_act_scales)
+  const bool scaled = c->math == CTN_MATH_F16X3;
   // weight preparation for all blocks: gLN2 folding, then (tensor-core modes) the swizzled hi/lo operand images
   {
     StageTimer tm(CTN_ST_PREP, st);
@@ -198,14 +179,12 @@ static int run_tcn(const ctn_config_t* c, const ctn_block_params_t* blocks, TcnW
       if (has_out) fj.push_back(FoldJob{p.out_w, p.out_b, p.norm2_g, p.norm2_b, f.Wf, f.v1, f.v2, Bc, H, 0, f.vb, Rh});
       fj.push_back(FoldJob{p.skip_w, p.skip_b, p.norm2_g, p.norm2_b, f.Wf, f.v1, f.v2, Sc, H, has_out ? Bc : 0, f.vb, Rh});
       sj->j[i] = ScaleJob{f.vb, p.norm1_g, p.norm1_b, p.dw_w, p.dw_b, p.prelu2, ws->dwp[i], has_out ? 1 : 0};
-      if (c->math != CTN_MATH_FP32) {
-        wj.push_back(WimgJob{p.bottleneck_w, ws->wimg1[i], H, Bc});
-        wj.push_back(WimgJob{f.Wf, ws->wimg2[i], has_out ? Bc + Sc : Sc, H});
-      }
+      wj.push_back(WimgJob{p.bottleneck_w, ws->wimg1[i], H, Bc});
+      wj.push_back(WimgJob{f.Wf, ws->wimg2[i], has_out ? Bc + Sc : Sc, H});
     }
     int rc = ctn_fold_batch(fj.data(), (int)fj.size(), st);
-    if (rc == CTN_OK && !wj.empty()) rc = ctn_umma_build_wimg_batch(wj.data(), (int)wj.size(), c->math, st);
-    if (rc == CTN_OK && c->math == CTN_MATH_F16X3) {
+    if (rc == CTN_OK) rc = ctn_pw_prepare_batch(wj.data(), (int)wj.size(), c->math, scaled, st);
+    if (rc == CTN_OK && scaled) {
       sj->n = R * X; sj->Bc = Bc; sj->Sc = Sc; sj->H = H; sj->P = c->sep_kernel; sj->R = Rh;
       sj->x0_bound = ws->x0_bound; sj->x0_n = ws->x0_n; sj->mask_slope = ws->mask_slope; sj->scales = ws->scales;
       rc = ctn_act_scales(*sj, st);
@@ -213,19 +192,10 @@ static int run_tcn(const ctn_config_t* c, const ctn_block_params_t* blocks, TcnW
     delete sj;
     CTN_TRY(rc);
   }
-  const bool scaled = c->math == CTN_MATH_F16X3;
-  // Sample groups: the blocks are walked group by group (G samples through all R*X blocks, then the next G).  The hidden tensor h
-  // of a group (G * H * pitch * 4 bytes = 8.4 MB per sample at cfg2) is written by pw1 and read by pw2 a few hundred microseconds
-  // later from the SAME buffer for every group and block, so it stays resident in the 126 MB L2 instead of making a round trip
-  // through HBM (12.6 GB of the 24 GB a cfg2 step moved).  Every mixture is independent, so the arithmetic is unchanged.
-  static const char* env_grp = getenv("CTN_TCN_GROUP");
-  int G = env_grp ? atoi(env_grp) : 0;
-  if (G <= 0 || G > B || c->math == CTN_MATH_FP32) G = B;
-  for (int g0 = 0; g0 < B; g0 += G) {
-  const int Bg = B - g0 < G ? B - g0 : G;
-  const size_t go = (size_t)g0 * pitch;  // sample offset in rows of `pitch` floats, times the tensor's channel count
-  float* hbuf = ws->h;                   // one group-sized region, reused by every group
-  float* ubuf = ws->u;
+  // tensor-core modes: the residual stream ping-pongs between ws->x and ws->xalt; block i >= 1 applies block i-1's
+  // update x += rstd2*r[:Bc] + c inside its own producer (PRO_RES) -- no separate finishing pass over x
+  const bool fuse_res = c->math != CTN_MATH_FP32;
+  float* xbuf[2] = {ws->x, ws->xalt};
   for (int r = 0; r < R; ++r) {
     for (int l = 0; l < X; ++l) {
       const int i = r * X + l;
@@ -233,22 +203,16 @@ static int run_tcn(const ctn_config_t* c, const ctn_block_params_t* blocks, TcnW
       const bool has_out = p.out_w != nullptr;
       if (!has_out && !(r == R - 1 && l == X - 1)) return CTN_EINVAL;
       const int dilation = dil ? dil[i] : (1 << l);  // dilated=True (tdcn.py:52-54)
-      double* st1 = ws->stats + (size_t)(2 * i) * B * 2 + 2 * g0;
-      double* st2 = ws->stats + (size_t)(2 * i + 1) * B * 2 + 2 * g0;
+      double* st1 = ws->stats + (size_t)(2 * i) * B * 2;
+      double* st2 = ws->stats + (size_t)(2 * i + 1) * B * 2;
+      // training: h_pre goes to the block's own buffer, kept for the backward
+      float* hbuf = hooks ? hooks->hpre[i] : ws->h;
       // K_A: h = PReLU(W1 x + b1), stats1
       PwArgs a;
       memset(&a, 0, sizeof(a));
-      // tensor-core modes: the residual stream ping-pongs between ws->x and ws->xalt; block i >= 1 applies block i-1's
-      // update x += rstd2*r[:Bc] + c inside its own producer (PRO_RES) -- no separate finishing pass over x
-      const bool fuse_res = c->math != CTN_MATH_FP32;
-      float* xbuf[2] = {ws->x + go * Bc, ws->xalt + go * Bc};
-      if (hooks) {  // per-block buffers: x_i is read from x_keep[i] (written by block i-1 below), kept for the backward
-        if (!fuse_res || g0 != 0) return CTN_EUNSUPPORTED;
-        hbuf = hooks->hpre[i];
-      }
       a.A = fuse_res ? xbuf[(i + 1) & 1] : xbuf[0];
       if (fuse_res && i == 0) a.A = hooks ? hooks->x_keep[0] : xbuf[0];
-      a.W = p.bottleneck_w; a.D = hbuf; a.B = Bg; a.M = H; a.K = Bc; a.frames = frames; a.pitch = pitch;
+      a.W = p.bottleneck_w; a.D = hbuf; a.B = B; a.M = H; a.K = Bc; a.frames = frames; a.pitch = pitch;
       a.store_pre = hooks ? 1 : 0;
       a.bias = p.bottleneck_b; a.slope = p.prelu1; a.stats_out = st1; a.wimg = ws->wimg1[i];
       if (scaled) a.act_scale = ws->scales + 2 * i;
@@ -257,15 +221,14 @@ static int run_tcn(const ctn_config_t* c, const ctn_block_params_t* blocks, TcnW
         // x_{i} = x_{i-1} + deferred gLN2 of block i-1;  x_{i-1} lives in xbuf[(i-1)&1], x_i goes to xbuf[i&1]
         pro1 = PRO_RES;
         a.A = hooks ? hooks->x_keep[i - 1] : xbuf[(i - 1) & 1];
-        a.res_r = ws->rblk[i - 1] + go * (Bc + Sc); a.res_Mt = Bc + Sc;  // block i-1 always has the out head (only the last block lacks it)
+        a.res_r = ws->rblk[i - 1]; a.res_Mt = Bc + Sc;  // block i-1 always has the out head (only the last block lacks it)
         a.res_v1 = ws->folds[i - 1].v1; a.res_v2 = ws->folds[i - 1].v2;
-        a.res_stats = ws->stats + (size_t)(2 * (i - 1) + 1) * B * 2 + 2 * g0; a.res_n = (double)H * (double)frames; a.res_eps = c->eps_tcn;
+        a.res_stats = ws->stats + (size_t)(2 * (i - 1) + 1) * B * 2; a.res_n = (double)H * (double)frames; a.res_eps = c->eps_tcn;
         a.res_x_out = hooks ? hooks->x_keep[i] : xbuf[i & 1];
       }
-      if (hooks && c->math != CTN_MATH_F16X3) return CTN_EUNSUPPORTED;
-      { StageTimer tm(CTN_ST_PW1, st); CTN_TRY(pw_dispatch(a, pro1, EPI_H, c->math, st)); }
+      { StageTimer tm(CTN_ST_PW1, st); CTN_TRY(ctn_pw(a, pro1, EPI_H, c->math, nullptr, st)); }
       const int Mt = has_out ? Bc + Sc : Sc;
-      float* rb = ws->rblk[i] + go * Mt;
+      float* rb = ws->rblk[i];
       const int pad_left = c->causal ? (c->sep_kernel - 1) * dilation : ((c->sep_kernel - 1) * dilation) / 2;
       // fused depthwise producer: 3 taps at dilation 1, 2 or a multiple of 4 (128-bit aligned tap loads); anything else runs the
       // stand-alone depthwise stage
@@ -275,37 +238,33 @@ static int run_tcn(const ctn_config_t* c, const ctn_block_params_t* blocks, TcnW
         // it straight to the tensor core; u never touches HBM.  r = [Wo;Ws] diag(gamma2) u
         StageTimer tm(CTN_ST_PW2, st);
         memset(&a, 0, sizeof(a));
-        a.A = hbuf; a.W = ws->folds[i].Wf; a.D = rb; a.B = Bg; a.M = Mt; a.K = H; a.frames = frames; a.pitch = pitch;
+        a.A = hbuf; a.W = ws->folds[i].Wf; a.D = rb; a.B = B; a.M = Mt; a.K = H; a.frames = frames; a.pitch = pitch;
         a.wimg = ws->wimg2[i];
         a.pro_slope = p.prelu2; a.dw_norm_g = p.norm1_g; a.dw_norm_b = p.norm1_b; a.dw_w = p.dw_w; a.dw_b = p.dw_b;
         a.dw_stats_in = st1; a.dw_stats_out = st2; a.dw_dilation = dilation; a.dw_pad_left = pad_left; a.dw_eps = c->eps_tcn;
         if (scaled) { a.act_scale = ws->scales + 2 * i + 1; a.dw_params = ws->dwp[i]; }
-        if (hooks) {
-          a.dw_in_slope = p.prelu1; a.dw_u_pre_out = hooks->upre[i];
-          if (c->math != CTN_MATH_F16X3) return CTN_EUNSUPPORTED;
-        }
-        CTN_TRY(pw_dispatch(a, PRO_DW, EPI_RAW, c->math, st));
+        if (hooks) { a.dw_in_slope = p.prelu1; a.dw_u_pre_out = hooks->upre[i]; }
+        CTN_TRY(ctn_pw(a, PRO_DW, EPI_RAW, c->math, nullptr, st));
       } else {
         if (hooks) return CTN_EUNSUPPORTED;
         // K_B: u = PReLU(dwconv(gLN1(h))), stats2
         { StageTimer tm(CTN_ST_DW, st);
-          CTN_TRY(ctn_dw_fwd(hbuf, ubuf, p.norm1_g, p.norm1_b, p.dw_w, p.dw_b, p.prelu2, st1, st2, Bg, H, frames, pitch,
+          CTN_TRY(ctn_dw_fwd(hbuf, ws->u, p.norm1_g, p.norm1_b, p.dw_w, p.dw_b, p.prelu2, st1, st2, B, H, frames, pitch,
                              c->sep_kernel, dilation, c->causal, c->eps_tcn, st)); }
         // K_C: r = [Wo;Ws] diag(gamma2) u
         memset(&a, 0, sizeof(a));
-        a.A = ubuf; a.W = ws->folds[i].Wf; a.D = rb; a.B = Bg; a.M = Mt; a.K = H; a.frames = frames; a.pitch = pitch;
+        a.A = ws->u; a.W = ws->folds[i].Wf; a.D = rb; a.B = B; a.M = Mt; a.K = H; a.frames = frames; a.pitch = pitch;
         a.wimg = ws->wimg2[i];
         if (scaled) a.act_scale = ws->scales + 2 * i + 1;
-        { StageTimer tm(CTN_ST_PW2, st); CTN_TRY(pw_dispatch(a, PRO_NONE, EPI_RAW, c->math, st)); }
+        { StageTimer tm(CTN_ST_PW2, st); CTN_TRY(ctn_pw(a, PRO_NONE, EPI_RAW, c->math, nullptr, st)); }
       }
       // K_F: residual update with the deferred gLN2 (x += rstd2*r[:Bc] + c); the skip rows are reduced once at the end
       if (has_out && c->math == CTN_MATH_FP32) {
         StageTimer tm(CTN_ST_FIN, st);
-        CTN_TRY(ctn_finish_fwd(rb, ws->folds[i], st2, (double)H * (double)frames, c->eps_tcn, xbuf[0], ws->skip + go * Sc, Bg, Bc,
-                               Sc, 1, 2 /* x rows only */, frames, pitch, st));
+        CTN_TRY(ctn_finish_fwd(rb, ws->folds[i], st2, (double)H * (double)frames, c->eps_tcn, xbuf[0], ws->skip, B, Bc, Sc, 1,
+                               2 /* x rows only */, frames, pitch, st));
       }
     }
-  }
   }
   {
     StageTimer tm(CTN_ST_FIN, st);
@@ -320,9 +279,8 @@ static int run_tcn(const ctn_config_t* c, const ctn_block_params_t* blocks, TcnW
   }
   if (x_final) {
     const int n = R * X;
-    float* xbuf[2] = {ws->x, ws->xalt};
-    float* xl = (c->math != CTN_MATH_FP32) ? xbuf[(n - 1) & 1] : ws->x;  // x_{n-1} (tensor-core modes defer every update to the next block)
-    if (c->math != CTN_MATH_FP32 && blocks[n - 1].out_w)
+    float* xl = fuse_res ? xbuf[(n - 1) & 1] : ws->x;  // x_{n-1} (tensor-core modes defer every update to the next block)
+    if (fuse_res && blocks[n - 1].out_w)
       CTN_TRY(ctn_finish_fwd(ws->rblk[n - 1], ws->folds[n - 1], ws->stats + (size_t)(2 * (n - 1) + 1) * B * 2, (double)H * (double)frames,
                              c->eps_tcn, xl, ws->skip, B, Bc, Sc, 1, 2 /* x rows only */, frames, pitch, st));
     *x_final = xl;
@@ -348,8 +306,8 @@ static void carve_tcn_train(Carver& cv, const ctn_config_t* c, int B, int pitch,
     ws->folds[i].v1 = cv.take<float>(Mt);
     ws->folds[i].v2 = cv.take<float>(Mt);
     ws->folds[i].vb = cv.take<float>(Mt);
-    ws->wimg1[i] = cv.take<float>(ctn_umma_wimg_bytes(c->hidden, c->bottleneck, c->math) / sizeof(float));
-    ws->wimg2[i] = cv.take<float>(ctn_umma_wimg_bytes(Mt, c->hidden, c->math) / sizeof(float));
+    ws->wimg1[i] = cv.take<float>(ctn_pw_wimg_bytes(c->hidden, c->bottleneck, c->math) / sizeof(float));
+    ws->wimg2[i] = cv.take<float>(ctn_pw_wimg_bytes(Mt, c->hidden, c->math) / sizeof(float));
     ws->dwp[i] = cv.take<float>((size_t)ctn_round_up(c->hidden, 16) * 8);
     ws->rblk[i] = cv.take<float>((size_t)B * pitch * Mt);
   }
@@ -495,8 +453,8 @@ static void carve_model(Carver& cv, const ctn_config_t* c, int B, int pitch, Mod
   ws->head.vb = cv.take<float>(c->bottleneck);
   ws->wimg_head = ws->wimg_mask = nullptr;
   if (c->math != CTN_MATH_FP32) {
-    ws->wimg_head = cv.take<float>(ctn_umma_wimg_bytes(c->bottleneck, c->n_basis, c->math) / sizeof(float));
-    ws->wimg_mask = cv.take<float>(ctn_umma_wimg_bytes(c->n_sources * c->n_basis, c->skip, c->math) / sizeof(float));
+    ws->wimg_head = cv.take<float>(ctn_pw_wimg_bytes(c->bottleneck, c->n_basis, c->math) / sizeof(float));
+    ws->wimg_mask = cv.take<float>(ctn_pw_wimg_bytes(c->n_sources * c->n_basis, c->skip, c->math) / sizeof(float));
   }
   const size_t bp = (size_t)B * pitch;
   ws->w = cv.take<float>(bp * c->n_basis);
@@ -523,63 +481,59 @@ struct DecFuse { float* out; int crop_left, T_out; bool fused; };
 static int run_separator(const ctn_config_t* c, const ctn_params_t* p, ModelWs* ws, int B, int frames, int pitch,
                          float* mask_out, cudaStream_t st, DecFuse* dec = nullptr) {
   const int N = c->n_basis, Bc = c->bottleneck, Sc = c->skip, S = c->n_sources;
+  // tail: PReLU -> mask 1x1 -> sigmoid -> * w  (conv_tasnet.py:373-376, 159-160).  fp16-piece mode: the operand PReLU(skip sum)
+  // is bounded by the scales of the fused stack; causal models (un-fused pipeline) have none
+  PwArgs m;
+  memset(&m, 0, sizeof(m));
+  m.A = ws->tcn.skip; m.W = p->mask_w; m.D = ws->what; m.B = B; m.M = S * N; m.K = Sc; m.frames = frames; m.pitch = pitch;
+  m.pro_slope = p->prelu_out; m.bias = p->mask_b; m.wenc = ws->w; m.Nb = N; m.mask_out = mask_out; m.wimg = ws->wimg_mask;
+  if (c->math == CTN_MATH_F16X3 && !c->causal) m.act_scale = ws->tcn.scales + 2 * c->num_blocks * c->num_layers;
   if (c->causal) {
     // cLN0 -> bottleneck 1x1; ws->what is free until the mask kernel writes it: use it as the (B, N, pitch) scratch
     CTN_TRY(ctn_causal_head(c, p, ws->w, ws->what, ws->tcn.x, B, frames, pitch, ws->tcn.causal_ws, st));
     if (c->math != CTN_MATH_FP32) {
       StageTimer tm(CTN_ST_PREP, st);
-      CTN_TRY(ctn_umma_build_wimg(p->mask_w, S * N, Sc, c->math == CTN_MATH_F16X3 ? CTN_MATH_TF32X3 : c->math, ws->wimg_mask, st));
+      CTN_TRY(ctn_pw_prepare(m, c->math, ws->wimg_mask, st));
     }
   } else {
     // head: gLN0 folded into the bottleneck 1x1 (conv_tasnet.py:370-371).  Its operand is the un-normalised encoder output
-    // (any input scale), so the fp16-piece mode falls back to the tf32 pieces here (0.14 ms of the step).
-    const int head_math = c->math == CTN_MATH_F16X3 ? CTN_MATH_TF32X3 : c->math;
-    { StageTimer tm(CTN_ST_PREP, st);
-      CTN_TRY(ctn_fold_conv(p->bn_w, p->bn_b, p->norm0_g, p->norm0_b, Bc, N, ws->head, 0, st, sqrtf((float)N * (float)frames) * 1.0001f));
-      if (c->math != CTN_MATH_FP32) {
-        CTN_TRY(ctn_umma_build_wimg(ws->head.Wf, Bc, N, head_math, ws->wimg_head, st));
-        CTN_TRY(ctn_umma_build_wimg(p->mask_w, S * N, Sc, c->math, ws->wimg_mask, st));
-      }
-    }
+    // (any input scale, no operand scale), so the fp16-piece mode runs it on the tf32 pieces (0.14 ms of the step).
     PwArgs a;
     memset(&a, 0, sizeof(a));
     a.A = ws->w; a.W = ws->head.Wf; a.D = ws->tcn.x; a.B = B; a.M = Bc; a.K = N; a.frames = frames; a.pitch = pitch;
     a.v1 = ws->head.v1; a.v2 = ws->head.v2; a.stats_in = ws->stats0; a.n_in = (double)N * (double)frames; a.eps = c->eps;
     a.wimg = ws->wimg_head;
-    { StageTimer tm(CTN_ST_HEAD, st); CTN_TRY(pw_dispatch(a, PRO_NONE, EPI_HEAD, head_math, st)); }
+    { StageTimer tm(CTN_ST_PREP, st);
+      CTN_TRY(ctn_fold_conv(p->bn_w, p->bn_b, p->norm0_g, p->norm0_b, Bc, N, ws->head, 0, st, sqrtf((float)N * (float)frames) * 1.0001f));
+      CTN_TRY(ctn_pw_prepare(a, c->math, ws->wimg_head, st));
+      CTN_TRY(ctn_pw_prepare(m, c->math, ws->wimg_mask, st));
+    }
+    { StageTimer tm(CTN_ST_HEAD, st); CTN_TRY(ctn_pw(a, PRO_NONE, EPI_HEAD, c->math, nullptr, st)); }
   }
   // TCN (conv_tasnet.py:372).  fp16-piece mode: |x_0| <= max_n of the head's row bounds; the mask operand is PReLU(skip sum)
   ws->tcn.x0_bound = ws->head.vb; ws->tcn.x0_n = Bc; ws->tcn.mask_slope = p->prelu_out;
   CTN_TRY(run_tcn(c, p->blocks, &ws->tcn, B, frames, pitch, st));
-  // tail: PReLU -> mask 1x1 -> sigmoid -> * w  (conv_tasnet.py:373-376, 159-160)
-  PwArgs a;
-  memset(&a, 0, sizeof(a));
-  a.A = ws->tcn.skip; a.W = p->mask_w; a.D = ws->what; a.B = B; a.M = S * N; a.K = Sc; a.frames = frames; a.pitch = pitch;
-  a.pro_slope = p->prelu_out; a.bias = p->mask_b; a.wenc = ws->w; a.Nb = N; a.mask_out = mask_out; a.wimg = ws->wimg_mask;
-  if (c->math == CTN_MATH_F16X3 && !c->causal) a.act_scale = ws->tcn.scales + 2 * c->num_blocks * c->num_layers;
-  // causal models: no operand scales (un-fused pipeline) -> the mask contraction stays on the tf32 pieces
-  const int mask_math = (c->causal && c->math == CTN_MATH_F16X3) ? CTN_MATH_TF32X3 : c->math;
   if (c->mask_softmax) {
     // nn.Softmax(dim=1) over ALL S*N mask channels (conv_tasnet.py:345-357 quirk): logits first, then one normalising pass
     StageTimer tm(CTN_ST_MASK, st);
-    a.mask_logits = 1;
-    a.mask_out = nullptr;
-    CTN_TRY(pw_dispatch(a, PRO_PRELU, EPI_MASK, mask_math, st));
+    m.mask_logits = 1;
+    m.mask_out = nullptr;
+    CTN_TRY(ctn_pw(m, PRO_PRELU, EPI_MASK, c->math, nullptr, st));
     return ctn_softmax_mask(ws->what, ws->w, mask_out, B, S * N, N, frames, pitch, st);
   }
-  if (dec && !mask_out && mask_math == CTN_MATH_F16X3 && c->kernel_size == 16 && c->stride == 8) {
-    PwArgs f = a;
+  if (dec && !mask_out && c->kernel_size == 16 && c->stride == 8) {
+    PwArgs f = m;
     f.D = dec->out; f.dec_w = p->dec_w; f.dec_crop_left = dec->crop_left; f.dec_T_out = dec->T_out;
-    if (ctn_pw_maskdec_supported(f, mask_math)) {
+    if (ctn_pw_maskdec_supported(f, c->math)) {
       StageTimer tm(CTN_ST_MASK, st);
       cudaError_t e = cudaMemsetAsync(dec->out, 0, sizeof(float) * (size_t)B * S * dec->T_out, st);  // tile seams are red.add'ed
       if (e != cudaSuccess) return (int)e;
-      CTN_TRY(ctn_pw_umma(f, PRO_PRELU, EPI_MASKDEC, mask_math, st));
+      CTN_TRY(ctn_pw(f, PRO_PRELU, EPI_MASKDEC, c->math, nullptr, st));
       dec->fused = true;
       return CTN_OK;
     }
   }
-  { StageTimer tm(CTN_ST_MASK, st); CTN_TRY(pw_dispatch(a, PRO_PRELU, EPI_MASK, mask_math, st)); }
+  { StageTimer tm(CTN_ST_MASK, st); CTN_TRY(ctn_pw(m, PRO_PRELU, EPI_MASK, c->math, nullptr, st)); }
   return CTN_OK;
 }
 
@@ -685,7 +639,7 @@ static void carve_stage(Carver& cv, int M, int K, int math, StageWs* ws) {
   ws->head.v1 = cv.take<float>(M);
   ws->head.v2 = cv.take<float>(M);
   ws->head.vb = nullptr;
-  ws->wimg = math != CTN_MATH_FP32 ? cv.take<float>(ctn_umma_wimg_bytes(M, K, math) / sizeof(float)) : nullptr;
+  ws->wimg = math != CTN_MATH_FP32 ? cv.take<float>(ctn_pw_wimg_bytes(M, K, math) / sizeof(float)) : nullptr;
 }
 extern "C" size_t ctn_stage_workspace_bytes(int M, int K) {
   if (M <= 0 || K <= 0) return 0;
@@ -705,7 +659,6 @@ extern "C" int ctn_sep_head_fwd(const float* w, const double* stats0, const floa
   if (!w || !stats0 || !norm_g || !norm_b || !bn_w || !x0 || !workspace || B <= 0 || N <= 0 || Bc <= 0 || frames <= 0) return CTN_EINVAL;
   if (pitch < frames || pitch % CTN_TILE_T != 0 || (((uintptr_t)workspace) & 255)) return CTN_EALIGN;
   if (workspace_bytes < ctn_stage_workspace_bytes(Bc, N)) return CTN_EWORKSPACE;
-  if (math == CTN_MATH_F16X3) math = CTN_MATH_TF32X3;
   cudaStream_t st = (cudaStream_t)stream;
   Carver cv(workspace);
   StageWs ws;
@@ -715,11 +668,7 @@ extern "C" int ctn_sep_head_fwd(const float* w, const double* stats0, const floa
   memset(&a, 0, sizeof(a));
   a.A = w; a.W = ws.head.Wf; a.D = x0; a.B = B; a.M = Bc; a.K = N; a.frames = frames; a.pitch = pitch;
   a.v1 = ws.head.v1; a.v2 = ws.head.v2; a.stats_in = stats0; a.n_in = (double)N * (double)frames; a.eps = eps;
-  if (math != CTN_MATH_FP32) {
-    CTN_TRY(ctn_umma_build_wimg(ws.head.Wf, Bc, N, math, ws.wimg, st));
-    a.wimg = ws.wimg;
-  }
-  return pw_dispatch(a, PRO_NONE, EPI_HEAD, math, st);
+  return ctn_pw(a, PRO_NONE, EPI_HEAD, math, ws.wimg, st);
 }
 
 // Separator tail + decoder (conv_tasnet.py:373-376, 158-169 == dprnn_tasnet.py:348-350 + 141-153): PReLU -> mask 1x1 -> sigmoid ->
@@ -734,7 +683,6 @@ extern "C" int ctn_sep_tail_fwd(const float* y, const float* w, const float* pre
     return CTN_EINVAL;
   if (pitch < frames || pitch % CTN_TILE_T != 0 || (((uintptr_t)workspace) & 255)) return CTN_EALIGN;
   if (workspace_bytes < ctn_stage_workspace_bytes(S * N, Bc)) return CTN_EWORKSPACE;
-  if (math == CTN_MATH_F16X3) math = CTN_MATH_TF32X3;  // un-normalised operand without a static bound: tf32 pieces
   cudaStream_t st = (cudaStream_t)stream;
   Carver cv(workspace);
   StageWs ws;
@@ -743,11 +691,7 @@ extern "C" int ctn_sep_tail_fwd(const float* y, const float* w, const float* pre
   memset(&a, 0, sizeof(a));
   a.A = y; a.W = mask_w; a.D = what; a.B = B; a.M = S * N; a.K = Bc; a.frames = frames; a.pitch = pitch;
   a.pro_slope = prelu; a.bias = mask_b; a.wenc = w; a.Nb = N;
-  if (math != CTN_MATH_FP32) {
-    CTN_TRY(ctn_umma_build_wimg(mask_w, S * N, Bc, math, ws.wimg, st));
-    a.wimg = ws.wimg;
-  }
-  CTN_TRY(pw_dispatch(a, PRO_PRELU, EPI_MASK, math, st));
+  CTN_TRY(ctn_pw(a, PRO_PRELU, EPI_MASK, math, ws.wimg, st));
   CTN_TRY(ctn_decoder_fwd(what, dec_w, out, B * S, N, frames, pitch, L, stride, crop_left, T, stream));
   if (latent) CTN_TRY(ctn_copy_from_pitch(what, latent, B * S * N, frames, pitch, st));
   return CTN_OK;
@@ -803,29 +747,4 @@ extern "C" int ctn_convtasnet_loss_host(const ctn_config_t* cfg, const ctn_param
   if ((e = cudaMemcpyAsync(loss_mean_host, io.loss_mean, sizeof(float), cudaMemcpyDeviceToHost, st)) != cudaSuccess) return (int)e;
   if ((e = cudaMemcpyAsync(perm_host, io.perm, sizeof(int64_t) * (size_t)B * S, cudaMemcpyDeviceToHost, st)) != cudaSuccess) return (int)e;
   return CTN_OK;
-}
-
-// ------------------------------------------------------------------------------------------------
-// test hook
-// ------------------------------------------------------------------------------------------------
-extern "C" int ctn_debug_pointwise(const float* A, const float* W, float* D, int B, int M, int K, int frames, int pitch,
-                                   const float* bias, const float* slope, double* stats_out, int epi, int math,
-                                   const uint32_t* dbg, void* workspace, size_t workspace_bytes, ctn_stream_t stream) {
-  LaunchScope scope(A);
-  if (!A || !W || !D || B <= 0 || M <= 0 || K <= 0 || frames <= 0 || pitch < frames || pitch % 128 != 0) return CTN_EINVAL;
-  if (epi != EPI_RAW && epi != EPI_H) return CTN_EUNSUPPORTED;
-  if (epi == EPI_H && (!bias || !slope || !stats_out)) return CTN_EINVAL;
-  cudaStream_t st = (cudaStream_t)stream;
-  PwArgs a;
-  memset(&a, 0, sizeof(a));
-  a.A = A; a.W = W; a.D = D; a.B = B; a.M = M; a.K = K; a.frames = frames; a.pitch = pitch;
-  a.bias = bias; a.slope = slope; a.stats_out = stats_out;
-  if (math == CTN_MATH_FP32) return ctn_pw_simt(a, PRO_NONE, epi, st);
-  const size_t need = ctn_umma_wimg_bytes(M, K, math) + 512;
-  if (!workspace || workspace_bytes < need) return CTN_EWORKSPACE;
-  float* wimg = (float*)(((uintptr_t)workspace + 255) & ~(uintptr_t)255);
-  CTN_TRY(ctn_umma_build_wimg(W, M, K, math, wimg, st));
-  a.wimg = wimg;
-  if (dbg && (dbg[0] | dbg[1] | dbg[2] | dbg[3])) return CTN_EUNSUPPORTED;  // the wgmma kernels take no descriptor overrides
-  return ctn_pw_umma(a, PRO_NONE, epi, math, st);
 }

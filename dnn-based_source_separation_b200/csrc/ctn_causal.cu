@@ -6,26 +6,14 @@
 //   h = PReLU(W1 x + b1)  [contraction, fused bias+PReLU epilogue]   -> cLN1 (step sums -> scan -> apply, in place)
 //   u = PReLU(dwconv_causal(h) + bd)                                  -> cLN2
 //   r = [Wo; Ws] u  [contraction]   ;   x += r[:Bc] + bo ; skip += r[Bc:] + bs
-// The contractions are the same wgmma / FFMA kernels as everywhere else; the rest are streaming kernels (HBM-bound).
+// The contractions are the same wgmma / FFMA kernels as everywhere else; their operands are materialised tensors without
+// operand scales, so the f16x3 mode runs them on tf32 pieces (ctn_pw).  The rest are streaming kernels (HBM-bound).
 // Note: the reference's own cLN cannot run on CUDA (its frame counter is built on the CPU, norm.py:83), so this path has
 // no GPU baseline in the reference at all.
 #include <string.h>
 #include "ctn_internal.h"
 
 namespace {
-
-struct Carver {
-  char* base;
-  size_t off;
-  explicit Carver(void* b) : base((char*)b), off(0) {}
-  template <typename T>
-  T* take(size_t count) {
-    off = (off + 255) & ~(size_t)255;
-    T* p = base ? (T*)(base + off) : nullptr;
-    off += count * sizeof(T);
-    return p;
-  }
-};
 
 struct CausalWs {
   double* cln;   // [B][frames<=pitch][2]
@@ -37,9 +25,9 @@ struct CausalWs {
 
 size_t max_wimg(const ctn_config_t* c) {
   if (c->math == CTN_MATH_FP32) return 256;
-  size_t a = ctn_umma_wimg_bytes(c->hidden, c->bottleneck, c->math);
-  size_t b = ctn_umma_wimg_bytes(c->bottleneck + c->skip, c->hidden, c->math);
-  size_t d = c->n_basis > 0 ? ctn_umma_wimg_bytes(c->bottleneck, c->n_basis, c->math) : 0;
+  size_t a = ctn_pw_wimg_bytes(c->hidden, c->bottleneck, c->math);
+  size_t b = ctn_pw_wimg_bytes(c->bottleneck + c->skip, c->hidden, c->math);
+  size_t d = c->n_basis > 0 ? ctn_pw_wimg_bytes(c->bottleneck, c->n_basis, c->math) : 0;
   size_t m = a > b ? a : b;
   return m > d ? m : d;
 }
@@ -106,15 +94,6 @@ __global__ void __launch_bounds__(256) k_bias_rows(float* __restrict__ y, const 
 
 inline dim3 grid_cb(int C, int B) { return dim3(C < 1024 ? C : 1024, B); }
 
-int pw(const ctn_config_t* c, CausalWs& ws, PwArgs& a, int pro, int epi, cudaStream_t st) {
-  if (c->math == CTN_MATH_FP32) return ctn_pw_simt(a, pro, epi, st);
-  // causal models: operands are materialised tensors without operand scales -> tf32 pieces in the fp16-piece mode
-  const int math = c->math == CTN_MATH_F16X3 ? CTN_MATH_TF32X3 : c->math;
-  CTN_TRY(ctn_umma_build_wimg(a.W, a.M, a.K, math, ws.wimg, st));
-  a.wimg = ws.wimg;
-  return ctn_pw_umma(a, pro, epi, math, st);
-}
-
 }  // namespace
 
 size_t ctn_causal_ws_bytes(const ctn_config_t* c, int B, int pitch) {
@@ -135,7 +114,7 @@ int ctn_causal_head(const ctn_config_t* c, const ctn_params_t* p, const float* w
   PwArgs a;
   memset(&a, 0, sizeof(a));
   a.A = tmp; a.W = p->bn_w; a.D = x0; a.B = B; a.M = Bc; a.K = N; a.frames = frames; a.pitch = pitch;
-  { StageTimer tm(CTN_ST_HEAD, st); CTN_TRY(pw(c, ws, a, PRO_NONE, EPI_RAW, st)); }
+  { StageTimer tm(CTN_ST_HEAD, st); CTN_TRY(ctn_pw(a, PRO_NONE, EPI_RAW, c->math, ws.wimg, st)); }
   k_bias_rows<<<grid_cb(Bc, B), 256, 0, st>>>(x0, p->bn_b, Bc, frames, pitch);
   CTN_COUNT_LAUNCH();
   CTN_RETURN_IF_CUDA_ERR();
@@ -160,7 +139,7 @@ int ctn_causal_tcn(const ctn_config_t* c, const ctn_block_params_t* blocks, floa
     memset(&a, 0, sizeof(a));
     a.A = x; a.W = q.bottleneck_w; a.D = h; a.B = B; a.M = H; a.K = Bc; a.frames = frames; a.pitch = pitch;
     a.bias = q.bottleneck_b; a.slope = q.prelu1; a.stats_out = ws.dummy;
-    { StageTimer tm(CTN_ST_PW1, st); CTN_TRY(pw(c, ws, a, PRO_NONE, EPI_H, st)); }
+    { StageTimer tm(CTN_ST_PW1, st); CTN_TRY(ctn_pw(a, PRO_NONE, EPI_H, c->math, ws.wimg, st)); }
     {
       StageTimer tm(CTN_ST_DW, st);
       CTN_TRY(ctn_cln_pitch_fwd(h, q.norm1_g, q.norm1_b, h, B, H, frames, pitch, c->eps_tcn, ws.cln, st));
@@ -177,7 +156,7 @@ int ctn_causal_tcn(const ctn_config_t* c, const ctn_block_params_t* blocks, floa
       return (int)e;
     memset(&a, 0, sizeof(a));
     a.A = u; a.W = ws.Wcat; a.D = ws.r; a.B = B; a.M = Mt; a.K = H; a.frames = frames; a.pitch = pitch;
-    { StageTimer tm(CTN_ST_PW2, st); CTN_TRY(pw(c, ws, a, PRO_NONE, EPI_RAW, st)); }
+    { StageTimer tm(CTN_ST_PW2, st); CTN_TRY(ctn_pw(a, PRO_NONE, EPI_RAW, c->math, ws.wimg, st)); }
     {
       StageTimer tm(CTN_ST_FIN, st);
       k_res_skip_inplace<<<grid_cb(Mt, B), 256, 0, st>>>(ws.r, Mt, x, skip, q.out_b, q.skip_b, Bc, Sc, has_out ? 1 : 0, i == 0 ? 1 : 0,

@@ -52,9 +52,8 @@ extern "C" int ctn_pointwise_conv1d_fwd(const float* x, const float* W, const fl
   LaunchScope scope(x);
   if (!x || !W || !y || !workspace || B <= 0 || M <= 0 || K <= 0 || frames <= 0) return CTN_EINVAL;
   if (pitch < frames || pitch % CTN_TILE_T != 0 || (((uintptr_t)workspace) & 255)) return CTN_EALIGN;
-  if (math == CTN_MATH_F16X3) math = CTN_MATH_TF32X3;  // arbitrary operand magnitudes: tf32 pieces
   const size_t ybytes = ((size_t)B * M * pitch * sizeof(float) + 255) & ~(size_t)255;
-  const size_t wbytes = math != CTN_MATH_FP32 ? ctn_umma_wimg_bytes(M, K, math) + 256 : 0;
+  const size_t wbytes = math != CTN_MATH_FP32 ? ctn_pw_wimg_bytes(M, K, math) + 256 : 0;
   if (workspace_bytes < ybytes + wbytes + (size_t)B * 2 * sizeof(double) + 64 * sizeof(float) + 512) return CTN_EWORKSPACE;
   cudaStream_t st = (cudaStream_t)stream;
   float* yp = (float*)workspace;
@@ -74,12 +73,6 @@ extern "C" int ctn_pointwise_conv1d_fwd(const float* x, const float* W, const fl
     a.bias = bias; a.slope = one; a.stats_out = stats;
     epi = EPI_H;
   }
-  if (math == CTN_MATH_FP32) {
-    CTN_TRY(ctn_pw_simt(a, PRO_NONE, epi, st));
-  } else {
-    CTN_TRY(ctn_umma_build_wimg(W, M, K, math, wimg, st));
-    a.wimg = wimg;
-    CTN_TRY(ctn_pw_umma(a, PRO_NONE, epi, math, st));
-  }
+  CTN_TRY(ctn_pw(a, PRO_NONE, epi, math, wimg, st));  // arbitrary operand magnitudes, no operand scale: tf32 pieces in f16x3
   return ctn_copy_from_pitch(yp, y, B * M, frames, pitch, st);
 }

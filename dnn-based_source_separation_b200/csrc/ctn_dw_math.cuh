@@ -1,4 +1,4 @@
-// Depthwise-stage math shared by the fused depthwise + pointwise producers (ctn_umma.cu).
+// Depthwise-stage math shared by the fused depthwise + pointwise producers (ctn_wgmma.cu).
 #pragma once
 #include "ctn_common.cuh"
 

@@ -13,6 +13,20 @@ struct FoldedConv {
               // of the gLN group) >= max |normalised value|  (activation envelope of the fp16-piece mode)
 };
 
+// Workspace carving: 256-byte aligned sub-buffers of one allocation.  base == nullptr only measures (off = bytes needed).
+struct Carver {
+  char* base;
+  size_t off;
+  explicit Carver(void* b) : base((char*)b), off(0) {}
+  template <typename T>
+  T* take(size_t count) {
+    off = (off + 255) & ~(size_t)255;
+    T* p = base ? (T*)(base + off) : nullptr;
+    off += count * sizeof(T);
+    return p;
+  }
+};
+
 #define CTN_MAX_BLOCKS 64
 // epilogue / prologue selectors of the pointwise (1x1) contraction kernels
 enum { PRO_NONE = 0, PRO_PRELU = 1, PRO_DW = 2, PRO_RES = 3 };
@@ -63,7 +77,7 @@ struct PwArgs {
   float res_eps;
   float* res_x_out;         // (B, K, pitch)
   // tensor-core path only
-  const float* wimg;       // pre-swizzled hi/lo weight images (ctn_umma_build_wimg)
+  const float* wimg;       // pre-swizzled hi/lo weight images (ctn_pw_prepare)
   // fp16-piece mode: power-of-two scale of the activation operand (device scalar, nullable = 1), chosen per forward from a
   // bound on |operand| derived from the weights alone (ctn_act_scales) so that fp16 can never saturate; undone in the epilogue
   const float* act_scale;
@@ -74,19 +88,21 @@ struct PwArgs {
   float* dw_u_pre_out;
 };
 
-// fp32 CUDA-core path (ctn_tcn_simt.cu)
-int ctn_pw_simt(const PwArgs& a, int pro, int epi, cudaStream_t st);
-// wgmma tensor-core path (ctn_umma.cu); math = CTN_MATH_TF32X3 / CTN_MATH_TF32 / CTN_MATH_F16X3
-int ctn_pw_umma(const PwArgs& a, int pro, int epi, int math, cudaStream_t st);
+// One 1x1 contraction (ctn_wgmma.cu).  math is the model's mode: fp32 runs the FFMA kernel; the tensor-core modes run the wgmma
+// kernel, on fp16 pieces in the f16x3 mode exactly when the operand has a static bound (a.act_scale), on tf32 pieces otherwise.
+// wimg_scratch == nullptr: a.wimg already holds the weight image (ctn_pw_prepare / ctn_pw_prepare_batch with the same
+// math); otherwise the image of a.W is built into wimg_scratch (ctn_pw_wimg_bytes) first.
+int ctn_pw(const PwArgs& a, int pro, int epi, int math, float* wimg_scratch, cudaStream_t st);
+size_t ctn_pw_wimg_bytes(int M, int K, int math);
+// weight image of a.W (a.M, a.K) for ctn_pw(a, .., math, nullptr, ..); nothing to do in the fp32 mode
+int ctn_pw_prepare(const PwArgs& a, int math, float* wimg, cudaStream_t st);
 // EPI_MASKDEC (PRO_PRELU) applies to this contraction: fp16-piece mode, n_basis a multiple of 128, decoder kernel 16 / stride 8 (caller)
 int ctn_pw_maskdec_supported(const PwArgs& a, int math);
-size_t ctn_umma_wimg_bytes(int M, int K, int math);
-int ctn_umma_build_wimg(const float* W, int M, int K, int math, float* wimg, cudaStream_t st);
 
-// wgmma weight gradient of a 1x1 conv (ctn_wgrad_umma.cu): dW (M,K) += sum_{b,t} dY[b][m][t] X[b][k][t]; rows
+// wgmma weight gradient of a 1x1 conv (ctn_wgrad_wgmma.cu): dW (M,K) += sum_{b,t} dY[b][m][t] X[b][k][t]; rows
 // [0,split_row) -> dWa, rest -> dWb (nullable).  dW must be zero-initialised by the caller (split-K partials are added).
-int ctn_wgrad_umma(const float* dy, size_t dy_bs, const float* x, size_t x_bs, float* dWa, float* dWb, int split_row, int M,
-                   int K, int B, int frames, int pitch, int math, cudaStream_t st);
+int ctn_wgrad_wgmma(const float* dy, size_t dy_bs, const float* x, size_t x_bs, float* dWa, float* dWb, int split_row, int M,
+                    int K, int B, int frames, int pitch, int math, cudaStream_t st);
 
 int ctn_fold_conv(const float* W, const float* bias, const float* gamma, const float* beta, int M, int K, FoldedConv out,
                   int row_offset, cudaStream_t st, float R = 0.f);
@@ -96,7 +112,8 @@ struct FoldJob { const float *W, *bias, *gamma, *beta; float *Wf, *v1, *v2; int 
 struct WimgJob { const float* W; float* wimg; int M, K; };
 #define CTN_MAX_JOBS 48
 int ctn_fold_batch(const FoldJob* jobs, int n, cudaStream_t st);
-int ctn_umma_build_wimg_batch(const WimgJob* jobs, int n, int math, cudaStream_t st);
+// weight images of the jobs in one launch; bounded: every one of these contractions carries an operand scale (see ctn_pw)
+int ctn_pw_prepare_batch(const WimgJob* jobs, int n, int math, bool bounded, cudaStream_t st);
 
 // Activation envelope of the fp16-piece mode.  Per residual block i the two operands that meet the tensor core as fp16
 // pieces are x_i (pw1) and u_i (fused depthwise output, pw2); the mask contraction sees PReLU(skip sum).  From the weights

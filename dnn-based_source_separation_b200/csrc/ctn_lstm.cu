@@ -14,7 +14,7 @@
 //     W_fc[:, dir*H:(dir+1)*H]^T on the freshly written h slabs; each direction stores its partial projection (NSEQ, T, F) and the
 //     gLN + residual kernel adds the two and the bias, so the (NSEQ, T, 2H) LSTM output is only materialised on request.
 #include "ctn_internal.h"
-#include "ctn_umma_ptx.cuh"
+#include "ctn_wgmma_ptx.cuh"
 
 namespace {
 
@@ -302,11 +302,6 @@ size_t lstm_fixed_smem(int F, int H) { return 2048 + (size_t)(F / 32 + H / 32) *
 size_t lstm_ws_bytes(int F, int H, int Fo) { return 256 + (size_t)2 * 4 * H * 4 + (size_t)2 * lstm_per_step(F, H, Fo > 0) * SLAB; }
 
 }  // namespace
-
-extern "C" int ctn_debug_lstm_timeline(unsigned long long* out, int n) {
-  if (!out || n <= 0 || n > 160) return CTN_EINVAL;
-  return CTN_EUNSUPPORTED;  // the recurrence kernel records no timeline
-}
 
 extern "C" int ctn_bilstm_supported(int F, int H, int Fo) { return lstm_supported(F, H, Fo) ? 1 : 0; }
 

@@ -5,7 +5,7 @@
 //
 // Structure (first cut: correctness and full coverage; the dense contractions already run on the wgmma kernels):
 //   * every 1x1 convolution, forward or data-gradient (W^T dY), is ONE call of the pointwise contraction kernels of the
-//     inference path (ctn_pw_umma / ctn_pw_simt, raw epilogue) -- 3xTF32 on the tensor cores by default;
+//     inference path (ctn_pw, raw epilogue) -- 3xTF32 on the tensor cores by default;
 //   * weight gradients dW = sum_{b,t} dY X^T reduce over B*frames (128 k at cfg2): a split-K FFMA kernel (k_wgrad,
 //     64x64 register-tiled, fp32 atomics across the splits);
 //   * everything between the contractions (bias, PReLU, gLN and their backward, dilated depthwise conv and its
@@ -13,27 +13,12 @@
 //     per-sample gLN reductions accumulated in double.
 // Saved per residual block: its input x_i, the pre-activations h_pre = W1 x + b1 and u_pre = dwconv(gLN1(PReLU h_pre)) + bd,
 // and the two (sum, sumsq) statistics; normalised tensors are recomputed in the backward.
-#include <stdlib.h>
 #include <string.h>
 #include <vector>
 #include <math.h>
-#include <stdlib.h>
 #include "ctn_internal.h"
 
 namespace {
-
-struct Carver {
-  char* base;
-  size_t off;
-  explicit Carver(void* b) : base((char*)b), off(0) {}
-  template <typename T>
-  T* take(size_t count) {
-    off = (off + 255) & ~(size_t)255;
-    T* p = base ? (T*)(base + off) : nullptr;
-    off += count * sizeof(T);
-    return p;
-  }
-};
 
 // ================================================================================================================
 // streaming kernels.  Layout (B, C, pitch), pitch % 128 == 0, rows 16-byte aligned; only columns t < frames carry data,
@@ -691,7 +676,7 @@ struct TrainWs {
   float *sp, *dsp;          // (B, Sc, pitch)
   double* sums;             // (B, 2)
   size_t stats_bytes;
-  void* tcn_mem;            // fp16-piece mode: state of the fused TCN forward (ctn_tcn_train_fwd)
+  void* tcn_mem;            // fused_tcn(): state of the fused TCN forward (ctn_tcn_train_fwd)
   size_t tcn_bytes;
 };
 
@@ -701,11 +686,17 @@ size_t max_wimg_bytes(const ctn_config_t* c) {
   const int shapes[][2] = {{H, Bc}, {Bc + Sc, H}, {H, Bc + Sc}, {Bc, H}, {Bc, N}, {N, Bc}, {SN, Sc}, {Sc, SN}};
   size_t mx = 0;
   for (auto& s : shapes) {
-    const size_t b = ctn_umma_wimg_bytes(s[0], s[1], c->math);
+    const size_t b = ctn_pw_wimg_bytes(s[0], s[1], c->math);
     if (b > mx) mx = b;
   }
   return mx;
 }
+
+// fp16-piece mode with 3-tap depthwise convs: the TCN forward runs through the SAME fused kernels as inference (pw1 with the
+// residual update fused, depthwise producer feeding the [out;skip] contraction), which additionally leave x_i, W1 x + b1 and
+// the depthwise pre-activation behind for the backward -- 2 launches per block instead of 7, no u / gLN2(u) round trips.
+// With check_train_cfg (non-causal, dilations 2^l) every block of such a config is within the fused kernels' envelope.
+bool fused_tcn(const ctn_config_t* c) { return c->math == CTN_MATH_F16X3 && c->sep_kernel == 3; }
 
 void carve_train(Carver& cv, const ctn_config_t* c, int B, int pitch, TrainWs* ws) {
   const int RX = c->num_blocks * c->num_layers;
@@ -733,7 +724,7 @@ void carve_train(Carver& cv, const ctn_config_t* c, int B, int pitch, TrainWs* w
   ws->head.vb = cv.take<float>(Bc);
   ws->tcn_mem = nullptr;
   ws->tcn_bytes = 0;
-  if (c->math == CTN_MATH_F16X3 && c->sep_kernel == 3) {
+  if (fused_tcn(c)) {
     ws->tcn_bytes = ctn_tcn_train_ws_bytes(c, B, pitch);
     ws->tcn_mem = cv.take<char>(ws->tcn_bytes);
   }
@@ -770,23 +761,15 @@ int check_train_cfg(const ctn_config_t* c) {
   return CTN_OK;
 }
 
-// D (B, M, pitch) = W (M, K) . A (B, K, pitch), raw epilogue, in the configured numeric mode
-// grad = true: the operand is a GRADIENT tensor.  Gradients have no fixed scale (1e-3 .. 1e-9 and below), which the fp16
-// pieces of 'f16x3' cannot represent (subnormal below 6e-5, zero below 6e-8), so data-gradient contractions always use the
-// tf32 pieces (8-bit exponent); 'f16x3' applies to the forward contractions, whose operands sit behind normalisations.
+// D (B, M, pitch) = W (M, K) . A (B, K, pitch), raw epilogue, in the configured numeric mode.  The operands here (gradients,
+// and the forward's materialised x_i / gLN2 output) carry no operand scale, so 'f16x3' runs these on the tf32 pieces: gradients
+// have no fixed scale (1e-3 .. 1e-9 and below), which fp16 pieces cannot represent (subnormal below 6e-5, zero below 6e-8).
 int gemm_raw(const ctn_config_t* c, TrainWs& ws, const float* W, int M, int K, const float* A, float* D, int B, int frames,
-             int pitch, cudaStream_t st, bool grad = false) {
+             int pitch, cudaStream_t st) {
   PwArgs a;
   memset(&a, 0, sizeof(a));
   a.A = A; a.W = W; a.D = D; a.B = B; a.M = M; a.K = K; a.frames = frames; a.pitch = pitch;
-  if (c->math == CTN_MATH_FP32) return ctn_pw_simt(a, PRO_NONE, EPI_RAW, st);
-  // the training path keeps every contraction on the tf32 pieces: its forward operands (x_i, gLN2 output, skip sum) are
-  // materialised tensors without the per-forward operand scales of the fused inference kernels (ctn_act_scales)
-  (void)grad;
-  const int math = c->math == CTN_MATH_F16X3 ? CTN_MATH_TF32X3 : c->math;
-  CTN_TRY(ctn_umma_build_wimg(W, M, K, math, ws.wimg, st));
-  a.wimg = ws.wimg;
-  return ctn_pw_umma(a, PRO_NONE, EPI_RAW, math, st);
+  return ctn_pw(a, PRO_NONE, EPI_RAW, c->math, ws.wimg, st);
 }
 
 int transpose(const float* W, float* Wt, int M, int K, cudaStream_t st) {
@@ -799,9 +782,8 @@ int transpose(const float* W, float* Wt, int M, int K, cudaStream_t st) {
 // configured mode is plain fp32, where the FFMA split-K kernel runs.
 int wgrad(const ctn_config_t* c, const float* dy, size_t dy_bs, const float* x, size_t x_bs, float* dWa, float* dWb, int split_row,
           int M, int K, int B, int frames, int pitch, cudaStream_t st) {
-  static const char* env = getenv("CTN_WGRAD_SIMT");  // debug: force the FFMA kernel
-  if (c->math != CTN_MATH_FP32 && !(env && atoi(env)))
-    return ctn_wgrad_umma(dy, dy_bs, x, x_bs, dWa, dWb, split_row, M, K, B, frames, pitch, c->math, st);
+  if (c->math != CTN_MATH_FP32)
+    return ctn_wgrad_wgmma(dy, dy_bs, x, x_bs, dWa, dWb, split_row, M, K, B, frames, pitch, c->math, st);
   const int parts = dWb ? 2 : 1;
   for (int part = 0; part < parts; ++part) {
     const int r0 = part == 0 ? 0 : split_row, Mp = part == 0 ? (dWb ? split_row : M) : M - split_row;
@@ -899,32 +881,16 @@ extern "C" int ctn_convtasnet_fwd_train(const ctn_config_t* c, const ctn_params_
     memset(&a, 0, sizeof(a));
     a.A = ws.w; a.W = ws.head.Wf; a.D = ws.x[0]; a.B = B; a.M = Bc; a.K = N; a.frames = frames; a.pitch = pitch;
     a.v1 = ws.head.v1; a.v2 = ws.head.v2; a.stats_in = ws.stats0; a.n_in = (double)N * (double)frames; a.eps = c->eps;
-    if (c->math == CTN_MATH_FP32) {
-      CTN_TRY(ctn_pw_simt(a, PRO_NONE, EPI_HEAD, st));
-    } else {
-      // the head reads the un-normalised encoder output: tf32 pieces even in the fp16-piece mode (see ctn_api.cu)
-      const int head_math = c->math == CTN_MATH_F16X3 ? CTN_MATH_TF32X3 : c->math;
-      CTN_TRY(ctn_umma_build_wimg(ws.head.Wf, Bc, N, head_math, ws.wimg, st));
-      a.wimg = ws.wimg;
-      CTN_TRY(ctn_pw_umma(a, PRO_NONE, EPI_HEAD, head_math, st));
-    }
+    // the head reads the un-normalised encoder output: no operand scale, tf32 pieces in the fp16-piece mode (see ctn_api.cu)
+    CTN_TRY(ctn_pw(a, PRO_NONE, EPI_HEAD, c->math, ws.wimg, st));
   }
   const double nH = (double)H * (double)frames;
-  // un-normalised operands (x_i, skip sum) without operand scales: tf32 pieces (8-bit exponent) in the fp16-piece mode
-  const int fmath = c->math == CTN_MATH_F16X3 ? CTN_MATH_TF32X3 : c->math;
-  // fp16-piece mode: the TCN runs through the SAME fused kernels as inference (pw1 with the residual update fused,
-  // depthwise producer feeding the [out;skip] contraction), which additionally leave x_i, W1 x + b1 and the depthwise
-  // pre-activation behind for the backward -- 2 launches per block instead of 7, no u / gLN2(u) round trips
-  bool fused = false;
-  const float* mask_scale = nullptr;
-  static const char* env_unf = getenv("CTN_TRAIN_UNFUSED");
-  if (ws.tcn_mem && !(env_unf && atoi(env_unf))) {
+  const bool fused = fused_tcn(c);
+  const float* mask_scale = nullptr;  // fused: operand scale of PReLU(skip sum), produced by the fused forward
+  if (fused) {
     TcnTrainHooks hk{ws.x.data(), ws.hpre.data(), ws.upre.data()};
-    const int rc = ctn_tcn_train_fwd(c, p->blocks, ws.tcn_mem, ws.tcn_bytes, &hk, ws.stats, ws.skip, ws.head.vb, Bc, p->prelu_out, &mask_scale,
-                                     B, frames, pitch, st);
-    if (rc == CTN_OK) fused = true;
-    else if (rc != CTN_EUNSUPPORTED) return rc;
-    else if ((e = cudaMemsetAsync(ws.stats, 0, ws.stats_bytes, st)) != cudaSuccess) return (int)e;  // shapes outside the fused envelope
+    CTN_TRY(ctn_tcn_train_fwd(c, p->blocks, ws.tcn_mem, ws.tcn_bytes, &hk, ws.stats, ws.skip, ws.head.vb, Bc, p->prelu_out, &mask_scale,
+                              B, frames, pitch, st));
   }
   for (int i = 0; i < (fused ? 0 : R * X); ++i) {
     const ctn_block_params_t& q = p->blocks[i];
@@ -944,9 +910,7 @@ extern "C" int ctn_convtasnet_fwd_train(const ctn_config_t* c, const ctn_params_
       memset(&a, 0, sizeof(a));
       a.A = ws.x[i]; a.W = q.bottleneck_w; a.D = ws.hpre[i]; a.B = B; a.M = H; a.K = Bc; a.frames = frames; a.pitch = pitch;
       a.bias = q.bottleneck_b; a.slope = q.prelu1; a.stats_out = st1; a.store_pre = 1;
-      CTN_TRY(ctn_umma_build_wimg(q.bottleneck_w, H, Bc, fmath, ws.wimg, st));
-      a.wimg = ws.wimg;
-      CTN_TRY(ctn_pw_umma(a, PRO_NONE, EPI_H, fmath, st));
+      CTN_TRY(ctn_pw(a, PRO_NONE, EPI_H, c->math, ws.wimg, st));
     }
     // u_pre = dwconv(gLN1(PReLU(h_pre))) + bd ; stats2 of PReLU(u_pre)
     k_dw_train_fwd<<<grid_cb(H, B), 256, 0, st>>>(ws.hpre[i], ws.upre[i], q.norm1_g, q.norm1_b, q.dw_w, q.dw_b, q.prelu1, q.prelu2,
@@ -971,16 +935,8 @@ extern "C" int ctn_convtasnet_fwd_train(const ctn_config_t* c, const ctn_params_
     PwArgs a;
     memset(&a, 0, sizeof(a));
     a.A = ws.skip; a.W = p->mask_w; a.D = ws.what; a.B = B; a.M = S * N; a.K = Sc; a.frames = frames; a.pitch = pitch;
-    a.pro_slope = p->prelu_out; a.bias = p->mask_b; a.wenc = ws.w; a.Nb = N; a.mask_out = ws.mask;
-    if (c->math == CTN_MATH_FP32) {
-      CTN_TRY(ctn_pw_simt(a, PRO_PRELU, EPI_MASK, st));
-    } else {
-      const int mmath = fused ? CTN_MATH_F16X3 : fmath;  // the fused forward also produced the operand scale of PReLU(skip sum)
-      if (fused) a.act_scale = mask_scale;
-      CTN_TRY(ctn_umma_build_wimg(p->mask_w, S * N, Sc, mmath, ws.wimg, st));
-      a.wimg = ws.wimg;
-      CTN_TRY(ctn_pw_umma(a, PRO_PRELU, EPI_MASK, mmath, st));
-    }
+    a.pro_slope = p->prelu_out; a.bias = p->mask_b; a.wenc = ws.w; a.Nb = N; a.mask_out = ws.mask; a.act_scale = mask_scale;
+    CTN_TRY(ctn_pw(a, PRO_PRELU, EPI_MASK, c->math, ws.wimg, st));
   }
   CTN_TRY(ctn_decoder_fwd(ws.what, p->dec_w, out, B * S, N, frames, pitch, c->kernel_size, c->stride, pl, T, stream));
   return CTN_OK;
@@ -1022,7 +978,7 @@ extern "C" int ctn_convtasnet_bwd(const ctn_config_t* c, const ctn_params_t* p, 
   CTN_TRY(wgrad(c, ws.dwhat, bsSN, ws.sp, bsSc, G(grads->mask_w), nullptr, 0, S * N, Sc, B, frames, pitch, st));
   CTN_TRY(rowsum(ws.dwhat, bsSN, S * N, B, frames, pitch, G(grads->mask_b), st));
   CTN_TRY(transpose(p->mask_w, ws.Wt, S * N, Sc, st));
-  CTN_TRY(gemm_raw(c, ws, ws.Wt, Sc, S * N, ws.dwhat, ws.dsp, B, frames, pitch, st, /*grad=*/true));
+  CTN_TRY(gemm_raw(c, ws, ws.Wt, Sc, S * N, ws.dwhat, ws.dsp, B, frames, pitch, st));
   // ---- PReLU on the skip sum (conv_tasnet.py:340,373): dS (the gradient of EVERY block's skip output)
   k_prelu_bwd<<<dim3(Sc, B), 256, 0, st>>>(ws.dsp, ws.skip, ws.dS, p->prelu_out, G(grads->prelu_out), Sc, frames, pitch);
   LAUNCH_CHECK();
@@ -1059,7 +1015,7 @@ extern "C" int ctn_convtasnet_bwd(const ctn_config_t* c, const ctn_params_t* p, 
       if ((e = cudaMemcpyAsync(ws.Wcat + (has_out ? (size_t)Bc * H : 0), q.skip_w, sizeof(float) * (size_t)Sc * H, cudaMemcpyDeviceToDevice, st)) != cudaSuccess) return (int)e;
     }
     CTN_TRY(transpose(ws.Wcat, ws.Wt, Mt, H, st));
-    CTN_TRY(gemm_raw(c, ws, ws.Wt, H, Mt, dY, ws.G1, B, frames, pitch, st, /*grad=*/true));
+    CTN_TRY(gemm_raw(c, ws, ws.Wt, H, Mt, dY, ws.G1, B, frames, pitch, st));
     // gLN2 + PReLU2 backward -> d_u_pre (G1 in place); dgamma2, dbeta2, da2, d(bd)
     CTN_TRY(gln_prelu_bwd(ws.G1, ws.upre[i], ws.G1, q.prelu2, q.norm2_g, st2, nH, c->eps_tcn, ws.sums, G(gq.norm2_g), G(gq.norm2_b),
                           G(gq.prelu2), G(gq.dw_b), B, H, frames, pitch, st));
@@ -1078,7 +1034,7 @@ extern "C" int ctn_convtasnet_bwd(const ctn_config_t* c, const ctn_params_t* p, 
     // bottleneck 1x1: dW1 = d_h_pre x_i^T ; d_x_i = W1^T d_h_pre (+ residual path)
     CTN_TRY(wgrad(c, ws.G2, bsH, ws.x[i], bsBc, G(gq.bottleneck_w), nullptr, 0, H, Bc, B, frames, pitch, st));
     CTN_TRY(transpose(q.bottleneck_w, ws.Wt, H, Bc, st));
-    CTN_TRY(gemm_raw(c, ws, ws.Wt, Bc, H, ws.G2, ws.dxtmp, B, frames, pitch, st, /*grad=*/true));
+    CTN_TRY(gemm_raw(c, ws, ws.Wt, Bc, H, ws.G2, ws.dxtmp, B, frames, pitch, st));
     k_rows<<<grid_cb(Bc, B), 256, 0, st>>>(ws.dcat, bsCat, ws.dxtmp, bsBc, Bc, has_out ? 1 : 0, frames, pitch);
     LAUNCH_CHECK();
   }
@@ -1092,7 +1048,7 @@ extern "C" int ctn_convtasnet_bwd(const ctn_config_t* c, const ctn_params_t* p, 
   k_rows<<<grid_cb(Bc, B), 256, 0, st>>>(ws.dxtmp, bsBc, ws.dcat, bsCat, Bc, 0, frames, pitch);
   LAUNCH_CHECK();
   CTN_TRY(transpose(p->bn_w, ws.Wt, Bc, N, st));
-  CTN_TRY(gemm_raw(c, ws, ws.Wt, N, Bc, ws.dxtmp, ws.nB, B, frames, pitch, st, /*grad=*/true));
+  CTN_TRY(gemm_raw(c, ws, ws.Wt, N, Bc, ws.dxtmp, ws.nB, B, frames, pitch, st));
   // gLN0 backward -> d_w (norm path) ; + product path ; ReLU mask of the encoder if any
   CTN_TRY(gln_prelu_bwd(ws.nB, ws.w, ws.nB, nullptr, p->norm0_g, ws.stats0, (double)N * frames, c->eps, ws.sums, G(grads->norm0_g),
                         G(grads->norm0_b), nullptr, nullptr, B, N, frames, pitch, st));

@@ -196,7 +196,6 @@ int ctn_dprnn_norm_res_fwd(const float* Y, const float* R, const float* gamma, c
  * (ctn_bilstm_supported); workspace >= ctn_bilstm_workspace_bytes(F,H,Fo), 256-byte aligned.  z_absmax (nullable): device word holding
  * the bit pattern of max|z| (the fp16 operand scale of x is derived from it); null = measured here with one more pass over z. */
 int ctn_bilstm_supported(int F, int H, int Fo);
-int ctn_debug_lstm_timeline(unsigned long long* out, int n); /* debug hook: returns CTN_EUNSUPPORTED (no timeline is recorded) */
 size_t ctn_bilstm_workspace_bytes(int F, int H, int Fo);
 int ctn_bilstm_proj_fwd(const float* z, int NSEQ, int T, int F, int H, const float* const* w, const float* w_fc, int Fo, float* P,
                         float* hout, const unsigned* z_absmax, void* workspace, size_t workspace_bytes, ctn_stream_t stream);
@@ -286,17 +285,6 @@ int ctn_clip_adam_step(const int32_t* chunk_table, int n_chunks, float* const* p
                        const int32_t* numel, int n_tensors, const float* flat_grad, size_t flat_numel, float* exp_avg,
                        float* exp_avg_sq, double* sumsq_scratch, const float* lr, long long* step, float beta1, float beta2, float eps,
                        float weight_decay, float max_norm, float* norm_out, ctn_stream_t stream);
-
-/* Test hook: ONE pointwise (1x1) contraction D[b][m][t] = epi(sum_k W[m][k] A[b][k][t]) in the selected numeric mode,
- * so tests can compare the wgmma kernels with the FFMA kernels operand by operand.  A (B,K,pitch), D (B,M,pitch),
- * pitch % 128 == 0.  epi: 0 = raw, 2 = +bias, PReLU(slope), (sum,sumsq) -> stats_out.  dbg (nullable): 4 words
- * kept for ABI compatibility; the wgmma kernels take no descriptor overrides, so any non-zero word -> CTN_EUNSUPPORTED.  workspace: >= 4*M*K*2 + 64 KiB bytes. */
-int ctn_debug_pointwise(const float* A, const float* W, float* D, int B, int M, int K, int frames, int pitch,
-                        const float* bias, const float* slope, double* stats_out, int epi, int math,
-                        const uint32_t* dbg, void* workspace, size_t workspace_bytes, ctn_stream_t stream);
-
-/* Debug hook kept for ABI stability: the wgmma pointwise kernels record no timeline, so it returns CTN_EUNSUPPORTED. */
-int ctn_debug_timeline(unsigned long long* host, int n);
 
 /* number of kernel launches the last ctn_* call on this thread enqueued (for bench.py's gpu_launches) */
 int ctn_last_launch_count(void);

@@ -454,7 +454,7 @@ def test_forward_and_loss_are_cuda_graph_capturable():
 @pytest.mark.skipif(not N.ctn_has_tcgen05(), reason="tensor-core family not built")
 @pytest.mark.parametrize("mode", ["tf32x3", "f16x3"])
 def test_split_modes_are_robust_to_weight_magnitudes(mode):
-    """The fp16-piece mode rescales every weight row by a power of two (ctn_umma.cu: wimg_f16_rows), so tiny (gamma-folded)
+    """The fp16-piece mode rescales every weight row by a power of two (ctn_wgmma.cu: wimg_f16_group), so tiny (gamma-folded)
     or huge rows keep fp32-level accuracy although fp16 itself spans only 6e-8 .. 65504."""
     cfg = O.OracleConfig(n_basis=64, kernel_size=16, sep_hidden_channels=96, sep_bottleneck_channels=48, sep_skip_channels=32,
                          sep_num_blocks=2, sep_num_layers=3, causal=False, n_sources=2)
