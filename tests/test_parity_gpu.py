@@ -69,7 +69,9 @@ def test_encoder_decoder_golden(golden_dir):
 
 
 @pytest.mark.parametrize("N_,L,S,T,B", [(512, 16, 8, 32000, 2), (64, 2, 1, 777, 3), (48, 20, 10, 1000, 2), (33, 8, 4, 203, 1),
-                                       (16, 32, 16, 4096, 2), (8, 16, 8, 16, 1)])
+                                       (16, 32, 16, 4096, 2), (8, 16, 8, 16, 1),
+                                       # L > 32: the longest encoder cases, decoded by k_decoder_generic; L = 32 again with an odd T
+                                       (24, 40, 20, 2000, 2), (64, 64, 32, 3000, 2), (40, 32, 16, 1001, 3)])
 def test_encoder_decoder_oracle(N_, L, S, T, B):
     g = torch.Generator().manual_seed(N_ + T)
     enc, dec = Encoder(1, N_, kernel_size=L, stride=S).cuda(), Decoder(N_, 1, kernel_size=L, stride=S).cuda()
@@ -231,6 +233,10 @@ def test_model_ragged_lengths_vs_oracle(mode, T):
          sep_num_blocks=1, sep_num_layers=2, n_sources=3),                       # > 256 output channels: several n-tiles
     dict(n_basis=16, kernel_size=2, stride=1, sep_hidden_channels=32, sep_bottleneck_channels=16, sep_skip_channels=16,
          sep_num_blocks=2, sep_num_layers=9, n_sources=2),                       # dilation 256 > 2 tiles; L=2, stride 1
+    dict(n_basis=24, kernel_size=40, stride=20, sep_hidden_channels=40, sep_bottleneck_channels=20, sep_skip_channels=12,
+         sep_kernel_size=4, sep_num_blocks=1, sep_num_layers=8, n_sources=2),     # P=4: asymmetric pad_left = (P-1)*d//2; L=40
+    dict(n_basis=40, kernel_size=20, stride=10, sep_hidden_channels=40, sep_bottleneck_channels=24, sep_skip_channels=24,
+         sep_kernel_size=7, sep_num_blocks=1, sep_num_layers=4, n_sources=2),     # P=7; k_encoder_v4<20,10>, k_decoder<10,2>
 ])
 def test_model_odd_shapes_vs_oracle(mode, shape):
     cfg = O.OracleConfig(causal=False, **shape)
@@ -522,11 +528,12 @@ def test_split_modes_are_robust_to_residual_and_skip_magnitude(mode, mag):
 
 
 @pytest.mark.skipif(not N.ctn_has_tcgen05(), reason="tensor-core family not built")
-@pytest.mark.parametrize("T,S", [(8000, 2), (8003, 3), (1031, 2)])
+@pytest.mark.parametrize("T,S", [(8000, 2), (8003, 3), (1031, 2), (4000, 5)])
 def test_fused_mask_decoder_matches_unfused_and_oracle(T, S):
     """forward() runs the fused mask 1x1 + sigmoid + w*mask + ConvTranspose1d + crop epilogue (w_hat never materialised, fp16-piece
     mode, N = 512); extract_latent() materialises w_hat and runs the stand-alone decoder.  Same estimates, and both == oracle.
-    T = 8003 / 1031 exercise the crop offset (padding_left != 0) and a partial last tile."""
+    T = 8003 / 1031 exercise the crop offset (padding_left != 0) and a partial last tile.  S = 5: S*N = 2560 > F16_MAX_ROWS, so
+    the mask contraction falls back to tf32 pieces and maskdec_ok refuses the fused epilogue; forward() must still match."""
     cfg = O.OracleConfig(n_basis=512, kernel_size=16, sep_hidden_channels=64, sep_bottleneck_channels=32, sep_skip_channels=32,
                          sep_num_blocks=1, sep_num_layers=3, causal=False, n_sources=S)
     sd = O.synth_state_dict(cfg, seed=61)
