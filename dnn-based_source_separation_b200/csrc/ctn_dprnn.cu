@@ -102,7 +102,8 @@ __global__ void __launch_bounds__(256) k_sample_stats(const float* __restrict__ 
   __shared__ double red[64];
   const int b = blockIdx.y;
   const float4* p = reinterpret_cast<const float4*>(Y + (size_t)b * n);
-  const size_t n4 = n / 4;
+  // 128-bit loads only when every sample starts 16-byte aligned (Y is; sample b sits b*n floats further): else all scalar
+  const size_t n4 = (n & 3) ? 0 : n / 4;
   double s = 0.0, ss = 0.0;
   for (size_t i0 = (size_t)blockIdx.x * blockDim.x; i0 < n4; i0 += (size_t)gridDim.x * blockDim.x * 4) {
     float ls = 0.f, lss = 0.f;
@@ -117,8 +118,11 @@ __global__ void __launch_bounds__(256) k_sample_stats(const float* __restrict__ 
     }
     s += ls; ss += lss;
   }
-  if (blockIdx.x == 0)
-    for (size_t i = n4 * 4 + threadIdx.x; i < n; i += blockDim.x) { const float v = Y[(size_t)b * n + i]; s += v; ss += (double)v * v; }
+  for (size_t i = n4 * 4 + (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (size_t)gridDim.x * blockDim.x) {
+    const float v = Y[(size_t)b * n + i];
+    s += v;
+    ss += (double)v * v;
+  }
   block_sum2_d(s, ss, red);
   if (threadIdx.x == 0) { atomicAdd(&stats[2 * b], s); atomicAdd(&stats[2 * b + 1], ss); }
 }

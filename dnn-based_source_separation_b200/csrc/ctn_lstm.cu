@@ -287,9 +287,11 @@ __global__ void __launch_bounds__(256) k_norm_res2(const float* __restrict__ P0,
     }
   }
   if (absmax) {  // max|out|: the operand scale of the next path's LSTM (saves its own pass over the state)
-#pragma unroll
-    for (int o = 16; o > 0; o >>= 1) amax = fmaxf(amax, __shfl_xor_sync(0xffffffffu, amax, o));
-    if (((threadIdx.y * blockDim.x + threadIdx.x) & 31) == 0 && amax > 0.f) atomicMax(absmax, __float_as_uint(amax));
+    // (F/4) x TY need not be a multiple of 32 (F = 12, 48, 96, ...): the last warp is then partial and the reduction names only
+    // its existing lanes.  amax >= 0, so the float order is the order of its bit patterns.
+    const int tid = threadIdx.y * blockDim.x + threadIdx.x, left = blockDim.x * blockDim.y - (tid & ~31);
+    const unsigned m = __reduce_max_sync(left >= 32 ? 0xffffffffu : (1u << left) - 1u, __float_as_uint(amax));
+    if ((tid & 31) == 0 && m != 0u) atomicMax(absmax, m);
   }
 }
 
