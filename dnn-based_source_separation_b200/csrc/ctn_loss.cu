@@ -7,6 +7,7 @@
 // and a finalize kernel enumerates the permutations in itertools (lexicographic) order, takes the first minimum
 // and writes the int64 permutation.  Accumulation is fp32 per thread-chunk, double across threads.
 #include "ctn_common.cuh"
+#include "ctn_sisdr_grad.cuh"
 
 #define CTN_MAX_S 6
 
@@ -327,8 +328,7 @@ extern "C" int ctn_sdr_fwd(const float* est, const float* tgt, int rows, int T, 
 
 // ------------------------------------------------------------------------------------------------
 // backward of PIT(NegSISDR) through the SELECTED permutation (pit.py:36-44: the indices carry no gradient).
-//   SI-SDR = k (ln P - ln Q),  P = alpha^2 |t|^2 + eps,  Q = |alpha t - x|^2 + eps,  alpha = <x,t> / (|t|^2 + eps)
-//   dSI-SDR/dx = k { [2 alpha tt / ((tt+eps) P)] t  -  [ (2 (alpha tt - xt)/(tt+eps) - 2 alpha) t + 2 x ] / Q }
+// The per-pair coefficients (ct, cx) come from sisdr_grad_coef (ctn_sisdr_grad.cuh).
 // The pair statistics <x,t>, |alpha t - x|^2, |t|^2 are the ones the forward left in its scratch (explicit residual,
 // double), so the backward is one streaming pass.  grid (chunks, B*S), block 256.
 // ------------------------------------------------------------------------------------------------
@@ -340,12 +340,8 @@ __global__ void __launch_bounds__(256) k_sisdr_pit_bwd(const float* __restrict__
   const int j = (int)perm[(size_t)b * S + i];
   const double* sc = scratch + (size_t)b * pit_scratch_per_sample(S);
   const double xt = sc[i * S + j], den = sc[S * S + i * S + j], tt = sc[2 * S * S + j];
-  const double e = (double)eps;
-  const double alpha = xt / (tt + e), P = alpha * alpha * tt + e, Q = den + e;
-  const double k10 = 4.342944819032518;  // 10 / ln 10
-  const double g = (gl ? (double)gl[b] : 1.0) * (double)coef;
-  const float ct = (float)(g * k10 * (2.0 * alpha * tt / ((tt + e) * P) - (2.0 * (alpha * tt - xt) / (tt + e) - 2.0 * alpha) / Q));
-  const float cx = (float)(g * k10 * (-2.0 / Q));
+  float ct, cx;
+  sisdr_grad_coef(xt, den, tt, (double)eps, [&] { return (gl ? (double)gl[b] : 1.0) * (double)coef; }, ct, cx);
   const float* x = est + (size_t)row * T;
   const float* t = tgt + ((size_t)b * S + j) * T;
   float* d = d_est + (size_t)row * T;

@@ -85,6 +85,12 @@ ctn_encoder_mc_fwd = _sig("ctn_encoder_mc_fwd", _i, _fp, _fp, _fp, _i, _i, _i, _
 ctn_decoder_mc_fwd = _sig("ctn_decoder_mc_fwd", _i, _fp, _fp, _fp, _i, _i, _i, _i, _i, _i, _i, _i, _i, _fp)
 ctn_sdr_fwd = _sig("ctn_sdr_fwd", _i, _fp, _fp, _i, _i, _f, _fp, _fp, _fp)
 ctn_sisdr_pit_bwd = _sig("ctn_sisdr_pit_bwd", _i, _fp, _fp, _fp, _i, _i, _i, _f, _fp, _fp, _f, _fp, _fp)
+ctn_orpit_scratch_bytes = _sig("ctn_orpit_scratch_bytes", _sz, _i, _i)
+ctn_orpit_fwd = _sig("ctn_orpit_fwd", _i, _fp, _fp, _fp, _i, _i, _i, _f, _i, _fp, _fp, _fp, _fp)
+ctn_orpit_bwd = _sig("ctn_orpit_bwd", _i, _fp, _fp, _fp, _fp, _i, _i, _i, _f, _i, _fp, _fp, _fp, _fp)
+ctn_sinkpit_scratch_bytes = _sig("ctn_sinkpit_scratch_bytes", _sz, _i, _i, _i)
+ctn_sinkpit_fwd = _sig("ctn_sinkpit_fwd", _i, _fp, _fp, _i, _i, _i, _i, C.c_double, _f, _i, _fp, _fp, _fp, _fp, _fp)
+ctn_sinkpit_bwd = _sig("ctn_sinkpit_bwd", _i, _fp, _fp, _i, _i, _i, _i, C.c_double, _f, _i, _fp, _fp, _fp, _fp, _fp, _fp)
 ctn_last_launch_count = _sig("ctn_last_launch_count", _i)
 ctn_total_launch_count = _sig("ctn_total_launch_count", C.c_longlong)
 # DPRNN-TasNet path (cfg4) + separator stages on the pitched layout
@@ -117,6 +123,7 @@ EXPORTED = [
     "ctn_clip_adam_chunks", "ctn_clip_adam_step", "ctn_tcn_blocks_fwd",
     "ctn_depthwise_conv1d_fwd", "ctn_pointwise_conv1d_fwd",
     "ctn_bilstm_supported", "ctn_bilstm_workspace_bytes", "ctn_bilstm_proj_fwd", "ctn_dprnn_norm_res2_fwd",
+    "ctn_orpit_scratch_bytes", "ctn_orpit_fwd", "ctn_orpit_bwd", "ctn_sinkpit_scratch_bytes", "ctn_sinkpit_fwd", "ctn_sinkpit_bwd",
 ]
 
 

@@ -274,6 +274,32 @@ int ctn_convtasnet_bwd(const ctn_config_t* cfg, const ctn_params_t* params, cons
 int ctn_sisdr_pit_bwd(const float* est, const float* tgt, const int64_t* perm, int B, int S, int T, float eps,
                       const double* fwd_scratch, const float* grad_loss_b, float coef, float* d_est, ctn_stream_t stream);
 
+/* ORPIT(NegSISDR | SISDR), one-and-rest PIT, src/criterion/pit.py:87-160.  est (B,2,T), tgt (B,n,T) contiguous (any T, no
+ * alignment needed); n_b (B) int32 device array, nullable (= n for every sample): sample b uses targets 0..n_b[b]-1, each n_b in
+ * [2, n] (checked by the caller, the rows past n_b are ignored).  Candidate i scores
+ *   v_i = SI-SDR(est_0, tgt_i) + SI-SDR(est_1, sum_{j<n_b, j!=i} tgt_j) / (n_b - 1)
+ * loss_b (B) = -v (maximize = 0, NegSISDR) or v (maximize = 1, SISDR) at the first best candidate, indices (B) int64.
+ * scratch: ctn_orpit_scratch_bytes(B, n), 8-byte aligned; ctn_orpit_bwd reads what the forward left there.
+ * d_est (B,2,T) = grad_loss_b[b] (nullable: 1) * d loss_b / d est through the selected candidate.  n <= 16. */
+size_t ctn_orpit_scratch_bytes(int B, int n);
+int ctn_orpit_fwd(const float* est, const float* tgt, const int32_t* n_b, int B, int n, int T, float eps, int maximize,
+                  float* loss_b, int64_t* indices, void* scratch, ctn_stream_t stream);
+int ctn_orpit_bwd(const float* est, const float* tgt, const int32_t* n_b, const int64_t* indices, int B, int n, int T, float eps,
+                  int maximize, void* scratch, const float* grad_loss_b, float* d_est, ctn_stream_t stream);
+
+/* sinkpit(NegSISDR | SISDR), Sinkhorn PIT, src/criterion/pit.py:162-213.  est, tgt (B,S,T) contiguous (any T).
+ * L[b,i,j] = -SI-SDR(est_i, tgt_j); Z = -coldness L; K times: Z -= logsumexp(Z, dim=1), Z -= logsumexp(Z, dim=2);
+ * P (B,S,S) = exp(Z); loss_b (B) = sign * sum_ij (L + Z/coldness) P, sign = -1 when maximize (SISDR), else 1.
+ * pair_sisdr (nullable) (B,S,S) = SI-SDR(est_i, tgt_j).  Iterations run in double, one CTA per sample.
+ * scratch: ctn_sinkpit_scratch_bytes(B, S, K), 8-byte aligned, holds the pair statistics and every logsumexp for the backward.
+ * ctn_sinkpit_bwd: grad_loss_b (B) nullable (= 1), grad_P (B,S,S) nullable (= 0) -> dL (B,S,S) = d loss / d L through all K
+ * iterations (the unrolled gradient, not the converged P), and d_est (B,S,T).  S <= 16, K >= 0, coldness > 0. */
+size_t ctn_sinkpit_scratch_bytes(int B, int S, int K);
+int ctn_sinkpit_fwd(const float* est, const float* tgt, int B, int S, int T, int K, double coldness, float eps, int maximize,
+                    float* loss_b, float* P, float* pair_sisdr, void* scratch, ctn_stream_t stream);
+int ctn_sinkpit_bwd(const float* est, const float* tgt, int B, int S, int T, int K, double coldness, float eps, int maximize,
+                    void* scratch, const float* grad_loss_b, const float* grad_P, float* dL, float* d_est, ctn_stream_t stream);
+
 /* Training-step remainder, egs/wsj0-mix/common/src/driver.py:152-155 (clip_grad_norm_(max_norm) + Adam.step()), on the flat
  * gradient bucket of ctn_convtasnet_bwd: g *= min(1, max_norm/(||g||+1e-6)) (max_norm <= 0: no clipping), then torch.optim.Adam
  * arithmetic (amsgrad off).  params: device array of n_tensors parameter pointers; flat_off / numel: element offset of each
