@@ -585,16 +585,15 @@ extern "C" int ctn_convtasnet_fwd(const ctn_config_t* cfg, const ctn_params_t* p
   return CTN_OK;
 }
 
-// stats of an already-encoded w in padded layout
+// stats of an already-encoded w in padded layout.  w is the caller's tensor (stand-alone Separator.forward), so every element
+// is summed in double, as in k_gln_stats: fp32 partial sums put an error on var = E[w^2] - mean^2 that grows with a DC offset^2
 __global__ void __launch_bounds__(256) k_stats_pitch(const float* __restrict__ x, int C, int frames, int pitch, double* __restrict__ stats) {
   __shared__ double red[64];
   const int b = blockIdx.y;
   double s = 0.0, ss = 0.0;
   for (int c = blockIdx.x; c < C; c += gridDim.x) {
     const float* r = x + ((size_t)b * C + c) * pitch;
-    float ls = 0.f, lss = 0.f;
-    for (int t = threadIdx.x; t < frames; t += 256) { const float v = r[t]; ls += v; lss += v * v; }
-    s += ls; ss += lss;
+    for (int t = threadIdx.x; t < frames; t += 256) { const double v = r[t]; s += v; ss = fma(v, v, ss); }
   }
   block_sum2_d(s, ss, red);
   if (threadIdx.x == 0) { atomicAdd(&stats[2 * b], s); atomicAdd(&stats[2 * b + 1], ss); }

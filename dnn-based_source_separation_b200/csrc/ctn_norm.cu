@@ -4,22 +4,22 @@
 #include "ctn_common.cuh"
 
 // ---- gLN: GroupNorm(1,C,eps), src/modules/norm.py:18,32 -------------------------------------------------
+// Every element is summed in double: the square of an fp32 value is exact there, so var = E[x^2] - mean^2 keeps its digits
+// under a DC offset.  With fp32 partial sums the variance error grows with offset^2, and at |mean| / std ~ 1e3 the output
+// was 3x outside the fp32 forward-error bound.  The input here is user data, not a normalised activation.
 __global__ void __launch_bounds__(256) k_gln_stats(const float* __restrict__ x, size_t per_sample, double* __restrict__ stats) {
   __shared__ double red[64];
   const int b = blockIdx.y;
   const float* xb = x + (size_t)b * per_sample;
   double s = 0.0, ss = 0.0;
   for (size_t i0 = (size_t)blockIdx.x * 256 * 8; i0 < per_sample; i0 += (size_t)gridDim.x * 256 * 8) {
-    float ls = 0.f, lss = 0.f;
 #pragma unroll
     for (int j = 0; j < 8; ++j) {
       const size_t i = i0 + (size_t)j * 256 + threadIdx.x;
-      const float v = i < per_sample ? xb[i] : 0.f;
-      ls += v;
-      lss += v * v;
+      const double v = i < per_sample ? (double)xb[i] : 0.0;
+      s += v;
+      ss = fma(v, v, ss);
     }
-    s += ls;
-    ss += lss;
   }
   block_sum2_d(s, ss, red);
   if (threadIdx.x == 0) { atomicAdd(&stats[2 * b], s); atomicAdd(&stats[2 * b + 1], ss); }
