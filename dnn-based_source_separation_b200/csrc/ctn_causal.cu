@@ -167,3 +167,19 @@ int ctn_causal_tcn(const ctn_config_t* c, const ctn_block_params_t* blocks, floa
   }
   return CTN_OK;
 }
+
+// The per-frame kernels above, for the online (chunk-by-chunk) pipeline of ctn_online.cu: same kernels, same launch shape.
+int ctn_res_skip_fwd(const float* r, int Mt, float* x, float* skip, const float* bo, const float* bs, int Bc, int Sc, int has_out,
+                     int skip_init, int B, int frames, int pitch, cudaStream_t st) {
+  k_res_skip_inplace<<<grid_cb(Mt, B), 256, 0, st>>>(r, Mt, x, skip, bo, bs, Bc, Sc, has_out, skip_init, frames, pitch);
+  CTN_COUNT_LAUNCH();
+  CTN_RETURN_IF_CUDA_ERR();
+  return CTN_OK;
+}
+
+int ctn_bias_rows_fwd(float* y, const float* bias, int C, int B, int frames, int pitch, cudaStream_t st) {
+  k_bias_rows<<<grid_cb(C, B), 256, 0, st>>>(y, bias, C, frames, pitch);
+  CTN_COUNT_LAUNCH();
+  CTN_RETURN_IF_CUDA_ERR();
+  return CTN_OK;
+}

@@ -177,3 +177,8 @@ int ctn_causal_tcn(const ctn_config_t* c, const ctn_block_params_t* blocks, floa
 // separator head for causal models: x0 = Wb cLN0(w) + bb;  tmp: (B, N, pitch) scratch
 int ctn_causal_head(const ctn_config_t* c, const ctn_params_t* p, const float* w, float* tmp, float* x0, int B, int frames,
                     int pitch, void* cws, cudaStream_t st);
+// The causal pipeline's per-frame kernels on their own (ctn_online.cu):  rows of r (B, Mt, pitch): m < Bc (has_out): x += r + bo[m];
+// else skip (+)= r + bs[j] (skip_init: =);  and  y[b][c][t] += bias[c].  Columns [frames, pitch) are written as zero.
+int ctn_res_skip_fwd(const float* r, int Mt, float* x, float* skip, const float* bo, const float* bs, int Bc, int Sc, int has_out,
+                     int skip_init, int B, int frames, int pitch, cudaStream_t st);
+int ctn_bias_rows_fwd(float* y, const float* bias, int C, int B, int frames, int pitch, cudaStream_t st);

@@ -109,6 +109,11 @@ ctn_clip_adam_chunks = _sig("ctn_clip_adam_chunks", _i, C.POINTER(_i), _i, C.POI
 ctn_clip_adam_step = _sig("ctn_clip_adam_step", _i, _fp, _i, _fp, _fp, _fp, _i, _fp, _sz, _fp, _fp, _fp, _fp, _fp, _f, _f, _f, _f, _f, _fp, _fp)
 ctn_depthwise_conv1d_fwd = _sig("ctn_depthwise_conv1d_fwd", _i, _fp, _fp, _fp, _fp, _i, _i, _i, _i, _i, _i, _i, _i, _fp)
 ctn_pointwise_conv1d_fwd = _sig("ctn_pointwise_conv1d_fwd", _i, _fp, _fp, _fp, _fp, _i, _i, _i, _i, _i, _i, _fp, _sz, _fp)
+ctn_online_state_bytes = _sig("ctn_online_state_bytes", _i, C.POINTER(Config), _i, _i, C.POINTER(_sz))
+ctn_online_init = _sig("ctn_online_init", _i, C.POINTER(Config), C.POINTER(Params), _i, _i, _fp, _sz, _fp)
+ctn_online_reset = _sig("ctn_online_reset", _i, C.POINTER(Config), _fp, _i, _fp)
+ctn_online_push = _sig("ctn_online_push", _i, C.POINTER(Config), C.POINTER(Params), _fp, _fp, _i, _i, _i, _fp, _fp)
+ctn_online_flush = _sig("ctn_online_flush", _i, C.POINTER(Config), _fp, _i, _fp, _fp)
 ctn_profile_enable = _sig("ctn_profile_enable", _i, _i)
 ctn_profile_read = _sig("ctn_profile_read", _i, C.POINTER(C.c_double), C.POINTER(_i))
 STAGES = ("prep", "enc", "head", "pw1", "dw", "pw2", "fin", "mask", "dec", "loss")
@@ -124,6 +129,7 @@ EXPORTED = [
     "ctn_depthwise_conv1d_fwd", "ctn_pointwise_conv1d_fwd",
     "ctn_bilstm_supported", "ctn_bilstm_workspace_bytes", "ctn_bilstm_proj_fwd", "ctn_dprnn_norm_res2_fwd",
     "ctn_orpit_scratch_bytes", "ctn_orpit_fwd", "ctn_orpit_bwd", "ctn_sinkpit_scratch_bytes", "ctn_sinkpit_fwd", "ctn_sinkpit_bwd",
+    "ctn_online_state_bytes", "ctn_online_init", "ctn_online_reset", "ctn_online_push", "ctn_online_flush",
 ]
 
 

@@ -282,6 +282,12 @@ class ConvTasNet(nn.Module):
             setattr(model, key, value)
         return model
 
+    def online(self, batch_size=1, max_chunk=256):
+        """Online (chunk-by-chunk) separator of this causal model for ``batch_size`` concurrent streams, pushes of at most
+        ``max_chunk`` samples (a multiple of the stride): see ``ctn_b200.models.online.OnlineSeparator``."""
+        from .online import OnlineSeparator
+        return OnlineSeparator(self, batch_size, max_chunk)
+
     @property
     def num_parameters(self):
         return sum(p.numel() for p in self.parameters() if p.requires_grad)

@@ -163,6 +163,29 @@ int ctn_tcn_blocks_fwd(const ctn_config_t* cfg, const ctn_block_params_t* blocks
 int ctn_convtasnet_fwd(const ctn_config_t* cfg, const ctn_params_t* params, const float* x, int B, int T, float* out,
                        float* latent, void* workspace, size_t workspace_bytes, ctn_stream_t stream);
 
+/* ---- online (chunk-by-chunk) inference of the causal model ---------------------------------------------------
+ * B streams advance together; each push takes n new samples per stream and returns n samples per source, delayed by
+ * D = kernel_size - stride samples.  With x = everything pushed since the last init / reset (T samples), Y = the
+ * concatenated push outputs and Z = the flush output: Y[..., :D] == 0 and cat(Y[..., D:], Z) == ctn_convtasnet_fwd(x).
+ * Envelope: causal = 1, in_channels <= 1 (else CTN_EUNSUPPORTED); sigmoid or softmax mask; every math mode.
+ * `state`: one device buffer of ctn_online_state_bytes(cfg, B, max_chunk_frames) bytes, 256-byte aligned, owned by the
+ * caller.  It holds the carried state (sample counter, running cLN sums, the depthwise history of every block, the
+ * filter-bank carries), the weight images of every contraction (built by ctn_online_init, kept by ctn_online_reset) and
+ * the scratch of one chunk.  Pushes read the counters from the state on the device, so a captured push replays.
+ * ctn_online_init: builds the images from `params` and zeroes the carries.  The weights must not change afterwards.
+ * ctn_online_reset: back to zero history / statistics / samples (images kept).
+ * ctn_online_push: x (B,1,n) -> y (B,S,n), contiguous; n % stride == 0, 0 < n <= max_chunk_frames * stride.  A push
+ * computes the frames its samples complete; its launch sequence depends on cfg alone.
+ * ctn_online_flush: y_tail (B,S,D) = the last D samples of the offline output.  CTN_EINVAL when fewer than kernel_size
+ * samples were pushed since the reset; reads that count from the device (synchronises the stream once). */
+int ctn_online_state_bytes(const ctn_config_t* cfg, int B, int max_chunk_frames, size_t* bytes);
+int ctn_online_init(const ctn_config_t* cfg, const ctn_params_t* params, int B, int max_chunk_frames, void* state, size_t state_bytes,
+                    ctn_stream_t stream);
+int ctn_online_reset(const ctn_config_t* cfg, void* state, int B, ctn_stream_t stream);
+int ctn_online_push(const ctn_config_t* cfg, const ctn_params_t* params, void* state, const float* x, int B, int max_chunk_frames, int n,
+                    float* y, ctn_stream_t stream);
+int ctn_online_flush(const ctn_config_t* cfg, void* state, int B, float* y_tail, ctn_stream_t stream);
+
 /* Separator.forward, src/models/conv_tasnet.py:359-378: w (B,N,frames) -> mask (B,S,N,frames), both contiguous. */
 int ctn_separator_fwd(const ctn_config_t* cfg, const ctn_params_t* params, const float* w, int B, int frames,
                       float* mask, void* workspace, size_t workspace_bytes, ctn_stream_t stream);
