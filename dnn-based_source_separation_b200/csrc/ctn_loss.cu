@@ -14,115 +14,119 @@
 // scratch layout per sample b (doubles): dot[S*S], den[S*S], tt[S]
 __host__ __device__ inline size_t pit_scratch_per_sample(int S) { return (size_t)(2 * S * S + S); }
 
+// Samples are looped over gridDim.y (at most 65535); up to that many samples each CTA row owns exactly one sample.
 template <int S>
-__global__ void __launch_bounds__(256) k_pit_pass1(const float* __restrict__ est, const float* __restrict__ tgt, int T,
+__global__ void __launch_bounds__(256) k_pit_pass1(const float* __restrict__ est, const float* __restrict__ tgt, int B, int T,
                                                    double* __restrict__ scratch) {
   __shared__ double red[64];
-  const int b = blockIdx.y;
-  const float* eb = est + (size_t)b * S * T;
-  const float* tb = tgt + (size_t)b * S * T;
-  double dot[S][S], tt[S];
+  for (int b = blockIdx.y; b < B; b += gridDim.y) {
+    const float* eb = est + (size_t)b * S * T;
+    const float* tb = tgt + (size_t)b * S * T;
+    double dot[S][S], tt[S];
 #pragma unroll
-  for (int i = 0; i < S; ++i) { tt[i] = 0.0;
+    for (int i = 0; i < S; ++i) { tt[i] = 0.0;
 #pragma unroll
-    for (int j = 0; j < S; ++j) dot[i][j] = 0.0; }
-  const bool vec = (T % 4 == 0);
-  const int nvec = vec ? T / 4 : 0;
-  for (int v0 = blockIdx.x * 256 + threadIdx.x; v0 < nvec; v0 += gridDim.x * 256) {
-    float4 e[S], t[S];
+      for (int j = 0; j < S; ++j) dot[i][j] = 0.0; }
+    // 128-bit loads need every row 16-byte aligned: T % 4 == 0 and the sample's base (an offset view may start anywhere)
+    const bool vec = (T % 4 == 0) && ((((uintptr_t)eb) | ((uintptr_t)tb)) & 15) == 0;
+    const int nvec = vec ? T / 4 : 0;
+    for (int v0 = blockIdx.x * 256 + threadIdx.x; v0 < nvec; v0 += gridDim.x * 256) {
+      float4 e[S], t[S];
 #pragma unroll
-    for (int i = 0; i < S; ++i) {
-      e[i] = __ldg(reinterpret_cast<const float4*>(eb + (size_t)i * T) + v0);
-      t[i] = __ldg(reinterpret_cast<const float4*>(tb + (size_t)i * T) + v0);
-    }
-#pragma unroll
-    for (int j = 0; j < S; ++j) {
-      tt[j] += (double)((t[j].x * t[j].x + t[j].y * t[j].y) + (t[j].z * t[j].z + t[j].w * t[j].w));
-#pragma unroll
-      for (int i = 0; i < S; ++i)
-        dot[i][j] += (double)((e[i].x * t[j].x + e[i].y * t[j].y) + (e[i].z * t[j].z + e[i].w * t[j].w));
-    }
-  }
-  if (!vec) {
-    for (int k = blockIdx.x * 256 + threadIdx.x; k < T; k += gridDim.x * 256) {
-      float e[S], t[S];
-#pragma unroll
-      for (int i = 0; i < S; ++i) { e[i] = eb[(size_t)i * T + k]; t[i] = tb[(size_t)i * T + k]; }
+      for (int i = 0; i < S; ++i) {
+        e[i] = __ldg(reinterpret_cast<const float4*>(eb + (size_t)i * T) + v0);
+        t[i] = __ldg(reinterpret_cast<const float4*>(tb + (size_t)i * T) + v0);
+      }
 #pragma unroll
       for (int j = 0; j < S; ++j) {
-        tt[j] += (double)(t[j] * t[j]);
+        tt[j] += (double)((t[j].x * t[j].x + t[j].y * t[j].y) + (t[j].z * t[j].z + t[j].w * t[j].w));
 #pragma unroll
-        for (int i = 0; i < S; ++i) dot[i][j] += (double)(e[i] * t[j]);
+        for (int i = 0; i < S; ++i)
+          dot[i][j] += (double)((e[i].x * t[j].x + e[i].y * t[j].y) + (e[i].z * t[j].z + e[i].w * t[j].w));
       }
     }
-  }
-  double* sc = scratch + (size_t)b * pit_scratch_per_sample(S);
+    if (!vec) {
+      for (int k = blockIdx.x * 256 + threadIdx.x; k < T; k += gridDim.x * 256) {
+        float e[S], t[S];
 #pragma unroll
-  for (int j = 0; j < S; ++j) {
+        for (int i = 0; i < S; ++i) { e[i] = eb[(size_t)i * T + k]; t[i] = tb[(size_t)i * T + k]; }
 #pragma unroll
-    for (int i = 0; i < S; i += 2) {
-      double a = dot[i][j], c = (i + 1 < S) ? dot[i + 1][j] : 0.0;
+        for (int j = 0; j < S; ++j) {
+          tt[j] += (double)(t[j] * t[j]);
+#pragma unroll
+          for (int i = 0; i < S; ++i) dot[i][j] += (double)(e[i] * t[j]);
+        }
+      }
+    }
+    double* sc = scratch + (size_t)b * pit_scratch_per_sample(S);
+#pragma unroll
+    for (int j = 0; j < S; ++j) {
+#pragma unroll
+      for (int i = 0; i < S; i += 2) {
+        double a = dot[i][j], c = (i + 1 < S) ? dot[i + 1][j] : 0.0;
+        block_sum2_d(a, c, red);
+        if (threadIdx.x == 0) {
+          atomicAdd(&sc[i * S + j], a);
+          if (i + 1 < S) atomicAdd(&sc[(i + 1) * S + j], c);
+        }
+        __syncthreads();
+      }
+    }
+#pragma unroll
+    for (int j = 0; j < S; j += 2) {
+      double a = tt[j], c = (j + 1 < S) ? tt[j + 1] : 0.0;
       block_sum2_d(a, c, red);
       if (threadIdx.x == 0) {
-        atomicAdd(&sc[i * S + j], a);
-        if (i + 1 < S) atomicAdd(&sc[(i + 1) * S + j], c);
+        atomicAdd(&sc[2 * S * S + j], a);
+        if (j + 1 < S) atomicAdd(&sc[2 * S * S + j + 1], c);
       }
       __syncthreads();
     }
-  }
-#pragma unroll
-  for (int j = 0; j < S; j += 2) {
-    double a = tt[j], c = (j + 1 < S) ? tt[j + 1] : 0.0;
-    block_sum2_d(a, c, red);
-    if (threadIdx.x == 0) {
-      atomicAdd(&sc[2 * S * S + j], a);
-      if (j + 1 < S) atomicAdd(&sc[2 * S * S + j + 1], c);
-    }
-    __syncthreads();
   }
 }
 
 template <int S>
-__global__ void __launch_bounds__(256) k_pit_pass2(const float* __restrict__ est, const float* __restrict__ tgt, int T,
+__global__ void __launch_bounds__(256) k_pit_pass2(const float* __restrict__ est, const float* __restrict__ tgt, int B, int T,
                                                    float eps, double* __restrict__ scratch) {
   __shared__ double red[64];
-  const int b = blockIdx.y;
-  const float* eb = est + (size_t)b * S * T;
-  const float* tb = tgt + (size_t)b * S * T;
-  double* sc = scratch + (size_t)b * pit_scratch_per_sample(S);
-  float alpha[S][S];
-#pragma unroll
-  for (int i = 0; i < S; ++i)
-#pragma unroll
-    for (int j = 0; j < S; ++j) alpha[i][j] = (float)sc[i * S + j] / ((float)sc[2 * S * S + j] + eps);  // sdr.py:135
-  double den[S][S];
-#pragma unroll
-  for (int i = 0; i < S; ++i)
-#pragma unroll
-    for (int j = 0; j < S; ++j) den[i][j] = 0.0;
-  for (int k = blockIdx.x * 256 + threadIdx.x; k < T; k += gridDim.x * 256) {
-    float e[S], t[S];
-#pragma unroll
-    for (int i = 0; i < S; ++i) { e[i] = __ldg(eb + (size_t)i * T + k); t[i] = __ldg(tb + (size_t)i * T + k); }
+  for (int b = blockIdx.y; b < B; b += gridDim.y) {
+    const float* eb = est + (size_t)b * S * T;
+    const float* tb = tgt + (size_t)b * S * T;
+    double* sc = scratch + (size_t)b * pit_scratch_per_sample(S);
+    float alpha[S][S];
 #pragma unroll
     for (int i = 0; i < S; ++i)
 #pragma unroll
-      for (int j = 0; j < S; ++j) {
-        const float d = alpha[i][j] * t[j] - e[i];  // sdr.py:136 (alpha*target - input)
-        den[i][j] += (double)(d * d);
-      }
-  }
+      for (int j = 0; j < S; ++j) alpha[i][j] = (float)sc[i * S + j] / ((float)sc[2 * S * S + j] + eps);  // sdr.py:135
+    double den[S][S];
 #pragma unroll
-  for (int i = 0; i < S; ++i) {
+    for (int i = 0; i < S; ++i)
 #pragma unroll
-    for (int j = 0; j < S; j += 2) {
-      double a = den[i][j], c = (j + 1 < S) ? den[i][j + 1] : 0.0;
-      block_sum2_d(a, c, red);
-      if (threadIdx.x == 0) {
-        atomicAdd(&sc[S * S + i * S + j], a);
-        if (j + 1 < S) atomicAdd(&sc[S * S + i * S + j + 1], c);
+      for (int j = 0; j < S; ++j) den[i][j] = 0.0;
+    for (int k = blockIdx.x * 256 + threadIdx.x; k < T; k += gridDim.x * 256) {
+      float e[S], t[S];
+#pragma unroll
+      for (int i = 0; i < S; ++i) { e[i] = __ldg(eb + (size_t)i * T + k); t[i] = __ldg(tb + (size_t)i * T + k); }
+#pragma unroll
+      for (int i = 0; i < S; ++i)
+#pragma unroll
+        for (int j = 0; j < S; ++j) {
+          const float d = alpha[i][j] * t[j] - e[i];  // sdr.py:136 (alpha*target - input)
+          den[i][j] += (double)(d * d);
+        }
+    }
+#pragma unroll
+    for (int i = 0; i < S; ++i) {
+#pragma unroll
+      for (int j = 0; j < S; j += 2) {
+        double a = den[i][j], c = (j + 1 < S) ? den[i][j + 1] : 0.0;
+        block_sum2_d(a, c, red);
+        if (threadIdx.x == 0) {
+          atomicAdd(&sc[S * S + i * S + j], a);
+          if (j + 1 < S) atomicAdd(&sc[S * S + i * S + j + 1], c);
+        }
+        __syncthreads();
       }
-      __syncthreads();
     }
   }
 }
@@ -197,17 +201,20 @@ __global__ void k_batch_mean(const float* __restrict__ loss_b, int B, float* __r
   if (threadIdx.x == 0) out[0] = (float)(s / (double)B);
 }
 
+// gridDim.y is at most 65535; the kernels loop over the rest of the rows
+static unsigned grid_rows(int rows) { return rows < 65535 ? (unsigned)rows : 65535u; }
+
 template <int S>
 static int launch_pit(const float* est, const float* tgt, int B, int T, float eps, double* scratch, cudaStream_t st) {
   int gx = (T / 4 + 255) / 256;
   if (gx < 1) gx = 1;
   if (gx > 32) gx = 32;
-  k_pit_pass1<S><<<dim3(gx, B), 256, 0, st>>>(est, tgt, T, scratch);
+  k_pit_pass1<S><<<dim3(gx, grid_rows(B)), 256, 0, st>>>(est, tgt, B, T, scratch);
   CTN_COUNT_LAUNCH();
   CTN_RETURN_IF_CUDA_ERR();
   int gx2 = (T + 255) / 256;
   if (gx2 > 64) gx2 = 64;
-  k_pit_pass2<S><<<dim3(gx2, B), 256, 0, st>>>(est, tgt, T, eps, scratch);
+  k_pit_pass2<S><<<dim3(gx2, grid_rows(B)), 256, 0, st>>>(est, tgt, B, T, eps, scratch);
   CTN_COUNT_LAUNCH();
   CTN_RETURN_IF_CUDA_ERR();
   return CTN_OK;
@@ -221,7 +228,6 @@ extern "C" int ctn_sisdr_pit_fwd(const float* est, const float* tgt, int B, int 
   LaunchScope scope(est);
   if (!est || !tgt || !loss_b || !perm || !scratch || B <= 0 || T <= 0) return CTN_EINVAL;
   if (S < 1 || S > CTN_MAX_S) return CTN_EUNSUPPORTED;
-  if ((((uintptr_t)est) | ((uintptr_t)tgt)) & 15) return CTN_EALIGN;
   cudaStream_t st = (cudaStream_t)stream;
   StageTimer tm(CTN_ST_LOSS, st);
   cudaError_t e = cudaMemsetAsync(scratch, 0, ctn_sisdr_pit_scratch_bytes(B, S), st);
@@ -265,7 +271,6 @@ extern "C" int ctn_sisdr_fwd(const float* est, const float* tgt, int rows, int T
                              ctn_stream_t stream) {
   LaunchScope scope(est);
   if (!est || !tgt || !out || !scratch || rows <= 0 || T <= 0) return CTN_EINVAL;
-  if (((((uintptr_t)est) | ((uintptr_t)tgt)) & 15) || (T % 4 != 0 && 0)) return CTN_EALIGN;
   cudaStream_t st = (cudaStream_t)stream;
   cudaError_t e = cudaMemsetAsync(scratch, 0, ctn_sisdr_pit_scratch_bytes(rows, 1), st);
   if (e != cudaSuccess) return (int)e;
@@ -280,28 +285,30 @@ extern "C" int ctn_sisdr_fwd(const float* est, const float* tgt, int rows, int T
 
 // ---- plain SDR (src/criterion/sdr.py:6-20): 10 log10((|t|^2 + eps) / (|t - x|^2 + eps)) per row -------------------------
 // The residual is accumulated explicitly (not as |t|^2 - 2<x,t> + |x|^2, which cancels catastrophically at high SDR), in double.
-__global__ void __launch_bounds__(256) k_sdr_partial(const float* __restrict__ est, const float* __restrict__ tgt, int T,
+__global__ void __launch_bounds__(256) k_sdr_partial(const float* __restrict__ est, const float* __restrict__ tgt, int rows, int T,
                                                      double* __restrict__ scratch) {
   __shared__ double red[64];
-  const int r = blockIdx.y;
-  const float* x = est + (size_t)r * T;
-  const float* t = tgt + (size_t)r * T;
-  double tt = 0.0, ee = 0.0;
-  const bool vec = ((((uintptr_t)x) | ((uintptr_t)t)) & 15) == 0;
-  const int n4 = vec ? T / 4 : 0;
-  for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n4; i += gridDim.x * blockDim.x) {
-    const float4 a = __ldg(reinterpret_cast<const float4*>(x) + i), b = __ldg(reinterpret_cast<const float4*>(t) + i);
-    const float d0 = b.x - a.x, d1 = b.y - a.y, d2 = b.z - a.z, d3 = b.w - a.w;
-    tt += (double)(fmaf(b.x, b.x, b.y * b.y) + fmaf(b.z, b.z, b.w * b.w));
-    ee += (double)(fmaf(d0, d0, d1 * d1) + fmaf(d2, d2, d3 * d3));
+  for (int r = blockIdx.y; r < rows; r += gridDim.y) {
+    const float* x = est + (size_t)r * T;
+    const float* t = tgt + (size_t)r * T;
+    double tt = 0.0, ee = 0.0;
+    const bool vec = ((((uintptr_t)x) | ((uintptr_t)t)) & 15) == 0;
+    const int n4 = vec ? T / 4 : 0;
+    for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n4; i += gridDim.x * blockDim.x) {
+      const float4 a = __ldg(reinterpret_cast<const float4*>(x) + i), b = __ldg(reinterpret_cast<const float4*>(t) + i);
+      const float d0 = b.x - a.x, d1 = b.y - a.y, d2 = b.z - a.z, d3 = b.w - a.w;
+      tt += (double)(fmaf(b.x, b.x, b.y * b.y) + fmaf(b.z, b.z, b.w * b.w));
+      ee += (double)(fmaf(d0, d0, d1 * d1) + fmaf(d2, d2, d3 * d3));
+    }
+    for (int i = n4 * 4 + blockIdx.x * blockDim.x + threadIdx.x; i < T; i += gridDim.x * blockDim.x) {
+      const float b = t[i], d = b - x[i];
+      tt += (double)b * b;
+      ee += (double)d * d;
+    }
+    block_sum2_d(tt, ee, red);
+    if (threadIdx.x == 0) { atomicAdd(&scratch[2 * r], tt); atomicAdd(&scratch[2 * r + 1], ee); }
+    if (r + gridDim.y < rows) __syncthreads();  // red is reused by the next row
   }
-  for (int i = n4 * 4 + blockIdx.x * blockDim.x + threadIdx.x; i < T; i += gridDim.x * blockDim.x) {
-    const float b = t[i], d = b - x[i];
-    tt += (double)b * b;
-    ee += (double)d * d;
-  }
-  block_sum2_d(tt, ee, red);
-  if (threadIdx.x == 0) { atomicAdd(&scratch[2 * r], tt); atomicAdd(&scratch[2 * r + 1], ee); }
 }
 __global__ void k_sdr_finalize(const double* __restrict__ scratch, int rows, float eps, float* __restrict__ out) {
   const int r = blockIdx.x * 128 + threadIdx.x;
@@ -311,14 +318,14 @@ __global__ void k_sdr_finalize(const double* __restrict__ scratch, int rows, flo
 
 extern "C" int ctn_sdr_fwd(const float* est, const float* tgt, int rows, int T, float eps, float* out, double* scratch, ctn_stream_t stream) {
   LaunchScope scope(est);
-  if (!est || !tgt || !out || !scratch || rows <= 0 || T <= 0 || rows > 65535) return CTN_EINVAL;
+  if (!est || !tgt || !out || !scratch || rows <= 0 || T <= 0) return CTN_EINVAL;
   cudaStream_t st = (cudaStream_t)stream;
   cudaError_t e = cudaMemsetAsync(scratch, 0, sizeof(double) * 2 * rows, st);
   if (e != cudaSuccess) return (int)e;
   int gx = (T / 4 + 1023) / 1024;
   if (gx < 1) gx = 1;
   if (gx > 64) gx = 64;
-  k_sdr_partial<<<dim3(gx, rows), 256, 0, st>>>(est, tgt, T, scratch);
+  k_sdr_partial<<<dim3(gx, grid_rows(rows)), 256, 0, st>>>(est, tgt, rows, T, scratch);
   CTN_COUNT_LAUNCH();
   k_sdr_finalize<<<(rows + 127) / 128, 128, 0, st>>>(scratch, rows, eps, out);
   CTN_COUNT_LAUNCH();
@@ -330,22 +337,25 @@ extern "C" int ctn_sdr_fwd(const float* est, const float* tgt, int rows, int T, 
 // backward of PIT(NegSISDR) through the SELECTED permutation (pit.py:36-44: the indices carry no gradient).
 // The per-pair coefficients (ct, cx) come from sisdr_grad_coef (ctn_sisdr_grad.cuh).
 // The pair statistics <x,t>, |alpha t - x|^2, |t|^2 are the ones the forward left in its scratch (explicit residual,
-// double), so the backward is one streaming pass.  grid (chunks, B*S), block 256.
+// double), so the backward is one streaming pass.  grid (chunks, min(B*S, 65535)), block 256.
 // ------------------------------------------------------------------------------------------------
-__global__ void __launch_bounds__(256) k_sisdr_pit_bwd(const float* __restrict__ est, const float* __restrict__ tgt,
-                                                       const int64_t* __restrict__ perm, const double* __restrict__ scratch,
-                                                       const float* __restrict__ gl, float coef, int S, int T, float eps,
-                                                       float* __restrict__ d_est) {
-  const int row = blockIdx.y, b = row / S, i = row % S;
-  const int j = (int)perm[(size_t)b * S + i];
-  const double* sc = scratch + (size_t)b * pit_scratch_per_sample(S);
-  const double xt = sc[i * S + j], den = sc[S * S + i * S + j], tt = sc[2 * S * S + j];
-  float ct, cx;
-  sisdr_grad_coef(xt, den, tt, (double)eps, [&] { return (gl ? (double)gl[b] : 1.0) * (double)coef; }, ct, cx);
-  const float* x = est + (size_t)row * T;
-  const float* t = tgt + ((size_t)b * S + j) * T;
-  float* d = d_est + (size_t)row * T;
-  for (int k = blockIdx.x * 256 + threadIdx.x; k < T; k += gridDim.x * 256) d[k] = fmaf(ct, t[k], cx * x[k]);
+// Bounded to six CTAs per SM (40 registers): the compiler versions the row loop on `gl`, which otherwise takes 48 (five CTAs).
+__global__ void __launch_bounds__(256, 6) k_sisdr_pit_bwd(const float* __restrict__ est, const float* __restrict__ tgt,
+                                                          const int64_t* __restrict__ perm, const double* __restrict__ scratch,
+                                                          const float* __restrict__ gl, float coef, int B, int S, int T,
+                                                          float eps, float* __restrict__ d_est) {
+  for (int row = blockIdx.y; row < B * S; row += gridDim.y) {
+    const int b = row / S, i = row % S;
+    const int j = (int)perm[(size_t)b * S + i];
+    const double* sc = scratch + (size_t)b * pit_scratch_per_sample(S);
+    const double xt = sc[i * S + j], den = sc[S * S + i * S + j], tt = sc[2 * S * S + j];
+    float ct, cx;
+    sisdr_grad_coef(xt, den, tt, (double)eps, [&] { return (gl ? (double)gl[b] : 1.0) * (double)coef; }, ct, cx);
+    const float* x = est + (size_t)row * T;
+    const float* t = tgt + ((size_t)b * S + j) * T;
+    float* d = d_est + (size_t)row * T;
+    for (int k = blockIdx.x * 256 + threadIdx.x; k < T; k += gridDim.x * 256) d[k] = fmaf(ct, t[k], cx * x[k]);
+  }
 }
 
 extern "C" int ctn_sisdr_pit_bwd(const float* est, const float* tgt, const int64_t* perm, int B, int S, int T, float eps,
@@ -356,7 +366,8 @@ extern "C" int ctn_sisdr_pit_bwd(const float* est, const float* tgt, const int64
   if (S < 1 || S > CTN_MAX_S) return CTN_EUNSUPPORTED;
   int gx = (T + 1023) / 1024;
   if (gx > 64) gx = 64;
-  k_sisdr_pit_bwd<<<dim3(gx, B * S), 256, 0, (cudaStream_t)stream>>>(est, tgt, perm, fwd_scratch, grad_loss_b, coef, S, T, eps, d_est);
+  k_sisdr_pit_bwd<<<dim3(gx, grid_rows(B * S)), 256, 0, (cudaStream_t)stream>>>(est, tgt, perm, fwd_scratch, grad_loss_b, coef, B, S, T,
+                                                                                 eps, d_est);
   CTN_COUNT_LAUNCH();
   CTN_RETURN_IF_CUDA_ERR();
   return CTN_OK;

@@ -10,23 +10,31 @@
 
 namespace {
 
-__global__ void __launch_bounds__(256) k_sumsq(const float* __restrict__ g, size_t n, double* __restrict__ out) {
+// chunk table entry: tensor index and element offset inside the tensor; one block per chunk of CHUNK elements
+constexpr int CHUNK = 2048;
+
+// Sum of squares over the chunks of the table, i.e. over exactly the tensors k_clip_adam updates: a frozen tensor or padding that
+// shares the bucket stays out of the norm, as its .grad stays out of torch.nn.utils.clip_grad_norm_.  One block per chunk, its
+// CHUNK / 256 loads per thread issued together; scalar loads, because the tensors' offsets are arbitrary; squares exact in double.
+__global__ void __launch_bounds__(256) k_sumsq(const int2* __restrict__ chunks, const long long* __restrict__ flat_off,
+                                               const int* __restrict__ numel, const float* __restrict__ g, double* __restrict__ out) {
   __shared__ double red[64];
-  double s = 0.0, dummy = 0.0;
-  const size_t n4 = n / 4;
-  const float4* g4 = reinterpret_cast<const float4*>(g);
-  for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < n4; i += (size_t)gridDim.x * blockDim.x) {
-    const float4 v = __ldg(g4 + i);
-    s += (double)(v.x * v.x + v.y * v.y) + (double)(v.z * v.z + v.w * v.w);
+  const int2 ch = chunks[blockIdx.x];
+  const float* gt = g + flat_off[ch.x] + ch.y;
+  const int len = numel[ch.x] - ch.y < CHUNK ? numel[ch.x] - ch.y : CHUNK;
+  float v[CHUNK / 256];
+#pragma unroll
+  for (int k = 0; k < CHUNK / 256; ++k) {
+    const int e = threadIdx.x + 256 * k;
+    v[k] = e < len ? gt[e] : 0.f;
   }
-  if (blockIdx.x == 0)
-    for (size_t i = n4 * 4 + threadIdx.x; i < n; i += blockDim.x) s += (double)g[i] * g[i];
+  double s = 0.0, dummy = 0.0;
+#pragma unroll
+  for (int k = 0; k < CHUNK / 256; ++k) s += (double)v[k] * v[k];
   block_sum2_d(s, dummy, red);
   if (threadIdx.x == 0) atomicAdd(out, s);
 }
 
-// chunk table entry: tensor index and element offset inside the tensor; one block per chunk of CHUNK elements
-constexpr int CHUNK = 2048;
 __global__ void __launch_bounds__(256) k_clip_adam(const int2* __restrict__ chunks, float* const* __restrict__ params,
                                                    const long long* __restrict__ flat_off, const int* __restrict__ numel,
                                                    const float* __restrict__ flat_grad, float* __restrict__ exp_avg,
@@ -85,15 +93,13 @@ extern "C" int ctn_clip_adam_step(const int32_t* chunk_table, int n_chunks, floa
   if (!chunk_table || n_chunks <= 0 || !params || !flat_off || !numel || n_tensors <= 0 || !flat_grad || !exp_avg || !exp_avg_sq ||
       !sumsq_scratch || !lr || !step)
     return CTN_EINVAL;
-  if (((uintptr_t)flat_grad) & 15) return CTN_EALIGN;
   cudaStream_t st = (cudaStream_t)stream;
   cudaError_t e = cudaMemsetAsync(sumsq_scratch, 0, sizeof(double), st);
   if (e != cudaSuccess) return (int)e;
-  // padding between the tensors of the bucket is zero (the backward starts from a zero-filled buffer), so the norm of the
-  // whole buffer is the norm of the gradients
-  k_sumsq<<<592, 256, 0, st>>>(flat_grad, flat_numel, sumsq_scratch);
+  const int2* chunks = reinterpret_cast<const int2*>(chunk_table);
+  k_sumsq<<<n_chunks, 256, 0, st>>>(chunks, flat_off, numel, flat_grad, sumsq_scratch);
   CTN_COUNT_LAUNCH();
-  k_clip_adam<<<n_chunks, 256, 0, st>>>(reinterpret_cast<const int2*>(chunk_table), params, flat_off, numel, flat_grad, exp_avg, exp_avg_sq,
+  k_clip_adam<<<n_chunks, 256, 0, st>>>(chunks, params, flat_off, numel, flat_grad, exp_avg, exp_avg_sq,
                                         sumsq_scratch, lr, step, beta1, beta2, eps, weight_decay, max_norm, norm_out);
   CTN_COUNT_LAUNCH();
   k_step_advance<<<1, 1, 0, st>>>(step);

@@ -249,18 +249,20 @@ int ctn_depthwise_conv1d_fwd(const float* x, const float* w, const float* bias, 
 int ctn_pointwise_conv1d_fwd(const float* x, const float* W, const float* bias, float* y, int B, int M, int K, int frames, int pitch,
                              int math, void* workspace, size_t workspace_bytes, ctn_stream_t stream);
 
-/* sisdr, src/criterion/sdr.py:122-139: est,tgt (rows,T) contiguous -> out (rows). scratch double[rows][4]. */
+/* sisdr, src/criterion/sdr.py:122-139: est,tgt (rows,T) contiguous -> out (rows). scratch double[rows][4].  Any row count and
+ * any 4-byte-aligned base: 128-bit loads are used only where T % 4 == 0 and both bases are 16-byte aligned. */
 int ctn_sisdr_fwd(const float* est, const float* tgt, int rows, int T, float eps, float* out, double* scratch,
                   ctn_stream_t stream);
 /* sdr(), src/criterion/sdr.py:6-20: out[r] = 10 log10((|tgt_r|^2 + eps) / (|tgt_r - est_r|^2 + eps)); est, tgt (rows,T) contiguous;
- * scratch: double[rows][2]. */
+ * any row count; scratch: double[rows][2]. */
 int ctn_sdr_fwd(const float* est, const float* tgt, int rows, int T, float eps, float* out, double* scratch, ctn_stream_t stream);
 
 /* PIT1d(NegSISDR(reduction='mean')), src/criterion/pit.py:9-44,71-77 + src/criterion/sdr.py:198-227.
  * est,tgt (B,S,T) contiguous.  loss_b (B) = min over permutations of -mean_i SI-SDR(est_i, tgt_perm[i]);
  * perm (B,S) int64, estimate i <-> target perm[i] (first minimum on ties, lexicographic permutation order);
  * loss_mean (1) = mean over the batch.  pair_sisdr (nullable) (B,S,S) = SI-SDR(est_i, tgt_j).
- * scratch: double[B][S*S*2 + S], zero-initialised by the callee.  S <= 6. */
+ * scratch: double[B][S*S*2 + S], zero-initialised by the callee.  S <= 6, any B.  est/tgt need no alignment beyond float's:
+ * 128-bit loads are used only for samples whose rows are all 16-byte aligned (T % 4 == 0 and aligned sample bases). */
 int ctn_sisdr_pit_fwd(const float* est, const float* tgt, int B, int S, int T, float eps, float* loss_b,
                       int64_t* perm, float* loss_mean, float* pair_sisdr, double* scratch, ctn_stream_t stream);
 size_t ctn_sisdr_pit_scratch_bytes(int B, int S);
@@ -328,7 +330,9 @@ int ctn_sinkpit_bwd(const float* est, const float* tgt, int B, int S, int T, int
  * arithmetic (amsgrad off).  params: device array of n_tensors parameter pointers; flat_off / numel: element offset of each
  * tensor's gradient inside flat_grad / its size; exp_avg, exp_avg_sq: Adam state laid out like flat_grad; lr (float) and step
  * (int64, advanced by one) are DEVICE scalars (graph-replayable); chunk_table: int32 pairs (tensor, offset) from
- * ctn_clip_adam_chunks (host helper: returns the chunk count; pass null outputs to size the table); norm_out nullable (1). */
+ * ctn_clip_adam_chunks (host helper: returns the chunk count; pass null outputs to size the table); norm_out nullable (1).
+ * ||g|| is the norm over the listed tensors only, so flat_grad may hold other values between or around them (padding, the
+ * gradients of frozen tensors); flat_numel is not read. */
 int ctn_clip_adam_chunks(const int* numel, int n_tensors, int* chunk_tensor, int* chunk_offset, int capacity);
 int ctn_clip_adam_step(const int32_t* chunk_table, int n_chunks, float* const* params, const long long* flat_off,
                        const int32_t* numel, int n_tensors, const float* flat_grad, size_t flat_numel, float* exp_avg,
