@@ -36,76 +36,79 @@ __device__ __forceinline__ double pitx_sisdr(const double* st, int P, int p, int
 }
 
 // est (B, ne, T), tgt (B, nt, T), n_b (B) nullable: targets in use per sample (ORPIT; the rest of the rows are padding).
-// grid (chunks, B), block 256.  PASS 1 accumulates dot and tt, PASS 2 den (needs the completed pass-1 sums).
+// grid (chunks, min(B, 65535)), block 256; samples loop over gridDim.y, so up to 65535 samples each CTA row owns one sample.
+// PASS 1 accumulates dot and tt, PASS 2 den (needs the completed pass-1 sums).  Bounded to 6 CTAs per SM: 40 registers.
 template <int PASS>
-__global__ void __launch_bounds__(256) k_pitx_stats(const float* __restrict__ est, const float* __restrict__ tgt,
-                                                    const int* __restrict__ n_b, int ne, int nt, int orpit, int T, float eps,
-                                                    double* __restrict__ stats) {
+__global__ void __launch_bounds__(256, 6) k_pitx_stats(const float* __restrict__ est, const float* __restrict__ tgt,
+                                                       const int* __restrict__ n_b, int B, int ne, int nt, int orpit, int T,
+                                                       float eps, double* __restrict__ stats) {
   __shared__ float sh[PITX_ROWS * PITX_CP];
-  const int b = blockIdx.y, tid = threadIdx.x;
-  const int nb = n_b ? n_b[b] : nt;
+  const int tid = threadIdx.x;
   const int P = pitx_pairs(ne, nt);
-  double* st = stats + (size_t)b * pitx_stats_per_sample(ne, nt, orpit);
   int KS = 32;  // threads per pair (consecutive lanes of one warp)
   while (KS > 1 && KS * P > 256) KS >>= 1;
   const int p = tid / KS, ks = tid % KS;
-  const bool act = p < P && (p % nt) < nb;
-  const int er = act ? p / nt : 0, vr = act ? (orpit ? p : p % nt) : 0;
-  const bool own_tt = act && (orpit || p < nt);
-  const float* xe = sh + er * PITX_CP;
-  const float* xv = sh + (ne + vr) * PITX_CP;
-  float alpha = 0.f;
-  if (PASS == 2 && act) alpha = (float)st[p] / ((float)st[2 * P + vr] + eps);  // sdr.py:135, as k_pit_pass2
-  double acc0 = 0.0, acc1 = 0.0;
   const int nrow = ne + nt;
-  for (int k0 = blockIdx.x * PITX_C; k0 < T; k0 += gridDim.x * PITX_C) {
-    __syncthreads();
-#pragma unroll 4
-    for (int idx = tid; idx < nrow * PITX_C; idx += 256) {
-      const int r = idx / PITX_C, k = idx % PITX_C, kk = k0 + k;
-      const float* row = r < ne ? est + ((size_t)b * ne + r) * T : tgt + ((size_t)b * nt + (r - ne)) * T;
-      sh[r * PITX_CP + k] = kk < T ? __ldg(row + kk) : 0.f;
-    }
-    if (orpit) {  // rests in the reference's order: sum over j of mask_rest * target (pit.py:135-138)
+  for (int b = blockIdx.y; b < B; b += gridDim.y) {
+    const int nb = n_b ? n_b[b] : nt;
+    double* st = stats + (size_t)b * pitx_stats_per_sample(ne, nt, orpit);
+    const bool act = p < P && (p % nt) < nb;
+    const int er = act ? p / nt : 0, vr = act ? (orpit ? p : p % nt) : 0;
+    const bool own_tt = act && (orpit || p < nt);
+    const float* xe = sh + er * PITX_CP;
+    const float* xv = sh + (ne + vr) * PITX_CP;
+    float alpha = 0.f;
+    if (PASS == 2 && act) alpha = (float)st[p] / ((float)st[2 * P + vr] + eps);  // sdr.py:135, as k_pit_pass2
+    double acc0 = 0.0, acc1 = 0.0;
+    for (int k0 = blockIdx.x * PITX_C; k0 < T; k0 += gridDim.x * PITX_C) {
       __syncthreads();
-      for (int idx = tid; idx < nb * PITX_C; idx += 256) {
-        const int i = idx / PITX_C, k = idx % PITX_C;
-        float r = 0.f;
-        for (int j = 0; j < nb; ++j)
-          if (j != i) r += sh[(ne + j) * PITX_CP + k];
-        sh[(ne + nt + i) * PITX_CP + k] = r;
-      }
-    }
-    __syncthreads();
-    if (act) {
-      float f0 = 0.f, f1 = 0.f;
-      int m = 0;
 #pragma unroll 4
-      for (int k = ks; k < PITX_C; k += KS) {
-        const float x = xe[k], v = xv[k];
-        if (PASS == 1) {
-          f0 += x * v;
-          if (own_tt) f1 += v * v;
-        } else {
-          const float d = alpha * v - x;  // sdr.py:136 (alpha*target - input)
-          f0 += d * d;
-        }
-        if ((++m & 3) == 0) { acc0 += (double)f0; acc1 += (double)f1; f0 = 0.f; f1 = 0.f; }
+      for (int idx = tid; idx < nrow * PITX_C; idx += 256) {
+        const int r = idx / PITX_C, k = idx % PITX_C, kk = k0 + k;
+        const float* row = r < ne ? est + ((size_t)b * ne + r) * T : tgt + ((size_t)b * nt + (r - ne)) * T;
+        sh[r * PITX_CP + k] = kk < T ? __ldg(row + kk) : 0.f;
       }
-      acc0 += (double)f0;
-      acc1 += (double)f1;
+      if (orpit) {  // rests in the reference's order: sum over j of mask_rest * target (pit.py:135-138)
+        __syncthreads();
+        for (int idx = tid; idx < nb * PITX_C; idx += 256) {
+          const int i = idx / PITX_C, k = idx % PITX_C;
+          float r = 0.f;
+          for (int j = 0; j < nb; ++j)
+            if (j != i) r += sh[(ne + j) * PITX_CP + k];
+          sh[(ne + nt + i) * PITX_CP + k] = r;
+        }
+      }
+      __syncthreads();
+      if (act) {
+        float f0 = 0.f, f1 = 0.f;
+        int m = 0;
+#pragma unroll 4
+        for (int k = ks; k < PITX_C; k += KS) {
+          const float x = xe[k], v = xv[k];
+          if (PASS == 1) {
+            f0 += x * v;
+            if (own_tt) f1 += v * v;
+          } else {
+            const float d = alpha * v - x;  // sdr.py:136 (alpha*target - input)
+            f0 += d * d;
+          }
+          if ((++m & 3) == 0) { acc0 += (double)f0; acc1 += (double)f1; f0 = 0.f; f1 = 0.f; }
+        }
+        acc0 += (double)f0;
+        acc1 += (double)f1;
+      }
     }
-  }
-  for (int o = KS >> 1; o > 0; o >>= 1) {
-    acc0 += __shfl_xor_sync(0xffffffffu, acc0, o);
-    acc1 += __shfl_xor_sync(0xffffffffu, acc1, o);
-  }
-  if (act && ks == 0) {
-    if (PASS == 1) {
-      atomicAdd(&st[p], acc0);
-      if (own_tt) atomicAdd(&st[2 * P + vr], acc1);
-    } else {
-      atomicAdd(&st[P + p], acc0);
+    for (int o = KS >> 1; o > 0; o >>= 1) {
+      acc0 += __shfl_xor_sync(0xffffffffu, acc0, o);
+      acc1 += __shfl_xor_sync(0xffffffffu, acc1, o);
+    }
+    if (act && ks == 0) {
+      if (PASS == 1) {
+        atomicAdd(&st[p], acc0);
+        if (own_tt) atomicAdd(&st[2 * P + vr], acc1);
+      } else {
+        atomicAdd(&st[P + p], acc0);
+      }
     }
   }
 }
@@ -117,37 +120,41 @@ static int launch_pitx_stats(const float* est, const float* tgt, const int* n_b,
   const int chunks = (T + PITX_C - 1) / PITX_C;
   int gx = (PITX_CTAS + B - 1) / B;
   if (gx > chunks) gx = chunks;
-  k_pitx_stats<1><<<dim3(gx, B), 256, 0, st>>>(est, tgt, n_b, ne, nt, orpit, T, eps, stats);
+  const dim3 grid(gx, B < 65535 ? B : 65535);
+  k_pitx_stats<1><<<grid, 256, 0, st>>>(est, tgt, n_b, B, ne, nt, orpit, T, eps, stats);
   CTN_COUNT_LAUNCH();
   CTN_RETURN_IF_CUDA_ERR();
-  k_pitx_stats<2><<<dim3(gx, B), 256, 0, st>>>(est, tgt, n_b, ne, nt, orpit, T, eps, stats);
+  k_pitx_stats<2><<<grid, 256, 0, st>>>(est, tgt, n_b, B, ne, nt, orpit, T, eps, stats);
   CTN_COUNT_LAUNCH();
   CTN_RETURN_IF_CUDA_ERR();
   return CTN_OK;
 }
 
-// d_est (B, ne, T) = cx[b,i] * est_i + sum_j W[b,i,j] * tgt_j, W (B, ne, nt), cx (B, ne).  grid (chunks, B), block 256.
+// d_est (B, ne, T) = cx[b,i] * est_i + sum_j W[b,i,j] * tgt_j, W (B, ne, nt), cx (B, ne).  grid (chunks, min(B, 65535)),
+// block 256; samples loop over gridDim.y as in k_pitx_stats, restaging w and c per sample.
 __global__ void __launch_bounds__(256) k_pitx_pair_bwd(const float* __restrict__ est, const float* __restrict__ tgt,
-                                                       const float* __restrict__ W, const float* __restrict__ cx, int ne, int nt,
-                                                       int T, float* __restrict__ d_est) {
+                                                       const float* __restrict__ W, const float* __restrict__ cx, int B, int ne,
+                                                       int nt, int T, float* __restrict__ d_est) {
   __shared__ float w[PITX_MAX * PITX_MAX], c[PITX_MAX];
-  const int b = blockIdx.y;
-  for (int q = threadIdx.x; q < ne * nt; q += 256) w[(q / nt) * PITX_MAX + q % nt] = W[(size_t)b * ne * nt + q];
-  if (threadIdx.x < ne) c[threadIdx.x] = cx[(size_t)b * ne + threadIdx.x];
-  __syncthreads();
-  const float* eb = est + (size_t)b * ne * T;
-  const float* tb = tgt + (size_t)b * nt * T;
-  float* db = d_est + (size_t)b * ne * T;
-  for (int k = blockIdx.x * 256 + threadIdx.x; k < T; k += gridDim.x * 256) {
-    float t[PITX_MAX];
+  for (int b = blockIdx.y; b < B; b += gridDim.y) {
+    __syncthreads();  // the previous sample's w and c are read until here
+    for (int q = threadIdx.x; q < ne * nt; q += 256) w[(q / nt) * PITX_MAX + q % nt] = W[(size_t)b * ne * nt + q];
+    if (threadIdx.x < ne) c[threadIdx.x] = cx[(size_t)b * ne + threadIdx.x];
+    __syncthreads();
+    const float* eb = est + (size_t)b * ne * T;
+    const float* tb = tgt + (size_t)b * nt * T;
+    float* db = d_est + (size_t)b * ne * T;
+    for (int k = blockIdx.x * 256 + threadIdx.x; k < T; k += gridDim.x * 256) {
+      float t[PITX_MAX];
 #pragma unroll
-    for (int j = 0; j < PITX_MAX; ++j) t[j] = j < nt ? __ldg(tb + (size_t)j * T + k) : 0.f;
-    for (int i = 0; i < ne; ++i) {
-      float a = c[i] * __ldg(eb + (size_t)i * T + k);
+      for (int j = 0; j < PITX_MAX; ++j) t[j] = j < nt ? __ldg(tb + (size_t)j * T + k) : 0.f;
+      for (int i = 0; i < ne; ++i) {
+        float a = c[i] * __ldg(eb + (size_t)i * T + k);
 #pragma unroll
-      for (int j = 0; j < PITX_MAX; ++j)
-        if (j < nt) a = fmaf(w[i * PITX_MAX + j], t[j], a);
-      db[(size_t)i * T + k] = a;
+        for (int j = 0; j < PITX_MAX; ++j)
+          if (j < nt) a = fmaf(w[i * PITX_MAX + j], t[j], a);
+        db[(size_t)i * T + k] = a;
+      }
     }
   }
 }
@@ -156,7 +163,7 @@ static int launch_pitx_pair_bwd(const float* est, const float* tgt, const float*
                                 int T, float* d_est, cudaStream_t st) {
   int gx = (T + 1023) / 1024;
   if (gx > 64) gx = 64;
-  k_pitx_pair_bwd<<<dim3(gx, B), 256, 0, st>>>(est, tgt, W, cx, ne, nt, T, d_est);
+  k_pitx_pair_bwd<<<dim3(gx, B < 65535 ? B : 65535), 256, 0, st>>>(est, tgt, W, cx, B, ne, nt, T, d_est);
   CTN_COUNT_LAUNCH();
   CTN_RETURN_IF_CUDA_ERR();
   return CTN_OK;
@@ -233,7 +240,7 @@ __global__ void k_orpit_coef(const double* __restrict__ stats, const int* __rest
 
 // argument checks run before any CUDA call
 static int orpit_check(const float* est, const float* tgt, const void* scratch, int B, int n, int T) {
-  if (!est || !tgt || !scratch || B <= 0 || B > 65535 || T <= 0 || n < 2) return CTN_EINVAL;
+  if (!est || !tgt || !scratch || B <= 0 || T <= 0 || n < 2) return CTN_EINVAL;
   if (n > PITX_MAX) return CTN_EUNSUPPORTED;
   return CTN_OK;
 }
@@ -412,7 +419,7 @@ __global__ void k_sinkhorn_bwd(const double* __restrict__ stats, const double* _
 }
 
 static int sinkpit_check(const float* est, const float* tgt, const void* scratch, int B, int S, int T, int K, double coldness) {
-  if (!est || !tgt || !scratch || B <= 0 || B > 65535 || T <= 0 || S < 1 || K < 0 || !(coldness > 0.0) || !std::isfinite(coldness))
+  if (!est || !tgt || !scratch || B <= 0 || T <= 0 || S < 1 || K < 0 || !(coldness > 0.0) || !std::isfinite(coldness))
     return CTN_EINVAL;
   if (S > PITX_MAX) return CTN_EUNSUPPORTED;
   return CTN_OK;

@@ -86,7 +86,8 @@ ORPIT_CASES = {  # name: (lens, T, seed, dup, packed)
     "n2_T32000_B64": ([2] * 64, 32000, 6, False, False),
     "packed_T1603": ([3, 2, 5, 2, 4, 16, 3], 1603, 7, False, True),
     "packed_T32000": ([2, 3, 3, 2], 32000, 8, False, True),
-    "dup_tie_T1001": ([3, 4, 2], 1001, 9, True, True),
+    # T <= 256: one chunk, so each sample's statistics come from one CTA and the tied candidates' scores are bit-equal
+    "dup_tie_T256": ([3, 4, 2], 256, 9, True, True),
 }
 
 
