@@ -89,7 +89,7 @@ struct TcnWs {
   std::vector<float*> wimg1, wimg2;  // per block: tensor-core weight images of the two pointwise convs (math != fp32)
   std::vector<float*> rblk;          // per block: raw [out;skip] contraction output r_i (B, Bc+Sc, pitch), kept for the
                                      // deferred skip reduction (the skip accumulator is written once, at the end)
-  float *x, *skip, *h, *u, *outraw;
+  float *x, *skip, *h, *u;
   void* causal_ws;  // causal (cLN) models: scratch of the un-fused pipeline (ctn_causal.cu)
   float* xalt;  // second residual-stream buffer (tensor-core modes ping-pong x between blocks: the update is fused into pw1)
   // fp16-piece mode: activation envelope (ctn_act_scales)
@@ -101,20 +101,21 @@ struct TcnWs {
   size_t stats_bytes;
 };
 
-static int check_tcn_cfg(const ctn_config_t* c) {
+int check_tcn_cfg(const ctn_config_t* c, int max_layers) {
   if (!c) return CTN_EINVAL;
   if (c->bottleneck <= 0 || c->hidden <= 0 || c->skip <= 0 || c->sep_kernel <= 0 || c->num_blocks <= 0 || c->num_layers <= 0)
     return CTN_EINVAL;
-  if (c->num_layers > 20 || c->num_blocks * c->num_layers > CTN_MAX_BLOCKS) return CTN_EUNSUPPORTED;
+  if (c->num_layers > max_layers || c->num_blocks * c->num_layers > CTN_MAX_BLOCKS) return CTN_EUNSUPPORTED;
   if (c->math != CTN_MATH_FP32 && c->math != CTN_MATH_TF32X3 && c->math != CTN_MATH_TF32 && c->math != CTN_MATH_F16X3) return CTN_EINVAL;
   return CTN_OK;
 }
 
-static void carve_tcn(Carver& cv, const ctn_config_t* c, int B, int pitch, TcnWs* ws) {
+// The per-forward preparation state of the stack (weights may change every step): per block the gLN2 folds, the weight images
+// of the two contractions (tensor-core modes) and the depthwise parameter pack; the operand scales and the x_0 bound.  The
+// per-block raw [out;skip] buffers and the causal scratch are left empty for the caller to carve.
+static void carve_tcn_prep(Carver& cv, const ctn_config_t* c, TcnWs* ws) {
   const int RX = c->num_blocks * c->num_layers;
   const int Mt = c->bottleneck + c->skip;
-  ws->stats_bytes = sizeof(double) * 2 * RX * B * 2;
-  ws->stats = cv.take<double>((size_t)2 * RX * B * 2);
   ws->folds.resize(RX);
   ws->wimg1.assign(RX, nullptr);
   ws->wimg2.assign(RX, nullptr);
@@ -134,15 +135,22 @@ static void carve_tcn(Carver& cv, const ctn_config_t* c, int B, int pitch, TcnWs
   ws->x0_bound = cv.take<float>(64);  // ctn_tcn_fwd: measured max |x|; the model path points x0_bound at the head's row bounds
   ws->x0_n = 1;
   ws->mask_slope = nullptr;
+  ws->rblk.assign(RX, nullptr);
+  ws->causal_ws = nullptr;
+}
+
+static void carve_tcn(Carver& cv, const ctn_config_t* c, int B, int pitch, TcnWs* ws) {
+  const int RX = c->num_blocks * c->num_layers;
+  const int Mt = c->bottleneck + c->skip;
+  ws->stats_bytes = sizeof(double) * 2 * RX * B * 2;
+  ws->stats = cv.take<double>((size_t)2 * RX * B * 2);
+  carve_tcn_prep(cv, c, ws);
   const size_t bp = (size_t)B * pitch;
   ws->x = cv.take<float>(bp * c->bottleneck);
   ws->xalt = cv.take<float>(bp * c->bottleneck);
   ws->skip = cv.take<float>(bp * c->skip);
   ws->h = cv.take<float>(bp * c->hidden);
   ws->u = cv.take<float>(bp * c->hidden);
-  ws->outraw = nullptr;
-  ws->rblk.assign(RX, nullptr);
-  ws->causal_ws = nullptr;
   if (c->causal) {
     ws->causal_ws = cv.take<char>(ctn_causal_ws_bytes(c, B, pitch));
   } else {
@@ -229,7 +237,7 @@ static int run_tcn(const ctn_config_t* c, const ctn_block_params_t* blocks, TcnW
       { StageTimer tm(CTN_ST_PW1, st); CTN_TRY(ctn_pw(a, pro1, EPI_H, c->math, nullptr, st)); }
       const int Mt = has_out ? Bc + Sc : Sc;
       float* rb = ws->rblk[i];
-      const int pad_left = c->causal ? (c->sep_kernel - 1) * dilation : ((c->sep_kernel - 1) * dilation) / 2;
+      const int pad_left = ((c->sep_kernel - 1) * dilation) / 2;
       // fused depthwise producer: 3 taps at dilation 1, 2 or a multiple of 4 (128-bit aligned tap loads); anything else runs the
       // stand-alone depthwise stage
       const bool dw_fusable = c->sep_kernel == 3 && (dilation == 1 || dilation == 2 || dilation % 4 == 0);
@@ -250,7 +258,7 @@ static int run_tcn(const ctn_config_t* c, const ctn_block_params_t* blocks, TcnW
         // K_B: u = PReLU(dwconv(gLN1(h))), stats2
         { StageTimer tm(CTN_ST_DW, st);
           CTN_TRY(ctn_dw_fwd(hbuf, ws->u, p.norm1_g, p.norm1_b, p.dw_w, p.dw_b, p.prelu2, st1, st2, B, H, frames, pitch,
-                             c->sep_kernel, dilation, c->causal, c->eps_tcn, st)); }
+                             c->sep_kernel, dilation, c->eps_tcn, st)); }
         // K_C: r = [Wo;Ws] diag(gamma2) u
         memset(&a, 0, sizeof(a));
         a.A = ws->u; a.W = ws->folds[i].Wf; a.D = rb; a.B = B; a.M = Mt; a.K = H; a.frames = frames; a.pitch = pitch;
@@ -289,34 +297,14 @@ static int run_tcn(const ctn_config_t* c, const ctn_block_params_t* blocks, TcnW
 }
 
 // ---- training forward through the fused kernels (called by ctn_convtasnet_fwd_train, ctn_train.cu) ----------------------------
-// The training workspace carries its own copy of the small per-forward state of the TCN (folds, weight images, depthwise
-// parameter packs, operand scales) and one raw [out;skip] tensor per block; x / h_pre / u_pre live in the caller's per-block
-// buffers, the statistics in the caller's array (same [2*RX][B][2] layout the backward reads).
+// The training workspace carries its own copy of the per-forward preparation state of the TCN (carve_tcn_prep) and one raw
+// [out;skip] tensor per block; x / h_pre / u_pre live in the caller's per-block buffers, the statistics in the caller's array
+// (same [2*RX][B][2] layout the backward reads).
 static void carve_tcn_train(Carver& cv, const ctn_config_t* c, int B, int pitch, TcnWs* ws) {
-  const int RX = c->num_blocks * c->num_layers;
-  const int Mt = c->bottleneck + c->skip;
   ws->stats = nullptr; ws->stats_bytes = 0;
-  ws->folds.resize(RX);
-  ws->wimg1.assign(RX, nullptr);
-  ws->wimg2.assign(RX, nullptr);
-  ws->dwp.assign(RX, nullptr);
-  ws->rblk.assign(RX, nullptr);
-  for (int i = 0; i < RX; ++i) {
-    ws->folds[i].Wf = cv.take<float>((size_t)Mt * c->hidden);
-    ws->folds[i].v1 = cv.take<float>(Mt);
-    ws->folds[i].v2 = cv.take<float>(Mt);
-    ws->folds[i].vb = cv.take<float>(Mt);
-    ws->wimg1[i] = cv.take<float>(ctn_pw_wimg_bytes(c->hidden, c->bottleneck, c->math) / sizeof(float));
-    ws->wimg2[i] = cv.take<float>(ctn_pw_wimg_bytes(Mt, c->hidden, c->math) / sizeof(float));
-    ws->dwp[i] = cv.take<float>((size_t)ctn_round_up(c->hidden, 16) * 8);
-    ws->rblk[i] = cv.take<float>((size_t)B * pitch * Mt);
-  }
-  ws->scales = cv.take<float>((size_t)5 * RX + 8);
-  ws->x0_bound = cv.take<float>(64);
-  ws->x0_n = 1;
-  ws->mask_slope = nullptr;
-  ws->x = ws->xalt = ws->skip = ws->h = ws->u = ws->outraw = nullptr;
-  ws->causal_ws = nullptr;
+  carve_tcn_prep(cv, c, ws);
+  for (float*& r : ws->rblk) r = cv.take<float>((size_t)B * pitch * (c->bottleneck + c->skip));
+  ws->x = ws->xalt = ws->skip = ws->h = ws->u = nullptr;
 }
 size_t ctn_tcn_train_ws_bytes(const ctn_config_t* c, int B, int pitch) {
   Carver cv(nullptr);
@@ -393,7 +381,7 @@ extern "C" int ctn_tcn_blocks_fwd(const ctn_config_t* cfg, const ctn_block_param
   ctn_config_t c = *cfg;
   c.num_blocks = 1;
   c.num_layers = n_blocks;
-  if (c.bottleneck <= 0 || c.hidden <= 0 || c.skip <= 0 || c.sep_kernel <= 0) return CTN_EINVAL;
+  CTN_TRY(check_tcn_cfg(&c, CTN_MAX_BLOCKS));
   if (c.causal) return CTN_EUNSUPPORTED;  // the causal pipeline takes its dilations from the layer index
   for (int i = 0; i < n_blocks; ++i) {
     if (dilations[i] < 1) return CTN_EINVAL;
@@ -436,7 +424,7 @@ struct ModelWs {
   TcnWs tcn;
 };
 
-static int check_model_cfg(const ctn_config_t* c) {
+int check_model_cfg(const ctn_config_t* c) {
   CTN_TRY(check_tcn_cfg(c));
   if (c->n_basis <= 0 || c->kernel_size <= 0 || c->stride <= 0 || c->n_sources <= 0) return CTN_EINVAL;
   if (c->kernel_size % c->stride != 0) return CTN_EINVAL;

@@ -65,20 +65,30 @@ __global__ void __launch_bounds__(256) k_dw_plain(const float* __restrict__ h, f
   }
 }
 
-// rows of r (B, Mt, pitch): m < Bc (has_out): x += r + bo[m] ; else skip (+)= r + bs[j]      (tdcn.py:144-145, :39)
-__global__ void __launch_bounds__(256) k_res_skip_inplace(const float* __restrict__ r, int Mt, float* __restrict__ x,
-                                                          float* __restrict__ skip, const float* __restrict__ bo,
-                                                          const float* __restrict__ bs, int Bc, int Sc, int has_out, int skip_init,
-                                                          int frames, int pitch) {
+// rows of r (B, Mt, pitch): m < Bc (has_out): xout = xin + r + bo[m] ; else skip (+)= r + bs[j]      (tdcn.py:144-145, :39)
+// xin == xout updates the residual stream in place.  A thread owns 4 consecutive frames (128-bit loads / stores).
+__global__ void __launch_bounds__(256) k_res_skip(const float* __restrict__ r, int Mt, const float* xin, float* xout,
+                                                  float* __restrict__ skip, const float* __restrict__ bo,
+                                                  const float* __restrict__ bs, int Bc, int Sc, int has_out, int skip_init,
+                                                  int frames, int pitch) {
   const int b = blockIdx.y;
   for (int m = blockIdx.x; m < Mt; m += gridDim.x) {
     const float* rr = r + ((size_t)b * Mt + m) * pitch;
     const bool is_x = has_out && m < Bc;
     const int j = m - (has_out ? Bc : 0);
-    float* dst = is_x ? x + ((size_t)b * Bc + m) * pitch : skip + ((size_t)b * Sc + j) * pitch;
+    const float* src = is_x ? xin + ((size_t)b * Bc + m) * pitch : skip + ((size_t)b * Sc + j) * pitch;
+    float* dst = is_x ? xout + ((size_t)b * Bc + m) * pitch : skip + ((size_t)b * Sc + j) * pitch;
     const float bb = is_x ? bo[m] : bs[j];
     const bool fresh = !is_x && skip_init;
-    for (int t = threadIdx.x; t < pitch; t += 256) dst[t] = t < frames ? (fresh ? 0.f : dst[t]) + rr[t] + bb : 0.f;
+    for (int t = threadIdx.x * 4; t < pitch; t += 1024) {
+      float4 v = zero4();
+      if (t < frames) {
+        const float4 q = ld4(rr + t);
+        const float4 base = fresh ? zero4() : ld4(src + t);
+        v = mask4(make_float4(base.x + q.x + bb, base.y + q.y + bb, base.z + q.z + bb, base.w + q.w + bb), t, frames);
+      }
+      st4(dst + t, v);
+    }
   }
 }
 
@@ -91,8 +101,6 @@ __global__ void __launch_bounds__(256) k_bias_rows(float* __restrict__ y, const 
     for (int t = threadIdx.x; t < pitch; t += 256) r[t] = t < frames ? r[t] + bc : 0.f;
   }
 }
-
-inline dim3 grid_cb(int C, int B) { return dim3(C < 1024 ? C : 1024, B); }
 
 }  // namespace
 
@@ -127,7 +135,6 @@ int ctn_causal_tcn(const ctn_config_t* c, const ctn_block_params_t* blocks, floa
   CausalWs ws;
   carve(cv, c, B, pitch, &ws);
   const int R = c->num_blocks, X = c->num_layers, Bc = c->bottleneck, H = c->hidden, Sc = c->skip, P = c->sep_kernel;
-  cudaError_t e;
   for (int i = 0; i < R * X; ++i) {
     const ctn_block_params_t& q = blocks[i];
     const bool has_out = q.out_w != nullptr;
@@ -149,32 +156,33 @@ int ctn_causal_tcn(const ctn_config_t* c, const ctn_block_params_t* blocks, floa
       CTN_TRY(ctn_cln_pitch_fwd(u, q.norm2_g, q.norm2_b, u, B, H, frames, pitch, c->eps_tcn, ws.cln, st));
     }
     const int Mt = has_out ? Bc + Sc : Sc;
-    if (has_out && (e = cudaMemcpyAsync(ws.Wcat, q.out_w, sizeof(float) * (size_t)Bc * H, cudaMemcpyDeviceToDevice, st)) != cudaSuccess)
-      return (int)e;
-    if ((e = cudaMemcpyAsync(ws.Wcat + (has_out ? (size_t)Bc * H : 0), q.skip_w, sizeof(float) * (size_t)Sc * H,
-                             cudaMemcpyDeviceToDevice, st)) != cudaSuccess)
-      return (int)e;
+    CTN_TRY(ctn_block_wcat(q, Bc, Sc, H, ws.Wcat, st));
     memset(&a, 0, sizeof(a));
     a.A = u; a.W = ws.Wcat; a.D = ws.r; a.B = B; a.M = Mt; a.K = H; a.frames = frames; a.pitch = pitch;
     { StageTimer tm(CTN_ST_PW2, st); CTN_TRY(ctn_pw(a, PRO_NONE, EPI_RAW, c->math, ws.wimg, st)); }
-    {
-      StageTimer tm(CTN_ST_FIN, st);
-      k_res_skip_inplace<<<grid_cb(Mt, B), 256, 0, st>>>(ws.r, Mt, x, skip, q.out_b, q.skip_b, Bc, Sc, has_out ? 1 : 0, i == 0 ? 1 : 0,
-                                                         frames, pitch);
-      CTN_COUNT_LAUNCH();
-      CTN_RETURN_IF_CUDA_ERR();
-    }
+    { StageTimer tm(CTN_ST_FIN, st);
+      CTN_TRY(ctn_res_skip_fwd(ws.r, Mt, x, x, skip, q.out_b, q.skip_b, Bc, Sc, has_out ? 1 : 0, i == 0 ? 1 : 0, B, frames, pitch, st)); }
   }
   return CTN_OK;
 }
 
-// The per-frame kernels above, for the online (chunk-by-chunk) pipeline of ctn_online.cu: same kernels, same launch shape.
-int ctn_res_skip_fwd(const float* r, int Mt, float* x, float* skip, const float* bo, const float* bs, int Bc, int Sc, int has_out,
-                     int skip_init, int B, int frames, int pitch, cudaStream_t st) {
-  k_res_skip_inplace<<<grid_cb(Mt, B), 256, 0, st>>>(r, Mt, x, skip, bo, bs, Bc, Sc, has_out, skip_init, frames, pitch);
+// The per-frame kernels above, shared with the online (chunk-by-chunk) pipeline of ctn_online.cu and the un-fused training
+// forward of ctn_train.cu: same kernels, same launch shape.
+int ctn_res_skip_fwd(const float* r, int Mt, const float* xin, float* xout, float* skip, const float* bo, const float* bs, int Bc, int Sc,
+                     int has_out, int skip_init, int B, int frames, int pitch, cudaStream_t st) {
+  k_res_skip<<<grid_cb(Mt, B), 256, 0, st>>>(r, Mt, xin, xout, skip, bo, bs, Bc, Sc, has_out, skip_init, frames, pitch);
   CTN_COUNT_LAUNCH();
   CTN_RETURN_IF_CUDA_ERR();
   return CTN_OK;
+}
+
+int ctn_block_wcat(const ctn_block_params_t& q, int Bc, int Sc, int H, float* wcat, cudaStream_t st) {
+  const bool has_out = q.out_w != nullptr;
+  cudaError_t e = cudaSuccess;
+  if (has_out) e = cudaMemcpyAsync(wcat, q.out_w, sizeof(float) * (size_t)Bc * H, cudaMemcpyDeviceToDevice, st);
+  if (e == cudaSuccess)
+    e = cudaMemcpyAsync(wcat + (has_out ? (size_t)Bc * H : 0), q.skip_w, sizeof(float) * (size_t)Sc * H, cudaMemcpyDeviceToDevice, st);
+  return e == cudaSuccess ? CTN_OK : (int)e;
 }
 
 int ctn_bias_rows_fwd(float* y, const float* bias, int C, int B, int frames, int pitch, cudaStream_t st) {

@@ -97,6 +97,20 @@ __device__ __forceinline__ float2 gln_mean_rstd(const double* __restrict__ st, d
 
 __device__ __forceinline__ float prelu_f(float v, float a) { return v >= 0.f ? v : a * v; }
 
+// 128-bit row access of the (B, C, pitch) layout (rows 16-byte aligned)
+__device__ __forceinline__ float4 ld4(const float* p) { return *reinterpret_cast<const float4*>(p); }
+__device__ __forceinline__ void st4(float* p, float4 v) { *reinterpret_cast<float4*>(p) = v; }
+__device__ __forceinline__ float4 zero4() { return make_float4(0.f, 0.f, 0.f, 0.f); }
+// zero the lanes of a 4-vector that fall at or beyond `frames`
+__device__ __forceinline__ float4 mask4(float4 v, int t, int frames) {
+  if (t + 3 < frames) return v;
+  if (t + 0 >= frames) v.x = 0.f;
+  if (t + 1 >= frames) v.y = 0.f;
+  if (t + 2 >= frames) v.z = 0.f;
+  if (t + 3 >= frames) v.w = 0.f;
+  return v;
+}
+
 // ---- optional stage timing (ctn_profile_enable / ctn_profile_read) -------------------------------------------
 void ctn_prof_begin(int stage, cudaStream_t st);
 void ctn_prof_end(int stage, cudaStream_t st);

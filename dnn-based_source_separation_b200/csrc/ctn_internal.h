@@ -28,6 +28,16 @@ struct Carver {
 };
 
 #define CTN_MAX_BLOCKS 64
+
+// Config checks shared by every pipeline (ctn_api.cu): CTN_EINVAL for a value no pipeline accepts, CTN_EUNSUPPORTED for one
+// outside the stack's envelope.  check_tcn_cfg covers the separator stack's fields; max_layers is the longest run of layers
+// with dilations 2^l (20), or CTN_MAX_BLOCKS where the caller passes the dilations itself.  check_model_cfg adds the
+// encoder / mask / decoder fields.  Each pipeline adds its own envelope refusals after these.
+int check_tcn_cfg(const ctn_config_t* c, int max_layers = 20);
+int check_model_cfg(const ctn_config_t* c);
+
+// launch grid of the (B, C, pitch) streaming kernels: a block walks channels c = blockIdx.x, += gridDim.x
+inline dim3 grid_cb(int C, int B) { return dim3(C < 1024 ? C : 1024, B); }
 // epilogue / prologue selectors of the pointwise (1x1) contraction kernels
 enum { PRO_NONE = 0, PRO_PRELU = 1, PRO_DW = 2, PRO_RES = 3 };
 enum { EPI_RAW = 0, EPI_HEAD = 1, EPI_H = 2, EPI_MASK = 3, EPI_MASKDEC = 4 };
@@ -148,7 +158,7 @@ int ctn_softmax_mask(float* logits_what, const float* wenc, float* mask_out, int
 // depthwise stage: u = PReLU(dwconv(gLN1(h))) (+ stats2), all (B,H,pitch)
 int ctn_dw_fwd(const float* h, float* u, const float* norm_g, const float* norm_b, const float* dw_w, const float* dw_b,
                const float* slope, const double* stats_in, double* stats_out, int B, int H, int frames, int pitch, int P,
-               int dilation, int causal, float eps, cudaStream_t st);
+               int dilation, float eps, cudaStream_t st);
 
 // finishing: x += rstd2*outraw[:Bc] + c ; skip (+)= rstd2*outraw[Bc:] + c
 int ctn_finish_fwd(const float* outraw, const FoldedConv f, const double* stats2, double n2, float eps, float* x,
@@ -177,8 +187,11 @@ int ctn_causal_tcn(const ctn_config_t* c, const ctn_block_params_t* blocks, floa
 // separator head for causal models: x0 = Wb cLN0(w) + bb;  tmp: (B, N, pitch) scratch
 int ctn_causal_head(const ctn_config_t* c, const ctn_params_t* p, const float* w, float* tmp, float* x0, int B, int frames,
                     int pitch, void* cws, cudaStream_t st);
-// The causal pipeline's per-frame kernels on their own (ctn_online.cu):  rows of r (B, Mt, pitch): m < Bc (has_out): x += r + bo[m];
-// else skip (+)= r + bs[j] (skip_init: =);  and  y[b][c][t] += bias[c].  Columns [frames, pitch) are written as zero.
-int ctn_res_skip_fwd(const float* r, int Mt, float* x, float* skip, const float* bo, const float* bs, int Bc, int Sc, int has_out,
-                     int skip_init, int B, int frames, int pitch, cudaStream_t st);
+// The un-folded pipelines' per-frame kernels on their own (causal, online, un-fused training forward):  rows of r (B, Mt, pitch):
+// m < Bc (has_out): xout = xin + r + bo[m] (xin == xout: in place); else skip (+)= r + bs[j] (skip_init: =);  and
+// y[b][c][t] += bias[c].  Columns [frames, pitch) are written as zero.
+int ctn_res_skip_fwd(const float* r, int Mt, const float* xin, float* xout, float* skip, const float* bo, const float* bs, int Bc, int Sc,
+                     int has_out, int skip_init, int B, int frames, int pitch, cudaStream_t st);
 int ctn_bias_rows_fwd(float* y, const float* bias, int C, int B, int frames, int pitch, cudaStream_t st);
+// a block's [out_w; skip_w] (skip_w alone when it has no output head) -> wcat (Mt, H), stream-ordered device copies
+int ctn_block_wcat(const ctn_block_params_t& q, int Bc, int Sc, int H, float* wcat, cudaStream_t st);

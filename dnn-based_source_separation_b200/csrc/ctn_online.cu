@@ -99,15 +99,8 @@ void carve(Carver& cv, const ctn_config_t* c, int B, int pitch, OnlineState* s) 
 }
 
 int check_cfg(const ctn_config_t* c) {
-  if (!c) return CTN_EINVAL;
-  if (c->causal != 1 || c->in_channels > 1) return CTN_EUNSUPPORTED;  // gLN needs the whole utterance; monaural only
-  if (c->n_basis <= 0 || c->kernel_size <= 0 || c->stride <= 0 || c->n_sources <= 0 || c->bottleneck <= 0 || c->hidden <= 0 ||
-      c->skip <= 0 || c->sep_kernel <= 0 || c->num_blocks <= 0 || c->num_layers <= 0 || c->in_channels < 0)
-    return CTN_EINVAL;
-  if (c->kernel_size % c->stride != 0) return CTN_EINVAL;
-  if (c->mask_softmax != 0 && c->mask_softmax != 1) return CTN_EINVAL;
-  if (c->math != CTN_MATH_FP32 && c->math != CTN_MATH_TF32X3 && c->math != CTN_MATH_TF32 && c->math != CTN_MATH_F16X3) return CTN_EINVAL;
-  if (c->num_layers > 20 || c->num_blocks * c->num_layers > CTN_MAX_BLOCKS) return CTN_EUNSUPPORTED;
+  if (c && (c->causal != 1 || c->in_channels > 1)) return CTN_EUNSUPPORTED;  // gLN needs the whole utterance; monaural only
+  CTN_TRY(check_model_cfg(c));
   if ((size_t)c->n_basis * (c->kernel_size / c->stride - 1) * sizeof(float) > 48 * 1024) return CTN_EUNSUPPORTED;  // decoder history
   return CTN_OK;
 }
@@ -393,13 +386,8 @@ extern "C" int ctn_online_init(const ctn_config_t* cfg, const ctn_params_t* para
   // the offline path copies [Wo; Ws] and builds every image on each call; here once
   for (int i = 0; i < RX; ++i) {
     const ctn_block_params_t& q = params->blocks[i];
-    const bool has_out = q.out_w != nullptr;
-    const int Mt = has_out ? Bc + Sc : Sc;
-    if (has_out && (e = cudaMemcpyAsync(s.wcat[i], q.out_w, sizeof(float) * (size_t)Bc * H, cudaMemcpyDeviceToDevice, st)) != cudaSuccess)
-      return (int)e;
-    if ((e = cudaMemcpyAsync(s.wcat[i] + (has_out ? (size_t)Bc * H : 0), q.skip_w, sizeof(float) * (size_t)Sc * H,
-                             cudaMemcpyDeviceToDevice, st)) != cudaSuccess)
-      return (int)e;
+    const int Mt = q.out_w ? Bc + Sc : Sc;
+    CTN_TRY(ctn_block_wcat(q, Bc, Sc, H, s.wcat[i], st));
     PwArgs a;
     memset(&a, 0, sizeof(a));
     a.W = q.bottleneck_w; a.M = H; a.K = Bc;
@@ -490,7 +478,7 @@ extern "C" int ctn_online_push(const ctn_config_t* cfg, const ctn_params_t* para
     a.A = s.u; a.W = s.wcat[i]; a.D = s.r; a.B = B; a.M = Mt; a.K = H; a.frames = F; a.pitch = pitch; a.wimg = s.wimg2[i];
     { StageTimer tm(CTN_ST_PW2, st); CTN_TRY(ctn_pw(a, PRO_NONE, EPI_RAW, cfg->math, nullptr, st)); }
     { StageTimer tm(CTN_ST_FIN, st);
-      CTN_TRY(ctn_res_skip_fwd(s.r, Mt, s.x, s.skip, q.out_b, q.skip_b, Bc, Sc, has_out ? 1 : 0, i == 0 ? 1 : 0, B, F, pitch, st)); }
+      CTN_TRY(ctn_res_skip_fwd(s.r, Mt, s.x, s.x, s.skip, q.out_b, q.skip_b, Bc, Sc, has_out ? 1 : 0, i == 0 ? 1 : 0, B, F, pitch, st)); }
   }
   {
     StageTimer tm(CTN_ST_MASK, st);

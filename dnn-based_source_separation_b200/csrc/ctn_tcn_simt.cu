@@ -332,7 +332,7 @@ int ctn_softmax_mask(float* logits_what, const float* wenc, float* mask_out, int
 // ------------------------------------------------------------------------------------------------
 // depthwise stage:  u[c][t] = PReLU( sum_k wd[c][k] * hn[c][t + k*d - pl] + bd[c] ),
 //   hn = gLN1(h) inside [0,frames), exactly 0 outside (F.pad after the norm, tdcn.py:123-132),
-//   pl = ((P-1)d)//2 (non-causal) or (P-1)d (causal).   + (sum, sumsq) of u -> stats_out.
+//   pl = ((P-1)d)//2.   + (sum, sumsq) of u -> stats_out.
 // thread = 4 consecutive frames of one channel; grid (pitch/512, H, B), block 128.
 // ------------------------------------------------------------------------------------------------
 template <int P>
@@ -387,9 +387,8 @@ __global__ void __launch_bounds__(128) k_dw(const float* __restrict__ h, float* 
 
 int ctn_dw_fwd(const float* h, float* u, const float* norm_g, const float* norm_b, const float* dw_w, const float* dw_b,
                const float* slope, const double* stats_in, double* stats_out, int B, int H, int frames, int pitch, int P,
-               int dilation, int causal, float eps, cudaStream_t st) {
-  const int pad = (P - 1) * dilation;
-  const int pad_left = causal ? pad : pad / 2;
+               int dilation, float eps, cudaStream_t st) {
+  const int pad_left = ((P - 1) * dilation) / 2;
   dim3 grid((pitch + 511) / 512, H, B);
   if (P == 3)
     k_dw<3><<<grid, 128, 0, st>>>(h, u, norm_g, norm_b, dw_w, dw_b, slope, stats_in, stats_out, H, frames, pitch, P, dilation, pad_left, eps);

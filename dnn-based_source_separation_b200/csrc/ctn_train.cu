@@ -25,18 +25,6 @@ namespace {
 // pad columns are written as zero.  A thread owns 4 consecutive time steps (128-bit loads / stores).
 // Unless noted: grid (min(C, 1024), B), block 256, a block walks channels c = blockIdx.x, += gridDim.x.
 // ================================================================================================================
-__device__ __forceinline__ float4 ld4(const float* p) { return *reinterpret_cast<const float4*>(p); }
-__device__ __forceinline__ void st4(float* p, float4 v) { *reinterpret_cast<float4*>(p) = v; }
-__device__ __forceinline__ float4 zero4() { return make_float4(0.f, 0.f, 0.f, 0.f); }
-// zero the lanes of a 4-vector that fall at or beyond `frames`
-__device__ __forceinline__ float4 mask4(float4 v, int t, int frames) {
-  if (t + 3 < frames) return v;
-  if (t + 0 >= frames) v.x = 0.f;
-  if (t + 1 >= frames) v.y = 0.f;
-  if (t + 2 >= frames) v.z = 0.f;
-  if (t + 3 >= frames) v.w = 0.f;
-  return v;
-}
 // 4 consecutive samples row[t0 .. t0+3] with zero outside [0, frames) (any alignment, any t0)
 __device__ __forceinline__ float4 ld4_shift(const float* __restrict__ row, int t0, int frames) {
   if ((t0 & 3) == 0 && t0 >= 0 && t0 + 3 < frames) return ld4(row + t0);
@@ -164,32 +152,6 @@ __global__ void __launch_bounds__(256) k_act_norm(const float* __restrict__ pre,
         }
         st4(o + t, v);
       }
-    }
-  }
-}
-
-// rows of r (B, Mt, pitch): m < Bc (has_out): x_out = x_in + r + bo[m] ; else skip (+)= r + bs[j]      (tdcn.py:144-145, :39)
-__global__ void __launch_bounds__(256) k_res_skip(const float* __restrict__ r, int Mt, const float* __restrict__ xin,
-                                                  float* __restrict__ xout, float* __restrict__ skip,
-                                                  const float* __restrict__ bo, const float* __restrict__ bs, int Bc, int Sc,
-                                                  int has_out, int skip_init, int frames, int pitch) {
-  const int b = blockIdx.y;
-  for (int m = blockIdx.x; m < Mt; m += gridDim.x) {
-    const float* rr = r + ((size_t)b * Mt + m) * pitch;
-    const bool is_x = has_out && m < Bc;
-    const int j = m - (has_out ? Bc : 0);
-    const float* src = is_x ? xin + ((size_t)b * Bc + m) * pitch : skip + ((size_t)b * Sc + j) * pitch;
-    float* dst = is_x ? xout + ((size_t)b * Bc + m) * pitch : skip + ((size_t)b * Sc + j) * pitch;
-    const float bb = is_x ? bo[m] : bs[j];
-    const bool fresh = !is_x && skip_init;
-    for (int t = threadIdx.x * 4; t < pitch; t += 1024) {
-      float4 v = zero4();
-      if (t < frames) {
-        const float4 q = ld4(rr + t);
-        const float4 base = fresh ? zero4() : ld4(src + t);
-        v = mask4(make_float4(base.x + q.x + bb, base.y + q.y + bb, base.z + q.z + bb, base.w + q.w + bb), t, frames);
-      }
-      st4(dst + t, v);
     }
   }
 }
@@ -652,8 +614,6 @@ __global__ void __launch_bounds__(256) k_wgrad(const float* __restrict__ dy, siz
 // ================================================================================================================
 // host side
 // ================================================================================================================
-inline dim3 grid_cb(int C, int B) { return dim3(C < 1024 ? C : 1024, B); }
-
 #define LAUNCH_CHECK()      \
   do {                      \
     CTN_COUNT_LAUNCH();     \
@@ -750,14 +710,8 @@ void carve_train(Carver& cv, const ctn_config_t* c, int B, int pitch, TrainWs* w
 }
 
 int check_train_cfg(const ctn_config_t* c) {
-  if (!c) return CTN_EINVAL;
-  if (c->n_basis <= 0 || c->kernel_size <= 0 || c->stride <= 0 || c->n_sources <= 0 || c->bottleneck <= 0 || c->hidden <= 0 ||
-      c->skip <= 0 || c->sep_kernel <= 0 || c->num_blocks <= 0 || c->num_layers <= 0)
-    return CTN_EINVAL;
-  if (c->kernel_size % c->stride != 0) return CTN_EINVAL;
-  if (c->num_layers > 20 || c->num_blocks * c->num_layers > CTN_MAX_BLOCKS) return CTN_EUNSUPPORTED;
-  if (c->causal || c->mask_softmax || c->in_channels > 1 || c->sep_kernel > CTN_MAX_P) return CTN_EUNSUPPORTED;  // softmax masks, multichannel: forward only
-  if (c->math != CTN_MATH_FP32 && c->math != CTN_MATH_TF32X3 && c->math != CTN_MATH_TF32 && c->math != CTN_MATH_F16X3) return CTN_EINVAL;
+  CTN_TRY(check_model_cfg(c));
+  if (c->causal || c->mask_softmax || c->in_channels > 1 || c->sep_kernel > CTN_MAX_P) return CTN_EUNSUPPORTED;  // causal, softmax masks, multichannel: forward only
   return CTN_OK;
 }
 
@@ -920,15 +874,11 @@ extern "C" int ctn_convtasnet_fwd_train(const ctn_config_t* c, const ctn_params_
     k_act_norm<<<grid_cb(H, B), 256, 0, st>>>(ws.upre[i], ws.T1, q.prelu2, q.norm2_g, q.norm2_b, st2, nH, c->eps_tcn, H, frames, pitch);
     LAUNCH_CHECK();
     const int Mt = has_out ? Bc + Sc : Sc;
-    if (has_out) {
-      if ((e = cudaMemcpyAsync(ws.Wcat, q.out_w, sizeof(float) * (size_t)Bc * H, cudaMemcpyDeviceToDevice, st)) != cudaSuccess) return (int)e;
-    }
-    if ((e = cudaMemcpyAsync(ws.Wcat + (has_out ? (size_t)Bc * H : 0), q.skip_w, sizeof(float) * (size_t)Sc * H, cudaMemcpyDeviceToDevice, st)) != cudaSuccess) return (int)e;
+    CTN_TRY(ctn_block_wcat(q, Bc, Sc, H, ws.Wcat, st));
     CTN_TRY(gemm_raw(c, ws, ws.Wcat, Mt, H, ws.T1, ws.r, B, frames, pitch, st));
     // x_{i+1} = x_i + out + bo ; skip += skip_i + bs
-    k_res_skip<<<grid_cb(Mt, B), 256, 0, st>>>(ws.r, Mt, ws.x[i], has_out ? ws.x[i + 1] : nullptr, ws.skip, q.out_b, q.skip_b, Bc, Sc,
-                                               has_out ? 1 : 0, i == 0 ? 1 : 0, frames, pitch);
-    LAUNCH_CHECK();
+    CTN_TRY(ctn_res_skip_fwd(ws.r, Mt, ws.x[i], has_out ? ws.x[i + 1] : nullptr, ws.skip, q.out_b, q.skip_b, Bc, Sc, has_out ? 1 : 0,
+                             i == 0 ? 1 : 0, B, frames, pitch, st));
   }
   // tail: PReLU -> mask 1x1 -> sigmoid -> * w (conv_tasnet.py:373-376, 158-160); keeps the mask
   {
@@ -1009,11 +959,7 @@ extern "C" int ctn_convtasnet_bwd(const ctn_config_t* c, const ctn_params_t* p, 
     const float* dYs = dY + (has_out ? bsBc : 0);
     CTN_TRY(rowsum(dYs, dY_bs, Sc, B, frames, pitch, G(gq.skip_b), st));
     // d_un = [Wo; Ws]^T dY
-    {
-      cudaError_t e;
-      if (has_out && (e = cudaMemcpyAsync(ws.Wcat, q.out_w, sizeof(float) * (size_t)Bc * H, cudaMemcpyDeviceToDevice, st)) != cudaSuccess) return (int)e;
-      if ((e = cudaMemcpyAsync(ws.Wcat + (has_out ? (size_t)Bc * H : 0), q.skip_w, sizeof(float) * (size_t)Sc * H, cudaMemcpyDeviceToDevice, st)) != cudaSuccess) return (int)e;
-    }
+    CTN_TRY(ctn_block_wcat(q, Bc, Sc, H, ws.Wcat, st));
     CTN_TRY(transpose(ws.Wcat, ws.Wt, Mt, H, st));
     CTN_TRY(gemm_raw(c, ws, ws.Wt, H, Mt, dY, ws.G1, B, frames, pitch, st));
     // gLN2 + PReLU2 backward -> d_u_pre (G1 in place); dgamma2, dbeta2, da2, d(bd)

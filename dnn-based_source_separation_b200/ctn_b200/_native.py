@@ -48,6 +48,37 @@ class Params(C.Structure):
                 ("blocks", C.POINTER(BlockParams)), ("prelu_out", _fp), ("mask_w", _fp), ("mask_b", _fp), ("dec_w", _fp)]
 
 
+TOP_FIELDS = tuple(n for n, _ in Params._fields_ if n != "blocks")
+
+
+def build_params(slots, dev):
+    """ctn_params_t over [(slot, tensor-or-None)], slot = a top-level field name or (block index, block field name); the block
+    array spans the highest block index.  Every tensor must be float32 on `dev`; a non-contiguous one is passed as a contiguous
+    copy.  -> (Params, keep): keep holds the block array and the copies and must outlive the C call."""
+    slots = list(slots)
+    arr = (BlockParams * (1 + max((s[0] for s, _ in slots if isinstance(s, tuple)), default=-1)))()
+    p = Params()
+    keep = [arr]
+    for slot, t in slots:
+        if t is not None:
+            if t.device != dev or t.dtype != torch.float32:
+                raise RuntimeError("parameter {} must be float32 on {}".format(slot, dev))
+            if not t.is_contiguous():
+                t = t.contiguous()
+                keep.append(t)
+        if isinstance(slot, tuple):
+            setattr(arr[slot[0]], slot[1], ptr(t))
+        else:
+            setattr(p, slot, ptr(t))
+    p.blocks = arr
+    return p, keep
+
+
+def norm_affine(norm):
+    """(gamma, beta) of a gLN (GroupNorm-backed) or cLN module"""
+    return (norm.norm.weight, norm.norm.bias) if hasattr(norm, "norm") else (norm.gamma, norm.beta)
+
+
 def _sig(name, restype, *argtypes):
     fn = getattr(lib, name)
     fn.restype = restype
@@ -188,6 +219,12 @@ def workspace(device: torch.device, nbytes: int, tag: str = "ws") -> torch.Tenso
         buf = torch.empty(int(nbytes) + 256, dtype=torch.uint8, device=device)
         _workspaces[key] = buf
     return buf
+
+
+def aligned(buf: torch.Tensor) -> Tuple[int, int]:
+    """(base, nbytes) of a uint8 device buffer: its first 256-byte-aligned address and the bytes usable from there"""
+    base = (buf.data_ptr() + 255) & ~255
+    return base, buf.numel() - (base - buf.data_ptr())
 
 
 def release_workspaces() -> None:

@@ -11,44 +11,12 @@ import torch
 
 from .. import _native as N
 
-TOP_FIELDS = ("enc_w", "norm0_g", "norm0_b", "bn_w", "bn_b", "prelu_out", "mask_w", "mask_b", "dec_w")
+TOP_FIELDS = N.TOP_FIELDS
 
 
 def param_list(model):
     """[(slot, tensor-or-None)] in a fixed order; slot = top-level field name or (block index, block field name)."""
-    sep = model.separator
-    g0 = sep.norm1d.norm.weight if hasattr(sep.norm1d, "norm") else sep.norm1d.gamma
-    b0 = sep.norm1d.norm.bias if hasattr(sep.norm1d, "norm") else sep.norm1d.beta
-    top = dict(enc_w=model.encoder.conv1d.weight, norm0_g=g0, norm0_b=b0, bn_w=sep.bottleneck_conv1d.weight,
-               bn_b=sep.bottleneck_conv1d.bias, prelu_out=sep.prelu.weight, mask_w=sep.mask_conv1d.weight,
-               mask_b=sep.mask_conv1d.bias, dec_w=model.decoder.conv_transpose1d.weight)
-    out = [(k, top[k]) for k in TOP_FIELDS]
-    for i, blk in enumerate(sep.tdcn.residual_blocks()):
-        for name, t in zip(N.BLOCK_FIELDS, blk.native_params()):
-            out.append(((i, name), t))
-    return out
-
-
-def _struct(slots, tensors, n_blocks, dev):
-    """ctn_params_t (or the identically laid out gradient struct) over `tensors`."""
-    arr = (N.BlockParams * n_blocks)()
-    p = N.Params()
-    keep = [arr]
-    for slot, t in zip(slots, tensors):
-        ptr = None
-        if t is not None:
-            if t.device != dev or t.dtype != torch.float32:
-                raise RuntimeError("parameter {} must be float32 on {}".format(slot, dev))
-            if not t.is_contiguous():
-                t = t.contiguous()
-                keep.append(t)
-            ptr = t.data_ptr()
-        if isinstance(slot, tuple):
-            setattr(arr[slot[0]], slot[1], ptr)
-        else:
-            setattr(p, slot, ptr)
-    p.blocks = arr
-    return p, keep
+    return model.separator.param_slots(enc_w=model.encoder.conv1d.weight, dec_w=model.decoder.conv_transpose1d.weight)
 
 
 class ConvTasNetTrainFn(torch.autograd.Function):
@@ -57,22 +25,20 @@ class ConvTasNetTrainFn(torch.autograd.Function):
         dev = N.require_cuda(x)
         B, _, T = x.shape
         slots = [s for s, _ in param_list(model)]
-        n_blocks = len(model.separator.tdcn.residual_blocks())
         cfg = model.native_config()
-        params, keep = _struct(slots, tensors, n_blocks, dev)
+        params, keep = N.build_params(zip(slots, tensors), dev)
         need = C.c_size_t(0)
         N.check(N.ctn_train_workspace_bytes(C.byref(cfg), B, T, C.byref(need)), "ctn_train_workspace_bytes")
         ws = torch.empty(need.value + 256, dtype=torch.uint8, device=dev)  # owned by this node until backward
-        base = (ws.data_ptr() + 255) & ~255
         out = torch.empty(B, model.n_sources, T, dtype=torch.float32, device=dev)
-        N.check(N.ctn_convtasnet_fwd_train(C.byref(cfg), C.byref(params), x.data_ptr(), B, T, out.data_ptr(), base,
-                                           ws.numel() - (base - ws.data_ptr()), N.stream_ptr(dev)), "ctn_convtasnet_fwd_train")
+        N.check(N.ctn_convtasnet_fwd_train(C.byref(cfg), C.byref(params), x.data_ptr(), B, T, out.data_ptr(), *N.aligned(ws),
+                                           N.stream_ptr(dev)), "ctn_convtasnet_fwd_train")
         model.last_launches = N.ctn_last_launch_count()
         # x and the parameters go through save_for_backward: an in-place update between forward and backward is detected by autograd
         # (version counters) instead of silently changing the weights the backward kernels see
         ctx.save_for_backward(x, *[t for t in tensors if t is not None])
         ctx.present = [t is not None for t in tensors]
-        ctx.cfg, ctx.ws, ctx.slots, ctx.n_blocks, ctx.model = cfg, ws, slots, n_blocks, model
+        ctx.cfg, ctx.ws, ctx.slots, ctx.model = cfg, ws, slots, model
         return out
 
     @staticmethod
@@ -88,7 +54,7 @@ class ConvTasNetTrainFn(torch.autograd.Function):
         B, _, T = x.shape
         d_out = d_out.contiguous()
         N.require_cuda(d_out)
-        params, keep = _struct(ctx.slots, tensors, ctx.n_blocks, dev)
+        params, keep = N.build_params(zip(ctx.slots, tensors), dev)
         # one flat zero-initialised gradient buffer; every tensor starts 64-float aligned
         offs, total = [], 0
         for t in tensors:
@@ -96,10 +62,9 @@ class ConvTasNetTrainFn(torch.autograd.Function):
             total += 0 if t is None else (t.numel() + 63) // 64 * 64
         flat = torch.zeros(total, dtype=torch.float32, device=dev)
         gviews = [None if t is None else flat[o:o + t.numel()].view(t.shape) for t, o in zip(tensors, offs)]
-        grads, keep2 = _struct(ctx.slots, gviews, ctx.n_blocks, dev)
-        base = (ws.data_ptr() + 255) & ~255
-        N.check(N.ctn_convtasnet_bwd(C.byref(cfg), C.byref(params), C.byref(grads), x.data_ptr(), d_out.data_ptr(), B, T, base,
-                                     ws.numel() - (base - ws.data_ptr()), N.stream_ptr(dev)), "ctn_convtasnet_bwd")
+        grads, keep2 = N.build_params(zip(ctx.slots, gviews), dev)
+        N.check(N.ctn_convtasnet_bwd(C.byref(cfg), C.byref(params), C.byref(grads), x.data_ptr(), d_out.data_ptr(), B, T,
+                                     *N.aligned(ws), N.stream_ptr(dev)), "ctn_convtasnet_bwd")
         ctx.model.last_bwd_launches = N.ctn_last_launch_count()
         ctx.model.last_flat_grad = flat
         ctx.ws = None

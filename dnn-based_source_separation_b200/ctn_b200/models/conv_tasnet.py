@@ -21,7 +21,7 @@ from .. import _native as N
 from ..utils.filterbank import choose_filterbank
 from ..utils.tasnet import choose_layer_norm
 from . import tdcn as _tdcn
-from .tdcn import TimeDilatedConvNet, block_param_array, resolve_math
+from .tdcn import TimeDilatedConvNet, block_slots, resolve_math
 
 EPS = 1e-12
 DEFAULT_MATH = None
@@ -33,10 +33,6 @@ def _load_checkpoint(path):
         return torch.load(path, map_location="cpu", weights_only=True)
     except Exception:
         return torch.load(path, map_location="cpu", weights_only=False)
-
-
-def _norm_affine(norm):
-    return (norm.norm.weight, norm.norm.bias) if hasattr(norm, "norm") else (norm.gamma, norm.beta)
 
 
 class Separator(nn.Module):
@@ -70,25 +66,15 @@ class Separator(nn.Module):
         cfg.eps = float(self.eps)
         return cfg
 
+    def param_slots(self, enc_w=None, dec_w=None):
+        """[(slot, tensor-or-None)] in the order of ctn_params_t: slot = top-level field name or (block index, block field name)"""
+        g0, b0 = N.norm_affine(self.norm1d)
+        top = dict(enc_w=enc_w, norm0_g=g0, norm0_b=b0, bn_w=self.bottleneck_conv1d.weight, bn_b=self.bottleneck_conv1d.bias,
+                   prelu_out=self.prelu.weight, mask_w=self.mask_conv1d.weight, mask_b=self.mask_conv1d.bias, dec_w=dec_w)
+        return [(k, top[k]) for k in N.TOP_FIELDS] + block_slots(self.tdcn.residual_blocks())
+
     def native_params(self, dev, enc_w=None, dec_w=None):
-        arr, keep = block_param_array(self.tdcn.residual_blocks(), dev)
-        g0, b0 = _norm_affine(self.norm1d)
-        tensors = dict(enc_w=enc_w, norm0_g=g0, norm0_b=b0, bn_w=self.bottleneck_conv1d.weight, bn_b=self.bottleneck_conv1d.bias,
-                       prelu_out=self.prelu.weight, mask_w=self.mask_conv1d.weight, mask_b=self.mask_conv1d.bias, dec_w=dec_w)
-        p = N.Params()
-        for name, t in tensors.items():
-            if t is None:
-                setattr(p, name, None)
-                continue
-            if t.device != dev or t.dtype != torch.float32:
-                raise RuntimeError("parameter {} must be float32 on {}".format(name, dev))
-            if not t.is_contiguous():
-                t = t.contiguous()
-                keep.append(t)
-            setattr(p, name, t.data_ptr())
-        p.blocks = arr
-        keep.append(arr)
-        return p, keep
+        return N.build_params(self.param_slots(enc_w, dec_w), dev)
 
     def forward(self, input):
         """input (batch_size, num_features, n_frames) -> mask (batch_size, n_sources, num_features, n_frames)"""
@@ -105,11 +91,10 @@ class Separator(nn.Module):
         N.check(N.ctn_workspace_bytes(C.byref(cfg), B, frames, C.byref(need)), "ctn_workspace_bytes")  # kernel 1, stride 1: T == frames
         pitch = N.ctn_pitch(frames)
         extra = 4 * B * self.n_sources * self.num_features * pitch + 1024
-        ws = N.workspace(dev, need.value + extra)
-        base = (ws.data_ptr() + 255) & ~255
+        base, nbytes = N.aligned(N.workspace(dev, need.value + extra))
         mask = torch.empty(B, self.n_sources, self.num_features, frames, dtype=torch.float32, device=dev)
-        N.check(N.ctn_separator_fwd(C.byref(cfg), C.byref(params), w.data_ptr(), B, frames, mask.data_ptr(), base,
-                                    ws.numel() - (base - ws.data_ptr()), N.stream_ptr(dev)), "ctn_separator_fwd")
+        N.check(N.ctn_separator_fwd(C.byref(cfg), C.byref(params), w.data_ptr(), B, frames, mask.data_ptr(), base, nbytes,
+                                    N.stream_ptr(dev)), "ctn_separator_fwd")
         return mask
 
 
@@ -156,27 +141,6 @@ class ConvTasNet(nn.Module):
     def extract_latent(self, input):
         """input (batch_size, 1, T) -> output (batch_size, n_sources, T), latent (batch_size, n_sources, n_basis, T')"""
         return self._run(input, want_latent=True)
-
-    def _run_multichannel(self, x, want_latent):
-        """x (batch, n_mics, T) -> (batch, n_sources, n_mics, T): same C call, multichannel filter banks (forward only)"""
-        if torch.is_grad_enabled() and any(p.requires_grad for p in self.parameters()):
-            raise NotImplementedError("multichannel models (in_channels > 1) are forward only: call under torch.no_grad()")
-        x = x.contiguous()
-        dev = N.require_cuda(x)
-        B, Cin, T = x.shape
-        frames, _, _ = N.frames_of(T, self.kernel_size, self.stride)
-        cfg = self.native_config()
-        params, keep = self.native_params(dev)
-        need = C.c_size_t(0)
-        N.check(N.ctn_workspace_bytes(C.byref(cfg), B, T, C.byref(need)), "ctn_workspace_bytes")
-        ws = N.workspace(dev, need.value)
-        base = (ws.data_ptr() + 255) & ~255
-        out = torch.empty(B, self.n_sources, Cin, T, dtype=torch.float32, device=dev)
-        latent = torch.empty(B, self.n_sources, self.n_basis, frames, dtype=torch.float32, device=dev) if want_latent else None
-        N.check(N.ctn_convtasnet_fwd(C.byref(cfg), C.byref(params), x.data_ptr(), B, T, out.data_ptr(), N.ptr(latent), base,
-                                     ws.numel() - (base - ws.data_ptr()), N.stream_ptr(dev)), "ctn_convtasnet_fwd")
-        self.last_launches = N.ctn_last_launch_count()
-        return out, latent
 
     def get_config(self):
         return {
@@ -313,15 +277,13 @@ class ConvTasNet(nn.Module):
         params, keep = self.native_params(dev)
         need = C.c_size_t(0)
         N.check(N.ctn_workspace_bytes(C.byref(cfg), B, T, C.byref(need)), "ctn_workspace_bytes")
-        ws = N.workspace(dev, need.value)
+        wbase, wbytes = N.aligned(N.workspace(dev, need.value))
         io_bytes = N.ctn_host_io_bytes(C.byref(cfg), B, T)
-        io = N.workspace(dev, io_bytes + 256, tag="host_io")
-        wbase, ibase = (ws.data_ptr() + 255) & ~255, (io.data_ptr() + 255) & ~255
+        ibase, ibytes = N.aligned(N.workspace(dev, io_bytes + 256, tag="host_io"))
         with torch.cuda.device(dev):
             N.check(N.ctn_convtasnet_loss_host(C.byref(cfg), C.byref(params), mixture_host.data_ptr(), sources_host.data_ptr(), B, T,
-                                               N.ptr(out_host), loss.data_ptr(), perm.data_ptr(), ibase, io.numel() - (ibase - io.data_ptr()),
-                                               wbase, ws.numel() - (wbase - ws.data_ptr()), float(loss_eps), N.stream_ptr(dev)),
-                    "ctn_convtasnet_loss_host")
+                                               N.ptr(out_host), loss.data_ptr(), perm.data_ptr(), ibase, ibytes, wbase, wbytes,
+                                               float(loss_eps), N.stream_ptr(dev)), "ctn_convtasnet_loss_host")
         self.last_launches = N.ctn_last_launch_count()
         return loss, perm
 
@@ -345,39 +307,40 @@ class ConvTasNet(nn.Module):
         n_dims = input.dim()
         if n_dims == 3:
             assert input.size(1) == 1, "input.size() is expected (?, 1, ?), but given {}".format(input.size())
+            if self.in_channels != 1:
+                raise ValueError("a model with in_channels={} takes the 4-D input (batch, 1, n_mics, T)".format(self.in_channels))
+            x = input
         elif n_dims == 4:
             # (batch, 1, n_mics, T) -> view (batch, n_mics, T) (conv_tasnet.py:138-141): the encoder consumes n_mics = in_channels
             # channels and the output gets the mic axis back (:167-168)
             assert input.size(1) == 1, "input.size() is expected (?, 1, ?, ?), but given {}".format(input.size())
             if input.size(2) != self.in_channels:
                 raise ValueError("n_mics={} does not match in_channels={}".format(input.size(2), self.in_channels))
-            if self.in_channels == 1:
-                out, latent = self._run(input.reshape(input.size(0), 1, input.size(3)), want_latent)
-                return out.unsqueeze(2), latent
-            return self._run_multichannel(input.reshape(input.size(0), input.size(2), input.size(3)), want_latent)
+            x = input.reshape(input.size(0), input.size(2), input.size(3))
         else:
             raise ValueError("Not support {} dimension input".format(n_dims))
-        if self.in_channels != 1:
-            raise ValueError("a model with in_channels={} takes the 4-D input (batch, 1, n_mics, T)".format(self.in_channels))
-        x = input.contiguous()
+        training = torch.is_grad_enabled() and any(p.requires_grad for p in self.parameters())
+        if training and self.in_channels > 1:
+            raise NotImplementedError("multichannel models (in_channels > 1) are forward only: call under torch.no_grad()")
+        x = x.contiguous()
         dev = N.require_cuda(x)
-        if torch.is_grad_enabled() and any(p.requires_grad for p in self.parameters()):
+        if training:
             # training: one autograd node over the whole model (ctn_convtasnet_fwd_train / ctn_convtasnet_bwd)
             if want_latent:
                 raise NotImplementedError("extract_latent under autograd is not built: call it under torch.no_grad()")
             from ._train import run_train
-            return run_train(self, x), None
-        B, _, T = x.shape
+            out = run_train(self, x)
+            return (out.unsqueeze(2) if n_dims == 4 else out), None
+        B, Cin, T = x.shape
         frames, _, _ = N.frames_of(T, self.kernel_size, self.stride)
         cfg = self.native_config()
         params, keep = self.native_params(dev)
         need = C.c_size_t(0)
         N.check(N.ctn_workspace_bytes(C.byref(cfg), B, T, C.byref(need)), "ctn_workspace_bytes")
-        ws = N.workspace(dev, need.value)
-        base = (ws.data_ptr() + 255) & ~255
-        out = torch.empty(B, self.n_sources, T, dtype=torch.float32, device=dev)
+        base, nbytes = N.aligned(N.workspace(dev, need.value))
+        out = torch.empty((B, self.n_sources, Cin, T) if n_dims == 4 else (B, self.n_sources, T), dtype=torch.float32, device=dev)
         latent = torch.empty(B, self.n_sources, self.n_basis, frames, dtype=torch.float32, device=dev) if want_latent else None
-        N.check(N.ctn_convtasnet_fwd(C.byref(cfg), C.byref(params), x.data_ptr(), B, T, out.data_ptr(), N.ptr(latent), base,
-                                     ws.numel() - (base - ws.data_ptr()), N.stream_ptr(dev)), "ctn_convtasnet_fwd")
+        N.check(N.ctn_convtasnet_fwd(C.byref(cfg), C.byref(params), x.data_ptr(), B, T, out.data_ptr(), N.ptr(latent), base, nbytes,
+                                     N.stream_ptr(dev)), "ctn_convtasnet_fwd")
         self.last_launches = N.ctn_last_launch_count()
         return out, latent

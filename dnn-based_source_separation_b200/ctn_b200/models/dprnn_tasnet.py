@@ -68,21 +68,20 @@ class Separator(nn.Module):
         B = w.shape[0]
         Nf, Bc, K, P = self.num_features, self.bottleneck_channels, self.chunk_size, self.hop_size
         ws_bytes = max(ctn_stage_workspace_bytes(Bc, Nf), ctn_stage_workspace_bytes(self.n_sources * Nf, Bc)) + 512
-        ws = N.workspace(dev, ws_bytes, tag="dprnn_stage")
-        base = (ws.data_ptr() + 255) & ~255
+        base, nbytes = N.aligned(N.workspace(dev, ws_bytes, tag="dprnn_stage"))
         st = N.stream_ptr(dev)
         x0 = torch.empty(B, Bc, pitch, dtype=torch.float32, device=dev)
         g0, b0 = self.norm1d.norm.weight, self.norm1d.norm.bias
         N.check(ctn_sep_head_fwd(w.data_ptr(), stats0.data_ptr(), g0.data_ptr(), b0.data_ptr(), self.bottleneck_conv1d.weight.data_ptr(),
                                  self.bottleneck_conv1d.bias.data_ptr(), x0.data_ptr(), B, Nf, Bc, frames, pitch, float(self.eps), self._math(),
-                                 base, ws.numel() - (base - ws.data_ptr()), st), "ctn_sep_head_fwd")
+                                 base, nbytes, st), "ctn_sep_head_fwd")
         pl, pr, S = self.segment_geometry(frames)
         z = torch.empty(B, S, K, Bc, dtype=torch.float32, device=dev)
         N.check(ctn_segment_fwd(x0.data_ptr(), z.data_ptr(), B, Bc, frames, pitch, K, P, pl, pr, 1, st), "ctn_segment_fwd")
         z = self.dprnn.forward_channels_last(z)
         y = x0  # reuse: (B, Bc, pitch)
         N.check(ctn_overlap_add_fwd(z.data_ptr(), y.data_ptr(), B, Bc, S, K, P, pl, frames, pitch, 1, st), "ctn_overlap_add_fwd")
-        return y, (base, ws.numel() - (base - ws.data_ptr()))
+        return y, (base, nbytes)
 
     def forward(self, input):
         """input (batch_size, num_features, n_frames) -> mask (batch_size, n_sources, num_features, n_frames)"""

@@ -47,7 +47,7 @@ class OnlineSeparator:
                 "ctn_online_state_bytes")
         self.state_bytes = need.value
         self._state = torch.empty(need.value + 256, dtype=torch.uint8, device=self.device)
-        self._base = (self._state.data_ptr() + 255) & ~255
+        self._base, _ = N.aligned(self._state)
         with torch.cuda.device(self.device):
             N.check(N.ctn_online_init(C.byref(self._cfg), C.byref(self._params), self.batch_size, self.max_chunk // self.stride,
                                       self._base, need.value, N.stream_ptr(self.device)), "ctn_online_init")

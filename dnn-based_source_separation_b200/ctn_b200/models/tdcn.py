@@ -90,9 +90,8 @@ class ResidualBlock1d(nn.Module):
     def native_params(self):
         """Device pointers in the order of ctn_block_params_t (include/ctn_b200.h)."""
         sep = self.separable_conv1d
-        n1, n2 = self.norm1d, sep.norm1d
-        g1, b1 = (n1.norm.weight, n1.norm.bias) if hasattr(n1, "norm") else (n1.gamma, n1.beta)
-        g2, b2 = (n2.norm.weight, n2.norm.bias) if hasattr(n2, "norm") else (n2.gamma, n2.beta)
+        g1, b1 = N.norm_affine(self.norm1d)
+        g2, b2 = N.norm_affine(sep.norm1d)
         out_w = sep.output_pointwise_conv1d.weight if self.dual_head else None
         out_b = sep.output_pointwise_conv1d.bias if self.dual_head else None
         return (self.bottleneck_conv1d.weight, self.bottleneck_conv1d.bias, self.nonlinear1d.weight, g1, b1,
@@ -147,31 +146,23 @@ def run_blocks(blocks, input, want_output, math=None):
     cfg2.num_layers = len(blocks)
     need = C.c_size_t(0)
     N.check(N.ctn_tcn_workspace_bytes(C.byref(cfg2), B, frames, C.byref(need)), "ctn_tcn_workspace_bytes")
-    ws = N.workspace(dev, need.value)
-    base = (ws.data_ptr() + 255) & ~255
+    base, nbytes = N.aligned(N.workspace(dev, need.value))
     skip = torch.empty(B, cfg.skip, frames, dtype=torch.float32, device=dev)
     out = torch.empty(B, cfg.bottleneck, frames, dtype=torch.float32, device=dev) if want_output else None
     N.check(N.ctn_tcn_blocks_fwd(C.byref(cfg2), arr, len(blocks), dil, x.data_ptr(), N.ptr(out), skip.data_ptr(), B, frames, base,
-                                 ws.numel() - (base - ws.data_ptr()), N.stream_ptr(dev)), "ctn_tcn_blocks_fwd")
+                                 nbytes, N.stream_ptr(dev)), "ctn_tcn_blocks_fwd")
     return out, skip
 
 
+def block_slots(residual_blocks):
+    """[((block index, block field name), tensor-or-None)] of a list of ResidualBlock1d, for N.build_params"""
+    return [((i, name), t) for i, blk in enumerate(residual_blocks) for name, t in zip(N.BLOCK_FIELDS, blk.native_params())]
+
+
 def block_param_array(residual_blocks, dev):
-    """ctypes array of ctn_block_params_t for a list of ResidualBlock1d; validates device / dtype / contiguity."""
-    arr = (N.BlockParams * len(residual_blocks))()
-    keep = []
-    for i, blk in enumerate(residual_blocks):
-        for name, t in zip(N.BLOCK_FIELDS, blk.native_params()):
-            if t is None:
-                setattr(arr[i], name, None)
-                continue
-            if t.device != dev or t.dtype != torch.float32:
-                raise RuntimeError("parameter {} must be float32 on {}".format(name, dev))
-            if not t.is_contiguous():
-                t = t.contiguous()
-                keep.append(t)
-            setattr(arr[i], name, t.data_ptr())
-    return arr, keep
+    """ctn_block_params_t array of a list of ResidualBlock1d -> (array pointer, keep)"""
+    p, keep = N.build_params(block_slots(residual_blocks), dev)
+    return p.blocks, keep
 
 
 class TimeDilatedConvNet(nn.Module):
@@ -219,9 +210,7 @@ class TimeDilatedConvNet(nn.Module):
         arr, keep = block_param_array(self.residual_blocks(), dev)
         need = C.c_size_t(0)
         N.check(N.ctn_tcn_workspace_bytes(C.byref(cfg), B, frames, C.byref(need)), "ctn_tcn_workspace_bytes")
-        ws = N.workspace(dev, need.value)
+        base, nbytes = N.aligned(N.workspace(dev, need.value))
         out = torch.empty(B, self.skip_channels, frames, dtype=torch.float32, device=dev)
-        base = (ws.data_ptr() + 255) & ~255
-        N.check(N.ctn_tcn_fwd(C.byref(cfg), arr, x.data_ptr(), out.data_ptr(), B, frames, base, ws.numel() - (base - ws.data_ptr()),
-                              N.stream_ptr(dev)), "ctn_tcn_fwd")
+        N.check(N.ctn_tcn_fwd(C.byref(cfg), arr, x.data_ptr(), out.data_ptr(), B, frames, base, nbytes, N.stream_ptr(dev)), "ctn_tcn_fwd")
         return out

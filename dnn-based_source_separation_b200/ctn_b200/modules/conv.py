@@ -43,8 +43,7 @@ class DepthwiseSeparableConv1d(nn.Module):
                 "ctn_depthwise_conv1d_fwd")
         y = torch.empty(B, M, To, dtype=torch.float32, device=dev)
         need = 4 * B * M * pitch + N.ctn_stage_workspace_bytes(M, Cc) + 16 * B + 4096
-        ws = N.workspace(dev, need, tag="conv")
-        base = (ws.data_ptr() + 255) & ~255
+        base, nbytes = N.aligned(N.workspace(dev, need, tag="conv"))
         N.check(N.ctn_pointwise_conv1d_fwd(u.data_ptr(), pw.weight.data_ptr(), N.ptr(pw.bias), y.data_ptr(), B, M, Cc, To, pitch,
-                                           resolve_math(self.math), base, ws.numel() - (base - ws.data_ptr()), st), "ctn_pointwise_conv1d_fwd")
+                                           resolve_math(self.math), base, nbytes, st), "ctn_pointwise_conv1d_fwd")
         return y
