@@ -195,3 +195,49 @@ int ctn_res_skip_fwd(const float* r, int Mt, const float* xin, float* xout, floa
 int ctn_bias_rows_fwd(float* y, const float* bias, int C, int B, int frames, int pitch, cudaStream_t st);
 // a block's [out_w; skip_w] (skip_w alone when it has no output head) -> wcat (Mt, H), stream-ordered device copies
 int ctn_block_wcat(const ctn_block_params_t& q, int Bc, int Sc, int H, float* wcat, cudaStream_t st);
+
+// Streaming and filter-bank gradient kernels of the training path (ctn_train.cu), one launcher each.  ctn_convtasnet_fwd_train /
+// ctn_convtasnet_bwd and the verification hook (ctn_probe.cu) launch them only through these, so both run the same grid shapes
+// and split counts.  Layout (B, C, pitch) as in the kernels' comments there; "+=" outputs accumulate with atomics.
+// y = y + bias[c] in place ; stats[b] += (sum, sumsq) of PReLU(y)
+int ctn_bias_prelu_stats(float* y, const float* bias, const float* slope, double* stats, int B, int C, int frames, int pitch,
+                         cudaStream_t st);
+// upre = dwconv(gLN1(PReLU(hpre; slope1))) + bd (P taps, dilation dil) ; stats2[b] += (sum, sumsq) of PReLU(upre; slope2)
+int ctn_dw_train_fwd(const float* hpre, float* upre, const float* g1, const float* b1, const float* wd, const float* bd,
+                     const float* slope1, const float* slope2, const double* stats1, double* stats2, int B, int C, int frames,
+                     int pitch, int P, int dil, int pad_left, double n1, float eps, cudaStream_t st);
+// y = gLN(act(pre)), act = PReLU(slope) or identity (slope == nullptr)
+int ctn_act_norm(const float* pre, float* y, const float* slope, const float* g, const float* bt, const double* stats, double n,
+                 float eps, int B, int C, int frames, int pitch, cudaStream_t st);
+// gLN (+ PReLU(slope) in front, slope nullable) backward: dy -> dpre (may alias dy); += dgamma, dbeta, dslope, dbias (the last
+// two nullable).  reduced: sums / dgamma / dbeta were already accumulated by the producer of dy (ctn_dw_bwd), only the apply runs.
+int ctn_gln_prelu_bwd(const float* dy, const float* pre, float* dpre, const float* slope, const float* g, const double* stats,
+                      double n, float eps, double* sums, float* dgamma, float* dbeta, float* dslope, float* dbias, int B, int C,
+                      int frames, int pitch, cudaStream_t st, bool reduced = false);
+// depthwise conv backward: d_hn, += dwd, and phase 1 of the gLN1 backward on d_hn (+= sums, dgamma, dbeta)
+int ctn_dw_bwd(const float* dupre, const float* hpre, float* dhn, const float* slope1, const float* g1, const float* b1,
+               const double* stats1, double n1, float eps, const float* wd, float* dwd, double* sums, float* dgamma, float* dbeta,
+               int B, int C, int frames, int pitch, int P, int dil, int pad_left, cudaStream_t st);
+// sigmoid-mask backward: dwhat (B, S*N, pitch) -> d_mpre in place ; dwprod (B, N, pitch) = sum_s dwhat * mask
+int ctn_mask_bwd(float* dwhat, const float* w, const float* mask, float* dwprod, int B, int S, int N, int frames, int pitch,
+                 cudaStream_t st);
+int ctn_prelu_apply(const float* x, float* y, const float* slope, int B, int C, int frames, int pitch, cudaStream_t st);
+// dpre = dy * (pre > 0 ? 1 : a) (may alias dy) ; dslope += sum_{pre <= 0} dy * pre
+int ctn_prelu_bwd(const float* dy, const float* pre, float* dpre, const float* slope, float* dslope, int B, int C, int frames,
+                  int pitch, cudaStream_t st);
+// dw = dw + dwprod, zeroed where !(w > 0) when relu
+int ctn_dw_combine(float* dw, const float* dwprod, const float* w, int relu, int B, int C, int frames, int pitch, cudaStream_t st);
+// dst[b][c] (+)= src[b][c] for c < C with independent batch strides (floats)
+int ctn_rows(float* dst, size_t dst_bs, const float* src, size_t src_bs, int C, int B, int accumulate, int frames, int pitch,
+             cudaStream_t st);
+// Wt (K, M) = W (M, K)^T
+int ctn_transpose(const float* W, float* Wt, int M, int K, cudaStream_t st);
+// dW (M, K) += sum dY X^T; rows [0, split_row) -> dWa, the rest -> dWb (nullable).  math: the model's numeric mode (fp32: the
+// FFMA split-K kernel; otherwise ctn_wgrad_wgmma)
+int ctn_wgrad(int math, const float* dy, size_t dy_bs, const float* x, size_t x_bs, float* dWa, float* dWb, int split_row, int M,
+              int K, int B, int frames, int pitch, cudaStream_t st);
+// filter-bank weight gradient dW (N, L) += sum_{r,f} act[r][n][f] * sig[r][f*stride + k - pad_left] (signal rows of T samples)
+int ctn_encdec_wgrad(const float* act, const float* sig, float* dW, int R, int N, int frames, int pitch, int T, int L, int stride,
+                     int pad_left, cudaStream_t st);
+// out[c] += sum_{b, t < frames} dy[b][c][t]
+int ctn_rowsum(const float* dy, size_t bs, int C, int B, int frames, int pitch, float* out, cudaStream_t st);

@@ -1,5 +1,6 @@
-// Verification hook (include/ctn_b200_probe.h): thin C entry points over the 1x1 contraction internals, so that tests can
-// compare one contraction with a high-precision reference.  No kernels here and no pipeline calls these.
+// Verification hook (include/ctn_b200_probe.h): thin C entry points over the 1x1 contraction internals and the training path's
+// launchers (ctn_internal.h), so that tests can compare one operation with a high-precision reference.  No kernels here and no
+// pipeline calls these.
 #include "ctn_internal.h"
 #include "ctn_b200_probe.h"
 
@@ -50,5 +51,76 @@ extern "C" size_t ctn_probe_pw_wimg_bytes(int M, int K, int math) { return ctn_p
 
 extern "C" int ctn_probe_wgrad(const float* dy, size_t dy_bs, const float* x, size_t x_bs, float* dWa, float* dWb, int split_row, int M,
                                int K, int B, int frames, int pitch, int math, ctn_stream_t stream) {
-  return ctn_wgrad_wgmma(dy, dy_bs, x, x_bs, dWa, dWb, split_row, M, K, B, frames, pitch, math, (cudaStream_t)stream);
+  return ctn_wgrad(math, dy, dy_bs, x, x_bs, dWa, dWb, split_row, M, K, B, frames, pitch, (cudaStream_t)stream);
+}
+
+extern "C" int ctn_probe_bias_prelu_stats(float* y, const float* bias, const float* slope, double* stats, int B, int C, int frames,
+                                          int pitch, ctn_stream_t stream) {
+  return ctn_bias_prelu_stats(y, bias, slope, stats, B, C, frames, pitch, (cudaStream_t)stream);
+}
+
+extern "C" int ctn_probe_dw_train_fwd(const float* hpre, float* upre, const float* g1, const float* b1, const float* wd,
+                                      const float* bd, const float* slope1, const float* slope2, const double* stats1, double* stats2,
+                                      int B, int C, int frames, int pitch, int P, int dil, int pad_left, double n1, float eps,
+                                      ctn_stream_t stream) {
+  return ctn_dw_train_fwd(hpre, upre, g1, b1, wd, bd, slope1, slope2, stats1, stats2, B, C, frames, pitch, P, dil, pad_left, n1, eps,
+                          (cudaStream_t)stream);
+}
+
+extern "C" int ctn_probe_act_norm(const float* pre, float* y, const float* slope, const float* g, const float* bt, const double* stats,
+                                  double n, float eps, int B, int C, int frames, int pitch, ctn_stream_t stream) {
+  return ctn_act_norm(pre, y, slope, g, bt, stats, n, eps, B, C, frames, pitch, (cudaStream_t)stream);
+}
+
+extern "C" int ctn_probe_gln_prelu_bwd(const float* dy, const float* pre, float* dpre, const float* slope, const float* g,
+                                       const double* stats, double n, float eps, double* sums, float* dgamma, float* dbeta,
+                                       float* dslope, float* dbias, int B, int C, int frames, int pitch, int reduced,
+                                       ctn_stream_t stream) {
+  return ctn_gln_prelu_bwd(dy, pre, dpre, slope, g, stats, n, eps, sums, dgamma, dbeta, dslope, dbias, B, C, frames, pitch,
+                           (cudaStream_t)stream, reduced != 0);
+}
+
+extern "C" int ctn_probe_dw_bwd(const float* dupre, const float* hpre, float* dhn, const float* slope1, const float* g1, const float* b1,
+                                const double* stats1, double n1, float eps, const float* wd, float* dwd, double* sums, float* dgamma,
+                                float* dbeta, int B, int C, int frames, int pitch, int P, int dil, int pad_left, ctn_stream_t stream) {
+  return ctn_dw_bwd(dupre, hpre, dhn, slope1, g1, b1, stats1, n1, eps, wd, dwd, sums, dgamma, dbeta, B, C, frames, pitch, P, dil,
+                    pad_left, (cudaStream_t)stream);
+}
+
+extern "C" int ctn_probe_mask_bwd(float* dwhat, const float* w, const float* mask, float* dwprod, int B, int S, int N, int frames,
+                                  int pitch, ctn_stream_t stream) {
+  return ctn_mask_bwd(dwhat, w, mask, dwprod, B, S, N, frames, pitch, (cudaStream_t)stream);
+}
+
+extern "C" int ctn_probe_prelu_apply(const float* x, float* y, const float* slope, int B, int C, int frames, int pitch,
+                                     ctn_stream_t stream) {
+  return ctn_prelu_apply(x, y, slope, B, C, frames, pitch, (cudaStream_t)stream);
+}
+
+extern "C" int ctn_probe_prelu_bwd(const float* dy, const float* pre, float* dpre, const float* slope, float* dslope, int B, int C,
+                                   int frames, int pitch, ctn_stream_t stream) {
+  return ctn_prelu_bwd(dy, pre, dpre, slope, dslope, B, C, frames, pitch, (cudaStream_t)stream);
+}
+
+extern "C" int ctn_probe_dw_combine(float* dw, const float* dwprod, const float* w, int relu, int B, int C, int frames, int pitch,
+                                    ctn_stream_t stream) {
+  return ctn_dw_combine(dw, dwprod, w, relu, B, C, frames, pitch, (cudaStream_t)stream);
+}
+
+extern "C" int ctn_probe_encdec_wgrad(const float* act, const float* sig, float* dW, int R, int N, int frames, int pitch, int T, int L,
+                                      int stride, int pad_left, ctn_stream_t stream) {
+  return ctn_encdec_wgrad(act, sig, dW, R, N, frames, pitch, T, L, stride, pad_left, (cudaStream_t)stream);
+}
+
+extern "C" int ctn_probe_rowsum(const float* dy, size_t bs, int C, int B, int frames, int pitch, float* out, ctn_stream_t stream) {
+  return ctn_rowsum(dy, bs, C, B, frames, pitch, out, (cudaStream_t)stream);
+}
+
+extern "C" int ctn_probe_rows(float* dst, size_t dst_bs, const float* src, size_t src_bs, int C, int B, int accumulate, int frames,
+                              int pitch, ctn_stream_t stream) {
+  return ctn_rows(dst, dst_bs, src, src_bs, C, B, accumulate, frames, pitch, (cudaStream_t)stream);
+}
+
+extern "C" int ctn_probe_transpose(const float* W, float* Wt, int M, int K, ctn_stream_t stream) {
+  return ctn_transpose(W, Wt, M, K, (cudaStream_t)stream);
 }

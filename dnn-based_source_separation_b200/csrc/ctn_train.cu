@@ -611,14 +611,151 @@ __global__ void __launch_bounds__(256) k_wgrad(const float* __restrict__ dy, siz
     }
 }
 
+}  // namespace
+
 // ================================================================================================================
-// host side
+// launchers (ctn_internal.h): the one launch of each kernel above, shared by the pipeline and the verification hook
 // ================================================================================================================
 #define LAUNCH_CHECK()      \
   do {                      \
     CTN_COUNT_LAUNCH();     \
     CTN_RETURN_IF_CUDA_ERR(); \
   } while (0)
+
+int ctn_bias_prelu_stats(float* y, const float* bias, const float* slope, double* stats, int B, int C, int frames, int pitch,
+                         cudaStream_t st) {
+  k_bias_prelu_stats<<<grid_cb(C, B), 256, 0, st>>>(y, bias, slope, stats, C, frames, pitch);
+  LAUNCH_CHECK();
+  return CTN_OK;
+}
+
+int ctn_dw_train_fwd(const float* hpre, float* upre, const float* g1, const float* b1, const float* wd, const float* bd,
+                     const float* slope1, const float* slope2, const double* stats1, double* stats2, int B, int C, int frames,
+                     int pitch, int P, int dil, int pad_left, double n1, float eps, cudaStream_t st) {
+  k_dw_train_fwd<<<grid_cb(C, B), 256, 0, st>>>(hpre, upre, g1, b1, wd, bd, slope1, slope2, stats1, stats2, C, frames, pitch, P, dil,
+                                                pad_left, n1, eps);
+  LAUNCH_CHECK();
+  return CTN_OK;
+}
+
+int ctn_act_norm(const float* pre, float* y, const float* slope, const float* g, const float* bt, const double* stats, double n,
+                 float eps, int B, int C, int frames, int pitch, cudaStream_t st) {
+  k_act_norm<<<grid_cb(C, B), 256, 0, st>>>(pre, y, slope, g, bt, stats, n, eps, C, frames, pitch);
+  LAUNCH_CHECK();
+  return CTN_OK;
+}
+
+int ctn_dw_bwd(const float* dupre, const float* hpre, float* dhn, const float* slope1, const float* g1, const float* b1,
+               const double* stats1, double n1, float eps, const float* wd, float* dwd, double* sums, float* dgamma, float* dbeta,
+               int B, int C, int frames, int pitch, int P, int dil, int pad_left, cudaStream_t st) {
+  k_dw_bwd<<<dim3(C, B), 256, 0, st>>>(dupre, hpre, dhn, slope1, g1, b1, stats1, n1, eps, wd, dwd, sums, dgamma, dbeta, C, frames,
+                                       pitch, P, dil, pad_left);
+  LAUNCH_CHECK();
+  return CTN_OK;
+}
+
+int ctn_mask_bwd(float* dwhat, const float* w, const float* mask, float* dwprod, int B, int S, int N, int frames, int pitch,
+                 cudaStream_t st) {
+  k_mask_bwd<<<grid_cb(N, B), 256, 0, st>>>(dwhat, w, mask, dwprod, S, N, frames, pitch);
+  LAUNCH_CHECK();
+  return CTN_OK;
+}
+
+int ctn_prelu_apply(const float* x, float* y, const float* slope, int B, int C, int frames, int pitch, cudaStream_t st) {
+  k_prelu_apply<<<grid_cb(C, B), 256, 0, st>>>(x, y, slope, C, frames, pitch);
+  LAUNCH_CHECK();
+  return CTN_OK;
+}
+
+int ctn_prelu_bwd(const float* dy, const float* pre, float* dpre, const float* slope, float* dslope, int B, int C, int frames,
+                  int pitch, cudaStream_t st) {
+  k_prelu_bwd<<<dim3(C, B), 256, 0, st>>>(dy, pre, dpre, slope, dslope, C, frames, pitch);
+  LAUNCH_CHECK();
+  return CTN_OK;
+}
+
+int ctn_dw_combine(float* dw, const float* dwprod, const float* w, int relu, int B, int C, int frames, int pitch, cudaStream_t st) {
+  k_dw_combine<<<grid_cb(C, B), 256, 0, st>>>(dw, dwprod, w, relu, C, frames, pitch);
+  LAUNCH_CHECK();
+  return CTN_OK;
+}
+
+int ctn_rows(float* dst, size_t dst_bs, const float* src, size_t src_bs, int C, int B, int accumulate, int frames, int pitch,
+             cudaStream_t st) {
+  k_rows<<<grid_cb(C, B), 256, 0, st>>>(dst, dst_bs, src, src_bs, C, accumulate, frames, pitch);
+  LAUNCH_CHECK();
+  return CTN_OK;
+}
+
+int ctn_transpose(const float* W, float* Wt, int M, int K, cudaStream_t st) {
+  k_transpose<<<(M * K + 255) / 256, 256, 0, st>>>(W, Wt, M, K);
+  LAUNCH_CHECK();
+  return CTN_OK;
+}
+
+// dW (M, K) += sum dY X^T; rows [0, split_row) -> dWa, the rest -> dWb (nullable).  Tensor cores (3xTF32 / TF32) unless the
+// numeric mode is plain fp32, where the FFMA split-K kernel runs.
+int ctn_wgrad(int math, const float* dy, size_t dy_bs, const float* x, size_t x_bs, float* dWa, float* dWb, int split_row, int M,
+              int K, int B, int frames, int pitch, cudaStream_t st) {
+  if (math != CTN_MATH_FP32)
+    return ctn_wgrad_wgmma(dy, dy_bs, x, x_bs, dWa, dWb, split_row, M, K, B, frames, pitch, math, st);
+  const int parts = dWb ? 2 : 1;
+  for (int part = 0; part < parts; ++part) {
+    const int r0 = part == 0 ? 0 : split_row, Mp = part == 0 ? (dWb ? split_row : M) : M - split_row;
+    float* dW = part == 0 ? dWa : dWb;
+    const float* dyp = dy + (size_t)r0 * pitch;
+    const int tiles = ((Mp + 63) / 64) * ((K + 63) / 64);
+    const long long total = (long long)B * ((frames + WG_T - 1) / WG_T);
+    long long splits = (4 * 148 + tiles - 1) / tiles;
+    if (splits > total) splits = total;
+    if (splits < 1) splits = 1;
+    const int upc = (int)((total + splits - 1) / splits);
+    splits = (total + upc - 1) / upc;
+    k_wgrad<<<dim3(tiles, (unsigned)splits), 256, 0, st>>>(dyp, dy_bs, x, x_bs, dW, Mp, K, B, frames, pitch, upc);
+    LAUNCH_CHECK();
+  }
+  return CTN_OK;
+}
+
+int ctn_encdec_wgrad(const float* act, const float* sig, float* dW, int R, int N, int frames, int pitch, int T, int L, int stride,
+                     int pad_left, cudaStream_t st) {
+  if (L <= ENCDEC_MAX_L) {
+    int gy = (4 * 148 + N - 1) / N;
+    if (gy > R) gy = R;
+    if (gy < 1) gy = 1;
+    k_encdec_wgrad<<<dim3(N, gy), 256, 0, st>>>(act, sig, dW, R, N, frames, pitch, T, L, stride, pad_left);
+  } else {
+    k_encdec_wgrad_generic<<<dim3(L, N), 256, 0, st>>>(act, sig, dW, R, N, frames, pitch, T, L, stride, pad_left);
+  }
+  LAUNCH_CHECK();
+  return CTN_OK;
+}
+
+int ctn_rowsum(const float* dy, size_t bs, int C, int B, int frames, int pitch, float* out, cudaStream_t st) {
+  k_rowsum<<<dim3(C, B), 256, 0, st>>>(dy, bs, frames, pitch, out);
+  LAUNCH_CHECK();
+  return CTN_OK;
+}
+
+// gLN (+ optional PReLU in front) backward: dy (B,C,pitch) -> dpre (may alias dy); accumulates dgamma, dbeta, dslope, dbias
+int ctn_gln_prelu_bwd(const float* dy, const float* pre, float* dpre, const float* slope, const float* g, const double* stats,
+                      double n, float eps, double* sums, float* dgamma, float* dbeta, float* dslope, float* dbias, int B, int C,
+                      int frames, int pitch, cudaStream_t st, bool reduced) {
+  if (!reduced) {  // phase 1 (skipped when the producer of dy already accumulated sums / dgamma / dbeta)
+    cudaError_t e = cudaMemsetAsync(sums, 0, sizeof(double) * 2 * B, st);
+    if (e != cudaSuccess) return (int)e;
+    k_gln_bwd_reduce<<<dim3(C, B), 256, 0, st>>>(dy, pre, slope, g, stats, n, eps, sums, dgamma, dbeta, C, frames, pitch);
+    LAUNCH_CHECK();
+  }
+  k_gln_prelu_bwd_apply<<<dim3(C, B), 256, 0, st>>>(dy, pre, dpre, slope, g, stats, n, eps, sums, dslope, dbias, C, frames, pitch);
+  LAUNCH_CHECK();
+  return CTN_OK;
+}
+
+// ================================================================================================================
+// pipelines
+// ================================================================================================================
+namespace {
 
 struct TrainWs {
   // ---- saved by the forward
@@ -726,71 +863,6 @@ int gemm_raw(const ctn_config_t* c, TrainWs& ws, const float* W, int M, int K, c
   return ctn_pw(a, PRO_NONE, EPI_RAW, c->math, ws.wimg, st);
 }
 
-int transpose(const float* W, float* Wt, int M, int K, cudaStream_t st) {
-  k_transpose<<<(M * K + 255) / 256, 256, 0, st>>>(W, Wt, M, K);
-  LAUNCH_CHECK();
-  return CTN_OK;
-}
-
-// dW (M, K) += sum dY X^T; rows [0, split_row) -> dWa, the rest -> dWb (nullable).  Tensor cores (3xTF32 / TF32) unless the
-// configured mode is plain fp32, where the FFMA split-K kernel runs.
-int wgrad(const ctn_config_t* c, const float* dy, size_t dy_bs, const float* x, size_t x_bs, float* dWa, float* dWb, int split_row,
-          int M, int K, int B, int frames, int pitch, cudaStream_t st) {
-  if (c->math != CTN_MATH_FP32)
-    return ctn_wgrad_wgmma(dy, dy_bs, x, x_bs, dWa, dWb, split_row, M, K, B, frames, pitch, c->math, st);
-  const int parts = dWb ? 2 : 1;
-  for (int part = 0; part < parts; ++part) {
-    const int r0 = part == 0 ? 0 : split_row, Mp = part == 0 ? (dWb ? split_row : M) : M - split_row;
-    float* dW = part == 0 ? dWa : dWb;
-    const float* dyp = dy + (size_t)r0 * pitch;
-    const int tiles = ((Mp + 63) / 64) * ((K + 63) / 64);
-    const long long total = (long long)B * ((frames + WG_T - 1) / WG_T);
-    long long splits = (4 * 148 + tiles - 1) / tiles;
-    if (splits > total) splits = total;
-    if (splits < 1) splits = 1;
-    const int upc = (int)((total + splits - 1) / splits);
-    splits = (total + upc - 1) / upc;
-    k_wgrad<<<dim3(tiles, (unsigned)splits), 256, 0, st>>>(dyp, dy_bs, x, x_bs, dW, Mp, K, B, frames, pitch, upc);
-    LAUNCH_CHECK();
-  }
-  return CTN_OK;
-}
-
-int encdec_wgrad(const float* act, const float* sig, float* dW, int R, int N, int frames, int pitch, int T, int L, int stride,
-                 int pad_left, cudaStream_t st) {
-  if (L <= ENCDEC_MAX_L) {
-    int gy = (4 * 148 + N - 1) / N;
-    if (gy > R) gy = R;
-    if (gy < 1) gy = 1;
-    k_encdec_wgrad<<<dim3(N, gy), 256, 0, st>>>(act, sig, dW, R, N, frames, pitch, T, L, stride, pad_left);
-  } else {
-    k_encdec_wgrad_generic<<<dim3(L, N), 256, 0, st>>>(act, sig, dW, R, N, frames, pitch, T, L, stride, pad_left);
-  }
-  LAUNCH_CHECK();
-  return CTN_OK;
-}
-
-int rowsum(const float* dy, size_t bs, int C, int B, int frames, int pitch, float* out, cudaStream_t st) {
-  k_rowsum<<<dim3(C, B), 256, 0, st>>>(dy, bs, frames, pitch, out);
-  LAUNCH_CHECK();
-  return CTN_OK;
-}
-
-// gLN (+ optional PReLU in front) backward: dy (B,C,pitch) -> dpre (may alias dy); accumulates dgamma, dbeta, dslope, dbias
-int gln_prelu_bwd(const float* dy, const float* pre, float* dpre, const float* slope, const float* g, const double* stats,
-                  double n, float eps, double* sums, float* dgamma, float* dbeta, float* dslope, float* dbias, int B, int C,
-                  int frames, int pitch, cudaStream_t st, bool reduced = false) {
-  if (!reduced) {  // phase 1 (skipped when the producer of dy already accumulated sums / dgamma / dbeta)
-    cudaError_t e = cudaMemsetAsync(sums, 0, sizeof(double) * 2 * B, st);
-    if (e != cudaSuccess) return (int)e;
-    k_gln_bwd_reduce<<<dim3(C, B), 256, 0, st>>>(dy, pre, slope, g, stats, n, eps, sums, dgamma, dbeta, C, frames, pitch);
-    LAUNCH_CHECK();
-  }
-  k_gln_prelu_bwd_apply<<<dim3(C, B), 256, 0, st>>>(dy, pre, dpre, slope, g, stats, n, eps, sums, dslope, dbias, C, frames, pitch);
-  LAUNCH_CHECK();
-  return CTN_OK;
-}
-
 }  // namespace
 
 extern "C" int ctn_train_workspace_bytes(const ctn_config_t* cfg, int batch, int T, size_t* bytes) {
@@ -857,8 +929,7 @@ extern "C" int ctn_convtasnet_fwd_train(const ctn_config_t* c, const ctn_params_
     // h_pre = W1 x + b1 ; stats1 of PReLU(h_pre)
     if (c->math == CTN_MATH_FP32) {
       CTN_TRY(gemm_raw(c, ws, q.bottleneck_w, H, Bc, ws.x[i], ws.hpre[i], B, frames, pitch, st));
-      k_bias_prelu_stats<<<grid_cb(H, B), 256, 0, st>>>(ws.hpre[i], q.bottleneck_b, q.prelu1, st1, H, frames, pitch);
-      LAUNCH_CHECK();
+      CTN_TRY(ctn_bias_prelu_stats(ws.hpre[i], q.bottleneck_b, q.prelu1, st1, B, H, frames, pitch, st));
     } else {  // bias, PReLU statistics fused into the contraction's epilogue; the PRE-activation is what gets stored
       PwArgs a;
       memset(&a, 0, sizeof(a));
@@ -867,12 +938,10 @@ extern "C" int ctn_convtasnet_fwd_train(const ctn_config_t* c, const ctn_params_
       CTN_TRY(ctn_pw(a, PRO_NONE, EPI_H, c->math, ws.wimg, st));
     }
     // u_pre = dwconv(gLN1(PReLU(h_pre))) + bd ; stats2 of PReLU(u_pre)
-    k_dw_train_fwd<<<grid_cb(H, B), 256, 0, st>>>(ws.hpre[i], ws.upre[i], q.norm1_g, q.norm1_b, q.dw_w, q.dw_b, q.prelu1, q.prelu2,
-                                                  st1, st2, H, frames, pitch, c->sep_kernel, dil, pad_left, nH, c->eps_tcn);
-    LAUNCH_CHECK();
+    CTN_TRY(ctn_dw_train_fwd(ws.hpre[i], ws.upre[i], q.norm1_g, q.norm1_b, q.dw_w, q.dw_b, q.prelu1, q.prelu2, st1, st2, B, H, frames,
+                             pitch, c->sep_kernel, dil, pad_left, nH, c->eps_tcn, st));
     // un = gLN2(PReLU(u_pre)) ; r = [Wo; Ws] un
-    k_act_norm<<<grid_cb(H, B), 256, 0, st>>>(ws.upre[i], ws.T1, q.prelu2, q.norm2_g, q.norm2_b, st2, nH, c->eps_tcn, H, frames, pitch);
-    LAUNCH_CHECK();
+    CTN_TRY(ctn_act_norm(ws.upre[i], ws.T1, q.prelu2, q.norm2_g, q.norm2_b, st2, nH, c->eps_tcn, B, H, frames, pitch, st));
     const int Mt = has_out ? Bc + Sc : Sc;
     CTN_TRY(ctn_block_wcat(q, Bc, Sc, H, ws.Wcat, st));
     CTN_TRY(gemm_raw(c, ws, ws.Wcat, Mt, H, ws.T1, ws.r, B, frames, pitch, st));
@@ -918,23 +987,19 @@ extern "C" int ctn_convtasnet_bwd(const ctn_config_t* c, const ctn_params_t* p, 
 
   // ---- decoder (filterbank.py:243-249): d_what = conv1d(d_out; Wd) (the transposed conv's adjoint), dWd
   CTN_TRY(ctn_encoder_fwd(d_out, p->dec_w, ws.dwhat, B * S, T, pl, pr, N, L, c->stride, 0, pitch, nullptr, stream));
-  CTN_TRY(encdec_wgrad(ws.what, d_out, G(grads->dec_w), B * S, N, frames, pitch, T, L, c->stride, pl, st));
+  CTN_TRY(ctn_encdec_wgrad(ws.what, d_out, G(grads->dec_w), B * S, N, frames, pitch, T, L, c->stride, pl, st));
   // ---- w_hat = w * sigmoid(m_pre): d_mpre (in place), d_wprod
-  k_mask_bwd<<<grid_cb(N, B), 256, 0, st>>>(ws.dwhat, ws.w, ws.mask, ws.nC, S, N, frames, pitch);
-  LAUNCH_CHECK();
+  CTN_TRY(ctn_mask_bwd(ws.dwhat, ws.w, ws.mask, ws.nC, B, S, N, frames, pitch, st));
   // ---- mask conv (conv_tasnet.py:341,374): dWm, dbm, d_sp = Wm^T d_mpre
-  k_prelu_apply<<<grid_cb(Sc, B), 256, 0, st>>>(ws.skip, ws.sp, p->prelu_out, Sc, frames, pitch);
-  LAUNCH_CHECK();
-  CTN_TRY(wgrad(c, ws.dwhat, bsSN, ws.sp, bsSc, G(grads->mask_w), nullptr, 0, S * N, Sc, B, frames, pitch, st));
-  CTN_TRY(rowsum(ws.dwhat, bsSN, S * N, B, frames, pitch, G(grads->mask_b), st));
-  CTN_TRY(transpose(p->mask_w, ws.Wt, S * N, Sc, st));
+  CTN_TRY(ctn_prelu_apply(ws.skip, ws.sp, p->prelu_out, B, Sc, frames, pitch, st));
+  CTN_TRY(ctn_wgrad(c->math, ws.dwhat, bsSN, ws.sp, bsSc, G(grads->mask_w), nullptr, 0, S * N, Sc, B, frames, pitch, st));
+  CTN_TRY(ctn_rowsum(ws.dwhat, bsSN, S * N, B, frames, pitch, G(grads->mask_b), st));
+  CTN_TRY(ctn_transpose(p->mask_w, ws.Wt, S * N, Sc, st));
   CTN_TRY(gemm_raw(c, ws, ws.Wt, Sc, S * N, ws.dwhat, ws.dsp, B, frames, pitch, st));
   // ---- PReLU on the skip sum (conv_tasnet.py:340,373): dS (the gradient of EVERY block's skip output)
-  k_prelu_bwd<<<dim3(Sc, B), 256, 0, st>>>(ws.dsp, ws.skip, ws.dS, p->prelu_out, G(grads->prelu_out), Sc, frames, pitch);
-  LAUNCH_CHECK();
+  CTN_TRY(ctn_prelu_bwd(ws.dsp, ws.skip, ws.dS, p->prelu_out, G(grads->prelu_out), B, Sc, frames, pitch, st));
   // dcat rows [Bc, Bc+Sc) = dS for all blocks with an output head; rows [0,Bc) = gradient of the block's residual output
-  k_rows<<<grid_cb(Sc, B), 256, 0, st>>>(ws.dcat + bsBc, bsCat, ws.dS, bsSc, Sc, 0, frames, pitch);
-  LAUNCH_CHECK();
+  CTN_TRY(ctn_rows(ws.dcat + bsBc, bsCat, ws.dS, bsSc, Sc, B, 0, frames, pitch, st));
   // ---- residual blocks, last to first
   for (int i = RX - 1; i >= 0; --i) {
     const ctn_block_params_t& q = p->blocks[i];
@@ -948,59 +1013,51 @@ extern "C" int ctn_convtasnet_bwd(const ctn_config_t* c, const ctn_params_t* p, 
     const float* dY = has_out ? ws.dcat : ws.dS;  // (B, Mt, pitch)
     const size_t dY_bs = has_out ? bsCat : bsSc;
     // un = gLN2(PReLU(u_pre)) recomputed for the weight gradients of the two heads
-    k_act_norm<<<grid_cb(H, B), 256, 0, st>>>(ws.upre[i], ws.T1, q.prelu2, q.norm2_g, q.norm2_b, st2, nH, c->eps_tcn, H, frames, pitch);
-    LAUNCH_CHECK();
+    CTN_TRY(ctn_act_norm(ws.upre[i], ws.T1, q.prelu2, q.norm2_g, q.norm2_b, st2, nH, c->eps_tcn, B, H, frames, pitch, st));
     if (has_out) {
-      CTN_TRY(wgrad(c, dY, dY_bs, ws.T1, bsH, G(gq.out_w), G(gq.skip_w), Bc, Bc + Sc, H, B, frames, pitch, st));
-      CTN_TRY(rowsum(dY, dY_bs, Bc, B, frames, pitch, G(gq.out_b), st));
+      CTN_TRY(ctn_wgrad(c->math, dY, dY_bs, ws.T1, bsH, G(gq.out_w), G(gq.skip_w), Bc, Bc + Sc, H, B, frames, pitch, st));
+      CTN_TRY(ctn_rowsum(dY, dY_bs, Bc, B, frames, pitch, G(gq.out_b), st));
     } else {
-      CTN_TRY(wgrad(c, dY, dY_bs, ws.T1, bsH, G(gq.skip_w), nullptr, 0, Sc, H, B, frames, pitch, st));
+      CTN_TRY(ctn_wgrad(c->math, dY, dY_bs, ws.T1, bsH, G(gq.skip_w), nullptr, 0, Sc, H, B, frames, pitch, st));
     }
     const float* dYs = dY + (has_out ? bsBc : 0);
-    CTN_TRY(rowsum(dYs, dY_bs, Sc, B, frames, pitch, G(gq.skip_b), st));
+    CTN_TRY(ctn_rowsum(dYs, dY_bs, Sc, B, frames, pitch, G(gq.skip_b), st));
     // d_un = [Wo; Ws]^T dY
     CTN_TRY(ctn_block_wcat(q, Bc, Sc, H, ws.Wcat, st));
-    CTN_TRY(transpose(ws.Wcat, ws.Wt, Mt, H, st));
+    CTN_TRY(ctn_transpose(ws.Wcat, ws.Wt, Mt, H, st));
     CTN_TRY(gemm_raw(c, ws, ws.Wt, H, Mt, dY, ws.G1, B, frames, pitch, st));
     // gLN2 + PReLU2 backward -> d_u_pre (G1 in place); dgamma2, dbeta2, da2, d(bd)
-    CTN_TRY(gln_prelu_bwd(ws.G1, ws.upre[i], ws.G1, q.prelu2, q.norm2_g, st2, nH, c->eps_tcn, ws.sums, G(gq.norm2_g), G(gq.norm2_b),
-                          G(gq.prelu2), G(gq.dw_b), B, H, frames, pitch, st));
+    CTN_TRY(ctn_gln_prelu_bwd(ws.G1, ws.upre[i], ws.G1, q.prelu2, q.norm2_g, st2, nH, c->eps_tcn, ws.sums, G(gq.norm2_g),
+                              G(gq.norm2_b), G(gq.prelu2), G(gq.dw_b), B, H, frames, pitch, st));
     // depthwise conv backward -> d_hn (G2), d(wd); fused: phase 1 of the gLN1 backward (per-sample sums, dgamma1, dbeta1)
     {
       cudaError_t e = cudaMemsetAsync(ws.sums, 0, sizeof(double) * 2 * B, st);
       if (e != cudaSuccess) return (int)e;
     }
-    k_dw_bwd<<<dim3(H, B), 256, 0, st>>>(ws.G1, ws.hpre[i], ws.G2, q.prelu1, q.norm1_g, q.norm1_b, st1, nH, c->eps_tcn, q.dw_w,
-                                         G(gq.dw_w), ws.sums, G(gq.norm1_g), G(gq.norm1_b), H, frames, pitch, c->sep_kernel, dil,
-                                         pad_left);
-    LAUNCH_CHECK();
+    CTN_TRY(ctn_dw_bwd(ws.G1, ws.hpre[i], ws.G2, q.prelu1, q.norm1_g, q.norm1_b, st1, nH, c->eps_tcn, q.dw_w, G(gq.dw_w), ws.sums,
+                       G(gq.norm1_g), G(gq.norm1_b), B, H, frames, pitch, c->sep_kernel, dil, pad_left, st));
     // gLN1 + PReLU1 backward, phase 2 -> d_h_pre (G2 in place); da1, db1
-    CTN_TRY(gln_prelu_bwd(ws.G2, ws.hpre[i], ws.G2, q.prelu1, q.norm1_g, st1, nH, c->eps_tcn, ws.sums, G(gq.norm1_g), G(gq.norm1_b),
-                          G(gq.prelu1), G(gq.bottleneck_b), B, H, frames, pitch, st, /*reduced=*/true));
+    CTN_TRY(ctn_gln_prelu_bwd(ws.G2, ws.hpre[i], ws.G2, q.prelu1, q.norm1_g, st1, nH, c->eps_tcn, ws.sums, G(gq.norm1_g),
+                              G(gq.norm1_b), G(gq.prelu1), G(gq.bottleneck_b), B, H, frames, pitch, st, /*reduced=*/true));
     // bottleneck 1x1: dW1 = d_h_pre x_i^T ; d_x_i = W1^T d_h_pre (+ residual path)
-    CTN_TRY(wgrad(c, ws.G2, bsH, ws.x[i], bsBc, G(gq.bottleneck_w), nullptr, 0, H, Bc, B, frames, pitch, st));
-    CTN_TRY(transpose(q.bottleneck_w, ws.Wt, H, Bc, st));
+    CTN_TRY(ctn_wgrad(c->math, ws.G2, bsH, ws.x[i], bsBc, G(gq.bottleneck_w), nullptr, 0, H, Bc, B, frames, pitch, st));
+    CTN_TRY(ctn_transpose(q.bottleneck_w, ws.Wt, H, Bc, st));
     CTN_TRY(gemm_raw(c, ws, ws.Wt, Bc, H, ws.G2, ws.dxtmp, B, frames, pitch, st));
-    k_rows<<<grid_cb(Bc, B), 256, 0, st>>>(ws.dcat, bsCat, ws.dxtmp, bsBc, Bc, has_out ? 1 : 0, frames, pitch);
-    LAUNCH_CHECK();
+    CTN_TRY(ctn_rows(ws.dcat, bsCat, ws.dxtmp, bsBc, Bc, B, has_out ? 1 : 0, frames, pitch, st));
   }
   // ---- head (conv_tasnet.py:333-335,370-371): x_0 = Wb gLN0(w) + bb.   d_x0 = dcat rows [0,Bc)
-  k_act_norm<<<grid_cb(N, B), 256, 0, st>>>(ws.w, ws.nA, nullptr, p->norm0_g, p->norm0_b, ws.stats0, (double)N * frames, c->eps, N,
-                                            frames, pitch);
-  LAUNCH_CHECK();
-  CTN_TRY(wgrad(c, ws.dcat, bsCat, ws.nA, bsN, G(grads->bn_w), nullptr, 0, Bc, N, B, frames, pitch, st));
-  CTN_TRY(rowsum(ws.dcat, bsCat, Bc, B, frames, pitch, G(grads->bn_b), st));
+  CTN_TRY(ctn_act_norm(ws.w, ws.nA, nullptr, p->norm0_g, p->norm0_b, ws.stats0, (double)N * frames, c->eps, B, N, frames, pitch, st));
+  CTN_TRY(ctn_wgrad(c->math, ws.dcat, bsCat, ws.nA, bsN, G(grads->bn_w), nullptr, 0, Bc, N, B, frames, pitch, st));
+  CTN_TRY(ctn_rowsum(ws.dcat, bsCat, Bc, B, frames, pitch, G(grads->bn_b), st));
   // d_wn = Wb^T d_x0 (the operand of the contraction must be dense (B, K, pitch): copy the rows out of dcat)
-  k_rows<<<grid_cb(Bc, B), 256, 0, st>>>(ws.dxtmp, bsBc, ws.dcat, bsCat, Bc, 0, frames, pitch);
-  LAUNCH_CHECK();
-  CTN_TRY(transpose(p->bn_w, ws.Wt, Bc, N, st));
+  CTN_TRY(ctn_rows(ws.dxtmp, bsBc, ws.dcat, bsCat, Bc, B, 0, frames, pitch, st));
+  CTN_TRY(ctn_transpose(p->bn_w, ws.Wt, Bc, N, st));
   CTN_TRY(gemm_raw(c, ws, ws.Wt, N, Bc, ws.dxtmp, ws.nB, B, frames, pitch, st));
   // gLN0 backward -> d_w (norm path) ; + product path ; ReLU mask of the encoder if any
-  CTN_TRY(gln_prelu_bwd(ws.nB, ws.w, ws.nB, nullptr, p->norm0_g, ws.stats0, (double)N * frames, c->eps, ws.sums, G(grads->norm0_g),
-                        G(grads->norm0_b), nullptr, nullptr, B, N, frames, pitch, st));
-  k_dw_combine<<<grid_cb(N, B), 256, 0, st>>>(ws.nB, ws.nC, ws.w, c->enc_relu, N, frames, pitch);
-  LAUNCH_CHECK();
+  CTN_TRY(ctn_gln_prelu_bwd(ws.nB, ws.w, ws.nB, nullptr, p->norm0_g, ws.stats0, (double)N * frames, c->eps, ws.sums,
+                            G(grads->norm0_g), G(grads->norm0_b), nullptr, nullptr, B, N, frames, pitch, st));
+  CTN_TRY(ctn_dw_combine(ws.nB, ws.nC, ws.w, c->enc_relu, B, N, frames, pitch, st));
   // ---- encoder (filterbank.py:212,222): dWe
-  CTN_TRY(encdec_wgrad(ws.nB, x, G(grads->enc_w), B, N, frames, pitch, T, L, c->stride, pl, st));
+  CTN_TRY(ctn_encdec_wgrad(ws.nB, x, G(grads->enc_w), B, N, frames, pitch, T, L, c->stride, pl, st));
   return CTN_OK;
 }

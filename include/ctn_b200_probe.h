@@ -1,9 +1,11 @@
-/* ctn_b200_probe.h -- verification hook: the library's 1x1 contraction kernels called one at a time.
+/* ctn_b200_probe.h -- verification hook: the library's 1x1 contraction kernels and the training path's streaming kernels
+ * called one at a time.
  *
- * The pipelines reach the pointwise contraction kernels (ctn_wgmma.cu, ctn_tcn_simt.cu) and the weight-gradient kernel
- * (ctn_wgrad_wgmma.cu) only inside whole models, where normalisations and nonlinearities dilute a kernel's error before any
- * output is compared.  These entry points expose those kernels directly so that a test can compare one contraction with a
- * high-precision reference.  No pipeline calls them; they add no kernels.  Conventions as in ctn_b200.h.
+ * The pipelines reach the pointwise contraction kernels (ctn_wgmma.cu, ctn_tcn_simt.cu), the weight-gradient kernels
+ * (ctn_wgrad_wgmma.cu, ctn_train.cu) and the training path's streaming kernels (ctn_train.cu) only inside whole models, where
+ * normalisations and nonlinearities dilute a kernel's error before any output is compared.  These entry points expose those
+ * kernels directly so that a test can compare one operation with a high-precision reference.  No pipeline calls them; they add
+ * no kernels.  Conventions as in ctn_b200.h.
  */
 #ifndef CTN_B200_PROBE_H
 #define CTN_B200_PROBE_H
@@ -69,9 +71,55 @@ int ctn_probe_pw(const ctn_pw_probe_t* p, int pro, int epi, int math, int route,
 /* bytes of the weight image of an (M, K) contraction */
 size_t ctn_probe_pw_wimg_bytes(int M, int K, int math);
 /* dW (M, K) += sum_{b, t < frames} dY[b][m][t] X[b][k][t]: rows [0, split_row) to dWa, the rest to dWb (nullable);
- * dY_b = dy + b * dy_bs, X_b = x + b * x_bs (floats).  dWa / dWb must be zeroed by the caller. */
+ * dY_b = dy + b * dy_bs, X_b = x + b * x_bs (floats).  dWa / dWb must be zeroed by the caller.  The training backward's launcher:
+ * CTN_MATH_FP32 runs the FFMA split-K kernel, the other modes the wgmma kernel. */
 int ctn_probe_wgrad(const float* dy, size_t dy_bs, const float* x, size_t x_bs, float* dWa, float* dWb, int split_row, int M, int K,
                     int B, int frames, int pitch, int math, ctn_stream_t stream);
+
+/* The training path's streaming and filter-bank gradient kernels (ctn_train.cu), one operation per entry point, through the same
+ * launchers ctn_convtasnet_fwd_train / ctn_convtasnet_bwd use.  Tensors are (B, C, pitch) floats with pitch % 4 == 0 and
+ * 16-byte-aligned rows; stats / sums are (B, 2) doubles; "+=" outputs are accumulated, never cleared.  Nullable pointers are
+ * the ones the pipeline passes as null. */
+/* y = y + bias[c] in place ; stats[b] += (sum, sumsq) of PReLU(y; slope) over t < frames */
+int ctn_probe_bias_prelu_stats(float* y, const float* bias, const float* slope, double* stats, int B, int C, int frames, int pitch,
+                               ctn_stream_t stream);
+/* upre = dwconv(gLN1(PReLU(hpre; slope1)), wd (C, P), dilation dil, pad_left) + bd ; stats2[b] += (sum, sumsq) of PReLU(upre; slope2).
+ * gLN1 from stats1 over n1 elements. */
+int ctn_probe_dw_train_fwd(const float* hpre, float* upre, const float* g1, const float* b1, const float* wd, const float* bd,
+                           const float* slope1, const float* slope2, const double* stats1, double* stats2, int B, int C, int frames,
+                           int pitch, int P, int dil, int pad_left, double n1, float eps, ctn_stream_t stream);
+/* y = gLN(act(pre)) from stats over n elements; act = PReLU(slope), identity when slope is null */
+int ctn_probe_act_norm(const float* pre, float* y, const float* slope, const float* g, const float* bt, const double* stats, double n,
+                       float eps, int B, int C, int frames, int pitch, ctn_stream_t stream);
+/* gLN (+ PReLU) backward: dpre (may alias dy); += dgamma, dbeta (phase 1, and sums = per-sample (sum g dy, sum g dy xhat), cleared
+ * first) unless reduced; += dslope, dbias (both nullable) */
+int ctn_probe_gln_prelu_bwd(const float* dy, const float* pre, float* dpre, const float* slope, const float* g, const double* stats,
+                            double n, float eps, double* sums, float* dgamma, float* dbeta, float* dslope, float* dbias, int B, int C,
+                            int frames, int pitch, int reduced, ctn_stream_t stream);
+/* depthwise backward: dhn = dwconv^T(dupre) ; dwd += taps' gradients ; phase 1 of the gLN1 backward on dhn (+= sums, dgamma, dbeta) */
+int ctn_probe_dw_bwd(const float* dupre, const float* hpre, float* dhn, const float* slope1, const float* g1, const float* b1,
+                     const double* stats1, double n1, float eps, const float* wd, float* dwd, double* sums, float* dgamma, float* dbeta,
+                     int B, int C, int frames, int pitch, int P, int dil, int pad_left, ctn_stream_t stream);
+/* sigmoid-mask backward: dwhat (B, S*N, pitch) -> d_mpre in place ; dwprod (B, N, pitch) = sum_s dwhat * mask */
+int ctn_probe_mask_bwd(float* dwhat, const float* w, const float* mask, float* dwprod, int B, int S, int N, int frames, int pitch,
+                       ctn_stream_t stream);
+int ctn_probe_prelu_apply(const float* x, float* y, const float* slope, int B, int C, int frames, int pitch, ctn_stream_t stream);
+/* dpre = dy * (pre > 0 ? 1 : slope) (may alias dy) ; dslope += sum_{pre <= 0} dy * pre */
+int ctn_probe_prelu_bwd(const float* dy, const float* pre, float* dpre, const float* slope, float* dslope, int B, int C, int frames,
+                        int pitch, ctn_stream_t stream);
+/* dw = dw + dwprod, and 0 where !(w > 0) when relu */
+int ctn_probe_dw_combine(float* dw, const float* dwprod, const float* w, int relu, int B, int C, int frames, int pitch,
+                         ctn_stream_t stream);
+/* dW (N, L) += sum_{r < R, f < frames} act[r][n][f] * sig[r][f*stride + k - pad_left] (0 outside [0, T)); act (R, N, pitch) */
+int ctn_probe_encdec_wgrad(const float* act, const float* sig, float* dW, int R, int N, int frames, int pitch, int T, int L,
+                           int stride, int pad_left, ctn_stream_t stream);
+/* out[c] += sum_{b, t < frames} dy[b * bs + c * pitch + t] */
+int ctn_probe_rowsum(const float* dy, size_t bs, int C, int B, int frames, int pitch, float* out, ctn_stream_t stream);
+/* dst[b][c] (+)= src[b][c], c < C, batch strides dst_bs / src_bs floats; columns [frames, pitch) of dst are written as 0 */
+int ctn_probe_rows(float* dst, size_t dst_bs, const float* src, size_t src_bs, int C, int B, int accumulate, int frames, int pitch,
+                   ctn_stream_t stream);
+/* Wt (K, M) = W (M, K)^T */
+int ctn_probe_transpose(const float* W, float* Wt, int M, int K, ctn_stream_t stream);
 
 #ifdef __cplusplus
 }

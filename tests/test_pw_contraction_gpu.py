@@ -20,6 +20,7 @@ import pytest
 import torch
 
 import pw_criterion as PC
+import train_kernel_ref as TKR
 from ctn_b200 import _native as N
 
 pytestmark = pytest.mark.gpu
@@ -393,7 +394,7 @@ def test_wgrad_vs_fp64(name):
     e_one = PC.gate_e(torch.einsum("bmt,bkt->mk", PC.round_sig(dy), PC.round_sig(x)), (ref, den, smag))
     split = r["split"]
     report = []
-    for mode in ("tf32x3", "tf32", "f16x3"):
+    for mode in ("fp32", "tf32x3", "tf32", "f16x3"):
         dWa = torch.zeros(split if split else M, K, device=DEV)
         dWb = torch.zeros(M - split, K, device=DEV) if split else None
         st = probe_wgrad(dyb.data_ptr(), dy_bs, xb.data_ptr(), x_bs, dWa.data_ptr(), N.ptr(dWb), split if split else M, M, K, B, T,
@@ -402,7 +403,9 @@ def test_wgrad_vs_fp64(name):
         assert st == N.CTN_OK, (name, mode, st)
         dW = torch.cat([dWa, dWb]) if split else dWa
         e = PC.gate_e(dW, (ref, den, smag))
-        if r.get("summation_only"):
+        if mode == "fp32":  # FFMA split-K: one thread's chain of 32 units_per_cta terms, then one fp32 atomic per split
+            b = TKR.wgrad_fp32_chain(M, K, B, T, split) * U
+        elif r.get("summation_only"):
             b = (B * T + 8) * U
         else:
             b = PC.bound(mode, B * T, e_drop, e_one)
