@@ -184,8 +184,8 @@ static int run_tcn(const ctn_config_t* c, const ctn_block_params_t* blocks, TcnW
       const ctn_block_params_t& p = blocks[i];
       const bool has_out = p.out_w != nullptr;
       const FoldedConv& f = ws->folds[i];
-      if (has_out) fj.push_back(FoldJob{p.out_w, p.out_b, p.norm2_g, p.norm2_b, f.Wf, f.v1, f.v2, Bc, H, 0, f.vb, Rh});
-      fj.push_back(FoldJob{p.skip_w, p.skip_b, p.norm2_g, p.norm2_b, f.Wf, f.v1, f.v2, Sc, H, has_out ? Bc : 0, f.vb, Rh});
+      if (has_out) fj.push_back(FoldJob{p.out_w, p.out_b, p.norm2_g, p.norm2_b, f, Bc, H, 0, Rh});
+      fj.push_back(FoldJob{p.skip_w, p.skip_b, p.norm2_g, p.norm2_b, f, Sc, H, has_out ? Bc : 0, Rh});
       sj->j[i] = ScaleJob{f.vb, p.norm1_g, p.norm1_b, p.dw_w, p.dw_b, p.prelu2, ws->dwp[i], has_out ? 1 : 0};
       wj.push_back(WimgJob{p.bottleneck_w, ws->wimg1[i], H, Bc});
       wj.push_back(WimgJob{f.Wf, ws->wimg2[i], has_out ? Bc + Sc : Sc, H});
@@ -492,7 +492,8 @@ static int run_separator(const ctn_config_t* c, const ctn_params_t* p, ModelWs* 
     a.v1 = ws->head.v1; a.v2 = ws->head.v2; a.stats_in = ws->stats0; a.n_in = (double)N * (double)frames; a.eps = c->eps;
     a.wimg = ws->wimg_head;
     { StageTimer tm(CTN_ST_PREP, st);
-      CTN_TRY(ctn_fold_conv(p->bn_w, p->bn_b, p->norm0_g, p->norm0_b, Bc, N, ws->head, 0, st, sqrtf((float)N * (float)frames) * 1.0001f));
+      const FoldJob fj{p->bn_w, p->bn_b, p->norm0_g, p->norm0_b, ws->head, Bc, N, 0, sqrtf((float)N * (float)frames) * 1.0001f};
+      CTN_TRY(ctn_fold_batch(&fj, 1, st));
       CTN_TRY(ctn_pw_prepare(a, c->math, ws->wimg_head, st));
       CTN_TRY(ctn_pw_prepare(m, c->math, ws->wimg_mask, st));
     }
@@ -650,7 +651,8 @@ extern "C" int ctn_sep_head_fwd(const float* w, const double* stats0, const floa
   Carver cv(workspace);
   StageWs ws;
   carve_stage(cv, Bc, N, math, &ws);
-  CTN_TRY(ctn_fold_conv(bn_w, bn_b, norm_g, norm_b, Bc, N, ws.head, 0, st));
+  const FoldJob fj{bn_w, bn_b, norm_g, norm_b, ws.head, Bc, N, 0, 0.f};  // no vb: carve_stage leaves it null
+  CTN_TRY(ctn_fold_batch(&fj, 1, st));
   PwArgs a;
   memset(&a, 0, sizeof(a));
   a.A = w; a.W = ws.head.Wf; a.D = x0; a.B = B; a.M = Bc; a.K = N; a.frames = frames; a.pitch = pitch;

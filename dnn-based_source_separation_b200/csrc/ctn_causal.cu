@@ -23,19 +23,13 @@ struct CausalWs {
   float* r;      // (B, Bc+Sc, pitch)
 };
 
-size_t max_wimg(const ctn_config_t* c) {
-  if (c->math == CTN_MATH_FP32) return 256;
-  size_t a = ctn_pw_wimg_bytes(c->hidden, c->bottleneck, c->math);
-  size_t b = ctn_pw_wimg_bytes(c->bottleneck + c->skip, c->hidden, c->math);
-  size_t d = c->n_basis > 0 ? ctn_pw_wimg_bytes(c->bottleneck, c->n_basis, c->math) : 0;
-  size_t m = a > b ? a : b;
-  return m > d ? m : d;
-}
-
 void carve(Carver& cv, const ctn_config_t* c, int B, int pitch, CausalWs* ws) {
+  // images of pw1, [out; skip] and (with an encoder) the head
+  const int Bc = c->bottleneck, H = c->hidden;
+  const int shapes[][2] = {{H, Bc}, {Bc + c->skip, H}, {Bc, c->n_basis}};
   ws->cln = cv.take<double>((size_t)B * pitch * 2);
   ws->dummy = cv.take<double>((size_t)B * 2);
-  ws->wimg = cv.take<float>(max_wimg(c) / sizeof(float));
+  ws->wimg = cv.take<float>(ctn_pw_wimg_max_bytes(shapes, c->n_basis > 0 ? 3 : 2, c->math) / sizeof(float));
   ws->Wcat = cv.take<float>((size_t)(c->bottleneck + c->skip) * c->hidden);
   ws->r = cv.take<float>((size_t)B * pitch * (c->bottleneck + c->skip));
 }

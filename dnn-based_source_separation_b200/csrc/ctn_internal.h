@@ -114,16 +114,17 @@ int ctn_pw_maskdec_supported(const PwArgs& a, int math);
 int ctn_wgrad_wgmma(const float* dy, size_t dy_bs, const float* x, size_t x_bs, float* dWa, float* dWb, int split_row, int M,
                     int K, int B, int frames, int pitch, int math, cudaStream_t st);
 
-int ctn_fold_conv(const float* W, const float* bias, const float* gamma, const float* beta, int M, int K, FoldedConv out,
-                  int row_offset, cudaStream_t st, float R = 0.f);
-
-// batched variants: all weight preparation of a forward in two launches (jobs travel in the kernel parameter block)
-struct FoldJob { const float *W, *bias, *gamma, *beta; float *Wf, *v1, *v2; int M, K, row_offset; float* vb; float R; };
+// weight preparation of one or many convs: gLN folds into rows [row_offset, row_offset + M) of a FoldedConv (R as in its vb),
+// weight images for ctn_pw; up to CTN_MAX_JOBS jobs per launch (they travel in the kernel parameter block)
+struct FoldJob { const float *W, *bias, *gamma, *beta; FoldedConv out; int M, K, row_offset; float R; };
 struct WimgJob { const float* W; float* wimg; int M, K; };
 #define CTN_MAX_JOBS 48
 int ctn_fold_batch(const FoldJob* jobs, int n, cudaStream_t st);
-// weight images of the jobs in one launch; bounded: every one of these contractions carries an operand scale (see ctn_pw)
+// weight images of the jobs, one launch per job when they take different pieces; bounded: every one of these contractions
+// carries an operand scale (see ctn_pw)
 int ctn_pw_prepare_batch(const WimgJob* jobs, int n, int math, bool bounded, cudaStream_t st);
+// largest ctn_pw_wimg_bytes over n (M, K) shapes; 256 in the fp32 mode, which builds no images
+size_t ctn_pw_wimg_max_bytes(const int (*shapes)[2], int n, int math);
 
 // Activation envelope of the fp16-piece mode.  Per residual block i the two operands that meet the tensor core as fp16
 // pieces are x_i (pw1) and u_i (fused depthwise output, pw2); the mask contraction sees PReLU(skip sum).  From the weights

@@ -11,12 +11,12 @@
 // ------------------------------------------------------------------------------------------------
 // weight folding: one warp per output row
 // ------------------------------------------------------------------------------------------------
-__global__ void __launch_bounds__(128) k_fold(const float* __restrict__ W, const float* __restrict__ bias,
-                                              const float* __restrict__ gamma, const float* __restrict__ beta, int M, int K,
-                                              float* __restrict__ Wf, float* __restrict__ v1, float* __restrict__ v2,
-                                              int row_offset, float* __restrict__ vb, float R) {
-  const int row = blockIdx.x * 4 + (threadIdx.x >> 5), lane = threadIdx.x & 31;
-  if (row >= M) return;
+// __restrict__ lets the compiler issue the loads of W, gamma and beta ahead of the stores to Wf; the pointers of a FoldJob carry
+// no such promise, hence the helper.
+__device__ __forceinline__ void fold_row(const float* __restrict__ W, const float* __restrict__ bias, const float* __restrict__ gamma,
+                                         const float* __restrict__ beta, int K, int row, int row_offset, float* __restrict__ Wf,
+                                         float* __restrict__ v1, float* __restrict__ v2, float* __restrict__ vb, float R) {
+  const int lane = threadIdx.x & 31;
   float s1 = 0.f, s2 = 0.f, s3 = 0.f;
   for (int k = lane; k < K; k += 32) {
     const float w = W[(size_t)row * K + k];
@@ -36,37 +36,14 @@ __global__ void __launch_bounds__(128) k_fold(const float* __restrict__ W, const
   }
 }
 
-int ctn_fold_conv(const float* W, const float* bias, const float* gamma, const float* beta, int M, int K, FoldedConv out,
-                  int row_offset, cudaStream_t st, float R) {
-  k_fold<<<(M + 3) / 4, 128, 0, st>>>(W, bias, gamma, beta, M, K, out.Wf, out.v1, out.v2, row_offset, out.vb, R);
-  CTN_COUNT_LAUNCH();
-  CTN_RETURN_IF_CUDA_ERR();
-  return CTN_OK;
-}
-
 struct FoldJobs { FoldJob j[CTN_MAX_JOBS]; };
+// grid ((rows of the largest job + 3) / 4, jobs): one warp per row of one job.  No grid-stride loop: with one, the loads lose
+// their early issue and a single fold takes twice as long (H100).
 __global__ void __launch_bounds__(128) k_fold_batch(const FoldJobs jobs) {
   const FoldJob& jb = jobs.j[blockIdx.y];
-  for (int row = blockIdx.x * 4 + (threadIdx.x >> 5); row < jb.M; row += gridDim.x * 4) {
-    const int lane = threadIdx.x & 31;
-    float s1 = 0.f, s2 = 0.f, s3 = 0.f;
-    for (int k = lane; k < jb.K; k += 32) {
-      const float w = jb.W[(size_t)row * jb.K + k];
-      const float wf = w * jb.gamma[k];
-      jb.Wf[(size_t)(row + jb.row_offset) * jb.K + k] = wf;
-      s1 = fmaf(w, jb.beta[k], s1);
-      s2 += wf;
-      s3 = fmaf(fabsf(w), fmaf(fabsf(jb.gamma[k]), jb.R, fabsf(jb.beta[k])), s3);
-    }
-    s1 = warp_sum(s1);
-    s2 = warp_sum(s2);
-    s3 = warp_sum(s3);
-    if (lane == 0) {
-      jb.v1[row + jb.row_offset] = s1 + (jb.bias ? jb.bias[row] : 0.f);
-      jb.v2[row + jb.row_offset] = s2;
-      if (jb.vb) jb.vb[row + jb.row_offset] = s3 + (jb.bias ? fabsf(jb.bias[row]) : 0.f);
-    }
-  }
+  const int row = blockIdx.x * 4 + (threadIdx.x >> 5);
+  if (row >= jb.M) return;
+  fold_row(jb.W, jb.bias, jb.gamma, jb.beta, jb.K, row, jb.row_offset, jb.out.Wf, jb.out.v1, jb.out.v2, jb.out.vb, jb.R);
 }
 
 int ctn_fold_batch(const FoldJob* jobs, int n, cudaStream_t st) {

@@ -777,18 +777,6 @@ struct TrainWs {
   size_t tcn_bytes;
 };
 
-size_t max_wimg_bytes(const ctn_config_t* c) {
-  if (c->math == CTN_MATH_FP32) return 256;
-  const int N = c->n_basis, Bc = c->bottleneck, H = c->hidden, Sc = c->skip, SN = c->n_sources * c->n_basis;
-  const int shapes[][2] = {{H, Bc}, {Bc + Sc, H}, {H, Bc + Sc}, {Bc, H}, {Bc, N}, {N, Bc}, {SN, Sc}, {Sc, SN}};
-  size_t mx = 0;
-  for (auto& s : shapes) {
-    const size_t b = ctn_pw_wimg_bytes(s[0], s[1], c->math);
-    if (b > mx) mx = b;
-  }
-  return mx;
-}
-
 // fp16-piece mode with 3-tap depthwise convs: the TCN forward runs through the SAME fused kernels as inference (pw1 with the
 // residual update fused, depthwise producer feeding the [out;skip] contraction), which additionally leave x_i, W1 x + b1 and
 // the depthwise pre-activation behind for the backward -- 2 launches per block instead of 7, no u / gLN2(u) round trips.
@@ -825,7 +813,10 @@ void carve_train(Carver& cv, const ctn_config_t* c, int B, int pitch, TrainWs* w
     ws->tcn_bytes = ctn_tcn_train_ws_bytes(c, B, pitch);
     ws->tcn_mem = cv.take<char>(ws->tcn_bytes);
   }
-  ws->wimg = cv.take<float>(max_wimg_bytes(c) / sizeof(float));
+  // the step's contractions outside the fused TCN build their weight images here, one at a time
+  const int SN = S * N;
+  const int shapes[][2] = {{H, Bc}, {Bc + Sc, H}, {H, Bc + Sc}, {Bc, H}, {Bc, N}, {N, Bc}, {SN, Sc}, {Sc, SN}};
+  ws->wimg = cv.take<float>(ctn_pw_wimg_max_bytes(shapes, 8, c->math) / sizeof(float));
   size_t wmax = (size_t)(Bc + Sc) * H;
   if ((size_t)S * N * Sc > wmax) wmax = (size_t)S * N * Sc;
   if ((size_t)Bc * N > wmax) wmax = (size_t)Bc * N;
@@ -902,7 +893,8 @@ extern "C" int ctn_convtasnet_fwd_train(const ctn_config_t* c, const ctn_params_
   CTN_TRY(ctn_encoder_fwd(x, p->enc_w, ws.w, B, T, pl, pr, N, c->kernel_size, c->stride, c->enc_relu, pitch, ws.stats0, stream));
   // head: x_0 = Wb gLN0(w) + bb (conv_tasnet.py:370-371), gLN0 folded into the contraction like the inference path
   {
-    CTN_TRY(ctn_fold_conv(p->bn_w, p->bn_b, p->norm0_g, p->norm0_b, Bc, N, ws.head, 0, st, sqrtf((float)N * (float)frames) * 1.0001f));
+    const FoldJob fj{p->bn_w, p->bn_b, p->norm0_g, p->norm0_b, ws.head, Bc, N, 0, sqrtf((float)N * (float)frames) * 1.0001f};
+    CTN_TRY(ctn_fold_batch(&fj, 1, st));
     PwArgs a;
     memset(&a, 0, sizeof(a));
     a.A = ws.w; a.W = ws.head.Wf; a.D = ws.x[0]; a.B = B; a.M = Bc; a.K = N; a.frames = frames; a.pitch = pitch;

@@ -363,33 +363,16 @@ __host__ __device__ __forceinline__ int wimg_offset(int nl, int kl) {
   return (nl >> 3) * 256 + (nl & 7) * 32 + ((((kl >> 2) ^ (nl & 7)) << 2) | (kl & 3));
 }
 
-// grid (k_slabs, n_tiles), block 256: builds the image(s) of one weight slab.
-__global__ void __launch_bounds__(256) k_build_wimg(const float* __restrict__ W, int M, int K, int n_tile, int k_slabs,
-                                                    int nprec, float* __restrict__ wimg) {
-  const int ks = blockIdx.x, nt = blockIdx.y;
-  const size_t per = (size_t)n_tile * KS;  // floats per precision
-  float* dst = wimg + ((size_t)nt * k_slabs + ks) * nprec * per;
-  for (int i = threadIdx.x; i < n_tile * KS; i += 256) {
-    const int nl = i / KS, kl = i % KS;
-    const int n = nt * n_tile + nl, k = ks * KS + kl;
-    const float x = (n < M && k < K) ? W[(size_t)n * K + k] : 0.f;
-    const int off = wimg_offset(nl, kl);
-    const float hi = ptx::to_tf32(x);
-    dst[off] = hi;
-    if (nprec == 2) dst[per + off] = ptx::to_tf32(x - hi);
-  }
-}
-
 // fp16 variant ("3xFP16"): K-major SWIZZLE_64B rows of 32 k x 2 B; per slab a hi image then a lo image of n_tile*64 bytes.
 // Every group of 16 weight ROWS (output channels) is first scaled by a power of two 2^e so that its largest entry lands in
 // [2^9, 2^10) (one scale per 16 rows = per 16-column epilogue chunk, so the epilogue needs a single scalar per chunk):
 // hi and lo pieces then sit in fp16's normal range whatever the magnitude of the weights (tiny gamma-folded rows would
 // otherwise lose their lo piece to fp16's subnormal floor of 6e-8, huge ones would saturate); the epilogue multiplies the
 // accumulator of channel n by the exact inverse 2^-e (oscale, stored behind the images).
-// One warp per row; block = 16 warps = one 16-row scale group (the epilogue reads one scale per 16-column chunk);
-// grid (ceil(n_tile/16), n_tiles).
+// One warp per row; block = 16 warps = one 16-row scale group (the epilogue reads one scale per 16-column chunk).
 __device__ __forceinline__ void wimg_f16_group(const float* __restrict__ W, int M, int K, int n_tile, int k_slabs, int nt, int grp,
                                                __half* __restrict__ img, float* __restrict__ oscale, float* smax) {
+  static_assert(KS == 32, "one lane per channel of a slab");
   const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
   const int nl = grp * 16 + wid;
   const int n = nt * n_tile + nl;
@@ -426,38 +409,38 @@ __device__ __forceinline__ void wimg_f16_group(const float* __restrict__ W, int 
 __host__ __device__ inline size_t wimg_f16_image_bytes(int n_tile, int n_tiles, int k_slabs) {
   return (size_t)n_tiles * k_slabs * 2 * n_tile * KS * sizeof(__half);
 }
-__global__ void __launch_bounds__(512) k_build_wimg_f16(const float* __restrict__ W, int M, int K, int n_tile, int k_slabs,
-                                                        int n_tiles, float* __restrict__ wimg) {
-  static_assert(KS == 32, "one lane per channel of a slab");
-  __shared__ float smax[16];
-  __half* img = reinterpret_cast<__half*>(wimg);
-  float* oscale = reinterpret_cast<float*>(reinterpret_cast<uint8_t*>(wimg) + wimg_f16_image_bytes(n_tile, n_tiles, k_slabs));
-  wimg_f16_group(W, M, K, n_tile, k_slabs, blockIdx.y, blockIdx.x, img, oscale, smax);
-}
 
 struct WimgJobs { WimgJob j[CTN_MAX_JOBS]; };
-// grid (max k_slabs * max n_tiles, jobs): one block per (slab, n-tile) of one job
-__global__ void __launch_bounds__(256) k_build_wimg_batch(const WimgJobs jobs, int nprec) {
-  const WimgJob& jb = jobs.j[blockIdx.y];
+// tf32 image(s) of slab ks of n-tile nt.  __restrict__ lets the compiler issue the loads of W ahead of the image stores; the
+// pointers of a WimgJob carry no such promise, hence the helper.
+__device__ __forceinline__ void wimg_tf32_slab(const float* __restrict__ W, int M, int K, int k_slabs, int nt, int ks, int nprec,
+                                               float* __restrict__ wimg) {
   const int n_tile = NT;
-  const int n_tiles = (jb.M + n_tile - 1) / n_tile, k_slabs = (jb.K + KS - 1) / KS;
-  const size_t per = (size_t)n_tile * KS;
-  for (int blk = blockIdx.x; blk < n_tiles * k_slabs; blk += gridDim.x) {
-    const int nt = blk / k_slabs, ks = blk - nt * k_slabs;
-    float* dst = jb.wimg + ((size_t)nt * k_slabs + ks) * nprec * per;
-    for (int i = threadIdx.x; i < n_tile * KS; i += 256) {
-      const int nl = i / KS, kl = i % KS;
-      const int n = nt * n_tile + nl, k = ks * KS + kl;
-      const float x = (n < jb.M && k < jb.K) ? jb.W[(size_t)n * jb.K + k] : 0.f;
-      const int off = wimg_offset(nl, kl);
-      const float hi = ptx::to_tf32(x);
-      dst[off] = hi;
-      if (nprec == 2) dst[per + off] = ptx::to_tf32(x - hi);
-    }
+  const size_t per = (size_t)n_tile * KS;  // floats per precision
+  float* dst = wimg + ((size_t)nt * k_slabs + ks) * nprec * per;
+  for (int i = threadIdx.x; i < n_tile * KS; i += 256) {
+    const int nl = i / KS, kl = i % KS;
+    const int n = nt * n_tile + nl, k = ks * KS + kl;
+    const float x = (n < M && k < K) ? W[(size_t)n * K + k] : 0.f;
+    const int off = wimg_offset(nl, kl);
+    const float hi = ptx::to_tf32(x);
+    dst[off] = hi;
+    if (nprec == 2) dst[per + off] = ptx::to_tf32(x - hi);
   }
 }
 
-// grid (64, jobs), block 512: blockIdx.x walks the (n-tile, 16-row group) pairs of its job
+// grid (blocks of the largest job, jobs): one block per (slab, n-tile) of one job.  No grid-stride loop: with one, the loads
+// lose their early issue and a single image takes about three times as long to build (H100).
+__global__ void __launch_bounds__(256) k_build_wimg_batch(const WimgJobs jobs, int nprec) {
+  const WimgJob& jb = jobs.j[blockIdx.y];
+  const int n_tiles = (jb.M + NT - 1) / NT, k_slabs = (jb.K + KS - 1) / KS;
+  const int blk = blockIdx.x;
+  if (blk >= n_tiles * k_slabs) return;
+  const int nt = blk / k_slabs, ks = blk - nt * k_slabs;
+  wimg_tf32_slab(jb.W, jb.M, jb.K, k_slabs, nt, ks, nprec, jb.wimg);
+}
+
+// grid (blocks of the largest job, jobs), block 512: blockIdx.x walks the (n-tile, 16-row group) pairs of its job
 __global__ void __launch_bounds__(512) k_build_wimg_batch_f16(const WimgJobs jobs) {
   __shared__ float smax[16];
   const WimgJob& jb = jobs.j[blockIdx.y];
@@ -508,18 +491,23 @@ int launch_math(const TcArgs& g, int math, cudaStream_t st) {
 // every other contraction of the f16x3 mode runs on tf32 pieces.  Weight images and kernels follow the same rule.
 int piece_math(int math, bool bounded) { return math == CTN_MATH_F16X3 && !bounded ? CTN_MATH_TF32X3 : math; }
 
-int build_wimg(const float* W, int M, int K, int math, float* wimg, cudaStream_t st) {
-  math = eff_math(M, math);
-  const int nprec = math == CTN_MATH_TF32 ? 1 : 2;  // hi [, lo]
-  const int n_tiles = (M + NT - 1) / NT, k_slabs = (K + KS - 1) / KS;
-  if (math == CTN_MATH_F16X3) {
-    k_build_wimg_f16<<<dim3(NT / 16, n_tiles), 512, 0, st>>>(W, M, K, NT, k_slabs, n_tiles, wimg);
+// weight images of jobs that all take the pieces `math` (eff_math already applied), CTN_MAX_JOBS per launch
+int build_images(const WimgJob* jobs, int n, int math, cudaStream_t st) {
+  const bool f16 = math == CTN_MATH_F16X3;
+  for (int i0 = 0; i0 < n; i0 += CTN_MAX_JOBS) {
+    WimgJobs wj;
+    const int m = n - i0 < CTN_MAX_JOBS ? n - i0 : CTN_MAX_JOBS;
+    int maxb = 1;
+    for (int i = 0; i < m; ++i) {
+      const WimgJob& jb = jobs[i0 + i];
+      wj.j[i] = jb;
+      const int blocks = ((jb.M + NT - 1) / NT) * (f16 ? NT / 16 : (jb.K + KS - 1) / KS);
+      if (blocks > maxb) maxb = blocks;
+    }
+    if (f16) k_build_wimg_batch_f16<<<dim3(maxb, m), 512, 0, st>>>(wj);
+    else k_build_wimg_batch<<<dim3(maxb, m), 256, 0, st>>>(wj, math == CTN_MATH_TF32 ? 1 : 2);  // hi [, lo]
     CTN_COUNT_LAUNCH();
-    CTN_RETURN_IF_CUDA_ERR();
-    return CTN_OK;
   }
-  k_build_wimg<<<dim3(k_slabs, n_tiles), 256, 0, st>>>(W, M, K, NT, k_slabs, nprec, wimg);
-  CTN_COUNT_LAUNCH();
   CTN_RETURN_IF_CUDA_ERR();
   return CTN_OK;
 }
@@ -574,35 +562,29 @@ size_t ctn_pw_wimg_bytes(int M, int K, int math) {
   return (size_t)n_tiles * k_slabs * nprec * NT * KS * sizeof(float) + (size_t)n_tiles * NT * sizeof(float) + 256;
 }
 
+size_t ctn_pw_wimg_max_bytes(const int (*shapes)[2], int n, int math) {
+  if (math == CTN_MATH_FP32) return 256;
+  size_t mx = 0;
+  for (int i = 0; i < n; ++i) {
+    const size_t b = ctn_pw_wimg_bytes(shapes[i][0], shapes[i][1], math);
+    if (b > mx) mx = b;
+  }
+  return mx;
+}
+
 int ctn_pw_prepare(const PwArgs& a, int math, float* wimg, cudaStream_t st) {
-  if (math == CTN_MATH_FP32) return CTN_OK;
-  return build_wimg(a.W, a.M, a.K, piece_math(math, a.act_scale != nullptr), wimg, st);
+  const WimgJob job{a.W, wimg, a.M, a.K};
+  return ctn_pw_prepare_batch(&job, 1, math, a.act_scale != nullptr, st);
 }
 
 int ctn_pw_prepare_batch(const WimgJob* jobs, int n, int math, bool bounded, cudaStream_t st) {
   if (math == CTN_MATH_FP32) return CTN_OK;
   math = piece_math(math, bounded);
-  const int nprec = math == CTN_MATH_TF32 ? 1 : 2;
   bool uniform = true;
   for (int i = 0; i < n; ++i) uniform = uniform && eff_math(jobs[i].M, math) == math;
-  if (!uniform) {
-    for (int i = 0; i < n; ++i) CTN_TRY(build_wimg(jobs[i].W, jobs[i].M, jobs[i].K, math, jobs[i].wimg, st));
-    return CTN_OK;
-  }
-  for (int i0 = 0; i0 < n; i0 += CTN_MAX_JOBS) {
-    WimgJobs wj;
-    const int m = n - i0 < CTN_MAX_JOBS ? n - i0 : CTN_MAX_JOBS;
-    int maxb = 1;
-    for (int i = 0; i < m; ++i) {
-      wj.j[i] = jobs[i0 + i];
-      const int blocks = ((jobs[i0 + i].M + NT - 1) / NT) * ((jobs[i0 + i].K + KS - 1) / KS);
-      if (blocks > maxb) maxb = blocks;
-    }
-    if (math == CTN_MATH_F16X3) k_build_wimg_batch_f16<<<dim3(64, m), 512, 0, st>>>(wj);
-    else k_build_wimg_batch<<<dim3(maxb, m), 256, 0, st>>>(wj, nprec);
-    CTN_COUNT_LAUNCH();
-  }
-  CTN_RETURN_IF_CUDA_ERR();
+  if (uniform) return build_images(jobs, n, math, st);
+  // f16x3 with some contraction past F16_MAX_ROWS (tf32 pieces): one launch per job, each in its own pieces
+  for (int i = 0; i < n; ++i) CTN_TRY(build_images(jobs + i, 1, eff_math(jobs[i].M, math), st));
   return CTN_OK;
 }
 
@@ -612,7 +594,7 @@ int ctn_pw(const PwArgs& a, int pro, int epi, int math, float* wimg_scratch, cud
   if (math == CTN_MATH_FP32) return ctn_pw_simt(a, pro, epi, st);
   const int pmath = piece_math(math, a.act_scale != nullptr);
   if (!wimg_scratch) return launch_wgmma(a, pro, epi, pmath, st);
-  CTN_TRY(build_wimg(a.W, a.M, a.K, pmath, wimg_scratch, st));
+  CTN_TRY(ctn_pw_prepare(a, math, wimg_scratch, st));
   PwArgs b = a;
   b.wimg = wimg_scratch;
   return launch_wgmma(b, pro, epi, pmath, st);

@@ -64,8 +64,9 @@ typedef struct ctn_pw_probe {
   float* dw_u_pre_out;
 } ctn_pw_probe_t;
 
-/* route 0: the weight image of W is built into wimg on every call (the per-call builders);
- * route 1: the batched builders prepare wimg first (operand scale present = fp16 pieces allowed), then the kernel reads it.
+/* route 0: the contraction builds the weight image of W into wimg on every call;
+ * route 1: the pipelines' batched preparation builds wimg first (operand scale present = fp16 pieces allowed), then the kernel
+ * reads it.  Both reach the same image builders.
  * Returns the contraction's status unchanged (CTN_EALIGN, CTN_EUNSUPPORTED, ...).  math CTN_MATH_FP32 ignores wimg. */
 int ctn_probe_pw(const ctn_pw_probe_t* p, int pro, int epi, int math, int route, void* wimg, size_t wimg_bytes, ctn_stream_t stream);
 /* bytes of the weight image of an (M, K) contraction */
