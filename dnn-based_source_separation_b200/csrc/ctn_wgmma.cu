@@ -2,19 +2,22 @@
 //
 //   D[b][n][t] = epi( sum_k W[n][k] * pro(A[b][k][t]) )        A: (B,K,pitch) fp32, time contiguous
 //
-// A CTA computes one tile of 128 time steps x 128 output channels.  Orientation: TIME runs along the wgmma M dimension
-// (two warpgroups of 64 rows each), output channels along N = 128:
+// TIME runs along the wgmma M dimension (64 rows per warpgroup), output channels along N = 128 per warpgroup.  A CTA computes
+// 128 time steps x 1 n-tile (time split over the two warpgroups) or, for the fp16-piece TCN block contractions, 64 time steps
+// x 2 n-tiles (channel split, see chan_split):
 //   * the activation operand is formed by the CTA's own threads (global -> registers -> prologue -> hi/lo split) and stored
-//     K-major (rows of one time step, 32 input channels per slab) in the same swizzled layout as the weights;
+//     swizzled: fp16 pieces MN-major (rows of 64 time steps of one input channel, read with wgmma's transpose), tf32 pieces
+//     K-major (rows of one time step, 32 input channels per slab);
 //   * the weight operand is K-major (PyTorch (out,in,1) layout), pre-arranged once per forward into the exact swizzled
-//     shared-memory image of a slab, so that one 1-D bulk async copy (TMA engine) brings a 32-channel slab in;
+//     shared-memory image of a slab, so that one 1-D bulk async copy (TMA engine) brings a 32-channel slab of an n-tile in;
 //   * the accumulator stays in registers; the fused epilogue runs on it directly.
 // fp32-parity numerics: x = hi + lo with 11-bit pieces, D = A_hi W_hi + A_lo W_hi + A_hi W_lo accumulated in fp32 (the dropped
-// lo*lo term is ~2^-22 relative).  Pieces are TF32 ("3xTF32", SWIZZLE_128B rows of 32 x 4 B) or FP16 ("3xFP16", SWIZZLE_64B
-// rows of 32 x 2 B, twice the tensor rate, weights pre-scaled per 16-row group, see wimg_f16_group) -- template parameter F16.
+// lo*lo term is ~2^-22 relative).  Pieces are TF32 ("3xTF32", SWIZZLE_128B rows of 32 x 4 B) or FP16 ("3xFP16", weights in
+// SWIZZLE_64B rows of 32 x 2 B, twice the tensor rate, weights pre-scaled per 16-row group, see wimg_f16_group) -- template
+// parameter F16.
 //
-// Pipeline: two shared-memory stages.  While the tensor core works on slab ks (wgmma is asynchronous), all 256 threads load
-// and stage slab ks + 1 and one thread issues the bulk copy of its weights.
+// Pipeline: two shared-memory stages.  While the tensor core works on slab ks (wgmma is asynchronous), all 256 threads form
+// and stage slab ks + 1, whose global loads went out one slab earlier, and one thread issues the bulk copy of its weights.
 #include "ctn_internal.h"
 #include "ctn_wgmma_ptx.cuh"
 #include "ctn_dw_math.cuh"
@@ -27,62 +30,110 @@ int ctn_pw_simt(const PwArgs& a, int pro, int epi, cudaStream_t st);
 
 namespace {
 
-constexpr int TM = 128;        // time steps per tile (2 warpgroups x wgmma M = 64)
-constexpr int KS = 32;         // input channels per smem slab (128-byte tf32 rows / 64-byte fp16 rows)
-constexpr int NT = 128;        // output channels per tile (wgmma N)
-constexpr int THREADS = 256;   // 8 warps: warp w stages channels [4w, 4w+4) of every slab, lane l time steps [4l, 4l+4)
+constexpr int TM = 128;        // time steps per tile of the time-split kernels (2 warpgroups x wgmma M = 64)
+constexpr int KS = 32;         // input channels per smem slab
+constexpr int NT = 128;        // output channels per n-tile (wgmma N)
+constexpr int THREADS = 256;   // 8 warps: warp w stages channels [4w, 4w+4) of every slab, each lane 4 consecutive time steps
 constexpr int CPW = 4;         // channels of a slab per warp
 constexpr int STAGES = 2;
 constexpr int SMEM_HEADER = 1024;   // mbarriers
 constexpr int F16_MAX_ROWS = 2048;  // fp16-piece mode: padded output channels of one contraction (see eff_math)
+
+// Tiling.  The fp16-piece TCN block contractions (PRO_DW, and EPI_H) split OUTPUT CHANNELS over the two warpgroups: a CTA owns 64
+// frames x 2 n-tiles, warpgroup w n-tile 2p + w, and both consume the same activation slab, so h and its depthwise stage (or the
+// residual update) are formed once per frame tile instead of once per n-tile.  With an odd n-tile count (e.g. the last block's
+// [out; skip] contraction, M = 128) the last CTA's second warpgroup has no n-tile: it still forms its share of each slab, and skips
+// its MMAs and epilogue.  Every other kernel splits TIME: 128 frames x 1 n-tile, warpgroup w frames [64w, 64w + 64).  EPI_MASKDEC
+// sums decoder taps per frame over the n-tiles of a source, and tf32 pieces are K-major only (see the operand store).
+template <int PRO, int EPI, bool F16>
+__host__ __device__ constexpr bool chan_split() { return F16 && (PRO == PRO_DW || EPI == EPI_H); }
+template <int PRO, int EPI, bool F16>
+__host__ __device__ constexpr int tile_frames() { return chan_split<PRO, EPI, F16>() ? 64 : TM; }
 
 struct TcArgs {
   PwArgs a;
   const float* wimg;    // [n_tiles][k_slabs][NPREC][NT*KS] swizzled images
   const float* oscale;  // fp16-piece mode: [n_tiles*NT] per-output-channel scale 2^-e (stored behind the images)
   int n_tiles, k_slabs, t_tiles;
+  int n_groups;    // CTAs per (sample, time tile)
   int nt_per_cta;  // n-tiles a CTA walks back to back: 1, or all n-tiles of one source (EPI_MASKDEC)
 };
 
-// u = PReLU(dwconv3(gLN1(h)) + bd) for this thread's 4 time steps of the CPW channels of warp pw in slab ks.
-// TRAIN: A holds the pre-activation of h; PReLU(dw_in_slope) is applied on load and the depthwise pre-activation goes to pre[].
-template <int DCLS, bool INTERIOR, bool TRAIN>
-__device__ __forceinline__ void dw_slab(const PwArgs& a, int b, int ks, int pw, int tbase, float2 mr1, float pslope, float4 (&v)[CPW],
-                                        float4 (&pre)[CPW], float2& dls, float2& dlss) {
-  const int d = a.dw_dilation, pl = a.dw_pad_left;
-  const int step = DCLS == 4 ? d : 4;
-  const int first = DCLS == 4 ? tbase - pl : tbase - 4;
+// A thread's global loads for one slab: CPT channels x 4 time steps, NQ float4 per channel (PRO_DW: the 3 depthwise taps; PRO_RES:
+// x and r).  They are issued one slab ahead of their use, so that their latency overlaps the store and the MMAs of the previous slab.
+template <int PRO>
+__host__ __device__ constexpr int raw_q() { return PRO == PRO_DW ? 3 : PRO == PRO_RES ? 2 : 1; }
+template <int PRO, int CPT>
+struct Raw { float4 q[CPT][raw_q<PRO>()]; };
+
+// channels [c0, c0 + CPT) of the operand, time steps [tbase, tbase + 4).  PRO_DW: taps at first + k * step (clamped to the row
+// outside interior tiles).
+template <int PRO, int CPT>
+__device__ __forceinline__ void load_raw(const PwArgs& a, int b, int c0, int tbase, int first, int step, bool interior, Raw<PRO, CPT>& r) {
+#pragma unroll
+  for (int j = 0; j < CPT; ++j) {
+    const int c = c0 + j;
+    if constexpr (PRO == PRO_DW) {
+      const int cc = interior ? c : (c < a.K ? c : a.K - 1);
+      const float* hr = a.A + ((size_t)b * a.K + cc) * a.pitch;
+#pragma unroll
+      for (int k = 0; k < 3; ++k) {
+        int ts = first + k * step;
+        if (!interior) ts = ts < 0 ? 0 : (ts > a.pitch - 4 ? a.pitch - 4 : ts);
+        r.q[j][k] = __ldg(reinterpret_cast<const float4*>(hr + ts));
+      }
+    } else {
+      const bool ok = c < a.K;
+      r.q[j][0] = ok ? __ldg(reinterpret_cast<const float4*>(a.A + ((size_t)b * a.K + c) * a.pitch + tbase)) : make_float4(0.f, 0.f, 0.f, 0.f);
+      if constexpr (PRO == PRO_RES)
+        r.q[j][1] = ok ? __ldg(reinterpret_cast<const float4*>(a.res_r + ((size_t)b * a.res_Mt + c) * a.pitch + tbase))
+                       : make_float4(0.f, 0.f, 0.f, 0.f);
+    }
+  }
+}
+
+// u = PReLU(dwconv3(gLN1(h)) + bd) for channels [c0, c0 + CPT) from their loaded taps.
+// TRAIN: A holds the pre-activation of h; PReLU(dw_in_slope) is applied here and the depthwise pre-activation is stored by the
+// CTA that holds n-tile 0 (store_side).
+template <int DCLS, bool INTERIOR, bool TRAIN, int CPT>
+__device__ __forceinline__ void dw_form(const PwArgs& a, int b, int c0, int tbase, int first, int step, float2 mr1, float pslope,
+                                        bool store_side, Raw<PRO_DW, CPT>& r, float4 (&v)[CPT], float2& dls, float2& dlss) {
   const float islope = TRAIN ? __ldg(a.dw_in_slope) : 0.f;
 #pragma unroll
-  for (int j = 0; j < CPW; ++j) {
-    const int c = ks * KS + pw * CPW + j;
+  for (int j = 0; j < CPT; ++j) {
+    const int c = c0 + j;
     const int cc = INTERIOR ? c : (c < a.K ? c : a.K - 1);
-    const float* hr = a.A + ((size_t)b * a.K + cc) * a.pitch;
-    float4 q[3];
+    float4* q = r.q[j];
+    if (TRAIN) {
 #pragma unroll
-    for (int k = 0; k < 3; ++k) {
-      int ts = first + k * step;
-      if (!INTERIOR) ts = ts < 0 ? 0 : (ts > a.pitch - 4 ? a.pitch - 4 : ts);
-      q[k] = __ldg(reinterpret_cast<const float4*>(hr + ts));
-      if (TRAIN) { q[k].x = prelu_f(q[k].x, islope); q[k].y = prelu_f(q[k].y, islope); q[k].z = prelu_f(q[k].z, islope); q[k].w = prelu_f(q[k].w, islope); }
+      for (int k = 0; k < 3; ++k) {
+        q[k].x = prelu_f(q[k].x, islope); q[k].y = prelu_f(q[k].y, islope); q[k].z = prelu_f(q[k].z, islope); q[k].w = prelu_f(q[k].w, islope);
+      }
     }
     const float pg = __ldg(a.dw_norm_g + cc), pb = __ldg(a.dw_norm_b + cc), pbd = __ldg(a.dw_b + cc);
     const float w0 = __ldg(a.dw_w + cc * 3), w1 = __ldg(a.dw_w + cc * 3 + 1), w2 = __ldg(a.dw_w + cc * 3 + 2);
     const float gsc = pg * mr1.y, gsh = pb - mr1.x * mr1.y * pg;
+    float4 pre;
     v[j] = dw_channel<DCLS, INTERIOR, TRAIN>(q[0], q[1], q[2], gsc, gsh, w0, w1, w2, pbd, pslope, first, step, tbase, a.frames, c < a.K,
-                                             dls, dlss, &pre[j]);
+                                             dls, dlss, &pre);
+    if (TRAIN && store_side && c < a.K) *reinterpret_cast<float4*>(a.dw_u_pre_out + ((size_t)b * a.K + c) * a.pitch + tbase) = pre;
   }
 }
 
-// F16 kernels fit two CTAs per SM (66 KB of shared memory each): measured 27.0 vs 36.7 ms per cfg2 step with one (H100 SXM, 700 W),
-// despite a few spilled registers under the 128-register cap.  The tf32 kernels need 130 KB, so one CTA per SM and no cap.
+// F16 kernels fit two CTAs per SM (82 KB of shared memory for the channel-split tile, 66 KB for the time-split one).  The tf32
+// kernels need 130 KB, so one CTA per SM and no register cap.
 template <int PRO, int EPI, int NPASS, bool F16, bool TRAIN>
 __global__ void __launch_bounds__(THREADS, F16 ? 2 : 1) k_pw_wgmma(const TcArgs g) {
-  constexpr int NPREC = NPASS == 3 ? 2 : 1;                   // precisions staged per operand (hi [, lo])
-  constexpr uint32_t ROWB = F16 ? 64u : 128u;                 // bytes of one operand row (32 channels)
-  constexpr uint32_t A_BYTES = TM * ROWB, W_BYTES = NT * ROWB;  // one precision of a slab
-  constexpr uint32_t STAGE_BYTES = NPREC * (A_BYTES + W_BYTES);
-  constexpr uint32_t LAYOUT = F16 ? ptx::SW64 : ptx::SW128;
+  constexpr bool CSPLIT = chan_split<PRO, EPI, F16>();
+  constexpr int TMC = tile_frames<PRO, EPI, F16>();          // frames of the CTA tile
+  constexpr int NWG = CSPLIT ? 2 : 1;                          // n-tiles staged per slab
+  constexpr int LPR = TMC / 4;                                 // lanes per channel (4 time steps per lane)
+  constexpr int CPT = CPW * LPR / 32;                          // channels a thread forms per slab: 4, or 2 with the channel split
+  constexpr int NPREC = NPASS == 3 ? 2 : 1;                    // precisions staged per operand (hi [, lo])
+  constexpr uint32_t ROWB = F16 ? 64u : 128u;                  // bytes of 32 channels
+  constexpr uint32_t A_BYTES = TMC * ROWB, W_BYTES = NT * ROWB;  // one precision of a slab
+  constexpr uint32_t STAGE_BYTES = NPREC * (A_BYTES + NWG * W_BYTES);
+  static_assert(F16 || CPT == CPW, "the K-major tf32 store takes a warp's 4 channels per time step");
   extern __shared__ uint8_t smem_raw[];
   const uint32_t raw = ptx::smem_u32(smem_raw);
   const uint32_t base = (raw + 1023u) & ~1023u;  // swizzle atoms need 1024-byte alignment
@@ -93,7 +144,7 @@ __global__ void __launch_bounds__(THREADS, F16 ? 2 : 1) k_pw_wgmma(const TcArgs 
   const PwArgs& a = g.a;
 
   // item -> (group of output-channel tiles, time tile, sample); the groups of one time tile are adjacent (activations shared in L2)
-  const int n_groups = g.n_tiles / g.nt_per_cta;
+  const int n_groups = g.n_groups;
   const int ngrp = (int)blockIdx.x % n_groups;
   const int tt = ((int)blockIdx.x / n_groups) % g.t_tiles;
   const int b = (int)blockIdx.x / (n_groups * g.t_tiles);
@@ -112,31 +163,39 @@ __global__ void __launch_bounds__(THREADS, F16 ? 2 : 1) k_pw_wgmma(const TcArgs 
   if (F16 && a.act_scale) act_s = __ldg(a.act_scale);
   float pslope = 0.f;
   if (PRO == PRO_PRELU || PRO == PRO_DW) pslope = __ldg(a.pro_slope);
-  const int tbase = tt * TM + lane * 4;  // first of this thread's 4 time steps
+  const int c_thr = warp * CPW + (lane / LPR) * CPT;  // first of this thread's CPT channels within a slab
+  const int tbase = tt * TMC + (lane % LPR) * 4;      // first of this thread's 4 time steps
   float2 mr1 = make_float2(0.f, 1.f), mr_res = make_float2(0.f, 1.f);
   if (PRO == PRO_DW) mr1 = gln_mean_rstd(a.dw_stats_in + 2 * b, (double)a.K * (double)a.frames, a.dw_eps);
   if (PRO == PRO_RES) mr_res = gln_mean_rstd(a.res_stats + 2 * b, a.res_n, a.res_eps);
-  int dcls = 4;
+  int dcls = 4, first = tbase, step = 0;
   bool dw_interior = false;
   if (PRO == PRO_DW) {
     const int d = a.dw_dilation;
     dcls = d >= 4 ? 4 : d;
+    step = dcls == 4 ? d : 4;  // d < 4: the aligned window [t - 4, t + 8)
+    first = dcls == 4 ? tbase - a.dw_pad_left : tbase - 4;
     const int reach = d >= 4 ? d : 4;  // furthest sample touched on either side of the tile
-    dw_interior = (tt * TM - reach >= 0) && (tt * TM + TM - 1 + reach + 3 < a.frames) && (a.K % KS == 0) && (a.dw_pad_left == d);
+    dw_interior = (tt * TMC - reach >= 0) && (tt * TMC + TMC - 1 + reach + 3 < a.frames) && (a.K % KS == 0) && (a.dw_pad_left == d);
   }
-  const float* Ab = a.A + (size_t)b * a.K * a.pitch + tbase;
   if (EPI == EPI_MASKDEC)
     for (int i = threadIdx.x; i < TM * 16; i += THREADS) dacc[i] = 0.f;
 
   for (int ntl = 0; ntl < g.nt_per_cta; ++ntl) {
-  const int nt = ngrp * g.nt_per_cta + ntl;
-  const int n0 = nt * NT;
-  const uint8_t* wsrc = reinterpret_cast<const uint8_t*>(g.wimg) + (size_t)nt * g.k_slabs * NPREC * W_BYTES;
+  // nt0: first n-tile of the CTA (the CTA holding n-tile 0 also stores the prologue's side outputs); nt: this warpgroup's n-tile
+  const int nt0 = CSPLIT ? 2 * ngrp : ngrp * g.nt_per_cta + ntl;
+  const int nt = CSPLIT ? nt0 + wg : nt0;
+  const bool wg_live = nt < g.n_tiles;  // false only for the second warpgroup of the last CTA at an odd n-tile count
+  const int nw = CSPLIT ? min(2, g.n_tiles - nt0) : 1;  // n-tiles whose weights a stage holds
+  const bool store_side = nt0 == 0;
+  const uint8_t* wsrc = reinterpret_cast<const uint8_t*>(g.wimg) + (size_t)nt0 * g.k_slabs * NPREC * W_BYTES;
   float2 dls = make_float2(0.f, 0.f), dlss = make_float2(0.f, 0.f);
   float acc[64];
 #pragma unroll
   for (int i = 0; i < 64; ++i) acc[i] = 0.f;
 
+  Raw<PRO, CPT> cur;
+  load_raw<PRO, CPT>(a, b, c_thr, tbase, first, step, dw_interior, cur);
   for (int ks = 0; ks < g.k_slabs; ++ks) {
     const int gk = ntl * g.k_slabs + ks;  // slab counter of the CTA: stage and mbarrier phase
     const int s = gk & 1;
@@ -144,43 +203,33 @@ __global__ void __launch_bounds__(THREADS, F16 ? 2 : 1) k_pw_wgmma(const TcArgs 
     // the stage was last read by the MMAs of slab ks - 2, complete in both warpgroups (wait + barrier at the end of ks - 1)
     if (threadIdx.x == 0) {
       const uint32_t fb = ptx::smem_u32(&wbar[s]);
-      ptx::mbar_arrive_expect_tx(fb, NPREC * W_BYTES);
-      ptx::bulk_g2s(st_base + NPREC * A_BYTES, wsrc + (size_t)ks * NPREC * W_BYTES, NPREC * W_BYTES, fb);
+      ptx::mbar_arrive_expect_tx(fb, (uint32_t)nw * NPREC * W_BYTES);
+      for (int w = 0; w < nw; ++w)
+        ptx::bulk_g2s(st_base + NPREC * (A_BYTES + w * W_BYTES), wsrc + ((size_t)w * g.k_slabs + ks) * NPREC * W_BYTES, NPREC * W_BYTES, fb);
     }
-    float4 v[CPW];
-    if (PRO == PRO_DW) {
-      float4 pre[CPW];
+    const int c0 = ks * KS + c_thr;
+    float4 v[CPT];
+    if constexpr (PRO == PRO_DW) {
       if (dw_interior) {
-        if (dcls == 4) dw_slab<4, true, TRAIN>(a, b, ks, warp, tbase, mr1, pslope, v, pre, dls, dlss);
-        else if (dcls == 2) dw_slab<2, true, TRAIN>(a, b, ks, warp, tbase, mr1, pslope, v, pre, dls, dlss);
-        else dw_slab<1, true, TRAIN>(a, b, ks, warp, tbase, mr1, pslope, v, pre, dls, dlss);
+        if (dcls == 4) dw_form<4, true, TRAIN>(a, b, c0, tbase, first, step, mr1, pslope, store_side, cur, v, dls, dlss);
+        else if (dcls == 2) dw_form<2, true, TRAIN>(a, b, c0, tbase, first, step, mr1, pslope, store_side, cur, v, dls, dlss);
+        else dw_form<1, true, TRAIN>(a, b, c0, tbase, first, step, mr1, pslope, store_side, cur, v, dls, dlss);
       } else {
-        if (dcls == 4) dw_slab<4, false, TRAIN>(a, b, ks, warp, tbase, mr1, pslope, v, pre, dls, dlss);
-        else if (dcls == 2) dw_slab<2, false, TRAIN>(a, b, ks, warp, tbase, mr1, pslope, v, pre, dls, dlss);
-        else dw_slab<1, false, TRAIN>(a, b, ks, warp, tbase, mr1, pslope, v, pre, dls, dlss);
-      }
-      if (TRAIN && nt == 0) {
-#pragma unroll
-        for (int j = 0; j < CPW; ++j) {
-          const int k = ks * KS + warp * CPW + j;
-          if (k < a.K) *reinterpret_cast<float4*>(a.dw_u_pre_out + ((size_t)b * a.K + k) * a.pitch + tbase) = pre[j];
-        }
+        if (dcls == 4) dw_form<4, false, TRAIN>(a, b, c0, tbase, first, step, mr1, pslope, store_side, cur, v, dls, dlss);
+        else if (dcls == 2) dw_form<2, false, TRAIN>(a, b, c0, tbase, first, step, mr1, pslope, store_side, cur, v, dls, dlss);
+        else dw_form<1, false, TRAIN>(a, b, c0, tbase, first, step, mr1, pslope, store_side, cur, v, dls, dlss);
       }
     } else {
 #pragma unroll
-      for (int j = 0; j < CPW; ++j) {
-        const int k = ks * KS + warp * CPW + j;
-        v[j] = k < a.K ? __ldg(reinterpret_cast<const float4*>(Ab + (size_t)k * a.pitch)) : make_float4(0.f, 0.f, 0.f, 0.f);
-      }
+      for (int j = 0; j < CPT; ++j) v[j] = cur.q[j][0];
       if (PRO == PRO_RES) {
         // x_new = x + rstd2*r + (v1 - mean2*rstd2*v2): the previous block's residual update, applied on the fly;
-        // the n-tile-0 CTA of each time tile also writes x_new for the block after next
-        const float* Rb = a.res_r + (size_t)b * a.res_Mt * a.pitch + tbase;
+        // the CTA holding n-tile 0 of each time tile also writes x_new for the block after next
 #pragma unroll
-        for (int j = 0; j < CPW; ++j) {
-          const int k = ks * KS + warp * CPW + j;
+        for (int j = 0; j < CPT; ++j) {
+          const int k = c0 + j;
           const int kc = k < a.K ? k : a.K - 1;
-          const float4 r = k < a.K ? __ldg(reinterpret_cast<const float4*>(Rb + (size_t)k * a.pitch)) : make_float4(0.f, 0.f, 0.f, 0.f);
+          const float4 r = cur.q[j][PRO == PRO_RES ? 1 : 0];
           const float cst = __ldg(a.res_v1 + kc) - mr_res.x * mr_res.y * __ldg(a.res_v2 + kc);
           float4 xn;
           xn.x = fmaf(mr_res.y, r.x, v[j].x + cst); xn.y = fmaf(mr_res.y, r.y, v[j].y + cst);
@@ -191,35 +240,45 @@ __global__ void __launch_bounds__(THREADS, F16 ? 2 : 1) k_pw_wgmma(const TcArgs 
           if (tbase + 3 >= a.frames) xn.w = 0.f;
           if (k >= a.K) xn = make_float4(0.f, 0.f, 0.f, 0.f);
           v[j] = xn;
-          if (nt == 0 && k < a.K) *reinterpret_cast<float4*>(a.res_x_out + ((size_t)b * a.K + k) * a.pitch + tbase) = xn;
+          if (store_side && k < a.K) *reinterpret_cast<float4*>(a.res_x_out + ((size_t)b * a.K + k) * a.pitch + tbase) = xn;
         }
       }
       if (PRO == PRO_PRELU) {
 #pragma unroll
-        for (int j = 0; j < CPW; ++j) {
+        for (int j = 0; j < CPT; ++j) {
           v[j].x = prelu_f(v[j].x, pslope); v[j].y = prelu_f(v[j].y, pslope);
           v[j].z = prelu_f(v[j].z, pslope); v[j].w = prelu_f(v[j].w, pslope);
         }
       }
     }
-    // K-major store: row = time step, this warp's 4 channels are 4 adjacent elements of the row
+    // the next slab's loads go out as soon as this slab's are consumed: they are in flight during its store and MMAs.  (Issuing
+    // them before the forming would keep two slabs of loads in registers, which PRO_DW cannot afford under the 128-register cap.)
+    if (ks + 1 < g.k_slabs) load_raw<PRO, CPT>(a, b, (ks + 1) * KS + c_thr, tbase, first, step, dw_interior, cur);
     uint8_t* sa = smem + SMEM_HEADER + (size_t)s * STAGE_BYTES;
+    if (F16) {
+      // MN-major SWIZZLE_128B (ptx::wg_desc_mn128): row = slab channel, 128 B = 64 consecutive frames, 16-byte chunk index XOR
+      // channel % 8; 8 channels per 1 KB atom, 4 atoms down the slab; each 64-frame half of a 128-frame tile is its own column of
+      // atoms (4 KB apart).  A thread's 4 frames are one 8-byte store per piece, and a warp's store covers two 128-byte rows.
+      const uint32_t f = (uint32_t)(tbase - tt * TMC);
 #pragma unroll
-    for (int e = 0; e < 4; ++e) {
-      const int t = lane * 4 + e;
-      float x[CPW];
-#pragma unroll
-      for (int j = 0; j < CPW; ++j) x[j] = e == 0 ? v[j].x : e == 1 ? v[j].y : e == 2 ? v[j].z : v[j].w;
-      if (F16) {
-        // SWIZZLE_64B: rows of 64 B, 16-byte chunk (8 channels) index XOR (row / 2) % 4
-        const uint32_t off = (uint32_t)t * 64u + (((uint32_t)(warp >> 1) ^ (uint32_t)((t >> 1) & 3)) << 4) + (uint32_t)(warp & 1) * 8u;
+      for (int j = 0; j < CPT; ++j) {
+        const uint32_t c = (uint32_t)(c_thr + j);
+        const uint32_t off = (f >> 6) * 4096u + (c >> 3) * 1024u + (c & 7) * 128u + ((((f >> 3) & 7) ^ (c & 7)) << 4) + (f & 7) * 2u;
         uint2 h2, l2;
-        ptx::split_f16x2(x[0] * act_s, x[1] * act_s, h2.x, l2.x);
-        ptx::split_f16x2(x[2] * act_s, x[3] * act_s, h2.y, l2.y);
+        ptx::split_f16x2(v[j].x * act_s, v[j].y * act_s, h2.x, l2.x);
+        ptx::split_f16x2(v[j].z * act_s, v[j].w * act_s, h2.y, l2.y);
         *reinterpret_cast<uint2*>(sa + off) = h2;
         *reinterpret_cast<uint2*>(sa + A_BYTES + off) = l2;
-      } else {
-        // SWIZZLE_128B: rows of 128 B, 16-byte chunk (4 channels) index XOR row % 8
+      }
+    } else {
+      // K-major SWIZZLE_128B (wgmma reads tf32 K-major only): row = time step, 128 B = 32 channels, 16-byte chunk (this warp's 4
+      // channels) index XOR row % 8
+#pragma unroll
+      for (int e = 0; e < 4; ++e) {
+        const int t = lane * 4 + e;
+        float x[CPW];
+#pragma unroll
+        for (int j = 0; j < CPW; ++j) x[j] = e == 0 ? v[j].x : e == 1 ? v[j].y : e == 2 ? v[j].z : v[j].w;
         const uint32_t off = (uint32_t)t * 128u + (((uint32_t)warp ^ (uint32_t)(t & 7)) << 4);
         float4 hi, lo;
         hi.x = ptx::hi_tf32(x[0]); hi.y = ptx::hi_tf32(x[1]); hi.z = ptx::hi_tf32(x[2]); hi.w = ptx::hi_tf32(x[3]);
@@ -231,29 +290,48 @@ __global__ void __launch_bounds__(THREADS, F16 ? 2 : 1) k_pw_wgmma(const TcArgs 
     ptx::fence_proxy_async_smem();
     __syncthreads();
     ptx::mbar_wait(ptx::smem_u32(&wbar[s]), (uint32_t)(gk >> 1) & 1u);
-    const uint32_t a_hi = st_base + (uint32_t)wg * 64u * ROWB, a_lo = a_hi + A_BYTES;
-    const uint32_t w_hi = st_base + NPREC * A_BYTES, w_lo = w_hi + W_BYTES;
-    ptx::wg_fence();
+    if (wg_live) {
+      // time split: warpgroup wg reads frames [64 wg, 64 wg + 64) (4 KB column / 64 K-major rows on); channel split: the whole slab
+      const uint32_t a_hi = st_base + (CSPLIT ? 0u : (uint32_t)wg * 64u * ROWB), a_lo = a_hi + A_BYTES;
+      const uint32_t w_hi = st_base + NPREC * (A_BYTES + (CSPLIT ? (uint32_t)wg * W_BYTES : 0u)), w_lo = w_hi + W_BYTES;
+      ptx::wg_fence();
 #pragma unroll
-    for (int kk = 0; kk < (F16 ? KS / 16 : KS / 8); ++kk) {  // 32 bytes of the rows per instruction
-      const uint64_t dah = ptx::wg_desc(a_hi + kk * 32, 8 * ROWB, LAYOUT), dwh = ptx::wg_desc(w_hi + kk * 32, 8 * ROWB, LAYOUT);
-      if (F16) ptx::wg_mma_f16(acc, dah, dwh); else ptx::wg_mma_tf32(acc, dah, dwh);
-      if (NPASS == 3) {
-        const uint64_t dal = ptx::wg_desc(a_lo + kk * 32, 8 * ROWB, LAYOUT), dwl = ptx::wg_desc(w_lo + kk * 32, 8 * ROWB, LAYOUT);
-        if (F16) { ptx::wg_mma_f16(acc, dal, dwh); ptx::wg_mma_f16(acc, dah, dwl); }
-        else { ptx::wg_mma_tf32(acc, dal, dwh); ptx::wg_mma_tf32(acc, dah, dwl); }
+      for (int kk = 0; kk < (F16 ? KS / 16 : KS / 8); ++kk) {  // 16 fp16 / 8 tf32 channels per instruction
+        if (F16) {
+          // A: 16 channels = 2 atoms per step (SBO 1 KB between 8-channel atoms; LBO, the next 64 frames, is never reached at M = 64)
+          const uint64_t dah = ptx::wg_desc_mn128(a_hi + kk * 2048, 4096u, 1024u), dwh = ptx::wg_desc(w_hi + kk * 32, 8 * ROWB, ptx::SW64);
+          ptx::wg_mma_f16(acc, dah, dwh);
+          if (NPASS == 3) {
+            const uint64_t dal = ptx::wg_desc_mn128(a_lo + kk * 2048, 4096u, 1024u), dwl = ptx::wg_desc(w_lo + kk * 32, 8 * ROWB, ptx::SW64);
+            ptx::wg_mma_f16(acc, dal, dwh);
+            ptx::wg_mma_f16(acc, dah, dwl);
+          }
+        } else {
+          const uint64_t dah = ptx::wg_desc(a_hi + kk * 32, 8 * ROWB, ptx::SW128), dwh = ptx::wg_desc(w_hi + kk * 32, 8 * ROWB, ptx::SW128);
+          ptx::wg_mma_tf32(acc, dah, dwh);
+          if (NPASS == 3) {
+            const uint64_t dal = ptx::wg_desc(a_lo + kk * 32, 8 * ROWB, ptx::SW128), dwl = ptx::wg_desc(w_lo + kk * 32, 8 * ROWB, ptx::SW128);
+            ptx::wg_mma_tf32(acc, dal, dwh);
+            ptx::wg_mma_tf32(acc, dah, dwl);
+          }
+        }
       }
+      ptx::wg_commit();
+      ptx::wg_wait<1>();  // the MMAs of slab ks - 1 are done: its stage may be refilled
     }
-    ptx::wg_commit();
-    ptx::wg_wait<1>();  // the MMAs of slab ks - 1 are done: its stage may be refilled
     __syncthreads();
   }
   ptx::wg_wait<0>();
 
-  if (PRO == PRO_DW && nt == 0) {
+  if (PRO == PRO_DW && store_side) {
     const double sd = warp_sum_d((double)dls.x + (double)dls.y), ssd = warp_sum_d((double)dlss.x + (double)dlss.y);
     if (lane == 0) { atomicAdd(&a.dw_stats_out[2 * b], sd); atomicAdd(&a.dw_stats_out[2 * b + 1], ssd); }
   }
+  if (!wg_live) continue;  // idle warpgroup (odd n-tile count): no outputs
+  // n0 reaches the epilogue through an opaque move: otherwise the compiler forms the epilogue's per-column addresses before the
+  // slab loop and spills them across it
+  int n0 = nt * NT;
+  asm volatile("" : "+r"(n0));
 
   // ===================================== EPILOGUE (on the accumulator fragment) =====================================
   float eslope = 0.f;
@@ -262,7 +340,7 @@ __global__ void __launch_bounds__(THREADS, F16 ? 2 : 1) k_pw_wgmma(const TcArgs 
   float2 mr = make_float2(0.f, 1.f);
   if (EPI == EPI_HEAD) mr = gln_mean_rstd(a.stats_in + 2 * b, a.n_in, a.eps);
   const float inv_act = 1.f / act_s;
-  const int row0 = wg * 64 + (warp & 3) * 16 + (lane >> 2);
+  const int row0 = (CSPLIT ? 0 : wg * 64) + (warp & 3) * 16 + (lane >> 2);  // frame within the tile
   float ls = 0.f, lss = 0.f;
   float dpart[2][16];  // EPI_MASKDEC: sum over this thread's columns of w_hat[n][t] * Dec[n][k], rows row0 and row0 + 8
 #pragma unroll
@@ -271,7 +349,7 @@ __global__ void __launch_bounds__(THREADS, F16 ? 2 : 1) k_pw_wgmma(const TcArgs 
   for (int i = 0; i < 64; ++i) {
     const int row = row0 + 8 * ((i >> 1) & 1);
     const int n = n0 + 8 * (i >> 2) + 2 * (lane & 3) + (i & 1);
-    const int t = tt * TM + row;
+    const int t = tt * TMC + row;
     if (n >= a.M) continue;
     const bool tvalid = t < a.frames;
     // F16: v * osc undoes the power-of-two row scaling of the weights and the activation scale (exact)
@@ -461,9 +539,15 @@ int eff_math(int M, int math) {
 }
 
 template <int PRO, int EPI, int NPASS, bool F16, bool TRAIN>
-int launch(const TcArgs& g, cudaStream_t st) {
+int launch(const TcArgs& g0, cudaStream_t st) {
   constexpr int NPREC = NPASS == 3 ? 2 : 1;
-  constexpr size_t smem = SMEM_HEADER + 1024 + (size_t)STAGES * NPREC * (TM + NT) * (F16 ? 64 : 128) + (EPI == EPI_MASKDEC ? TM * 16 * 4 : 0);
+  constexpr bool CSPLIT = chan_split<PRO, EPI, F16>();
+  constexpr int TMC = tile_frames<PRO, EPI, F16>();
+  constexpr size_t smem = SMEM_HEADER + 1024 + (size_t)STAGES * NPREC * (TMC + (CSPLIT ? 2 : 1) * NT) * (F16 ? 64 : 128) +
+                          (EPI == EPI_MASKDEC ? TM * 16 * 4 : 0);
+  TcArgs g = g0;
+  g.t_tiles = g.a.pitch / TMC;
+  g.n_groups = CSPLIT ? (g.n_tiles + 1) / 2 : g.n_tiles / g.nt_per_cta;
   static bool attr_done[CTN_MAX_DEVICES] = {false};  // the opt-in is per device (context)
   const int dev = ctn_current_device();
   if (!attr_done[dev]) {
@@ -471,7 +555,7 @@ int launch(const TcArgs& g, cudaStream_t st) {
     if (e != cudaSuccess) return (int)e;
     attr_done[dev] = true;
   }
-  const long long grid = (long long)g.a.B * g.t_tiles * (g.n_tiles / g.nt_per_cta);
+  const long long grid = (long long)g.a.B * g.t_tiles * g.n_groups;
   if (grid > 0x7fffffffLL) return CTN_EUNSUPPORTED;
   k_pw_wgmma<PRO, EPI, NPASS, F16, TRAIN><<<(unsigned)grid, THREADS, smem, st>>>(g);
   CTN_COUNT_LAUNCH();
@@ -529,7 +613,6 @@ int launch_wgmma(const PwArgs& a, int pro, int epi, int pmath, cudaStream_t st) 
   g.wimg = a.wimg;
   g.n_tiles = (a.M + NT - 1) / NT;
   g.k_slabs = (a.K + KS - 1) / KS;
-  g.t_tiles = a.pitch / TM;
   g.oscale = math == CTN_MATH_F16X3
                  ? reinterpret_cast<const float*>(reinterpret_cast<const uint8_t*>(a.wimg) + wimg_f16_image_bytes(NT, g.n_tiles, g.k_slabs))
                  : nullptr;

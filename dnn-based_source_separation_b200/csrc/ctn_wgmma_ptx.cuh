@@ -126,7 +126,7 @@ __device__ __forceinline__ void st_peer_v4(uint32_t local_addr, uint32_t rank, u
 
 // ---- wgmma (Hopper warpgroup MMA) -----------------------------------------------------------------------------------
 // D (64 x 128, fp32, registers of the 128 threads of a warpgroup) += A (64 x K, shared memory) * B (128 x K, shared memory)^T.
-// Both operands K-major.  Accumulator fragment of thread (warp w of the group, lane l), register i:
+// B K-major; A K-major (tf32) or MN-major (f16).  Accumulator fragment of thread (warp w of the group, lane l), register i:
 //   row = 16 w + l / 4 + 8 ((i / 2) % 2),  column = 8 (i / 4) + 2 (l % 4) + i % 2.
 __device__ __forceinline__ void wg_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
 __device__ __forceinline__ void wg_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
@@ -140,10 +140,11 @@ __device__ __forceinline__ void wg_mma_tf32(float (&d)[64], uint64_t da, uint64_
       : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
       : "l"(da), "l"(db));
 }
+// fp16: A is MN-major (imm-trans-a = 1, descriptor from wg_desc_mn128), B K-major
 __device__ __forceinline__ void wg_mma_f16(float (&d)[64], uint64_t da, uint64_t db) {
   asm volatile(
       "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, 1, 0;\n\twgmma.mma_async.sync.aligned.m64n128k16.f32.f16.f16 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, %64, %65, p, 1, 1, 0, 0;\n\t}"
+      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, %64, %65, p, 1, 1, 1, 0;\n\t}"
       : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
       : "l"(da), "l"(db));
 }
@@ -183,6 +184,15 @@ __device__ __forceinline__ float hi_tf32(float x) { return __uint_as_float((__fl
 constexpr uint32_t SW128 = 1u, SW64 = 2u;
 __device__ __forceinline__ uint64_t wg_desc(uint32_t smem_addr, uint32_t sbo_bytes, uint32_t layout) {
   return (uint64_t)((smem_addr & 0x3FFFFu) >> 4) | ((uint64_t)1 << 16) | ((uint64_t)(sbo_bytes >> 4) << 32) | ((uint64_t)layout << 62);
+}
+
+// Descriptor of an MN-major 16-bit operand in the canonical SWIZZLE_128B layout, ((T,8,m),(8,k)) : ((1,T,LBO),(8T,SBO)) with
+// T = 8 elements (PTX ISA, "Shared Memory Matrix Layout"): a 128-byte row holds 64 consecutive M (or N) elements of one k, 16-byte
+// chunk index XOR (row % 8); 8 rows of consecutive k form a 1 KB atom.  LBO = bytes between atoms along M (the next 64 elements),
+// SBO = bytes between atoms along K (the next 8 k).  The k-th 16-deep instruction step starts 2 atoms further on.
+__device__ __forceinline__ uint64_t wg_desc_mn128(uint32_t smem_addr, uint32_t lbo_bytes, uint32_t sbo_bytes) {
+  return (uint64_t)((smem_addr & 0x3FFFFu) >> 4) | ((uint64_t)(lbo_bytes >> 4) << 16) | ((uint64_t)(sbo_bytes >> 4) << 32) |
+         ((uint64_t)SW128 << 62);
 }
 
 }  // namespace ptx
