@@ -450,6 +450,37 @@ static void carve_model(Carver& cv, const ctn_config_t* c, int B, int pitch, Mod
   carve_tcn(cv, c, B, pitch, &ws->tcn);
 }
 
+int ctn_envelope_view(const ctn_config_t* c, int B, int frames, int path, void* mem, EnvelopeView* v) {
+  CTN_TRY(check_tcn_cfg(c, CTN_MAX_BLOCKS));
+  if (!mem || !v || B <= 0 || frames <= 0) return CTN_EINVAL;
+  const int pitch = ctn_pitch(frames);
+  TcnWs t;
+  if (path == ENV_TCN) {
+    Carver cv(mem);
+    carve_tcn(cv, c, B, pitch, &t);
+    v->x0_bound = t.x0_bound; v->x0_n = 1;
+  } else if (path == ENV_MODEL) {
+    Carver cv(mem);
+    ModelWs m;
+    carve_model(cv, c, B, pitch, &m);
+    t = m.tcn;
+    v->x0_bound = m.head.vb; v->x0_n = c->bottleneck;  // run_separator points the TCN's x0_bound here
+  } else if (path == ENV_TRAIN) {
+    void* tm = nullptr;
+    ctn_train_tcn_region(c, B, pitch, mem, &tm, &v->x0_bound);
+    if (!tm) return CTN_EUNSUPPORTED;
+    Carver cv(tm);
+    carve_tcn_train(cv, c, B, pitch, &t);
+    v->x0_n = c->bottleneck;
+  } else {
+    return CTN_EINVAL;
+  }
+  v->n = c->num_blocks * c->num_layers;
+  v->scales = t.scales;
+  for (int i = 0; i < v->n; ++i) { v->dwp[i] = t.dwp[i]; v->vb[i] = t.folds[i].vb; }
+  return CTN_OK;
+}
+
 extern "C" int ctn_workspace_bytes(const ctn_config_t* cfg, int batch, int T, size_t* bytes) {
   CTN_TRY(check_model_cfg(cfg));
   if (batch <= 0 || !bytes) return CTN_EINVAL;

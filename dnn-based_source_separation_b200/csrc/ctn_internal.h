@@ -144,6 +144,16 @@ struct ScaleJobs {
 int ctn_act_scales(const ScaleJobs& jobs, cudaStream_t st);
 // max |x| over rows x frames of a pitched tensor -> *out (float, must be zeroed by the caller)
 int ctn_absmax_pitch(const float* x, int rows, int frames, int pitch, float* out, cudaStream_t st);
+// Where a forward left its activation envelope: the workspace re-carved the way the forward carved it (ctn_api.cu), for the
+// verification hook to read back.  path ENV_TCN: ctn_tcn_fwd, or ctn_tcn_blocks_fwd with num_blocks = 1, num_layers = n_blocks;
+// ENV_MODEL: ctn_convtasnet_fwd / ctn_separator_fwd; ENV_TRAIN: ctn_convtasnet_fwd_train (fused TCN only).  x0_bound holds the
+// x0_n candidates the scales took |x_0| from (the measured max |x| of a stand-alone TCN, the head's row bounds of a model).
+enum { ENV_TCN = 0, ENV_MODEL = 1, ENV_TRAIN = 2 };
+struct EnvelopeView { const float* scales; const float* dwp[CTN_MAX_BLOCKS]; const float* vb[CTN_MAX_BLOCKS]; const float* x0_bound; int n, x0_n; };
+int ctn_envelope_view(const ctn_config_t* c, int B, int frames, int path, void* mem, EnvelopeView* v);
+// training workspace (ctn_train.cu): the region of the fused TCN forward (nullptr when the config does not fuse it) and the head's
+// row bounds
+void ctn_train_tcn_region(const ctn_config_t* c, int B, int pitch, void* mem, void** tcn_mem, const float** head_vb);
 
 // training forward of the TCN through the fused inference kernels (ctn_api.cu); per-block buffers owned by the training workspace
 struct TcnTrainHooks { float* const* x_keep; float* const* hpre; float* const* upre; };

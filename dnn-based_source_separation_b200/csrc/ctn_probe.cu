@@ -124,3 +124,27 @@ extern "C" int ctn_probe_rows(float* dst, size_t dst_bs, const float* src, size_
 extern "C" int ctn_probe_transpose(const float* W, float* Wt, int M, int K, ctn_stream_t stream) {
   return ctn_transpose(W, Wt, M, K, (cudaStream_t)stream);
 }
+
+static_assert((int)CTN_ENV_TCN == (int)ENV_TCN && (int)CTN_ENV_MODEL == (int)ENV_MODEL && (int)CTN_ENV_TRAIN == (int)ENV_TRAIN,
+              "envelope paths");
+
+extern "C" int ctn_probe_tcn_envelope(const ctn_config_t* cfg, int B, int frames, int path, void* workspace, float* scales_out,
+                                      float* dwp_out, float* vb_out, float* x0_out, ctn_stream_t stream) {
+  if (!scales_out || !dwp_out || !vb_out || !x0_out) return CTN_EINVAL;
+  EnvelopeView v;
+  CTN_TRY(ctn_envelope_view(cfg, B, frames, path, workspace, &v));
+  cudaStream_t st = (cudaStream_t)stream;
+  const size_t dwp_n = (size_t)ctn_round_up(cfg->hidden, 16) * 8, vb_n = (size_t)cfg->bottleneck + cfg->skip;
+  const cudaMemcpyKind d2d = cudaMemcpyDeviceToDevice;
+  cudaError_t e = cudaMemcpyAsync(scales_out, v.scales, sizeof(float) * (2 * v.n + 1), d2d, st);
+  if (e == cudaSuccess) e = cudaMemcpyAsync(x0_out, v.x0_bound, sizeof(float) * v.x0_n, d2d, st);
+  for (int i = 0; i < v.n && e == cudaSuccess; ++i) {
+    e = cudaMemcpyAsync(dwp_out + i * dwp_n, v.dwp[i], sizeof(float) * dwp_n, d2d, st);
+    if (e == cudaSuccess) e = cudaMemcpyAsync(vb_out + i * vb_n, v.vb[i], sizeof(float) * vb_n, d2d, st);
+  }
+  return (int)e;
+}
+
+extern "C" int ctn_probe_absmax_pitch(const float* x, int rows, int frames, int pitch, float* out, ctn_stream_t stream) {
+  return ctn_absmax_pitch(x, rows, frames, pitch, out, (cudaStream_t)stream);
+}

@@ -856,6 +856,14 @@ int gemm_raw(const ctn_config_t* c, TrainWs& ws, const float* W, int M, int K, c
 
 }  // namespace
 
+void ctn_train_tcn_region(const ctn_config_t* c, int B, int pitch, void* mem, void** tcn_mem, const float** head_vb) {
+  Carver cv(mem);
+  TrainWs ws;
+  carve_train(cv, c, B, pitch, &ws);
+  *tcn_mem = ws.tcn_mem;
+  *head_vb = ws.head.vb;
+}
+
 extern "C" int ctn_train_workspace_bytes(const ctn_config_t* cfg, int batch, int T, size_t* bytes) {
   CTN_TRY(check_train_cfg(cfg));
   if (batch <= 0 || !bytes) return CTN_EINVAL;

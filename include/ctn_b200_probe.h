@@ -122,6 +122,24 @@ int ctn_probe_rows(float* dst, size_t dst_bs, const float* src, size_t src_bs, i
 /* Wt (K, M) = W (M, K)^T */
 int ctn_probe_transpose(const float* W, float* Wt, int M, int K, ctn_stream_t stream);
 
+/* The activation envelope of the fp16-piece mode as a forward computed it (ctn_act_scales), read back from the workspace that
+ * forward ran in; call it after the forward, on the same stream.  path: which forward carved the workspace (B, frames, cfg as
+ * given to it):
+ *   CTN_ENV_TCN    ctn_tcn_fwd, or ctn_tcn_blocks_fwd with cfg.num_blocks = 1, cfg.num_layers = n_blocks;
+ *   CTN_ENV_MODEL  ctn_convtasnet_fwd (frames = ctn_frames of its T) or ctn_separator_fwd;
+ *   CTN_ENV_TRAIN  ctn_convtasnet_fwd_train (CTN_EUNSUPPORTED when the config does not run the fused TCN forward).
+ * With n = num_blocks * num_layers, Hp = hidden rounded up to 16 and Mt = bottleneck + skip, device buffers receive:
+ *   scales_out [2n + 1]   the operand scales: [2i] pw1 of block i (x_i), [2i + 1] pw2 (u_i), [2n] the mask contraction;
+ *   dwp_out    [n][Hp][8] the packed depthwise parameters (written by the forward only when sep_kernel == 3);
+ *   vb_out     [n][Mt]    each block's row bounds of its [out; skip] contraction (skip rows first when it has no out head;
+ *                         the Bc rows past them are then not written by the forward);
+ *   x0_out     the |x_0| candidates: [1] the measured max |x| (CTN_ENV_TCN), [bottleneck] the head's row bounds otherwise. */
+enum { CTN_ENV_TCN = 0, CTN_ENV_MODEL = 1, CTN_ENV_TRAIN = 2 };
+int ctn_probe_tcn_envelope(const ctn_config_t* cfg, int B, int frames, int path, void* workspace, float* scales_out, float* dwp_out,
+                           float* vb_out, float* x0_out, ctn_stream_t stream);
+/* *out = max(*out, max |x| over rows x frames of a pitched (rows, pitch) tensor); *out must hold a non-negative float */
+int ctn_probe_absmax_pitch(const float* x, int rows, int frames, int pitch, float* out, ctn_stream_t stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -87,7 +87,7 @@ ROWS = {
     "dw_d4_k96": _row("dw", "raw", 300, 96, 1000, "PRO_DW d = 4 (DCLS 4), interior + boundary, three n-tiles", d=4,
                       modes=MODES + ["f16x3-low"]),
     "dw_d12_k100": _row("dw", "raw", 128, 100, 129, "PRO_DW d = 12, K = 100", d=12, B=3),
-    "dw_d128_k96": _row("dw", "raw", 128, 96, 1000, "PRO_DW d = 128 = one tile", d=128),
+    "dw_d128_k96": _row("dw", "raw", 128, 96, 1000, "PRO_DW d = 128 = two 64-frame tiles", d=128),
     "dw_d520_k96": _row("dw", "raw", 128, 96, 500, "PRO_DW d = 520 > pitch = 512: every outer tap is padding", d=520),
     "dw_train_d2_k96": _row("dw", "raw", 300, 96, 1000, "PRO_DW TRAIN: PReLU on load, dw_u_pre_out, d = 2", d=2, train=True, B=3),
     "dw_train_d12_k100": _row("dw", "raw", 128, 100, 129, "PRO_DW TRAIN, boundary tiles only, d = 12", d=12, train=True),
@@ -110,6 +110,32 @@ ROWS = {
     "maskdec_nb512_s1_f129": _row("prelu", "maskdec", 512, 128, 129, "EPI_MASKDEC Nb = 512, S = 1", Nb=512, crop=0),
     "maskdec_nb40": _row("prelu", "maskdec", 80, 96, 129, "EPI_MASKDEC refused: Nb = 40 is no multiple of 128", Nb=40, crop=0,
                          refuse=True),
+    # ---- the pipelines' own shapes on the fp16 channel-split tile (64 frames x 2 n-tiles; side outputs from n-tile 0 only) ----
+    "res_k128_m512_b3": _row("res", "h", 512, 128, 1000, "pw1 shape: four n-tiles = two full groups, every warpgroup live", B=3),
+    "res_k128_m128": _row("res", "h", 128, 128, 1000, "one n-tile: warpgroup 1 idle in every CTA"),
+    "h_k128_m512": _row("none", "h", 512, 128, 1000, "block 0's pw1 shape (PRO_NONE)"),
+    **{f"dw_k512_m256_d{d}": _row("dw", "raw", 256, 512, 1000, f"pw2 shape, d = {d}" + (" = one 64-frame tile" if d == 64 else ""),
+                                  d=d) for d in (1, 2, 4, 64, 128)},
+    "dw_train_k512_m256_d2": _row("dw", "raw", 256, 512, 1000, "pw2 shape, TRAIN variant, d = 2", d=2, train=True),
+    "dw_k512_m128": _row("dw", "raw", 128, 512, 1000, "the last block's pw2 (skip head only): one n-tile", d=1),
+    **{f"res_k128_m512_f{T}": _row("res", "h", 512, 128, T, f"pw1 shape, frames = {T} at a 64-frame tile edge") for T in (63, 64, 65, 4001)},
+    **{f"dw_k512_m256_f{T}": _row("dw", "raw", 256, 512, T, f"pw2 shape, frames = {T} at a 64-frame tile edge", d=4)
+       for T in (63, 64, 65, 4001)},
+}
+
+# Headroom sweep: the f16x3 mode with the operand scale 2^k below the top of its range, on the pipelines' (pro, epi) pairs and
+# shapes.  The lo piece x s - hi is stored as a plain fp16, so far below the top it turns subnormal and the gate eventually
+# breaks; it must hold SWEEP_REQUIRED binades below the top, at least two more than the largest headroom test_act_envelope_gpu.py
+# measured on the paper config (17.3 binades at 60 s, DESIGN section 2).
+SWEEP_SHIFTS = (0, 9, 15, 18, 21)
+SWEEP_REQUIRED = 21
+SWEEP_ROWS = {
+    "pw1_res": _row("res", "h", 512, 128, 1000, "PRO_RES / EPI_H", B=2),
+    "pw1_none": _row("none", "h", 512, 128, 1000, "PRO_NONE / EPI_H (block 0)"),
+    "pw2_dw": _row("dw", "raw", 256, 512, 1000, "PRO_DW / EPI_RAW", d=4),
+    "pw2_dw_m128": _row("dw", "raw", 128, 512, 1000, "PRO_DW / EPI_RAW, M = 128 (last block)", d=4),
+    "mask": _row("prelu", "mask", 1024, 128, 1000, "PRO_PRELU / EPI_MASK", Nb=512),
+    "maskdec": _row("prelu", "maskdec", 1024, 128, 1000, "PRO_PRELU / EPI_MASKDEC", Nb=512, crop=4),
 }
 
 
@@ -223,8 +249,8 @@ def _supported(r, mode):
     return True
 
 
-def _run(c, r, mode, route=0):
-    """one probe call -> (status, outputs on cuda)"""
+def _run(c, r, mode, route=0, shift=None):
+    """one probe call -> (status, outputs on cuda); shift: f16x3 with the operand scale 2^shift below the top of its range"""
     B, M, K, T, pitch = r["B"], r["M"], r["K"], r["frames"], c["pitch"]
     a = ProbeArgs.from_buffer_copy(c["args"])
     out = {}
@@ -251,7 +277,9 @@ def _run(c, r, mode, route=0):
     scale = None
     if mode in ("f16x3", "f16x3-low"):
         # |operand| * s in [2^14, 2^15): the top of the legal range; f16x3-low: 2^-15 of that
-        e = 14 - math.floor(math.log2(c["pmax"])) - (15 if mode == "f16x3-low" else 0)
+        if shift is None:
+            shift = 15 if mode == "f16x3-low" else 0
+        e = 14 - math.floor(math.log2(c["pmax"])) - shift
         scale = torch.tensor([2.0 ** e], device=DEV)
         a.act_scale = scale.data_ptr()
     nbytes = probe_wimg_bytes(M, K, MATH[mode])
@@ -339,6 +367,22 @@ def _run_mode(name, c, r, mode):
         st1, out1 = _run(c, r, mode, route=1)
         assert st1 == N.CTN_OK and torch.equal(out1["D"], out["D"]), f"{name} {mode}: batched weight image differs"
     return " ".join(f"{k} {v:.3f}" for k, v in res.items())
+
+
+@pytest.mark.parametrize("name", list(SWEEP_ROWS))
+def test_pw_headroom_sweep(name):
+    r = SWEEP_ROWS[name]
+    c = _case("sweep_" + name, r)
+    ratios = {}
+    for k in SWEEP_SHIFTS:
+        st, out = _run(c, r, "f16x3", shift=k)
+        assert st == N.CTN_OK, (name, k, st)
+        y = out["D"] if r["epi"] == "maskdec" else out["D"][..., :r["frames"]]
+        ratios[k] = PC.gate_e(y, c["ref"].out["D"]) / c["ref"].bound("f16x3")
+    broken = [k for k in SWEEP_SHIFTS if ratios[k] > 1.0]
+    print(f"sweep {name} [{r['reaches']}]: e/bound " + ", ".join(f"2^-{k}: {v:.3f}" for k, v in ratios.items()) +
+          f"; gate breaks at {('2^-%d' % broken[0]) if broken else 'none of these'}")
+    assert all(ratios[k] <= 1.0 for k in SWEEP_SHIFTS if k <= SWEEP_REQUIRED), ratios
 
 
 def test_pw_host_refusals():
