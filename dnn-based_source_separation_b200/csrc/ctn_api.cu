@@ -269,8 +269,8 @@ static int run_tcn(const ctn_config_t* c, const ctn_block_params_t* blocks, TcnW
       // K_F: residual update with the deferred gLN2 (x += rstd2*r[:Bc] + c); the skip rows are reduced once at the end
       if (has_out && c->math == CTN_MATH_FP32) {
         StageTimer tm(CTN_ST_FIN, st);
-        CTN_TRY(ctn_finish_fwd(rb, ws->folds[i], st2, (double)H * (double)frames, c->eps_tcn, xbuf[0], ws->skip, B, Bc, Sc, 1,
-                               2 /* x rows only */, frames, pitch, st));
+        CTN_TRY(ctn_finish_fwd(rb, ws->folds[i], st2, (double)H * (double)frames, c->eps_tcn, xbuf[0], B, Bc, Sc, frames, pitch,
+                               st));
       }
     }
   }
@@ -290,7 +290,7 @@ static int run_tcn(const ctn_config_t* c, const ctn_block_params_t* blocks, TcnW
     float* xl = fuse_res ? xbuf[(n - 1) & 1] : ws->x;  // x_{n-1} (tensor-core modes defer every update to the next block)
     if (fuse_res && blocks[n - 1].out_w)
       CTN_TRY(ctn_finish_fwd(ws->rblk[n - 1], ws->folds[n - 1], ws->stats + (size_t)(2 * (n - 1) + 1) * B * 2, (double)H * (double)frames,
-                             c->eps_tcn, xl, ws->skip, B, Bc, Sc, 1, 2 /* x rows only */, frames, pitch, st));
+                             c->eps_tcn, xl, B, Bc, Sc, frames, pitch, st));
     *x_final = xl;
   }
   return CTN_OK;
@@ -618,6 +618,13 @@ __global__ void __launch_bounds__(256) k_stats_pitch(const float* __restrict__ x
   block_sum2_d(s, ss, red);
   if (threadIdx.x == 0) { atomicAdd(&stats[2 * b], s); atomicAdd(&stats[2 * b + 1], ss); }
 }
+int ctn_stats_pitch(const float* x, int B, int C, int frames, int pitch, double* stats, cudaStream_t st) {
+  const int gx = C < 64 ? C : 64;
+  k_stats_pitch<<<dim3(gx, B), 256, 0, st>>>(x, C, frames, pitch, stats);
+  CTN_COUNT_LAUNCH();
+  CTN_RETURN_IF_CUDA_ERR();
+  return CTN_OK;
+}
 
 extern "C" int ctn_separator_fwd(const ctn_config_t* cfg, const ctn_params_t* params, const float* w, int B, int frames,
                                  float* mask, void* workspace, size_t workspace_bytes, ctn_stream_t stream) {
@@ -640,10 +647,7 @@ extern "C" int ctn_separator_fwd(const ctn_config_t* cfg, const ctn_params_t* pa
   e = cudaMemsetAsync(ws.tcn.stats, 0, ws.tcn.stats_bytes, st);
   if (e != cudaSuccess) return (int)e;
   CTN_TRY(ctn_copy_to_pitch(w, ws.w, B * cfg->n_basis, frames, pitch, st));
-  int gx = cfg->n_basis < 64 ? cfg->n_basis : 64;
-  k_stats_pitch<<<dim3(gx, B), 256, 0, st>>>(ws.w, cfg->n_basis, frames, pitch, ws.stats0);
-  CTN_COUNT_LAUNCH();
-  CTN_RETURN_IF_CUDA_ERR();
+  CTN_TRY(ctn_stats_pitch(ws.w, B, cfg->n_basis, frames, pitch, ws.stats0, st));
   CTN_TRY(run_separator(cfg, params, &ws, B, frames, pitch, mask_p, st));
   CTN_TRY(ctn_copy_from_pitch(mask_p, mask, B * cfg->n_sources * cfg->n_basis, frames, pitch, st));
   return CTN_OK;

@@ -144,9 +144,7 @@ int ctn_causal_tcn(const ctn_config_t* c, const ctn_block_params_t* blocks, floa
     {
       StageTimer tm(CTN_ST_DW, st);
       CTN_TRY(ctn_cln_pitch_fwd(h, q.norm1_g, q.norm1_b, h, B, H, frames, pitch, c->eps_tcn, ws.cln, st));
-      k_dw_plain<<<grid_cb(H, B), 256, 0, st>>>(h, u, q.dw_w, q.dw_b, q.prelu2, H, frames, pitch, P, dil, pad_left);
-      CTN_COUNT_LAUNCH();
-      CTN_RETURN_IF_CUDA_ERR();
+      CTN_TRY(ctn_dw_plain_fwd(h, u, q.dw_w, q.dw_b, q.prelu2, B, H, frames, pitch, P, dil, pad_left, st));
       CTN_TRY(ctn_cln_pitch_fwd(u, q.norm2_g, q.norm2_b, u, B, H, frames, pitch, c->eps_tcn, ws.cln, st));
     }
     const int Mt = has_out ? Bc + Sc : Sc;
@@ -177,6 +175,14 @@ int ctn_block_wcat(const ctn_block_params_t& q, int Bc, int Sc, int H, float* wc
   if (e == cudaSuccess)
     e = cudaMemcpyAsync(wcat + (has_out ? (size_t)Bc * H : 0), q.skip_w, sizeof(float) * (size_t)Sc * H, cudaMemcpyDeviceToDevice, st);
   return e == cudaSuccess ? CTN_OK : (int)e;
+}
+
+int ctn_dw_plain_fwd(const float* h, float* u, const float* wd, const float* bd, const float* slope, int B, int C, int frames, int pitch,
+                     int P, int dil, int pad_left, cudaStream_t st) {
+  k_dw_plain<<<grid_cb(C, B), 256, 0, st>>>(h, u, wd, bd, slope, C, frames, pitch, P, dil, pad_left);
+  CTN_COUNT_LAUNCH();
+  CTN_RETURN_IF_CUDA_ERR();
+  return CTN_OK;
 }
 
 int ctn_bias_rows_fwd(float* y, const float* bias, int C, int B, int frames, int pitch, cudaStream_t st) {

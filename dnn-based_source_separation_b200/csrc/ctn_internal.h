@@ -171,9 +171,10 @@ int ctn_dw_fwd(const float* h, float* u, const float* norm_g, const float* norm_
                const float* slope, const double* stats_in, double* stats_out, int B, int H, int frames, int pitch, int P,
                int dilation, float eps, cudaStream_t st);
 
-// finishing: x += rstd2*outraw[:Bc] + c ; skip (+)= rstd2*outraw[Bc:] + c
-int ctn_finish_fwd(const float* outraw, const FoldedConv f, const double* stats2, double n2, float eps, float* x,
-                   float* skip, int B, int Bc, int Sc, int has_out, int skip_init, int frames, int pitch, cudaStream_t st);
+// finishing of a block with an output head: x += rstd2*outraw[:Bc] + c, outraw (B, Bc + Sc, pitch); its skip rows are reduced
+// by ctn_skip_reduce
+int ctn_finish_fwd(const float* outraw, const FoldedConv f, const double* stats2, double n2, float eps, float* x, int B, int Bc,
+                   int Sc, int frames, int pitch, cudaStream_t st);
 
 // deferred skip reduction: skip[b][m][t] = sum_i ( rstd2_i[b] * r_i[b][off_i + m][t] + (v1_i[off_i+m] - mean_i rstd_i v2_i[off_i+m]) )
 // over all residual blocks i -- reads every block's skip rows ONCE instead of read-modify-writing the accumulator per block
@@ -204,6 +205,11 @@ int ctn_causal_head(const ctn_config_t* c, const ctn_params_t* p, const float* w
 int ctn_res_skip_fwd(const float* r, int Mt, const float* xin, float* xout, float* skip, const float* bo, const float* bs, int Bc, int Sc,
                      int has_out, int skip_init, int B, int frames, int pitch, cudaStream_t st);
 int ctn_bias_rows_fwd(float* y, const float* bias, int C, int B, int frames, int pitch, cudaStream_t st);
+// u = PReLU(dwconv(h) + bd), P taps at dilation dil, h = 0 outside [0, frames) (the causal layout passes pad_left = (P-1) dil)
+int ctn_dw_plain_fwd(const float* h, float* u, const float* wd, const float* bd, const float* slope, int B, int C, int frames, int pitch,
+                     int P, int dil, int pad_left, cudaStream_t st);
+// stats[b] += (sum, sumsq) over c < C, t < frames of a (B, C, pitch) tensor, every element summed in double (ctn_api.cu)
+int ctn_stats_pitch(const float* x, int B, int C, int frames, int pitch, double* stats, cudaStream_t st);
 // a block's [out_w; skip_w] (skip_w alone when it has no output head) -> wcat (Mt, H), stream-ordered device copies
 int ctn_block_wcat(const ctn_block_params_t& q, int Bc, int Sc, int H, float* wcat, cudaStream_t st);
 

@@ -1,6 +1,8 @@
-// Verification hook (include/ctn_b200_probe.h): thin C entry points over the 1x1 contraction internals and the training path's
-// launchers (ctn_internal.h), so that tests can compare one operation with a high-precision reference.  No kernels here and no
-// pipeline calls these.
+// Verification hook (include/ctn_b200_probe.h): thin C entry points over the 1x1 contraction internals and the training and
+// inference paths' launchers (ctn_internal.h), so that tests can compare one operation with a high-precision reference.  No
+// kernels here and no pipeline calls these.
+#include <vector>
+
 #include "ctn_internal.h"
 #include "ctn_b200_probe.h"
 
@@ -147,4 +149,58 @@ extern "C" int ctn_probe_tcn_envelope(const ctn_config_t* cfg, int B, int frames
 
 extern "C" int ctn_probe_absmax_pitch(const float* x, int rows, int frames, int pitch, float* out, ctn_stream_t stream) {
   return ctn_absmax_pitch(x, rows, frames, pitch, out, (cudaStream_t)stream);
+}
+
+extern "C" int ctn_probe_fold(const ctn_fold_probe_t* jobs, int n, ctn_stream_t stream) {
+  if (!jobs || n <= 0) return CTN_EINVAL;
+  std::vector<FoldJob> fj((size_t)n);
+  for (int i = 0; i < n; ++i) {
+    const ctn_fold_probe_t& p = jobs[i];
+    fj[i] = FoldJob{p.W, p.bias, p.gamma, p.beta, FoldedConv{p.Wf, p.v1, p.v2, p.vb}, p.M, p.K, p.row_offset, p.R};
+  }
+  return ctn_fold_batch(fj.data(), n, (cudaStream_t)stream);
+}
+
+extern "C" int ctn_probe_dw_fwd(const float* h, float* u, const float* norm_g, const float* norm_b, const float* dw_w, const float* dw_b,
+                                const float* slope, const double* stats_in, double* stats_out, int B, int H, int frames, int pitch, int P,
+                                int dil, float eps, ctn_stream_t stream) {
+  return ctn_dw_fwd(h, u, norm_g, norm_b, dw_w, dw_b, slope, stats_in, stats_out, B, H, frames, pitch, P, dil, eps, (cudaStream_t)stream);
+}
+
+extern "C" int ctn_probe_finish(const float* r, const float* v1, const float* v2, const double* stats2, double n2, float eps, float* x,
+                                int B, int Bc, int Sc, int frames, int pitch, ctn_stream_t stream) {
+  const FoldedConv f{nullptr, const_cast<float*>(v1), const_cast<float*>(v2), nullptr};  // k_finish reads v1 / v2 only
+  return ctn_finish_fwd(r, f, stats2, n2, eps, x, B, Bc, Sc, frames, pitch, (cudaStream_t)stream);
+}
+
+extern "C" int ctn_probe_skip_reduce(const ctn_skip_probe_t* jobs, int n, double n2, float eps, float* skip, int B, int Sc, int frames,
+                                     int pitch, ctn_stream_t stream) {
+  if (!jobs || n <= 0 || n > CTN_MAX_BLOCKS) return CTN_EINVAL;
+  SkipJobs sj;
+  sj.n = n;
+  for (int i = 0; i < n; ++i) sj.j[i] = SkipJob{jobs[i].r, jobs[i].v1, jobs[i].v2, jobs[i].stats2, jobs[i].off, jobs[i].Mt};
+  return ctn_skip_reduce(sj, n2, eps, skip, B, Sc, frames, pitch, (cudaStream_t)stream);
+}
+
+extern "C" int ctn_probe_stats_pitch(const float* x, int B, int C, int frames, int pitch, double* stats, ctn_stream_t stream) {
+  return ctn_stats_pitch(x, B, C, frames, pitch, stats, (cudaStream_t)stream);
+}
+
+extern "C" int ctn_probe_dw_plain(const float* h, float* u, const float* wd, const float* bd, const float* slope, int B, int C, int frames,
+                                  int pitch, int P, int dil, int pad_left, ctn_stream_t stream) {
+  return ctn_dw_plain_fwd(h, u, wd, bd, slope, B, C, frames, pitch, P, dil, pad_left, (cudaStream_t)stream);
+}
+
+extern "C" int ctn_probe_res_skip(const float* r, int Mt, const float* xin, float* xout, float* skip, const float* bo, const float* bs,
+                                  int Bc, int Sc, int has_out, int skip_init, int B, int frames, int pitch, ctn_stream_t stream) {
+  return ctn_res_skip_fwd(r, Mt, xin, xout, skip, bo, bs, Bc, Sc, has_out, skip_init, B, frames, pitch, (cudaStream_t)stream);
+}
+
+extern "C" int ctn_probe_bias_rows(float* y, const float* bias, int C, int B, int frames, int pitch, ctn_stream_t stream) {
+  return ctn_bias_rows_fwd(y, bias, C, B, frames, pitch, (cudaStream_t)stream);
+}
+
+extern "C" int ctn_probe_cln_pitch(const float* x, const float* gamma, const float* beta, float* y, int B, int C, int frames, int pitch,
+                                   float eps, double* scratch, ctn_stream_t stream) {
+  return ctn_cln_pitch_fwd(x, gamma, beta, y, B, C, frames, pitch, eps, scratch, (cudaStream_t)stream);
 }

@@ -5,7 +5,7 @@
 //   K_A  (pointwise, EPI_H):   h = PReLU_a1(W1 x + b1)                      + (sum, sumsq) of h        -> stats1
 //   K_B  (ctn_dw_fwd):         u = PReLU_a2(dwconv_d(zero-pad(gLN1(h))) + bd) + (sum, sumsq) of u        -> stats2
 //   K_C  (pointwise, EPI_RAW): r = [Wo;Ws] diag(gamma2) u                   (gLN2 folded, see ctn_internal.h)
-//   K_F  (ctn_finish_fwd):     x += rstd2*r[:B] + c_o ;  skip += rstd2*r[B:] + c_s
+//   K_F  (ctn_finish_fwd):     x += rstd2*r[:B] + c_o   (the skip rows: ctn_skip_reduce, once over all blocks)
 #include "ctn_internal.h"
 
 // ------------------------------------------------------------------------------------------------
@@ -377,29 +377,22 @@ int ctn_dw_fwd(const float* h, float* u, const float* norm_g, const float* norm_
 }
 
 // ------------------------------------------------------------------------------------------------
-// finishing: residual + skip accumulation with the deferred gLN2 scale/shift
-// grid (pitch/512, Bc+Sc, B), block 128
+// finishing: residual update with the deferred gLN2 scale/shift, x += rstd2*r[:Bc] + c (the skip rows go to k_skip_reduce)
+// grid (pitch/512, Bc, B), block 128
 // ------------------------------------------------------------------------------------------------
 __global__ void __launch_bounds__(128) k_finish(const float* __restrict__ outraw, const float* __restrict__ v1,
                                                 const float* __restrict__ v2, const double* __restrict__ stats2, double n2,
-                                                float eps, float* __restrict__ x, float* __restrict__ skip, int Bc, int Sc,
-                                                int has_out, int skip_init, int frames, int pitch) {
+                                                float eps, float* __restrict__ x, int Bc, int Sc, int frames, int pitch) {
   const int b = blockIdx.z, m = blockIdx.y;
   const int t = (blockIdx.x * 128 + threadIdx.x) * 4;
   if (t >= pitch) return;
-  const int Mtot = has_out ? Bc + Sc : Sc;
   const float2 mr = gln_mean_rstd(stats2 + 2 * b, n2, eps);
   const float c = v1[m] - mr.x * mr.y * v2[m];
-  float4 r = *reinterpret_cast<const float4*>(outraw + ((size_t)b * Mtot + m) * pitch + t);
+  float4 r = *reinterpret_cast<const float4*>(outraw + ((size_t)b * (Bc + Sc) + m) * pitch + t);
   r.x = fmaf(mr.y, r.x, c); r.y = fmaf(mr.y, r.y, c); r.z = fmaf(mr.y, r.z, c); r.w = fmaf(mr.y, r.w, c);
-  float* dst;
-  bool accumulate;
-  if (has_out && m < Bc) { dst = x + ((size_t)b * Bc + m) * pitch + t; accumulate = true; }
-  else { dst = skip + ((size_t)b * Sc + (has_out ? m - Bc : m)) * pitch + t; accumulate = !skip_init; }
-  if (accumulate) {
-    const float4 o = *reinterpret_cast<const float4*>(dst);
-    r.x += o.x; r.y += o.y; r.z += o.z; r.w += o.w;
-  }
+  float* dst = x + ((size_t)b * Bc + m) * pitch + t;
+  const float4 o = *reinterpret_cast<const float4*>(dst);
+  r.x += o.x; r.y += o.y; r.z += o.z; r.w += o.w;
   if (t + 0 >= frames) r.x = 0.f;
   if (t + 1 >= frames) r.y = 0.f;
   if (t + 2 >= frames) r.z = 0.f;
@@ -407,12 +400,10 @@ __global__ void __launch_bounds__(128) k_finish(const float* __restrict__ outraw
   *reinterpret_cast<float4*>(dst) = r;
 }
 
-int ctn_finish_fwd(const float* outraw, const FoldedConv f, const double* stats2, double n2, float eps, float* x,
-                   float* skip, int B, int Bc, int Sc, int has_out, int skip_init, int frames, int pitch, cudaStream_t st) {
-  const int Mtot = has_out ? Bc + Sc : Sc;
-  // skip_init == 2: residual rows only (the skip rows are handled by ctn_skip_reduce)
-  dim3 grid((pitch + 511) / 512, skip_init == 2 ? Bc : Mtot, B);
-  k_finish<<<grid, 128, 0, st>>>(outraw, f.v1, f.v2, stats2, n2, eps, x, skip, Bc, Sc, has_out, skip_init, frames, pitch);
+int ctn_finish_fwd(const float* outraw, const FoldedConv f, const double* stats2, double n2, float eps, float* x, int B, int Bc,
+                   int Sc, int frames, int pitch, cudaStream_t st) {
+  dim3 grid((pitch + 511) / 512, Bc, B);
+  k_finish<<<grid, 128, 0, st>>>(outraw, f.v1, f.v2, stats2, n2, eps, x, Bc, Sc, frames, pitch);
   CTN_COUNT_LAUNCH();
   CTN_RETURN_IF_CUDA_ERR();
   return CTN_OK;

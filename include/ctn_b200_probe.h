@@ -1,10 +1,11 @@
-/* ctn_b200_probe.h -- verification hook: the library's 1x1 contraction kernels and the training path's streaming kernels
- * called one at a time.
+/* ctn_b200_probe.h -- verification hook: the library's 1x1 contraction kernels, the training path's streaming kernels and the
+ * inference forward's gLN folds, depthwise, residual / skip and statistics kernels called one at a time.
  *
  * The pipelines reach the pointwise contraction kernels (ctn_wgmma.cu, ctn_tcn_simt.cu), the weight-gradient kernels
- * (ctn_wgrad_wgmma.cu, ctn_train.cu) and the training path's streaming kernels (ctn_train.cu) only inside whole models, where
- * normalisations and nonlinearities dilute a kernel's error before any output is compared.  These entry points expose those
- * kernels directly so that a test can compare one operation with a high-precision reference.  No pipeline calls them; they add
+ * (ctn_wgrad_wgmma.cu, ctn_train.cu), the training path's streaming kernels (ctn_train.cu) and the forward's streaming kernels
+ * (ctn_tcn_simt.cu, ctn_causal.cu, ctn_norm.cu, ctn_api.cu) only inside whole models, where normalisations and nonlinearities
+ * dilute a kernel's error before any output is compared.  These entry points expose those kernels directly, through the launchers
+ * the pipelines call, so that a test can compare one operation with a high-precision reference.  No pipeline calls them; they add
  * no kernels.  Conventions as in ctn_b200.h.
  */
 #ifndef CTN_B200_PROBE_H
@@ -139,6 +140,59 @@ int ctn_probe_tcn_envelope(const ctn_config_t* cfg, int B, int frames, int path,
                            float* vb_out, float* x0_out, ctn_stream_t stream);
 /* *out = max(*out, max |x| over rows x frames of a pitched (rows, pitch) tensor); *out must hold a non-negative float */
 int ctn_probe_absmax_pitch(const float* x, int rows, int frames, int pitch, float* out, ctn_stream_t stream);
+
+/* The inference forward's streaming kernels, through the launchers ctn_convtasnet_fwd / ctn_separator_fwd / ctn_tcn_fwd /
+ * ctn_tcn_blocks_fwd and the causal pipeline call.  Tensors (B, C, pitch) floats as above; stats (B, 2) doubles, "+=". */
+/* One gLN fold into rows [row_offset, row_offset + M) of (Wf, v1, v2, vb):  Wf[m][k] = W[m][k] gamma[k],
+ * v1[m] = sum_k W[m][k] beta[k] + bias[m],  v2[m] = sum_k Wf[m][k],  vb[m] = sum_k |W[m][k]| (|gamma[k]| R + |beta[k]|) + |bias[m]|.
+ * bias and vb nullable. */
+typedef struct ctn_fold_probe {
+  const float* W;
+  const float* bias;
+  const float* gamma;
+  const float* beta;
+  int32_t M, K, row_offset;
+  float R;
+  float* Wf;
+  float* v1;
+  float* v2;
+  float* vb;
+} ctn_fold_probe_t;
+/* n >= 1 jobs in one call; more than one launch's worth are split the way the pipelines' preparation splits them */
+int ctn_probe_fold(const ctn_fold_probe_t* jobs, int n, ctn_stream_t stream);
+/* u = PReLU(dwconv(gLN1(h)) + bd; slope) with gLN1 from stats_in over H frames elements, P taps at dilation dil, pad_left
+ * ((P-1) dil) / 2 ; stats_out[b] += (sum, sumsq) of u */
+int ctn_probe_dw_fwd(const float* h, float* u, const float* norm_g, const float* norm_b, const float* dw_w, const float* dw_b,
+                     const float* slope, const double* stats_in, double* stats_out, int B, int H, int frames, int pitch, int P, int dil,
+                     float eps, ctn_stream_t stream);
+/* x (B, Bc, pitch) += rstd2 r[:, :Bc] + (v1 - mean2 rstd2 v2), r (B, Bc + Sc, pitch), (mean2, rstd2) from stats2 over n2 elements */
+int ctn_probe_finish(const float* r, const float* v1, const float* v2, const double* stats2, double n2, float eps, float* x, int B,
+                     int Bc, int Sc, int frames, int pitch, ctn_stream_t stream);
+/* One block's share of the skip sum: rows [off, off + Sc) of r (B, Mt, pitch), folded constants v1 / v2 (indexed like r's rows) */
+typedef struct ctn_skip_probe {
+  const float* r;
+  const float* v1;
+  const float* v2;
+  const double* stats2;
+  int32_t off, Mt;
+} ctn_skip_probe_t;
+/* skip (B, Sc, pitch) = sum_i rstd2_i r_i[:, off_i:off_i + Sc] + (v1_i - mean2_i rstd2_i v2_i)[off_i:], 1 <= n <= 64 jobs */
+int ctn_probe_skip_reduce(const ctn_skip_probe_t* jobs, int n, double n2, float eps, float* skip, int B, int Sc, int frames, int pitch,
+                          ctn_stream_t stream);
+/* stats[b] += (sum, sumsq) over c < C, t < frames, in double */
+int ctn_probe_stats_pitch(const float* x, int B, int C, int frames, int pitch, double* stats, ctn_stream_t stream);
+/* u = PReLU(sum_k wd[c][k] h[c][t + k dil - pad_left] + bd[c]; slope), h = 0 outside [0, frames) */
+int ctn_probe_dw_plain(const float* h, float* u, const float* wd, const float* bd, const float* slope, int B, int C, int frames,
+                       int pitch, int P, int dil, int pad_left, ctn_stream_t stream);
+/* rows of r (B, Mt, pitch): m < Bc (has_out): xout = xin + r + bo[m] (xin == xout: in place); else skip (+)= r + bs[m - Bc]
+ * (skip_init: =) */
+int ctn_probe_res_skip(const float* r, int Mt, const float* xin, float* xout, float* skip, const float* bo, const float* bs, int Bc,
+                       int Sc, int has_out, int skip_init, int B, int frames, int pitch, ctn_stream_t stream);
+/* y[b][c][t] += bias[c] */
+int ctn_probe_bias_rows(float* y, const float* bias, int C, int B, int frames, int pitch, ctn_stream_t stream);
+/* cLN over the first frames columns (in place allowed); scratch double[B][frames][2] */
+int ctn_probe_cln_pitch(const float* x, const float* gamma, const float* beta, float* y, int B, int C, int frames, int pitch, float eps,
+                        double* scratch, ctn_stream_t stream);
 
 #ifdef __cplusplus
 }
