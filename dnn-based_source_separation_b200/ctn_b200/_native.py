@@ -145,6 +145,15 @@ ctn_online_init = _sig("ctn_online_init", _i, C.POINTER(Config), C.POINTER(Param
 ctn_online_reset = _sig("ctn_online_reset", _i, C.POINTER(Config), _fp, _i, _fp)
 ctn_online_push = _sig("ctn_online_push", _i, C.POINTER(Config), C.POINTER(Params), _fp, _fp, _i, _i, _i, _fp, _fp)
 ctn_online_flush = _sig("ctn_online_flush", _i, C.POINTER(Config), _fp, _i, _fp, _fp)
+# recordings of any length: chunk plan, gather, permutation alignment, overlap-add, and the call around ctn_convtasnet_fwd
+ctn_chunk_plan = _sig("ctn_chunk_plan", _i, _i, _i, _i, C.POINTER(_i), _i)
+ctn_chunk_gather = _sig("ctn_chunk_gather", _i, _fp, _i, _i, _i, _i, _i, _i, _fp, _fp)
+ctn_chunk_align_scratch_bytes = _sig("ctn_chunk_align_scratch_bytes", _sz, _i, _i, _i, _i, _i)
+ctn_chunk_align = _sig("ctn_chunk_align", _i, _fp, _i, _i, _i, _i, _i, _fp, _fp, _sz, _fp)
+ctn_chunk_overlap_add = _sig("ctn_chunk_overlap_add", _i, _fp, _fp, _i, _i, _i, _i, _i, _fp, _fp)
+ctn_separate_long_workspace_bytes = _sig("ctn_separate_long_workspace_bytes", _i, C.POINTER(Config), _i, _i, _i, _i, _i, C.POINTER(_sz))
+ctn_convtasnet_separate_long = _sig("ctn_convtasnet_separate_long", _i, C.POINTER(Config), C.POINTER(Params), _fp, _i, _i, _i, _i, _i, _i,
+                                    _fp, _fp, _fp, _sz, _fp)
 ctn_profile_enable = _sig("ctn_profile_enable", _i, _i)
 ctn_profile_read = _sig("ctn_profile_read", _i, C.POINTER(C.c_double), C.POINTER(_i))
 STAGES = ("prep", "enc", "head", "pw1", "dw", "pw2", "fin", "mask", "dec", "loss")
@@ -161,6 +170,8 @@ EXPORTED = [
     "ctn_bilstm_supported", "ctn_bilstm_workspace_bytes", "ctn_bilstm_proj_fwd", "ctn_dprnn_norm_res2_fwd",
     "ctn_orpit_scratch_bytes", "ctn_orpit_fwd", "ctn_orpit_bwd", "ctn_sinkpit_scratch_bytes", "ctn_sinkpit_fwd", "ctn_sinkpit_bwd",
     "ctn_online_state_bytes", "ctn_online_init", "ctn_online_reset", "ctn_online_push", "ctn_online_flush",
+    "ctn_chunk_plan", "ctn_chunk_gather", "ctn_chunk_align_scratch_bytes", "ctn_chunk_align", "ctn_chunk_overlap_add",
+    "ctn_separate_long_workspace_bytes", "ctn_convtasnet_separate_long",
 ]
 
 

@@ -132,6 +132,7 @@ class ConvTasNet(nn.Module):
         self.decoder = decoder
         self.math = None  # numeric mode override: 'fp32' | 'tf32x3' | 'tf32'
         self.last_launches = 0
+        self.last_chunk_perms = None  # separate_long: the chunk permutations of the last call
 
     # ---- reference API ---------------------------------------------------------------------------
     def forward(self, input):
@@ -251,6 +252,43 @@ class ConvTasNet(nn.Module):
         ``max_chunk`` samples (a multiple of the stride): see ``ctn_b200.models.online.OnlineSeparator``."""
         from .online import OnlineSeparator
         return OnlineSeparator(self, batch_size, max_chunk)
+
+    def separate_long(self, mixture, chunk, hop=None, chunk_batch=16, align=True):
+        """Separate recordings of any length: mixture (batch, 1, T) -> (batch, n_sources, T), inference only, one C call
+        (ctn_convtasnet_separate_long) without a host synchronisation.  The signal is cut into chunks of ``chunk`` samples every
+        ``hop`` (default chunk // 2; chunk // 2 <= hop <= chunk), the last one moved left to end at T; the chunks run through
+        the forward ``chunk_batch`` at a time; with ``align`` (and n_sources > 1; needs hop < chunk, n_sources <= 6) each
+        chunk's sources are put in the order of the chunk before it by the inner products over the samples they share; the
+        chunks are cross-faded with sin^2 ramps.  T <= chunk gives ``self(mixture)``.  The permutations used are kept in
+        ``last_chunk_perms`` (batch, n_chunks, n_sources) int32: row [b, k, s] of chunk k carries output source s."""
+        if mixture.dim() != 3 or mixture.size(1) != 1:
+            if mixture.dim() == 4:
+                raise NotImplementedError("separate_long takes (batch, 1, T): multichannel input is not built")
+            raise ValueError("mixture.size() is expected (?, 1, ?), but given {}".format(tuple(mixture.size())))
+        if torch.is_grad_enabled() and any(p.requires_grad for p in self.parameters()):
+            raise NotImplementedError("separate_long is inference-only: call it under torch.no_grad()")
+        x = mixture.contiguous()
+        dev = N.require_cuda(x)
+        B, _, T = x.shape
+        chunk, chunk_batch = int(chunk), int(chunk_batch)
+        hop = chunk // 2 if hop is None else int(hop)
+        K = N.ctn_chunk_plan(T, chunk, hop, None, 0)
+        if K < 0:
+            N.check(K, "ctn_chunk_plan(T={}, chunk={}, hop={})".format(T, chunk, hop))
+        cfg = self.native_config()
+        params, keep = self.native_params(dev)
+        need = C.c_size_t(0)
+        N.check(N.ctn_separate_long_workspace_bytes(C.byref(cfg), B, T, chunk, hop, chunk_batch, C.byref(need)),
+                "ctn_separate_long_workspace_bytes")
+        base, nbytes = N.aligned(N.workspace(dev, need.value, tag="separate_long"))
+        out = torch.empty(B, self.n_sources, T, dtype=torch.float32, device=dev)
+        perms = torch.empty(B, K, self.n_sources, dtype=torch.int32, device=dev)
+        N.check(N.ctn_convtasnet_separate_long(C.byref(cfg), C.byref(params), x.data_ptr(), B, T, chunk, hop, chunk_batch, int(bool(align)),
+                                               out.data_ptr(), perms.data_ptr(), base, nbytes, N.stream_ptr(dev)),
+                "ctn_convtasnet_separate_long")
+        self.last_launches = N.ctn_last_launch_count()
+        self.last_chunk_perms = perms
+        return out
 
     @property
     def num_parameters(self):

@@ -186,6 +186,41 @@ int ctn_online_push(const ctn_config_t* cfg, const ctn_params_t* params, void* s
                     float* y, ctn_stream_t stream);
 int ctn_online_flush(const ctn_config_t* cfg, void* state, int B, float* y_tail, ctn_stream_t stream);
 
+/* ---- recordings of any length through a model that sees fixed-size chunks (no counterpart in the reference) -----------
+ * Plan: chunk/2 <= hop <= chunk (integer division), else CTN_EINVAL.  K = 1 chunk of T samples when T <= chunk; otherwise
+ * K = ceil((T - chunk) / hop) + 1 chunks of `chunk` samples, chunk k starting at k*hop and the last one at T - chunk, so it
+ * ends at T and no chunk sees padding the signal does not contain.  Chunk index g = b*K + k throughout.
+ * ctn_chunk_plan (host only): returns K (or < 0); starts (nullable) receives the K chunk starts, capacity >= K.
+ * ctn_chunk_gather: x (B,1,T) -> xc (n,1,Lc), Lc = min(chunk, T): chunks first .. first + n - 1; n <= 65535.
+ * ctn_chunk_align: est (B*K,S,Lc) chunk estimates -> perms (B,K,S) int32: row perms[b][k][s] of chunk k carries source s.
+ *   For each neighbouring pair, over the samples both chunks cover, c[i][j] = <e_k[i], e_{k+1}[j]> in double; the local
+ *   permutation maximises sum_i c[i][pi(i)] (itertools.permutations order, first maximum on ties, as in ctn_sisdr_pit_fwd);
+ *   perms[b][0] = identity, perms[b][k+1][s] = pi_k(perms[b][k][s]).  Two launches (scores of every pair; one scan per
+ *   recording), no atomics.  S <= 6 (else CTN_EUNSUPPORTED); S > 1 needs hop < chunk (CTN_EINVAL) and, when K > 1, scratch
+ *   of ctn_chunk_align_scratch_bytes() bytes, 8-byte aligned; B*(K-1) <= 65535.
+ * ctn_chunk_overlap_add: out (B,S,T), out[b][s][t] = sum_k w_k(t) est[b*K+k][perms[b][k][s]][t - start_k] / sum_k w_k(t) over the
+ *   chunks covering t, k ascending, accumulated in double (gather form: deterministic).  w_k = rise * fall, rise =
+ *   sin^2(pi/2 (r + 1/2)/a) over the first a samples of the chunk (a = samples shared with chunk k-1), fall = cos^2(pi/2 (q + 1/2)/n)
+ *   over its last n (shared with chunk k+1), 1 elsewhere.  perms nullable (identity).  Any S. */
+int ctn_chunk_plan(int T, int chunk, int hop, int* starts, int capacity);
+int ctn_chunk_gather(const float* x, int B, int T, int chunk, int hop, int first, int n, float* xc, ctn_stream_t stream);
+size_t ctn_chunk_align_scratch_bytes(int B, int S, int T, int chunk, int hop);
+int ctn_chunk_align(const float* est, int B, int S, int T, int chunk, int hop, int32_t* perms, void* scratch, size_t scratch_bytes,
+                    ctn_stream_t stream);
+int ctn_chunk_overlap_add(const float* est, const int32_t* perms, int B, int S, int T, int chunk, int hop, float* out,
+                          ctn_stream_t stream);
+/* The whole call: x (B,1,T) -> out (B,S,T).  The B*K chunks are gathered into batches of at most chunk_batch and run through
+ * ctn_convtasnet_fwd (a smaller last batch runs at its own size), then aligned (align != 0 and S > 1; needs hop < chunk and
+ * S <= 6) and overlap-added.  T <= chunk: ctn_convtasnet_fwd on x itself, in batches of chunk_batch recordings.  perms_out
+ * (nullable) (B,K,S) int32 receives the permutations used.  Every launch goes to `stream`, nothing is read back to the host.
+ * Envelope: whatever ctn_convtasnet_fwd accepts with in_channels <= 1.  Workspace (256-byte aligned), for T > chunk:
+ * the forward's workspace for min(chunk_batch, B*K) chunks + one gathered batch + 4*B*K*S*chunk bytes of chunk estimates
+ * + B*K*S*4 (permutations) + the alignment scratch: only the last three grow with T. */
+int ctn_separate_long_workspace_bytes(const ctn_config_t* cfg, int B, int T, int chunk, int hop, int chunk_batch, size_t* bytes);
+int ctn_convtasnet_separate_long(const ctn_config_t* cfg, const ctn_params_t* params, const float* x, int B, int T, int chunk, int hop,
+                                 int chunk_batch, int align, float* out, int32_t* perms_out, void* workspace, size_t workspace_bytes,
+                                 ctn_stream_t stream);
+
 /* Separator.forward, src/models/conv_tasnet.py:359-378: w (B,N,frames) -> mask (B,S,N,frames), both contiguous. */
 int ctn_separator_fwd(const ctn_config_t* cfg, const ctn_params_t* params, const float* w, int B, int frames,
                       float* mask, void* workspace, size_t workspace_bytes, ctn_stream_t stream);
