@@ -503,11 +503,12 @@ extern "C" int ctn_online_push(const ctn_config_t* cfg, const ctn_params_t* para
 
 extern "C" int ctn_online_flush(const ctn_config_t* cfg, void* state, int B, float* y_tail, ctn_stream_t stream) {
   CTN_TRY(check_cfg(cfg));
-  if (!state || !y_tail || B <= 0) return CTN_EINVAL;
+  const int L = cfg->kernel_size, S = cfg->stride, D = L - S, N = cfg->n_basis, R = L / S;
+  // a zero-delay model (kernel_size == stride) has no tail: y_tail holds 0 samples and may be null
+  if (!state || (D > 0 && !y_tail) || B <= 0) return CTN_EINVAL;
   if (((uintptr_t)state) & 255) return CTN_EALIGN;
   LaunchScope scope(state);
   cudaStream_t st = (cudaStream_t)stream;
-  const int L = cfg->kernel_size, S = cfg->stride, D = L - S, N = cfg->n_basis, R = L / S;
   Carver cv(state);
   OnlineState s;
   carve(cv, cfg, B, CTN_TILE_T, &s);

@@ -177,7 +177,8 @@ int ctn_convtasnet_fwd(const ctn_config_t* cfg, const ctn_params_t* params, cons
  * ctn_online_push: x (B,1,n) -> y (B,S,n), contiguous; n % stride == 0, 0 < n <= max_chunk_frames * stride.  A push
  * computes the frames its samples complete; its launch sequence depends on cfg alone.
  * ctn_online_flush: y_tail (B,S,D) = the last D samples of the offline output.  CTN_EINVAL when fewer than kernel_size
- * samples were pushed since the reset; reads that count from the device (synchronises the stream once). */
+ * samples were pushed since the reset; reads that count from the device (synchronises the stream once).  y_tail must be
+ * non-null when D > 0; a zero-delay model (kernel_size == stride) writes nothing, so y_tail may then be null. */
 int ctn_online_state_bytes(const ctn_config_t* cfg, int B, int max_chunk_frames, size_t* bytes);
 int ctn_online_init(const ctn_config_t* cfg, const ctn_params_t* params, int B, int max_chunk_frames, void* state, size_t state_bytes,
                     ctn_stream_t stream);
