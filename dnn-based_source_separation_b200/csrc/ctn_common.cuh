@@ -95,6 +95,18 @@ __device__ __forceinline__ float2 gln_mean_rstd(const double* __restrict__ st, d
   return make_float2((float)mean, (float)(1.0 / sqrt(var + (double)eps)));
 }
 
+// (mean, 1 / (std + eps)) of cLN frame t from the inclusive prefix sums st = (S_t, Q_t) over n = C (t + 1) elements; eps
+// OUTSIDE the sqrt (src/modules/norm.py:90).  The reference can go NaN where rounding makes the variance negative
+// (SURVEY.md 8a-6); we clamp.
+__device__ __forceinline__ float2 cln_mean_inv(const double* __restrict__ st, double n, float eps) {
+  const double mean = st[0] / n;
+  double var = st[1] / n - mean * mean;
+  var = var > 0.0 ? var : 0.0;
+  return make_float2((float)mean, 1.f / ((float)sqrt(var) + eps));
+}
+// one element of cLN, as the inference forward (k_cln_apply) and the training forward evaluate it
+__device__ __forceinline__ float cln_affine(float x, float2 mi, float g, float b) { return (x - mi.x) * mi.y * g + b; }
+
 __device__ __forceinline__ float prelu_f(float v, float a) { return v >= 0.f ? v : a * v; }
 
 // 128-bit row access of the (B, C, pitch) layout (rows 16-byte aligned)

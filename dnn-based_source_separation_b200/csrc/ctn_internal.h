@@ -28,6 +28,7 @@ struct Carver {
 };
 
 #define CTN_MAX_BLOCKS 64
+#define CTN_MAX_P 8  // most depthwise taps the training path takes
 
 // Config checks shared by every pipeline (ctn_api.cu): CTN_EINVAL for a value no pipeline accepts, CTN_EUNSUPPORTED for one
 // outside the stack's envelope.  check_tcn_cfg covers the separator stack's fields; max_layers is the longest run of layers
@@ -188,6 +189,28 @@ int ctn_copy_from_pitch(const float* src, float* dst, int rows, int frames, int 
 // cLN (src/modules/norm.py:78-90) on the padded (B, C, pitch) layout, in place allowed; scratch double[B][frames][2]
 int ctn_cln_pitch_fwd(const float* x, const float* gamma, const float* beta, float* y, int B, int C, int frames, int pitch,
                       float eps, double* scratch, cudaStream_t st);
+
+// cLN in pieces, for the causal training path: the prefix sums (S_t, Q_t) of act(x) (act = PReLU(slope), identity when slope is
+// null) into st double[B][frames][2] [2 launches], with mi (nullable, float2[B][frames]) the table of (mean_t, 1 / (std_t + eps));
+// and the normalisation y = cLN(act(x)) from st [1 launch].  ctn_cln_pitch_fwd is the two in a row without a slope.
+int ctn_cln_stats(const float* x, const float* slope, int B, int C, int frames, int pitch, float eps, double* st, float2* mi,
+                  cudaStream_t stream);
+int ctn_cln_apply(const float* x, const float* slope, const float* gamma, const float* beta, float* y, int B, int C, int frames,
+                  int pitch, float eps, const double* st, cudaStream_t stream);
+// cLN (+ PReLU(slope) in front, slope nullable) backward from the forward's st: dy -> dpre (may alias dy); += dgamma, dbeta, dslope,
+// dbias (the last two nullable).  Scratch: part double[ctn_cln_bwd_part_doubles(B, frames)], tab float4[B][frames].  3 launches.
+size_t ctn_cln_bwd_part_doubles(int B, int frames);
+int ctn_cln_bwd_pitch(const float* dy, const float* pre, float* dpre, const float* slope, const float* gamma, const double* st,
+                      float eps, double* part, float4* tab, float* dgamma, float* dbeta, float* dslope, float* dbias, int B, int C,
+                      int frames, int pitch, cudaStream_t stream);
+// Depthwise conv of the causal training path (ctn_causal_train.cu), pad_left = (P - 1) dil; mi: the cLN1 table of ctn_cln_stats.
+// upre = dwconv(cLN1(PReLU(hpre; slope1))) + bd
+int ctn_cdw_train_fwd(const float* hpre, float* upre, const float2* mi, const float* g1, const float* b1, const float* wd,
+                      const float* bd, const float* slope1, int B, int C, int frames, int pitch, int P, int dil, cudaStream_t st);
+// dhn = dwconv^T(dupre) ; dwd += the taps' gradients, hn = cLN1(PReLU(hpre)) rebuilt on load.  P <= CTN_MAX_P
+int ctn_cdw_bwd(const float* dupre, const float* hpre, float* dhn, const float2* mi, const float* g1, const float* b1,
+                const float* slope1, const float* wd, float* dwd, int B, int C, int frames, int pitch, int P, int dil,
+                cudaStream_t st);
 
 // Causal (cLN) models: un-fused pipeline in the reference's operation order (ctn_causal.cu).  The cumulative statistics of
 // cLN depend on every earlier frame, so the gLN tricks of the fused stack (statistics from the producing epilogue, affine

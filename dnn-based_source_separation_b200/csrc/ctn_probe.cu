@@ -204,3 +204,32 @@ extern "C" int ctn_probe_cln_pitch(const float* x, const float* gamma, const flo
                                    float eps, double* scratch, ctn_stream_t stream) {
   return ctn_cln_pitch_fwd(x, gamma, beta, y, B, C, frames, pitch, eps, scratch, (cudaStream_t)stream);
 }
+
+extern "C" int ctn_probe_cln_stats(const float* x, const float* slope, int B, int C, int frames, int pitch, float eps, double* st,
+                                   float* mi, ctn_stream_t stream) {
+  return ctn_cln_stats(x, slope, B, C, frames, pitch, eps, st, reinterpret_cast<float2*>(mi), (cudaStream_t)stream);
+}
+
+extern "C" int ctn_probe_cln_bwd(const float* dy, const float* pre, float* dpre, const float* slope, const float* gamma, const double* st,
+                                 float eps, void* scratch, float* dgamma, float* dbeta, float* dslope, float* dbias, int B, int C,
+                                 int frames, int pitch, ctn_stream_t stream) {
+  if (!scratch || (((uintptr_t)scratch) & 15)) return CTN_EALIGN;
+  double* part = static_cast<double*>(scratch);
+  float4* tab = reinterpret_cast<float4*>(part + ctn_cln_bwd_part_doubles(B, frames));
+  return ctn_cln_bwd_pitch(dy, pre, dpre, slope, gamma, st, eps, part, tab, dgamma, dbeta, dslope, dbias, B, C, frames, pitch,
+                           (cudaStream_t)stream);
+}
+
+extern "C" int ctn_probe_cdw_train_fwd(const float* hpre, float* upre, const float* mi, const float* g1, const float* b1, const float* wd,
+                                       const float* bd, const float* slope1, int B, int C, int frames, int pitch, int P, int dil,
+                                       ctn_stream_t stream) {
+  return ctn_cdw_train_fwd(hpre, upre, reinterpret_cast<const float2*>(mi), g1, b1, wd, bd, slope1, B, C, frames, pitch, P, dil,
+                           (cudaStream_t)stream);
+}
+
+extern "C" int ctn_probe_cdw_bwd(const float* dupre, const float* hpre, float* dhn, const float* mi, const float* g1, const float* b1,
+                                 const float* slope1, const float* wd, float* dwd, int B, int C, int frames, int pitch, int P, int dil,
+                                 ctn_stream_t stream) {
+  return ctn_cdw_bwd(dupre, hpre, dhn, reinterpret_cast<const float2*>(mi), g1, b1, slope1, wd, dwd, B, C, frames, pitch, P, dil,
+                     (cudaStream_t)stream);
+}

@@ -73,7 +73,6 @@ __global__ void __launch_bounds__(256) k_bias_prelu_stats(float* __restrict__ y,
 
 // u_pre[c][t] = sum_k wd[c][k] * hn[c][t + k*d - pl] + bd[c],  hn = gLN1(PReLU(h_pre)) inside [0,frames), 0 outside
 // (tdcn.py:120-130,181); stats2[b] += (sum, sumsq) of PReLU(u_pre; a2)
-#define CTN_MAX_P 8
 __global__ void __launch_bounds__(256) k_dw_train_fwd(const float* __restrict__ hpre, float* __restrict__ upre,
                                                       const float* __restrict__ g1, const float* __restrict__ b1,
                                                       const float* __restrict__ wd, const float* __restrict__ bd,
@@ -854,6 +853,35 @@ int gemm_raw(const ctn_config_t* c, TrainWs& ws, const float* W, int M, int K, c
   return ctn_pw(a, PRO_NONE, EPI_RAW, c->math, ws.wimg, st);
 }
 
+// Backward from d_out to the gradient of every block's skip output: decoder, sigmoid mask, mask conv, PReLU on the skip sum.
+// Leaves dS, rows [Bc, Bc + Sc) of dcat (= dS) and nC = d_wprod.  The same for gLN and cLN models.
+int bwd_tail(const ctn_config_t* c, const ctn_params_t* p, const ctn_params_t* grads, TrainWs& ws, const float* d_out, int B, int T,
+             cudaStream_t st) {
+  int pl = 0, pr = 0;
+  const int frames = ctn_frames(T, c->kernel_size, c->stride, &pl, &pr);
+  const int pitch = ctn_pitch(frames);
+  ctn_stream_t stream = (ctn_stream_t)st;
+  const int N = c->n_basis, Bc = c->bottleneck, Sc = c->skip, S = c->n_sources, L = c->kernel_size;
+  const size_t bsBc = (size_t)Bc * pitch, bsSc = (size_t)Sc * pitch, bsCat = (size_t)(Bc + Sc) * pitch, bsSN = (size_t)S * N * pitch;
+  auto G = [](const float* q) { return const_cast<float*>(q); };
+  // ---- decoder (filterbank.py:243-249): d_what = conv1d(d_out; Wd) (the transposed conv's adjoint), dWd
+  CTN_TRY(ctn_encoder_fwd(d_out, p->dec_w, ws.dwhat, B * S, T, pl, pr, N, L, c->stride, 0, pitch, nullptr, stream));
+  CTN_TRY(ctn_encdec_wgrad(ws.what, d_out, G(grads->dec_w), B * S, N, frames, pitch, T, L, c->stride, pl, st));
+  // ---- w_hat = w * sigmoid(m_pre): d_mpre (in place), d_wprod
+  CTN_TRY(ctn_mask_bwd(ws.dwhat, ws.w, ws.mask, ws.nC, B, S, N, frames, pitch, st));
+  // ---- mask conv (conv_tasnet.py:341,374): dWm, dbm, d_sp = Wm^T d_mpre
+  CTN_TRY(ctn_prelu_apply(ws.skip, ws.sp, p->prelu_out, B, Sc, frames, pitch, st));
+  CTN_TRY(ctn_wgrad(c->math, ws.dwhat, bsSN, ws.sp, bsSc, G(grads->mask_w), nullptr, 0, S * N, Sc, B, frames, pitch, st));
+  CTN_TRY(ctn_rowsum(ws.dwhat, bsSN, S * N, B, frames, pitch, G(grads->mask_b), st));
+  CTN_TRY(ctn_transpose(p->mask_w, ws.Wt, S * N, Sc, st));
+  CTN_TRY(gemm_raw(c, ws, ws.Wt, Sc, S * N, ws.dwhat, ws.dsp, B, frames, pitch, st));
+  // ---- PReLU on the skip sum (conv_tasnet.py:340,373): dS (the gradient of EVERY block's skip output)
+  CTN_TRY(ctn_prelu_bwd(ws.dsp, ws.skip, ws.dS, p->prelu_out, G(grads->prelu_out), B, Sc, frames, pitch, st));
+  // dcat rows [Bc, Bc+Sc) = dS for all blocks with an output head; rows [0,Bc) = gradient of the block's residual output
+  CTN_TRY(ctn_rows(ws.dcat + bsBc, bsCat, ws.dS, bsSc, Sc, B, 0, frames, pitch, st));
+  return CTN_OK;
+}
+
 }  // namespace
 
 void ctn_train_tcn_region(const ctn_config_t* c, int B, int pitch, void* mem, void** tcn_mem, const float** head_vb) {
@@ -978,28 +1006,14 @@ extern "C" int ctn_convtasnet_bwd(const ctn_config_t* c, const ctn_params_t* p, 
   Carver cv(train_ws);
   TrainWs ws;
   carve_train(cv, c, B, pitch, &ws);
-  const int N = c->n_basis, Bc = c->bottleneck, H = c->hidden, Sc = c->skip, S = c->n_sources, RX = c->num_blocks * c->num_layers,
-            X = c->num_layers, L = c->kernel_size;
+  const int N = c->n_basis, Bc = c->bottleneck, H = c->hidden, Sc = c->skip, RX = c->num_blocks * c->num_layers, X = c->num_layers,
+            L = c->kernel_size;
   const size_t bsN = (size_t)N * pitch, bsH = (size_t)H * pitch, bsBc = (size_t)Bc * pitch, bsSc = (size_t)Sc * pitch,
-               bsCat = (size_t)(Bc + Sc) * pitch, bsSN = (size_t)S * N * pitch;
+               bsCat = (size_t)(Bc + Sc) * pitch;
   const double nH = (double)H * (double)frames;
   auto G = [](const float* q) { return const_cast<float*>(q); };
 
-  // ---- decoder (filterbank.py:243-249): d_what = conv1d(d_out; Wd) (the transposed conv's adjoint), dWd
-  CTN_TRY(ctn_encoder_fwd(d_out, p->dec_w, ws.dwhat, B * S, T, pl, pr, N, L, c->stride, 0, pitch, nullptr, stream));
-  CTN_TRY(ctn_encdec_wgrad(ws.what, d_out, G(grads->dec_w), B * S, N, frames, pitch, T, L, c->stride, pl, st));
-  // ---- w_hat = w * sigmoid(m_pre): d_mpre (in place), d_wprod
-  CTN_TRY(ctn_mask_bwd(ws.dwhat, ws.w, ws.mask, ws.nC, B, S, N, frames, pitch, st));
-  // ---- mask conv (conv_tasnet.py:341,374): dWm, dbm, d_sp = Wm^T d_mpre
-  CTN_TRY(ctn_prelu_apply(ws.skip, ws.sp, p->prelu_out, B, Sc, frames, pitch, st));
-  CTN_TRY(ctn_wgrad(c->math, ws.dwhat, bsSN, ws.sp, bsSc, G(grads->mask_w), nullptr, 0, S * N, Sc, B, frames, pitch, st));
-  CTN_TRY(ctn_rowsum(ws.dwhat, bsSN, S * N, B, frames, pitch, G(grads->mask_b), st));
-  CTN_TRY(ctn_transpose(p->mask_w, ws.Wt, S * N, Sc, st));
-  CTN_TRY(gemm_raw(c, ws, ws.Wt, Sc, S * N, ws.dwhat, ws.dsp, B, frames, pitch, st));
-  // ---- PReLU on the skip sum (conv_tasnet.py:340,373): dS (the gradient of EVERY block's skip output)
-  CTN_TRY(ctn_prelu_bwd(ws.dsp, ws.skip, ws.dS, p->prelu_out, G(grads->prelu_out), B, Sc, frames, pitch, st));
-  // dcat rows [Bc, Bc+Sc) = dS for all blocks with an output head; rows [0,Bc) = gradient of the block's residual output
-  CTN_TRY(ctn_rows(ws.dcat + bsBc, bsCat, ws.dS, bsSc, Sc, B, 0, frames, pitch, st));
+  CTN_TRY(bwd_tail(c, p, grads, ws, d_out, B, T, st));
   // ---- residual blocks, last to first
   for (int i = RX - 1; i >= 0; --i) {
     const ctn_block_params_t& q = p->blocks[i];
@@ -1060,4 +1074,205 @@ extern "C" int ctn_convtasnet_bwd(const ctn_config_t* c, const ctn_params_t* p, 
   // ---- encoder (filterbank.py:212,222): dWe
   CTN_TRY(ctn_encdec_wgrad(ws.nB, x, G(grads->enc_w), B, N, frames, pitch, T, L, c->stride, pl, st));
   return CTN_OK;
+}
+
+// ================================================================================================================
+// Causal (cLN) models.  Block for block the un-fused branch above with cLN in place of gLN and all of the depthwise padding on
+// the left, in the operation order of the inference pipeline (ctn_causal.cu): the same estimate, so a model trained here
+// streams through the online pipeline unchanged.  cLN's statistics are per frame, so nothing of them fits a (B, 2) slot: the
+// forward keeps the scanned prefix sums (S_t, Q_t) of all 1 + 2 R X norms (16 bytes per frame and norm) and, for the norm in
+// front of each depthwise conv, the (mean_t, 1 / (std_t + eps)) table its kernels normalise with on load (8 bytes).
+// The contractions carry no operand scale: the f16x3 mode runs them on tf32 pieces.
+// Launches, g = 1 (fp32) or 2 (tensor-core modes: weight image + contraction) per 1x1 contraction, R X blocks:
+//   forward   6 + 2 g + R X (9 + g)
+//   backward  19 + 2 g + (R X - 1) (14 + 2 g + q) + (14 + 2 g),  q = 2 (fp32: the two-part FFMA weight gradient) or 1
+// ================================================================================================================
+namespace {
+
+struct CausalTrainWs {
+  double* st0;                  // cLN0:   [B][frames][2]
+  std::vector<double*> st1, st2;  // cLN1 / cLN2 of every block
+  std::vector<float2*> mi1;     // [B][frames] (mean, 1 / (std + eps)) of cLN1
+  double* part;                 // backward: partial frame sums
+  float4* tab;                  // backward: (m_t, r_t, U_t, V_t)
+};
+
+void carve_causal_train(Carver& cv, const ctn_config_t* c, int B, int frames, int pitch, TrainWs* ws, CausalTrainWs* cw) {
+  carve_train(cv, c, B, pitch, ws);
+  const int RX = c->num_blocks * c->num_layers;
+  const size_t bf = (size_t)B * frames;
+  cw->st0 = cv.take<double>(bf * 2);
+  cw->st1.assign(RX, nullptr);
+  cw->st2.assign(RX, nullptr);
+  cw->mi1.assign(RX, nullptr);
+  for (int i = 0; i < RX; ++i) {
+    cw->st1[i] = cv.take<double>(bf * 2);
+    cw->st2[i] = cv.take<double>(bf * 2);
+    cw->mi1[i] = cv.take<float2>(bf);
+  }
+  cw->part = cv.take<double>(ctn_cln_bwd_part_doubles(B, frames));
+  cw->tab = cv.take<float4>(bf);
+}
+
+int check_causal_train_cfg(const ctn_config_t* c) {
+  CTN_TRY(check_model_cfg(c));
+  if (!c->causal || c->mask_softmax || c->in_channels > 1 || c->sep_kernel > CTN_MAX_P) return CTN_EUNSUPPORTED;
+  return CTN_OK;
+}
+
+int check_causal_train_call(const ctn_config_t* c, int B, int T, const void* train_ws, size_t train_ws_bytes) {
+  if (((uintptr_t)train_ws) & 255) return CTN_EALIGN;
+  size_t need = 0;
+  CTN_TRY(ctn_causal_train_workspace_bytes(c, B, T, &need));
+  return train_ws_bytes < need ? CTN_EWORKSPACE : CTN_OK;
+}
+
+}  // namespace
+
+extern "C" int ctn_causal_train_workspace_bytes(const ctn_config_t* cfg, int batch, int T, size_t* bytes) {
+  CTN_TRY(check_causal_train_cfg(cfg));
+  if (batch <= 0 || !bytes) return CTN_EINVAL;
+  const int frames = ctn_frames(T, cfg->kernel_size, cfg->stride, nullptr, nullptr);
+  if (frames <= 0) return CTN_EINVAL;
+  Carver cv(nullptr);
+  TrainWs ws;
+  CausalTrainWs cw;
+  carve_causal_train(cv, cfg, batch, frames, ctn_pitch(frames), &ws, &cw);
+  *bytes = cv.off + 256;
+  return CTN_OK;
+}
+
+extern "C" int ctn_causal_fwd_train(const ctn_config_t* c, const ctn_params_t* p, const float* x, int B, int T, float* out,
+                                    void* train_ws, size_t train_ws_bytes, ctn_stream_t stream) {
+  LaunchScope scope(x);
+  CTN_TRY(check_causal_train_cfg(c));
+  if (!p || !p->blocks || !x || !out || !train_ws || B <= 0 || T <= 0) return CTN_EINVAL;
+  CTN_TRY(check_causal_train_call(c, B, T, train_ws, train_ws_bytes));
+  int pl = 0, pr = 0;
+  const int frames = ctn_frames(T, c->kernel_size, c->stride, &pl, &pr);
+  const int pitch = ctn_pitch(frames);
+  cudaStream_t st = (cudaStream_t)stream;
+  Carver cv(train_ws);
+  TrainWs ws;
+  CausalTrainWs cw;
+  carve_causal_train(cv, c, B, frames, pitch, &ws, &cw);
+  const int N = c->n_basis, Bc = c->bottleneck, H = c->hidden, Sc = c->skip, S = c->n_sources, RX = c->num_blocks * c->num_layers,
+            X = c->num_layers, P = c->sep_kernel;
+  CTN_TRY(ctn_encoder_fwd(x, p->enc_w, ws.w, B, T, pl, pr, N, c->kernel_size, c->stride, c->enc_relu, pitch, nullptr, stream));
+  // head: x_0 = Wb cLN0(w) + bb (conv_tasnet.py:333-335,370-371), as ctn_causal_head
+  CTN_TRY(ctn_cln_stats(ws.w, nullptr, B, N, frames, pitch, c->eps, cw.st0, nullptr, st));
+  CTN_TRY(ctn_cln_apply(ws.w, nullptr, p->norm0_g, p->norm0_b, ws.nA, B, N, frames, pitch, c->eps, cw.st0, st));
+  CTN_TRY(gemm_raw(c, ws, p->bn_w, Bc, N, ws.nA, ws.x[0], B, frames, pitch, st));
+  CTN_TRY(ctn_bias_rows_fwd(ws.x[0], p->bn_b, Bc, B, frames, pitch, st));
+  for (int i = 0; i < RX; ++i) {
+    const ctn_block_params_t& q = p->blocks[i];
+    const bool has_out = q.out_w != nullptr;
+    if (!has_out && i != RX - 1) return CTN_EINVAL;
+    const int dil = 1 << (i % X);
+    // h_pre = W1 x + b1
+    if (c->math == CTN_MATH_FP32) {
+      CTN_TRY(gemm_raw(c, ws, q.bottleneck_w, H, Bc, ws.x[i], ws.hpre[i], B, frames, pitch, st));
+      CTN_TRY(ctn_bias_rows_fwd(ws.hpre[i], q.bottleneck_b, H, B, frames, pitch, st));
+    } else {  // bias in the contraction's epilogue, the PRE-activation stored; its gLN statistics go to a sink nobody reads
+      PwArgs a;
+      memset(&a, 0, sizeof(a));
+      a.A = ws.x[i]; a.W = q.bottleneck_w; a.D = ws.hpre[i]; a.B = B; a.M = H; a.K = Bc; a.frames = frames; a.pitch = pitch;
+      a.bias = q.bottleneck_b; a.slope = q.prelu1; a.stats_out = ws.sums; a.store_pre = 1;
+      CTN_TRY(ctn_pw(a, PRO_NONE, EPI_H, c->math, ws.wimg, st));
+    }
+    // cLN1 statistics of PReLU(h_pre) ; u_pre = dwconv(cLN1(PReLU(h_pre))) + bd ; un = cLN2(PReLU(u_pre)) ; r = [Wo; Ws] un
+    CTN_TRY(ctn_cln_stats(ws.hpre[i], q.prelu1, B, H, frames, pitch, c->eps_tcn, cw.st1[i], cw.mi1[i], st));
+    CTN_TRY(ctn_cdw_train_fwd(ws.hpre[i], ws.upre[i], cw.mi1[i], q.norm1_g, q.norm1_b, q.dw_w, q.dw_b, q.prelu1, B, H, frames, pitch, P,
+                              dil, st));
+    CTN_TRY(ctn_cln_stats(ws.upre[i], q.prelu2, B, H, frames, pitch, c->eps_tcn, cw.st2[i], nullptr, st));
+    CTN_TRY(ctn_cln_apply(ws.upre[i], q.prelu2, q.norm2_g, q.norm2_b, ws.T1, B, H, frames, pitch, c->eps_tcn, cw.st2[i], st));
+    const int Mt = has_out ? Bc + Sc : Sc;
+    CTN_TRY(ctn_block_wcat(q, Bc, Sc, H, ws.Wcat, st));
+    CTN_TRY(gemm_raw(c, ws, ws.Wcat, Mt, H, ws.T1, ws.r, B, frames, pitch, st));
+    CTN_TRY(ctn_res_skip_fwd(ws.r, Mt, ws.x[i], has_out ? ws.x[i + 1] : nullptr, ws.skip, q.out_b, q.skip_b, Bc, Sc, has_out ? 1 : 0,
+                             i == 0 ? 1 : 0, B, frames, pitch, st));
+  }
+  // tail: PReLU -> mask 1x1 -> sigmoid -> * w (conv_tasnet.py:373-376, 158-160); keeps the mask
+  {
+    PwArgs a;
+    memset(&a, 0, sizeof(a));
+    a.A = ws.skip; a.W = p->mask_w; a.D = ws.what; a.B = B; a.M = S * N; a.K = Sc; a.frames = frames; a.pitch = pitch;
+    a.pro_slope = p->prelu_out; a.bias = p->mask_b; a.wenc = ws.w; a.Nb = N; a.mask_out = ws.mask;
+    CTN_TRY(ctn_pw(a, PRO_PRELU, EPI_MASK, c->math, ws.wimg, st));
+  }
+  return ctn_decoder_fwd(ws.what, p->dec_w, out, B * S, N, frames, pitch, c->kernel_size, c->stride, pl, T, stream);
+}
+
+// grads: same layout as params; every tensor must be ZERO on entry (the kernels accumulate with atomics)
+extern "C" int ctn_causal_bwd(const ctn_config_t* c, const ctn_params_t* p, const ctn_params_t* grads, const float* x, const float* d_out,
+                              int B, int T, void* train_ws, size_t train_ws_bytes, ctn_stream_t stream) {
+  LaunchScope scope(x);
+  CTN_TRY(check_causal_train_cfg(c));
+  if (!p || !p->blocks || !grads || !grads->blocks || !x || !d_out || !train_ws || B <= 0 || T <= 0) return CTN_EINVAL;
+  CTN_TRY(check_causal_train_call(c, B, T, train_ws, train_ws_bytes));
+  int pl = 0, pr = 0;
+  const int frames = ctn_frames(T, c->kernel_size, c->stride, &pl, &pr);
+  const int pitch = ctn_pitch(frames);
+  cudaStream_t st = (cudaStream_t)stream;
+  Carver cv(train_ws);
+  TrainWs ws;
+  CausalTrainWs cw;
+  carve_causal_train(cv, c, B, frames, pitch, &ws, &cw);
+  const int N = c->n_basis, Bc = c->bottleneck, H = c->hidden, Sc = c->skip, RX = c->num_blocks * c->num_layers, X = c->num_layers,
+            P = c->sep_kernel;
+  const size_t bsN = (size_t)N * pitch, bsH = (size_t)H * pitch, bsBc = (size_t)Bc * pitch, bsSc = (size_t)Sc * pitch,
+               bsCat = (size_t)(Bc + Sc) * pitch;
+  const float eps = c->eps_tcn;
+  auto G = [](const float* q) { return const_cast<float*>(q); };
+  CTN_TRY(bwd_tail(c, p, grads, ws, d_out, B, T, st));
+  // ---- residual blocks, last to first
+  for (int i = RX - 1; i >= 0; --i) {
+    const ctn_block_params_t& q = p->blocks[i];
+    const ctn_block_params_t& gq = grads->blocks[i];
+    const bool has_out = q.out_w != nullptr;
+    const int dil = 1 << (i % X);
+    const int Mt = has_out ? Bc + Sc : Sc;
+    const float* dY = has_out ? ws.dcat : ws.dS;  // (B, Mt, pitch)
+    const size_t dY_bs = has_out ? bsCat : bsSc;
+    // un = cLN2(PReLU(u_pre)) recomputed for the weight gradients of the two heads
+    CTN_TRY(ctn_cln_apply(ws.upre[i], q.prelu2, q.norm2_g, q.norm2_b, ws.T1, B, H, frames, pitch, eps, cw.st2[i], st));
+    if (has_out) {
+      CTN_TRY(ctn_wgrad(c->math, dY, dY_bs, ws.T1, bsH, G(gq.out_w), G(gq.skip_w), Bc, Bc + Sc, H, B, frames, pitch, st));
+      CTN_TRY(ctn_rowsum(dY, dY_bs, Bc, B, frames, pitch, G(gq.out_b), st));
+    } else {
+      CTN_TRY(ctn_wgrad(c->math, dY, dY_bs, ws.T1, bsH, G(gq.skip_w), nullptr, 0, Sc, H, B, frames, pitch, st));
+    }
+    CTN_TRY(ctn_rowsum(dY + (has_out ? bsBc : 0), dY_bs, Sc, B, frames, pitch, G(gq.skip_b), st));
+    // d_un = [Wo; Ws]^T dY
+    CTN_TRY(ctn_block_wcat(q, Bc, Sc, H, ws.Wcat, st));
+    CTN_TRY(ctn_transpose(ws.Wcat, ws.Wt, Mt, H, st));
+    CTN_TRY(gemm_raw(c, ws, ws.Wt, H, Mt, dY, ws.G1, B, frames, pitch, st));
+    // cLN2 + PReLU2 backward -> d_u_pre (G1 in place); dgamma2, dbeta2, da2, d(bd)
+    CTN_TRY(ctn_cln_bwd_pitch(ws.G1, ws.upre[i], ws.G1, q.prelu2, q.norm2_g, cw.st2[i], eps, cw.part, cw.tab, G(gq.norm2_g), G(gq.norm2_b),
+                              G(gq.prelu2), G(gq.dw_b), B, H, frames, pitch, st));
+    // causal depthwise conv backward -> d_hn (G2), d(wd)
+    CTN_TRY(ctn_cdw_bwd(ws.G1, ws.hpre[i], ws.G2, cw.mi1[i], q.norm1_g, q.norm1_b, q.prelu1, q.dw_w, G(gq.dw_w), B, H, frames, pitch, P,
+                        dil, st));
+    // cLN1 + PReLU1 backward -> d_h_pre (G2 in place); dgamma1, dbeta1, da1, db1
+    CTN_TRY(ctn_cln_bwd_pitch(ws.G2, ws.hpre[i], ws.G2, q.prelu1, q.norm1_g, cw.st1[i], eps, cw.part, cw.tab, G(gq.norm1_g), G(gq.norm1_b),
+                              G(gq.prelu1), G(gq.bottleneck_b), B, H, frames, pitch, st));
+    // bottleneck 1x1: dW1 = d_h_pre x_i^T ; d_x_i = W1^T d_h_pre (+ residual path)
+    CTN_TRY(ctn_wgrad(c->math, ws.G2, bsH, ws.x[i], bsBc, G(gq.bottleneck_w), nullptr, 0, H, Bc, B, frames, pitch, st));
+    CTN_TRY(ctn_transpose(q.bottleneck_w, ws.Wt, H, Bc, st));
+    CTN_TRY(gemm_raw(c, ws, ws.Wt, Bc, H, ws.G2, ws.dxtmp, B, frames, pitch, st));
+    CTN_TRY(ctn_rows(ws.dcat, bsCat, ws.dxtmp, bsBc, Bc, B, has_out ? 1 : 0, frames, pitch, st));
+  }
+  // ---- head: x_0 = Wb cLN0(w) + bb.   d_x0 = dcat rows [0,Bc)
+  CTN_TRY(ctn_cln_apply(ws.w, nullptr, p->norm0_g, p->norm0_b, ws.nA, B, N, frames, pitch, c->eps, cw.st0, st));
+  CTN_TRY(ctn_wgrad(c->math, ws.dcat, bsCat, ws.nA, bsN, G(grads->bn_w), nullptr, 0, Bc, N, B, frames, pitch, st));
+  CTN_TRY(ctn_rowsum(ws.dcat, bsCat, Bc, B, frames, pitch, G(grads->bn_b), st));
+  CTN_TRY(ctn_rows(ws.dxtmp, bsBc, ws.dcat, bsCat, Bc, B, 0, frames, pitch, st));
+  CTN_TRY(ctn_transpose(p->bn_w, ws.Wt, Bc, N, st));
+  CTN_TRY(gemm_raw(c, ws, ws.Wt, N, Bc, ws.dxtmp, ws.nB, B, frames, pitch, st));
+  // cLN0 backward -> d_w (norm path) ; + product path ; ReLU mask of the encoder if any
+  CTN_TRY(ctn_cln_bwd_pitch(ws.nB, ws.w, ws.nB, nullptr, p->norm0_g, cw.st0, c->eps, cw.part, cw.tab, G(grads->norm0_g), G(grads->norm0_b),
+                            nullptr, nullptr, B, N, frames, pitch, st));
+  CTN_TRY(ctn_dw_combine(ws.nB, ws.nC, ws.w, c->enc_relu, B, N, frames, pitch, st));
+  // ---- encoder (filterbank.py:212,222): dWe
+  return ctn_encdec_wgrad(ws.nB, x, G(grads->enc_w), B, N, frames, pitch, T, c->kernel_size, c->stride, pl, st);
 }

@@ -97,6 +97,7 @@ ctn_encoder_fwd = _sig("ctn_encoder_fwd", _i, _fp, _fp, _fp, _i, _i, _i, _i, _i,
 ctn_decoder_fwd = _sig("ctn_decoder_fwd", _i, _fp, _fp, _fp, _i, _i, _i, _i, _i, _i, _i, _i, _fp)
 ctn_gln_fwd = _sig("ctn_gln_fwd", _i, _fp, _fp, _fp, _fp, _i, _i, _i, _f, _fp, _fp)
 ctn_cln_fwd = _sig("ctn_cln_fwd", _i, _fp, _fp, _fp, _fp, _i, _i, _i, _f, _fp, _fp)
+ctn_cln_bwd = _sig("ctn_cln_bwd", _i, _fp, _fp, _fp, _fp, _fp, _fp, _fp, _i, _i, _i, _f, _fp)
 ctn_tcn_workspace_bytes = _sig("ctn_tcn_workspace_bytes", _i, C.POINTER(Config), _i, _i, C.POINTER(_sz))
 ctn_tcn_fwd = _sig("ctn_tcn_fwd", _i, C.POINTER(Config), C.POINTER(BlockParams), _fp, _fp, _i, _i, _fp, _sz, _fp)
 ctn_tcn_blocks_fwd = _sig("ctn_tcn_blocks_fwd", _i, C.POINTER(Config), C.POINTER(BlockParams), _i, C.POINTER(_i), _fp, _fp, _fp, _i, _i, _fp, _sz, _fp)
@@ -112,6 +113,9 @@ ctn_train_workspace_bytes = _sig("ctn_train_workspace_bytes", _i, C.POINTER(Conf
 ctn_convtasnet_fwd_train = _sig("ctn_convtasnet_fwd_train", _i, C.POINTER(Config), C.POINTER(Params), _fp, _i, _i, _fp, _fp, _sz, _fp)
 ctn_convtasnet_bwd = _sig("ctn_convtasnet_bwd", _i, C.POINTER(Config), C.POINTER(Params), C.POINTER(Params), _fp, _fp, _i, _i,
                           _fp, _sz, _fp)
+ctn_causal_train_workspace_bytes = _sig("ctn_causal_train_workspace_bytes", _i, C.POINTER(Config), _i, _i, C.POINTER(_sz))
+ctn_causal_fwd_train = _sig("ctn_causal_fwd_train", _i, C.POINTER(Config), C.POINTER(Params), _fp, _i, _i, _fp, _fp, _sz, _fp)
+ctn_causal_bwd = _sig("ctn_causal_bwd", _i, C.POINTER(Config), C.POINTER(Params), C.POINTER(Params), _fp, _fp, _i, _i, _fp, _sz, _fp)
 ctn_encoder_mc_fwd = _sig("ctn_encoder_mc_fwd", _i, _fp, _fp, _fp, _i, _i, _i, _i, _i, _i, _i, _i, _i, _i, _fp, _fp)
 ctn_decoder_mc_fwd = _sig("ctn_decoder_mc_fwd", _i, _fp, _fp, _fp, _i, _i, _i, _i, _i, _i, _i, _i, _i, _fp)
 ctn_sdr_fwd = _sig("ctn_sdr_fwd", _i, _fp, _fp, _i, _i, _f, _fp, _fp, _fp)
@@ -172,6 +176,7 @@ EXPORTED = [
     "ctn_online_state_bytes", "ctn_online_init", "ctn_online_reset", "ctn_online_push", "ctn_online_flush",
     "ctn_chunk_plan", "ctn_chunk_gather", "ctn_chunk_align_scratch_bytes", "ctn_chunk_align", "ctn_chunk_overlap_add",
     "ctn_separate_long_workspace_bytes", "ctn_convtasnet_separate_long",
+    "ctn_cln_bwd", "ctn_causal_train_workspace_bytes", "ctn_causal_fwd_train", "ctn_causal_bwd",
 ]
 
 

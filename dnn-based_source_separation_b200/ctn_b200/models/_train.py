@@ -1,4 +1,5 @@
-"""Autograd glue of the training path (ctn_convtasnet_fwd_train / ctn_convtasnet_bwd, include/ctn_b200.h).
+"""Autograd glue of the training path (ctn_convtasnet_fwd_train / ctn_convtasnet_bwd, and ctn_causal_fwd_train / ctn_causal_bwd
+for causal models; include/ctn_b200.h).
 
 The reference trains with plain autograd over its nn.Module graph (egs/wsj0-mix/common/src/driver.py:146-150:
 ``estimated = model(mixture); loss, _ = pit_criterion(estimated, sources); loss.backward()``).  Here the whole
@@ -19,20 +20,29 @@ def param_list(model):
     return model.separator.param_slots(enc_w=model.encoder.conv1d.weight, dec_w=model.decoder.conv_transpose1d.weight)
 
 
-class ConvTasNetTrainFn(torch.autograd.Function):
+class _Entry:
+    """the three C entry points of a training node, by name in _native"""
+
+    def __init__(self, workspace_bytes, fwd, bwd):
+        self.WORKSPACE_BYTES, self.FWD, self.BWD = workspace_bytes, fwd, bwd
+
+
+class _Node:
+    """Body of the training nodes; cls: the _Entry the node runs."""
+
     @staticmethod
-    def forward(ctx, model, x, *tensors):
+    def forward(cls, ctx, model, x, *tensors):
         dev = N.require_cuda(x)
         B, _, T = x.shape
         slots = [s for s, _ in param_list(model)]
         cfg = model.native_config()
         params, keep = N.build_params(zip(slots, tensors), dev)
         need = C.c_size_t(0)
-        N.check(N.ctn_train_workspace_bytes(C.byref(cfg), B, T, C.byref(need)), "ctn_train_workspace_bytes")
+        N.check(getattr(N, cls.WORKSPACE_BYTES)(C.byref(cfg), B, T, C.byref(need)), cls.WORKSPACE_BYTES)
         ws = torch.empty(need.value + 256, dtype=torch.uint8, device=dev)  # owned by this node until backward
         out = torch.empty(B, model.n_sources, T, dtype=torch.float32, device=dev)
-        N.check(N.ctn_convtasnet_fwd_train(C.byref(cfg), C.byref(params), x.data_ptr(), B, T, out.data_ptr(), *N.aligned(ws),
-                                           N.stream_ptr(dev)), "ctn_convtasnet_fwd_train")
+        N.check(getattr(N, cls.FWD)(C.byref(cfg), C.byref(params), x.data_ptr(), B, T, out.data_ptr(), *N.aligned(ws),
+                                    N.stream_ptr(dev)), cls.FWD)
         model.last_launches = N.ctn_last_launch_count()
         # x and the parameters go through save_for_backward: an in-place update between forward and backward is detected by autograd
         # (version counters) instead of silently changing the weights the backward kernels see
@@ -42,9 +52,9 @@ class ConvTasNetTrainFn(torch.autograd.Function):
         return out
 
     @staticmethod
-    def backward(ctx, d_out):
+    def backward(cls, ctx, d_out):
         if ctx.ws is None:
-            raise RuntimeError("ConvTasNetTrainFn: backward was already run on this graph; the saved activations are released after the "
+            raise RuntimeError("training node: backward was already run on this graph; the saved activations are released after the "
                                "first backward (retain_graph is not supported by the native training path)")
         saved = list(ctx.saved_tensors)
         x, it = saved[0], iter(saved[1:])
@@ -63,16 +73,41 @@ class ConvTasNetTrainFn(torch.autograd.Function):
         flat = torch.zeros(total, dtype=torch.float32, device=dev)
         gviews = [None if t is None else flat[o:o + t.numel()].view(t.shape) for t, o in zip(tensors, offs)]
         grads, keep2 = N.build_params(zip(ctx.slots, gviews), dev)
-        N.check(N.ctn_convtasnet_bwd(C.byref(cfg), C.byref(params), C.byref(grads), x.data_ptr(), d_out.data_ptr(), B, T,
-                                     *N.aligned(ws), N.stream_ptr(dev)), "ctn_convtasnet_bwd")
+        N.check(getattr(N, cls.BWD)(C.byref(cfg), C.byref(params), C.byref(grads), x.data_ptr(), d_out.data_ptr(), B, T,
+                                    *N.aligned(ws), N.stream_ptr(dev)), cls.BWD)
         ctx.model.last_bwd_launches = N.ctn_last_launch_count()
         ctx.model.last_flat_grad = flat
         ctx.ws = None
         return (None, None) + tuple(g if (t is not None and t.requires_grad) else None for g, t in zip(gviews, tensors))
 
 
+class ConvTasNetTrainFn(torch.autograd.Function):
+    ENTRY = _Entry("ctn_train_workspace_bytes", "ctn_convtasnet_fwd_train", "ctn_convtasnet_bwd")
+
+    @staticmethod
+    def forward(ctx, model, x, *tensors):
+        return _Node.forward(ConvTasNetTrainFn.ENTRY, ctx, model, x, *tensors)
+
+    @staticmethod
+    def backward(ctx, d_out):
+        return _Node.backward(ConvTasNetTrainFn.ENTRY, ctx, d_out)
+
+
+class CausalTrainFn(torch.autograd.Function):
+    """The same node over the causal (cLN) pipeline."""
+    ENTRY = _Entry("ctn_causal_train_workspace_bytes", "ctn_causal_fwd_train", "ctn_causal_bwd")
+
+    @staticmethod
+    def forward(ctx, model, x, *tensors):
+        return _Node.forward(CausalTrainFn.ENTRY, ctx, model, x, *tensors)
+
+    @staticmethod
+    def backward(ctx, d_out):
+        return _Node.backward(CausalTrainFn.ENTRY, ctx, d_out)
+
+
 def run_train(model, x):
     if x.requires_grad:
         raise NotImplementedError("gradient w.r.t. the mixture is not built (the native backward stops at the encoder weights)")
     tensors = [t for _, t in param_list(model)]
-    return ConvTasNetTrainFn.apply(model, x, *tensors)
+    return (CausalTrainFn if model.causal else ConvTasNetTrainFn).apply(model, x, *tensors)

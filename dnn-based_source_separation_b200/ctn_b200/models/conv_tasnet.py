@@ -10,7 +10,8 @@ the crop fused.  Internally activations are (batch, channels, pitch) fp32 with p
 
 Kernel envelope (anything else raises NotImplementedError, there is no eager fallback): enc_basis = dec_basis =
 'trainable', in_channels = 1, 3-D input, dilated, separable, sep_nonlinear='prelu', sep_norm, mask_nonlinear='sigmoid'.
-causal=False (gLN) runs the fused stack; causal=True (cLN) an un-fused pipeline (forward only, csrc/ctn_causal.cu).
+causal=False (gLN) runs the fused stack; causal=True (cLN) an un-fused pipeline (csrc/ctn_causal.cu), which trains natively
+once ``model.causal_training = True`` is set.
 """
 import ctypes as C
 
@@ -131,6 +132,8 @@ class ConvTasNet(nn.Module):
                                    eps=eps)
         self.decoder = decoder
         self.math = None  # numeric mode override: 'fp32' | 'tf32x3' | 'tf32'
+        # causal (cLN) models train through the native causal pipeline only when this is set; off, they refuse autograd as before
+        self.causal_training = False
         self.last_launches = 0
         self.last_chunk_perms = None  # separate_long: the chunk permutations of the last call
 
@@ -360,6 +363,9 @@ class ConvTasNet(nn.Module):
         training = torch.is_grad_enabled() and any(p.requires_grad for p in self.parameters())
         if training and self.in_channels > 1:
             raise NotImplementedError("multichannel models (in_channels > 1) are forward only: call under torch.no_grad()")
+        if training and self.causal and not self.causal_training:
+            raise NotImplementedError("causal (cLN) models train natively only with model.causal_training = True (ctn_causal_fwd_train / "
+                                      "ctn_causal_bwd); without it they are forward only: call under torch.no_grad()")
         x = x.contiguous()
         dev = N.require_cuda(x)
         if training:

@@ -40,6 +40,38 @@ class GlobalLayerNorm(nn.Module):
         return "{}({}, eps={})".format(self.__class__.__name__, self.num_features, self.eps)
 
 
+class _CLNFn(torch.autograd.Function):
+    """cLN under autograd: ctn_cln_fwd / ctn_cln_bwd on the (B, C, T) view of the input"""
+
+    @staticmethod
+    def forward(ctx, x, gamma, beta, eps):
+        dev = N.require_cuda(x, gamma, beta)
+        B, Cc = x.shape[0], x.shape[1]
+        T = x.numel() // (B * Cc)
+        y = torch.empty_like(x)
+        scratch = torch.empty(2 * B * T, dtype=torch.float64, device=dev)
+        N.check(N.ctn_cln_fwd(x.data_ptr(), gamma.data_ptr(), beta.data_ptr(), y.data_ptr(), B, Cc, T, float(eps),
+                              scratch.data_ptr(), N.stream_ptr(dev)), "ctn_cln_fwd")
+        ctx.save_for_backward(x, gamma)
+        ctx.eps = float(eps)
+        return y
+
+    @staticmethod
+    def backward(ctx, dy):
+        x, gamma = ctx.saved_tensors
+        dev = x.device
+        B, Cc = x.shape[0], x.shape[1]
+        T = x.numel() // (B * Cc)
+        dy = dy.contiguous()
+        N.require_cuda(dy)
+        dx = torch.empty_like(x)
+        dg = torch.zeros(2, Cc, dtype=torch.float32, device=dev)  # dgamma, dbeta: accumulated by the kernel
+        scratch = torch.empty(20 * B * T, dtype=torch.float64, device=dev)
+        N.check(N.ctn_cln_bwd(dy.data_ptr(), x.data_ptr(), gamma.data_ptr(), scratch.data_ptr(), dx.data_ptr(), dg[0].data_ptr(),
+                              dg[1].data_ptr(), B, Cc, T, ctx.eps, N.stream_ptr(dev)), "ctn_cln_bwd")
+        return dx, dg[0].view(gamma.shape), dg[1].view(gamma.shape), None
+
+
 class CumulativeLayerNorm1d(nn.Module):
     def __init__(self, num_features, eps=EPS):
         super().__init__()
@@ -55,6 +87,8 @@ class CumulativeLayerNorm1d(nn.Module):
         x = input.contiguous()
         dev = N.require_cuda(x, self.gamma)
         B, Cc = x.shape[0], x.shape[1]
+        if torch.is_grad_enabled() and (x.requires_grad or self.gamma.requires_grad or self.beta.requires_grad):
+            return _CLNFn.apply(x, self.gamma.contiguous(), self.beta.contiguous(), self.eps)
         T = x.numel() // (B * Cc)
         y = torch.empty_like(x)
         scratch = torch.empty(2 * B * T, dtype=torch.float64, device=dev)

@@ -142,6 +142,11 @@ int ctn_gln_fwd(const float* x, const float* gamma, const float* beta, float* y,
 /* CumulativeLayerNorm1d.forward, src/modules/norm.py:78-90.  x,y (B,C,T) contiguous; scratch double[B][T][2]. */
 int ctn_cln_fwd(const float* x, const float* gamma, const float* beta, float* y, int B, int C, int T, float eps,
                 double* scratch, ctn_stream_t stream);
+/* Backward of ctn_cln_fwd: dy (B,C,T) -> dx (B,C,T) (dx may alias dy); dgamma, dbeta (C) are ACCUMULATED (zero them first).
+ * scratch: 160 * B * T bytes, 16-byte aligned (the forward's prefix sums are recomputed there).  Frames whose cumulative
+ * variance the forward clamped to 0 take the variance as a constant (the reference's autograd yields inf / NaN there). */
+int ctn_cln_bwd(const float* dy, const float* x, const float* gamma, void* scratch, float* dx, float* dgamma, float* dbeta,
+                int B, int C, int T, float eps, ctn_stream_t stream);
 
 /* TimeDilatedConvNet.forward == TemporalConvNet.forward, src/models/tdcn.py:29-41 (src/models/tcn.py:37-49).
  * x (B,bottleneck,frames) contiguous -> skip sum (B,skip,frames) contiguous.  Uses cfg fields bottleneck, hidden,
@@ -327,6 +332,15 @@ int ctn_convtasnet_fwd_train(const ctn_config_t* cfg, const ctn_params_t* params
                              void* train_ws, size_t train_ws_bytes, ctn_stream_t stream);
 int ctn_convtasnet_bwd(const ctn_config_t* cfg, const ctn_params_t* params, const ctn_grads_t* grads, const float* x,
                        const float* d_out, int B, int T, void* train_ws, size_t train_ws_bytes, ctn_stream_t stream);
+/* The same three calls for causal (cLN) models, with the same arguments and the same contract: the estimate of
+ * ctn_convtasnet_fwd on a causal config, and what the backward needs kept in train_ws (per block as above, with the cumulative
+ * prefix sums of every cLN in double in place of the gLN statistics).  Envelope: causal = 1, sigmoid mask, in_channels = 1,
+ * sep_kernel <= 8; anything else CTN_EUNSUPPORTED (non-causal configs train through the three calls above). */
+int ctn_causal_train_workspace_bytes(const ctn_config_t* cfg, int batch, int T, size_t* bytes);
+int ctn_causal_fwd_train(const ctn_config_t* cfg, const ctn_params_t* params, const float* x, int B, int T, float* out,
+                         void* train_ws, size_t train_ws_bytes, ctn_stream_t stream);
+int ctn_causal_bwd(const ctn_config_t* cfg, const ctn_params_t* params, const ctn_grads_t* grads, const float* x,
+                   const float* d_out, int B, int T, void* train_ws, size_t train_ws_bytes, ctn_stream_t stream);
 
 /* Backward of ctn_sisdr_pit_fwd through the selected permutation (src/criterion/pit.py:36-44; sdr.py:135-137):
  * d_est (B,S,T) = grad_loss_b[b] * coef * dSI-SDR(est_i, tgt_perm[i])/d est_i.  fwd_scratch = the scratch buffer the

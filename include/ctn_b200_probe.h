@@ -194,6 +194,26 @@ int ctn_probe_bias_rows(float* y, const float* bias, int C, int B, int frames, i
 int ctn_probe_cln_pitch(const float* x, const float* gamma, const float* beta, float* y, int B, int C, int frames, int pitch, float eps,
                         double* scratch, ctn_stream_t stream);
 
+/* The causal training path's streaming kernels (ctn_norm.cu, ctn_causal_train.cu), through the launchers ctn_causal_fwd_train /
+ * ctn_causal_bwd call.  mi: float[B][frames][2], the (mean_t, 1 / (std_t + eps)) table of a cLN. */
+/* st double[B][frames][2] = inclusive prefix sums over frames of (sum_c, sum_c of squares) of PReLU(x; slope) (slope nullable:
+ * of x); mi nullable */
+int ctn_probe_cln_stats(const float* x, const float* slope, int B, int C, int frames, int pitch, float eps, double* st, float* mi,
+                        ctn_stream_t stream);
+/* cLN (+ PReLU(slope) in front, slope nullable) backward from the forward's st: dpre (may alias dy); += dgamma, dbeta, dslope,
+ * dbias (the last two nullable).  scratch: 144 * B * frames bytes, 16-byte aligned. */
+int ctn_probe_cln_bwd(const float* dy, const float* pre, float* dpre, const float* slope, const float* gamma, const double* st,
+                      float eps, void* scratch, float* dgamma, float* dbeta, float* dslope, float* dbias, int B, int C, int frames,
+                      int pitch, ctn_stream_t stream);
+/* upre = dwconv(cLN1(PReLU(hpre; slope1)), wd (C, P), dilation dil, all (P - 1) dil of the padding on the left) + bd */
+int ctn_probe_cdw_train_fwd(const float* hpre, float* upre, const float* mi, const float* g1, const float* b1, const float* wd,
+                            const float* bd, const float* slope1, int B, int C, int frames, int pitch, int P, int dil,
+                            ctn_stream_t stream);
+/* dhn = dwconv^T(dupre) ; dwd += the taps' gradients against hn = cLN1(PReLU(hpre; slope1)) */
+int ctn_probe_cdw_bwd(const float* dupre, const float* hpre, float* dhn, const float* mi, const float* g1, const float* b1,
+                      const float* slope1, const float* wd, float* dwd, int B, int C, int frames, int pitch, int P, int dil,
+                      ctn_stream_t stream);
+
 #ifdef __cplusplus
 }
 #endif
