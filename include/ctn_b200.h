@@ -389,6 +389,19 @@ int ctn_clip_adam_step(const int32_t* chunk_table, int n_chunks, float* const* p
                        float* exp_avg_sq, double* sumsq_scratch, const float* lr, long long* step, float beta1, float beta2, float eps,
                        float weight_decay, float max_norm, float* norm_out, ctn_stream_t stream);
 
+/* BSS Eval, src/utils/bss.py:4-30 (mir_eval 0.7 bss_eval_sources, filter length 512) in fp64.  ref (B,S,T) references,
+ * est (B,K,S,T): K sets of S estimates scored against the same references (the tester's estimate and repeated mixture share the
+ * Gram matrix of the references and its factorisations).  Outputs (B,K,S), indexed by reference j: sdr, sir, sar of the estimate
+ * perm[j] assigned to reference j.  compute_permutation = 1: perm maximises the mean SIR over itertools.permutations order (first
+ * maximum); 0: perm is the identity.  status (B) int32: 0, or the CTN_BSS_* bits of the item (its outputs are then undefined).
+ * A Gram matrix that is not numerically positive definite is reported (CTN_BSS_NOT_PD), where mir_eval falls back to lstsq.
+ * All arithmetic in double, no atomics: the same inputs give the same bits.  S <= 4 and B*K*S <= 65535 (else CTN_EUNSUPPORTED).
+ * ws: ctn_bss_workspace_bytes(), 256-byte aligned; it depends on (B, K, S) only, not on T.  No host synchronisation inside. */
+enum ctn_bss_status { CTN_BSS_SILENT_REF = 1, CTN_BSS_SILENT_EST = 2, CTN_BSS_NOT_PD = 4 };
+int ctn_bss_workspace_bytes(int B, int K, int S, int T, size_t* bytes);
+int ctn_bss_eval_sources(const float* ref, const float* est, int B, int K, int S, int T, int compute_permutation, double* sdr,
+                         double* sir, double* sar, int32_t* perm, int32_t* status, void* ws, size_t ws_bytes, ctn_stream_t stream);
+
 /* number of kernel launches the last ctn_* call on this thread enqueued (for bench.py's gpu_launches) */
 int ctn_last_launch_count(void);
 /* kernels launched by this thread through the library since it was loaded (paths made of several entry calls: DPRNN) */
