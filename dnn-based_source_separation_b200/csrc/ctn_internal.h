@@ -107,7 +107,8 @@ int ctn_pw(const PwArgs& a, int pro, int epi, int math, float* wimg_scratch, cud
 size_t ctn_pw_wimg_bytes(int M, int K, int math);
 // weight image of a.W (a.M, a.K) for ctn_pw(a, .., math, nullptr, ..); nothing to do in the fp32 mode
 int ctn_pw_prepare(const PwArgs& a, int math, float* wimg, cudaStream_t st);
-// EPI_MASKDEC (PRO_PRELU) applies to this contraction: fp16-piece mode, n_basis a multiple of 128, decoder kernel 16 / stride 8 (caller)
+// EPI_MASKDEC (PRO_PRELU) applies to this contraction: fp16-piece mode, n_basis a multiple of 128, K <= 128 (the operand stays
+// resident in shared memory), decoder kernel 16 / stride 8 (caller)
 int ctn_pw_maskdec_supported(const PwArgs& a, int math);
 
 // wgmma weight gradient of a 1x1 conv (ctn_wgrad_wgmma.cu): dW (M,K) += sum_{b,t} dY[b][m][t] X[b][k][t]; rows

@@ -43,8 +43,8 @@ constexpr int F16_MAX_ROWS = 2048;  // fp16-piece mode: padded output channels o
 // frames x 2 n-tiles, warpgroup w n-tile 2p + w, and both consume the same activation slab, so h and its depthwise stage (or the
 // residual update) are formed once per frame tile instead of once per n-tile.  With an odd n-tile count (e.g. the last block's
 // [out; skip] contraction, M = 128) the last CTA's second warpgroup has no n-tile: it still forms its share of each slab, and skips
-// its MMAs and epilogue.  Every other kernel splits TIME: 128 frames x 1 n-tile, warpgroup w frames [64w, 64w + 64).  EPI_MASKDEC
-// sums decoder taps per frame over the n-tiles of a source, and tf32 pieces are K-major only (see the operand store).
+// its MMAs and epilogue.  Every other kernel splits TIME: 128 frames x 1 n-tile, warpgroup w frames [64w, 64w + 64): tf32 pieces
+// are K-major only (see the operand store).  The fused mask + decoder has a kernel of its own (k_maskdec).
 template <int PRO, int EPI, bool F16>
 __host__ __device__ constexpr bool chan_split() { return F16 && (PRO == PRO_DW || EPI == EPI_H); }
 template <int PRO, int EPI, bool F16>
@@ -56,7 +56,10 @@ struct TcArgs {
   const float* oscale;  // fp16-piece mode: [n_tiles*NT] per-output-channel scale 2^-e (stored behind the images)
   int n_tiles, k_slabs, t_tiles;
   int n_groups;    // CTAs per (sample, time tile)
-  int nt_per_cta;  // n-tiles a CTA walks back to back: 1, or all n-tiles of one source (EPI_MASKDEC)
+  // n-tiles a CTA walks back to back, always 1: a runtime loop count on purpose.  With the loop flattened the compiler lays the
+  // block contractions out differently: pw1 6.87-7.15 -> 7.20-7.44 ms and pw2 7.25-7.50 -> 7.65-7.89 ms per cfg2 step (H100,
+  // three runs each, alternated); with the loop kept their SASS is unchanged.
+  int nt_per_cta;
 };
 
 // A thread's global loads for one slab: CPT channels x 4 time steps, NQ float4 per channel (PRO_DW: the 3 depthwise taps; PRO_RES:
@@ -148,8 +151,6 @@ __global__ void __launch_bounds__(THREADS, F16 ? 2 : 1) k_pw_wgmma(const TcArgs 
   const int ngrp = (int)blockIdx.x % n_groups;
   const int tt = ((int)blockIdx.x / n_groups) % g.t_tiles;
   const int b = (int)blockIdx.x / (n_groups * g.t_tiles);
-  // EPI_MASKDEC: decoder partial sums of the tile, [frame][tap], accumulated over the n-tiles of the source
-  float* dacc = reinterpret_cast<float*>(smem + SMEM_HEADER + STAGES * STAGE_BYTES);
 
   if (threadIdx.x == 0) {
     for (int s = 0; s < STAGES; ++s) ptx::mbar_init(ptx::smem_u32(&wbar[s]), 1);
@@ -178,8 +179,6 @@ __global__ void __launch_bounds__(THREADS, F16 ? 2 : 1) k_pw_wgmma(const TcArgs 
     const int reach = d >= 4 ? d : 4;  // furthest sample touched on either side of the tile
     dw_interior = (tt * TMC - reach >= 0) && (tt * TMC + TMC - 1 + reach + 3 < a.frames) && (a.K % KS == 0) && (a.dw_pad_left == d);
   }
-  if (EPI == EPI_MASKDEC)
-    for (int i = threadIdx.x; i < TM * 16; i += THREADS) dacc[i] = 0.f;
 
   for (int ntl = 0; ntl < g.nt_per_cta; ++ntl) {
   // nt0: first n-tile of the CTA (the CTA holding n-tile 0 also stores the prologue's side outputs); nt: this warpgroup's n-tile
@@ -342,9 +341,6 @@ __global__ void __launch_bounds__(THREADS, F16 ? 2 : 1) k_pw_wgmma(const TcArgs 
   const float inv_act = 1.f / act_s;
   const int row0 = (CSPLIT ? 0 : wg * 64) + (warp & 3) * 16 + (lane >> 2);  // frame within the tile
   float ls = 0.f, lss = 0.f;
-  float dpart[2][16];  // EPI_MASKDEC: sum over this thread's columns of w_hat[n][t] * Dec[n][k], rows row0 and row0 + 8
-#pragma unroll
-  for (int k = 0; k < 32; ++k) dpart[k >> 4][k & 15] = 0.f;
 #pragma unroll
   for (int i = 0; i < 64; ++i) {
     const int row = row0 + 8 * ((i >> 1) & 1);
@@ -377,19 +373,6 @@ __global__ void __launch_bounds__(THREADS, F16 ? 2 : 1) k_pw_wgmma(const TcArgs 
         v = tvalid ? mk * __ldg(a.wenc + ((size_t)b * a.Nb + n % a.Nb) * a.pitch + t) : 0.f;
       }
       if (a.mask_out) a.mask_out[((size_t)b * a.M + n) * a.pitch + t] = tvalid ? mk : 0.f;
-    } else if (EPI == EPI_MASKDEC) {
-      // w_hat[n][t] = w[n][t] * sigmoid(logit), contracted on the spot with the decoder basis (ConvTranspose1d(N, 1, 16, stride 8),
-      // filterbank.py:245-247): frame t contributes w_hat[n][t] * Dec[n][k] to sample 8 t + k
-      const float logit = F16 ? fmaf(v, osc, __ldg(a.bias + n)) : v + __ldg(a.bias + n);
-      const float o = tvalid ? __fdividef(__ldg(a.wenc + ((size_t)b * a.Nb + n % a.Nb) * a.pitch + t), 1.f + __expf(-logit)) : 0.f;
-      const float4* dr = reinterpret_cast<const float4*>(a.dec_w + (size_t)(n % a.Nb) * 16);
-#pragma unroll
-      for (int q4 = 0; q4 < 4; ++q4) {
-        const float4 d4 = __ldg(dr + q4);
-        float* dp = dpart[(i >> 1) & 1] + 4 * q4;
-        dp[0] = fmaf(o, d4.x, dp[0]); dp[1] = fmaf(o, d4.y, dp[1]); dp[2] = fmaf(o, d4.z, dp[2]); dp[3] = fmaf(o, d4.w, dp[3]);
-      }
-      continue;
     }
     *q = tvalid ? v : 0.f;
   }
@@ -397,39 +380,212 @@ __global__ void __launch_bounds__(THREADS, F16 ? 2 : 1) k_pw_wgmma(const TcArgs 
     const double s = warp_sum_d((double)ls), ss = warp_sum_d((double)lss);
     if (lane == 0) { atomicAdd(&a.stats_out[2 * b], s); atomicAdd(&a.stats_out[2 * b + 1], ss); }
   }
-  if (EPI == EPI_MASKDEC) {
-    // the 4 lanes of a quad hold the same two frames: reduce over them, lane 0 of the quad adds the frame's 16 taps to the tile sums
-#pragma unroll
-    for (int k = 0; k < 32; ++k) {
-      float v = dpart[k >> 4][k & 15];
-      v += __shfl_xor_sync(0xffffffffu, v, 1);
-      v += __shfl_xor_sync(0xffffffffu, v, 2);
-      dpart[k >> 4][k & 15] = v;
+  }  // n-tiles of the CTA
+}
+
+// ---- fused mask + decoder ----------------------------------------------------------------------------------------
+// estimates[b][s][8 t + k - crop] = sum_t' sum_n w[b][n][t'] * sigmoid(logit[b][s N + n][t']) * Dec[n][k'] (ConvTranspose1d(N, 1, 16,
+// stride 8), filterbank.py:245-247), logit = Wm PReLU(skip) + bm: mask 1x1, sigmoid, w * mask and the decoder in one launch, w_hat
+// never reaches HBM.  fp16 pieces, time split (warpgroup w frames [64 w, 64 w + 64)).  One CTA per (sample, 128-frame tile) walks
+// every n-tile of every source:
+//   * the operand PReLU(skip) * act_s is formed once, and the hi / lo pieces of all its K <= MD_MAX_K channels stay resident in
+//     shared memory (MN-major SWIZZLE_128B, as in k_pw_wgmma, one 16 KB slab after the other);
+//   * weight slabs stream through a ring of MD_STAGES bulk-copy stages that runs on across n-tile and source boundaries: while an
+//     n-tile's epilogue runs, the next n-tile's slabs are already in flight;
+//   * each thread loads its 64 encoder values of an n-tile before issuing that n-tile's MMAs, so their HBM latency hides behind the
+//     tensor core instead of stalling the epilogue; the n-tile's decoder taps, scales and biases go into a shared-memory table,
+//     so the epilogue issues no global loads.  About 158 KB of shared memory: one CTA per SM.
+// The MMAs are not overlapped with the epilogue: at cfg2 (H100) the launch takes 0.59 ms, 0.56 ms of it with the MMAs removed.
+// The logits come from the same 3-piece wgmma sequence as k_pw_wgmma's (slab, then kk, then hi.hi, lo.hi, hi.lo), and w_hat and
+// the decoder sums from the same float operations in the same order: per source, n-tiles ascending; per n-tile each thread's
+// columns in fragment order, then the quad reduction (lane ^ 1, then lane ^ 2), then the add into the tile sums.
+constexpr int MD_MAX_K = 128;  // resident operand: 4 slabs x hi / lo x 128 frames x 64 B = 64 KB
+constexpr int MD_STAGES = 4;
+constexpr int MD_ROW = 20;     // floats per frame row of the tile sums: 16 taps + 4 of padding, see the quad reduction
+constexpr uint32_t MD_A_BYTES = TM * 64u, MD_W_BYTES = NT * 64u;  // one fp16 piece of an operand / weight slab
+constexpr int MD_TAB = NT * 16 + 2 * NT;  // floats of an n-tile's epilogue table: decoder taps [tap / 4][column] (float4), scale, bias
+constexpr size_t MD_SMEM = 1024 + SMEM_HEADER + (size_t)(MD_MAX_K / KS) * 2 * MD_A_BYTES + (size_t)MD_STAGES * 2 * MD_W_BYTES +
+                           (size_t)TM * MD_ROW * sizeof(float) + 2 * (size_t)MD_TAB * sizeof(float);
+
+__global__ void __launch_bounds__(THREADS, 1) k_maskdec(const TcArgs g) {
+  extern __shared__ uint8_t smem_raw[];
+  const uint32_t raw = ptx::smem_u32(smem_raw);
+  const uint32_t base = (raw + 1023u) & ~1023u;
+  uint8_t* smem = smem_raw + (base - raw);
+  uint64_t* wbar = reinterpret_cast<uint64_t*>(smem);
+  const uint32_t op0 = base + SMEM_HEADER;                                                 // resident operand
+  const uint32_t ring0 = op0 + (uint32_t)(MD_MAX_K / KS) * 2 * MD_A_BYTES;                 // weight ring
+  float* dacc = reinterpret_cast<float*>(smem + (ring0 - base) + MD_STAGES * 2 * MD_W_BYTES);  // [frame][MD_ROW] tile sums
+  float* tab0 = dacc + TM * MD_ROW;  // two epilogue tables, n-tile parity
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, wg = warp >> 2;
+  const PwArgs& a = g.a;
+  const int tt = (int)blockIdx.x % g.t_tiles, b = (int)blockIdx.x / g.t_tiles;
+  const int ntps = a.Nb / NT, n_tiles = g.n_tiles, k_slabs = g.k_slabs;
+  const int total = n_tiles * k_slabs;  // weight slabs of the launch, in image order (n-tile major)
+  const uint8_t* wimg = reinterpret_cast<const uint8_t*>(g.wimg);
+
+  for (int i = threadIdx.x; i < TM * MD_ROW; i += THREADS) dacc[i] = 0.f;
+  if (threadIdx.x == 0) {
+    for (int s = 0; s < MD_STAGES; ++s) ptx::mbar_init(ptx::smem_u32(&wbar[s]), 1);
+    ptx::fence_mbar_init();
+  }
+  __syncthreads();
+  // slab q goes to stage q % MD_STAGES; it may be issued once slab q - MD_STAGES has been consumed by both warpgroups
+  int issued = 0;
+  auto refill = [&](int consumed) {
+    for (; issued < total && issued < consumed + MD_STAGES; ++issued) {
+      const uint32_t fb = ptx::smem_u32(&wbar[issued % MD_STAGES]);
+      ptx::mbar_arrive_expect_tx(fb, 2 * MD_W_BYTES);
+      ptx::bulk_g2s(ring0 + (uint32_t)(issued % MD_STAGES) * 2 * MD_W_BYTES, wimg + (size_t)issued * 2 * MD_W_BYTES, 2 * MD_W_BYTES, fb);
     }
-    if ((lane & 3) == 0) {
+  };
+  if (threadIdx.x == 0) refill(0);
+
+  // ---- the operand, once: warp w forms channels [4 w, 4 w + 4) of every slab, lane l frames [4 l, 4 l + 4) of the tile
+  const float act_s = __ldg(a.act_scale), pslope = __ldg(a.pro_slope);
+  {
+    const int tbase = tt * TM + lane * 4;
+    float4 v[MD_MAX_K / KS][CPW];
 #pragma unroll
-      for (int k = 0; k < 32; ++k) dacc[(row0 + 8 * (k >> 4)) * 16 + (k & 15)] += dpart[k >> 4][k & 15];
+    for (int ks = 0; ks < MD_MAX_K / KS; ++ks)
+#pragma unroll
+      for (int j = 0; j < CPW; ++j) {
+        const int c = ks * KS + warp * CPW + j;
+        v[ks][j] = ks < k_slabs && c < a.K ? __ldg(reinterpret_cast<const float4*>(a.A + ((size_t)b * a.K + c) * a.pitch + tbase))
+                                           : make_float4(0.f, 0.f, 0.f, 0.f);
+      }
+    const uint32_t f = (uint32_t)lane * 4u;
+#pragma unroll
+    for (int ks = 0; ks < MD_MAX_K / KS; ++ks) {
+      if (ks >= k_slabs) break;
+      uint8_t* sa = smem + (op0 - base) + (size_t)ks * 2 * MD_A_BYTES;
+#pragma unroll
+      for (int j = 0; j < CPW; ++j) {
+        float4 x = v[ks][j];
+        x.x = prelu_f(x.x, pslope); x.y = prelu_f(x.y, pslope); x.z = prelu_f(x.z, pslope); x.w = prelu_f(x.w, pslope);
+        const uint32_t c = (uint32_t)(warp * CPW + j);
+        const uint32_t off = (f >> 6) * 4096u + (c >> 3) * 1024u + (c & 7) * 128u + ((((f >> 3) & 7) ^ (c & 7)) << 4) + (f & 7) * 2u;
+        uint2 h2, l2;
+        ptx::split_f16x2(x.x * act_s, x.y * act_s, h2.x, l2.x);
+        ptx::split_f16x2(x.z * act_s, x.w * act_s, h2.y, l2.y);
+        *reinterpret_cast<uint2*>(sa + off) = h2;
+        *reinterpret_cast<uint2*>(sa + MD_A_BYTES + off) = l2;
+      }
     }
   }
-  }  // n-tiles of the CTA
+  ptx::fence_proxy_async_smem();
+  __syncthreads();
 
-  if (EPI == EPI_MASKDEC) {
-    // sample 8 f + k of the tile = taps k < 8 of frame f + taps 8 + k of frame f - 1, then the crop (conv_tasnet.py:169).  The first 8
-    // samples also receive the previous tile's last frame and the 8 samples after the tile belong to the next tile's first frame:
-    // those are added to the zero-initialised output with red.add, exactly two operands each, so the result is order-independent.
-    __syncthreads();
-    const int src = ngrp, S = a.M / a.Nb;
-    float* yo = a.D + ((size_t)b * S + src) * (size_t)a.dec_T_out;
-    const long long base = 8LL * tt * TM - a.dec_crop_left;
-    for (int sidx = threadIdx.x; sidx < 8 * TM + 8; sidx += THREADS) {
-      const int f = sidx >> 3, k = sidx & 7;
-      float v = 0.f;
-      if (f < TM) v += dacc[f * 16 + k];
-      if (f >= 1) v += dacc[(f - 1) * 16 + 8 + k];
-      const long long tau = base + sidx;
-      if (tau < 0 || tau >= a.dec_T_out) continue;
-      if (sidx < 8 || sidx >= 8 * TM) atomicAdd(yo + tau, v);
-      else yo[tau] = v;
+  const float inv_act = 1.f / act_s;
+  const int row0 = wg * 64 + (warp & 3) * 16 + (lane >> 2);  // frame within the tile (and row0 + 8)
+  const int t0 = tt * TM + row0;
+  const int S = a.M / a.Nb;
+  for (int nt = 0; nt < n_tiles; ++nt) {
+    const int src = nt / ntps, nb0 = (nt - src * ntps) * NT;  // source, first basis channel of the n-tile
+    // this thread's encoder values, in flight during the MMAs (pitch columns are always readable; those past frames are not used)
+    float wv[64];
+    {
+      const float* wr = a.wenc + ((size_t)b * a.Nb + nb0 + 2 * (lane & 3)) * a.pitch + t0;
+#pragma unroll
+      for (int i = 0; i < 64; ++i) wv[i] = __ldg(wr + (size_t)(8 * (i >> 2) + (i & 1)) * a.pitch + 8 * ((i >> 1) & 1));
+    }
+    // this thread's share of the n-tile's epilogue table (column threadIdx.x % 128: taps [8 h, 8 h + 8), h = threadIdx.x / 128,
+    // and the scale (h = 0) or the bias (h = 1)); loaded now, stored after the MMAs
+    const int tc = threadIdx.x & (NT - 1), th = threadIdx.x >> 7;
+    const float4* dsrc = reinterpret_cast<const float4*>(a.dec_w + (size_t)(nb0 + tc) * 16) + 2 * th;
+    const float4 td0 = __ldg(dsrc), td1 = __ldg(dsrc + 1);
+    const float tsb = th == 0 ? __ldg(g.oscale + nt * NT + tc) * inv_act : __ldg(a.bias + nt * NT + tc);
+    float acc[64];
+#pragma unroll
+    for (int i = 0; i < 64; ++i) acc[i] = 0.f;
+    for (int ks = 0; ks < k_slabs; ++ks) {
+      const int q = nt * k_slabs + ks;
+      const uint32_t w_hi = ring0 + (uint32_t)(q % MD_STAGES) * 2 * MD_W_BYTES, w_lo = w_hi + MD_W_BYTES;
+      const uint32_t a_hi = op0 + (uint32_t)ks * 2 * MD_A_BYTES + (uint32_t)wg * 4096u, a_lo = a_hi + MD_A_BYTES;
+      ptx::mbar_wait(ptx::smem_u32(&wbar[q % MD_STAGES]), (uint32_t)(q / MD_STAGES) & 1u);
+      ptx::wg_fence();
+#pragma unroll
+      for (int kk = 0; kk < KS / 16; ++kk) {
+        const uint64_t dah = ptx::wg_desc_mn128(a_hi + kk * 2048, 4096u, 1024u), dwh = ptx::wg_desc(w_hi + kk * 32, 8 * 64, ptx::SW64);
+        const uint64_t dal = ptx::wg_desc_mn128(a_lo + kk * 2048, 4096u, 1024u), dwl = ptx::wg_desc(w_lo + kk * 32, 8 * 64, ptx::SW64);
+        ptx::wg_mma_f16(acc, dah, dwh);
+        ptx::wg_mma_f16(acc, dal, dwh);
+        ptx::wg_mma_f16(acc, dah, dwl);
+      }
+      ptx::wg_commit();
+    }
+    ptx::wg_wait<0>();
+    // the table of parity nt & 1 was last read in the epilogue of n-tile nt - 2, which every thread left before the barrier of nt - 1
+    float* tab = tab0 + (nt & 1) * MD_TAB;
+    float4* tdec = reinterpret_cast<float4*>(tab);  // [q4][column]: a warp's 4 distinct columns 2 apart, on distinct banks
+    tdec[(2 * th) * NT + tc] = td0;
+    tdec[(2 * th + 1) * NT + tc] = td1;
+    tab[NT * 16 + th * NT + tc] = tsb;
+    __syncthreads();  // both warpgroups are done with this n-tile's slabs (and with the previous source's flush); the table is in
+    if (threadIdx.x == 0) refill((nt + 1) * k_slabs);
+
+    // w_hat[n][t] = w[n][t] * sigmoid(logit), contracted on the spot with the decoder taps: frame t adds w_hat[n][t] * Dec[n][k] to
+    // sample 8 t + k.  dpart: sum over this thread's columns, rows row0 and row0 + 8
+    float dpart[2][16];
+#pragma unroll
+    for (int k = 0; k < 32; ++k) dpart[k >> 4][k & 15] = 0.f;
+#pragma unroll
+    for (int i = 0; i < 64; ++i) {
+      const int c = 8 * (i >> 2) + 2 * (lane & 3) + (i & 1);
+      const bool tvalid = t0 + 8 * ((i >> 1) & 1) < a.frames;
+      const float osc = tab[NT * 16 + c];
+      const float logit = fmaf(acc[i], osc, tab[NT * 17 + c]);
+      const float o = tvalid ? __fdividef(wv[i], 1.f + __expf(-logit)) : 0.f;
+#pragma unroll
+      for (int q4 = 0; q4 < 4; ++q4) {
+        const float4 d4 = tdec[q4 * NT + c];
+        float* dp = dpart[(i >> 1) & 1] + 4 * q4;
+        dp[0] = fmaf(o, d4.x, dp[0]); dp[1] = fmaf(o, d4.y, dp[1]); dp[2] = fmaf(o, d4.z, dp[2]); dp[3] = fmaf(o, d4.w, dp[3]);
+      }
+    }
+    // quad reduction as reduce-scatter: lane bit 0 keeps row row0 + 8 (bit set) or row0, lane bit 1 taps 8..15 or 0..7.  Every
+    // kept sum is (v_q + v_q^1) + (v_q^2 + v_q^3), bit for bit the value a full butterfly leaves in every lane.  Row stride
+    // MD_ROW = 20 floats puts the 32 lanes' 16-byte chunks on distinct banks.
+    const bool hb0 = lane & 1, hb1 = lane & 2;
+    float r1[16];
+#pragma unroll
+    for (int j = 0; j < 16; ++j) {
+      const float keep = hb0 ? dpart[1][j] : dpart[0][j], send = hb0 ? dpart[0][j] : dpart[1][j];
+      r1[j] = keep + __shfl_xor_sync(0xffffffffu, send, 1);
+    }
+    float r2[8];
+#pragma unroll
+    for (int j = 0; j < 8; ++j) {
+      const float keep = hb1 ? r1[8 + j] : r1[j], send = hb1 ? r1[j] : r1[8 + j];
+      r2[j] = keep + __shfl_xor_sync(0xffffffffu, send, 2);
+    }
+    float4* dst = reinterpret_cast<float4*>(dacc + (row0 + (hb0 ? 8 : 0)) * MD_ROW + (hb1 ? 8 : 0));
+    float4 u0 = dst[0], u1 = dst[1];
+    u0.x += r2[0]; u0.y += r2[1]; u0.z += r2[2]; u0.w += r2[3];
+    u1.x += r2[4]; u1.y += r2[5]; u1.z += r2[6]; u1.w += r2[7];
+    dst[0] = u0; dst[1] = u1;
+
+    if (nt - src * ntps == ntps - 1) {
+      // the source is complete: sample 8 f + k of the tile = taps k < 8 of frame f + taps 8 + k of frame f - 1, then the crop
+      // (conv_tasnet.py:169).  The first 8 samples also receive the previous tile's last frame and the 8 samples after the tile
+      // belong to the next tile's first frame: those are added to the zero-initialised output with red.add, exactly two operands
+      // each, so the result is order-independent.  Each tile sum is read by one thread, which clears it for the next source.  A
+      // warp takes frames f, f + 2, f + 4, f + 6 (8 samples each): at the 20-float row stride their taps lie on distinct banks.
+      __syncthreads();
+      float* yo = a.D + ((size_t)b * S + src) * (size_t)a.dec_T_out;
+      const long long tb = 8LL * tt * TM - a.dec_crop_left;
+      for (int j = threadIdx.x; j < 2 * 32 * (TM / 8 + 1); j += THREADS) {
+        const int u = j >> 5, f = (u >> 1) * 8 + 2 * ((j & 31) >> 3) + (u & 1), k = j & 7;
+        if (f > TM) continue;
+        const int sidx = 8 * f + k;
+        float v = 0.f;
+        if (f < TM) { v += dacc[f * MD_ROW + k]; dacc[f * MD_ROW + k] = 0.f; }
+        if (f >= 1) { v += dacc[(f - 1) * MD_ROW + 8 + k]; dacc[(f - 1) * MD_ROW + 8 + k] = 0.f; }
+        const long long tau = tb + sidx;
+        if (tau < 0 || tau >= a.dec_T_out) continue;
+        if (sidx < 8 || sidx >= 8 * TM) atomicAdd(yo + tau, v);
+        else yo[tau] = v;
+      }
     }
   }
 }
@@ -543,8 +699,7 @@ int launch(const TcArgs& g0, cudaStream_t st) {
   constexpr int NPREC = NPASS == 3 ? 2 : 1;
   constexpr bool CSPLIT = chan_split<PRO, EPI, F16>();
   constexpr int TMC = tile_frames<PRO, EPI, F16>();
-  constexpr size_t smem = SMEM_HEADER + 1024 + (size_t)STAGES * NPREC * (TMC + (CSPLIT ? 2 : 1) * NT) * (F16 ? 64 : 128) +
-                          (EPI == EPI_MASKDEC ? TM * 16 * 4 : 0);
+  constexpr size_t smem = SMEM_HEADER + 1024 + (size_t)STAGES * NPREC * (TMC + (CSPLIT ? 2 : 1) * NT) * (F16 ? 64 : 128);
   TcArgs g = g0;
   g.t_tiles = g.a.pitch / TMC;
   g.n_groups = CSPLIT ? (g.n_tiles + 1) / 2 : g.n_tiles / g.nt_per_cta;
@@ -596,10 +751,30 @@ int build_images(const WimgJob* jobs, int n, int math, cudaStream_t st) {
   return CTN_OK;
 }
 
-// fused mask + decoder epilogue: fp16-piece mode, whole n-tiles per source, decoder basis (Nb, 1, 16) with kernel 16 / stride 8
+// fused mask + decoder (k_maskdec): fp16-piece mode, whole n-tiles per source, decoder basis (Nb, 1, 16) with kernel 16 /
+// stride 8, and an operand small enough to stay resident (K <= MD_MAX_K); otherwise the caller runs EPI_MASK and the decoder
 bool maskdec_ok(const PwArgs& a, int pmath) {
-  return eff_math(a.M, pmath) == CTN_MATH_F16X3 && a.dec_w && a.Nb > 0 && a.Nb % NT == 0 && a.M % a.Nb == 0 &&
+  return eff_math(a.M, pmath) == CTN_MATH_F16X3 && a.dec_w && a.Nb > 0 && a.Nb % NT == 0 && a.M % a.Nb == 0 && a.K <= MD_MAX_K &&
          (((uintptr_t)a.dec_w) & 15) == 0;
+}
+
+int launch_maskdec(const TcArgs& g0, cudaStream_t st) {
+  TcArgs g = g0;
+  g.t_tiles = g.a.pitch / TM;
+  g.n_groups = 1;
+  static bool attr_done[CTN_MAX_DEVICES] = {false};
+  const int dev = ctn_current_device();
+  if (!attr_done[dev]) {
+    cudaError_t e = cudaFuncSetAttribute(k_maskdec, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)MD_SMEM);
+    if (e != cudaSuccess) return (int)e;
+    attr_done[dev] = true;
+  }
+  const long long grid = (long long)g.a.B * g.t_tiles;
+  if (grid > 0x7fffffffLL) return CTN_EUNSUPPORTED;
+  k_maskdec<<<(unsigned)grid, THREADS, MD_SMEM, st>>>(g);
+  CTN_COUNT_LAUNCH();
+  CTN_RETURN_IF_CUDA_ERR();
+  return CTN_OK;
 }
 
 // a.wimg holds the image of a.W in the pieces `pmath`
@@ -627,8 +802,7 @@ int launch_wgmma(const PwArgs& a, int pro, int epi, int pmath, cudaStream_t st) 
   if (pro == PRO_PRELU && epi == EPI_MASK) return launch_math<PRO_PRELU, EPI_MASK>(g, math, st);
   if (pro == PRO_PRELU && epi == EPI_MASKDEC) {
     if (!maskdec_ok(a, pmath)) return CTN_EUNSUPPORTED;
-    g.nt_per_cta = a.Nb / NT;  // one CTA per (sample, time tile, source): the decoder sums over the source's channels
-    return launch<PRO_PRELU, EPI_MASKDEC, 3, true, false>(g, st);
+    return launch_maskdec(g, st);
   }
   return CTN_EUNSUPPORTED;
 }
