@@ -25,7 +25,6 @@
 #define BSS_MAX_S 4
 #define BSS_NCH 16     // time chunks of the correlation partial sums
 #define BSS_TU 1024    // samples per shared-memory tile of the correlation kernel
-#define BSS_NB 64      // Cholesky tile
 #define BSS_LD 65      // padded row of a shared tile (conflict-free column reads)
 #define BSS_NTT 64     // time ranges of the projection pass per estimate
 #define BSS_PT 256     // output samples per projection sub-tile (one per thread)
@@ -112,15 +111,8 @@ __global__ void __launch_bounds__(256) k_bss_build(const double* __restrict__ co
 }
 
 // ---- 2. batched Cholesky and solves -------------------------------------------------------------------------------------------
-// nmat row-major N x N matrices (N a multiple of 64); the factor L overwrites the lower triangle.  W: the inverse of every
-// diagonal tile of L, (nmat, N/64, 64, 64), zero above the diagonal.  flag[mat] = 1 when a pivot was not positive and finite.
-struct MatSet {
-  double* A;
-  double* W;
-  int* flag;
-  int N, nt, nmat;
-};
-
+// MatSet (ctn_internal.h): nmat row-major N x N matrices (N a multiple of 64), factor in the lower triangle, W the inverses of
+// its diagonal tiles, flag[mat] = 1 when a pivot was not positive and finite.
 #define BSS_TILE_SMEM (2 * BSS_NB * BSS_LD * sizeof(double))
 
 __device__ __forceinline__ void bss_load_tile(double (*s)[BSS_LD], const double* g, int ld) {
@@ -294,7 +286,11 @@ __global__ void __launch_bounds__(256) k_chol_solve(MatSet s, double* __restrict
   for (int e = tid; e < s.N; e += 256) v[e] = y[e];
 }
 
-static int launch_cholesky(const MatSet& s, cudaStream_t st) {
+int ctn_chol_factor(const MatSet& s, cudaStream_t st) {
+  for (auto k : {(const void*)k_chol_diag, (const void*)k_chol_panel, (const void*)k_chol_update}) {
+    cudaError_t e = cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)BSS_TILE_SMEM);
+    if (e != cudaSuccess) return (int)e;
+  }
   for (int kt = 0; kt < s.nt; ++kt) {
     k_chol_diag<<<s.nmat, 256, BSS_TILE_SMEM, st>>>(s, kt);
     CTN_COUNT_LAUNCH();
@@ -305,6 +301,13 @@ static int launch_cholesky(const MatSet& s, cudaStream_t st) {
     k_chol_update<<<dim3(n * (n + 1) / 2, s.nmat), 256, BSS_TILE_SMEM, st>>>(s, kt);
     CTN_COUNT_LAUNCH();
   }
+  CTN_RETURN_IF_CUDA_ERR();
+  return CTN_OK;
+}
+
+int ctn_chol_solve_cols(const MatSet& s, double* rhs, int nrhs, cudaStream_t st) {
+  k_chol_solve<<<dim3(nrhs, s.nmat), 256, sizeof(double) * s.N, st>>>(s, rhs, nrhs);
+  CTN_COUNT_LAUNCH();
   CTN_RETURN_IF_CUDA_ERR();
   return CTN_OK;
 }
@@ -543,19 +546,12 @@ extern "C" int ctn_bss_eval_sources(const float* ref, const float* est, int B, i
   CTN_COUNT_LAUNCH();
   CTN_RETURN_IF_CUDA_ERR();
 
-  for (auto k : {(const void*)k_chol_diag, (const void*)k_chol_panel, (const void*)k_chol_update}) {
-    cudaError_t e = cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)BSS_TILE_SMEM);
-    if (e != cudaSuccess) return (int)e;
-  }
   const MatSet g{w.G, w.Wg, w.flagG, d.N, d.N / BSS_NB, B};
   const MatSet blk{w.Bk, w.Wb, w.flagB, BSS_L, BSS_L / BSS_NB, B * S};
-  CTN_TRY(launch_cholesky(g, st));
-  CTN_TRY(launch_cholesky(blk, st));
-  k_chol_solve<<<dim3(d.KS, g.nmat), 256, sizeof(double) * g.N, st>>>(g, w.rhsG, d.KS);
-  CTN_COUNT_LAUNCH();
-  k_chol_solve<<<dim3(d.KS, blk.nmat), 256, sizeof(double) * blk.N, st>>>(blk, w.rhsB, d.KS);
-  CTN_COUNT_LAUNCH();
-  CTN_RETURN_IF_CUDA_ERR();
+  CTN_TRY(ctn_chol_factor(g, st));
+  CTN_TRY(ctn_chol_factor(blk, st));
+  CTN_TRY(ctn_chol_solve_cols(g, w.rhsG, d.KS, st));
+  CTN_TRY(ctn_chol_solve_cols(blk, w.rhsB, d.KS, st));
 
   switch (S) {
     case 1: CTN_TRY(launch_project<1>(ref, est, w.rhsG, w.rhsB, w.epart, d, st)); break;

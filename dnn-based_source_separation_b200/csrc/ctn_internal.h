@@ -282,3 +282,21 @@ int ctn_encdec_wgrad(const float* act, const float* sig, float* dW, int R, int N
                      int pad_left, cudaStream_t st);
 // out[c] += sum_{b, t < frames} dy[b][c][t]
 int ctn_rowsum(const float* dy, size_t bs, int C, int B, int frames, int pitch, float* out, cudaStream_t st);
+
+// Batched tiled Cholesky of BSS Eval (ctn_bss.cu).  nmat row-major N x N matrices (N a multiple of BSS_NB); the factor L
+// overwrites the lower triangle.  W: the inverse of every diagonal tile of L, (nmat, N/64, 64, 64), zero above the diagonal.
+// flag[mat] = 1 when a pivot was not positive and finite.
+#define BSS_NB 64
+struct MatSet {
+  double* A;
+  double* W;
+  int* flag;
+  int N, nt, nmat;
+};
+// factor every matrix of s: 3 nt - 2 launches
+int ctn_chol_factor(const MatSet& s, cudaStream_t st);
+// G x = b in place for nrhs right-hand sides per matrix, rhs (nmat, nrhs, N): one CTA per (matrix, right-hand side), 1 launch
+int ctn_chol_solve_cols(const MatSet& s, double* rhs, int nrhs, cudaStream_t st);
+// G X = B for nrhs <= 8 right-hand sides per matrix, rhs (nmat, N, nrhs) row-major: X overwrites rhs, tmp (same size) holds the
+// forward sweep's result.  Each sweep reads every factor tile once for all columns (ctn_bss_images.cu), 2 nt launches
+int ctn_chol_solve_multi(const MatSet& s, double* rhs, double* tmp, int nrhs, cudaStream_t st);

@@ -233,3 +233,19 @@ extern "C" int ctn_probe_cdw_bwd(const float* dupre, const float* hpre, float* d
   return ctn_cdw_bwd(dupre, hpre, dhn, reinterpret_cast<const float2*>(mi), g1, b1, slope1, wd, dwd, B, C, frames, pitch, P, dil,
                      (cudaStream_t)stream);
 }
+
+extern "C" int ctn_probe_chol_factor(double* A, double* W, int32_t* flag, int N, int nmat, ctn_stream_t stream) {
+  LaunchScope scope(A);
+  if (!A || !W || !flag || N < BSS_NB || N % BSS_NB || nmat < 1 || nmat > 65535) return CTN_EINVAL;
+  return ctn_chol_factor(MatSet{A, W, flag, N, N / BSS_NB, nmat}, (cudaStream_t)stream);
+}
+
+extern "C" int ctn_probe_chol_solve(const double* A, const double* W, double* rhs, double* tmp, int N, int nmat, int nrhs, int route,
+                                    ctn_stream_t stream) {
+  LaunchScope scope(A);
+  if (!A || !W || !rhs || N < BSS_NB || N % BSS_NB || nmat < 1 || nmat > 65535 || nrhs < 1 || nrhs > 8) return CTN_EINVAL;
+  const MatSet s{const_cast<double*>(A), const_cast<double*>(W), nullptr, N, N / BSS_NB, nmat};
+  if (route == 0) return ctn_chol_solve_cols(s, rhs, nrhs, (cudaStream_t)stream);
+  if (route == 1 && tmp) return ctn_chol_solve_multi(s, rhs, tmp, nrhs, (cudaStream_t)stream);
+  return CTN_EINVAL;
+}

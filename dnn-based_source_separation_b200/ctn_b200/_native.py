@@ -162,6 +162,9 @@ ctn_convtasnet_separate_long = _sig("ctn_convtasnet_separate_long", _i, C.POINTE
 ctn_bss_workspace_bytes = _sig("ctn_bss_workspace_bytes", _i, _i, _i, _i, _i, C.POINTER(_sz))
 ctn_bss_eval_sources = _sig("ctn_bss_eval_sources", _i, _fp, _fp, _i, _i, _i, _i, _i, _fp, _fp, _fp, _fp, _fp, _fp, _sz, _fp)
 BSS_SILENT_REF, BSS_SILENT_EST, BSS_NOT_PD = 1, 2, 4
+# BSS Eval v4 of multichannel source images (museval evaluate, mode='v4') in fp64
+ctn_bss_images_workspace_bytes = _sig("ctn_bss_images_workspace_bytes", _i, _i, _i, _i, _i, _i, C.POINTER(_sz))
+ctn_bss_eval_images = _sig("ctn_bss_eval_images", _i, _fp, _fp, _i, _i, _i, _i, _i, _fp, _fp, _fp, _fp, _fp, _fp, _sz, _fp)
 ctn_profile_enable = _sig("ctn_profile_enable", _i, _i)
 ctn_profile_read = _sig("ctn_profile_read", _i, C.POINTER(C.c_double), C.POINTER(_i))
 STAGES = ("prep", "enc", "head", "pw1", "dw", "pw2", "fin", "mask", "dec", "loss")
@@ -181,7 +184,7 @@ EXPORTED = [
     "ctn_chunk_plan", "ctn_chunk_gather", "ctn_chunk_align_scratch_bytes", "ctn_chunk_align", "ctn_chunk_overlap_add",
     "ctn_separate_long_workspace_bytes", "ctn_convtasnet_separate_long",
     "ctn_cln_bwd", "ctn_causal_train_workspace_bytes", "ctn_causal_fwd_train", "ctn_causal_bwd",
-    "ctn_bss_workspace_bytes", "ctn_bss_eval_sources",
+    "ctn_bss_workspace_bytes", "ctn_bss_eval_sources", "ctn_bss_images_workspace_bytes", "ctn_bss_eval_images",
 ]
 
 

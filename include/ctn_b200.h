@@ -402,6 +402,20 @@ int ctn_bss_workspace_bytes(int B, int K, int S, int T, size_t* bytes);
 int ctn_bss_eval_sources(const float* ref, const float* est, int B, int K, int S, int T, int compute_permutation, double* sdr,
                          double* sir, double* sar, int32_t* perm, int32_t* status, void* ws, size_t ws_bytes, ctn_stream_t stream);
 
+/* BSS Eval v4 of multichannel source images: museval 0.4 `evaluate(references, estimates, win, hop, mode='v4')` in fp64
+ * (distortion filters of 512 taps over all sources and channels, computed once over the whole track; SDR / ISR / SIR / SAR per
+ * window).  ref, est (J, I, T): J sources of I channels, time-contiguous, estimate j scored against reference j (no permutation).
+ * Outputs sdr, isr, sir, sar (J, nwin) with nwin = floor((T - win + hop) / hop); a window in which the channel sum of some source
+ * is zero throughout, in the references or in the estimates, is NaN for every source; a zero denominator gives +inf.
+ * status (1) int32: 0, or CTN_BSS_NOT_PD when a Cholesky pivot of G + eps I or of a diagonal block was not positive and finite
+ * (museval would fall back to lstsq; the outputs are then undefined), e.g. when J I 512 > T + 511.
+ * J I <= 8 (else CTN_EUNSUPPORTED); J, I, T, win, hop >= 1 and nwin >= 1 (else CTN_EINVAL).  All arithmetic in double, no
+ * atomics and no host synchronisation: the same inputs give the same bits, and a call can be captured in a CUDA graph.
+ * ws: ctn_bss_images_workspace_bytes(), 256-byte aligned; it depends on (J, I) and nwin, not otherwise on T. */
+int ctn_bss_images_workspace_bytes(int J, int I, int T, int win, int hop, size_t* bytes);
+int ctn_bss_eval_images(const float* ref, const float* est, int J, int I, int T, int win, int hop, double* sdr, double* isr,
+                        double* sir, double* sar, int32_t* status, void* ws, size_t ws_bytes, ctn_stream_t stream);
+
 /* number of kernel launches the last ctn_* call on this thread enqueued (for bench.py's gpu_launches) */
 int ctn_last_launch_count(void);
 /* kernels launched by this thread through the library since it was loaded (paths made of several entry calls: DPRNN) */

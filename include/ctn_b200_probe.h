@@ -213,6 +213,14 @@ int ctn_probe_cdw_train_fwd(const float* hpre, float* upre, const float* mi, con
 int ctn_probe_cdw_bwd(const float* dupre, const float* hpre, float* dhn, const float* mi, const float* g1, const float* b1,
                       const float* slope1, const float* wd, float* dwd, int B, int C, int frames, int pitch, int P, int dil,
                       ctn_stream_t stream);
+/* The batched tiled Cholesky of BSS Eval on nmat row-major N x N matrices (N a multiple of 64): the factor overwrites the lower
+ * triangle of A, W (nmat, N/64, 64, 64) receives the inverses of its diagonal tiles, flag (nmat) 1 where a pivot was not positive
+ * and finite.  Then G X = B for nrhs <= 8 right-hand sides with the factor: route 0 is the one-CTA-per-column solve of
+ * ctn_bss_eval_sources, rhs (nmat, nrhs, N); route 1 the all-columns solve of ctn_bss_eval_images, rhs (nmat, N, nrhs) with tmp
+ * of the same size.  X overwrites rhs. */
+int ctn_probe_chol_factor(double* A, double* W, int32_t* flag, int N, int nmat, ctn_stream_t stream);
+int ctn_probe_chol_solve(const double* A, const double* W, double* rhs, double* tmp, int N, int nmat, int nrhs, int route,
+                         ctn_stream_t stream);
 
 #ifdef __cplusplus
 }
