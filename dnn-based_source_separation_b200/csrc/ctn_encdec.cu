@@ -301,10 +301,190 @@ extern "C" int ctn_decoder_fwd(const float* w_hat, const float* dec_w, float* y,
 
 // ------------------------------------------------------------------------------------------------
 // Multichannel filter banks (in_channels = n_mics > 1: the 4-D input form of conv_tasnet.py:138-141, 167-168; MUSDB18 recipes).
-// Forward only, straightforward kernels (thread = frame / output sample): this is the widened input format, not the measured path.
 //   encoder: w[b][n][f] = sum_c sum_k W[n][c][k] * xpad[b][c][f*stride + k]      (Conv1d(C, N, L, stride), filterbank.py:212,222-229)
 //   decoder: y[bs][c][t] = sum_n sum_{f,k: f*stride + k = t + crop} what[bs][n][f] * Wd[n][c][k]  (ConvTranspose1d(N, C, L, stride))
+// The training path also runs the encoder as the decoder's adjoint: ConvTranspose1d(N, C)'s weight (N, C, L) has the index order
+// of Conv1d(C, N)'s, so d_what = conv1d(d_out; Wd) is this encoder over the (B*S, C, T) rows of d_out, without ReLU or statistics.
 // ------------------------------------------------------------------------------------------------
+// Fast encoder (kernel = 2 x stride, L <= 20): k_encoder_v4 over C input channels.  Block = 128 frames x all N bases, 4 warps each
+// owning a quarter of the bases; every channel's filter slice W[:, c, :] is staged transposed ([L][N4]) in shared memory next to
+// its input window, and the channel sum runs in registers (the 4 x 4 accumulators of a base group take every channel before they
+// are stored).  The window of a lane's 4 frames is staged once per lane (XWP floats, XWP / 4 odd) so that the per-channel reload
+// is LDS.128 without bank conflicts: the 8 lanes of a quarter-warp start XWP floats apart, on 8 distinct 4-bank groups.
+template <int L, int STRIDE>
+__global__ void __launch_bounds__(128) k_encoder_v4_mc(const float* __restrict__ x, const float* __restrict__ W, float* __restrict__ w, int C,
+                                                       int T, int pad_left, int N, int frames, int pitch, int relu, double* __restrict__ stats) {
+  constexpr int XW = 3 * STRIDE + L;        // input samples under 4 consecutive frames
+  constexpr int XW4 = (XW + 3) / 4 * 4;
+  constexpr int XWP = (XW4 / 4) % 2 ? XW4 : XW4 + 4;
+  extern __shared__ __align__(16) float sm[];
+  const int N4 = (N + 3) & ~3;
+  float* Wt = sm;                           // [C][L][N4]
+  float* xl = sm + (size_t)C * L * N4;      // [C][32 lanes][XWP]
+  __shared__ double red[64];
+  const int b = blockIdx.y, f0 = blockIdx.x * 128, tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+  for (int i = tid; i < C * L * N4; i += 128) {
+    const int c = i / (L * N4), r = i - c * L * N4, k = r / N4, n = r - k * N4;
+    Wt[i] = n < N ? W[((size_t)n * C + c) * L + k] : 0.f;
+  }
+  const float* xb = x + (size_t)b * C * T;
+  for (int i = tid; i < C * 32 * XW; i += 128) {
+    const int c = i / (32 * XW), r = i - c * 32 * XW, ln = r / XW, k = r - ln * XW;
+    const int t = (f0 + ln * 4) * STRIDE + k - pad_left;
+    xl[(c * 32 + ln) * XWP + k] = (t >= 0 && t < T) ? xb[(size_t)c * T + t] : 0.f;
+  }
+  __syncthreads();
+  const int f = f0 + lane * 4;
+  const bool v0 = f < frames, v1 = f + 1 < frames, v2 = f + 2 < frames, v3 = f + 3 < frames;
+  const int nq = ((N4 / 4 + 3) / 4) * 4;  // bases per warp, a multiple of 4
+  const int n_beg = warp * nq, n_end = min(N, n_beg + nq);
+  double s = 0.0, ss = 0.0;
+  float ls = 0.f, lss = 0.f;
+  int since = 0;
+  for (int n = n_beg; n < n_end; n += 4) {
+    float a[4][4];
+#pragma unroll
+    for (int cc = 0; cc < 4; ++cc)
+#pragma unroll
+      for (int q = 0; q < 4; ++q) a[cc][q] = 0.f;
+    for (int c = 0; c < C; ++c) {
+      float xw[XW4];
+      const float4* xp = reinterpret_cast<const float4*>(xl + (c * 32 + lane) * XWP);
+#pragma unroll
+      for (int k4 = 0; k4 < XW4 / 4; ++k4) {
+        const float4 q = xp[k4];
+        xw[4 * k4] = q.x; xw[4 * k4 + 1] = q.y; xw[4 * k4 + 2] = q.z; xw[4 * k4 + 3] = q.w;
+      }
+      const float* Wc = Wt + (size_t)c * L * N4;
+#pragma unroll
+      for (int k = 0; k < L; ++k) {
+        const float4 wv = *reinterpret_cast<const float4*>(&Wc[k * N4 + n]);
+        const float wc[4] = {wv.x, wv.y, wv.z, wv.w};
+#pragma unroll
+        for (int cc = 0; cc < 4; ++cc)
+#pragma unroll
+          for (int q = 0; q < 4; ++q) a[cc][q] = fmaf(wc[cc], xw[q * STRIDE + k], a[cc][q]);
+      }
+    }
+#pragma unroll
+    for (int cc = 0; cc < 4; ++cc) {
+      if (n + cc >= N) break;
+      float4 o = make_float4(a[cc][0], a[cc][1], a[cc][2], a[cc][3]);
+      if (relu) { o.x = fmaxf(o.x, 0.f); o.y = fmaxf(o.y, 0.f); o.z = fmaxf(o.z, 0.f); o.w = fmaxf(o.w, 0.f); }
+      if (!v0) o.x = 0.f;
+      if (!v1) o.y = 0.f;
+      if (!v2) o.z = 0.f;
+      if (!v3) o.w = 0.f;
+      *reinterpret_cast<float4*>(w + ((size_t)b * N + n + cc) * pitch + f) = o;
+      ls += (o.x + o.y) + (o.z + o.w);
+      lss = fmaf(o.x, o.x, fmaf(o.y, o.y, fmaf(o.z, o.z, fmaf(o.w, o.w, lss))));
+    }
+    if (++since == 4) { s += ls; ss += lss; ls = 0.f; lss = 0.f; since = 0; }  // spill fp32 partials (<= 64 values) to double
+  }
+  if (stats != nullptr) {
+    s += ls; ss += lss;
+    block_sum2_d(s, ss, red);
+    if (tid == 0) { atomicAdd(&stats[2 * b], s); atomicAdd(&stats[2 * b + 1], ss); }
+  }
+}
+
+constexpr int NO_FAST_PATH = 1 << 30;  // not a status: a launcher's answer that its kernel does not apply
+
+template <int L>
+static size_t encoder_v4_mc_smem(int C, int N) {
+  constexpr int XW4 = (3 * (L / 2) + L + 3) / 4 * 4;
+  constexpr int XWP = (XW4 / 4) % 2 ? XW4 : XW4 + 4;
+  return sizeof(float) * ((size_t)C * L * ((N + 3) & ~3) + (size_t)C * 32 * XWP);
+}
+
+// NO_FAST_PATH: outside the fast path (the caller launches k_encoder_mc)
+template <int L>
+static int launch_encoder_v4_mc(const float* x, const float* W, float* w, int B, int C, int T, int pad_left, int N, int frames, int pitch,
+                                int relu, double* stats, cudaStream_t st) {
+  const size_t smem = encoder_v4_mc_smem<L>(C, N);
+  if (smem > 200 * 1024) return NO_FAST_PATH;
+  if (smem > 48 * 1024) {
+    cudaError_t e = cudaFuncSetAttribute(k_encoder_v4_mc<L, L / 2>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+    if (e != cudaSuccess) return (int)e;
+  }
+  k_encoder_v4_mc<L, L / 2><<<dim3(pitch / 128, B), 128, smem, st>>>(x, W, w, C, T, pad_left, N, frames, pitch, relu, stats);
+  CTN_COUNT_LAUNCH();
+  CTN_RETURN_IF_CUDA_ERR();
+  return CTN_OK;
+}
+
+// Fast decoder: k_decoder over one output channel per CTA (Wd[:, c, :] in shared memory, the basis sum split over DEC_SPLIT thread
+// groups).  The channel is the fastest-varying block index, so the C CTAs of a 128-segment tile read the same w_hat rows close in
+// time and all but the first find them in L2: w_hat (B*S*N*frames floats, 0.58 GB at the MUSDB18 recipe) comes from HBM once.
+template <int STRIDE, int R>
+__global__ void __launch_bounds__(128 * DEC_SPLIT) k_decoder_mc_v(const float* __restrict__ what, const float* __restrict__ Wd,
+                                                                  float* __restrict__ y, int C, int N, int frames, int in_pitch,
+                                                                  int crop_left, int T_out) {
+  constexpr int L = STRIDE * R;
+  extern __shared__ float sm[];  // Wd[:, c, :] as [N][L], then the partial sums [DEC_SPLIT-1][STRIDE][128]
+  float* red = sm + (size_t)N * L;
+  const int tid = threadIdx.x, bs = blockIdx.y, tile = blockIdx.x / C, c = blockIdx.x - tile * C;
+  const int seg = tid & 127, part = tid >> 7;
+  for (int i = tid; i < N * L; i += 128 * DEC_SPLIT) {
+    const int n = i / L, k = i - n * L;
+    sm[i] = Wd[((size_t)n * C + c) * L + k];
+  }
+  __syncthreads();
+  const int j = tile * 128 + seg;  // segment index, 0 .. frames+R-2
+  const float* wb = what + (size_t)bs * N * in_pitch;
+  float acc[STRIDE];
+#pragma unroll
+  for (int q = 0; q < STRIDE; ++q) acc[q] = 0.f;
+  bool ok[R];
+#pragma unroll
+  for (int r = 0; r < R; ++r) ok[r] = (j - r) >= 0 && (j - r) < frames;
+  const int nper = (N + DEC_SPLIT - 1) / DEC_SPLIT;
+  const int n_begin = part * nper, n_end = min(N, n_begin + nper);
+  for (int n = n_begin; n < n_end; ++n) {
+    const float* wrow = wb + (size_t)n * in_pitch;
+#pragma unroll
+    for (int r = 0; r < R; ++r) {
+      const float v = ok[r] ? __ldg(wrow + (j - r)) : 0.f;
+#pragma unroll
+      for (int q = 0; q < STRIDE; ++q) acc[q] = fmaf(v, sm[n * L + r * STRIDE + q], acc[q]);
+    }
+  }
+  if (part > 0) {
+#pragma unroll
+    for (int q = 0; q < STRIDE; ++q) red[((part - 1) * STRIDE + q) * 128 + seg] = acc[q];
+  }
+  __syncthreads();
+  if (part == 0) {
+    float* yb = y + ((size_t)bs * C + c) * T_out;
+#pragma unroll
+    for (int q = 0; q < STRIDE; ++q) {
+      float v = acc[q];
+#pragma unroll
+      for (int p2 = 0; p2 < DEC_SPLIT - 1; ++p2) v += red[(p2 * STRIDE + q) * 128 + seg];
+      const int t = j * STRIDE + q - crop_left;
+      if (t >= 0 && t < T_out && j < frames + R - 1) yb[t] = v;
+    }
+  }
+}
+
+// NO_FAST_PATH: outside the fast path (the caller launches k_decoder_mc)
+template <int STRIDE, int R>
+static int launch_decoder_mc_v(const float* what, const float* Wd, float* y, int BS, int C, int N, int frames, int in_pitch, int crop_left,
+                               int T_out, cudaStream_t st) {
+  const size_t smem = sizeof(float) * ((size_t)N * STRIDE * R + (size_t)(DEC_SPLIT - 1) * STRIDE * 128);
+  const long long nblk = (long long)C * ((frames + R - 1 + 127) / 128);
+  if (smem > 200 * 1024 || nblk > 0x7fffffffLL) return NO_FAST_PATH;
+  if (smem > 48 * 1024) {
+    cudaError_t e = cudaFuncSetAttribute(k_decoder_mc_v<STRIDE, R>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+    if (e != cudaSuccess) return (int)e;
+  }
+  k_decoder_mc_v<STRIDE, R><<<dim3((unsigned)nblk, BS), 128 * DEC_SPLIT, smem, st>>>(what, Wd, y, C, N, frames, in_pitch, crop_left, T_out);
+  CTN_COUNT_LAUNCH();
+  CTN_RETURN_IF_CUDA_ERR();
+  return CTN_OK;
+}
+
+// Fallbacks for the geometries the fast paths do not cover (thread = frame / output sample)
 __global__ void __launch_bounds__(128) k_encoder_mc(const float* __restrict__ x, const float* __restrict__ W, float* __restrict__ w, int C,
                                                     int T, int pad_left, int N, int L, int stride, int frames, int pitch, int relu,
                                                     double* __restrict__ stats) {
@@ -363,6 +543,13 @@ extern "C" int ctn_encoder_mc_fwd(const float* x, const float* enc_w, float* w, 
   const int frames = (Tp - L) / stride + 1;
   if (w_pitch < frames) return CTN_EALIGN;
   cudaStream_t st = (cudaStream_t)stream;
+  if (L == 2 * stride && w_pitch % 128 == 0 && (((uintptr_t)w) & 15) == 0) {
+    int rc = NO_FAST_PATH;
+#define ENC_MC_CASE(LL) case LL: rc = launch_encoder_v4_mc<LL>(x, enc_w, w, B, C, T, pad_left, N, frames, w_pitch, relu, stats, st); break
+    switch (L) { ENC_MC_CASE(2); ENC_MC_CASE(4); ENC_MC_CASE(8); ENC_MC_CASE(16); ENC_MC_CASE(20); default: break; }
+#undef ENC_MC_CASE
+    if (rc != NO_FAST_PATH) return rc;
+  }
   k_encoder_mc<<<dim3((w_pitch + 127) / 128, B), 128, 0, st>>>(x, enc_w, w, C, T, pad_left, N, L, stride, frames, w_pitch, relu, stats);
   CTN_COUNT_LAUNCH();
   CTN_RETURN_IF_CUDA_ERR();
@@ -379,6 +566,13 @@ extern "C" int ctn_decoder_mc_fwd(const float* w_hat, const float* dec_w, float*
   const int full = (frames - 1) * stride + L;
   if (crop_left < 0 || T_out <= 0 || crop_left + T_out > full) return CTN_EINVAL;
   cudaStream_t st = (cudaStream_t)stream;
+  const int R = L / stride;
+  int rc = NO_FAST_PATH;
+  if (stride == 8 && R == 2) rc = launch_decoder_mc_v<8, 2>(w_hat, dec_w, y, BS, C, N, frames, in_pitch, crop_left, T_out, st);
+  if (stride == 1 && R == 2) rc = launch_decoder_mc_v<1, 2>(w_hat, dec_w, y, BS, C, N, frames, in_pitch, crop_left, T_out, st);
+  if (stride == 10 && R == 2) rc = launch_decoder_mc_v<10, 2>(w_hat, dec_w, y, BS, C, N, frames, in_pitch, crop_left, T_out, st);
+  if (stride == 2 && R == 2) rc = launch_decoder_mc_v<2, 2>(w_hat, dec_w, y, BS, C, N, frames, in_pitch, crop_left, T_out, st);
+  if (rc != NO_FAST_PATH) return rc;
   k_decoder_mc<<<dim3((T_out + 127) / 128, C, BS), 128, 0, st>>>(w_hat, dec_w, y, C, N, frames, in_pitch, L, stride, crop_left, T_out);
   CTN_COUNT_LAUNCH();
   CTN_RETURN_IF_CUDA_ERR();

@@ -277,8 +277,9 @@ int ctn_transpose(const float* W, float* Wt, int M, int K, cudaStream_t st);
 // FFMA split-K kernel; otherwise ctn_wgrad_wgmma)
 int ctn_wgrad(int math, const float* dy, size_t dy_bs, const float* x, size_t x_bs, float* dWa, float* dWb, int split_row, int M,
               int K, int B, int frames, int pitch, cudaStream_t st);
-// filter-bank weight gradient dW (N, L) += sum_{r,f} act[r][n][f] * sig[r][f*stride + k - pad_left] (signal rows of T samples)
-int ctn_encdec_wgrad(const float* act, const float* sig, float* dW, int R, int N, int frames, int pitch, int T, int L, int stride,
+// filter-bank weight gradient dW (N, C, L) += sum_{r,f} act[r][n][f] * sig[r*C + c][f*stride + k - pad_left] (signal rows of T
+// samples, C per act row)
+int ctn_encdec_wgrad(const float* act, const float* sig, float* dW, int R, int N, int C, int frames, int pitch, int T, int L, int stride,
                      int pad_left, cudaStream_t st);
 // out[c] += sum_{b, t < frames} dy[b][c][t]
 int ctn_rowsum(const float* dy, size_t bs, int C, int B, int frames, int pitch, float* out, cudaStream_t st);

@@ -111,7 +111,13 @@ extern "C" int ctn_probe_dw_combine(float* dw, const float* dwprod, const float*
 
 extern "C" int ctn_probe_encdec_wgrad(const float* act, const float* sig, float* dW, int R, int N, int frames, int pitch, int T, int L,
                                       int stride, int pad_left, ctn_stream_t stream) {
-  return ctn_encdec_wgrad(act, sig, dW, R, N, frames, pitch, T, L, stride, pad_left, (cudaStream_t)stream);
+  return ctn_encdec_wgrad(act, sig, dW, R, N, 1, frames, pitch, T, L, stride, pad_left, (cudaStream_t)stream);
+}
+
+extern "C" int ctn_probe_encdec_wgrad_mc(const float* act, const float* sig, float* dW, int R, int N, int C, int frames, int pitch, int T,
+                                         int L, int stride, int pad_left, ctn_stream_t stream) {
+  if (C < 1) return CTN_EINVAL;
+  return ctn_encdec_wgrad(act, sig, dW, R, N, C, frames, pitch, T, L, stride, pad_left, (cudaStream_t)stream);
 }
 
 extern "C" int ctn_probe_rowsum(const float* dy, size_t bs, int C, int B, int frames, int pitch, float* out, ctn_stream_t stream) {

@@ -465,16 +465,18 @@ __global__ void __launch_bounds__(256) k_dw_combine(float* __restrict__ dw, cons
   }
 }
 
-// ---- filter-bank weight gradients: dW[n][k] += sum_{r,f} act[r][n][f] * sig[r][f*stride + k - pl]
-// (encoder: act = d_w, sig = mixture, filterbank.py:212,222; decoder: act = w_hat, sig = d_out, filterbank.py:243).
-// Fast variant (L <= 32): grid (N, row groups), block 256; a thread walks frames of its rows with all L taps in registers
+// ---- filter-bank weight gradients: dW[n][c][k] += sum_{r,f} act[r][n][f] * sig[r*C + c][f*stride + k - pl]
+// (encoder: act = d_w, sig = mixture, filterbank.py:212,222; decoder: act = w_hat, sig = d_out, filterbank.py:243; C = in_channels,
+// the signal rows of one act row are its C channels).  One CTA column per (n, c) pair, blockIdx = n*C + c: at C = 1 the grid, the
+// accumulation order and so the bits are those of the monaural kernels.
+// Fast variant (L <= 32): grid (N*C, row groups), block 256; a thread walks frames of its rows with all L taps in registers
 // (the signal window comes from L1: neighbouring frames share L - stride samples), one reduction per block at the end.
 #define ENCDEC_MAX_L 32
 __global__ void __launch_bounds__(256) k_encdec_wgrad(const float* __restrict__ act, const float* __restrict__ sig,
-                                                      float* __restrict__ dW, int R, int N, int frames, int pitch, int T, int L,
+                                                      float* __restrict__ dW, int R, int N, int C, int frames, int pitch, int T, int L,
                                                       int stride, int pad_left) {
   __shared__ float sacc[ENCDEC_MAX_L];
-  const int n = blockIdx.x;
+  const int n = blockIdx.x / C, c = blockIdx.x - n * C;
   float acc[ENCDEC_MAX_L];
 #pragma unroll
   for (int k = 0; k < ENCDEC_MAX_L; ++k) acc[k] = 0.f;
@@ -483,7 +485,7 @@ __global__ void __launch_bounds__(256) k_encdec_wgrad(const float* __restrict__ 
   const bool vec = (L % 4 == 0) && (stride % 4 == 0) && (pad_left % 4 == 0) && (T % 4 == 0) && ((((uintptr_t)sig) & 15) == 0);
   for (int r = blockIdx.y; r < R; r += gridDim.y) {
     const float* a = act + ((size_t)r * N + n) * pitch;
-    const float* sg = sig + (size_t)r * T;
+    const float* sg = sig + ((size_t)r * C + c) * T;
     for (int f = threadIdx.x; f < frames; f += 256) {
       const float av = a[f];
       const int t0 = f * stride - pad_left;
@@ -518,18 +520,18 @@ __global__ void __launch_bounds__(256) k_encdec_wgrad(const float* __restrict__ 
     }
   }
   __syncthreads();
-  if (threadIdx.x < L) atomicAdd(&dW[n * L + threadIdx.x], sacc[threadIdx.x]);
+  if (threadIdx.x < L) atomicAdd(&dW[(size_t)blockIdx.x * L + threadIdx.x], sacc[threadIdx.x]);
 }
-// generic variant (any L): grid (L, N), block 256
+// generic variant (any L): grid (L, N*C), block 256
 __global__ void __launch_bounds__(256) k_encdec_wgrad_generic(const float* __restrict__ act, const float* __restrict__ sig,
-                                                              float* __restrict__ dW, int R, int N, int frames, int pitch, int T,
+                                                              float* __restrict__ dW, int R, int N, int C, int frames, int pitch, int T,
                                                               int L, int stride, int pad_left) {
   __shared__ double red[64];
-  const int k = blockIdx.x, n = blockIdx.y;
+  const int k = blockIdx.x, n = blockIdx.y / C, c = blockIdx.y - n * C;
   double s = 0.0, z = 0.0;
   for (int r = 0; r < R; ++r) {
     const float* a = act + ((size_t)r * N + n) * pitch;
-    const float* sg = sig + (size_t)r * T;
+    const float* sg = sig + ((size_t)r * C + c) * T;
     float ls = 0.f;
     for (int f = threadIdx.x; f < frames; f += 256) {
       const int t = f * stride + k - pad_left;
@@ -538,7 +540,7 @@ __global__ void __launch_bounds__(256) k_encdec_wgrad_generic(const float* __res
     s += ls;
   }
   block_sum2_d(s, z, red);
-  if (threadIdx.x == 0) atomicAdd(&dW[n * L + k], (float)s);
+  if (threadIdx.x == 0) atomicAdd(&dW[(size_t)blockIdx.y * L + k], (float)s);
 }
 
 // ---- weight gradient of a 1x1 conv: dW[m][k] += sum_{b, t<frames} dY[b][m][t] * X[b][k][t]
@@ -716,15 +718,16 @@ int ctn_wgrad(int math, const float* dy, size_t dy_bs, const float* x, size_t x_
   return CTN_OK;
 }
 
-int ctn_encdec_wgrad(const float* act, const float* sig, float* dW, int R, int N, int frames, int pitch, int T, int L, int stride,
+int ctn_encdec_wgrad(const float* act, const float* sig, float* dW, int R, int N, int C, int frames, int pitch, int T, int L, int stride,
                      int pad_left, cudaStream_t st) {
+  const int NC = N * C;
   if (L <= ENCDEC_MAX_L) {
-    int gy = (4 * 148 + N - 1) / N;
+    int gy = (4 * 148 + NC - 1) / NC;
     if (gy > R) gy = R;
     if (gy < 1) gy = 1;
-    k_encdec_wgrad<<<dim3(N, gy), 256, 0, st>>>(act, sig, dW, R, N, frames, pitch, T, L, stride, pad_left);
+    k_encdec_wgrad<<<dim3(NC, gy), 256, 0, st>>>(act, sig, dW, R, N, C, frames, pitch, T, L, stride, pad_left);
   } else {
-    k_encdec_wgrad_generic<<<dim3(L, N), 256, 0, st>>>(act, sig, dW, R, N, frames, pitch, T, L, stride, pad_left);
+    k_encdec_wgrad_generic<<<dim3(L, NC), 256, 0, st>>>(act, sig, dW, R, N, C, frames, pitch, T, L, stride, pad_left);
   }
   LAUNCH_CHECK();
   return CTN_OK;
@@ -842,6 +845,25 @@ int check_train_cfg(const ctn_config_t* c) {
   return CTN_OK;
 }
 
+// the ctn_multichannel_* entries: the same pipeline with in_channels = C in [2, 64] (check_model_cfg bounds C at 64)
+int check_mc_train_cfg(const ctn_config_t* c) {
+  CTN_TRY(check_model_cfg(c));
+  if (c->causal || c->mask_softmax || c->in_channels <= 1 || c->sep_kernel > CTN_MAX_P) return CTN_EUNSUPPORTED;
+  return CTN_OK;
+}
+
+// workspace of the gLN training step for a config already checked; no activation depends on the input channel count
+int train_ws_need(const ctn_config_t* cfg, int batch, int T, size_t* bytes) {
+  if (batch <= 0 || !bytes) return CTN_EINVAL;
+  const int frames = ctn_frames(T, cfg->kernel_size, cfg->stride, nullptr, nullptr);
+  if (frames <= 0) return CTN_EINVAL;
+  Carver cv(nullptr);
+  TrainWs ws;
+  carve_train(cv, cfg, batch, ctn_pitch(frames), &ws);
+  *bytes = cv.off + 256;
+  return CTN_OK;
+}
+
 // D (B, M, pitch) = W (M, K) . A (B, K, pitch), raw epilogue, in the configured numeric mode.  The operands here (gradients,
 // and the forward's materialised x_i / gLN2 output) carry no operand scale, so 'f16x3' runs these on the tf32 pieces: gradients
 // have no fixed scale (1e-3 .. 1e-9 and below), which fp16 pieces cannot represent (subnormal below 6e-5, zero below 6e-8).
@@ -856,7 +878,7 @@ int gemm_raw(const ctn_config_t* c, TrainWs& ws, const float* W, int M, int K, c
 // Backward from d_out to the gradient of every block's skip output: decoder, sigmoid mask, mask conv, PReLU on the skip sum.
 // Leaves dS, rows [Bc, Bc + Sc) of dcat (= dS) and nC = d_wprod.  The same for gLN and cLN models.
 int bwd_tail(const ctn_config_t* c, const ctn_params_t* p, const ctn_params_t* grads, TrainWs& ws, const float* d_out, int B, int T,
-             cudaStream_t st) {
+             cudaStream_t st, int Cin = 1) {
   int pl = 0, pr = 0;
   const int frames = ctn_frames(T, c->kernel_size, c->stride, &pl, &pr);
   const int pitch = ctn_pitch(frames);
@@ -864,9 +886,14 @@ int bwd_tail(const ctn_config_t* c, const ctn_params_t* p, const ctn_params_t* g
   const int N = c->n_basis, Bc = c->bottleneck, Sc = c->skip, S = c->n_sources, L = c->kernel_size;
   const size_t bsBc = (size_t)Bc * pitch, bsSc = (size_t)Sc * pitch, bsCat = (size_t)(Bc + Sc) * pitch, bsSN = (size_t)S * N * pitch;
   auto G = [](const float* q) { return const_cast<float*>(q); };
-  // ---- decoder (filterbank.py:243-249): d_what = conv1d(d_out; Wd) (the transposed conv's adjoint), dWd
-  CTN_TRY(ctn_encoder_fwd(d_out, p->dec_w, ws.dwhat, B * S, T, pl, pr, N, L, c->stride, 0, pitch, nullptr, stream));
-  CTN_TRY(ctn_encdec_wgrad(ws.what, d_out, G(grads->dec_w), B * S, N, frames, pitch, T, L, c->stride, pl, st));
+  // ---- decoder (filterbank.py:243-249): d_what = conv1d(d_out; Wd) (the transposed conv's adjoint), dWd.  Multichannel: Wd (N, C, L)
+  // is indexed like a Conv1d(C, N) weight, so the adjoint is the multichannel encoder over the (B*S, C, T) rows of d_out
+  if (Cin == 1) {
+    CTN_TRY(ctn_encoder_fwd(d_out, p->dec_w, ws.dwhat, B * S, T, pl, pr, N, L, c->stride, 0, pitch, nullptr, stream));
+  } else {
+    CTN_TRY(ctn_encoder_mc_fwd(d_out, p->dec_w, ws.dwhat, B * S, Cin, T, pl, pr, N, L, c->stride, 0, pitch, nullptr, stream));
+  }
+  CTN_TRY(ctn_encdec_wgrad(ws.what, d_out, G(grads->dec_w), B * S, N, Cin, frames, pitch, T, L, c->stride, pl, st));
   // ---- w_hat = w * sigmoid(m_pre): d_mpre (in place), d_wprod
   CTN_TRY(ctn_mask_bwd(ws.dwhat, ws.w, ws.mask, ws.nC, B, S, N, frames, pitch, st));
   // ---- mask conv (conv_tasnet.py:341,374): dWm, dbm, d_sp = Wm^T d_mpre
@@ -894,24 +921,19 @@ void ctn_train_tcn_region(const ctn_config_t* c, int B, int pitch, void* mem, vo
 
 extern "C" int ctn_train_workspace_bytes(const ctn_config_t* cfg, int batch, int T, size_t* bytes) {
   CTN_TRY(check_train_cfg(cfg));
-  if (batch <= 0 || !bytes) return CTN_EINVAL;
-  const int frames = ctn_frames(T, cfg->kernel_size, cfg->stride, nullptr, nullptr);
-  if (frames <= 0) return CTN_EINVAL;
-  Carver cv(nullptr);
-  TrainWs ws;
-  carve_train(cv, cfg, batch, ctn_pitch(frames), &ws);
-  *bytes = cv.off + 256;
-  return CTN_OK;
+  return train_ws_need(cfg, batch, T, bytes);
 }
 
-extern "C" int ctn_convtasnet_fwd_train(const ctn_config_t* c, const ctn_params_t* p, const float* x, int B, int T, float* out,
-                                        void* train_ws, size_t train_ws_bytes, ctn_stream_t stream) {
-  LaunchScope scope(x);
-  CTN_TRY(check_train_cfg(c));
+namespace {
+
+// The gLN training step over Cin input channels (x (B, Cin, T), out (B, S, Cin, T)); the config is checked by the caller.  Only the
+// filter banks see Cin: the encoder, the decoder, the decoder's adjoint and the two filter-bank weight gradients.
+int fwd_train(const ctn_config_t* c, const ctn_params_t* p, const float* x, int B, int T, float* out, void* train_ws,
+              size_t train_ws_bytes, ctn_stream_t stream, int Cin) {
   if (!p || !p->blocks || !x || !out || !train_ws || B <= 0 || T <= 0) return CTN_EINVAL;
   if (((uintptr_t)train_ws) & 255) return CTN_EALIGN;
   size_t need = 0;
-  CTN_TRY(ctn_train_workspace_bytes(c, B, T, &need));
+  CTN_TRY(train_ws_need(c, B, T, &need));
   if (train_ws_bytes < need) return CTN_EWORKSPACE;
   int pl = 0, pr = 0;
   const int frames = ctn_frames(T, c->kernel_size, c->stride, &pl, &pr);
@@ -926,7 +948,11 @@ extern "C" int ctn_convtasnet_fwd_train(const ctn_config_t* c, const ctn_params_
   e = cudaMemsetAsync(ws.stats, 0, ws.stats_bytes, st);
   if (e != cudaSuccess) return (int)e;
   // encoder + gLN0 statistics (filterbank.py:222-229)
-  CTN_TRY(ctn_encoder_fwd(x, p->enc_w, ws.w, B, T, pl, pr, N, c->kernel_size, c->stride, c->enc_relu, pitch, ws.stats0, stream));
+  if (Cin == 1) {
+    CTN_TRY(ctn_encoder_fwd(x, p->enc_w, ws.w, B, T, pl, pr, N, c->kernel_size, c->stride, c->enc_relu, pitch, ws.stats0, stream));
+  } else {
+    CTN_TRY(ctn_encoder_mc_fwd(x, p->enc_w, ws.w, B, Cin, T, pl, pr, N, c->kernel_size, c->stride, c->enc_relu, pitch, ws.stats0, stream));
+  }
   // head: x_0 = Wb gLN0(w) + bb (conv_tasnet.py:370-371), gLN0 folded into the contraction like the inference path
   {
     const FoldJob fj{p->bn_w, p->bn_b, p->norm0_g, p->norm0_b, ws.head, Bc, N, 0, sqrtf((float)N * (float)frames) * 1.0001f};
@@ -985,19 +1011,17 @@ extern "C" int ctn_convtasnet_fwd_train(const ctn_config_t* c, const ctn_params_
     a.pro_slope = p->prelu_out; a.bias = p->mask_b; a.wenc = ws.w; a.Nb = N; a.mask_out = ws.mask; a.act_scale = mask_scale;
     CTN_TRY(ctn_pw(a, PRO_PRELU, EPI_MASK, c->math, ws.wimg, st));
   }
-  CTN_TRY(ctn_decoder_fwd(ws.what, p->dec_w, out, B * S, N, frames, pitch, c->kernel_size, c->stride, pl, T, stream));
-  return CTN_OK;
+  if (Cin == 1) return ctn_decoder_fwd(ws.what, p->dec_w, out, B * S, N, frames, pitch, c->kernel_size, c->stride, pl, T, stream);
+  return ctn_decoder_mc_fwd(ws.what, p->dec_w, out, B * S, Cin, N, frames, pitch, c->kernel_size, c->stride, pl, T, stream);
 }
 
 // grads: same layout as params; every tensor must be ZERO on entry (the kernels accumulate with atomics)
-extern "C" int ctn_convtasnet_bwd(const ctn_config_t* c, const ctn_params_t* p, const ctn_params_t* grads, const float* x,
-                                  const float* d_out, int B, int T, void* train_ws, size_t train_ws_bytes, ctn_stream_t stream) {
-  LaunchScope scope(x);
-  CTN_TRY(check_train_cfg(c));
+int bwd(const ctn_config_t* c, const ctn_params_t* p, const ctn_params_t* grads, const float* x, const float* d_out, int B, int T,
+        void* train_ws, size_t train_ws_bytes, ctn_stream_t stream, int Cin) {
   if (!p || !p->blocks || !grads || !grads->blocks || !x || !d_out || !train_ws || B <= 0 || T <= 0) return CTN_EINVAL;
   if (((uintptr_t)train_ws) & 255) return CTN_EALIGN;
   size_t need = 0;
-  CTN_TRY(ctn_train_workspace_bytes(c, B, T, &need));
+  CTN_TRY(train_ws_need(c, B, T, &need));
   if (train_ws_bytes < need) return CTN_EWORKSPACE;
   int pl = 0, pr = 0;
   const int frames = ctn_frames(T, c->kernel_size, c->stride, &pl, &pr);
@@ -1013,7 +1037,7 @@ extern "C" int ctn_convtasnet_bwd(const ctn_config_t* c, const ctn_params_t* p, 
   const double nH = (double)H * (double)frames;
   auto G = [](const float* q) { return const_cast<float*>(q); };
 
-  CTN_TRY(bwd_tail(c, p, grads, ws, d_out, B, T, st));
+  CTN_TRY(bwd_tail(c, p, grads, ws, d_out, B, T, st, Cin));
   // ---- residual blocks, last to first
   for (int i = RX - 1; i >= 0; --i) {
     const ctn_block_params_t& q = p->blocks[i];
@@ -1072,8 +1096,43 @@ extern "C" int ctn_convtasnet_bwd(const ctn_config_t* c, const ctn_params_t* p, 
                             G(grads->norm0_g), G(grads->norm0_b), nullptr, nullptr, B, N, frames, pitch, st));
   CTN_TRY(ctn_dw_combine(ws.nB, ws.nC, ws.w, c->enc_relu, B, N, frames, pitch, st));
   // ---- encoder (filterbank.py:212,222): dWe
-  CTN_TRY(ctn_encdec_wgrad(ws.nB, x, G(grads->enc_w), B, N, frames, pitch, T, L, c->stride, pl, st));
-  return CTN_OK;
+  return ctn_encdec_wgrad(ws.nB, x, G(grads->enc_w), B, N, Cin, frames, pitch, T, L, c->stride, pl, st);
+}
+
+}  // namespace
+
+extern "C" int ctn_convtasnet_fwd_train(const ctn_config_t* c, const ctn_params_t* p, const float* x, int B, int T, float* out,
+                                        void* train_ws, size_t train_ws_bytes, ctn_stream_t stream) {
+  LaunchScope scope(x);
+  CTN_TRY(check_train_cfg(c));
+  return fwd_train(c, p, x, B, T, out, train_ws, train_ws_bytes, stream, 1);
+}
+
+extern "C" int ctn_convtasnet_bwd(const ctn_config_t* c, const ctn_params_t* p, const ctn_params_t* grads, const float* x,
+                                  const float* d_out, int B, int T, void* train_ws, size_t train_ws_bytes, ctn_stream_t stream) {
+  LaunchScope scope(x);
+  CTN_TRY(check_train_cfg(c));
+  return bwd(c, p, grads, x, d_out, B, T, train_ws, train_ws_bytes, stream, 1);
+}
+
+// Multichannel (in_channels = C > 1) models: the same step with the multichannel filter banks; x (B, C, T), out / d_out (B, S, C, T)
+extern "C" int ctn_multichannel_train_workspace_bytes(const ctn_config_t* cfg, int batch, int T, size_t* bytes) {
+  CTN_TRY(check_mc_train_cfg(cfg));
+  return train_ws_need(cfg, batch, T, bytes);
+}
+
+extern "C" int ctn_multichannel_fwd_train(const ctn_config_t* c, const ctn_params_t* p, const float* x, int B, int T, float* out,
+                                          void* train_ws, size_t train_ws_bytes, ctn_stream_t stream) {
+  LaunchScope scope(x);
+  CTN_TRY(check_mc_train_cfg(c));
+  return fwd_train(c, p, x, B, T, out, train_ws, train_ws_bytes, stream, c->in_channels);
+}
+
+extern "C" int ctn_multichannel_bwd(const ctn_config_t* c, const ctn_params_t* p, const ctn_params_t* grads, const float* x,
+                                    const float* d_out, int B, int T, void* train_ws, size_t train_ws_bytes, ctn_stream_t stream) {
+  LaunchScope scope(x);
+  CTN_TRY(check_mc_train_cfg(c));
+  return bwd(c, p, grads, x, d_out, B, T, train_ws, train_ws_bytes, stream, c->in_channels);
 }
 
 // ================================================================================================================
@@ -1274,5 +1333,5 @@ extern "C" int ctn_causal_bwd(const ctn_config_t* c, const ctn_params_t* p, cons
                             nullptr, nullptr, B, N, frames, pitch, st));
   CTN_TRY(ctn_dw_combine(ws.nB, ws.nC, ws.w, c->enc_relu, B, N, frames, pitch, st));
   // ---- encoder (filterbank.py:212,222): dWe
-  return ctn_encdec_wgrad(ws.nB, x, G(grads->enc_w), B, N, frames, pitch, T, c->kernel_size, c->stride, pl, st);
+  return ctn_encdec_wgrad(ws.nB, x, G(grads->enc_w), B, N, 1, frames, pitch, T, c->kernel_size, c->stride, pl, st);
 }

@@ -1,5 +1,5 @@
-"""Autograd glue of the training path (ctn_convtasnet_fwd_train / ctn_convtasnet_bwd, and ctn_causal_fwd_train / ctn_causal_bwd
-for causal models; include/ctn_b200.h).
+"""Autograd glue of the training path (ctn_convtasnet_fwd_train / ctn_convtasnet_bwd, ctn_causal_fwd_train / ctn_causal_bwd
+for causal models and ctn_multichannel_fwd_train / ctn_multichannel_bwd for in_channels > 1; include/ctn_b200.h).
 
 The reference trains with plain autograd over its nn.Module graph (egs/wsj0-mix/common/src/driver.py:146-150:
 ``estimated = model(mixture); loss, _ = pit_criterion(estimated, sources); loss.backward()``).  Here the whole
@@ -23,8 +23,9 @@ def param_list(model):
 class _Entry:
     """the three C entry points of a training node, by name in _native"""
 
-    def __init__(self, workspace_bytes, fwd, bwd):
+    def __init__(self, workspace_bytes, fwd, bwd, multichannel=False):
         self.WORKSPACE_BYTES, self.FWD, self.BWD = workspace_bytes, fwd, bwd
+        self.multichannel = multichannel  # x (B, C, T) -> out (B, S, C, T); otherwise x (B, 1, T) -> out (B, S, T)
 
 
 class _Node:
@@ -33,14 +34,15 @@ class _Node:
     @staticmethod
     def forward(cls, ctx, model, x, *tensors):
         dev = N.require_cuda(x)
-        B, _, T = x.shape
+        B, Cin, T = x.shape
         slots = [s for s, _ in param_list(model)]
         cfg = model.native_config()
         params, keep = N.build_params(zip(slots, tensors), dev)
         need = C.c_size_t(0)
         N.check(getattr(N, cls.WORKSPACE_BYTES)(C.byref(cfg), B, T, C.byref(need)), cls.WORKSPACE_BYTES)
         ws = torch.empty(need.value + 256, dtype=torch.uint8, device=dev)  # owned by this node until backward
-        out = torch.empty(B, model.n_sources, T, dtype=torch.float32, device=dev)
+        shape = (B, model.n_sources, Cin, T) if cls.multichannel else (B, model.n_sources, T)
+        out = torch.empty(shape, dtype=torch.float32, device=dev)
         N.check(getattr(N, cls.FWD)(C.byref(cfg), C.byref(params), x.data_ptr(), B, T, out.data_ptr(), *N.aligned(ws),
                                     N.stream_ptr(dev)), cls.FWD)
         model.last_launches = N.ctn_last_launch_count()
@@ -106,8 +108,25 @@ class CausalTrainFn(torch.autograd.Function):
         return _Node.backward(CausalTrainFn.ENTRY, ctx, d_out)
 
 
+class MultichannelTrainFn(torch.autograd.Function):
+    """The same node over the multichannel pipeline: x (B, C, T) -> (B, S, C, T)."""
+    ENTRY = _Entry("ctn_multichannel_train_workspace_bytes", "ctn_multichannel_fwd_train", "ctn_multichannel_bwd", multichannel=True)
+
+    @staticmethod
+    def forward(ctx, model, x, *tensors):
+        return _Node.forward(MultichannelTrainFn.ENTRY, ctx, model, x, *tensors)
+
+    @staticmethod
+    def backward(ctx, d_out):
+        return _Node.backward(MultichannelTrainFn.ENTRY, ctx, d_out)
+
+
 def run_train(model, x):
     if x.requires_grad:
         raise NotImplementedError("gradient w.r.t. the mixture is not built (the native backward stops at the encoder weights)")
     tensors = [t for _, t in param_list(model)]
-    return (CausalTrainFn if model.causal else ConvTasNetTrainFn).apply(model, x, *tensors)
+    if model.in_channels > 1:
+        fn = MultichannelTrainFn
+    else:
+        fn = CausalTrainFn if model.causal else ConvTasNetTrainFn
+    return fn.apply(model, x, *tensors)

@@ -11,7 +11,8 @@ the crop fused.  Internally activations are (batch, channels, pitch) fp32 with p
 Kernel envelope (anything else raises NotImplementedError, there is no eager fallback): enc_basis = dec_basis =
 'trainable', in_channels = 1, 3-D input, dilated, separable, sep_nonlinear='prelu', sep_norm, mask_nonlinear='sigmoid'.
 causal=False (gLN) runs the fused stack; causal=True (cLN) an un-fused pipeline (csrc/ctn_causal.cu), which trains natively
-once ``model.causal_training = True`` is set.
+once ``model.causal_training = True`` is set.  Multichannel models (in_channels = C > 1, the 4-D input (B, 1, C, T) of the MUSDB18
+recipes) train natively once ``model.multichannel_training = True`` is set (non-causal, sigmoid mask).
 """
 import ctypes as C
 
@@ -134,6 +135,9 @@ class ConvTasNet(nn.Module):
         self.math = None  # numeric mode override: 'fp32' | 'tf32x3' | 'tf32'
         # causal (cLN) models train through the native causal pipeline only when this is set; off, they refuse autograd as before
         self.causal_training = False
+        # multichannel (in_channels > 1) models train through the native multichannel step only when this is set; off, they refuse
+        # autograd as before
+        self.multichannel_training = False
         self.last_launches = 0
         self.last_chunk_perms = None  # separate_long: the chunk permutations of the last call
 
@@ -362,7 +366,13 @@ class ConvTasNet(nn.Module):
             raise ValueError("Not support {} dimension input".format(n_dims))
         training = torch.is_grad_enabled() and any(p.requires_grad for p in self.parameters())
         if training and self.in_channels > 1:
-            raise NotImplementedError("multichannel models (in_channels > 1) are forward only: call under torch.no_grad()")
+            if not self.multichannel_training:
+                raise NotImplementedError("multichannel models (in_channels > 1) train natively only with model.multichannel_training = True "
+                                          "(ctn_multichannel_fwd_train / ctn_multichannel_bwd); without it they are forward only: call "
+                                          "under torch.no_grad()")
+            if self.causal or self.separator.mask_softmax:
+                raise NotImplementedError("multichannel training is built for non-causal models with a sigmoid mask; causal or softmax "
+                                          "multichannel models are forward only: call under torch.no_grad()")
         if training and self.causal and not self.causal_training:
             raise NotImplementedError("causal (cLN) models train natively only with model.causal_training = True (ctn_causal_fwd_train / "
                                       "ctn_causal_bwd); without it they are forward only: call under torch.no_grad()")
@@ -373,8 +383,8 @@ class ConvTasNet(nn.Module):
             if want_latent:
                 raise NotImplementedError("extract_latent under autograd is not built: call it under torch.no_grad()")
             from ._train import run_train
-            out = run_train(self, x)
-            return (out.unsqueeze(2) if n_dims == 4 else out), None
+            out = run_train(self, x)  # multichannel: already (B, S, C, T)
+            return (out.unsqueeze(2) if n_dims == 4 and self.in_channels == 1 else out), None
         B, Cin, T = x.shape
         frames, _, _ = N.frames_of(T, self.kernel_size, self.stride)
         cfg = self.native_config()

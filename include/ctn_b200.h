@@ -67,7 +67,7 @@ typedef struct ctn_config {
   int32_t math;         /* enum ctn_math */
   float eps;            /* Separator head norm eps (ConvTasNet eps)            */
   float eps_tcn;        /* eps of the norms inside the TDCN (reference passes the default 1e-12) */
-  int32_t in_channels;  /* C = n_mics of the 4-D input form (conv_tasnet.py:75,138-141); 0 or 1: monaural.  > 1: forward only */
+  int32_t in_channels;  /* C = n_mics of the 4-D input form (conv_tasnet.py:75,138-141); 0 or 1: monaural.  > 1: trains through ctn_multichannel_* */
 } ctn_config_t;
 
 /* Parameters of one ResidualBlock1d (+ its DepthwiseSeparableConv1d), src/models/tdcn.py:77-196.
@@ -341,6 +341,16 @@ int ctn_causal_fwd_train(const ctn_config_t* cfg, const ctn_params_t* params, co
                          void* train_ws, size_t train_ws_bytes, ctn_stream_t stream);
 int ctn_causal_bwd(const ctn_config_t* cfg, const ctn_params_t* params, const ctn_grads_t* grads, const float* x,
                    const float* d_out, int B, int T, void* train_ws, size_t train_ws_bytes, ctn_stream_t stream);
+/* The same three calls for multichannel models (in_channels = C, the 4-D input form of conv_tasnet.py:138-141,167-168; the
+ * MUSDB18 recipes): x (B,C,T), out and d_out (B,S,C,T); enc_w and dec_w (N,C,L).  One pipeline with ctn_convtasnet_fwd_train /
+ * ctn_convtasnet_bwd: the same separator, the same launch count and the same workspace; the filter banks, the decoder's adjoint
+ * and the two filter-bank weight gradients run over C channels.  Envelope: causal = 0, sigmoid mask, 2 <= in_channels <= 64,
+ * sep_kernel <= 8; an invalid field is CTN_EINVAL, causal, softmax or in_channels <= 1 CTN_EUNSUPPORTED. */
+int ctn_multichannel_train_workspace_bytes(const ctn_config_t* cfg, int batch, int T, size_t* bytes);
+int ctn_multichannel_fwd_train(const ctn_config_t* cfg, const ctn_params_t* params, const float* x, int B, int T, float* out,
+                               void* train_ws, size_t train_ws_bytes, ctn_stream_t stream);
+int ctn_multichannel_bwd(const ctn_config_t* cfg, const ctn_params_t* params, const ctn_grads_t* grads, const float* x,
+                         const float* d_out, int B, int T, void* train_ws, size_t train_ws_bytes, ctn_stream_t stream);
 
 /* Backward of ctn_sisdr_pit_fwd through the selected permutation (src/criterion/pit.py:36-44; sdr.py:135-137):
  * d_est (B,S,T) = grad_loss_b[b] * coef * dSI-SDR(est_i, tgt_perm[i])/d est_i.  fwd_scratch = the scratch buffer the

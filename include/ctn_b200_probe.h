@@ -115,6 +115,10 @@ int ctn_probe_dw_combine(float* dw, const float* dwprod, const float* w, int rel
 /* dW (N, L) += sum_{r < R, f < frames} act[r][n][f] * sig[r][f*stride + k - pad_left] (0 outside [0, T)); act (R, N, pitch) */
 int ctn_probe_encdec_wgrad(const float* act, const float* sig, float* dW, int R, int N, int frames, int pitch, int T, int L,
                            int stride, int pad_left, ctn_stream_t stream);
+/* the same over C signal channels per act row: dW (N, C, L) += sum_{r,f} act[r][n][f] * sig[r*C + c][f*stride + k - pad_left];
+ * sig (R*C, T).  C = 1 is ctn_probe_encdec_wgrad. */
+int ctn_probe_encdec_wgrad_mc(const float* act, const float* sig, float* dW, int R, int N, int C, int frames, int pitch, int T,
+                              int L, int stride, int pad_left, ctn_stream_t stream);
 /* out[c] += sum_{b, t < frames} dy[b * bs + c * pitch + t] */
 int ctn_probe_rowsum(const float* dy, size_t bs, int C, int B, int frames, int pitch, float* out, ctn_stream_t stream);
 /* dst[b][c] (+)= src[b][c], c < C, batch strides dst_bs / src_bs floats; columns [frames, pitch) of dst are written as 0 */
