@@ -137,20 +137,24 @@ __global__ void __launch_bounds__(128) k_encoder_v4(const float* __restrict__ x,
   }
 }
 
+// The encoder kernels' static red[64] counts against the same 48 KB as their dynamic shared memory: a dynamic size within 512 B of
+// 48 KB needs the opt-in too.
+constexpr size_t ENC_STATIC_SMEM = sizeof(double) * 64;
+
 template <int L>
 static int launch_encoder(const float* x, const float* W, float* w, int B, int T, int pad_left, int N, int stride,
                           int frames, int pitch, int relu, double* stats, cudaStream_t st) {
   const int N4 = (N + 3) & ~3;
   const size_t smem = sizeof(float) * ((size_t)L * N4 + 127 * stride + L);
   if (smem > 200 * 1024) return CTN_EUNSUPPORTED;
-  if (smem > 48 * 1024) {
+  if (smem + ENC_STATIC_SMEM > 48 * 1024) {
     cudaError_t e = cudaFuncSetAttribute(k_encoder<L>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
     if (e != cudaSuccess) return (int)e;
   }
   dim3 grid((pitch + 127) / 128, B);
   if constexpr (L <= 20) {  // longer kernels: the 3*stride + L input window no longer fits the register file
   if (stride * 2 == L && pitch % 128 == 0 && (((uintptr_t)w) & 15) == 0) {
-    if (smem > 48 * 1024) {
+    if (smem + ENC_STATIC_SMEM > 48 * 1024) {
       cudaError_t e = cudaFuncSetAttribute(k_encoder_v4<L, L / 2>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
       if (e != cudaSuccess) return (int)e;
     }
@@ -403,7 +407,7 @@ static int launch_encoder_v4_mc(const float* x, const float* W, float* w, int B,
                                 int relu, double* stats, cudaStream_t st) {
   const size_t smem = encoder_v4_mc_smem<L>(C, N);
   if (smem > 200 * 1024) return NO_FAST_PATH;
-  if (smem > 48 * 1024) {
+  if (smem + ENC_STATIC_SMEM > 48 * 1024) {
     cudaError_t e = cudaFuncSetAttribute(k_encoder_v4_mc<L, L / 2>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
     if (e != cudaSuccess) return (int)e;
   }
@@ -542,6 +546,7 @@ extern "C" int ctn_encoder_mc_fwd(const float* x, const float* enc_w, float* w, 
   if (Tp < L || (Tp - L) % stride != 0) return CTN_EINVAL;
   const int frames = (Tp - L) / stride + 1;
   if (w_pitch < frames) return CTN_EALIGN;
+  if (B > 65535) return CTN_EUNSUPPORTED;  // samples ride on gridDim.y (the decoder's adjoint passes B*S rows)
   cudaStream_t st = (cudaStream_t)stream;
   if (L == 2 * stride && w_pitch % 128 == 0 && (((uintptr_t)w) & 15) == 0) {
     int rc = NO_FAST_PATH;

@@ -522,12 +522,13 @@ __global__ void __launch_bounds__(256) k_encdec_wgrad(const float* __restrict__ 
   __syncthreads();
   if (threadIdx.x < L) atomicAdd(&dW[(size_t)blockIdx.x * L + threadIdx.x], sacc[threadIdx.x]);
 }
-// generic variant (any L): grid (L, N*C), block 256
+// generic variant (any L): one CTA per (n, c, k), block 256, flat grid (L*N*C) with k fastest, so the L CTAs that read the same act
+// and sig rows run side by side and share them through L2.  N*C alone reaches 65536 (N = 1024, C = 64): it cannot ride on gridDim.y.
 __global__ void __launch_bounds__(256) k_encdec_wgrad_generic(const float* __restrict__ act, const float* __restrict__ sig,
                                                               float* __restrict__ dW, int R, int N, int C, int frames, int pitch, int T,
                                                               int L, int stride, int pad_left) {
   __shared__ double red[64];
-  const int k = blockIdx.x, n = blockIdx.y / C, c = blockIdx.y - n * C;
+  const int nc = blockIdx.x / L, k = blockIdx.x - nc * L, n = nc / C, c = nc - n * C;
   double s = 0.0, z = 0.0;
   for (int r = 0; r < R; ++r) {
     const float* a = act + ((size_t)r * N + n) * pitch;
@@ -540,7 +541,7 @@ __global__ void __launch_bounds__(256) k_encdec_wgrad_generic(const float* __res
     s += ls;
   }
   block_sum2_d(s, z, red);
-  if (threadIdx.x == 0) atomicAdd(&dW[(size_t)blockIdx.y * L + k], (float)s);
+  if (threadIdx.x == 0) atomicAdd(&dW[(size_t)nc * L + k], (float)s);
 }
 
 // ---- weight gradient of a 1x1 conv: dW[m][k] += sum_{b, t<frames} dY[b][m][t] * X[b][k][t]
@@ -727,7 +728,9 @@ int ctn_encdec_wgrad(const float* act, const float* sig, float* dW, int R, int N
     if (gy < 1) gy = 1;
     k_encdec_wgrad<<<dim3(NC, gy), 256, 0, st>>>(act, sig, dW, R, N, C, frames, pitch, T, L, stride, pad_left);
   } else {
-    k_encdec_wgrad_generic<<<dim3(L, NC), 256, 0, st>>>(act, sig, dW, R, N, C, frames, pitch, T, L, stride, pad_left);
+    const long long ctas = (long long)L * N * C;
+    if (ctas > 0x7fffffffLL) return CTN_EUNSUPPORTED;  // gridDim.x
+    k_encdec_wgrad_generic<<<(unsigned)ctas, 256, 0, st>>>(act, sig, dW, R, N, C, frames, pitch, T, L, stride, pad_left);
   }
   LAUNCH_CHECK();
   return CTN_OK;

@@ -339,6 +339,8 @@ ENC["L16_s4"] = _r("k_encoder<16>, stride 4", L=16, S=4, N=24, T=2003)
 for _N in (1, 3, 512):
     ENC[f"v4_N{_N}"] = _r(f"v4, N = {_N}", L=16, S=8, N=_N, T=2003)
     ENC[f"L16_pitch4_N{_N}"] = _r(f"k_encoder<16>, N = {_N}", L=16, S=8, N=_N, T=2003, wpad=4)
+ENC["v4_N700"] = _r("v4, N = 700: 48 928 B dynamic, over 48 KB only with the static red[64]: the opt-in", L=16, S=8, N=700, T=2003)
+ENC["L16_pitch4_N700"] = _r("k_encoder<16>, N = 700: the opt-in for its static red[64]", L=16, S=8, N=700, T=2003, wpad=4)
 ENC["v4_relu"] = _r("v4, ReLU", L=16, S=8, N=33, T=2003, relu=True)
 ENC["L16_pitch4_relu"] = _r("k_encoder<16>, ReLU", L=16, S=8, N=33, T=2003, relu=True, wpad=4)
 ENC["v4_pl"] = _r("v4, pad_left = 8: the first window reads padding", L=16, S=8, N=33, T=2001, pl=8)

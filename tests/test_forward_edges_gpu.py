@@ -6,7 +6,10 @@ branches, and every row's `reaches` field names the branch and the constant that
      grid and a leading run of exact-zero frames; the causal Conv-TasNet (ctn_causal.cu) through extract_latent and forward,
      its separator() and TimeDilatedConvNet past 1024 frames, and the causality of separator().
   B. The softmax mask (k_softmax_mask) over S*N channels below, at and above F16_MAX_ROWS, and with logits beyond +-100.
-  C. The multichannel filter banks (k_encoder_mc / k_decoder_mc) as modules and inside ConvTasNet(in_channels=C).
+  C. The multichannel filter banks as modules and inside ConvTasNet(in_channels=C): the fast k_encoder_v4_mc / k_decoder_mc_v
+     and the fallback k_encoder_mc / k_decoder_mc, as each row's `reaches` names.  The modules pass w_pitch = frames, so their
+     encoder is fast only at a multiple of 128 frames; the model passes a 128-frame pitch.  test_mc_filterbank_gpu.py tests each
+     of these kernels alone at its edges.
   D. Stand-alone gLN (k_gln_stats / k_gln_apply) past both grid-stride limits, both stand-alone norms under a DC offset, and
      the gLN statistics of stand-alone separator() (k_stats_pitch) under the same offsets.
 
@@ -418,13 +421,13 @@ def test_softmax_mask_vs_fp64(case, mode):
 McMod = collections.namedtuple("McMod", "C L S T relu reaches")
 
 MC_MODULES = {
-    "C2-L2S1": McMod(2, 2, 1, 300, False, "L=2, stride 1: 299 frames"),
-    "C3-L16S8-relu": McMod(3, 16, 8, 1037, True, "ragged T: the module drops a 5-sample tail; ReLU encoder; 128 frames"),
-    "C8-L20S10": McMod(8, 20, 10, 1290, False, "L=20, stride 10; 128 frames"),
-    "C64-L40S20": McMod(64, 40, 20, 2620, False, "C=64, the largest in_channels; L=40, stride 20; 130 frames"),
-    "C3-L16S16": McMod(3, 16, 16, 2064, False, "stride = L: no overlap in the decoder; 129 frames"),
-    "C8-L16S4-T=L": McMod(8, 16, 4, 16, False, "T = L: one frame; the decoder's f_lo / f_hi clamps at both ends"),
-    "C2-L16S4": McMod(2, 16, 4, 532, False, "L / stride = 4 frames per output sample; 130 frames"),
+    "C2-L2S1": McMod(2, 2, 1, 300, False, "k_encoder_mc (w_pitch = 299), k_decoder_mc_v<1,2>: L=2, stride 1: 299 frames"),
+    "C3-L16S8-relu": McMod(3, 16, 8, 1037, True, "k_encoder_v4_mc<16,8>, k_decoder_mc_v<8,2>: ragged T: the module drops a 5-sample tail; ReLU encoder; 128 frames"),
+    "C8-L20S10": McMod(8, 20, 10, 1290, False, "k_encoder_v4_mc<20,10>, k_decoder_mc_v<10,2>: L=20, stride 10; 128 frames"),
+    "C64-L40S20": McMod(64, 40, 20, 2620, False, "k_encoder_mc, k_decoder_mc: C=64, the largest in_channels; L=40, stride 20; 130 frames"),
+    "C3-L16S16": McMod(3, 16, 16, 2064, False, "k_encoder_mc, k_decoder_mc: stride = L: no overlap in the decoder; 129 frames"),
+    "C8-L16S4-T=L": McMod(8, 16, 4, 16, False, "k_encoder_mc, k_decoder_mc: T = L: one frame; the decoder's f_lo / f_hi clamps at both ends"),
+    "C2-L16S4": McMod(2, 16, 4, 532, False, "k_encoder_mc, k_decoder_mc: L / stride = 4 frames per output sample; 130 frames"),
 }
 MC_N = 40
 
@@ -468,13 +471,13 @@ def test_multichannel_filterbank_modules_vs_fp64(case):
 McModel = collections.namedtuple("McModel", "C L S T frames causal relu reaches")
 
 MC_MODELS = {
-    "C2-L2S1": McModel(2, 2, 1, 300, 299, False, False, "L=2, stride 1: no padding"),
-    "C3-L20S10-ragged": McModel(3, 20, 10, 1283, 128, False, False, "pad 3 / 4: decoder crop_left = 3; 128 frames"),
-    "C8-L16S4": McModel(8, 16, 4, 526, 129, False, False, "L / stride = 4, pad 1 / 1; 129 frames"),
-    "C64-L40S20": McModel(64, 40, 20, 415, 20, False, False, "C=64, L=40, stride 20, pad 2 / 3"),
-    "C3-L16S16-T=L": McModel(3, 16, 16, 16, 1, False, False, "stride = L and T = L: one frame, no padding"),
-    "C8-L16S8-relu": McModel(8, 16, 8, 1037, 129, False, True, "ReLU encoder (its gLN statistics from k_encoder_mc); pad 1 / 2"),
-    "C2-causal": McModel(2, 16, 8, 1037, 129, True, False, "causal: the cLN pipeline between multichannel filter banks"),
+    "C2-L2S1": McModel(2, 2, 1, 300, 299, False, False, "k_encoder_v4_mc<2,1>, k_decoder_mc_v<1,2>: L=2, stride 1: no padding"),
+    "C3-L20S10-ragged": McModel(3, 20, 10, 1283, 128, False, False, "k_encoder_v4_mc<20,10>, k_decoder_mc_v<10,2>: pad 3 / 4: decoder crop_left = 3; 128 frames"),
+    "C8-L16S4": McModel(8, 16, 4, 526, 129, False, False, "k_encoder_mc, k_decoder_mc: L / stride = 4, pad 1 / 1; 129 frames"),
+    "C64-L40S20": McModel(64, 40, 20, 415, 20, False, False, "k_encoder_mc, k_decoder_mc: C=64, L=40, stride 20, pad 2 / 3"),
+    "C3-L16S16-T=L": McModel(3, 16, 16, 16, 1, False, False, "k_encoder_mc, k_decoder_mc: stride = L and T = L: one frame, no padding"),
+    "C8-L16S8-relu": McModel(8, 16, 8, 1037, 129, False, True, "k_encoder_v4_mc<16,8> past the 48 KB opt-in (64 KB), k_decoder_mc_v<8,2>: ReLU encoder and its gLN statistics; pad 1 / 2"),
+    "C2-causal": McModel(2, 16, 8, 1037, 129, True, False, "k_encoder_v4_mc<16,8>, k_decoder_mc_v<8,2>: causal: the cLN pipeline between multichannel filter banks"),
 }
 
 
