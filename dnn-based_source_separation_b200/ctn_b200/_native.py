@@ -162,6 +162,16 @@ ctn_chunk_overlap_add = _sig("ctn_chunk_overlap_add", _i, _fp, _fp, _i, _i, _i, 
 ctn_separate_long_workspace_bytes = _sig("ctn_separate_long_workspace_bytes", _i, C.POINTER(Config), _i, _i, _i, _i, _i, C.POINTER(_sz))
 ctn_convtasnet_separate_long = _sig("ctn_convtasnet_separate_long", _i, C.POINTER(Config), C.POINTER(Params), _fp, _i, _i, _i, _i, _i, _i,
                                     _fp, _fp, _fp, _sz, _fp)
+# whole tracks through a model trained on standardised segments: plan, statistics, standardising gather, de-standardising
+# overlap-add, and the call around ctn_convtasnet_fwd
+ctn_track_plan = _sig("ctn_track_plan", _i, _i, _i, _i, C.POINTER(_i), _i)
+ctn_track_stats_scratch_bytes = _sig("ctn_track_stats_scratch_bytes", _sz, _i, _i, _i, _i, _i)
+ctn_track_stats = _sig("ctn_track_stats", _i, _fp, _i, _i, _i, _i, _i, _fp, _fp, _sz, _fp)
+ctn_track_gather = _sig("ctn_track_gather", _i, _fp, _fp, _i, _i, _i, _i, _i, C.c_float, _i, _i, _fp, _fp)
+ctn_track_overlap_add = _sig("ctn_track_overlap_add", _i, _fp, _fp, _i, _i, _i, _i, _i, _i, _fp, _fp)
+ctn_separate_track_workspace_bytes = _sig("ctn_separate_track_workspace_bytes", _i, C.POINTER(Config), _i, _i, _i, _i, _i, C.POINTER(_sz))
+ctn_convtasnet_separate_track = _sig("ctn_convtasnet_separate_track", _i, C.POINTER(Config), C.POINTER(Params), _fp, _i, _i, _i, _i, _i,
+                                     _fp, _fp, _sz, _fp)
 # BSS Eval (mir_eval bss_eval_sources) in fp64
 ctn_bss_workspace_bytes = _sig("ctn_bss_workspace_bytes", _i, _i, _i, _i, _i, C.POINTER(_sz))
 ctn_bss_eval_sources = _sig("ctn_bss_eval_sources", _i, _fp, _fp, _i, _i, _i, _i, _i, _fp, _fp, _fp, _fp, _fp, _fp, _sz, _fp)
@@ -187,6 +197,8 @@ EXPORTED = [
     "ctn_online_state_bytes", "ctn_online_init", "ctn_online_reset", "ctn_online_push", "ctn_online_flush",
     "ctn_chunk_plan", "ctn_chunk_gather", "ctn_chunk_align_scratch_bytes", "ctn_chunk_align", "ctn_chunk_overlap_add",
     "ctn_separate_long_workspace_bytes", "ctn_convtasnet_separate_long",
+    "ctn_track_plan", "ctn_track_stats_scratch_bytes", "ctn_track_stats", "ctn_track_gather", "ctn_track_overlap_add",
+    "ctn_separate_track_workspace_bytes", "ctn_convtasnet_separate_track",
     "ctn_cln_bwd", "ctn_causal_train_workspace_bytes", "ctn_causal_fwd_train", "ctn_causal_bwd",
     "ctn_multichannel_train_workspace_bytes", "ctn_multichannel_fwd_train", "ctn_multichannel_bwd",
     "ctn_bss_workspace_bytes", "ctn_bss_eval_sources", "ctn_bss_images_workspace_bytes", "ctn_bss_eval_images",

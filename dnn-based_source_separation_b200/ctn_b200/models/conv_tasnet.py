@@ -27,6 +27,9 @@ from .tdcn import TimeDilatedConvNet, block_slots, resolve_math
 
 EPS = 1e-12
 DEFAULT_MATH = None
+# separate_track's default segments per forward: one batch of model workspace stays under about 8 GB at the MUSDB18 recipe's size
+# (ctn_separate_track_workspace_bytes; see the method's docstring)
+TRACK_CHUNK_BATCH = 3
 
 
 def _load_checkpoint(path):
@@ -270,7 +273,8 @@ class ConvTasNet(nn.Module):
         ``last_chunk_perms`` (batch, n_chunks, n_sources) int32: row [b, k, s] of chunk k carries output source s."""
         if mixture.dim() != 3 or mixture.size(1) != 1:
             if mixture.dim() == 4:
-                raise NotImplementedError("separate_long takes (batch, 1, T): multichannel input is not built")
+                raise NotImplementedError("separate_long takes (batch, 1, T): multichannel input is not built (whole multichannel "
+                                          "tracks separate through separate_track)")
             raise ValueError("mixture.size() is expected (?, 1, ?), but given {}".format(tuple(mixture.size())))
         if torch.is_grad_enabled() and any(p.requires_grad for p in self.parameters()):
             raise NotImplementedError("separate_long is inference-only: call it under torch.no_grad()")
@@ -295,6 +299,59 @@ class ConvTasNet(nn.Module):
                 "ctn_convtasnet_separate_long")
         self.last_launches = N.ctn_last_launch_count()
         self.last_chunk_perms = perms
+        return out
+
+    def separate_track(self, mixture, segment, hop=None, chunk_batch=TRACK_CHUNK_BATCH):
+        """Separate whole tracks the way the MUSDB18 recipe's tester does, in one C call (ctn_convtasnet_separate_track) without a
+        host synchronisation, inference only.  A multichannel model takes (batch, 1, n_mics, T) and returns (batch, n_sources,
+        n_mics, T); a monaural one (batch, 1, T) -> (batch, n_sources, T).
+
+        Every segment and channel is standardised on its own, (x - mean) / (std + eps) with the unbiased std and this model's
+        ``eps``, run through the model, and mapped back with std * estimate + mean (the mixture's statistics for every source).
+        ``hop=None`` is the tester's layout: the track is zero-padded to a multiple of ``segment`` (the zeros count in the
+        statistics), cut into segments that share no samples, and the estimates are concatenated and cropped to T.
+        ``segment // 2 <= hop <= segment`` instead cuts chunks every ``hop`` samples like ``separate_long`` (the last one moved
+        left to end at T, nothing padded) and cross-fades them with sin^2 ramps.  There is no permutation alignment: stems
+        have a fixed order.
+
+        The segments run through the forward ``chunk_batch`` at a time.  The default, 3, keeps one batch of model workspace at
+        7.9 GB (2.6 GB per segment) for the recipe's separator (N = 256, L = 20, H = 512, B = 256, Sc = 128, X = 10, R = 4,
+        four stereo sources, f16x3) on 8 s segments at 44.1 kHz; the whole call then needs 8.2 GB of workspace for a 240 s track."""
+        C_in = int(self.in_channels)
+        n_dims = mixture.dim()
+        if n_dims == 3:
+            if mixture.size(1) != 1:
+                raise ValueError("input.size() is expected (?, 1, ?), but given {}".format(tuple(mixture.size())))
+            if C_in != 1:
+                raise ValueError("a model with in_channels={} takes the 4-D input (batch, 1, n_mics, T)".format(C_in))
+        elif n_dims == 4:
+            if mixture.size(1) != 1:
+                raise ValueError("input.size() is expected (?, 1, ?, ?), but given {}".format(tuple(mixture.size())))
+            if mixture.size(2) != C_in:
+                raise ValueError("n_mics={} does not match in_channels={}".format(mixture.size(2), C_in))
+        else:
+            raise ValueError("Not support {} dimension input".format(n_dims))
+        if torch.is_grad_enabled() and any(p.requires_grad for p in self.parameters()):
+            raise NotImplementedError("separate_track is inference-only: call it under torch.no_grad()")
+        B, T = mixture.size(0), mixture.size(-1)
+        x = mixture.reshape(B, C_in, T).contiguous()
+        dev = N.require_cuda(x)
+        segment, chunk_batch = int(segment), int(chunk_batch)
+        hop = 0 if hop is None else int(hop)
+        K = N.ctn_track_plan(T, segment, hop, None, 0)
+        if K < 0:
+            N.check(K, "ctn_track_plan(T={}, segment={}, hop={})".format(T, segment, hop))
+        cfg = self.native_config()
+        params, keep = self.native_params(dev)
+        need = C.c_size_t(0)
+        N.check(N.ctn_separate_track_workspace_bytes(C.byref(cfg), B, T, segment, hop, chunk_batch, C.byref(need)),
+                "ctn_separate_track_workspace_bytes")
+        base, nbytes = N.aligned(N.workspace(dev, need.value, tag="separate_track"))
+        out = torch.empty((B, self.n_sources, C_in, T) if n_dims == 4 else (B, self.n_sources, T), dtype=torch.float32, device=dev)
+        N.check(N.ctn_convtasnet_separate_track(C.byref(cfg), C.byref(params), x.data_ptr(), B, T, segment, hop, chunk_batch,
+                                                out.data_ptr(), base, nbytes, N.stream_ptr(dev)),
+                "ctn_convtasnet_separate_track")
+        self.last_launches = N.ctn_last_launch_count()
         return out
 
     @property

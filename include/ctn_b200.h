@@ -227,6 +227,40 @@ int ctn_convtasnet_separate_long(const ctn_config_t* cfg, const ctn_params_t* pa
                                  int chunk_batch, int align, float* out, int32_t* perms_out, void* workspace, size_t workspace_bytes,
                                  ctn_stream_t stream);
 
+/* ---- whole tracks through a model trained on standardised segments (the MUSDB18 recipe's tester) -----------------------------
+ * Each segment and channel is standardised on its own, (x - mean) / (std + eps) with the unbiased std, run through the model,
+ * mapped back with std * est + mean (the mixture's statistics for every source) and overlap-added.  x (B,C,T), C = in_channels.
+ * Plan: hop = 0 is the tester's layout: Lc = segment, K = ceil(T / segment), segment k starts at k*segment, samples at or past T
+ *   read as zero (and count in the statistics), segments share no samples.  segment/2 <= hop <= segment (integer division) is
+ *   the cross-faded layout of ctn_chunk_plan (Lc = min(segment, T), the last chunk ends at T).  Anything else CTN_EINVAL.
+ *   Chunk index g = b*K + k, row (g, c) throughout.  Lc >= 2 (an unbiased std needs two samples), 1 <= C <= 64, else CTN_EINVAL.
+ * ctn_track_plan (host only): returns K (or < 0); starts (nullable) receives the K segment starts, capacity >= K.
+ * ctn_track_stats: stats (B,K,C,2) double = (mean, unbiased std) of every row, in double: per row several CTAs write partial sums
+ *   of x - x[start] and its square into scratch (ctn_track_stats_scratch_bytes(), 8-byte aligned), a second launch sums them
+ *   in a fixed order.  No atomics: the same input gives the same bits.  2 launches.
+ * ctn_track_gather: xc (n,C,Lc) = (float)((x - mean) / (std + eps)) of chunks first .. first + n - 1, computed in double and
+ *   rounded once; an all-zero segment gives zeros when eps > 0.  n*C <= 65535 (else CTN_EUNSUPPORTED).
+ * ctn_track_overlap_add: est (B*K,S,C,Lc) -> out (B,S,C,T), out[b][s][c][t] = sum_k w_k(t) (std_kc est_k[s][c][t - start_k] +
+ *   mean_kc) / sum_k w_k(t), k ascending, in double; w_k as in ctn_chunk_overlap_add (every w_k = 1 in the tester layout, where
+ *   this is concatenate-and-crop).  No permutation alignment: the stems have a fixed order.  B*C <= 65535. */
+int ctn_track_plan(int T, int segment, int hop, int* starts, int capacity);
+size_t ctn_track_stats_scratch_bytes(int B, int C, int T, int segment, int hop);
+int ctn_track_stats(const float* x, int B, int C, int T, int segment, int hop, double* stats, void* scratch, size_t scratch_bytes,
+                    ctn_stream_t stream);
+int ctn_track_gather(const float* x, const double* stats, int B, int C, int T, int segment, int hop, float eps, int first, int n, float* xc,
+                     ctn_stream_t stream);
+int ctn_track_overlap_add(const float* est, const double* stats, int B, int S, int C, int T, int segment, int hop, float* out,
+                          ctn_stream_t stream);
+/* The whole call: x (B,C,T) -> out (B,S,C,T) (C = 1: (B,1,T) -> (B,S,T)).  Statistics; per batch of at most chunk_batch chunks
+ * the standardising gather (eps = cfg->eps) and ctn_convtasnet_fwd (a smaller last batch runs at its own size); then the
+ * overlap-add.  Every launch goes to `stream`, nothing is read back to the host (CUDA-graph capturable).  Envelope: whatever
+ * ctn_convtasnet_fwd accepts (1 <= in_channels <= 64, causal or not, sigmoid or softmax mask, every math mode); B*C <= 65535.
+ * Workspace (256-byte aligned): the forward's workspace for min(chunk_batch, B*K) chunks + one standardised batch
+ * + 4*B*K*S*C*Lc bytes of chunk estimates + the statistics and their partials: only the last two grow with T. */
+int ctn_separate_track_workspace_bytes(const ctn_config_t* cfg, int B, int T, int segment, int hop, int chunk_batch, size_t* bytes);
+int ctn_convtasnet_separate_track(const ctn_config_t* cfg, const ctn_params_t* params, const float* x, int B, int T, int segment, int hop,
+                                  int chunk_batch, float* out, void* workspace, size_t workspace_bytes, ctn_stream_t stream);
+
 /* Separator.forward, src/models/conv_tasnet.py:359-378: w (B,N,frames) -> mask (B,S,N,frames), both contiguous. */
 int ctn_separator_fwd(const ctn_config_t* cfg, const ctn_params_t* params, const float* w, int B, int frames,
                       float* mask, void* workspace, size_t workspace_bytes, ctn_stream_t stream);
