@@ -262,6 +262,10 @@ int ctn_dw_bwd(const float* dupre, const float* hpre, float* dhn, const float* s
 // sigmoid-mask backward: dwhat (B, S*N, pitch) -> d_mpre in place ; dwprod (B, N, pitch) = sum_s dwhat * mask
 int ctn_mask_bwd(float* dwhat, const float* w, const float* mask, float* dwprod, int B, int S, int N, int frames, int pitch,
                  cudaStream_t st);
+// softmax-mask backward (softmax over all S*N channels of a frame): dwhat (B, S*N, pitch) -> d_z = m * (dwhat * w - dot) in place,
+// dot = sum_n w * dwprod ; dwprod (B, N, pitch) = sum_s dwhat * mask.  Pad lanes [frames, pitch) of both are written as 0
+int ctn_softmax_mask_bwd(float* dwhat, const float* w, const float* mask, float* dwprod, int B, int S, int N, int frames, int pitch,
+                         cudaStream_t st);
 int ctn_prelu_apply(const float* x, float* y, const float* slope, int B, int C, int frames, int pitch, cudaStream_t st);
 // dpre = dy * (pre > 0 ? 1 : a) (may alias dy) ; dslope += sum_{pre <= 0} dy * pre
 int ctn_prelu_bwd(const float* dy, const float* pre, float* dpre, const float* slope, float* dslope, int B, int C, int frames,

@@ -94,6 +94,12 @@ extern "C" int ctn_probe_mask_bwd(float* dwhat, const float* w, const float* mas
   return ctn_mask_bwd(dwhat, w, mask, dwprod, B, S, N, frames, pitch, (cudaStream_t)stream);
 }
 
+extern "C" int ctn_probe_softmax_mask_bwd(float* dwhat, const float* w, const float* mask, float* dwprod, int B, int S, int N,
+                                          int frames, int pitch, ctn_stream_t stream) {
+  LaunchScope scope(dwhat);
+  return ctn_softmax_mask_bwd(dwhat, w, mask, dwprod, B, S, N, frames, pitch, (cudaStream_t)stream);
+}
+
 extern "C" int ctn_probe_prelu_apply(const float* x, float* y, const float* slope, int B, int C, int frames, int pitch,
                                      ctn_stream_t stream) {
   return ctn_prelu_apply(x, y, slope, B, C, frames, pitch, (cudaStream_t)stream);

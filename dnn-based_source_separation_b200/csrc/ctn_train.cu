@@ -412,6 +412,55 @@ __global__ void __launch_bounds__(256) k_mask_bwd(float* __restrict__ dwhat, con
   }
 }
 
+// ---- softmax mask head backward (conv_tasnet.py:345-357, 375-376): m = softmax over ALL M = S*N channels of a frame,
+// w_hat[s][n] = w[n] * m[s*N + n].  With g_c = d_what_c * w_n:
+//   d_wprod[n] = sum_s d_what[s][n] * m[s][n]
+//   dot        = sum_c m_c g_c = sum_n w[n] * d_wprod[n]
+//   d_z_c      = m_c * (g_c - dot)                                (in place over d_what)
+// One CTA per (32-frame tile, b), lane = frame (each warp moves 128-byte row segments), warps split n.  Sweep 1 writes d_wprod
+// and each warp's part of dot; the parts are summed in warp order through shared memory; sweep 2 re-reads d_what, m and w and
+// writes d_z.  Lanes t >= frames write 0 to d_z and d_wprod and read nothing.                     grid (pitch / 32, B)
+#define SMB_WARPS 8
+__global__ void __launch_bounds__(SMB_WARPS * 32) k_softmax_mask_bwd(float* __restrict__ dwhat, const float* __restrict__ w,
+                                                                     const float* __restrict__ mask, float* __restrict__ dwprod,
+                                                                     int S, int N, int frames, int pitch) {
+  __shared__ float part[SMB_WARPS][32];
+  const int b = blockIdx.y, lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
+  const int t = blockIdx.x * 32 + lane;
+  const bool valid = t < frames;
+  const size_t rowN = (size_t)b * N, rowSN = (size_t)b * S * N;
+  float dot = 0.f;
+  for (int n = wid; n < N; n += SMB_WARPS) {
+    float acc = 0.f, wv = 0.f;
+    if (valid) {
+      wv = w[(rowN + n) * pitch + t];
+      for (int s = 0; s < S; ++s) {
+        const size_t idx = (rowSN + (size_t)s * N + n) * pitch + t;
+        acc = fmaf(dwhat[idx], mask[idx], acc);
+      }
+      dot = fmaf(wv, acc, dot);
+    }
+    dwprod[(rowN + n) * pitch + t] = acc;
+  }
+  part[wid][lane] = dot;
+  __syncthreads();
+  dot = 0.f;
+#pragma unroll
+  for (int k = 0; k < SMB_WARPS; ++k) dot += part[k][lane];
+  for (int n = wid; n < N; n += SMB_WARPS) {
+    const float wv = valid ? w[(rowN + n) * pitch + t] : 0.f;
+    for (int s = 0; s < S; ++s) {
+      const size_t idx = (rowSN + (size_t)s * N + n) * pitch + t;
+      float v = 0.f;
+      if (valid) {
+        const float m = mask[idx];
+        v = m * fmaf(dwhat[idx], wv, -dot);
+      }
+      dwhat[idx] = v;
+    }
+  }
+}
+
 __global__ void __launch_bounds__(256) k_prelu_apply(const float* __restrict__ x, float* __restrict__ y,
                                                      const float* __restrict__ slope, int C, int frames, int pitch) {
   const int b = blockIdx.y;
@@ -663,6 +712,15 @@ int ctn_mask_bwd(float* dwhat, const float* w, const float* mask, float* dwprod,
   return CTN_OK;
 }
 
+int ctn_softmax_mask_bwd(float* dwhat, const float* w, const float* mask, float* dwprod, int B, int S, int N, int frames, int pitch,
+                         cudaStream_t st) {
+  if (B <= 0 || S <= 0 || N <= 0 || frames <= 0 || pitch < frames || pitch % 32 != 0) return CTN_EINVAL;
+  if (B > 65535) return CTN_EUNSUPPORTED;
+  k_softmax_mask_bwd<<<dim3(pitch / 32, B), SMB_WARPS * 32, 0, st>>>(dwhat, w, mask, dwprod, S, N, frames, pitch);
+  LAUNCH_CHECK();
+  return CTN_OK;
+}
+
 int ctn_prelu_apply(const float* x, float* y, const float* slope, int B, int C, int frames, int pitch, cudaStream_t st) {
   k_prelu_apply<<<grid_cb(C, B), 256, 0, st>>>(x, y, slope, C, frames, pitch);
   LAUNCH_CHECK();
@@ -855,6 +913,13 @@ int check_mc_train_cfg(const ctn_config_t* c) {
   return CTN_OK;
 }
 
+// the ctn_softmax_* entries: the gLN pipeline with the softmax mask (mask_softmax = 1), monaural and non-causal
+int check_softmax_train_cfg(const ctn_config_t* c) {
+  CTN_TRY(check_model_cfg(c));
+  if (!c->mask_softmax || c->causal || c->in_channels > 1 || c->sep_kernel > CTN_MAX_P) return CTN_EUNSUPPORTED;
+  return CTN_OK;
+}
+
 // workspace of the gLN training step for a config already checked; no activation depends on the input channel count
 int train_ws_need(const ctn_config_t* cfg, int batch, int T, size_t* bytes) {
   if (batch <= 0 || !bytes) return CTN_EINVAL;
@@ -878,8 +943,8 @@ int gemm_raw(const ctn_config_t* c, TrainWs& ws, const float* W, int M, int K, c
   return ctn_pw(a, PRO_NONE, EPI_RAW, c->math, ws.wimg, st);
 }
 
-// Backward from d_out to the gradient of every block's skip output: decoder, sigmoid mask, mask conv, PReLU on the skip sum.
-// Leaves dS, rows [Bc, Bc + Sc) of dcat (= dS) and nC = d_wprod.  The same for gLN and cLN models.
+// Backward from d_out to the gradient of every block's skip output: decoder, sigmoid (or softmax) mask, mask conv, PReLU on the
+// skip sum.  Leaves dS, rows [Bc, Bc + Sc) of dcat (= dS) and nC = d_wprod.  The same for gLN and cLN models.
 int bwd_tail(const ctn_config_t* c, const ctn_params_t* p, const ctn_params_t* grads, TrainWs& ws, const float* d_out, int B, int T,
              cudaStream_t st, int Cin = 1) {
   int pl = 0, pr = 0;
@@ -897,8 +962,12 @@ int bwd_tail(const ctn_config_t* c, const ctn_params_t* p, const ctn_params_t* g
     CTN_TRY(ctn_encoder_mc_fwd(d_out, p->dec_w, ws.dwhat, B * S, Cin, T, pl, pr, N, L, c->stride, 0, pitch, nullptr, stream));
   }
   CTN_TRY(ctn_encdec_wgrad(ws.what, d_out, G(grads->dec_w), B * S, N, Cin, frames, pitch, T, L, c->stride, pl, st));
-  // ---- w_hat = w * sigmoid(m_pre): d_mpre (in place), d_wprod
-  CTN_TRY(ctn_mask_bwd(ws.dwhat, ws.w, ws.mask, ws.nC, B, S, N, frames, pitch, st));
+  // ---- w_hat = w * sigmoid(m_pre) (or w * softmax over all S*N channels of m_pre): d_mpre (in place), d_wprod
+  if (c->mask_softmax) {
+    CTN_TRY(ctn_softmax_mask_bwd(ws.dwhat, ws.w, ws.mask, ws.nC, B, S, N, frames, pitch, st));
+  } else {
+    CTN_TRY(ctn_mask_bwd(ws.dwhat, ws.w, ws.mask, ws.nC, B, S, N, frames, pitch, st));
+  }
   // ---- mask conv (conv_tasnet.py:341,374): dWm, dbm, d_sp = Wm^T d_mpre
   CTN_TRY(ctn_prelu_apply(ws.skip, ws.sp, p->prelu_out, B, Sc, frames, pitch, st));
   CTN_TRY(ctn_wgrad(c->math, ws.dwhat, bsSN, ws.sp, bsSc, G(grads->mask_w), nullptr, 0, S * N, Sc, B, frames, pitch, st));
@@ -1006,21 +1075,30 @@ int fwd_train(const ctn_config_t* c, const ctn_params_t* p, const float* x, int 
     CTN_TRY(ctn_res_skip_fwd(ws.r, Mt, ws.x[i], has_out ? ws.x[i + 1] : nullptr, ws.skip, q.out_b, q.skip_b, Bc, Sc, has_out ? 1 : 0,
                              i == 0 ? 1 : 0, B, frames, pitch, st));
   }
-  // tail: PReLU -> mask 1x1 -> sigmoid -> * w (conv_tasnet.py:373-376, 158-160); keeps the mask
+  // tail: PReLU -> mask 1x1 -> sigmoid -> * w (conv_tasnet.py:373-376, 158-160); keeps the mask.  Softmax masks: the logits
+  // first, then one normalising pass over all S*N channels that keeps the softmax in ws.mask (exactly run_separator's two calls)
   {
     PwArgs a;
     memset(&a, 0, sizeof(a));
     a.A = ws.skip; a.W = p->mask_w; a.D = ws.what; a.B = B; a.M = S * N; a.K = Sc; a.frames = frames; a.pitch = pitch;
     a.pro_slope = p->prelu_out; a.bias = p->mask_b; a.wenc = ws.w; a.Nb = N; a.mask_out = ws.mask; a.act_scale = mask_scale;
-    CTN_TRY(ctn_pw(a, PRO_PRELU, EPI_MASK, c->math, ws.wimg, st));
+    if (c->mask_softmax) {
+      a.mask_logits = 1;
+      a.mask_out = nullptr;
+      CTN_TRY(ctn_pw(a, PRO_PRELU, EPI_MASK, c->math, ws.wimg, st));
+      CTN_TRY(ctn_softmax_mask(ws.what, ws.w, ws.mask, B, S * N, N, frames, pitch, st));
+    } else {
+      CTN_TRY(ctn_pw(a, PRO_PRELU, EPI_MASK, c->math, ws.wimg, st));
+    }
   }
   if (Cin == 1) return ctn_decoder_fwd(ws.what, p->dec_w, out, B * S, N, frames, pitch, c->kernel_size, c->stride, pl, T, stream);
   return ctn_decoder_mc_fwd(ws.what, p->dec_w, out, B * S, Cin, N, frames, pitch, c->kernel_size, c->stride, pl, T, stream);
 }
 
-// grads: same layout as params; every tensor must be ZERO on entry (the kernels accumulate with atomics)
-int bwd(const ctn_config_t* c, const ctn_params_t* p, const ctn_params_t* grads, const float* x, const float* d_out, int B, int T,
-        void* train_ws, size_t train_ws_bytes, ctn_stream_t stream, int Cin) {
+// grads: same layout as params; every tensor must be ZERO on entry (the kernels accumulate with atomics).  d_x (B, Cin = 1, T), when
+// not null, is overwritten with the gradient w.r.t. the mixture
+int bwd(const ctn_config_t* c, const ctn_params_t* p, const ctn_params_t* grads, const float* x, const float* d_out, float* d_x, int B,
+        int T, void* train_ws, size_t train_ws_bytes, ctn_stream_t stream, int Cin) {
   if (!p || !p->blocks || !grads || !grads->blocks || !x || !d_out || !train_ws || B <= 0 || T <= 0) return CTN_EINVAL;
   if (((uintptr_t)train_ws) & 255) return CTN_EALIGN;
   size_t need = 0;
@@ -1099,7 +1177,11 @@ int bwd(const ctn_config_t* c, const ctn_params_t* p, const ctn_params_t* grads,
                             G(grads->norm0_g), G(grads->norm0_b), nullptr, nullptr, B, N, frames, pitch, st));
   CTN_TRY(ctn_dw_combine(ws.nB, ws.nC, ws.w, c->enc_relu, B, N, frames, pitch, st));
   // ---- encoder (filterbank.py:212,222): dWe
-  return ctn_encdec_wgrad(ws.nB, x, G(grads->enc_w), B, N, Cin, frames, pitch, T, L, c->stride, pl, st);
+  CTN_TRY(ctn_encdec_wgrad(ws.nB, x, G(grads->enc_w), B, N, Cin, frames, pitch, T, L, c->stride, pl, st));
+  if (!d_x) return CTN_OK;
+  // ---- mixture: d_x = conv_transpose1d(d_w, We) cropped by the encoder's left pad to T, the encoder's adjoint.  We (N, 1, L) has
+  // the layout of a ConvTranspose1d(N, 1, L) weight, and d_w (nB) has zero pad lanes, so this is the decoder over B rows
+  return ctn_decoder_fwd(ws.nB, p->enc_w, d_x, B, N, frames, pitch, L, c->stride, pl, T, stream);
 }
 
 }  // namespace
@@ -1115,7 +1197,7 @@ extern "C" int ctn_convtasnet_bwd(const ctn_config_t* c, const ctn_params_t* p, 
                                   const float* d_out, int B, int T, void* train_ws, size_t train_ws_bytes, ctn_stream_t stream) {
   LaunchScope scope(x);
   CTN_TRY(check_train_cfg(c));
-  return bwd(c, p, grads, x, d_out, B, T, train_ws, train_ws_bytes, stream, 1);
+  return bwd(c, p, grads, x, d_out, nullptr, B, T, train_ws, train_ws_bytes, stream, 1);
 }
 
 // Multichannel (in_channels = C > 1) models: the same step with the multichannel filter banks; x (B, C, T), out / d_out (B, S, C, T)
@@ -1135,7 +1217,28 @@ extern "C" int ctn_multichannel_bwd(const ctn_config_t* c, const ctn_params_t* p
                                     const float* d_out, int B, int T, void* train_ws, size_t train_ws_bytes, ctn_stream_t stream) {
   LaunchScope scope(x);
   CTN_TRY(check_mc_train_cfg(c));
-  return bwd(c, p, grads, x, d_out, B, T, train_ws, train_ws_bytes, stream, c->in_channels);
+  return bwd(c, p, grads, x, d_out, nullptr, B, T, train_ws, train_ws_bytes, stream, c->in_channels);
+}
+
+// Softmax-mask models (mask_nonlinear='softmax', the ORPIT / Sinkhorn PIT recipes): the same step with the softmax over all S*N
+// mask channels; the workspace of the sigmoid step (ws.mask holds the softmax, d_z goes in place over d_what).  d_x may be null
+extern "C" int ctn_softmax_train_workspace_bytes(const ctn_config_t* cfg, int batch, int T, size_t* bytes) {
+  CTN_TRY(check_softmax_train_cfg(cfg));
+  return train_ws_need(cfg, batch, T, bytes);
+}
+
+extern "C" int ctn_softmax_fwd_train(const ctn_config_t* c, const ctn_params_t* p, const float* x, int B, int T, float* out,
+                                     void* train_ws, size_t train_ws_bytes, ctn_stream_t stream) {
+  LaunchScope scope(x);
+  CTN_TRY(check_softmax_train_cfg(c));
+  return fwd_train(c, p, x, B, T, out, train_ws, train_ws_bytes, stream, 1);
+}
+
+extern "C" int ctn_softmax_bwd(const ctn_config_t* c, const ctn_params_t* p, const ctn_params_t* grads, const float* x,
+                               const float* d_out, float* d_x, int B, int T, void* train_ws, size_t train_ws_bytes, ctn_stream_t stream) {
+  LaunchScope scope(x);
+  CTN_TRY(check_softmax_train_cfg(c));
+  return bwd(c, p, grads, x, d_out, d_x, B, T, train_ws, train_ws_bytes, stream, 1);
 }
 
 // ================================================================================================================

@@ -120,6 +120,10 @@ ctn_multichannel_train_workspace_bytes = _sig("ctn_multichannel_train_workspace_
 ctn_multichannel_fwd_train = _sig("ctn_multichannel_fwd_train", _i, C.POINTER(Config), C.POINTER(Params), _fp, _i, _i, _fp, _fp, _sz, _fp)
 ctn_multichannel_bwd = _sig("ctn_multichannel_bwd", _i, C.POINTER(Config), C.POINTER(Params), C.POINTER(Params), _fp, _fp, _i, _i, _fp, _sz,
                             _fp)
+ctn_softmax_train_workspace_bytes = _sig("ctn_softmax_train_workspace_bytes", _i, C.POINTER(Config), _i, _i, C.POINTER(_sz))
+ctn_softmax_fwd_train = _sig("ctn_softmax_fwd_train", _i, C.POINTER(Config), C.POINTER(Params), _fp, _i, _i, _fp, _fp, _sz, _fp)
+ctn_softmax_bwd = _sig("ctn_softmax_bwd", _i, C.POINTER(Config), C.POINTER(Params), C.POINTER(Params), _fp, _fp, _fp, _i, _i, _fp, _sz,
+                       _fp)
 ctn_encoder_mc_fwd = _sig("ctn_encoder_mc_fwd", _i, _fp, _fp, _fp, _i, _i, _i, _i, _i, _i, _i, _i, _i, _i, _fp, _fp)
 ctn_decoder_mc_fwd = _sig("ctn_decoder_mc_fwd", _i, _fp, _fp, _fp, _i, _i, _i, _i, _i, _i, _i, _i, _i, _fp)
 ctn_sdr_fwd = _sig("ctn_sdr_fwd", _i, _fp, _fp, _i, _i, _f, _fp, _fp, _fp)
@@ -201,6 +205,7 @@ EXPORTED = [
     "ctn_separate_track_workspace_bytes", "ctn_convtasnet_separate_track",
     "ctn_cln_bwd", "ctn_causal_train_workspace_bytes", "ctn_causal_fwd_train", "ctn_causal_bwd",
     "ctn_multichannel_train_workspace_bytes", "ctn_multichannel_fwd_train", "ctn_multichannel_bwd",
+    "ctn_softmax_train_workspace_bytes", "ctn_softmax_fwd_train", "ctn_softmax_bwd",
     "ctn_bss_workspace_bytes", "ctn_bss_eval_sources", "ctn_bss_images_workspace_bytes", "ctn_bss_eval_images",
 ]
 

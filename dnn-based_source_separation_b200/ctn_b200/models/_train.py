@@ -1,11 +1,17 @@
 """Autograd glue of the training path (ctn_convtasnet_fwd_train / ctn_convtasnet_bwd, ctn_causal_fwd_train / ctn_causal_bwd
-for causal models and ctn_multichannel_fwd_train / ctn_multichannel_bwd for in_channels > 1; include/ctn_b200.h).
+for causal models, ctn_multichannel_fwd_train / ctn_multichannel_bwd for in_channels > 1 and ctn_softmax_fwd_train /
+ctn_softmax_bwd for softmax masks; include/ctn_b200.h).
 
 The reference trains with plain autograd over its nn.Module graph (egs/wsj0-mix/common/src/driver.py:146-150:
 ``estimated = model(mixture); loss, _ = pit_criterion(estimated, sources); loss.backward()``).  Here the whole
 model is ONE autograd node: the forward keeps the per-block activations in a device buffer owned by the node, the
 backward is one C call that fills the gradients of all parameter tensors.  Gradients come back as views of one flat
-zero-initialised buffer (the natural bucket for the data-parallel all-reduce, see ctn_b200/dist.py)."""
+zero-initialised buffer (the natural bucket for the data-parallel all-reduce, see ctn_b200/dist.py).
+
+Only the softmax node takes a mixture that requires grad, and returns its gradient: the ORPIT fine-tune step feeds an estimate
+back in as the next stage's mixture (egs/wsj0-mix/orpit_conv-tasnet/src/adhoc_driver.py, FinetuneTrainer.run_one_epoch_train)
+and calls backward once over all stages.  So that clip + Adam still see one flat bucket, the softmax nodes of one backward pass
+share it: the first to run owns the bucket, each later one adds its gradients into it in place."""
 import ctypes as C
 
 import torch
@@ -23,9 +29,10 @@ def param_list(model):
 class _Entry:
     """the three C entry points of a training node, by name in _native"""
 
-    def __init__(self, workspace_bytes, fwd, bwd, multichannel=False):
+    def __init__(self, workspace_bytes, fwd, bwd, multichannel=False, mixture_grad=False):
         self.WORKSPACE_BYTES, self.FWD, self.BWD = workspace_bytes, fwd, bwd
         self.multichannel = multichannel  # x (B, C, T) -> out (B, S, C, T); otherwise x (B, 1, T) -> out (B, S, T)
+        self.mixture_grad = mixture_grad  # BWD takes a nullable d_x after d_out, and the nodes of one backward pass share a bucket
 
 
 class _Node:
@@ -75,12 +82,28 @@ class _Node:
         flat = torch.zeros(total, dtype=torch.float32, device=dev)
         gviews = [None if t is None else flat[o:o + t.numel()].view(t.shape) for t, o in zip(tensors, offs)]
         grads, keep2 = N.build_params(zip(ctx.slots, gviews), dev)
-        N.check(getattr(N, cls.BWD)(C.byref(cfg), C.byref(params), C.byref(grads), x.data_ptr(), d_out.data_ptr(), B, T,
-                                    *N.aligned(ws), N.stream_ptr(dev)), cls.BWD)
+        d_x = None
+        if cls.mixture_grad:
+            d_x = torch.empty_like(x) if ctx.needs_input_grad[1] else None  # null: no gradient, no launch
+            N.check(getattr(N, cls.BWD)(C.byref(cfg), C.byref(params), C.byref(grads), x.data_ptr(), d_out.data_ptr(), N.ptr(d_x), B,
+                                        T, *N.aligned(ws), N.stream_ptr(dev)), cls.BWD)
+        else:
+            N.check(getattr(N, cls.BWD)(C.byref(cfg), C.byref(params), C.byref(grads), x.data_ptr(), d_out.data_ptr(), B, T,
+                                        *N.aligned(ws), N.stream_ptr(dev)), cls.BWD)
         ctx.model.last_bwd_launches = N.ctn_last_launch_count()
-        ctx.model.last_flat_grad = flat
         ctx.ws = None
-        return (None, None) + tuple(g if (t is not None and t.requires_grad) else None for g, t in zip(gviews, tensors))
+        if cls.mixture_grad:
+            # a node that ran earlier in this backward pass (a later fine-tune stage) owns the bucket: its views are what autograd
+            # accumulates into the parameters' .grad, so add into them and pass nothing for the parameters
+            task = torch._C._current_graph_task_id()
+            owner = getattr(ctx.model, "_flat_grad_task", None)
+            prev = getattr(ctx.model, "last_flat_grad", None)
+            if task >= 0 and owner == (task, total) and prev is not None and prev.device == flat.device:
+                prev.add_(flat)
+                return (None, d_x) + (None,) * len(tensors)
+            ctx.model._flat_grad_task = (task, total)
+        ctx.model.last_flat_grad = flat
+        return (None, d_x) + tuple(g if (t is not None and t.requires_grad) else None for g, t in zip(gviews, tensors))
 
 
 class ConvTasNetTrainFn(torch.autograd.Function):
@@ -121,12 +144,28 @@ class MultichannelTrainFn(torch.autograd.Function):
         return _Node.backward(MultichannelTrainFn.ENTRY, ctx, d_out)
 
 
+class SoftmaxTrainFn(torch.autograd.Function):
+    """The same node over the softmax-mask step; the only node that returns the gradient w.r.t. the mixture."""
+    ENTRY = _Entry("ctn_softmax_train_workspace_bytes", "ctn_softmax_fwd_train", "ctn_softmax_bwd", mixture_grad=True)
+
+    @staticmethod
+    def forward(ctx, model, x, *tensors):
+        return _Node.forward(SoftmaxTrainFn.ENTRY, ctx, model, x, *tensors)
+
+    @staticmethod
+    def backward(ctx, d_out):
+        return _Node.backward(SoftmaxTrainFn.ENTRY, ctx, d_out)
+
+
 def run_train(model, x):
-    if x.requires_grad:
+    softmax = model.softmax_training and model.separator.mask_softmax and not model.causal and model.in_channels <= 1
+    if x.requires_grad and not softmax:
         raise NotImplementedError("gradient w.r.t. the mixture is not built (the native backward stops at the encoder weights)")
     tensors = [t for _, t in param_list(model)]
     if model.in_channels > 1:
         fn = MultichannelTrainFn
+    elif softmax:
+        fn = SoftmaxTrainFn
     else:
         fn = CausalTrainFn if model.causal else ConvTasNetTrainFn
     return fn.apply(model, x, *tensors)

@@ -12,7 +12,10 @@ Kernel envelope (anything else raises NotImplementedError, there is no eager fal
 'trainable', in_channels = 1, 3-D input, dilated, separable, sep_nonlinear='prelu', sep_norm, mask_nonlinear='sigmoid'.
 causal=False (gLN) runs the fused stack; causal=True (cLN) an un-fused pipeline (csrc/ctn_causal.cu), which trains natively
 once ``model.causal_training = True`` is set.  Multichannel models (in_channels = C > 1, the 4-D input (B, 1, C, T) of the MUSDB18
-recipes) train natively once ``model.multichannel_training = True`` is set (non-causal, sigmoid mask).
+recipes) train natively once ``model.multichannel_training = True`` is set (non-causal, sigmoid mask).  Softmax-mask models
+(mask_nonlinear='softmax', the ORPIT and Sinkhorn PIT recipes) run forward in every configuration and train natively once
+``model.softmax_training = True`` is set (non-causal, monaural); that step also returns the gradient w.r.t. a mixture that
+requires grad, which the ORPIT recipe's recursive fine-tune step needs.
 """
 import ctypes as C
 
@@ -57,7 +60,7 @@ class Separator(nn.Module):
         if mask_nonlinear == 'sigmoid':
             self.mask_softmax = False
         elif mask_nonlinear == 'softmax':
-            self.mask_softmax = True   # nn.Softmax(dim=1) over ALL n_sources*num_features channels (conv_tasnet.py:345-357); inference only
+            self.mask_softmax = True   # nn.Softmax(dim=1) over ALL n_sources*num_features channels (conv_tasnet.py:345-357); trains with ConvTasNet.softmax_training
         else:
             raise ValueError("Cannot support {}".format(mask_nonlinear))
         self.math = None
@@ -141,6 +144,8 @@ class ConvTasNet(nn.Module):
         # multichannel (in_channels > 1) models train through the native multichannel step only when this is set; off, they refuse
         # autograd as before
         self.multichannel_training = False
+        # softmax-mask models train through the native softmax step only when this is set; off, they refuse autograd as before
+        self.softmax_training = False
         self.last_launches = 0
         self.last_chunk_perms = None  # separate_long: the chunk permutations of the last call
 
@@ -430,6 +435,10 @@ class ConvTasNet(nn.Module):
             if self.causal or self.separator.mask_softmax:
                 raise NotImplementedError("multichannel training is built for non-causal models with a sigmoid mask; causal or softmax "
                                           "multichannel models are forward only: call under torch.no_grad()")
+        if training and self.separator.mask_softmax and self.softmax_training and (self.causal or self.in_channels > 1):
+            raise NotImplementedError("softmax-mask training is built for non-causal monaural models (ctn_softmax_fwd_train / "
+                                      "ctn_softmax_bwd); causal or multichannel softmax models are forward only: call under "
+                                      "torch.no_grad()")
         if training and self.causal and not self.causal_training:
             raise NotImplementedError("causal (cLN) models train natively only with model.causal_training = True (ctn_causal_fwd_train / "
                                       "ctn_causal_bwd); without it they are forward only: call under torch.no_grad()")

@@ -63,7 +63,7 @@ typedef struct ctn_config {
   int32_t n_sources;    /* S  */
   int32_t causal;       /* 0: gLN (supported), 1: cLN (CTN_EUNSUPPORTED in the fused path) */
   int32_t enc_relu;     /* enc_nonlinear == 'relu' */
-  int32_t mask_softmax; /* mask_nonlinear == 'softmax' -> CTN_EUNSUPPORTED */
+  int32_t mask_softmax; /* mask_nonlinear == 'softmax'; trains through ctn_softmax_* (the other training entries: CTN_EUNSUPPORTED) */
   int32_t math;         /* enum ctn_math */
   float eps;            /* Separator head norm eps (ConvTasNet eps)            */
   float eps_tcn;        /* eps of the norms inside the TDCN (reference passes the default 1e-12) */
@@ -385,6 +385,19 @@ int ctn_multichannel_fwd_train(const ctn_config_t* cfg, const ctn_params_t* para
                                void* train_ws, size_t train_ws_bytes, ctn_stream_t stream);
 int ctn_multichannel_bwd(const ctn_config_t* cfg, const ctn_params_t* params, const ctn_grads_t* grads, const float* x,
                          const float* d_out, int B, int T, void* train_ws, size_t train_ws_bytes, ctn_stream_t stream);
+/* The same three calls for softmax-mask models (mask_nonlinear='softmax': nn.Softmax(dim=1) over ALL S*N mask channels of a frame,
+ * conv_tasnet.py:345-357; the ORPIT and Sinkhorn PIT recipes).  The forward is ctn_convtasnet_fwd's estimate (mask logits, then one
+ * softmax pass that keeps the mask in train_ws): one launch more than the sigmoid step.  The workspace equals
+ * ctn_train_workspace_bytes of the same config with mask_softmax = 0.  ctn_softmax_bwd takes one more argument, d_x (B,1,T),
+ * nullable: when given it is OVERWRITTEN with the gradient w.r.t. the mixture (the encoder's adjoint, one more launch), which a
+ * recursive fine-tune step needs when the mixture is an earlier estimate; null skips it.  Envelope: mask_softmax = 1, causal = 0,
+ * in_channels <= 1, sep_kernel <= 8; an invalid field is CTN_EINVAL, mask_softmax = 0, causal or in_channels > 1 CTN_EUNSUPPORTED;
+ * a null pointer other than d_x is CTN_EINVAL before any CUDA call. */
+int ctn_softmax_train_workspace_bytes(const ctn_config_t* cfg, int batch, int T, size_t* bytes);
+int ctn_softmax_fwd_train(const ctn_config_t* cfg, const ctn_params_t* params, const float* x, int B, int T, float* out,
+                          void* train_ws, size_t train_ws_bytes, ctn_stream_t stream);
+int ctn_softmax_bwd(const ctn_config_t* cfg, const ctn_params_t* params, const ctn_grads_t* grads, const float* x,
+                    const float* d_out, float* d_x, int B, int T, void* train_ws, size_t train_ws_bytes, ctn_stream_t stream);
 
 /* Backward of ctn_sisdr_pit_fwd through the selected permutation (src/criterion/pit.py:36-44; sdr.py:135-137):
  * d_est (B,S,T) = grad_loss_b[b] * coef * dSI-SDR(est_i, tgt_perm[i])/d est_i.  fwd_scratch = the scratch buffer the

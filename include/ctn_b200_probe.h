@@ -105,6 +105,11 @@ int ctn_probe_dw_bwd(const float* dupre, const float* hpre, float* dhn, const fl
 /* sigmoid-mask backward: dwhat (B, S*N, pitch) -> d_mpre in place ; dwprod (B, N, pitch) = sum_s dwhat * mask */
 int ctn_probe_mask_bwd(float* dwhat, const float* w, const float* mask, float* dwprod, int B, int S, int N, int frames, int pitch,
                        ctn_stream_t stream);
+/* softmax-mask backward (softmax over all S*N channels of a frame): dwprod (B, N, pitch) = sum_s dwhat * mask ; dwhat -> d_z =
+ * mask * (dwhat * w - dot) in place, dot = sum_n w * dwprod per frame.  Pad lanes [frames, pitch) of both are written as 0.
+ * pitch % 32 == 0 (else CTN_EINVAL) */
+int ctn_probe_softmax_mask_bwd(float* dwhat, const float* w, const float* mask, float* dwprod, int B, int S, int N, int frames,
+                               int pitch, ctn_stream_t stream);
 int ctn_probe_prelu_apply(const float* x, float* y, const float* slope, int B, int C, int frames, int pitch, ctn_stream_t stream);
 /* dpre = dy * (pre > 0 ? 1 : slope) (may alias dy) ; dslope += sum_{pre <= 0} dy * pre */
 int ctn_probe_prelu_bwd(const float* dy, const float* pre, float* dpre, const float* slope, float* dslope, int B, int C, int frames,
