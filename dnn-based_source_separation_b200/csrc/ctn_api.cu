@@ -467,7 +467,7 @@ int ctn_envelope_view(const ctn_config_t* c, int B, int frames, int path, void* 
     v->x0_bound = m.head.vb; v->x0_n = c->bottleneck;  // run_separator points the TCN's x0_bound here
   } else if (path == ENV_TRAIN) {
     void* tm = nullptr;
-    ctn_train_tcn_region(c, B, pitch, mem, &tm, &v->x0_bound);
+    ctn_train_tcn_region(c, B, frames, mem, &tm, &v->x0_bound);
     if (!tm) return CTN_EUNSUPPORTED;
     Carver cv(tm);
     carve_tcn_train(cv, c, B, pitch, &t);

@@ -155,7 +155,7 @@ struct EnvelopeView { const float* scales; const float* dwp[CTN_MAX_BLOCKS]; con
 int ctn_envelope_view(const ctn_config_t* c, int B, int frames, int path, void* mem, EnvelopeView* v);
 // training workspace (ctn_train.cu): the region of the fused TCN forward (nullptr when the config does not fuse it) and the head's
 // row bounds
-void ctn_train_tcn_region(const ctn_config_t* c, int B, int pitch, void* mem, void** tcn_mem, const float** head_vb);
+void ctn_train_tcn_region(const ctn_config_t* c, int B, int frames, void* mem, void** tcn_mem, const float** head_vb);
 
 // training forward of the TCN through the fused inference kernels (ctn_api.cu); per-block buffers owned by the training workspace
 struct TcnTrainHooks { float* const* x_keep; float* const* hpre; float* const* upre; };

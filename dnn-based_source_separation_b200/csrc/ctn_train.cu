@@ -838,15 +838,22 @@ struct TrainWs {
   size_t stats_bytes;
   void* tcn_mem;            // fused_tcn(): state of the fused TCN forward (ctn_tcn_train_fwd)
   size_t tcn_bytes;
+  // ---- causal (cLN) configs only: cLN's statistics are per frame, so nothing of them fits a (B, 2) slot
+  double* st0 = nullptr;          // cLN0: [B][frames][2] scanned prefix sums (S_t, Q_t)
+  std::vector<double*> st1, st2;  // cLN1 / cLN2 of every block
+  std::vector<float2*> mi1;       // [B][frames] (mean, 1 / (std + eps)) of cLN1
+  double* part = nullptr;         // backward: partial frame sums
+  float4* tab = nullptr;          // backward: (m_t, r_t, U_t, V_t)
 };
 
 // fp16-piece mode with 3-tap depthwise convs: the TCN forward runs through the SAME fused kernels as inference (pw1 with the
 // residual update fused, depthwise producer feeding the [out;skip] contraction), which additionally leave x_i, W1 x + b1 and
 // the depthwise pre-activation behind for the backward -- 2 launches per block instead of 7, no u / gLN2(u) round trips.
-// With check_train_cfg (non-causal, dilations 2^l) every block of such a config is within the fused kernels' envelope.
-bool fused_tcn(const ctn_config_t* c) { return c->math == CTN_MATH_F16X3 && c->sep_kernel == 3; }
+// The fused kernels are gLN kernels; with check_train (dilations 2^l) every block of a non-causal config is within their envelope.
+bool fused_tcn(const ctn_config_t* c) { return !c->causal && c->math == CTN_MATH_F16X3 && c->sep_kernel == 3; }
 
-void carve_train(Carver& cv, const ctn_config_t* c, int B, int pitch, TrainWs* ws) {
+void carve_train(Carver& cv, const ctn_config_t* c, int B, int frames, TrainWs* ws) {
+  const int pitch = ctn_pitch(frames);
   const int RX = c->num_blocks * c->num_layers;
   const int N = c->n_basis, Bc = c->bottleneck, H = c->hidden, Sc = c->skip, S = c->n_sources;
   const size_t bp = (size_t)B * pitch;
@@ -898,42 +905,51 @@ void carve_train(Carver& cv, const ctn_config_t* c, int B, int pitch, TrainWs* w
   ws->nC = cv.take<float>(bp * N);
   ws->sp = cv.take<float>(bp * Sc);
   ws->dsp = cv.take<float>(bp * Sc);
+  if (!c->causal) return;
+  const size_t bf = (size_t)B * frames;
+  ws->st0 = cv.take<double>(bf * 2);
+  ws->st1.assign(RX, nullptr);
+  ws->st2.assign(RX, nullptr);
+  ws->mi1.assign(RX, nullptr);
+  for (int i = 0; i < RX; ++i) {
+    ws->st1[i] = cv.take<double>(bf * 2);
+    ws->st2[i] = cv.take<double>(bf * 2);
+    ws->mi1[i] = cv.take<float2>(bf);
+  }
+  ws->part = cv.take<double>(ctn_cln_bwd_part_doubles(B, frames));
+  ws->tab = cv.take<float4>(bf);
 }
 
-int check_train_cfg(const ctn_config_t* c) {
+// The four training steps: gLN with the sigmoid mask over one input channel (ctn_convtasnet_*) or C in [2, 64] of them
+// (ctn_multichannel_*; check_model_cfg bounds C at 64), gLN with the softmax mask over all S*N channels (ctn_softmax_*), and
+// cLN with the sigmoid mask (ctn_causal_*).  Everything else trains nowhere: forward only.
+enum TrainKind { TRAIN_NONE, TRAIN_GLN, TRAIN_MULTICHANNEL, TRAIN_SOFTMAX, TRAIN_CAUSAL };
+
+// check_model_cfg's status, else CTN_OK when the config trains through the step `want`, else CTN_EUNSUPPORTED
+int check_train(const ctn_config_t* c, TrainKind want) {
   CTN_TRY(check_model_cfg(c));
-  if (c->causal || c->mask_softmax || c->in_channels > 1 || c->sep_kernel > CTN_MAX_P) return CTN_EUNSUPPORTED;  // causal, softmax masks, multichannel: forward only
-  return CTN_OK;
+  TrainKind kind;
+  if (c->sep_kernel > CTN_MAX_P) kind = TRAIN_NONE;
+  else if (c->causal) kind = c->mask_softmax || c->in_channels > 1 ? TRAIN_NONE : TRAIN_CAUSAL;
+  else if (c->in_channels > 1) kind = c->mask_softmax ? TRAIN_NONE : TRAIN_MULTICHANNEL;
+  else kind = c->mask_softmax ? TRAIN_SOFTMAX : TRAIN_GLN;
+  return kind == want ? CTN_OK : CTN_EUNSUPPORTED;
 }
 
-// the ctn_multichannel_* entries: the same pipeline with in_channels = C in [2, 64] (check_model_cfg bounds C at 64)
-int check_mc_train_cfg(const ctn_config_t* c) {
-  CTN_TRY(check_model_cfg(c));
-  if (c->causal || c->mask_softmax || c->in_channels <= 1 || c->sep_kernel > CTN_MAX_P) return CTN_EUNSUPPORTED;
-  return CTN_OK;
-}
-
-// the ctn_softmax_* entries: the gLN pipeline with the softmax mask (mask_softmax = 1), monaural and non-causal
-int check_softmax_train_cfg(const ctn_config_t* c) {
-  CTN_TRY(check_model_cfg(c));
-  if (!c->mask_softmax || c->causal || c->in_channels > 1 || c->sep_kernel > CTN_MAX_P) return CTN_EUNSUPPORTED;
-  return CTN_OK;
-}
-
-// workspace of the gLN training step for a config already checked; no activation depends on the input channel count
+// workspace of the training step for a config already checked; no activation depends on the input channel count
 int train_ws_need(const ctn_config_t* cfg, int batch, int T, size_t* bytes) {
   if (batch <= 0 || !bytes) return CTN_EINVAL;
   const int frames = ctn_frames(T, cfg->kernel_size, cfg->stride, nullptr, nullptr);
   if (frames <= 0) return CTN_EINVAL;
   Carver cv(nullptr);
   TrainWs ws;
-  carve_train(cv, cfg, batch, ctn_pitch(frames), &ws);
+  carve_train(cv, cfg, batch, frames, &ws);
   *bytes = cv.off + 256;
   return CTN_OK;
 }
 
 // D (B, M, pitch) = W (M, K) . A (B, K, pitch), raw epilogue, in the configured numeric mode.  The operands here (gradients,
-// and the forward's materialised x_i / gLN2 output) carry no operand scale, so 'f16x3' runs these on the tf32 pieces: gradients
+// and the forward's materialised x_i / norm outputs) carry no operand scale, so 'f16x3' runs these on the tf32 pieces: gradients
 // have no fixed scale (1e-3 .. 1e-9 and below), which fp16 pieces cannot represent (subnormal below 6e-5, zero below 6e-8).
 int gemm_raw(const ctn_config_t* c, TrainWs& ws, const float* W, int M, int K, const float* A, float* D, int B, int frames,
              int pitch, cudaStream_t st) {
@@ -943,10 +959,25 @@ int gemm_raw(const ctn_config_t* c, TrainWs& ws, const float* W, int M, int K, c
   return ctn_pw(a, PRO_NONE, EPI_RAW, c->math, ws.wimg, st);
 }
 
+// wn = norm0(w) -> ws.nA (gLN0 or cLN0 over the saved statistics)
+int head_norm(const ctn_config_t* c, const ctn_params_t* p, TrainWs& ws, int B, int frames, int pitch, cudaStream_t st) {
+  const int N = c->n_basis;
+  if (c->causal) return ctn_cln_apply(ws.w, nullptr, p->norm0_g, p->norm0_b, ws.nA, B, N, frames, pitch, c->eps, ws.st0, st);
+  return ctn_act_norm(ws.w, ws.nA, nullptr, p->norm0_g, p->norm0_b, ws.stats0, (double)N * frames, c->eps, B, N, frames, pitch, st);
+}
+
+// un = norm2(PReLU(u_pre)) of block i -> ws.T1 (gLN2 or cLN2 over the saved statistics)
+int block_norm2(const ctn_config_t* c, const ctn_block_params_t& q, TrainWs& ws, int i, int B, int frames, int pitch, cudaStream_t st) {
+  const int H = c->hidden;
+  if (c->causal) return ctn_cln_apply(ws.upre[i], q.prelu2, q.norm2_g, q.norm2_b, ws.T1, B, H, frames, pitch, c->eps_tcn, ws.st2[i], st);
+  return ctn_act_norm(ws.upre[i], ws.T1, q.prelu2, q.norm2_g, q.norm2_b, ws.stats + (size_t)(2 * i + 1) * B * 2, (double)H * frames,
+                      c->eps_tcn, B, H, frames, pitch, st);
+}
+
 // Backward from d_out to the gradient of every block's skip output: decoder, sigmoid (or softmax) mask, mask conv, PReLU on the
 // skip sum.  Leaves dS, rows [Bc, Bc + Sc) of dcat (= dS) and nC = d_wprod.  The same for gLN and cLN models.
 int bwd_tail(const ctn_config_t* c, const ctn_params_t* p, const ctn_params_t* grads, TrainWs& ws, const float* d_out, int B, int T,
-             cudaStream_t st, int Cin = 1) {
+             cudaStream_t st, int Cin) {
   int pl = 0, pr = 0;
   const int frames = ctn_frames(T, c->kernel_size, c->stride, &pl, &pr);
   const int pitch = ctn_pitch(frames);
@@ -983,23 +1014,27 @@ int bwd_tail(const ctn_config_t* c, const ctn_params_t* p, const ctn_params_t* g
 
 }  // namespace
 
-void ctn_train_tcn_region(const ctn_config_t* c, int B, int pitch, void* mem, void** tcn_mem, const float** head_vb) {
+void ctn_train_tcn_region(const ctn_config_t* c, int B, int frames, void* mem, void** tcn_mem, const float** head_vb) {
   Carver cv(mem);
   TrainWs ws;
-  carve_train(cv, c, B, pitch, &ws);
+  carve_train(cv, c, B, frames, &ws);
   *tcn_mem = ws.tcn_mem;
   *head_vb = ws.head.vb;
 }
 
-extern "C" int ctn_train_workspace_bytes(const ctn_config_t* cfg, int batch, int T, size_t* bytes) {
-  CTN_TRY(check_train_cfg(cfg));
-  return train_ws_need(cfg, batch, T, bytes);
-}
-
 namespace {
 
-// The gLN training step over Cin input channels (x (B, Cin, T), out (B, S, Cin, T)); the config is checked by the caller.  Only the
+// The training step over Cin input channels (x (B, Cin, T), out (B, S, Cin, T)); the config is checked by the caller.  Only the
 // filter banks see Cin: the encoder, the decoder, the decoder's adjoint and the two filter-bank weight gradients.
+//
+// Causal (cLN) configs run the un-fused gLN step with cLN in place of gLN and all of the depthwise padding on the left, in the
+// operation order of the inference pipeline (ctn_causal.cu): the same estimate, so a model trained here streams through the
+// online pipeline unchanged.  For each norm the forward keeps the scanned prefix sums (S_t, Q_t) (16 bytes per frame and norm)
+// and, for the norm in front of each depthwise conv, the (mean_t, 1 / (std_t + eps)) table its kernels normalise with on load
+// (8 bytes).  The contractions carry no operand scale: the f16x3 mode runs them on tf32 pieces.
+// Causal launches, g = 1 (fp32) or 2 (tensor-core modes: weight image + contraction) per 1x1 contraction, R X blocks:
+//   forward   6 + 2 g + R X (9 + g)
+//   backward  19 + 2 g + (R X - 1) (14 + 2 g + q) + (14 + 2 g),  q = 2 (fp32: the two-part FFMA weight gradient) or 1
 int fwd_train(const ctn_config_t* c, const ctn_params_t* p, const float* x, int B, int T, float* out, void* train_ws,
               size_t train_ws_bytes, ctn_stream_t stream, int Cin) {
   if (!p || !p->blocks || !x || !out || !train_ws || B <= 0 || T <= 0) return CTN_EINVAL;
@@ -1013,20 +1048,29 @@ int fwd_train(const ctn_config_t* c, const ctn_params_t* p, const float* x, int 
   cudaStream_t st = (cudaStream_t)stream;
   Carver cv(train_ws);
   TrainWs ws;
-  carve_train(cv, c, B, pitch, &ws);
+  carve_train(cv, c, B, frames, &ws);
   const int N = c->n_basis, Bc = c->bottleneck, H = c->hidden, Sc = c->skip, S = c->n_sources, R = c->num_blocks, X = c->num_layers;
-  cudaError_t e = cudaMemsetAsync(ws.stats0, 0, sizeof(double) * 2 * B, st);
-  if (e != cudaSuccess) return (int)e;
-  e = cudaMemsetAsync(ws.stats, 0, ws.stats_bytes, st);
-  if (e != cudaSuccess) return (int)e;
-  // encoder + gLN0 statistics (filterbank.py:222-229)
-  if (Cin == 1) {
-    CTN_TRY(ctn_encoder_fwd(x, p->enc_w, ws.w, B, T, pl, pr, N, c->kernel_size, c->stride, c->enc_relu, pitch, ws.stats0, stream));
-  } else {
-    CTN_TRY(ctn_encoder_mc_fwd(x, p->enc_w, ws.w, B, Cin, T, pl, pr, N, c->kernel_size, c->stride, c->enc_relu, pitch, ws.stats0, stream));
+  const bool cln = c->causal;
+  if (!cln) {
+    cudaError_t e = cudaMemsetAsync(ws.stats0, 0, sizeof(double) * 2 * B, st);
+    if (e != cudaSuccess) return (int)e;
+    e = cudaMemsetAsync(ws.stats, 0, ws.stats_bytes, st);
+    if (e != cudaSuccess) return (int)e;
   }
-  // head: x_0 = Wb gLN0(w) + bb (conv_tasnet.py:370-371), gLN0 folded into the contraction like the inference path
-  {
+  // encoder (filterbank.py:222-229) + gLN0 statistics
+  double* enc_stats = cln ? nullptr : ws.stats0;
+  if (Cin == 1) {
+    CTN_TRY(ctn_encoder_fwd(x, p->enc_w, ws.w, B, T, pl, pr, N, c->kernel_size, c->stride, c->enc_relu, pitch, enc_stats, stream));
+  } else {
+    CTN_TRY(ctn_encoder_mc_fwd(x, p->enc_w, ws.w, B, Cin, T, pl, pr, N, c->kernel_size, c->stride, c->enc_relu, pitch, enc_stats, stream));
+  }
+  // head: x_0 = Wb norm0(w) + bb (conv_tasnet.py:333-335,370-371)
+  if (cln) {  // as ctn_causal_head
+    CTN_TRY(ctn_cln_stats(ws.w, nullptr, B, N, frames, pitch, c->eps, ws.st0, nullptr, st));
+    CTN_TRY(head_norm(c, p, ws, B, frames, pitch, st));
+    CTN_TRY(gemm_raw(c, ws, p->bn_w, Bc, N, ws.nA, ws.x[0], B, frames, pitch, st));
+    CTN_TRY(ctn_bias_rows_fwd(ws.x[0], p->bn_b, Bc, B, frames, pitch, st));
+  } else {  // gLN0 folded into the contraction like the inference path
     const FoldJob fj{p->bn_w, p->bn_b, p->norm0_g, p->norm0_b, ws.head, Bc, N, 0, sqrtf((float)N * (float)frames) * 1.0001f};
     CTN_TRY(ctn_fold_batch(&fj, 1, st));
     PwArgs a;
@@ -1052,22 +1096,34 @@ int fwd_train(const ctn_config_t* c, const ctn_params_t* p, const float* x, int 
     const int pad_left = ((c->sep_kernel - 1) * dil) / 2;
     double* st1 = ws.stats + (size_t)(2 * i) * B * 2;
     double* st2 = ws.stats + (size_t)(2 * i + 1) * B * 2;
-    // h_pre = W1 x + b1 ; stats1 of PReLU(h_pre)
+    // h_pre = W1 x + b1 ; gLN: stats1 of PReLU(h_pre)
     if (c->math == CTN_MATH_FP32) {
       CTN_TRY(gemm_raw(c, ws, q.bottleneck_w, H, Bc, ws.x[i], ws.hpre[i], B, frames, pitch, st));
-      CTN_TRY(ctn_bias_prelu_stats(ws.hpre[i], q.bottleneck_b, q.prelu1, st1, B, H, frames, pitch, st));
+      if (cln) {
+        CTN_TRY(ctn_bias_rows_fwd(ws.hpre[i], q.bottleneck_b, H, B, frames, pitch, st));
+      } else {
+        CTN_TRY(ctn_bias_prelu_stats(ws.hpre[i], q.bottleneck_b, q.prelu1, st1, B, H, frames, pitch, st));
+      }
     } else {  // bias, PReLU statistics fused into the contraction's epilogue; the PRE-activation is what gets stored
       PwArgs a;
       memset(&a, 0, sizeof(a));
       a.A = ws.x[i]; a.W = q.bottleneck_w; a.D = ws.hpre[i]; a.B = B; a.M = H; a.K = Bc; a.frames = frames; a.pitch = pitch;
-      a.bias = q.bottleneck_b; a.slope = q.prelu1; a.stats_out = st1; a.store_pre = 1;
+      a.bias = q.bottleneck_b; a.slope = q.prelu1; a.store_pre = 1;
+      a.stats_out = cln ? ws.sums : st1;  // cLN: the gLN statistics go to a sink nobody reads
       CTN_TRY(ctn_pw(a, PRO_NONE, EPI_H, c->math, ws.wimg, st));
     }
-    // u_pre = dwconv(gLN1(PReLU(h_pre))) + bd ; stats2 of PReLU(u_pre)
-    CTN_TRY(ctn_dw_train_fwd(ws.hpre[i], ws.upre[i], q.norm1_g, q.norm1_b, q.dw_w, q.dw_b, q.prelu1, q.prelu2, st1, st2, B, H, frames,
-                             pitch, c->sep_kernel, dil, pad_left, nH, c->eps_tcn, st));
-    // un = gLN2(PReLU(u_pre)) ; r = [Wo; Ws] un
-    CTN_TRY(ctn_act_norm(ws.upre[i], ws.T1, q.prelu2, q.norm2_g, q.norm2_b, st2, nH, c->eps_tcn, B, H, frames, pitch, st));
+    // u_pre = dwconv(norm1(PReLU(h_pre))) + bd ; un = norm2(PReLU(u_pre))
+    if (cln) {
+      CTN_TRY(ctn_cln_stats(ws.hpre[i], q.prelu1, B, H, frames, pitch, c->eps_tcn, ws.st1[i], ws.mi1[i], st));
+      CTN_TRY(ctn_cdw_train_fwd(ws.hpre[i], ws.upre[i], ws.mi1[i], q.norm1_g, q.norm1_b, q.dw_w, q.dw_b, q.prelu1, B, H, frames, pitch,
+                                c->sep_kernel, dil, st));
+      CTN_TRY(ctn_cln_stats(ws.upre[i], q.prelu2, B, H, frames, pitch, c->eps_tcn, ws.st2[i], nullptr, st));
+    } else {  // gLN: stats2 of PReLU(u_pre) accumulated by the depthwise conv
+      CTN_TRY(ctn_dw_train_fwd(ws.hpre[i], ws.upre[i], q.norm1_g, q.norm1_b, q.dw_w, q.dw_b, q.prelu1, q.prelu2, st1, st2, B, H, frames,
+                               pitch, c->sep_kernel, dil, pad_left, nH, c->eps_tcn, st));
+    }
+    CTN_TRY(block_norm2(c, q, ws, i, B, frames, pitch, st));
+    // r = [Wo; Ws] un
     const int Mt = has_out ? Bc + Sc : Sc;
     CTN_TRY(ctn_block_wcat(q, Bc, Sc, H, ws.Wcat, st));
     CTN_TRY(gemm_raw(c, ws, ws.Wcat, Mt, H, ws.T1, ws.r, B, frames, pitch, st));
@@ -1110,12 +1166,13 @@ int bwd(const ctn_config_t* c, const ctn_params_t* p, const ctn_params_t* grads,
   cudaStream_t st = (cudaStream_t)stream;
   Carver cv(train_ws);
   TrainWs ws;
-  carve_train(cv, c, B, pitch, &ws);
+  carve_train(cv, c, B, frames, &ws);
   const int N = c->n_basis, Bc = c->bottleneck, H = c->hidden, Sc = c->skip, RX = c->num_blocks * c->num_layers, X = c->num_layers,
             L = c->kernel_size;
   const size_t bsN = (size_t)N * pitch, bsH = (size_t)H * pitch, bsBc = (size_t)Bc * pitch, bsSc = (size_t)Sc * pitch,
                bsCat = (size_t)(Bc + Sc) * pitch;
   const double nH = (double)H * (double)frames;
+  const bool cln = c->causal;
   auto G = [](const float* q) { return const_cast<float*>(q); };
 
   CTN_TRY(bwd_tail(c, p, grads, ws, d_out, B, T, st, Cin));
@@ -1131,8 +1188,8 @@ int bwd(const ctn_config_t* c, const ctn_params_t* p, const ctn_params_t* grads,
     const int Mt = has_out ? Bc + Sc : Sc;
     const float* dY = has_out ? ws.dcat : ws.dS;  // (B, Mt, pitch)
     const size_t dY_bs = has_out ? bsCat : bsSc;
-    // un = gLN2(PReLU(u_pre)) recomputed for the weight gradients of the two heads
-    CTN_TRY(ctn_act_norm(ws.upre[i], ws.T1, q.prelu2, q.norm2_g, q.norm2_b, st2, nH, c->eps_tcn, B, H, frames, pitch, st));
+    // un = norm2(PReLU(u_pre)) recomputed for the weight gradients of the two heads
+    CTN_TRY(block_norm2(c, q, ws, i, B, frames, pitch, st));
     if (has_out) {
       CTN_TRY(ctn_wgrad(c->math, dY, dY_bs, ws.T1, bsH, G(gq.out_w), G(gq.skip_w), Bc, Bc + Sc, H, B, frames, pitch, st));
       CTN_TRY(ctn_rowsum(dY, dY_bs, Bc, B, frames, pitch, G(gq.out_b), st));
@@ -1145,36 +1202,47 @@ int bwd(const ctn_config_t* c, const ctn_params_t* p, const ctn_params_t* grads,
     CTN_TRY(ctn_block_wcat(q, Bc, Sc, H, ws.Wcat, st));
     CTN_TRY(ctn_transpose(ws.Wcat, ws.Wt, Mt, H, st));
     CTN_TRY(gemm_raw(c, ws, ws.Wt, H, Mt, dY, ws.G1, B, frames, pitch, st));
-    // gLN2 + PReLU2 backward -> d_u_pre (G1 in place); dgamma2, dbeta2, da2, d(bd)
-    CTN_TRY(ctn_gln_prelu_bwd(ws.G1, ws.upre[i], ws.G1, q.prelu2, q.norm2_g, st2, nH, c->eps_tcn, ws.sums, G(gq.norm2_g),
-                              G(gq.norm2_b), G(gq.prelu2), G(gq.dw_b), B, H, frames, pitch, st));
-    // depthwise conv backward -> d_hn (G2), d(wd); fused: phase 1 of the gLN1 backward (per-sample sums, dgamma1, dbeta1)
-    {
+    // norm2 + PReLU2 backward -> d_u_pre (G1 in place); dgamma2, dbeta2, da2, d(bd).  Depthwise conv backward -> d_hn (G2), d(wd).
+    // norm1 + PReLU1 backward -> d_h_pre (G2 in place); dgamma1, dbeta1, da1, db1
+    if (cln) {
+      CTN_TRY(ctn_cln_bwd_pitch(ws.G1, ws.upre[i], ws.G1, q.prelu2, q.norm2_g, ws.st2[i], c->eps_tcn, ws.part, ws.tab, G(gq.norm2_g),
+                                G(gq.norm2_b), G(gq.prelu2), G(gq.dw_b), B, H, frames, pitch, st));
+      CTN_TRY(ctn_cdw_bwd(ws.G1, ws.hpre[i], ws.G2, ws.mi1[i], q.norm1_g, q.norm1_b, q.prelu1, q.dw_w, G(gq.dw_w), B, H, frames, pitch,
+                          c->sep_kernel, dil, st));
+      CTN_TRY(ctn_cln_bwd_pitch(ws.G2, ws.hpre[i], ws.G2, q.prelu1, q.norm1_g, ws.st1[i], c->eps_tcn, ws.part, ws.tab, G(gq.norm1_g),
+                                G(gq.norm1_b), G(gq.prelu1), G(gq.bottleneck_b), B, H, frames, pitch, st));
+    } else {  // the depthwise backward also runs phase 1 of the gLN1 backward (per-sample sums, dgamma1, dbeta1)
+      CTN_TRY(ctn_gln_prelu_bwd(ws.G1, ws.upre[i], ws.G1, q.prelu2, q.norm2_g, st2, nH, c->eps_tcn, ws.sums, G(gq.norm2_g),
+                                G(gq.norm2_b), G(gq.prelu2), G(gq.dw_b), B, H, frames, pitch, st));
       cudaError_t e = cudaMemsetAsync(ws.sums, 0, sizeof(double) * 2 * B, st);
       if (e != cudaSuccess) return (int)e;
+      CTN_TRY(ctn_dw_bwd(ws.G1, ws.hpre[i], ws.G2, q.prelu1, q.norm1_g, q.norm1_b, st1, nH, c->eps_tcn, q.dw_w, G(gq.dw_w), ws.sums,
+                         G(gq.norm1_g), G(gq.norm1_b), B, H, frames, pitch, c->sep_kernel, dil, pad_left, st));
+      CTN_TRY(ctn_gln_prelu_bwd(ws.G2, ws.hpre[i], ws.G2, q.prelu1, q.norm1_g, st1, nH, c->eps_tcn, ws.sums, G(gq.norm1_g),
+                                G(gq.norm1_b), G(gq.prelu1), G(gq.bottleneck_b), B, H, frames, pitch, st, /*reduced=*/true));
     }
-    CTN_TRY(ctn_dw_bwd(ws.G1, ws.hpre[i], ws.G2, q.prelu1, q.norm1_g, q.norm1_b, st1, nH, c->eps_tcn, q.dw_w, G(gq.dw_w), ws.sums,
-                       G(gq.norm1_g), G(gq.norm1_b), B, H, frames, pitch, c->sep_kernel, dil, pad_left, st));
-    // gLN1 + PReLU1 backward, phase 2 -> d_h_pre (G2 in place); da1, db1
-    CTN_TRY(ctn_gln_prelu_bwd(ws.G2, ws.hpre[i], ws.G2, q.prelu1, q.norm1_g, st1, nH, c->eps_tcn, ws.sums, G(gq.norm1_g),
-                              G(gq.norm1_b), G(gq.prelu1), G(gq.bottleneck_b), B, H, frames, pitch, st, /*reduced=*/true));
     // bottleneck 1x1: dW1 = d_h_pre x_i^T ; d_x_i = W1^T d_h_pre (+ residual path)
     CTN_TRY(ctn_wgrad(c->math, ws.G2, bsH, ws.x[i], bsBc, G(gq.bottleneck_w), nullptr, 0, H, Bc, B, frames, pitch, st));
     CTN_TRY(ctn_transpose(q.bottleneck_w, ws.Wt, H, Bc, st));
     CTN_TRY(gemm_raw(c, ws, ws.Wt, Bc, H, ws.G2, ws.dxtmp, B, frames, pitch, st));
     CTN_TRY(ctn_rows(ws.dcat, bsCat, ws.dxtmp, bsBc, Bc, B, has_out ? 1 : 0, frames, pitch, st));
   }
-  // ---- head (conv_tasnet.py:333-335,370-371): x_0 = Wb gLN0(w) + bb.   d_x0 = dcat rows [0,Bc)
-  CTN_TRY(ctn_act_norm(ws.w, ws.nA, nullptr, p->norm0_g, p->norm0_b, ws.stats0, (double)N * frames, c->eps, B, N, frames, pitch, st));
+  // ---- head (conv_tasnet.py:333-335,370-371): x_0 = Wb norm0(w) + bb.   d_x0 = dcat rows [0,Bc)
+  CTN_TRY(head_norm(c, p, ws, B, frames, pitch, st));
   CTN_TRY(ctn_wgrad(c->math, ws.dcat, bsCat, ws.nA, bsN, G(grads->bn_w), nullptr, 0, Bc, N, B, frames, pitch, st));
   CTN_TRY(ctn_rowsum(ws.dcat, bsCat, Bc, B, frames, pitch, G(grads->bn_b), st));
   // d_wn = Wb^T d_x0 (the operand of the contraction must be dense (B, K, pitch): copy the rows out of dcat)
   CTN_TRY(ctn_rows(ws.dxtmp, bsBc, ws.dcat, bsCat, Bc, B, 0, frames, pitch, st));
   CTN_TRY(ctn_transpose(p->bn_w, ws.Wt, Bc, N, st));
   CTN_TRY(gemm_raw(c, ws, ws.Wt, N, Bc, ws.dxtmp, ws.nB, B, frames, pitch, st));
-  // gLN0 backward -> d_w (norm path) ; + product path ; ReLU mask of the encoder if any
-  CTN_TRY(ctn_gln_prelu_bwd(ws.nB, ws.w, ws.nB, nullptr, p->norm0_g, ws.stats0, (double)N * frames, c->eps, ws.sums,
-                            G(grads->norm0_g), G(grads->norm0_b), nullptr, nullptr, B, N, frames, pitch, st));
+  // norm0 backward -> d_w (norm path) ; + product path ; ReLU mask of the encoder if any
+  if (cln) {
+    CTN_TRY(ctn_cln_bwd_pitch(ws.nB, ws.w, ws.nB, nullptr, p->norm0_g, ws.st0, c->eps, ws.part, ws.tab, G(grads->norm0_g),
+                              G(grads->norm0_b), nullptr, nullptr, B, N, frames, pitch, st));
+  } else {
+    CTN_TRY(ctn_gln_prelu_bwd(ws.nB, ws.w, ws.nB, nullptr, p->norm0_g, ws.stats0, (double)N * frames, c->eps, ws.sums,
+                              G(grads->norm0_g), G(grads->norm0_b), nullptr, nullptr, B, N, frames, pitch, st));
+  }
   CTN_TRY(ctn_dw_combine(ws.nB, ws.nC, ws.w, c->enc_relu, B, N, frames, pitch, st));
   // ---- encoder (filterbank.py:212,222): dWe
   CTN_TRY(ctn_encdec_wgrad(ws.nB, x, G(grads->enc_w), B, N, Cin, frames, pitch, T, L, c->stride, pl, st));
@@ -1186,258 +1254,82 @@ int bwd(const ctn_config_t* c, const ctn_params_t* p, const ctn_params_t* grads,
 
 }  // namespace
 
+extern "C" int ctn_train_workspace_bytes(const ctn_config_t* cfg, int batch, int T, size_t* bytes) {
+  CTN_TRY(check_train(cfg, TRAIN_GLN));
+  return train_ws_need(cfg, batch, T, bytes);
+}
+
 extern "C" int ctn_convtasnet_fwd_train(const ctn_config_t* c, const ctn_params_t* p, const float* x, int B, int T, float* out,
                                         void* train_ws, size_t train_ws_bytes, ctn_stream_t stream) {
   LaunchScope scope(x);
-  CTN_TRY(check_train_cfg(c));
+  CTN_TRY(check_train(c, TRAIN_GLN));
   return fwd_train(c, p, x, B, T, out, train_ws, train_ws_bytes, stream, 1);
 }
 
 extern "C" int ctn_convtasnet_bwd(const ctn_config_t* c, const ctn_params_t* p, const ctn_params_t* grads, const float* x,
                                   const float* d_out, int B, int T, void* train_ws, size_t train_ws_bytes, ctn_stream_t stream) {
   LaunchScope scope(x);
-  CTN_TRY(check_train_cfg(c));
+  CTN_TRY(check_train(c, TRAIN_GLN));
   return bwd(c, p, grads, x, d_out, nullptr, B, T, train_ws, train_ws_bytes, stream, 1);
 }
 
 // Multichannel (in_channels = C > 1) models: the same step with the multichannel filter banks; x (B, C, T), out / d_out (B, S, C, T)
 extern "C" int ctn_multichannel_train_workspace_bytes(const ctn_config_t* cfg, int batch, int T, size_t* bytes) {
-  CTN_TRY(check_mc_train_cfg(cfg));
+  CTN_TRY(check_train(cfg, TRAIN_MULTICHANNEL));
   return train_ws_need(cfg, batch, T, bytes);
 }
 
 extern "C" int ctn_multichannel_fwd_train(const ctn_config_t* c, const ctn_params_t* p, const float* x, int B, int T, float* out,
                                           void* train_ws, size_t train_ws_bytes, ctn_stream_t stream) {
   LaunchScope scope(x);
-  CTN_TRY(check_mc_train_cfg(c));
+  CTN_TRY(check_train(c, TRAIN_MULTICHANNEL));
   return fwd_train(c, p, x, B, T, out, train_ws, train_ws_bytes, stream, c->in_channels);
 }
 
 extern "C" int ctn_multichannel_bwd(const ctn_config_t* c, const ctn_params_t* p, const ctn_params_t* grads, const float* x,
                                     const float* d_out, int B, int T, void* train_ws, size_t train_ws_bytes, ctn_stream_t stream) {
   LaunchScope scope(x);
-  CTN_TRY(check_mc_train_cfg(c));
+  CTN_TRY(check_train(c, TRAIN_MULTICHANNEL));
   return bwd(c, p, grads, x, d_out, nullptr, B, T, train_ws, train_ws_bytes, stream, c->in_channels);
 }
 
 // Softmax-mask models (mask_nonlinear='softmax', the ORPIT / Sinkhorn PIT recipes): the same step with the softmax over all S*N
 // mask channels; the workspace of the sigmoid step (ws.mask holds the softmax, d_z goes in place over d_what).  d_x may be null
 extern "C" int ctn_softmax_train_workspace_bytes(const ctn_config_t* cfg, int batch, int T, size_t* bytes) {
-  CTN_TRY(check_softmax_train_cfg(cfg));
+  CTN_TRY(check_train(cfg, TRAIN_SOFTMAX));
   return train_ws_need(cfg, batch, T, bytes);
 }
 
 extern "C" int ctn_softmax_fwd_train(const ctn_config_t* c, const ctn_params_t* p, const float* x, int B, int T, float* out,
                                      void* train_ws, size_t train_ws_bytes, ctn_stream_t stream) {
   LaunchScope scope(x);
-  CTN_TRY(check_softmax_train_cfg(c));
+  CTN_TRY(check_train(c, TRAIN_SOFTMAX));
   return fwd_train(c, p, x, B, T, out, train_ws, train_ws_bytes, stream, 1);
 }
 
 extern "C" int ctn_softmax_bwd(const ctn_config_t* c, const ctn_params_t* p, const ctn_params_t* grads, const float* x,
                                const float* d_out, float* d_x, int B, int T, void* train_ws, size_t train_ws_bytes, ctn_stream_t stream) {
   LaunchScope scope(x);
-  CTN_TRY(check_softmax_train_cfg(c));
+  CTN_TRY(check_train(c, TRAIN_SOFTMAX));
   return bwd(c, p, grads, x, d_out, d_x, B, T, train_ws, train_ws_bytes, stream, 1);
 }
 
-// ================================================================================================================
-// Causal (cLN) models.  Block for block the un-fused branch above with cLN in place of gLN and all of the depthwise padding on
-// the left, in the operation order of the inference pipeline (ctn_causal.cu): the same estimate, so a model trained here
-// streams through the online pipeline unchanged.  cLN's statistics are per frame, so nothing of them fits a (B, 2) slot: the
-// forward keeps the scanned prefix sums (S_t, Q_t) of all 1 + 2 R X norms (16 bytes per frame and norm) and, for the norm in
-// front of each depthwise conv, the (mean_t, 1 / (std_t + eps)) table its kernels normalise with on load (8 bytes).
-// The contractions carry no operand scale: the f16x3 mode runs them on tf32 pieces.
-// Launches, g = 1 (fp32) or 2 (tensor-core modes: weight image + contraction) per 1x1 contraction, R X blocks:
-//   forward   6 + 2 g + R X (9 + g)
-//   backward  19 + 2 g + (R X - 1) (14 + 2 g + q) + (14 + 2 g),  q = 2 (fp32: the two-part FFMA weight gradient) or 1
-// ================================================================================================================
-namespace {
-
-struct CausalTrainWs {
-  double* st0;                  // cLN0:   [B][frames][2]
-  std::vector<double*> st1, st2;  // cLN1 / cLN2 of every block
-  std::vector<float2*> mi1;     // [B][frames] (mean, 1 / (std + eps)) of cLN1
-  double* part;                 // backward: partial frame sums
-  float4* tab;                  // backward: (m_t, r_t, U_t, V_t)
-};
-
-void carve_causal_train(Carver& cv, const ctn_config_t* c, int B, int frames, int pitch, TrainWs* ws, CausalTrainWs* cw) {
-  carve_train(cv, c, B, pitch, ws);
-  const int RX = c->num_blocks * c->num_layers;
-  const size_t bf = (size_t)B * frames;
-  cw->st0 = cv.take<double>(bf * 2);
-  cw->st1.assign(RX, nullptr);
-  cw->st2.assign(RX, nullptr);
-  cw->mi1.assign(RX, nullptr);
-  for (int i = 0; i < RX; ++i) {
-    cw->st1[i] = cv.take<double>(bf * 2);
-    cw->st2[i] = cv.take<double>(bf * 2);
-    cw->mi1[i] = cv.take<float2>(bf);
-  }
-  cw->part = cv.take<double>(ctn_cln_bwd_part_doubles(B, frames));
-  cw->tab = cv.take<float4>(bf);
-}
-
-int check_causal_train_cfg(const ctn_config_t* c) {
-  CTN_TRY(check_model_cfg(c));
-  if (!c->causal || c->mask_softmax || c->in_channels > 1 || c->sep_kernel > CTN_MAX_P) return CTN_EUNSUPPORTED;
-  return CTN_OK;
-}
-
-int check_causal_train_call(const ctn_config_t* c, int B, int T, const void* train_ws, size_t train_ws_bytes) {
-  if (((uintptr_t)train_ws) & 255) return CTN_EALIGN;
-  size_t need = 0;
-  CTN_TRY(ctn_causal_train_workspace_bytes(c, B, T, &need));
-  return train_ws_bytes < need ? CTN_EWORKSPACE : CTN_OK;
-}
-
-}  // namespace
-
+// Causal (cLN) models: the same step with cLN in place of gLN (see fwd_train)
 extern "C" int ctn_causal_train_workspace_bytes(const ctn_config_t* cfg, int batch, int T, size_t* bytes) {
-  CTN_TRY(check_causal_train_cfg(cfg));
-  if (batch <= 0 || !bytes) return CTN_EINVAL;
-  const int frames = ctn_frames(T, cfg->kernel_size, cfg->stride, nullptr, nullptr);
-  if (frames <= 0) return CTN_EINVAL;
-  Carver cv(nullptr);
-  TrainWs ws;
-  CausalTrainWs cw;
-  carve_causal_train(cv, cfg, batch, frames, ctn_pitch(frames), &ws, &cw);
-  *bytes = cv.off + 256;
-  return CTN_OK;
+  CTN_TRY(check_train(cfg, TRAIN_CAUSAL));
+  return train_ws_need(cfg, batch, T, bytes);
 }
 
 extern "C" int ctn_causal_fwd_train(const ctn_config_t* c, const ctn_params_t* p, const float* x, int B, int T, float* out,
                                     void* train_ws, size_t train_ws_bytes, ctn_stream_t stream) {
   LaunchScope scope(x);
-  CTN_TRY(check_causal_train_cfg(c));
-  if (!p || !p->blocks || !x || !out || !train_ws || B <= 0 || T <= 0) return CTN_EINVAL;
-  CTN_TRY(check_causal_train_call(c, B, T, train_ws, train_ws_bytes));
-  int pl = 0, pr = 0;
-  const int frames = ctn_frames(T, c->kernel_size, c->stride, &pl, &pr);
-  const int pitch = ctn_pitch(frames);
-  cudaStream_t st = (cudaStream_t)stream;
-  Carver cv(train_ws);
-  TrainWs ws;
-  CausalTrainWs cw;
-  carve_causal_train(cv, c, B, frames, pitch, &ws, &cw);
-  const int N = c->n_basis, Bc = c->bottleneck, H = c->hidden, Sc = c->skip, S = c->n_sources, RX = c->num_blocks * c->num_layers,
-            X = c->num_layers, P = c->sep_kernel;
-  CTN_TRY(ctn_encoder_fwd(x, p->enc_w, ws.w, B, T, pl, pr, N, c->kernel_size, c->stride, c->enc_relu, pitch, nullptr, stream));
-  // head: x_0 = Wb cLN0(w) + bb (conv_tasnet.py:333-335,370-371), as ctn_causal_head
-  CTN_TRY(ctn_cln_stats(ws.w, nullptr, B, N, frames, pitch, c->eps, cw.st0, nullptr, st));
-  CTN_TRY(ctn_cln_apply(ws.w, nullptr, p->norm0_g, p->norm0_b, ws.nA, B, N, frames, pitch, c->eps, cw.st0, st));
-  CTN_TRY(gemm_raw(c, ws, p->bn_w, Bc, N, ws.nA, ws.x[0], B, frames, pitch, st));
-  CTN_TRY(ctn_bias_rows_fwd(ws.x[0], p->bn_b, Bc, B, frames, pitch, st));
-  for (int i = 0; i < RX; ++i) {
-    const ctn_block_params_t& q = p->blocks[i];
-    const bool has_out = q.out_w != nullptr;
-    if (!has_out && i != RX - 1) return CTN_EINVAL;
-    const int dil = 1 << (i % X);
-    // h_pre = W1 x + b1
-    if (c->math == CTN_MATH_FP32) {
-      CTN_TRY(gemm_raw(c, ws, q.bottleneck_w, H, Bc, ws.x[i], ws.hpre[i], B, frames, pitch, st));
-      CTN_TRY(ctn_bias_rows_fwd(ws.hpre[i], q.bottleneck_b, H, B, frames, pitch, st));
-    } else {  // bias in the contraction's epilogue, the PRE-activation stored; its gLN statistics go to a sink nobody reads
-      PwArgs a;
-      memset(&a, 0, sizeof(a));
-      a.A = ws.x[i]; a.W = q.bottleneck_w; a.D = ws.hpre[i]; a.B = B; a.M = H; a.K = Bc; a.frames = frames; a.pitch = pitch;
-      a.bias = q.bottleneck_b; a.slope = q.prelu1; a.stats_out = ws.sums; a.store_pre = 1;
-      CTN_TRY(ctn_pw(a, PRO_NONE, EPI_H, c->math, ws.wimg, st));
-    }
-    // cLN1 statistics of PReLU(h_pre) ; u_pre = dwconv(cLN1(PReLU(h_pre))) + bd ; un = cLN2(PReLU(u_pre)) ; r = [Wo; Ws] un
-    CTN_TRY(ctn_cln_stats(ws.hpre[i], q.prelu1, B, H, frames, pitch, c->eps_tcn, cw.st1[i], cw.mi1[i], st));
-    CTN_TRY(ctn_cdw_train_fwd(ws.hpre[i], ws.upre[i], cw.mi1[i], q.norm1_g, q.norm1_b, q.dw_w, q.dw_b, q.prelu1, B, H, frames, pitch, P,
-                              dil, st));
-    CTN_TRY(ctn_cln_stats(ws.upre[i], q.prelu2, B, H, frames, pitch, c->eps_tcn, cw.st2[i], nullptr, st));
-    CTN_TRY(ctn_cln_apply(ws.upre[i], q.prelu2, q.norm2_g, q.norm2_b, ws.T1, B, H, frames, pitch, c->eps_tcn, cw.st2[i], st));
-    const int Mt = has_out ? Bc + Sc : Sc;
-    CTN_TRY(ctn_block_wcat(q, Bc, Sc, H, ws.Wcat, st));
-    CTN_TRY(gemm_raw(c, ws, ws.Wcat, Mt, H, ws.T1, ws.r, B, frames, pitch, st));
-    CTN_TRY(ctn_res_skip_fwd(ws.r, Mt, ws.x[i], has_out ? ws.x[i + 1] : nullptr, ws.skip, q.out_b, q.skip_b, Bc, Sc, has_out ? 1 : 0,
-                             i == 0 ? 1 : 0, B, frames, pitch, st));
-  }
-  // tail: PReLU -> mask 1x1 -> sigmoid -> * w (conv_tasnet.py:373-376, 158-160); keeps the mask
-  {
-    PwArgs a;
-    memset(&a, 0, sizeof(a));
-    a.A = ws.skip; a.W = p->mask_w; a.D = ws.what; a.B = B; a.M = S * N; a.K = Sc; a.frames = frames; a.pitch = pitch;
-    a.pro_slope = p->prelu_out; a.bias = p->mask_b; a.wenc = ws.w; a.Nb = N; a.mask_out = ws.mask;
-    CTN_TRY(ctn_pw(a, PRO_PRELU, EPI_MASK, c->math, ws.wimg, st));
-  }
-  return ctn_decoder_fwd(ws.what, p->dec_w, out, B * S, N, frames, pitch, c->kernel_size, c->stride, pl, T, stream);
+  CTN_TRY(check_train(c, TRAIN_CAUSAL));
+  return fwd_train(c, p, x, B, T, out, train_ws, train_ws_bytes, stream, 1);
 }
 
-// grads: same layout as params; every tensor must be ZERO on entry (the kernels accumulate with atomics)
 extern "C" int ctn_causal_bwd(const ctn_config_t* c, const ctn_params_t* p, const ctn_params_t* grads, const float* x, const float* d_out,
                               int B, int T, void* train_ws, size_t train_ws_bytes, ctn_stream_t stream) {
   LaunchScope scope(x);
-  CTN_TRY(check_causal_train_cfg(c));
-  if (!p || !p->blocks || !grads || !grads->blocks || !x || !d_out || !train_ws || B <= 0 || T <= 0) return CTN_EINVAL;
-  CTN_TRY(check_causal_train_call(c, B, T, train_ws, train_ws_bytes));
-  int pl = 0, pr = 0;
-  const int frames = ctn_frames(T, c->kernel_size, c->stride, &pl, &pr);
-  const int pitch = ctn_pitch(frames);
-  cudaStream_t st = (cudaStream_t)stream;
-  Carver cv(train_ws);
-  TrainWs ws;
-  CausalTrainWs cw;
-  carve_causal_train(cv, c, B, frames, pitch, &ws, &cw);
-  const int N = c->n_basis, Bc = c->bottleneck, H = c->hidden, Sc = c->skip, RX = c->num_blocks * c->num_layers, X = c->num_layers,
-            P = c->sep_kernel;
-  const size_t bsN = (size_t)N * pitch, bsH = (size_t)H * pitch, bsBc = (size_t)Bc * pitch, bsSc = (size_t)Sc * pitch,
-               bsCat = (size_t)(Bc + Sc) * pitch;
-  const float eps = c->eps_tcn;
-  auto G = [](const float* q) { return const_cast<float*>(q); };
-  CTN_TRY(bwd_tail(c, p, grads, ws, d_out, B, T, st));
-  // ---- residual blocks, last to first
-  for (int i = RX - 1; i >= 0; --i) {
-    const ctn_block_params_t& q = p->blocks[i];
-    const ctn_block_params_t& gq = grads->blocks[i];
-    const bool has_out = q.out_w != nullptr;
-    const int dil = 1 << (i % X);
-    const int Mt = has_out ? Bc + Sc : Sc;
-    const float* dY = has_out ? ws.dcat : ws.dS;  // (B, Mt, pitch)
-    const size_t dY_bs = has_out ? bsCat : bsSc;
-    // un = cLN2(PReLU(u_pre)) recomputed for the weight gradients of the two heads
-    CTN_TRY(ctn_cln_apply(ws.upre[i], q.prelu2, q.norm2_g, q.norm2_b, ws.T1, B, H, frames, pitch, eps, cw.st2[i], st));
-    if (has_out) {
-      CTN_TRY(ctn_wgrad(c->math, dY, dY_bs, ws.T1, bsH, G(gq.out_w), G(gq.skip_w), Bc, Bc + Sc, H, B, frames, pitch, st));
-      CTN_TRY(ctn_rowsum(dY, dY_bs, Bc, B, frames, pitch, G(gq.out_b), st));
-    } else {
-      CTN_TRY(ctn_wgrad(c->math, dY, dY_bs, ws.T1, bsH, G(gq.skip_w), nullptr, 0, Sc, H, B, frames, pitch, st));
-    }
-    CTN_TRY(ctn_rowsum(dY + (has_out ? bsBc : 0), dY_bs, Sc, B, frames, pitch, G(gq.skip_b), st));
-    // d_un = [Wo; Ws]^T dY
-    CTN_TRY(ctn_block_wcat(q, Bc, Sc, H, ws.Wcat, st));
-    CTN_TRY(ctn_transpose(ws.Wcat, ws.Wt, Mt, H, st));
-    CTN_TRY(gemm_raw(c, ws, ws.Wt, H, Mt, dY, ws.G1, B, frames, pitch, st));
-    // cLN2 + PReLU2 backward -> d_u_pre (G1 in place); dgamma2, dbeta2, da2, d(bd)
-    CTN_TRY(ctn_cln_bwd_pitch(ws.G1, ws.upre[i], ws.G1, q.prelu2, q.norm2_g, cw.st2[i], eps, cw.part, cw.tab, G(gq.norm2_g), G(gq.norm2_b),
-                              G(gq.prelu2), G(gq.dw_b), B, H, frames, pitch, st));
-    // causal depthwise conv backward -> d_hn (G2), d(wd)
-    CTN_TRY(ctn_cdw_bwd(ws.G1, ws.hpre[i], ws.G2, cw.mi1[i], q.norm1_g, q.norm1_b, q.prelu1, q.dw_w, G(gq.dw_w), B, H, frames, pitch, P,
-                        dil, st));
-    // cLN1 + PReLU1 backward -> d_h_pre (G2 in place); dgamma1, dbeta1, da1, db1
-    CTN_TRY(ctn_cln_bwd_pitch(ws.G2, ws.hpre[i], ws.G2, q.prelu1, q.norm1_g, cw.st1[i], eps, cw.part, cw.tab, G(gq.norm1_g), G(gq.norm1_b),
-                              G(gq.prelu1), G(gq.bottleneck_b), B, H, frames, pitch, st));
-    // bottleneck 1x1: dW1 = d_h_pre x_i^T ; d_x_i = W1^T d_h_pre (+ residual path)
-    CTN_TRY(ctn_wgrad(c->math, ws.G2, bsH, ws.x[i], bsBc, G(gq.bottleneck_w), nullptr, 0, H, Bc, B, frames, pitch, st));
-    CTN_TRY(ctn_transpose(q.bottleneck_w, ws.Wt, H, Bc, st));
-    CTN_TRY(gemm_raw(c, ws, ws.Wt, Bc, H, ws.G2, ws.dxtmp, B, frames, pitch, st));
-    CTN_TRY(ctn_rows(ws.dcat, bsCat, ws.dxtmp, bsBc, Bc, B, has_out ? 1 : 0, frames, pitch, st));
-  }
-  // ---- head: x_0 = Wb cLN0(w) + bb.   d_x0 = dcat rows [0,Bc)
-  CTN_TRY(ctn_cln_apply(ws.w, nullptr, p->norm0_g, p->norm0_b, ws.nA, B, N, frames, pitch, c->eps, cw.st0, st));
-  CTN_TRY(ctn_wgrad(c->math, ws.dcat, bsCat, ws.nA, bsN, G(grads->bn_w), nullptr, 0, Bc, N, B, frames, pitch, st));
-  CTN_TRY(ctn_rowsum(ws.dcat, bsCat, Bc, B, frames, pitch, G(grads->bn_b), st));
-  CTN_TRY(ctn_rows(ws.dxtmp, bsBc, ws.dcat, bsCat, Bc, B, 0, frames, pitch, st));
-  CTN_TRY(ctn_transpose(p->bn_w, ws.Wt, Bc, N, st));
-  CTN_TRY(gemm_raw(c, ws, ws.Wt, N, Bc, ws.dxtmp, ws.nB, B, frames, pitch, st));
-  // cLN0 backward -> d_w (norm path) ; + product path ; ReLU mask of the encoder if any
-  CTN_TRY(ctn_cln_bwd_pitch(ws.nB, ws.w, ws.nB, nullptr, p->norm0_g, cw.st0, c->eps, cw.part, cw.tab, G(grads->norm0_g), G(grads->norm0_b),
-                            nullptr, nullptr, B, N, frames, pitch, st));
-  CTN_TRY(ctn_dw_combine(ws.nB, ws.nC, ws.w, c->enc_relu, B, N, frames, pitch, st));
-  // ---- encoder (filterbank.py:212,222): dWe
-  return ctn_encdec_wgrad(ws.nB, x, G(grads->enc_w), B, N, 1, frames, pitch, T, c->kernel_size, c->stride, pl, st);
+  CTN_TRY(check_train(c, TRAIN_CAUSAL));
+  return bwd(c, p, grads, x, d_out, nullptr, B, T, train_ws, train_ws_bytes, stream, 1);
 }

@@ -8,7 +8,7 @@ model is ONE autograd node: the forward keeps the per-block activations in a dev
 backward is one C call that fills the gradients of all parameter tensors.  Gradients come back as views of one flat
 zero-initialised buffer (the natural bucket for the data-parallel all-reduce, see ctn_b200/dist.py).
 
-Only the softmax node takes a mixture that requires grad, and returns its gradient: the ORPIT fine-tune step feeds an estimate
+Only the softmax step takes a mixture that requires grad, and returns its gradient: the ORPIT fine-tune step feeds an estimate
 back in as the next stage's mixture (egs/wsj0-mix/orpit_conv-tasnet/src/adhoc_driver.py, FinetuneTrainer.run_one_epoch_train)
 and calls backward once over all stages.  So that clip + Adam still see one flat bucket, the softmax nodes of one backward pass
 share it: the first to run owns the bucket, each later one adds its gradients into it in place."""
@@ -27,7 +27,7 @@ def param_list(model):
 
 
 class _Entry:
-    """the three C entry points of a training node, by name in _native"""
+    """the three C entry points of a training step, by name in _native"""
 
     def __init__(self, workspace_bytes, fwd, bwd, multichannel=False, mixture_grad=False):
         self.WORKSPACE_BYTES, self.FWD, self.BWD = workspace_bytes, fwd, bwd
@@ -35,40 +35,73 @@ class _Entry:
         self.mixture_grad = mixture_grad  # BWD takes a nullable d_x after d_out, and the nodes of one backward pass share a bucket
 
 
-class _Node:
-    """Body of the training nodes; cls: the _Entry the node runs."""
+GLN = _Entry("ctn_train_workspace_bytes", "ctn_convtasnet_fwd_train", "ctn_convtasnet_bwd")
+CAUSAL = _Entry("ctn_causal_train_workspace_bytes", "ctn_causal_fwd_train", "ctn_causal_bwd")
+MULTICHANNEL = _Entry("ctn_multichannel_train_workspace_bytes", "ctn_multichannel_fwd_train", "ctn_multichannel_bwd", multichannel=True)
+SOFTMAX = _Entry("ctn_softmax_train_workspace_bytes", "ctn_softmax_fwd_train", "ctn_softmax_bwd", mixture_grad=True)
+
+
+def train_entry(model):
+    """The training step a ConvTasNet runs under autograd, or NotImplementedError for a model that trains nowhere.  A softmax model
+    without softmax_training takes the sigmoid step, and a causal softmax model with causal_training the causal step: their C
+    entries refuse the mask."""
+    if model.in_channels > 1:
+        if not model.multichannel_training:
+            raise NotImplementedError("multichannel models (in_channels > 1) train natively only with model.multichannel_training = True "
+                                      "(ctn_multichannel_fwd_train / ctn_multichannel_bwd); without it they are forward only: call "
+                                      "under torch.no_grad()")
+        if model.causal or model.separator.mask_softmax:
+            raise NotImplementedError("multichannel training is built for non-causal models with a sigmoid mask; causal or softmax "
+                                      "multichannel models are forward only: call under torch.no_grad()")
+        return MULTICHANNEL
+    if model.separator.mask_softmax and model.softmax_training:
+        if model.causal:
+            raise NotImplementedError("softmax-mask training is built for non-causal monaural models (ctn_softmax_fwd_train / "
+                                      "ctn_softmax_bwd); causal or multichannel softmax models are forward only: call under "
+                                      "torch.no_grad()")
+        return SOFTMAX
+    if model.causal:
+        if not model.causal_training:
+            raise NotImplementedError("causal (cLN) models train natively only with model.causal_training = True (ctn_causal_fwd_train / "
+                                      "ctn_causal_bwd); without it they are forward only: call under torch.no_grad()")
+        return CAUSAL
+    return GLN
+
+
+class TrainFn(torch.autograd.Function):
+    """The whole model as one autograd node over the training step `entry` (an _Entry)."""
 
     @staticmethod
-    def forward(cls, ctx, model, x, *tensors):
+    def forward(ctx, entry, model, x, *tensors):
         dev = N.require_cuda(x)
         B, Cin, T = x.shape
         slots = [s for s, _ in param_list(model)]
         cfg = model.native_config()
         params, keep = N.build_params(zip(slots, tensors), dev)
         need = C.c_size_t(0)
-        N.check(getattr(N, cls.WORKSPACE_BYTES)(C.byref(cfg), B, T, C.byref(need)), cls.WORKSPACE_BYTES)
+        N.check(getattr(N, entry.WORKSPACE_BYTES)(C.byref(cfg), B, T, C.byref(need)), entry.WORKSPACE_BYTES)
         ws = torch.empty(need.value + 256, dtype=torch.uint8, device=dev)  # owned by this node until backward
-        shape = (B, model.n_sources, Cin, T) if cls.multichannel else (B, model.n_sources, T)
+        shape = (B, model.n_sources, Cin, T) if entry.multichannel else (B, model.n_sources, T)
         out = torch.empty(shape, dtype=torch.float32, device=dev)
-        N.check(getattr(N, cls.FWD)(C.byref(cfg), C.byref(params), x.data_ptr(), B, T, out.data_ptr(), *N.aligned(ws),
-                                    N.stream_ptr(dev)), cls.FWD)
+        N.check(getattr(N, entry.FWD)(C.byref(cfg), C.byref(params), x.data_ptr(), B, T, out.data_ptr(), *N.aligned(ws),
+                                      N.stream_ptr(dev)), entry.FWD)
         model.last_launches = N.ctn_last_launch_count()
         # x and the parameters go through save_for_backward: an in-place update between forward and backward is detected by autograd
         # (version counters) instead of silently changing the weights the backward kernels see
         ctx.save_for_backward(x, *[t for t in tensors if t is not None])
         ctx.present = [t is not None for t in tensors]
-        ctx.cfg, ctx.ws, ctx.slots, ctx.model = cfg, ws, slots, model
+        ctx.entry, ctx.cfg, ctx.ws, ctx.slots, ctx.model = entry, cfg, ws, slots, model
         return out
 
     @staticmethod
-    def backward(cls, ctx, d_out):
+    def backward(ctx, d_out):
         if ctx.ws is None:
             raise RuntimeError("training node: backward was already run on this graph; the saved activations are released after the "
                                "first backward (retain_graph is not supported by the native training path)")
         saved = list(ctx.saved_tensors)
         x, it = saved[0], iter(saved[1:])
         tensors = tuple(next(it) if pres else None for pres in ctx.present)
-        ws, cfg = ctx.ws, ctx.cfg
+        entry, ws, cfg = ctx.entry, ctx.ws, ctx.cfg
         dev = x.device
         B, _, T = x.shape
         d_out = d_out.contiguous()
@@ -83,16 +116,16 @@ class _Node:
         gviews = [None if t is None else flat[o:o + t.numel()].view(t.shape) for t, o in zip(tensors, offs)]
         grads, keep2 = N.build_params(zip(ctx.slots, gviews), dev)
         d_x = None
-        if cls.mixture_grad:
-            d_x = torch.empty_like(x) if ctx.needs_input_grad[1] else None  # null: no gradient, no launch
-            N.check(getattr(N, cls.BWD)(C.byref(cfg), C.byref(params), C.byref(grads), x.data_ptr(), d_out.data_ptr(), N.ptr(d_x), B,
-                                        T, *N.aligned(ws), N.stream_ptr(dev)), cls.BWD)
+        if entry.mixture_grad:
+            d_x = torch.empty_like(x) if ctx.needs_input_grad[2] else None  # null: no gradient, no launch
+            N.check(getattr(N, entry.BWD)(C.byref(cfg), C.byref(params), C.byref(grads), x.data_ptr(), d_out.data_ptr(), N.ptr(d_x), B,
+                                          T, *N.aligned(ws), N.stream_ptr(dev)), entry.BWD)
         else:
-            N.check(getattr(N, cls.BWD)(C.byref(cfg), C.byref(params), C.byref(grads), x.data_ptr(), d_out.data_ptr(), B, T,
-                                        *N.aligned(ws), N.stream_ptr(dev)), cls.BWD)
+            N.check(getattr(N, entry.BWD)(C.byref(cfg), C.byref(params), C.byref(grads), x.data_ptr(), d_out.data_ptr(), B, T,
+                                          *N.aligned(ws), N.stream_ptr(dev)), entry.BWD)
         ctx.model.last_bwd_launches = N.ctn_last_launch_count()
         ctx.ws = None
-        if cls.mixture_grad:
+        if entry.mixture_grad:
             # a node that ran earlier in this backward pass (a later fine-tune stage) owns the bucket: its views are what autograd
             # accumulates into the parameters' .grad, so add into them and pass nothing for the parameters
             task = torch._C._current_graph_task_id()
@@ -100,72 +133,14 @@ class _Node:
             prev = getattr(ctx.model, "last_flat_grad", None)
             if task >= 0 and owner == (task, total) and prev is not None and prev.device == flat.device:
                 prev.add_(flat)
-                return (None, d_x) + (None,) * len(tensors)
+                return (None, None, d_x) + (None,) * len(tensors)
             ctx.model._flat_grad_task = (task, total)
         ctx.model.last_flat_grad = flat
-        return (None, d_x) + tuple(g if (t is not None and t.requires_grad) else None for g, t in zip(gviews, tensors))
+        return (None, None, d_x) + tuple(g if (t is not None and t.requires_grad) else None for g, t in zip(gviews, tensors))
 
 
-class ConvTasNetTrainFn(torch.autograd.Function):
-    ENTRY = _Entry("ctn_train_workspace_bytes", "ctn_convtasnet_fwd_train", "ctn_convtasnet_bwd")
-
-    @staticmethod
-    def forward(ctx, model, x, *tensors):
-        return _Node.forward(ConvTasNetTrainFn.ENTRY, ctx, model, x, *tensors)
-
-    @staticmethod
-    def backward(ctx, d_out):
-        return _Node.backward(ConvTasNetTrainFn.ENTRY, ctx, d_out)
-
-
-class CausalTrainFn(torch.autograd.Function):
-    """The same node over the causal (cLN) pipeline."""
-    ENTRY = _Entry("ctn_causal_train_workspace_bytes", "ctn_causal_fwd_train", "ctn_causal_bwd")
-
-    @staticmethod
-    def forward(ctx, model, x, *tensors):
-        return _Node.forward(CausalTrainFn.ENTRY, ctx, model, x, *tensors)
-
-    @staticmethod
-    def backward(ctx, d_out):
-        return _Node.backward(CausalTrainFn.ENTRY, ctx, d_out)
-
-
-class MultichannelTrainFn(torch.autograd.Function):
-    """The same node over the multichannel pipeline: x (B, C, T) -> (B, S, C, T)."""
-    ENTRY = _Entry("ctn_multichannel_train_workspace_bytes", "ctn_multichannel_fwd_train", "ctn_multichannel_bwd", multichannel=True)
-
-    @staticmethod
-    def forward(ctx, model, x, *tensors):
-        return _Node.forward(MultichannelTrainFn.ENTRY, ctx, model, x, *tensors)
-
-    @staticmethod
-    def backward(ctx, d_out):
-        return _Node.backward(MultichannelTrainFn.ENTRY, ctx, d_out)
-
-
-class SoftmaxTrainFn(torch.autograd.Function):
-    """The same node over the softmax-mask step; the only node that returns the gradient w.r.t. the mixture."""
-    ENTRY = _Entry("ctn_softmax_train_workspace_bytes", "ctn_softmax_fwd_train", "ctn_softmax_bwd", mixture_grad=True)
-
-    @staticmethod
-    def forward(ctx, model, x, *tensors):
-        return _Node.forward(SoftmaxTrainFn.ENTRY, ctx, model, x, *tensors)
-
-    @staticmethod
-    def backward(ctx, d_out):
-        return _Node.backward(SoftmaxTrainFn.ENTRY, ctx, d_out)
-
-
-def run_train(model, x):
-    softmax = model.softmax_training and model.separator.mask_softmax and not model.causal and model.in_channels <= 1
-    if x.requires_grad and not softmax:
+def run_train(model, x, entry):
+    """model(x) as one autograd node over the training step `entry` (train_entry(model)); x (B, Cin, T) on the device."""
+    if x.requires_grad and not entry.mixture_grad:
         raise NotImplementedError("gradient w.r.t. the mixture is not built (the native backward stops at the encoder weights)")
-    tensors = [t for _, t in param_list(model)]
-    if model.in_channels > 1:
-        fn = MultichannelTrainFn
-    elif softmax:
-        fn = SoftmaxTrainFn
-    else:
-        fn = CausalTrainFn if model.causal else ConvTasNetTrainFn
-    return fn.apply(model, x, *tensors)
+    return TrainFn.apply(entry, model, x, *[t for _, t in param_list(model)])

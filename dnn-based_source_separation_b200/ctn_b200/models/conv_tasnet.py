@@ -427,29 +427,16 @@ class ConvTasNet(nn.Module):
         else:
             raise ValueError("Not support {} dimension input".format(n_dims))
         training = torch.is_grad_enabled() and any(p.requires_grad for p in self.parameters())
-        if training and self.in_channels > 1:
-            if not self.multichannel_training:
-                raise NotImplementedError("multichannel models (in_channels > 1) train natively only with model.multichannel_training = True "
-                                          "(ctn_multichannel_fwd_train / ctn_multichannel_bwd); without it they are forward only: call "
-                                          "under torch.no_grad()")
-            if self.causal or self.separator.mask_softmax:
-                raise NotImplementedError("multichannel training is built for non-causal models with a sigmoid mask; causal or softmax "
-                                          "multichannel models are forward only: call under torch.no_grad()")
-        if training and self.separator.mask_softmax and self.softmax_training and (self.causal or self.in_channels > 1):
-            raise NotImplementedError("softmax-mask training is built for non-causal monaural models (ctn_softmax_fwd_train / "
-                                      "ctn_softmax_bwd); causal or multichannel softmax models are forward only: call under "
-                                      "torch.no_grad()")
-        if training and self.causal and not self.causal_training:
-            raise NotImplementedError("causal (cLN) models train natively only with model.causal_training = True (ctn_causal_fwd_train / "
-                                      "ctn_causal_bwd); without it they are forward only: call under torch.no_grad()")
+        if training:
+            from ._train import run_train, train_entry
+            entry = train_entry(self)
         x = x.contiguous()
         dev = N.require_cuda(x)
         if training:
-            # training: one autograd node over the whole model (ctn_convtasnet_fwd_train / ctn_convtasnet_bwd)
+            # training: one autograd node over the whole model
             if want_latent:
                 raise NotImplementedError("extract_latent under autograd is not built: call it under torch.no_grad()")
-            from ._train import run_train
-            out = run_train(self, x)  # multichannel: already (B, S, C, T)
+            out = run_train(self, x, entry)  # multichannel: already (B, S, C, T)
             return (out.unsqueeze(2) if n_dims == 4 and self.in_channels == 1 else out), None
         B, Cin, T = x.shape
         frames, _, _ = N.frames_of(T, self.kernel_size, self.stride)

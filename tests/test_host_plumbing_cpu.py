@@ -97,22 +97,27 @@ def test_blocks_fwd_checks_the_config():
 BYTES = {
     ("paper", 0, N.MATH_FP32): dict(ws=311111936, tcn=260516352, train=1163137024),
     ("paper", 0, N.MATH_F16X3): dict(ws=350524672, tcn=298351104, train=1416402176),
-    ("paper", 1, N.MATH_FP32): dict(ws=118830080, tcn=68234496, online=22563584),
-    ("paper", 1, N.MATH_F16X3): dict(ws=159292416, tcn=107118848, online=61976320),
+    ("paper", 1, N.MATH_FP32): dict(ws=118830080, tcn=68234496, online=22563584, train=1172096736),
+    ("paper", 1, N.MATH_F16X3): dict(ws=159292416, tcn=107118848, online=61976320, train=1173149408),
     ("tiny", 0, N.MATH_FP32): dict(ws=30572800, tcn=24272128, train=78686464),
     ("tiny", 0, N.MATH_F16X3): dict(ws=31471360, tcn=25070848, train=96548608),
-    ("tiny", 1, N.MATH_FP32): dict(ws=16040960, tcn=9740288, online=692992),
-    ("tiny", 1, N.MATH_F16X3): dict(ws=17005568, tcn=10605056, online=1591552),
+    ("tiny", 1, N.MATH_FP32): dict(ws=16040960, tcn=9740288, online=692992, train=82526176),
+    ("tiny", 1, N.MATH_F16X3): dict(ws=17005568, tcn=10605056, online=1591552, train=82657760),
 }
 
 
 @pytest.mark.parametrize("key", list(BYTES), ids=[f"{n}-{'causal' if c else 'gln'}-math{m}" for n, c, m in BYTES])
 def test_workspace_bytes(key):
     name, causal, math = key
-    c = _cfg(PAPER if name == "paper" else TINY, causal=causal, math=math)
+    base = PAPER if name == "paper" else TINY
+    c = _cfg(base, causal=causal, math=math)
     got = dict(ws=_query(N.ctn_workspace_bytes, c, 2, 32000), tcn=_query(N.ctn_tcn_workspace_bytes, c, 2, 4000))
     if causal:
         got["online"] = _query(N.ctn_online_state_bytes, c, 2, 64)
+        got["train"] = _query(N.ctn_causal_train_workspace_bytes, c, 2, 32000)
+        # the causal step runs its contractions on tf32 pieces in the fp16-piece mode: the same workspace as tf32x3
+        if math == N.MATH_F16X3:
+            assert got["train"] == _query(N.ctn_causal_train_workspace_bytes, _cfg(base, causal=1, math=N.MATH_TF32X3), 2, 32000)
     else:
         got["train"] = _query(N.ctn_train_workspace_bytes, c, 2, 32000)
     for what, want in BYTES[key].items():
