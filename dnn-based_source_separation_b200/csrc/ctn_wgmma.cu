@@ -44,7 +44,8 @@ constexpr int F16_MAX_ROWS = 2048;  // fp16-piece mode: padded output channels o
 // residual update) are formed once per frame tile instead of once per n-tile.  With an odd n-tile count (e.g. the last block's
 // [out; skip] contraction, M = 128) the last CTA's second warpgroup has no n-tile: it still forms its share of each slab, and skips
 // its MMAs and epilogue.  Every other kernel splits TIME: 128 frames x 1 n-tile, warpgroup w frames [64w, 64w + 64): tf32 pieces
-// are K-major only (see the operand store).  The fused mask + decoder has a kernel of its own (k_maskdec).
+// are K-major only (see the operand store).  The fused mask + decoder (k_maskdec) and the fp16-piece EPI_H contractions with K <=
+// P1_MAX_K (pw1, k_pw1_resident) have kernels of their own; the channel-split EPI_H tile here serves K > P1_MAX_K.
 template <int PRO, int EPI, bool F16>
 __host__ __device__ constexpr bool chan_split() { return F16 && (PRO == PRO_DW || EPI == EPI_H); }
 template <int PRO, int EPI, bool F16>
@@ -93,6 +94,38 @@ __device__ __forceinline__ void load_raw(const PwArgs& a, int b, int c0, int tba
                        : make_float4(0.f, 0.f, 0.f, 0.f);
     }
   }
+}
+
+// x_new = x + rstd2*r + (v1 - mean2*rstd2*v2) for channels [c0, c0 + CPT): the previous block's deferred residual update, 0 past
+// frames and past K.  `store`: also write x_new (to res_x_out, for the block after next).
+template <int CPT>
+__device__ __forceinline__ void res_form(const PwArgs& a, int b, int c0, int tbase, float2 mr_res, bool store, const Raw<PRO_RES, CPT>& cur,
+                                         float4 (&v)[CPT]) {
+#pragma unroll
+  for (int j = 0; j < CPT; ++j) {
+    const int k = c0 + j;
+    const int kc = k < a.K ? k : a.K - 1;
+    const float4 x = cur.q[j][0], r = cur.q[j][1];
+    const float cst = __ldg(a.res_v1 + kc) - mr_res.x * mr_res.y * __ldg(a.res_v2 + kc);
+    float4 xn;
+    xn.x = fmaf(mr_res.y, r.x, x.x + cst); xn.y = fmaf(mr_res.y, r.y, x.y + cst);
+    xn.z = fmaf(mr_res.y, r.z, x.z + cst); xn.w = fmaf(mr_res.y, r.w, x.w + cst);
+    if (tbase + 0 >= a.frames) xn.x = 0.f;
+    if (tbase + 1 >= a.frames) xn.y = 0.f;
+    if (tbase + 2 >= a.frames) xn.z = 0.f;
+    if (tbase + 3 >= a.frames) xn.w = 0.f;
+    if (k >= a.K) xn = make_float4(0.f, 0.f, 0.f, 0.f);
+    v[j] = xn;
+    if (store && k < a.K) *reinterpret_cast<float4*>(a.res_x_out + ((size_t)b * a.K + k) * a.pitch + tbase) = xn;
+  }
+}
+
+// Byte offset of (frame f, channel c) in a 32-channel slab of fp16 pieces, MN-major SWIZZLE_128B (ptx::wg_desc_mn128): row =
+// slab channel, 128 B = 64 consecutive frames, 16-byte chunk index XOR channel % 8; 8 channels per 1 KB atom, 4 atoms down the
+// slab; each 64-frame column of a 128-frame tile is its own column of atoms (4 KB apart).  A thread's 4 frames are one 8-byte store
+// per piece, and a warp's store covers two 128-byte rows.
+__device__ __forceinline__ uint32_t mn128_offset(uint32_t f, uint32_t c) {
+  return (f >> 6) * 4096u + (c >> 3) * 1024u + (c & 7) * 128u + ((((f >> 3) & 7) ^ (c & 7)) << 4) + (f & 7) * 2u;
 }
 
 // u = PReLU(dwconv3(gLN1(h)) + bd) for channels [c0, c0 + CPT) from their loaded taps.
@@ -221,27 +254,8 @@ __global__ void __launch_bounds__(THREADS, F16 ? 2 : 1) k_pw_wgmma(const TcArgs 
     } else {
 #pragma unroll
       for (int j = 0; j < CPT; ++j) v[j] = cur.q[j][0];
-      if (PRO == PRO_RES) {
-        // x_new = x + rstd2*r + (v1 - mean2*rstd2*v2): the previous block's residual update, applied on the fly;
-        // the CTA holding n-tile 0 of each time tile also writes x_new for the block after next
-#pragma unroll
-        for (int j = 0; j < CPT; ++j) {
-          const int k = c0 + j;
-          const int kc = k < a.K ? k : a.K - 1;
-          const float4 r = cur.q[j][PRO == PRO_RES ? 1 : 0];
-          const float cst = __ldg(a.res_v1 + kc) - mr_res.x * mr_res.y * __ldg(a.res_v2 + kc);
-          float4 xn;
-          xn.x = fmaf(mr_res.y, r.x, v[j].x + cst); xn.y = fmaf(mr_res.y, r.y, v[j].y + cst);
-          xn.z = fmaf(mr_res.y, r.z, v[j].z + cst); xn.w = fmaf(mr_res.y, r.w, v[j].w + cst);
-          if (tbase + 0 >= a.frames) xn.x = 0.f;
-          if (tbase + 1 >= a.frames) xn.y = 0.f;
-          if (tbase + 2 >= a.frames) xn.z = 0.f;
-          if (tbase + 3 >= a.frames) xn.w = 0.f;
-          if (k >= a.K) xn = make_float4(0.f, 0.f, 0.f, 0.f);
-          v[j] = xn;
-          if (store_side && k < a.K) *reinterpret_cast<float4*>(a.res_x_out + ((size_t)b * a.K + k) * a.pitch + tbase) = xn;
-        }
-      }
+      // the CTA holding n-tile 0 of each time tile also writes x_new
+      if constexpr (PRO == PRO_RES) res_form<CPT>(a, b, c0, tbase, mr_res, store_side, cur, v);
       if (PRO == PRO_PRELU) {
 #pragma unroll
         for (int j = 0; j < CPT; ++j) {
@@ -255,14 +269,10 @@ __global__ void __launch_bounds__(THREADS, F16 ? 2 : 1) k_pw_wgmma(const TcArgs 
     if (ks + 1 < g.k_slabs) load_raw<PRO, CPT>(a, b, (ks + 1) * KS + c_thr, tbase, first, step, dw_interior, cur);
     uint8_t* sa = smem + SMEM_HEADER + (size_t)s * STAGE_BYTES;
     if (F16) {
-      // MN-major SWIZZLE_128B (ptx::wg_desc_mn128): row = slab channel, 128 B = 64 consecutive frames, 16-byte chunk index XOR
-      // channel % 8; 8 channels per 1 KB atom, 4 atoms down the slab; each 64-frame half of a 128-frame tile is its own column of
-      // atoms (4 KB apart).  A thread's 4 frames are one 8-byte store per piece, and a warp's store covers two 128-byte rows.
       const uint32_t f = (uint32_t)(tbase - tt * TMC);
 #pragma unroll
       for (int j = 0; j < CPT; ++j) {
-        const uint32_t c = (uint32_t)(c_thr + j);
-        const uint32_t off = (f >> 6) * 4096u + (c >> 3) * 1024u + (c & 7) * 128u + ((((f >> 3) & 7) ^ (c & 7)) << 4) + (f & 7) * 2u;
+        const uint32_t off = mn128_offset(f, (uint32_t)(c_thr + j));
         uint2 h2, l2;
         ptx::split_f16x2(v[j].x * act_s, v[j].y * act_s, h2.x, l2.x);
         ptx::split_f16x2(v[j].z * act_s, v[j].w * act_s, h2.y, l2.y);
@@ -463,8 +473,7 @@ __global__ void __launch_bounds__(THREADS, 1) k_maskdec(const TcArgs g) {
       for (int j = 0; j < CPW; ++j) {
         float4 x = v[ks][j];
         x.x = prelu_f(x.x, pslope); x.y = prelu_f(x.y, pslope); x.z = prelu_f(x.z, pslope); x.w = prelu_f(x.w, pslope);
-        const uint32_t c = (uint32_t)(warp * CPW + j);
-        const uint32_t off = (f >> 6) * 4096u + (c >> 3) * 1024u + (c & 7) * 128u + ((((f >> 3) & 7) ^ (c & 7)) << 4) + (f & 7) * 2u;
+        const uint32_t off = mn128_offset(f, (uint32_t)(warp * CPW + j));
         uint2 h2, l2;
         ptx::split_f16x2(x.x * act_s, x.y * act_s, h2.x, l2.x);
         ptx::split_f16x2(x.z * act_s, x.w * act_s, h2.y, l2.y);
@@ -587,6 +596,187 @@ __global__ void __launch_bounds__(THREADS, 1) k_maskdec(const TcArgs g) {
         else yo[tau] = v;
       }
     }
+  }
+}
+
+// ---- pw1 on a resident operand -----------------------------------------------------------------------------------
+// h = PReLU(W1 x + b1) with its gLN statistics (EPI_H), fp16 pieces, K <= P1_MAX_K; x is the block input (PRO_NONE) or the previous
+// block's deferred residual update (PRO_RES, which also writes x_new).  One CTA per (sample, 64-frame tile) walks every n-tile:
+//   * every global load of the tile's operand is issued before any of it is formed (at K = 128, 8 float4 of x and 8 of r per
+//     thread); x_new is formed and stored once, and its hi / lo pieces stay resident in shared memory for every pass (32 KB,
+//     the MN-major layout of mn128_offset);
+//   * channel split as in k_pw_wgmma: warpgroup w computes n-tile 2p + w in pass p (at an odd n-tile count the second warpgroup
+//     has one pass less).  Each warpgroup streams its own n-tile's weight slabs through a ring of P1_WST bulk-copy stages that
+//     runs on across passes, so the next pass's first slabs arrive during this pass's epilogue; the warpgroups only meet again
+//     at the end;
+//   * each pass's output scales and biases are loaded while its MMAs run and go into a shared-memory table, so the epilogue
+//     issues no global loads;
+//   * the gLN statistics are reduced per CTA before the double atomics.
+// h and x_new are bit for bit those of k_pw_wgmma's channel-split tile: the same prologue, the same 3-piece wgmma sequence
+// (slab, then kk, then hi.hi, lo.hi, hi.lo) and the same epilogue operations.  Only the order of the double statistics sums differs.
+// About 102 KB of shared memory: two CTAs per SM, so one CTA's loads overlap the other's epilogue stores.
+constexpr int P1_MAX_K = 128;
+constexpr int P1_TF = 64;   // frames per CTA
+constexpr int P1_WST = 2;   // weight stages per warpgroup
+constexpr uint32_t P1_A_BYTES = P1_TF * 64u, P1_W_BYTES = NT * 64u;  // one fp16 piece of an operand / weight slab
+constexpr size_t P1_SMEM = 1024 + SMEM_HEADER + (size_t)(P1_MAX_K / KS) * 2 * P1_A_BYTES + (size_t)2 * P1_WST * 2 * P1_W_BYTES +
+                           (size_t)2 * 2 * 2 * NT * sizeof(float) + (size_t)(THREADS / 32) * 2 * sizeof(double);
+
+// the 128 threads of warpgroup wg
+__device__ __forceinline__ void wg_bar(int wg) {
+  if (wg == 0) ptx::named_bar_sync<1, 128>();
+  else ptx::named_bar_sync<2, 128>();
+}
+
+template <int PRO>
+__global__ void __launch_bounds__(THREADS, 2) k_pw1_resident(const TcArgs g) {
+  static_assert(PRO == PRO_NONE || PRO == PRO_RES, "pw1 prologues");
+  constexpr int NSL = P1_MAX_K / KS;
+  constexpr int CPT = 2;  // channels a thread forms per slab: warp w channels [4 w, 4 w + 4), 16 lanes x 4 frames per channel
+  extern __shared__ uint8_t smem_raw[];
+  const uint32_t raw = ptx::smem_u32(smem_raw);
+  const uint32_t base = (raw + 1023u) & ~1023u;
+  uint8_t* smem = smem_raw + (base - raw);
+  uint64_t* wbar = reinterpret_cast<uint64_t*>(smem);  // [warpgroup][stage]
+  const uint32_t op0 = base + SMEM_HEADER;                                                  // resident operand
+  const uint32_t ring0 = op0 + (uint32_t)NSL * 2 * P1_A_BYTES;                               // weight rings
+  float* tab0 = reinterpret_cast<float*>(smem + (ring0 - base) + 2 * P1_WST * 2 * P1_W_BYTES);  // [warpgroup][parity][scale | bias]
+  double* red = reinterpret_cast<double*>(tab0 + 2 * 2 * 2 * NT);                             // [warp][sum, sumsq]
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, wg = warp >> 2, lt = threadIdx.x & (NT - 1);
+  const PwArgs& a = g.a;
+  const int tt = (int)blockIdx.x % g.t_tiles, b = (int)blockIdx.x / g.t_tiles;
+  const int k_slabs = g.k_slabs;
+  const int passes = g.n_tiles > wg ? (g.n_tiles - wg + 1) / 2 : 0;  // this warpgroup's n-tiles 2p + wg
+  const int total = passes * k_slabs;                                 // its weight slabs, pass-major
+  const uint8_t* wimg = reinterpret_cast<const uint8_t*>(g.wimg);
+  const uint32_t ring = ring0 + (uint32_t)wg * P1_WST * 2 * P1_W_BYTES;
+
+  if (threadIdx.x == 0) {
+    for (int s = 0; s < 2 * P1_WST; ++s) ptx::mbar_init(ptx::smem_u32(&wbar[s]), 1);
+    ptx::fence_mbar_init();
+  }
+  __syncthreads();
+  // slab u of the warpgroup goes to stage u % P1_WST; it may be issued once slab u - P1_WST has been consumed by all 4 warps
+  int issued = 0;
+  auto refill = [&](int consumed) {
+    for (; issued < total && issued < consumed + P1_WST; ++issued) {
+      const int p = issued / k_slabs, ks = issued - p * k_slabs;
+      const uint32_t fb = ptx::smem_u32(&wbar[wg * P1_WST + issued % P1_WST]);
+      ptx::mbar_arrive_expect_tx(fb, 2 * P1_W_BYTES);
+      ptx::bulk_g2s(ring + (uint32_t)(issued % P1_WST) * 2 * P1_W_BYTES, wimg + ((size_t)(2 * p + wg) * k_slabs + ks) * 2 * P1_W_BYTES,
+                    2 * P1_W_BYTES, fb);
+    }
+  };
+  if (lt == 0) refill(0);
+
+  // ---- the operand, once
+  const float act_s = __ldg(a.act_scale);
+  {
+    const int c_thr = warp * CPW + (lane / 16) * CPT;
+    const int tbase = tt * P1_TF + (lane % 16) * 4;
+    Raw<PRO, CPT> cur[NSL];
+#pragma unroll
+    for (int ks = 0; ks < NSL; ++ks)
+      if (ks < k_slabs) load_raw<PRO, CPT>(a, b, ks * KS + c_thr, tbase, 0, 0, false, cur[ks]);
+    float2 mr_res = make_float2(0.f, 1.f);
+    if (PRO == PRO_RES) mr_res = gln_mean_rstd(a.res_stats + 2 * b, a.res_n, a.res_eps);
+    const uint32_t f = (uint32_t)(tbase - tt * P1_TF);
+#pragma unroll
+    for (int ks = 0; ks < NSL; ++ks) {
+      if (ks >= k_slabs) break;
+      float4 v[CPT];
+      if constexpr (PRO == PRO_RES) {
+        res_form<CPT>(a, b, ks * KS + c_thr, tbase, mr_res, true, cur[ks], v);
+      } else {
+#pragma unroll
+        for (int j = 0; j < CPT; ++j) v[j] = cur[ks].q[j][0];
+      }
+      uint8_t* sa = smem + (op0 - base) + (size_t)ks * 2 * P1_A_BYTES;
+#pragma unroll
+      for (int j = 0; j < CPT; ++j) {
+        const uint32_t off = mn128_offset(f, (uint32_t)(c_thr + j));
+        uint2 h2, l2;
+        ptx::split_f16x2(v[j].x * act_s, v[j].y * act_s, h2.x, l2.x);
+        ptx::split_f16x2(v[j].z * act_s, v[j].w * act_s, h2.y, l2.y);
+        *reinterpret_cast<uint2*>(sa + off) = h2;
+        *reinterpret_cast<uint2*>(sa + P1_A_BYTES + off) = l2;
+      }
+    }
+  }
+  ptx::fence_proxy_async_smem();
+  __syncthreads();
+
+  const float inv_act = 1.f / act_s, eslope = __ldg(a.slope);
+  const bool store_pre = a.store_pre != 0;  // training forward: keep the PRE-activation, statistics of PReLU(.)
+  const int row0 = (warp & 3) * 16 + (lane >> 2);  // frame within the tile (and row0 + 8)
+  double cs = 0.0, css = 0.0;
+  for (int p = 0; p < passes; ++p) {
+    const int nt = 2 * p + wg;
+    // this thread's column of the pass's epilogue table, in flight during the MMAs
+    const int tn = nt * NT + lt;
+    const float tsc = tn < a.M ? __ldg(g.oscale + tn) * inv_act : 0.f;
+    const float tbi = tn < a.M ? __ldg(a.bias + tn) : 0.f;
+    float acc[64];
+#pragma unroll
+    for (int i = 0; i < 64; ++i) acc[i] = 0.f;
+    for (int ks = 0; ks < k_slabs; ++ks) {
+      const int u = p * k_slabs + ks;
+      const uint32_t w_hi = ring + (uint32_t)(u % P1_WST) * 2 * P1_W_BYTES, w_lo = w_hi + P1_W_BYTES;
+      const uint32_t a_hi = op0 + (uint32_t)ks * 2 * P1_A_BYTES, a_lo = a_hi + P1_A_BYTES;
+      ptx::mbar_wait(ptx::smem_u32(&wbar[wg * P1_WST + u % P1_WST]), (uint32_t)(u / P1_WST) & 1u);
+      ptx::wg_fence();
+#pragma unroll
+      for (int kk = 0; kk < KS / 16; ++kk) {
+        const uint64_t dah = ptx::wg_desc_mn128(a_hi + kk * 2048, 4096u, 1024u), dwh = ptx::wg_desc(w_hi + kk * 32, 8 * 64, ptx::SW64);
+        const uint64_t dal = ptx::wg_desc_mn128(a_lo + kk * 2048, 4096u, 1024u), dwl = ptx::wg_desc(w_lo + kk * 32, 8 * 64, ptx::SW64);
+        ptx::wg_mma_f16(acc, dah, dwh);
+        ptx::wg_mma_f16(acc, dal, dwh);
+        ptx::wg_mma_f16(acc, dah, dwl);
+      }
+      ptx::wg_commit();
+      if (ks > 0) {
+        ptx::wg_wait<1>();  // slab u - 1 is consumed in this warp ...
+        wg_bar(wg);         // ... and in the warpgroup: its stage may be refilled
+        if (lt == 0) refill(u);
+      }
+    }
+    ptx::wg_wait<0>();
+    // the table of parity p & 1 was last read in the epilogue of pass p - 2, which every warp of the warpgroup left before the
+    // barrier of pass p - 1
+    float* tab = tab0 + (wg * 2 + (p & 1)) * 2 * NT;
+    tab[lt] = tsc;
+    tab[NT + lt] = tbi;
+    wg_bar(wg);  // the pass's slabs are consumed and the table is in
+    if (lt == 0) refill((p + 1) * k_slabs);
+
+    // n0 reaches the epilogue through an opaque move, so that the per-column addresses are not formed ahead of the slab loop
+    int n0 = nt * NT;
+    asm volatile("" : "+r"(n0));
+    float ls = 0.f, lss = 0.f;
+#pragma unroll
+    for (int i = 0; i < 64; ++i) {
+      const int row = row0 + 8 * ((i >> 1) & 1);
+      const int c = 8 * (i >> 2) + 2 * (lane & 3) + (i & 1);
+      const int n = n0 + c;
+      const int t = tt * P1_TF + row;
+      if (n >= a.M) continue;
+      const bool tvalid = t < a.frames;
+      // v * scale undoes the power-of-two row scaling of the weights and the activation scale (exact)
+      const float pre = fmaf(acc[i], tab[c], tab[NT + c]);
+      const float act = prelu_f(pre, eslope);
+      if (tvalid) { ls += act; lss = fmaf(act, act, lss); }  // gLN statistics are always those of PReLU(.)
+      a.D[((size_t)b * a.M + n) * a.pitch + t] = tvalid ? (store_pre ? pre : act) : 0.f;
+    }
+    cs += warp_sum_d((double)ls);
+    css += warp_sum_d((double)lss);
+  }
+  if (lane == 0) { red[2 * warp] = cs; red[2 * warp + 1] = css; }
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    double s = 0.0, ss = 0.0;
+    for (int w = 0; w < THREADS / 32; ++w) { s += red[2 * w]; ss += red[2 * w + 1]; }
+    atomicAdd(&a.stats_out[2 * b], s);
+    atomicAdd(&a.stats_out[2 * b + 1], ss);
   }
 }
 
@@ -777,6 +967,26 @@ int launch_maskdec(const TcArgs& g0, cudaStream_t st) {
   return CTN_OK;
 }
 
+template <int PRO>
+int launch_pw1(const TcArgs& g0, cudaStream_t st) {
+  TcArgs g = g0;
+  g.t_tiles = g.a.pitch / P1_TF;
+  g.n_groups = 1;
+  static bool attr_done[CTN_MAX_DEVICES] = {false};
+  const int dev = ctn_current_device();
+  if (!attr_done[dev]) {
+    cudaError_t e = cudaFuncSetAttribute(k_pw1_resident<PRO>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)P1_SMEM);
+    if (e != cudaSuccess) return (int)e;
+    attr_done[dev] = true;
+  }
+  const long long grid = (long long)g.a.B * g.t_tiles;
+  if (grid > 0x7fffffffLL) return CTN_EUNSUPPORTED;
+  k_pw1_resident<PRO><<<(unsigned)grid, THREADS, P1_SMEM, st>>>(g);
+  CTN_COUNT_LAUNCH();
+  CTN_RETURN_IF_CUDA_ERR();
+  return CTN_OK;
+}
+
 // a.wimg holds the image of a.W in the pieces `pmath`
 int launch_wgmma(const PwArgs& a, int pro, int epi, int pmath, cudaStream_t st) {
   if (!a.wimg) return CTN_EINVAL;
@@ -797,6 +1007,11 @@ int launch_wgmma(const PwArgs& a, int pro, int epi, int pmath, cudaStream_t st) 
   if (pro == PRO_DW && epi == EPI_RAW)
     return train_dw ? launch_math<PRO_DW, EPI_RAW, true>(g, math, st) : launch_math<PRO_DW, EPI_RAW>(g, math, st);
   if (pro == PRO_NONE && epi == EPI_HEAD) return launch_math<PRO_NONE, EPI_HEAD>(g, math, st);
+  // pw1 on fp16 pieces: the resident-operand kernel up to P1_MAX_K input channels, k_pw_wgmma's channel-split tile beyond
+  if (epi == EPI_H && math == CTN_MATH_F16X3 && a.K <= P1_MAX_K) {
+    if (pro == PRO_NONE) return launch_pw1<PRO_NONE>(g, st);
+    if (pro == PRO_RES) return launch_pw1<PRO_RES>(g, st);
+  }
   if (pro == PRO_NONE && epi == EPI_H) return launch_math<PRO_NONE, EPI_H>(g, math, st);
   if (pro == PRO_RES && epi == EPI_H) return launch_math<PRO_RES, EPI_H>(g, math, st);
   if (pro == PRO_PRELU && epi == EPI_MASK) return launch_math<PRO_PRELU, EPI_MASK>(g, math, st);

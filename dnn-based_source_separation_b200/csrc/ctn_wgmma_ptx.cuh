@@ -31,6 +31,13 @@ __device__ __forceinline__ void mbar_wait(uint32_t bar, uint32_t parity) {
       "}" ::"r"(bar), "r"(parity) : "memory");
 }
 
+// named barrier ID (1..15; 0 is __syncthreads) over THREADS threads, e.g. the 128 of one warpgroup.  Immediate operands: with a
+// register id ptxas reserves all 16 barriers of the CTA.
+template <uint32_t ID, uint32_t THREADS>
+__device__ __forceinline__ void named_bar_sync() {
+  asm volatile("bar.sync %0, %1;" ::"n"(ID), "n"(THREADS) : "memory");
+}
+
 // ---- async proxy -----------------------------------------------------------------------------------------------
 // generic-proxy st.shared writes -> visible to the async proxy (wgmma operand reads, bulk copies)
 __device__ __forceinline__ void fence_proxy_async_smem() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
