@@ -681,6 +681,7 @@ extern "C" int ctn_sep_head_fwd(const float* w, const double* stats0, const floa
   LaunchScope scope(w);
   if (!w || !stats0 || !norm_g || !norm_b || !bn_w || !x0 || !workspace || B <= 0 || N <= 0 || Bc <= 0 || frames <= 0) return CTN_EINVAL;
   if (pitch < frames || pitch % CTN_TILE_T != 0 || (((uintptr_t)workspace) & 255)) return CTN_EALIGN;
+  if ((((uintptr_t)w) | ((uintptr_t)x0)) & 15) return CTN_EALIGN;  // 128-bit operand loads and output stores
   if (workspace_bytes < ctn_stage_workspace_bytes(Bc, N)) return CTN_EWORKSPACE;
   cudaStream_t st = (cudaStream_t)stream;
   Carver cv(workspace);
@@ -706,7 +707,10 @@ extern "C" int ctn_sep_tail_fwd(const float* y, const float* w, const float* pre
   if (!y || !w || !prelu || !mask_w || !mask_b || !dec_w || !out || !what || !workspace || B <= 0 || N <= 0 || Bc <= 0 || S <= 0 || frames <= 0)
     return CTN_EINVAL;
   if (pitch < frames || pitch % CTN_TILE_T != 0 || (((uintptr_t)workspace) & 255)) return CTN_EALIGN;
+  if ((((uintptr_t)y) | ((uintptr_t)w) | ((uintptr_t)what)) & 15) return CTN_EALIGN;  // 128-bit operand loads and stores
   if (workspace_bytes < ctn_stage_workspace_bytes(S * N, Bc)) return CTN_EWORKSPACE;
+  // the decoder's refusals, before the mask contraction launches
+  CTN_TRY(ctn_decoder_check(B * S, N, frames, pitch, L, stride, crop_left, T));
   cudaStream_t st = (cudaStream_t)stream;
   Carver cv(workspace);
   StageWs ws;

@@ -52,6 +52,7 @@ extern "C" int ctn_pointwise_conv1d_fwd(const float* x, const float* W, const fl
   LaunchScope scope(x);
   if (!x || !W || !y || !workspace || B <= 0 || M <= 0 || K <= 0 || frames <= 0) return CTN_EINVAL;
   if (pitch < frames || pitch % CTN_TILE_T != 0 || (((uintptr_t)workspace) & 255)) return CTN_EALIGN;
+  if (((uintptr_t)x) & 15) return CTN_EALIGN;  // 128-bit operand loads
   const size_t ybytes = ((size_t)B * M * pitch * sizeof(float) + 255) & ~(size_t)255;
   const size_t wbytes = math != CTN_MATH_FP32 ? ctn_pw_wimg_bytes(M, K, math) + 256 : 0;
   if (workspace_bytes < ybytes + wbytes + (size_t)B * 2 * sizeof(double) + 64 * sizeof(float) + 512) return CTN_EWORKSPACE;

@@ -268,8 +268,7 @@ __global__ void __launch_bounds__(128) k_decoder_generic(const float* __restrict
 template <int STRIDE, int R>
 static int launch_decoder(const float* what, const float* Wd, float* y, int BS, int N, int frames, int in_pitch,
                           int crop_left, int T_out, cudaStream_t st) {
-  const size_t smem = sizeof(float) * ((size_t)N * STRIDE * R + (size_t)(DEC_SPLIT - 1) * STRIDE * 128);
-  if (smem > 200 * 1024) return CTN_EUNSUPPORTED;
+  const size_t smem = sizeof(float) * ((size_t)N * STRIDE * R + (size_t)(DEC_SPLIT - 1) * STRIDE * 128);  // <= 200 KB: ctn_decoder_check
   if (smem > 48 * 1024) {
     cudaError_t e = cudaFuncSetAttribute(k_decoder<STRIDE, R>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
     if (e != cudaSuccess) return (int)e;
@@ -282,14 +281,22 @@ static int launch_decoder(const float* what, const float* Wd, float* y, int BS, 
   return CTN_OK;
 }
 
-extern "C" int ctn_decoder_fwd(const float* w_hat, const float* dec_w, float* y, int BS, int N, int frames,
-                               int in_pitch, int L, int stride, int crop_left, int T_out, ctn_stream_t stream) {
-  LaunchScope scope(w_hat);
-  if (!w_hat || !dec_w || !y || BS <= 0 || N <= 0 || frames <= 0 || L <= 0 || stride <= 0 || L % stride != 0)
-    return CTN_EINVAL;
+int ctn_decoder_check(int BS, int N, int frames, int in_pitch, int L, int stride, int crop_left, int T_out) {
+  if (BS <= 0 || N <= 0 || frames <= 0 || L <= 0 || stride <= 0 || L % stride != 0) return CTN_EINVAL;
   if (in_pitch < frames) return CTN_EINVAL;
   const int full = (frames - 1) * stride + L;
   if (crop_left < 0 || T_out <= 0 || crop_left + T_out > full) return CTN_EINVAL;
+  const int R = L / stride;
+  const bool special = R == 2 && (stride == 8 || stride == 1 || stride == 10 || stride == 2);
+  if (special && sizeof(float) * ((size_t)N * L + (size_t)(DEC_SPLIT - 1) * stride * 128) > 200 * 1024) return CTN_EUNSUPPORTED;
+  return CTN_OK;
+}
+
+extern "C" int ctn_decoder_fwd(const float* w_hat, const float* dec_w, float* y, int BS, int N, int frames,
+                               int in_pitch, int L, int stride, int crop_left, int T_out, ctn_stream_t stream) {
+  LaunchScope scope(w_hat);
+  if (!w_hat || !dec_w || !y) return CTN_EINVAL;
+  CTN_TRY(ctn_decoder_check(BS, N, frames, in_pitch, L, stride, crop_left, T_out));
   cudaStream_t st = (cudaStream_t)stream;
   const int R = L / stride;
   if (stride == 8 && R == 2) return launch_decoder<8, 2>(w_hat, dec_w, y, BS, N, frames, in_pitch, crop_left, T_out, st);

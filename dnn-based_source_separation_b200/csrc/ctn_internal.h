@@ -184,6 +184,9 @@ struct SkipJob { const float* r; const float* v1; const float* v2; const double*
 struct SkipJobs { SkipJob j[CTN_MAX_BLOCKS]; int n; };
 int ctn_skip_reduce(const SkipJobs& jobs, double n2, float eps, float* skip, int B, int Sc, int frames, int pitch, cudaStream_t st);
 
+// the refusals of ctn_decoder_fwd, for callers that must refuse before their own launches (ctn_sep_tail_fwd)
+int ctn_decoder_check(int BS, int N, int frames, int in_pitch, int L, int stride, int crop_left, int T_out);
+
 int ctn_copy_to_pitch(const float* src, float* dst, int rows, int frames, int pitch, cudaStream_t st);
 int ctn_copy_from_pitch(const float* src, float* dst, int rows, int frames, int pitch, cudaStream_t st);
 

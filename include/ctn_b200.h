@@ -303,14 +303,15 @@ int ctn_dprnn_norm_res2_fwd(const float* P, const float* fc_bias, const float* R
                             int B, int D1, int D2, int F, float eps, int swap, double* scratch, unsigned* out_absmax, ctn_stream_t stream);
 /* Separator head on the padded layout, src/models/conv_tasnet.py:370-371 == src/models/dprnn_tasnet.py:335-336:
  * x0 (B,Bc,pitch) = Wb gLN(w) + bb; w (B,N,pitch), stats0 double[B][2] = (sum, sumsq) of w (as ctn_encoder_fwd leaves them).
- * workspace >= ctn_stage_workspace_bytes(Bc, N). */
+ * workspace >= ctn_stage_workspace_bytes(Bc, N), 256-byte aligned; w and x0 16-byte aligned.  Every refusal comes before the first launch. */
 size_t ctn_stage_workspace_bytes(int M, int K);
 int ctn_sep_head_fwd(const float* w, const double* stats0, const float* norm_g, const float* norm_b, const float* bn_w,
                      const float* bn_b, float* x0, int B, int N, int Bc, int frames, int pitch, float eps, int math, void* workspace,
                      size_t workspace_bytes, ctn_stream_t stream);
 /* Separator tail + decoder, conv_tasnet.py:373-376,158-169 == dprnn_tasnet.py:348-350,141-153: PReLU -> mask 1x1 -> sigmoid ->
  * w*mask -> ConvTranspose1d -> crop.  y (B,Bc,pitch), w (B,N,pitch); out (B,S,T); latent nullable (B,S,N,frames);
- * what (B,S*N,pitch) scratch; workspace >= ctn_stage_workspace_bytes(S*N, Bc). */
+ * what (B,S*N,pitch) scratch; workspace >= ctn_stage_workspace_bytes(S*N, Bc), 256-byte aligned; y, w and what 16-byte aligned.
+ * Every refusal, the decoder's included (crop_left + T past the full length, L % stride != 0), comes before the first launch. */
 int ctn_sep_tail_fwd(const float* y, const float* w, const float* prelu, const float* mask_w, const float* mask_b,
                      const float* dec_w, float* out, float* latent, float* what, int B, int N, int Bc, int S, int frames, int pitch,
                      int L, int stride, int crop_left, int T, int math, void* workspace, size_t workspace_bytes, ctn_stream_t stream);
@@ -318,7 +319,8 @@ int ctn_sep_tail_fwd(const float* y, const float* w, const float* prelu, const f
 /* modules.conv.DepthwiseSeparableConv1d.forward, src/modules/conv.py:24-28 (not on Conv-TasNet's path; API completeness).
  * Depthwise stage: x (B,C,T) contiguous, w (C,1,K), bias nullable -> y (B,C,y_pitch) with T_out = (T + 2 padding - dilation (K-1) - 1)
  * / stride + 1 valid columns, the rest zero.  Pointwise stage: x (B,K,pitch) padded layout with `frames` valid columns, W (M,K,1),
- * bias nullable -> y (B,M,frames) contiguous; workspace >= 4*B*M*pitch + ctn_stage_workspace_bytes(M,K) + 16*B + 4096 bytes. */
+ * bias nullable -> y (B,M,frames) contiguous, x 16-byte aligned; workspace >= 4*B*M*pitch + ctn_stage_workspace_bytes(M,K) + 16*B + 4096
+ * bytes, 256-byte aligned.  Both stages refuse before any launch. */
 int ctn_depthwise_conv1d_fwd(const float* x, const float* w, const float* bias, float* y, int B, int C, int T, int K, int stride, int padding,
                              int dilation, int y_pitch, ctn_stream_t stream);
 int ctn_pointwise_conv1d_fwd(const float* x, const float* W, const float* bias, float* y, int B, int M, int K, int frames, int pitch,
