@@ -6,6 +6,8 @@
 //   pass 2: den[i][j] = |alpha_ij t_j - e_i|^2 (explicit residual, no cancellation), num = sum (alpha t)^2
 // and a finalize kernel enumerates the permutations in itertools (lexicographic) order, takes the first minimum
 // and writes the int64 permutation.  Accumulation is fp32 per thread-chunk, double across threads.
+// PIT over plain SDR (further down) needs one pass only: its pair value is a function of |t_j|^2 and |t_j - e_i|^2, and it shares
+// the permutation scoring through k_pit_finalize's Pair parameter.
 #include "ctn_common.cuh"
 #include "ctn_sisdr_grad.cuh"
 
@@ -131,23 +133,33 @@ __global__ void __launch_bounds__(256) k_pit_pass2(const float* __restrict__ est
   }
 }
 
-// one block per sample, thread p = permutation index (lexicographic); block = 32*ceil(S!/32)
-__global__ void k_pit_finalize(const double* __restrict__ scratch, int S, int nperm, float eps, float* __restrict__ loss_b,
-                               int64_t* __restrict__ perm, float* __restrict__ pair_sisdr) {
-  __shared__ float sd[CTN_MAX_S * CTN_MAX_S];
-  __shared__ float best_v[32];
-  __shared__ int best_i[32];
-  const int b = blockIdx.x, p = threadIdx.x;
-  const double* sc = scratch + (size_t)b * pit_scratch_per_sample(S);
-  if (p < S * S) {
+// Pair value of the SI-SDR PIT: v[i][j] = SI-SDR(est_i, tgt_j) from the pass statistics (dot, den, tt).
+struct SisdrPair {
+  static __device__ size_t per_sample(int S) { return pit_scratch_per_sample(S); }
+  static __device__ float value(const double* sc, int S, int p, float eps) {
     const int j = p % S;
     const float tt = (float)sc[2 * S * S + j];
     const float alpha = (float)sc[p] / (tt + eps);
     const float num = alpha * alpha * tt;  // sum((alpha*target)^2), sdr.py:136
     const float den = (float)sc[S * S + p];
-    const float v = 10.f * log10f((num + eps) / (den + eps));  // sdr.py:136-137
+    return 10.f * log10f((num + eps) / (den + eps));  // sdr.py:136-137
+  }
+};
+
+// One block per sample, thread p = permutation index (lexicographic); block = 32*ceil(S!/32).  Pair supplies the sample's
+// scratch stride and the value of pair p = i*S + j; everything after the pair table is shared by the SI-SDR and SDR PITs.
+template <class Pair>
+__global__ void k_pit_finalize(const double* __restrict__ scratch, int S, int nperm, float eps, float* __restrict__ loss_b,
+                               int64_t* __restrict__ perm, float* __restrict__ pair_out) {
+  __shared__ float sd[CTN_MAX_S * CTN_MAX_S];
+  __shared__ float best_v[32];
+  __shared__ int best_i[32];
+  const int b = blockIdx.x, p = threadIdx.x;
+  const double* sc = scratch + (size_t)b * Pair::per_sample(S);
+  if (p < S * S) {
+    const float v = Pair::value(sc, S, p, eps);
     sd[p] = v;
-    if (pair_sisdr) pair_sisdr[(size_t)b * S * S + p] = v;
+    if (pair_out) pair_out[(size_t)b * S * S + p] = v;
   }
   __syncthreads();
   float myloss = INFINITY;
@@ -167,7 +179,7 @@ __global__ void k_pit_finalize(const double* __restrict__ scratch, int S, int np
       if (S - 1 - i > 0) fact /= (S - 1 - i);
     }
     float acc = 0.f;
-    for (int i = 0; i < S; ++i) acc += -sd[i * S + pi[i]];  // NegSISDR (sdr.py:212), target permuted (pit.py:30)
+    for (int i = 0; i < S; ++i) acc += -sd[i * S + pi[i]];  // NegSISDR / NegSDR (sdr.py:212), target permuted (pit.py:30)
     myloss = acc / (float)S;                                // reduction='mean' over sources (sdr.py:216)
   }
   // first-minimum argmin over p (torch.min, pit.py:39)
@@ -203,6 +215,24 @@ __global__ void k_batch_mean(const float* __restrict__ loss_b, int B, float* __r
 
 // gridDim.y is at most 65535; the kernels loop over the rest of the rows
 static unsigned grid_rows(int rows) { return rows < 65535 ? (unsigned)rows : 65535u; }
+
+// permutation scoring (+ the batch mean when loss_mean is given) from the pair statistics in scratch
+template <class Pair>
+static int launch_pit_finalize(const double* scratch, int B, int S, float eps, float* loss_b, int64_t* perm, float* loss_mean,
+                               float* pair_out, cudaStream_t st) {
+  int nperm = 1;
+  for (int i = 2; i <= S; ++i) nperm *= i;
+  int threads = ((nperm > S * S ? nperm : S * S) + 31) / 32 * 32;
+  k_pit_finalize<Pair><<<B, threads, 0, st>>>(scratch, S, nperm, eps, loss_b, perm, pair_out);
+  CTN_COUNT_LAUNCH();
+  CTN_RETURN_IF_CUDA_ERR();
+  if (loss_mean) {
+    k_batch_mean<<<1, 32, 0, st>>>(loss_b, B, loss_mean);
+    CTN_COUNT_LAUNCH();
+    CTN_RETURN_IF_CUDA_ERR();
+  }
+  return CTN_OK;
+}
 
 template <int S>
 static int launch_pit(const float* est, const float* tgt, int B, int T, float eps, double* scratch, cudaStream_t st) {
@@ -242,18 +272,7 @@ extern "C" int ctn_sisdr_pit_fwd(const float* est, const float* tgt, int B, int 
     default: rc = launch_pit<6>(est, tgt, B, T, eps, scratch, st); break;
   }
   if (rc) return rc;
-  int nperm = 1;
-  for (int i = 2; i <= S; ++i) nperm *= i;
-  int threads = ((nperm > S * S ? nperm : S * S) + 31) / 32 * 32;
-  k_pit_finalize<<<B, threads, 0, st>>>(scratch, S, nperm, eps, loss_b, perm, pair_sisdr);
-  CTN_COUNT_LAUNCH();
-  CTN_RETURN_IF_CUDA_ERR();
-  if (loss_mean) {
-    k_batch_mean<<<1, 32, 0, st>>>(loss_b, B, loss_mean);
-    CTN_COUNT_LAUNCH();
-    CTN_RETURN_IF_CUDA_ERR();
-  }
-  return CTN_OK;
+  return launch_pit_finalize<SisdrPair>(scratch, B, S, eps, loss_b, perm, loss_mean, pair_sisdr, st);
 }
 
 __global__ void k_sisdr_finalize(const double* __restrict__ scratch, int rows, float eps, float* __restrict__ out) {
@@ -328,6 +347,200 @@ extern "C" int ctn_sdr_fwd(const float* est, const float* tgt, int rows, int T, 
   k_sdr_partial<<<dim3(gx, grid_rows(rows)), 256, 0, st>>>(est, tgt, rows, T, scratch);
   CTN_COUNT_LAUNCH();
   k_sdr_finalize<<<(rows + 127) / 128, 128, 0, st>>>(scratch, rows, eps, out);
+  CTN_COUNT_LAUNCH();
+  CTN_RETURN_IF_CUDA_ERR();
+  return CTN_OK;
+}
+
+// ---- SDR gradient and PIT over SDR -------------------------------------------------------------------------------------------
+// d SDR(x, t) / d x = 20 / (ln 10 (|t - x|^2 + eps)) (t - x): one row coefficient, formed in double from the forward's residual
+// sum, times the fp32 difference.  sdr_row_grad streams one row with 128-bit accesses when all three bases are 16-byte aligned
+// (a view may start anywhere; T need not be a multiple of 4: the tail goes element by element).
+__device__ __forceinline__ void sdr_row_grad(const float* __restrict__ x, const float* __restrict__ t, float* __restrict__ d, int T,
+                                             float c) {
+  const bool vec = ((((uintptr_t)x) | ((uintptr_t)t) | ((uintptr_t)d)) & 15) == 0;
+  const int n4 = vec ? T / 4 : 0;
+  for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n4; i += gridDim.x * blockDim.x) {
+    const float4 a = __ldg(reinterpret_cast<const float4*>(x) + i), b = __ldg(reinterpret_cast<const float4*>(t) + i);
+    reinterpret_cast<float4*>(d)[i] = make_float4(c * (b.x - a.x), c * (b.y - a.y), c * (b.z - a.z), c * (b.w - a.w));
+  }
+  for (int i = n4 * 4 + blockIdx.x * blockDim.x + threadIdx.x; i < T; i += gridDim.x * blockDim.x) d[i] = c * (__ldg(t + i) - __ldg(x + i));
+}
+
+__device__ __forceinline__ float sdr_grad_coef(double ee, double eps, double g) {
+  return (float)(g * 8.685889638065035 / (ee + eps));  // 20 / ln 10
+}
+
+// grid (chunks, min(rows, 65535)), block 256; scratch = ctn_sdr_fwd's (|t|^2, |t - x|^2) per row
+__global__ void __launch_bounds__(256) k_sdr_bwd(const float* __restrict__ est, const float* __restrict__ tgt, int rows, int T, float eps,
+                                                 const double* __restrict__ scratch, const float* __restrict__ g, float coef,
+                                                 float* __restrict__ d_est) {
+  for (int r = blockIdx.y; r < rows; r += gridDim.y) {
+    const float c = sdr_grad_coef(scratch[2 * r + 1], (double)eps, (g ? (double)g[r] : 1.0) * (double)coef);
+    sdr_row_grad(est + (size_t)r * T, tgt + (size_t)r * T, d_est + (size_t)r * T, T, c);
+  }
+}
+
+static int sdr_grad_chunks(int T) {
+  int gx = (T / 4 + 1023) / 1024;
+  if (gx < 1) gx = 1;
+  return gx > 64 ? 64 : gx;
+}
+
+extern "C" int ctn_sdr_bwd(const float* est, const float* tgt, int rows, int T, float eps, const double* fwd_scratch, const float* grad_out,
+                           float coef, float* d_est, ctn_stream_t stream) {
+  LaunchScope scope(est);
+  if (!est || !tgt || !fwd_scratch || !d_est || rows <= 0 || T <= 0) return CTN_EINVAL;
+  k_sdr_bwd<<<dim3(sdr_grad_chunks(T), grid_rows(rows)), 256, 0, (cudaStream_t)stream>>>(est, tgt, rows, T, eps, fwd_scratch, grad_out,
+                                                                                          coef, d_est);
+  CTN_COUNT_LAUNCH();
+  CTN_RETURN_IF_CUDA_ERR();
+  return CTN_OK;
+}
+
+// PIT over SDR.  Scratch per sample (doubles): ee[S*S] = |t_j - x_i|^2 at i*S + j, then tt[S] = |t_j|^2.  One streaming pass forms
+// both with the explicit residual, in fp32 runs of at most four summed in double (k_sdr_partial's arithmetic); the finalize kernel
+// is the SI-SDR PIT's with SdrPair's value.
+__host__ __device__ inline size_t sdr_pit_scratch_per_sample(int S) { return (size_t)(S * S + S); }
+
+struct SdrPair {
+  static __device__ size_t per_sample(int S) { return sdr_pit_scratch_per_sample(S); }
+  static __device__ float value(const double* sc, int S, int p, float eps) {
+    return 10.f * log10f(((float)sc[S * S + p % S] + eps) / ((float)sc[p] + eps));  // k_sdr_finalize's expression
+  }
+};
+
+template <int S>
+__global__ void __launch_bounds__(256) k_sdr_pit_pass(const float* __restrict__ est, const float* __restrict__ tgt, int B, int T,
+                                                      double* __restrict__ scratch) {
+  __shared__ double red[64];
+  for (int b = blockIdx.y; b < B; b += gridDim.y) {
+    const float* eb = est + (size_t)b * S * T;
+    const float* tb = tgt + (size_t)b * S * T;
+    double ee[S][S], tt[S];
+#pragma unroll
+    for (int i = 0; i < S; ++i) { tt[i] = 0.0;
+#pragma unroll
+      for (int j = 0; j < S; ++j) ee[i][j] = 0.0; }
+    // 128-bit loads need every row of the sample 16-byte aligned: T % 4 == 0 and aligned sample bases
+    const bool vec = (T % 4 == 0) && ((((uintptr_t)eb) | ((uintptr_t)tb)) & 15) == 0;
+    const int nvec = vec ? T / 4 : 0;
+    for (int v0 = blockIdx.x * 256 + threadIdx.x; v0 < nvec; v0 += gridDim.x * 256) {
+      float4 e[S], t[S];
+#pragma unroll
+      for (int i = 0; i < S; ++i) {
+        e[i] = __ldg(reinterpret_cast<const float4*>(eb + (size_t)i * T) + v0);
+        t[i] = __ldg(reinterpret_cast<const float4*>(tb + (size_t)i * T) + v0);
+      }
+#pragma unroll
+      for (int j = 0; j < S; ++j) {
+        tt[j] += (double)(fmaf(t[j].x, t[j].x, t[j].y * t[j].y) + fmaf(t[j].z, t[j].z, t[j].w * t[j].w));
+#pragma unroll
+        for (int i = 0; i < S; ++i) {
+          const float d0 = t[j].x - e[i].x, d1 = t[j].y - e[i].y, d2 = t[j].z - e[i].z, d3 = t[j].w - e[i].w;
+          ee[i][j] += (double)(fmaf(d0, d0, d1 * d1) + fmaf(d2, d2, d3 * d3));
+        }
+      }
+    }
+    if (!vec) {
+      for (int k = blockIdx.x * 256 + threadIdx.x; k < T; k += gridDim.x * 256) {
+        float e[S], t[S];
+#pragma unroll
+        for (int i = 0; i < S; ++i) { e[i] = __ldg(eb + (size_t)i * T + k); t[i] = __ldg(tb + (size_t)i * T + k); }
+#pragma unroll
+        for (int j = 0; j < S; ++j) {
+          tt[j] += (double)t[j] * t[j];
+#pragma unroll
+          for (int i = 0; i < S; ++i) {
+            const float d = t[j] - e[i];
+            ee[i][j] += (double)d * d;
+          }
+        }
+      }
+    }
+    double* sc = scratch + (size_t)b * sdr_pit_scratch_per_sample(S);
+#pragma unroll
+    for (int i = 0; i < S; ++i) {
+#pragma unroll
+      for (int j = 0; j < S; j += 2) {
+        double a = ee[i][j], c = (j + 1 < S) ? ee[i][j + 1] : 0.0;
+        block_sum2_d(a, c, red);
+        if (threadIdx.x == 0) {
+          atomicAdd(&sc[i * S + j], a);
+          if (j + 1 < S) atomicAdd(&sc[i * S + j + 1], c);
+        }
+        __syncthreads();
+      }
+    }
+#pragma unroll
+    for (int j = 0; j < S; j += 2) {
+      double a = tt[j], c = (j + 1 < S) ? tt[j + 1] : 0.0;
+      block_sum2_d(a, c, red);
+      if (threadIdx.x == 0) {
+        atomicAdd(&sc[S * S + j], a);
+        if (j + 1 < S) atomicAdd(&sc[S * S + j + 1], c);
+      }
+      __syncthreads();
+    }
+  }
+}
+
+template <int S>
+static int launch_sdr_pit(const float* est, const float* tgt, int B, int T, double* scratch, cudaStream_t st) {
+  int gx = (T / 4 + 255) / 256;
+  if (gx < 1) gx = 1;
+  if (gx > 32) gx = 32;
+  k_sdr_pit_pass<S><<<dim3(gx, grid_rows(B)), 256, 0, st>>>(est, tgt, B, T, scratch);
+  CTN_COUNT_LAUNCH();
+  CTN_RETURN_IF_CUDA_ERR();
+  return CTN_OK;
+}
+
+extern "C" size_t ctn_sdr_pit_scratch_bytes(int B, int S) { return sizeof(double) * (size_t)B * sdr_pit_scratch_per_sample(S); }
+
+extern "C" int ctn_sdr_pit_fwd(const float* est, const float* tgt, int B, int S, int T, float eps, float* loss_b, int64_t* perm,
+                               float* loss_mean, float* pair_sdr, double* scratch, ctn_stream_t stream) {
+  LaunchScope scope(est);
+  if (!est || !tgt || !loss_b || !perm || !scratch || B <= 0 || T <= 0) return CTN_EINVAL;
+  if (S < 1 || S > CTN_MAX_S) return CTN_EUNSUPPORTED;
+  cudaStream_t st = (cudaStream_t)stream;
+  StageTimer tm(CTN_ST_LOSS, st);
+  cudaError_t e = cudaMemsetAsync(scratch, 0, ctn_sdr_pit_scratch_bytes(B, S), st);
+  if (e != cudaSuccess) return (int)e;
+  int rc;
+  switch (S) {
+    case 1: rc = launch_sdr_pit<1>(est, tgt, B, T, scratch, st); break;
+    case 2: rc = launch_sdr_pit<2>(est, tgt, B, T, scratch, st); break;
+    case 3: rc = launch_sdr_pit<3>(est, tgt, B, T, scratch, st); break;
+    case 4: rc = launch_sdr_pit<4>(est, tgt, B, T, scratch, st); break;
+    case 5: rc = launch_sdr_pit<5>(est, tgt, B, T, scratch, st); break;
+    default: rc = launch_sdr_pit<6>(est, tgt, B, T, scratch, st); break;
+  }
+  if (rc) return rc;
+  return launch_pit_finalize<SdrPair>(scratch, B, S, eps, loss_b, perm, loss_mean, pair_sdr, st);
+}
+
+// backward through the selected permutation: row (b, i) reads ee[i][perm[b][i]] from the forward's scratch
+__global__ void __launch_bounds__(256) k_sdr_pit_bwd(const float* __restrict__ est, const float* __restrict__ tgt,
+                                                     const int64_t* __restrict__ perm, const double* __restrict__ scratch,
+                                                     const float* __restrict__ gl, float coef, int B, int S, int T, float eps,
+                                                     float* __restrict__ d_est) {
+  for (int row = blockIdx.y; row < B * S; row += gridDim.y) {
+    const int b = row / S, i = row % S;
+    const int j = (int)perm[(size_t)b * S + i];
+    const double ee = scratch[(size_t)b * sdr_pit_scratch_per_sample(S) + i * S + j];
+    const float c = sdr_grad_coef(ee, (double)eps, (gl ? (double)gl[b] : 1.0) * (double)coef);
+    sdr_row_grad(est + (size_t)row * T, tgt + ((size_t)b * S + j) * T, d_est + (size_t)row * T, T, c);
+  }
+}
+
+extern "C" int ctn_sdr_pit_bwd(const float* est, const float* tgt, const int64_t* perm, int B, int S, int T, float eps,
+                               const double* fwd_scratch, const float* grad_loss_b, float coef, float* d_est, ctn_stream_t stream) {
+  LaunchScope scope(est);
+  if (!est || !tgt || !perm || !fwd_scratch || !d_est || B <= 0 || T <= 0) return CTN_EINVAL;
+  if (S < 1 || S > CTN_MAX_S) return CTN_EUNSUPPORTED;
+  k_sdr_pit_bwd<<<dim3(sdr_grad_chunks(T), grid_rows(B * S)), 256, 0, (cudaStream_t)stream>>>(est, tgt, perm, fwd_scratch, grad_loss_b,
+                                                                                               coef, B, S, T, eps, d_est);
   CTN_COUNT_LAUNCH();
   CTN_RETURN_IF_CUDA_ERR();
   return CTN_OK;

@@ -128,6 +128,10 @@ ctn_encoder_mc_fwd = _sig("ctn_encoder_mc_fwd", _i, _fp, _fp, _fp, _i, _i, _i, _
 ctn_decoder_mc_fwd = _sig("ctn_decoder_mc_fwd", _i, _fp, _fp, _fp, _i, _i, _i, _i, _i, _i, _i, _i, _i, _fp)
 ctn_sdr_fwd = _sig("ctn_sdr_fwd", _i, _fp, _fp, _i, _i, _f, _fp, _fp, _fp)
 ctn_sisdr_pit_bwd = _sig("ctn_sisdr_pit_bwd", _i, _fp, _fp, _fp, _i, _i, _i, _f, _fp, _fp, _f, _fp, _fp)
+ctn_sdr_bwd = _sig("ctn_sdr_bwd", _i, _fp, _fp, _i, _i, _f, _fp, _fp, _f, _fp, _fp)
+ctn_sdr_pit_scratch_bytes = _sig("ctn_sdr_pit_scratch_bytes", _sz, _i, _i)
+ctn_sdr_pit_fwd = _sig("ctn_sdr_pit_fwd", _i, _fp, _fp, _i, _i, _i, _f, _fp, _fp, _fp, _fp, _fp, _fp)
+ctn_sdr_pit_bwd = _sig("ctn_sdr_pit_bwd", _i, _fp, _fp, _fp, _i, _i, _i, _f, _fp, _fp, _f, _fp, _fp)
 ctn_orpit_scratch_bytes = _sig("ctn_orpit_scratch_bytes", _sz, _i, _i)
 ctn_orpit_fwd = _sig("ctn_orpit_fwd", _i, _fp, _fp, _fp, _i, _i, _i, _f, _i, _fp, _fp, _fp, _fp)
 ctn_orpit_bwd = _sig("ctn_orpit_bwd", _i, _fp, _fp, _fp, _fp, _i, _i, _i, _f, _i, _fp, _fp, _fp, _fp)
@@ -192,7 +196,8 @@ EXPORTED = [
     "ctn_decoder_fwd", "ctn_gln_fwd", "ctn_cln_fwd", "ctn_tcn_workspace_bytes", "ctn_tcn_fwd", "ctn_convtasnet_fwd",
     "ctn_separator_fwd", "ctn_sisdr_fwd", "ctn_sisdr_pit_fwd", "ctn_sisdr_pit_scratch_bytes", "ctn_host_io_bytes",
     "ctn_convtasnet_loss_host", "ctn_train_workspace_bytes", "ctn_convtasnet_fwd_train", "ctn_convtasnet_bwd",
-    "ctn_sisdr_pit_bwd", "ctn_sdr_fwd", "ctn_encoder_mc_fwd", "ctn_decoder_mc_fwd", "ctn_last_launch_count", "ctn_total_launch_count", "ctn_profile_enable", "ctn_profile_read",
+    "ctn_sisdr_pit_bwd", "ctn_sdr_fwd", "ctn_sdr_bwd", "ctn_sdr_pit_scratch_bytes", "ctn_sdr_pit_fwd", "ctn_sdr_pit_bwd",
+    "ctn_encoder_mc_fwd", "ctn_decoder_mc_fwd", "ctn_last_launch_count", "ctn_total_launch_count", "ctn_profile_enable", "ctn_profile_read",
     "ctn_segment_fwd", "ctn_overlap_add_fwd", "ctn_dprnn_norm_res_fwd", "ctn_stage_workspace_bytes", "ctn_sep_head_fwd", "ctn_sep_tail_fwd",
     "ctn_clip_adam_chunks", "ctn_clip_adam_step", "ctn_tcn_blocks_fwd",
     "ctn_depthwise_conv1d_fwd", "ctn_pointwise_conv1d_fwd",

@@ -1,39 +1,55 @@
 """Permutation-invariant training, mirroring src/criterion/pit.py: ``pit`` (:9-44), ``PIT`` (:46-69), ``PIT1d``
-(:71-77).  When the criterion is (Neg)SISDR with reduction 'mean'/'sum' on (batch_size, n_sources, T) tensors the whole
-thing is ONE fused call (ctn_sisdr_pit_fwd): the S x S pairwise SI-SDR table is computed in two streaming passes and
-the S! permutations are scored from it (lexicographic order, first minimum).  Any other criterion goes through the
-generic loop of the reference semantics."""
+(:71-77).  When the criterion is (Neg)SISDR or (Neg)SDR with reduction 'mean'/'sum' on (batch_size, n_sources, T) tensors,
+n_sources <= 6, the whole thing is ONE fused call (ctn_sisdr_pit_fwd / ctn_sdr_pit_fwd): the S x S table of pair statistics is
+computed in streaming passes and the S! permutations are scored from it (lexicographic order, first minimum).  Any other
+criterion, or a subset of the permutations, goes through the generic loop of the reference semantics."""
 import itertools
 
 import torch
 import torch.nn as nn
 
 from .. import _native as N
-from .sdr import NegSISDR, SISDR
+from .sdr import NegSDR, NegSISDR, SDR, SISDR
+
+# (forward, backward, scratch bytes) of the fused PIT, by criterion
+_SISDR_PIT = (N.ctn_sisdr_pit_fwd, N.ctn_sisdr_pit_bwd, N.ctn_sisdr_pit_scratch_bytes)
+_SDR_PIT = (N.ctn_sdr_pit_fwd, N.ctn_sdr_pit_bwd, N.ctn_sdr_pit_scratch_bytes)
 
 
 def _fused_ok(criterion, input, target):
-    return (isinstance(criterion, (NegSISDR, SISDR)) and criterion.reduction in ('mean', 'sum') and input.dim() == 3
+    return (isinstance(criterion, (NegSISDR, SISDR, NegSDR, SDR)) and criterion.reduction in ('mean', 'sum') and input.dim() == 3
             and input.shape == target.shape and input.is_cuda and input.size(1) <= 6)
+
+
+def _pit_fwd(kernels, x, t, eps, loss_mean=None):
+    """(loss_b, perm, scratch) of the fused forward: loss_b (B) = min_perm -mean_i criterion(est_i, tgt_perm[i])"""
+    fwd, _, scratch_bytes = kernels
+    dev = N.require_cuda(x, t)
+    B, S, T = x.shape
+    loss_b = torch.empty(B, dtype=torch.float32, device=dev)
+    perm = torch.empty(B, S, dtype=torch.int64, device=dev)
+    scratch = torch.empty(scratch_bytes(B, S) // 8, dtype=torch.float64, device=dev)
+    N.check(fwd(x.data_ptr(), t.data_ptr(), B, S, T, float(eps), loss_b.data_ptr(), perm.data_ptr(), N.ptr(loss_mean), None,
+                scratch.data_ptr(), N.stream_ptr(dev)), fwd.__name__)
+    return loss_b, perm, scratch
+
+
+def _pit_fn_forward(ctx, kernels, x, t, eps):
+    loss_b, perm, scratch = _pit_fwd(kernels, x, t, eps)
+    ctx.save_for_backward(x, t, perm, scratch)
+    ctx.eps, ctx.bwd = float(eps), kernels[1]
+    ctx.mark_non_differentiable(perm)
+    return loss_b, perm
 
 
 class _PitNegSisdrFn(torch.autograd.Function):
     """loss_b (B) = min_perm -mean_i SI-SDR(est_i, tgt_perm[i]) with its gradient w.r.t. the estimate through the selected
     permutation (the indices carry no gradient, pit.py:36-44); ctn_sisdr_pit_fwd / ctn_sisdr_pit_bwd."""
+    kernels = _SISDR_PIT
 
     @staticmethod
     def forward(ctx, x, t, eps):
-        dev = N.require_cuda(x, t)
-        B, S, T = x.shape
-        loss_b = torch.empty(B, dtype=torch.float32, device=dev)
-        perm = torch.empty(B, S, dtype=torch.int64, device=dev)
-        scratch = torch.empty(N.ctn_sisdr_pit_scratch_bytes(B, S) // 8, dtype=torch.float64, device=dev)
-        N.check(N.ctn_sisdr_pit_fwd(x.data_ptr(), t.data_ptr(), B, S, T, float(eps), loss_b.data_ptr(), perm.data_ptr(), None,
-                                    None, scratch.data_ptr(), N.stream_ptr(dev)), "ctn_sisdr_pit_fwd")
-        ctx.save_for_backward(x, t, perm, scratch)
-        ctx.eps = float(eps)
-        ctx.mark_non_differentiable(perm)
-        return loss_b, perm
+        return _pit_fn_forward(ctx, _SISDR_PIT, x, t, eps)
 
     @staticmethod
     def backward(ctx, g_loss_b, _g_perm):
@@ -41,34 +57,36 @@ class _PitNegSisdrFn(torch.autograd.Function):
         B, S, T = x.shape
         g = g_loss_b.contiguous().to(torch.float32)
         d_est = torch.empty_like(x)
-        N.check(N.ctn_sisdr_pit_bwd(x.data_ptr(), t.data_ptr(), perm.data_ptr(), B, S, T, ctx.eps, scratch.data_ptr(),
-                                    g.data_ptr(), -1.0 / S, d_est.data_ptr(), N.stream_ptr(x.device)), "ctn_sisdr_pit_bwd")
+        N.check(ctx.bwd(x.data_ptr(), t.data_ptr(), perm.data_ptr(), B, S, T, ctx.eps, scratch.data_ptr(), g.data_ptr(), -1.0 / S,
+                        d_est.data_ptr(), N.stream_ptr(x.device)), ctx.bwd.__name__)
         return d_est, None, None
+
+
+class _PitNegSdrFn(_PitNegSisdrFn):
+    """loss_b (B) = min_perm -mean_i SDR(est_i, tgt_perm[i]) with its gradient w.r.t. the estimate through the selected
+    permutation; ctn_sdr_pit_fwd / ctn_sdr_pit_bwd."""
+    kernels = _SDR_PIT
+
+    @staticmethod
+    def forward(ctx, x, t, eps):
+        return _pit_fn_forward(ctx, _SDR_PIT, x, t, eps)
 
 
 def _fused(criterion, input, target, batch_mean):
     x, t = input.contiguous(), target.contiguous()
     if torch.is_grad_enabled() and target.requires_grad:
         raise NotImplementedError("gradient w.r.t. the PIT target is not built")
-    if torch.is_grad_enabled() and x.requires_grad:
-        loss_b, perm = _PitNegSisdrFn.apply(x, t, float(criterion.eps))
-        S = x.shape[1]
-        scale = (S if criterion.reduction == 'sum' else 1) * (-1.0 if criterion.maximize else 1.0)
-        loss = loss_b.mean(dim=0) if batch_mean else loss_b
-        if scale != 1:
-            loss = loss * scale
-        return loss, perm
-    dev = N.require_cuda(x, t)
-    B, S, T = x.shape
-    loss_b = torch.empty(B, dtype=torch.float32, device=dev)
-    perm = torch.empty(B, S, dtype=torch.int64, device=dev)
-    loss_mean = torch.empty(1, dtype=torch.float32, device=dev)
-    scratch = torch.empty(N.ctn_sisdr_pit_scratch_bytes(B, S) // 8, dtype=torch.float64, device=dev)
-    N.check(N.ctn_sisdr_pit_fwd(x.data_ptr(), t.data_ptr(), B, S, T, float(criterion.eps), loss_b.data_ptr(), perm.data_ptr(),
-                                loss_mean.data_ptr(), None, scratch.data_ptr(), N.stream_ptr(dev)), "ctn_sisdr_pit_fwd")
-    # the kernel scores -mean_i SI-SDR; SISDR (maximize) = its negation, 'sum' = * S
+    fn = _PitNegSdrFn if isinstance(criterion, (NegSDR, SDR)) else _PitNegSisdrFn
+    S = x.shape[1]
+    # the kernels score -mean_i criterion; a maximised criterion (SISDR, SDR) is its negation, 'sum' = * S
     scale = (S if criterion.reduction == 'sum' else 1) * (-1.0 if criterion.maximize else 1.0)
-    loss = loss_mean[0] if batch_mean else loss_b
+    if torch.is_grad_enabled() and x.requires_grad:
+        loss_b, perm = fn.apply(x, t, float(criterion.eps))
+        loss = loss_b.mean(dim=0) if batch_mean else loss_b
+    else:
+        loss_mean = torch.empty(1, dtype=torch.float32, device=x.device)
+        loss_b, perm, _ = _pit_fwd(fn.kernels, x, t, criterion.eps, loss_mean)
+        loss = loss_mean[0] if batch_mean else loss_b
     if scale != 1:
         loss = loss * scale
     return loss, perm
@@ -79,6 +97,11 @@ def pit(criterion, input, target, n_sources=None, patterns=None, batch_mean=True
     estimate i <-> target pattern[i]."""
     if _fused_ok(criterion, input, target) and (patterns is None or len(patterns) == _nperm(input.size(1))):
         return _fused(criterion, input, target, batch_mean)
+    return _pit_generic(criterion, input, target, n_sources, patterns, batch_mean)
+
+
+def _pit_generic(criterion, input, target, n_sources=None, patterns=None, batch_mean=True):
+    """the reference's loop over the permutations (pit.py:20-44)"""
     if patterns is None:
         if n_sources is None:
             n_sources = input.size(1)

@@ -408,6 +408,25 @@ int ctn_softmax_bwd(const ctn_config_t* cfg, const ctn_params_t* params, const c
 int ctn_sisdr_pit_bwd(const float* est, const float* tgt, const int64_t* perm, int B, int S, int T, float eps,
                       const double* fwd_scratch, const float* grad_loss_b, float coef, float* d_est, ctn_stream_t stream);
 
+/* Backward of ctn_sdr_fwd (src/criterion/sdr.py:6-20): d_est (rows,T) = coef * grad_out[r] * 20 / (ln 10 (|tgt_r - est_r|^2 + eps))
+ * * (tgt_r - est_r), the row coefficient in double from fwd_scratch, the buffer the forward call filled (|t|^2, |t - x|^2 per
+ * row).  grad_out (rows) nullable (= 1).  Any row count, any T; 128-bit accesses where est, tgt and d_est rows are 16-byte aligned. */
+int ctn_sdr_bwd(const float* est, const float* tgt, int rows, int T, float eps, const double* fwd_scratch, const float* grad_out,
+                float coef, float* d_est, ctn_stream_t stream);
+
+/* PIT1d(NegSDR(reduction='mean')), src/criterion/pit.py:9-44 + src/criterion/sdr.py:6-20,72-110.  est,tgt (B,S,T) contiguous.
+ * loss_b (B) = min over permutations of -mean_i SDR(est_i, tgt_perm[i]); perm (B,S) int64 (first minimum on ties, lexicographic
+ * permutation order); loss_mean (1, nullable) = mean over the batch; pair_sdr (nullable) (B,S,S) = SDR(est_i, tgt_j).
+ * One pass forms |t_j|^2 and the explicit residual table |t_j - est_i|^2, then ctn_sisdr_pit_fwd's permutation scoring.
+ * scratch: ctn_sdr_pit_scratch_bytes(B, S) = double[B][S*S + S], zero-initialised by the callee.  S <= 6, any B, any T.
+ * ctn_sdr_pit_bwd: d_est (B,S,T) = grad_loss_b[b] (nullable: 1) * coef * dSDR(est_i, tgt_perm[i])/d est_i from the forward's
+ * scratch and perm; coef = -1/S for NegSDR(reduction='mean'), -1 for 'sum'. */
+size_t ctn_sdr_pit_scratch_bytes(int B, int S);
+int ctn_sdr_pit_fwd(const float* est, const float* tgt, int B, int S, int T, float eps, float* loss_b, int64_t* perm, float* loss_mean,
+                    float* pair_sdr, double* scratch, ctn_stream_t stream);
+int ctn_sdr_pit_bwd(const float* est, const float* tgt, const int64_t* perm, int B, int S, int T, float eps, const double* fwd_scratch,
+                    const float* grad_loss_b, float coef, float* d_est, ctn_stream_t stream);
+
 /* ORPIT(NegSISDR | SISDR), one-and-rest PIT, src/criterion/pit.py:87-160.  est (B,2,T), tgt (B,n,T) contiguous (any T, no
  * alignment needed); n_b (B) int32 device array, nullable (= n for every sample): sample b uses targets 0..n_b[b]-1, each n_b in
  * [2, n] (checked by the caller, the rows past n_b are ignored).  Candidate i scores
