@@ -304,7 +304,8 @@ static int carve_long(Carver& cv, const ctn_config_t* c, int B, const ChunkPlan&
   const int S = c->n_sources;
   const long long chunks = (long long)B * p.K;
   ws->nb = (int)(chunks < chunk_batch ? chunks : chunk_batch);
-  if (ws->nb > 65535) ws->nb = 65535;  // a batch's chunks ride on gridDim.y
+  // a batch's chunks ride on gridDim.y, and the forward's decoder puts their nb * S source rows there
+  if ((long long)ws->nb * S > 65535) ws->nb = 65535 / S;
   CTN_TRY(ctn_workspace_bytes(c, ws->nb, p.Lc, &ws->model_bytes));
   ws->perms = cv.take<int32_t>((size_t)chunks * S);
   ws->partial = nullptr; ws->xc = nullptr; ws->est = nullptr;
@@ -631,7 +632,9 @@ static int carve_track(Carver& cv, const ctn_config_t* c, int B, const TrackPlan
   const int S = c->n_sources, C = track_channels(c);
   const long long chunks = (long long)B * tp.p.K;
   ws->nb = (int)(chunks < chunk_batch ? chunks : chunk_batch);
-  if ((long long)ws->nb * C > 65535) ws->nb = 65535 / C;  // a batch's (chunk, channel) rows ride on gridDim.y
+  // a batch's (chunk, channel) rows ride on gridDim.y, and so do the nb * S source rows of the forward's decoder
+  const int rows = C > S ? C : S;
+  if ((long long)ws->nb * rows > 65535) ws->nb = 65535 / rows;
   CTN_TRY(ctn_workspace_bytes(c, ws->nb, tp.p.Lc, &ws->model_bytes));
   ws->stats = cv.take<double>(track_rows(B, C, tp) * 2);
   ws->partial = cv.take<double>(stats_scratch_bytes(B, C, tp) / sizeof(double));
