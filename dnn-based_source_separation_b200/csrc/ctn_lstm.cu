@@ -94,8 +94,9 @@ __device__ __forceinline__ void mma_slab(float (&acc)[64], uint32_t a_addr, uint
   }
 }
 
-// NCH = H / 32 gate chunks, KSX = F / 32 input slabs
-template <int NCH, int KSX>
+// NCH = H / 32 gate chunks, KSX = F / 32 input slabs.  RELU_PROJ: the projection sees ReLU(h_t) (DPTNet's FeedForwardBlock,
+// dptnet.py:560-562), the recurrence and hout the raw h_t
+template <int NCH, int KSX, bool RELU_PROJ = false>
 __global__ void __launch_bounds__(LTHREADS, 1) k_bilstm(const LstmArgs g) {
   constexpr int H = NCH * 32, F = KSX * 32, KT = KSX + NCH;
   extern __shared__ uint8_t smem_raw[];
@@ -182,7 +183,9 @@ __global__ void __launch_bounds__(LTHREADS, 1) k_bilstm(const LstmArgs g) {
     __syncthreads();
     for (int i = tid; i < LSEQ * H / 4; i += LTHREADS) {
       const int row = i / (H / 4), c4 = i % (H / 4);
-      put4(a_slabs, KSX, row, c4, *reinterpret_cast<const float4*>(hs + row * H + 4 * c4));
+      float4 v = *reinterpret_cast<const float4*>(hs + row * H + 4 * c4);
+      if (RELU_PROJ) v = make_float4(fmaxf(v.x, 0.f), fmaxf(v.y, 0.f), fmaxf(v.z, 0.f), fmaxf(v.w, 0.f));
+      put4(a_slabs, KSX, row, c4, v);
     }
     ptx::fence_proxy_async_smem();
     __syncthreads();
@@ -197,19 +200,25 @@ __global__ void __launch_bounds__(LTHREADS, 1) k_bilstm(const LstmArgs g) {
         if (o < g.Fo && seq < g.NSEQ) g.P[(((size_t)dir * g.NSEQ + seq) * g.T + t) * g.Fo + o] = acc[i];
       }
     }
+    if (RELU_PROJ)  // the next step's gates read the raw h_t: every MMA on the slabs has completed (consume waits and syncs), and
+                    // the next step's operand fence + barrier orders these stores before them
+      for (int i = tid; i < LSEQ * H / 4; i += LTHREADS) {
+        const int row = i / (H / 4), c4 = i % (H / 4);
+        put4(a_slabs, KSX, row, c4, *reinterpret_cast<const float4*>(hs + row * H + 4 * c4));
+      }
   }
 }
 
-template <int NCH, int KSX>
+template <int NCH, int KSX, bool RELU_PROJ>
 int launch_bilstm(const LstmArgs& a, size_t smem, cudaStream_t st) {
   static bool done[CTN_MAX_DEVICES] = {};
   const int dev = ctn_current_device();
   if (!done[dev]) {
-    cudaError_t e = cudaFuncSetAttribute(k_bilstm<NCH, KSX>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_LIMIT);
+    cudaError_t e = cudaFuncSetAttribute(k_bilstm<NCH, KSX, RELU_PROJ>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_LIMIT);
     if (e != cudaSuccess) return (int)e;
     done[dev] = true;
   }
-  k_bilstm<NCH, KSX><<<dim3((a.NSEQ + LSEQ - 1) / LSEQ, 2), LTHREADS, smem, st>>>(a);
+  k_bilstm<NCH, KSX, RELU_PROJ><<<dim3((a.NSEQ + LSEQ - 1) / LSEQ, 2), LTHREADS, smem, st>>>(a);
   return CTN_OK;
 }
 
@@ -309,11 +318,11 @@ extern "C" int ctn_bilstm_supported(int F, int H, int Fo) { return lstm_supporte
 
 extern "C" size_t ctn_bilstm_workspace_bytes(int F, int H, int Fo) { return lstm_supported(F, H, Fo) ? lstm_ws_bytes(F, H, Fo) : 0; }
 
-extern "C" int ctn_bilstm_proj_fwd(const float* z, int NSEQ, int T, int F, int H, const float* const* w, const float* w_fc, int Fo, float* P,
-                                   float* hout, const unsigned* z_absmax, void* workspace, size_t workspace_bytes, ctn_stream_t stream) {
-  LaunchScope scope(z);
-  (void)z_absmax;  // 3xTF32 pieces keep fp32's exponent range: the recurrence needs no operand scale
+namespace {
+int bilstm_proj(const float* z, int NSEQ, int T, int F, int H, const float* const* w, const float* w_fc, int Fo, float* P, float* hout,
+                bool relu_proj, void* workspace, size_t workspace_bytes, cudaStream_t stream) {
   if (!z || !w || !workspace || NSEQ <= 0 || T <= 0) return CTN_EINVAL;
+  if (relu_proj && !w_fc) return CTN_EINVAL;
   for (int i = 0; i < 8; ++i)
     if (!w[i]) return CTN_EINVAL;
   if ((w_fc == nullptr) != (P == nullptr)) return CTN_EINVAL;
@@ -326,7 +335,7 @@ extern "C" int ctn_bilstm_proj_fwd(const float* z, int NSEQ, int T, int F, int H
   int nst = (int)((SMEM_LIMIT - fixed) / SLAB);
   if (nst > MAX_NST) nst = MAX_NST;
   if (nst < 2) return CTN_EUNSUPPORTED;
-  cudaStream_t st = (cudaStream_t)stream;
+  cudaStream_t st = stream;
   uint8_t* ws = static_cast<uint8_t*>(workspace);
   LstmWeights wts;
   for (int i = 0; i < 8; ++i) wts.w[i] = w[i];
@@ -340,7 +349,9 @@ extern "C" int ctn_bilstm_proj_fwd(const float* z, int NSEQ, int T, int F, int H
   const size_t smem = fixed + (size_t)nst * SLAB;
   int rc = CTN_EUNSUPPORTED;
   const int NCH = H / 32, KSX = F / 32;
-#define CTN_LSTM_CASE(nch, ksx) if (NCH == nch && KSX == ksx) rc = launch_bilstm<nch, ksx>(a, smem, st);
+#define CTN_LSTM_CASE(nch, ksx)                                                                       \
+  if (NCH == nch && KSX == ksx)                                                                       \
+    rc = relu_proj ? launch_bilstm<nch, ksx, true>(a, smem, st) : launch_bilstm<nch, ksx, false>(a, smem, st);
   CTN_LSTM_CASE(1, 1) CTN_LSTM_CASE(1, 2) CTN_LSTM_CASE(1, 4) CTN_LSTM_CASE(2, 1) CTN_LSTM_CASE(2, 2) CTN_LSTM_CASE(2, 4)
   CTN_LSTM_CASE(4, 1) CTN_LSTM_CASE(4, 2) CTN_LSTM_CASE(4, 4)
 #undef CTN_LSTM_CASE
@@ -348,6 +359,20 @@ extern "C" int ctn_bilstm_proj_fwd(const float* z, int NSEQ, int T, int F, int H
   CTN_COUNT_LAUNCH();
   CTN_RETURN_IF_CUDA_ERR();
   return CTN_OK;
+}
+}  // namespace
+
+extern "C" int ctn_bilstm_proj_fwd(const float* z, int NSEQ, int T, int F, int H, const float* const* w, const float* w_fc, int Fo, float* P,
+                                   float* hout, const unsigned* z_absmax, void* workspace, size_t workspace_bytes, ctn_stream_t stream) {
+  LaunchScope scope(z);
+  (void)z_absmax;  // 3xTF32 pieces keep fp32's exponent range: the recurrence needs no operand scale
+  return bilstm_proj(z, NSEQ, T, F, H, w, w_fc, Fo, P, hout, false, workspace, workspace_bytes, (cudaStream_t)stream);
+}
+
+extern "C" int ctn_bilstm_relu_proj_fwd(const float* z, int NSEQ, int T, int F, int H, const float* const* w, const float* w_fc, int Fo,
+                                        float* P, float* hout, void* workspace, size_t workspace_bytes, ctn_stream_t stream) {
+  LaunchScope scope(z);
+  return bilstm_proj(z, NSEQ, T, F, H, w, w_fc, Fo, P, hout, true, workspace, workspace_bytes, (cudaStream_t)stream);
 }
 
 extern "C" int ctn_dprnn_norm_res2_fwd(const float* P, const float* fc_bias, const float* R, const float* gamma, const float* beta,

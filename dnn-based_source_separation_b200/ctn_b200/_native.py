@@ -152,6 +152,17 @@ ctn_stage_workspace_bytes = _sig("ctn_stage_workspace_bytes", _sz, _i, _i)
 ctn_sep_head_fwd = _sig("ctn_sep_head_fwd", _i, _fp, _fp, _fp, _fp, _fp, _fp, _fp, _i, _i, _i, _i, _i, _f, _i, _fp, _sz, _fp)
 ctn_sep_tail_fwd = _sig("ctn_sep_tail_fwd", _i, _fp, _fp, _fp, _fp, _fp, _fp, _fp, _fp, _fp, _i, _i, _i, _i, _i, _i, _i, _i, _i, _i, _i,
                         _fp, _sz, _fp)
+# DPTNet path: ReLU-projection bi-LSTM, multi-head self-attention, per-sequence gLN, separator head and tail
+ctn_bilstm_relu_proj_fwd = _sig("ctn_bilstm_relu_proj_fwd", _i, _fp, _i, _i, _i, _i, C.POINTER(_fp), _fp, _i, _fp, _fp, _fp, _sz, _fp)
+ctn_mha_supported = _sig("ctn_mha_supported", _i, _i, _i)
+ctn_mha_workspace_bytes = _sig("ctn_mha_workspace_bytes", _sz, _i, _i, _i)
+ctn_mha_fwd = _sig("ctn_mha_fwd", _i, _fp, _i, _i, _i, _i, _fp, _fp, _fp, _fp, _fp, _fp, _sz, _fp)
+ctn_seq_norm_fwd = _sig("ctn_seq_norm_fwd", _i, _fp, _fp, _fp, _fp, _fp, _fp, _fp, _i, _i, _i, _i, _f, _i, _fp)
+ctn_dpt_head_workspace_bytes = _sig("ctn_dpt_head_workspace_bytes", _sz, _i, _i, _i, _i, _i, _i)
+ctn_dpt_head_fwd = _sig("ctn_dpt_head_fwd", _i, _fp, _fp, _fp, _fp, _fp, _fp, _i, _i, _i, _i, _i, _i, _i, _i, _i, _f, _i, _fp, _sz, _fp)
+ctn_dpt_tail_workspace_bytes = _sig("ctn_dpt_tail_workspace_bytes", _sz, _i, _i, _i, _i, _i)
+ctn_dpt_tail_fwd = _sig("ctn_dpt_tail_fwd", _i, _fp, _fp, _fp, _fp, _fp, _fp, _fp, _fp, _fp, _fp, _fp, _fp, _fp, _i, _i, _i, _i, _i, _i, _i,
+                        _i, _i, _i, _i, _i, _fp, _sz, _fp)
 ctn_clip_adam_chunks = _sig("ctn_clip_adam_chunks", _i, C.POINTER(_i), _i, C.POINTER(_i), C.POINTER(_i), _i)
 ctn_clip_adam_step = _sig("ctn_clip_adam_step", _i, _fp, _i, _fp, _fp, _fp, _i, _fp, _sz, _fp, _fp, _fp, _fp, _fp, _f, _f, _f, _f, _f, _fp, _fp)
 ctn_depthwise_conv1d_fwd = _sig("ctn_depthwise_conv1d_fwd", _i, _fp, _fp, _fp, _fp, _i, _i, _i, _i, _i, _i, _i, _i, _fp)
@@ -212,6 +223,8 @@ EXPORTED = [
     "ctn_multichannel_train_workspace_bytes", "ctn_multichannel_fwd_train", "ctn_multichannel_bwd",
     "ctn_softmax_train_workspace_bytes", "ctn_softmax_fwd_train", "ctn_softmax_bwd",
     "ctn_bss_workspace_bytes", "ctn_bss_eval_sources", "ctn_bss_images_workspace_bytes", "ctn_bss_eval_images",
+    "ctn_bilstm_relu_proj_fwd", "ctn_mha_supported", "ctn_mha_workspace_bytes", "ctn_mha_fwd", "ctn_seq_norm_fwd",
+    "ctn_dpt_head_workspace_bytes", "ctn_dpt_head_fwd", "ctn_dpt_tail_workspace_bytes", "ctn_dpt_tail_fwd",
 ]
 
 

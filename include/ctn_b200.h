@@ -301,6 +301,43 @@ int ctn_bilstm_proj_fwd(const float* z, int NSEQ, int T, int F, int H, const flo
  * out_absmax (nullable): receives the bit pattern of max|out| -- the z_absmax of the next ctn_bilstm_proj_fwd. */
 int ctn_dprnn_norm_res2_fwd(const float* P, const float* fc_bias, const float* R, const float* gamma, const float* beta, float* out,
                             int B, int D1, int D2, int F, float eps, int swap, double* scratch, unsigned* out_absmax, ctn_stream_t stream);
+/* ---- DPTNet path: the dual-path transformer (src/models/dptnet.py) ----
+ *
+ * ctn_bilstm_proj_fwd with w_fc required and ReLU applied to the projection's operand only: P = W_fc ReLU(h) per direction (the
+ * ReLU between the LSTM and the Linear of FeedForwardBlock, dptnet.py:560-562); the recurrence and hout use the raw h. */
+int ctn_bilstm_relu_proj_fwd(const float* z, int NSEQ, int T, int F, int H, const float* const* w, const float* w_fc, int Fo, float* P,
+                             float* hout, void* workspace, size_t workspace_bytes, ctn_stream_t stream);
+/* nn.MultiheadAttention(F, heads)(z, z, z) without mask (dptnet.py:512), on channels-last sequences: z (NSEQ,T,F) -> y (NSEQ,T,F) =
+ * out_proj(attention) + out_b, no residual.  in_w (3F,F), in_b (3F), out_w (F,F), out_b (F); scale 1/sqrt(F/heads).  fp32 FMAs, keys
+ * streamed through an online softmax: any T.  Envelope (ctn_mha_supported): F <= 128, F % 4 == 0, F/heads in {8,16,32,64};
+ * NSEQ <= 65535.  workspace >= ctn_mha_workspace_bytes(NSEQ,T,F), 256-byte aligned.  3 launches. */
+int ctn_mha_supported(int F, int heads);
+size_t ctn_mha_workspace_bytes(int NSEQ, int T, int F);
+int ctn_mha_fwd(const float* z, int NSEQ, int T, int F, int heads, const float* in_w, const float* in_b, const float* out_w,
+                const float* out_b, float* y, void* workspace, size_t workspace_bytes, ctn_stream_t stream);
+/* The norm of MultiheadAttentionBlock / FeedForwardBlock (dptnet.py:513-521 / 563-568): x = Y0 + Y1 + bias[f] + R (Y1, bias, R
+ * nullable; all (B,D1,D2,F) channels-last), out = GroupNorm(1,F) of each SEQUENCE, i.e. each (b, d1) row of D2*F values, with
+ * gamma, beta (F).  swap = 1 stores out as (B,D2,D1,F) and then must not alias an input.  The statistics are summed in double in a
+ * fixed order: repeated calls give the same bits.  1 launch. */
+int ctn_seq_norm_fwd(const float* Y0, const float* Y1, const float* bias, const float* R, const float* gamma, const float* beta,
+                     float* out, int B, int D1, int D2, int F, float eps, int swap, ctn_stream_t stream);
+/* Separator head, dptnet.py:334-337: z (B,S,chunk,Bc) = gLN(Segment1d(pad(Wb w + bb))) with the gLN per sample over the segmented
+ * tensor (overlap duplicates and padding zeros included).  w (B,N,pitch) pitched, 16-byte aligned; S = (frames + pad_left +
+ * pad_right - chunk) / hop + 1.  The 1x1 follows ctn_pw's numeric mode `math`.  workspace >= ctn_dpt_head_workspace_bytes(B, N, Bc,
+ * pitch, S, chunk), 256-byte aligned.  Every refusal comes before the first launch. */
+size_t ctn_dpt_head_workspace_bytes(int B, int N, int Bc, int pitch, int S, int chunk_size);
+int ctn_dpt_head_fwd(const float* w, const float* bn_w, const float* bn_b, const float* norm_g, const float* norm_b, float* z, int B,
+                     int N, int Bc, int frames, int pitch, int chunk_size, int hop_size, int pad_left, int pad_right, float eps, int math,
+                     void* workspace, size_t workspace_bytes, ctn_stream_t stream);
+/* Separator tail + decoder, dptnet.py:341-346 and 136-143: PReLU -> map 1x1 (Bc -> S*N) -> GTU1d per source (tanh(map) *
+ * sigmoid(map_gate), N -> N, gtu.py:37-42) -> ReLU (mask_relu = 1) or sigmoid -> w * mask -> ConvTranspose1d -> crop.
+ * y (B,Bc,pitch), w (B,N,pitch); out (B,S,T); latent nullable (B,S,N,frames); what (B,S*N,pitch) scratch; B*S <= 65535.
+ * workspace >= ctn_dpt_tail_workspace_bytes(B,N,Bc,S,pitch), 256-byte aligned.  Every refusal comes before the first launch. */
+size_t ctn_dpt_tail_workspace_bytes(int B, int N, int Bc, int S, int pitch);
+int ctn_dpt_tail_fwd(const float* y, const float* w, const float* prelu, const float* map_w, const float* map_b, const float* gtu_w,
+                     const float* gtu_b, const float* gate_w, const float* gate_b, const float* dec_w, float* out, float* latent, float* what,
+                     int B, int N, int Bc, int S, int frames, int pitch, int L, int stride, int crop_left, int T, int mask_relu, int math,
+                     void* workspace, size_t workspace_bytes, ctn_stream_t stream);
 /* Separator head on the padded layout, src/models/conv_tasnet.py:370-371 == src/models/dprnn_tasnet.py:335-336:
  * x0 (B,Bc,pitch) = Wb gLN(w) + bb; w (B,N,pitch), stats0 double[B][2] = (sum, sumsq) of w (as ctn_encoder_fwd leaves them).
  * workspace >= ctn_stage_workspace_bytes(Bc, N), 256-byte aligned; w and x0 16-byte aligned.  Every refusal comes before the first launch. */
