@@ -163,6 +163,20 @@ ctn_dpt_head_fwd = _sig("ctn_dpt_head_fwd", _i, _fp, _fp, _fp, _fp, _fp, _fp, _i
 ctn_dpt_tail_workspace_bytes = _sig("ctn_dpt_tail_workspace_bytes", _sz, _i, _i, _i, _i, _i)
 ctn_dpt_tail_fwd = _sig("ctn_dpt_tail_fwd", _i, _fp, _fp, _fp, _fp, _fp, _fp, _fp, _fp, _fp, _fp, _fp, _fp, _fp, _i, _i, _i, _i, _i, _i, _i,
                         _i, _i, _i, _i, _i, _fp, _sz, _fp)
+# SepFormer path: pitched channel-first dual-path state, strided attention, token LayerNorm, per-sequence gLN + residual, encoder, tail
+ctn_sfm_segment_fwd = _sig("ctn_sfm_segment_fwd", _i, _fp, _fp, _i, _i, _i, _i, _i, _i, _i, _i, _i, _fp)
+ctn_sfm_overlap_add_fwd = _sig("ctn_sfm_overlap_add_fwd", _i, _fp, _fp, _i, _i, _i, _i, _i, _i, _i, _i, _i, _fp)
+ctn_sfm_attn_supported = _sig("ctn_sfm_attn_supported", _i, _i, _i)
+ctn_sfm_attn_fwd = _sig("ctn_sfm_attn_fwd", _i, _fp, _fp, _fp, _i, _i, _i, _i, _i, _i, _i, _fp)
+ctn_sfm_token_ln_fwd = _sig("ctn_sfm_token_ln_fwd", _i, _fp, _fp, _fp, _fp, _fp, _fp, _i, _i, _i, _i, _f, _fp)
+ctn_sfm_seq_norm_res_fwd = _sig("ctn_sfm_seq_norm_res_fwd", _i, _fp, _fp, _fp, _fp, _fp, _i, _i, _i, _i, _i, _i, _f, _fp)
+ctn_sfm_pos_enc_fwd = _sig("ctn_sfm_pos_enc_fwd", _i, _fp, _fp, _fp, _i, _i, _i, _i, _i, _i, _fp)
+ctn_sfm_transformer_workspace_bytes = _sig("ctn_sfm_transformer_workspace_bytes", _sz, _i, _i, _i, _i, _i, _i)
+ctn_sfm_transformer_fwd = _sig("ctn_sfm_transformer_fwd", _i, _fp, _fp, C.POINTER(_fp), _i, _i, _i, _i, _i, _i, _i, _i, _i, _f, _i, _fp,
+                               _sz, _fp)
+ctn_sfm_tail_workspace_bytes = _sig("ctn_sfm_tail_workspace_bytes", _sz, _i, _i, _i, _i, _i)
+ctn_sfm_tail_fwd = _sig("ctn_sfm_tail_fwd", _i, _fp, _fp, _fp, _fp, _fp, _fp, _fp, _fp, _fp, _fp, _fp, _fp, _fp, _fp, _fp, _i, _i, _i, _i,
+                        _i, _i, _i, _i, _i, _i, _i, _i, _fp, _sz, _fp)
 ctn_clip_adam_chunks = _sig("ctn_clip_adam_chunks", _i, C.POINTER(_i), _i, C.POINTER(_i), C.POINTER(_i), _i)
 ctn_clip_adam_step = _sig("ctn_clip_adam_step", _i, _fp, _i, _fp, _fp, _fp, _i, _fp, _sz, _fp, _fp, _fp, _fp, _fp, _f, _f, _f, _f, _f, _fp, _fp)
 ctn_depthwise_conv1d_fwd = _sig("ctn_depthwise_conv1d_fwd", _i, _fp, _fp, _fp, _fp, _i, _i, _i, _i, _i, _i, _i, _i, _fp)
@@ -225,6 +239,9 @@ EXPORTED = [
     "ctn_bss_workspace_bytes", "ctn_bss_eval_sources", "ctn_bss_images_workspace_bytes", "ctn_bss_eval_images",
     "ctn_bilstm_relu_proj_fwd", "ctn_mha_supported", "ctn_mha_workspace_bytes", "ctn_mha_fwd", "ctn_seq_norm_fwd",
     "ctn_dpt_head_workspace_bytes", "ctn_dpt_head_fwd", "ctn_dpt_tail_workspace_bytes", "ctn_dpt_tail_fwd",
+    "ctn_sfm_segment_fwd", "ctn_sfm_overlap_add_fwd", "ctn_sfm_attn_supported", "ctn_sfm_attn_fwd", "ctn_sfm_token_ln_fwd",
+    "ctn_sfm_seq_norm_res_fwd", "ctn_sfm_pos_enc_fwd", "ctn_sfm_transformer_workspace_bytes", "ctn_sfm_transformer_fwd",
+    "ctn_sfm_tail_workspace_bytes", "ctn_sfm_tail_fwd",
 ]
 
 

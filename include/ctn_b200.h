@@ -353,6 +353,63 @@ int ctn_sep_tail_fwd(const float* y, const float* w, const float* prelu, const f
                      const float* dec_w, float* out, float* latent, float* what, int B, int N, int Bc, int S, int frames, int pitch,
                      int L, int stride, int crop_left, int T, int math, void* workspace, size_t workspace_bytes, ctn_stream_t stream);
 
+/* ---- SepFormer path: the dual-path transformer of src/models/sepformer.py (csrc/ctn_sepformer.cu) ----
+ *
+ * The dual-path state is channel-first and pitched: X (B,F,pitch), token s*C + k for chunk s < S and frame k < C, pitch >= S*C
+ * (ctn_pitch(S*C) in the model); columns [S*C, pitch) are zero wherever these entries write the state.  intra = 1 selects the
+ * sequences of IntraTransformer (the C tokens of one chunk), intra = 0 those of InterTransformer (the S tokens of one frame, C apart).
+ * Every entry refuses before its first launch and is CUDA-graph capturable.
+ *
+ * Segment1d / OverlapAdd1d on that layout (sepformer.py:348-352): Z (B,F,z_pitch), Z[b][f][s*C + k] = the zero-padded x at frame
+ * s*hop + k - pad_left, columns [S*C, z_pitch) = 0; the overlap-add sums the chunks covering frame t + crop_left in ascending s into
+ * y (B,F,out_pitch), columns [T_out, out_pitch) = 0.  1 launch each. */
+int ctn_sfm_segment_fwd(const float* x, float* Z, int B, int F, int frames, int pitch, int chunk_size, int hop_size, int pad_left,
+                        int pad_right, int z_pitch, ctn_stream_t stream);
+int ctn_sfm_overlap_add_fwd(const float* Z, float* y, int B, int F, int S, int chunk_size, int hop_size, int z_pitch, int crop_left,
+                            int T_out, int out_pitch, ctn_stream_t stream);
+/* Scaled dot-product attention of nn.MultiheadAttention(F, heads) over every sequence of the path: qkv (B,3F,pitch) = the
+ * in-projection WITHOUT its bias (as ctn_pw leaves it, channel-first), in_b (3F) added on load; O (B,F,pitch) receives the
+ * concatenated heads before out_proj; its columns outside the sequences are not written.  Scale 1/sqrt(F/heads), online softmax
+ * over 64-key tiles (any length), fp32 FMAs.  Envelope (ctn_sfm_attn_supported): F/heads in {8,16,32,64}.  1 launch. */
+int ctn_sfm_attn_supported(int F, int heads);
+int ctn_sfm_attn_fwd(const float* qkv, const float* in_b, float* O, int B, int F, int heads, int S, int C, int pitch, int intra,
+                     ctn_stream_t stream);
+/* The post-norm LayerNorm of nn.TransformerEncoderLayer: out = LayerNorm_F(X + (Y + bias); gamma, beta, eps) per token (column) of
+ * (B,F,pitch) tensors, statistics in double (mean, then the centred variance).  Y, bias nullable; out may alias X (not Y).  Columns
+ * [ntok, pitch) of out = 0.  1 launch. */
+int ctn_sfm_token_ln_fwd(const float* X, const float* Y, const float* bias, const float* gamma, const float* beta, float* out, int B,
+                         int F, int ntok, int pitch, float eps, ctn_stream_t stream);
+/* The end of IntraTransformer / InterTransformer (sepformer.py:473-476 / 515-518): out = GroupNorm(1,F) of each SEQUENCE of X (its F x
+ * len values; gamma, beta per feature) + R, R the block input without the positional encoding.  Summed in double in a fixed order,
+ * no atomics: repeated calls give the same bits.  out may alias R, not X.  1 launch. */
+int ctn_sfm_seq_norm_res_fwd(const float* X, const float* R, const float* gamma, const float* beta, float* out, int B, int F, int S,
+                             int C, int pitch, int intra, float eps, ctn_stream_t stream);
+/* The encoder input of sepformer.py:471-472: out = X + (X + pe[p]) with p the token's position in its sequence (PositionalEncoding
+ * returns input + encoding and the caller adds the input again).  pe = the module's (5000,1,F) buffer, read as it is.  1 launch. */
+int ctn_sfm_pos_enc_fwd(const float* X, const float* pe, float* out, int B, int F, int S, int C, int pitch, int intra, ctn_stream_t stream);
+/* One IntraTransformer (intra = 1) or InterTransformer (intra = 0): positional encoding, `layers` post-norm ReLU encoder layers
+ * (heads, d_ff, LayerNorm eps) and the final per-sequence gLN + residual.  X, out (B,F,pitch), distinct, X 16-byte aligned.
+ * w: host array of 12*layers + 3 device pointers: per layer in_proj_weight (3F,F), in_proj_bias, out_proj.weight (F,F),
+ * out_proj.bias, linear1.weight (d_ff,F), linear1.bias, linear2.weight (F,d_ff), linear2.bias, norm1.weight, norm1.bias,
+ * norm2.weight, norm2.bias; then the positional-encoding buffer and the final gLN's weight and bias.  The four contractions of a
+ * layer run through ctn_pw in the numeric mode `math`; every weight image of the call is built in one batch first.  Sequences
+ * longer than 5000 tokens: CTN_EINVAL.  workspace >= ctn_sfm_transformer_workspace_bytes(), 256-byte aligned.
+ * Launches: 7*layers + 2, plus ceil(4*layers / 48) weight-image launches outside the fp32 mode. */
+size_t ctn_sfm_transformer_workspace_bytes(int B, int F, int d_ff, int layers, int pitch, int math);
+int ctn_sfm_transformer_fwd(const float* X, float* out, const float* const* w, int B, int F, int heads, int d_ff, int layers, int S, int C,
+                            int pitch, int intra, float eps, int math, void* workspace, size_t workspace_bytes, ctn_stream_t stream);
+/* Separator tail + decoder, sepformer.py:353-359 and 142-155: PReLU -> map 1x1 (Bc -> S*N) -> GTU1d per source -> bottleneck_conv1d_out
+ * (N -> N, bias) -> ReLU (mask_relu = 1) or sigmoid -> w * mask -> ConvTranspose1d -> crop.  y (B,Bc,pitch), w (B,N,pitch);
+ * out (B,S,T); latent nullable (B,S,N,frames); what (B,S*N,pitch) scratch; B*S <= 65535.  The three weight images are built in one
+ * batch.  workspace >= ctn_sfm_tail_workspace_bytes(B,N,Bc,S,pitch), 256-byte aligned.  Launches: 6 + the decoder's (+ 1 weight-image
+ * launch outside the fp32 mode, + 1 with latent). */
+size_t ctn_sfm_tail_workspace_bytes(int B, int N, int Bc, int S, int pitch);
+int ctn_sfm_tail_fwd(const float* y, const float* w, const float* prelu, const float* map_w, const float* map_b, const float* gtu_w,
+                     const float* gtu_b, const float* gate_w, const float* gate_b, const float* bout_w, const float* bout_b,
+                     const float* dec_w, float* out, float* latent, float* what, int B, int N, int Bc, int S, int frames, int pitch, int L,
+                     int stride, int crop_left, int T, int mask_relu, int math, void* workspace, size_t workspace_bytes,
+                     ctn_stream_t stream);
+
 /* modules.conv.DepthwiseSeparableConv1d.forward, src/modules/conv.py:24-28 (not on Conv-TasNet's path; API completeness).
  * Depthwise stage: x (B,C,T) contiguous, w (C,1,K), bias nullable -> y (B,C,y_pitch) with T_out = (T + 2 padding - dilation (K-1) - 1)
  * / stride + 1 valid columns, the rest zero.  Pointwise stage: x (B,K,pitch) padded layout with `frames` valid columns, W (M,K,1),
