@@ -177,6 +177,18 @@ ctn_sfm_transformer_fwd = _sig("ctn_sfm_transformer_fwd", _i, _fp, _fp, C.POINTE
 ctn_sfm_tail_workspace_bytes = _sig("ctn_sfm_tail_workspace_bytes", _sz, _i, _i, _i, _i, _i)
 ctn_sfm_tail_fwd = _sig("ctn_sfm_tail_fwd", _i, _fp, _fp, _fp, _fp, _fp, _fp, _fp, _fp, _fp, _fp, _fp, _fp, _fp, _fp, _fp, _i, _i, _i, _i,
                         _i, _i, _i, _i, _i, _i, _i, _i, _fp, _sz, _fp)
+# LSTM-TasNet: gated encoder + frame norm, the persistent (bi-)LSTM layer, and the fc / mask / decoder tail
+ctn_tas_enc_gated_fwd = _sig("ctn_tas_enc_gated_fwd", _i, _fp, _fp, _fp, _fp, _fp, _fp, _fp, _fp, _i, _i, _i, _i, _i, _i, _i, _i, _f, _f,
+                             _fp)
+ctn_tas_frame_norm_fwd = _sig("ctn_tas_frame_norm_fwd", _i, _fp, _fp, _fp, _fp, _i, _i, _i, _i, _f, _fp)
+ctn_tas_lstm_max_hidden = _sig("ctn_tas_lstm_max_hidden", _i, _i)
+ctn_tas_lstm_supported = _sig("ctn_tas_lstm_supported", _i, _i, _i, _i)
+ctn_tas_lstm_group = _sig("ctn_tas_lstm_group", _i, _i, _i)
+ctn_tas_lstm_workspace_bytes = _sig("ctn_tas_lstm_workspace_bytes", _sz, _i, _i, _i, _i, _i, _i)
+ctn_tas_lstm_fwd = _sig("ctn_tas_lstm_fwd", _i, _fp, C.POINTER(_fp), _fp, _fp, _fp, _i, _i, _i, _i, _i, _i, _i, _fp, _sz, _fp)
+ctn_tas_tail_workspace_bytes = _sig("ctn_tas_tail_workspace_bytes", _sz, _i, _i, _i, _i)
+ctn_tas_tail_fwd = _sig("ctn_tas_tail_fwd", _i, _fp, _fp, _fp, _fp, _fp, _fp, _fp, _fp, _i, _i, _i, _i, _i, _i, _i, _i, _i, _i, _i, _i,
+                        _fp, _sz, _fp)
 ctn_clip_adam_chunks = _sig("ctn_clip_adam_chunks", _i, C.POINTER(_i), _i, C.POINTER(_i), C.POINTER(_i), _i)
 ctn_clip_adam_step = _sig("ctn_clip_adam_step", _i, _fp, _i, _fp, _fp, _fp, _i, _fp, _sz, _fp, _fp, _fp, _fp, _fp, _f, _f, _f, _f, _f, _fp, _fp)
 ctn_depthwise_conv1d_fwd = _sig("ctn_depthwise_conv1d_fwd", _i, _fp, _fp, _fp, _fp, _i, _i, _i, _i, _i, _i, _i, _i, _fp)
@@ -242,6 +254,8 @@ EXPORTED = [
     "ctn_sfm_segment_fwd", "ctn_sfm_overlap_add_fwd", "ctn_sfm_attn_supported", "ctn_sfm_attn_fwd", "ctn_sfm_token_ln_fwd",
     "ctn_sfm_seq_norm_res_fwd", "ctn_sfm_pos_enc_fwd", "ctn_sfm_transformer_workspace_bytes", "ctn_sfm_transformer_fwd",
     "ctn_sfm_tail_workspace_bytes", "ctn_sfm_tail_fwd",
+    "ctn_tas_enc_gated_fwd", "ctn_tas_frame_norm_fwd", "ctn_tas_lstm_max_hidden", "ctn_tas_lstm_supported", "ctn_tas_lstm_group",
+    "ctn_tas_lstm_workspace_bytes", "ctn_tas_lstm_fwd", "ctn_tas_tail_workspace_bytes", "ctn_tas_tail_fwd",
 ]
 
 

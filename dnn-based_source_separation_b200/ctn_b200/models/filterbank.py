@@ -87,3 +87,44 @@ class Decoder(nn.Module):
 
     def get_basis(self):
         return self.conv_transpose1d.weight
+
+
+class GatedEncoder(nn.Module):
+    """GatedEncoder of the reference (src/models/filterbank.py:325-346): ReLU(U x~) * sigmoid(V x~), x~ = x / (||x||_2 + eps) with the
+    norm over the whole signal of each sample.  conv1d_U / conv1d_V are parameter containers; the arithmetic runs in
+    ctn_tas_enc_gated_fwd (csrc/ctn_tasnet.cu), which LSTM-TasNet calls fused with its frame norm.  Monaural input only."""
+
+    def __init__(self, in_channels, n_basis, kernel_size=16, stride=8, eps=1e-12):
+        super().__init__()
+        self.in_channels, self.n_basis = in_channels, n_basis
+        self.kernel_size, self.stride = kernel_size, stride
+        self.eps = eps
+        self.conv1d_U = nn.Conv1d(in_channels, n_basis, kernel_size=kernel_size, stride=stride, bias=False)
+        self.conv1d_V = nn.Conv1d(in_channels, n_basis, kernel_size=kernel_size, stride=stride, bias=False)
+        self.relu = nn.ReLU()
+        self.sigmoid = nn.Sigmoid()
+
+    def forward(self, input):
+        """input (batch_size, 1, T) -> (batch_size, n_basis, (T - kernel_size) // stride + 1)"""
+        if input.dim() != 3 or input.size(1) != self.in_channels:
+            raise ValueError("input.size() is expected (?, {}, ?), but given {}".format(self.in_channels, tuple(input.size())))
+        if self.in_channels != 1:
+            raise NotImplementedError("the multichannel gated encoder is outside the sm_90a path")
+        if torch.is_grad_enabled() and (input.requires_grad or self.conv1d_U.weight.requires_grad):
+            raise NotImplementedError("the gated encoder is forward only: call under torch.no_grad()")
+        x = input.contiguous()
+        dev = N.require_cuda(x, self.conv1d_U.weight, self.conv1d_V.weight)
+        B, _, T = x.shape
+        L, S = self.kernel_size, self.stride
+        if T < L:
+            raise ValueError("input is shorter than the kernel")
+        frames = (T - L) // S + 1
+        pitch = N.ctn_pitch(frames)
+        w = torch.empty(B, self.n_basis, pitch, dtype=torch.float32, device=dev)
+        xn = torch.empty_like(w)  # the frame norm the kernel also forms, unused here
+        nrm = torch.empty(B, dtype=torch.float64, device=dev)
+        ones = torch.ones(self.n_basis, dtype=torch.float32, device=dev)
+        N.check(N.ctn_tas_enc_gated_fwd(x.data_ptr(), self.conv1d_U.weight.data_ptr(), self.conv1d_V.weight.data_ptr(), ones.data_ptr(),
+                                        ones.data_ptr(), w.data_ptr(), xn.data_ptr(), nrm.data_ptr(), B, T, 0, 0, self.n_basis,
+                                        L, S, pitch, float(self.eps), 1.0, N.stream_ptr(dev)), "ctn_tas_enc_gated_fwd")
+        return w[:, :, :frames].contiguous()

@@ -410,6 +410,45 @@ int ctn_sfm_tail_fwd(const float* y, const float* w, const float* prelu, const f
                      int stride, int crop_left, int T, int mask_relu, int math, void* workspace, size_t workspace_bytes,
                      ctn_stream_t stream);
 
+/* ---- LSTM-TasNet path (src/models/tasnet.py, csrc/ctn_tasnet.cu) ----
+ *
+ * GatedEncoder (filterbank.py:325-346) + the Separator's frame norm (tasnet.py:356-359): x (B,1,T) -> w (B,N,pitch) =
+ * ReLU(U x~) * sigmoid(V x~) with x~ = x / (||x||_2 + enc_eps), the norm over the whole padded signal of each sample (nrm: double[B]
+ * scratch), and xn (B,N,pitch) = gamma (w - mean) / (sqrt(var) + eps) + beta over the N channels of each frame, mean and centred
+ * variance in double (an all-zero frame gives exactly beta).  u_w, v_w (N,1,L); virtual zero padding pad_left / pad_right, frames =
+ * (T + pad_left + pad_right - L) / stride + 1 (a ragged tail makes no frame but counts in the norm); columns [frames, pitch) of w and xn are 0.  2 launches.
+ * ctn_tas_frame_norm_fwd: the frame norm alone, w (B,N,pitch) -> xn (as ctn_encoder_fwd leaves w for the plain Encoder).  1 launch. */
+int ctn_tas_enc_gated_fwd(const float* x, const float* u_w, const float* v_w, const float* gamma, const float* beta, float* w, float* xn,
+                          double* nrm, int B, int T, int pad_left, int pad_right, int N, int L, int stride, int pitch, float enc_eps,
+                          float eps, ctn_stream_t stream);
+int ctn_tas_frame_norm_fwd(const float* w, const float* gamma, const float* beta, float* xn, int B, int N, int frames, int pitch,
+                           float eps, ctn_stream_t stream);
+/* One nn.LSTM layer (batch_first, bidirectional when dirs = 2) on the channel-first layout: x (B,F,pitch) -> out (B,dirs*H,pitch),
+ * forward direction in rows [0,H), reverse in [H,2H) (torch's concat order), zero initial state, gate order i,f,g,o.
+ * w[4*dirs] = host array of device pointers in torch order: weight_ih_l{k} (4H,F), weight_hh_l{k} (4H,H), bias_ih_l{k}, bias_hh_l{k}
+ * (4H), then the *_reverse tensors.  skip_in / skip_out (both or neither, (B,dirs*H,pitch)): skip_out = out + skip_in, in place
+ * allowed.  The input projections of both directions are one ctn_pw contraction in the numeric mode `math`; the recurrence is one
+ * cooperative launch whose CTAs keep their rows of W_hh resident in shared memory (fp32 FMAs, expf / tanhf gates, fixed summation
+ * order: repeated calls give the same bits).  Envelope (ctn_tas_lstm_supported): any F, 1 <= H <= ctn_tas_lstm_max_hidden(dirs)
+ * (from the current device's SM count and shared memory), any B (ctn_tas_lstm_group(H, dirs) sequences per pass), any frames.
+ * workspace >= ctn_tas_lstm_workspace_bytes(), 256-byte aligned.  Every refusal comes before the first launch; a refused
+ * cooperative launch returns its error.  Launches: 3 (+ 1 weight-image launch outside the fp32 mode). */
+int ctn_tas_lstm_max_hidden(int dirs);
+int ctn_tas_lstm_supported(int F, int H, int dirs);
+int ctn_tas_lstm_group(int H, int dirs);
+size_t ctn_tas_lstm_workspace_bytes(int B, int F, int H, int dirs, int pitch, int math);
+int ctn_tas_lstm_fwd(const float* x, const float* const* w, float* out, const float* skip_in, float* skip_out, int B, int F, int H, int dirs,
+                     int frames, int pitch, int math, void* workspace, size_t workspace_bytes, ctn_stream_t stream);
+/* Separator tail + decoder, tasnet.py:365-381 and 177-184: fc (Hd -> S*N, bias; row s*N + n) -> sigmoid (softmax = 0) or softmax
+ * over the S sources of each (n, t) (softmax = 1) -> w * mask -> ConvTranspose1d -> crop.  skip (B,Hd,pitch), w (B,N,pitch);
+ * out (B,S,T); latent nullable (B,S,N,frames); what (B,S*N,pitch) scratch; B*S <= 65535.  workspace >=
+ * ctn_tas_tail_workspace_bytes(N,Hd,S,math), 256-byte aligned.  Launches: 1 (+1 softmax, +1 weight image outside the fp32 mode,
+ * +1 with latent) + the decoder's. */
+size_t ctn_tas_tail_workspace_bytes(int N, int Hd, int S, int math);
+int ctn_tas_tail_fwd(const float* skip, const float* w, const float* fc_w, const float* fc_b, const float* dec_w, float* out, float* latent,
+                     float* what, int B, int N, int Hd, int S, int frames, int pitch, int L, int stride, int crop_left, int T, int softmax,
+                     int math, void* workspace, size_t workspace_bytes, ctn_stream_t stream);
+
 /* modules.conv.DepthwiseSeparableConv1d.forward, src/modules/conv.py:24-28 (not on Conv-TasNet's path; API completeness).
  * Depthwise stage: x (B,C,T) contiguous, w (C,1,K), bias nullable -> y (B,C,y_pitch) with T_out = (T + 2 padding - dilation (K-1) - 1)
  * / stride + 1 valid columns, the rest zero.  Pointwise stage: x (B,K,pitch) padded layout with `frames` valid columns, W (M,K,1),
