@@ -152,14 +152,17 @@ __global__ void __launch_bounds__(256) k_seq_norm(const float* Y0, const float* 
   }
 }
 
-// gLN per sample over n values of z (B, n): partial (sum, sumsq) of G slices -> part[b][g][2] ...
-__global__ void __launch_bounds__(256) k_sample_part(const float* __restrict__ z, size_t n, double* __restrict__ part) {
+// gLN per sample over n values of x = z + z2 (B, n), z2 nullable: partial (sum, sumsq) of G slices -> part[b][g][2] ...
+__global__ void __launch_bounds__(256) k_sample_part(const float* __restrict__ z, const float* __restrict__ z2, size_t n,
+                                                     double* __restrict__ part) {
   __shared__ double red[64];
   const int b = blockIdx.y, G = gridDim.x;
   const size_t lo = n * blockIdx.x / G, hi = n * (blockIdx.x + 1) / G;
   double s = 0.0, ss = 0.0;
   for (size_t i = lo + threadIdx.x; i < hi; i += blockDim.x) {
-    const double x = z[(size_t)b * n + i];
+    float v = z[(size_t)b * n + i];
+    if (z2) v += z2[(size_t)b * n + i];
+    const double x = v;
     s += x;
     ss = fma(x, x, ss);
   }
@@ -171,13 +174,7 @@ __global__ void __launch_bounds__(256) k_sample_apply(float* __restrict__ z, siz
                                                       const float* __restrict__ gamma, const float* __restrict__ beta, float eps) {
   __shared__ double st[2];
   const int b = blockIdx.y;
-  if (threadIdx.x == 0) {
-    double s = 0.0, ss = 0.0;
-    for (int g = 0; g < G; ++g) { s += part[((size_t)b * G + g) * 2]; ss += part[((size_t)b * G + g) * 2 + 1]; }
-    st[0] = s; st[1] = ss;
-  }
-  __syncthreads();
-  const float2 mr = gln_mean_rstd(st, (double)n, eps);
+  const float2 mr = sample_gln_mean_rstd(part, G, b, (double)n, eps, st);
   for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (size_t)gridDim.x * blockDim.x) {
     const int f = (int)(i % F);
     float* p = z + (size_t)b * n + i;
@@ -211,9 +208,10 @@ bool mha_ok(int F, int heads) {
 
 size_t up256(size_t b) { return (b + 255) & ~(size_t)255; }
 
-// device scalar 1.0: the PReLU slope that turns the EPI_H epilogue of ctn_pw into a plain bias add
+// device scalar 1.0: the PReLU slope that turns the EPI_H epilogue of ctn_pw into a plain bias add.  The source has static
+// storage: a CUDA graph that captures this copy reads it again at every replay.
 int put_one(float* one, cudaStream_t st) {
-  const float onev = 1.f;
+  static const float onev = 1.f;
   cudaError_t e = cudaMemcpyAsync(one, &onev, sizeof(float), cudaMemcpyHostToDevice, st);
   return e == cudaSuccess ? CTN_OK : (int)e;
 }
@@ -230,12 +228,30 @@ int pw_bias(const float* A, const float* W, const float* bias, float* D, int B, 
   return ctn_pw(a, PRO_NONE, EPI_H, math, wimg, st);
 }
 
-int head_parts(size_t n) {
+}  // namespace
+
+// ---- per-sample gLN over a contiguous tensor (ctn_internal.h) -------------------------------------------------------------------
+int ctn_sample_gln_parts(size_t n) {
   size_t g = (n + 256 * 16 - 1) / (256 * 16);
   return g < 1 ? 1 : (g > 128 ? 128 : (int)g);
 }
 
-}  // namespace
+int ctn_sample_gln_stats(const float* z, const float* z2, size_t n, int B, double* part, int G, cudaStream_t st) {
+  k_sample_part<<<dim3(G, B), 256, 0, st>>>(z, z2, n, part);
+  CTN_COUNT_LAUNCH();
+  CTN_RETURN_IF_CUDA_ERR();
+  return CTN_OK;
+}
+
+int ctn_sample_gln_apply(float* z, size_t n, int B, int F, const double* part, int G, const float* gamma, const float* beta, float eps,
+                         cudaStream_t st) {
+  int ga = (int)((n + 255) / 256);
+  if (ga > 512) ga = 512;
+  k_sample_apply<<<dim3(ga, B), 256, 0, st>>>(z, n, F, part, G, gamma, beta, eps);
+  CTN_COUNT_LAUNCH();
+  CTN_RETURN_IF_CUDA_ERR();
+  return CTN_OK;
+}
 
 // ---- multi-head self-attention --------------------------------------------------------------------------------------------------
 extern "C" int ctn_mha_supported(int F, int heads) { return mha_ok(F, heads) ? 1 : 0; }
@@ -292,7 +308,7 @@ extern "C" size_t ctn_dpt_head_workspace_bytes(int B, int N, int Bc, int pitch, 
   if (B <= 0 || N <= 0 || Bc <= 0 || pitch <= 0 || S <= 0 || K <= 0) return 0;
   const size_t n = (size_t)S * K * Bc;
   return up256((size_t)B * Bc * pitch * sizeof(float)) + up256(ctn_pw_wimg_bytes(Bc, N, CTN_MATH_TF32X3)) + up256(2 * B * sizeof(double)) +
-         up256(sizeof(float)) + up256((size_t)B * head_parts(n) * 2 * sizeof(double)) + 256;
+         up256(sizeof(float)) + up256((size_t)B * ctn_sample_gln_parts(n) * 2 * sizeof(double)) + 256;
 }
 
 extern "C" int ctn_dpt_head_fwd(const float* w, const float* bn_w, const float* bn_b, const float* norm_g, const float* norm_b, float* z,
@@ -309,7 +325,7 @@ extern "C" int ctn_dpt_head_fwd(const float* w, const float* bn_w, const float* 
   if (workspace_bytes < ctn_dpt_head_workspace_bytes(B, N, Bc, pitch, S, chunk_size)) return CTN_EWORKSPACE;
   cudaStream_t st = (cudaStream_t)stream;
   const size_t n = (size_t)S * chunk_size * Bc;
-  const int G = head_parts(n);
+  const int G = ctn_sample_gln_parts(n);
   Carver cv(workspace);
   float* x0 = cv.take<float>((size_t)B * Bc * pitch);
   float* wimg = cv.take<float>(ctn_pw_wimg_bytes(Bc, N, CTN_MATH_TF32X3) / sizeof(float));
@@ -319,14 +335,8 @@ extern "C" int ctn_dpt_head_fwd(const float* w, const float* bn_w, const float* 
   CTN_TRY(put_one(one, st));
   CTN_TRY(pw_bias(w, bn_w, bn_b, x0, B, Bc, N, frames, pitch, one, stats, math, math != CTN_MATH_FP32 ? wimg : nullptr, st));
   CTN_TRY(ctn_segment_fwd(x0, z, B, Bc, frames, pitch, chunk_size, hop_size, pad_left, pad_right, 1, stream));
-  k_sample_part<<<dim3(G, B), 256, 0, st>>>(z, n, part);
-  CTN_COUNT_LAUNCH();
-  int ga = (int)((n + 255) / 256);
-  if (ga > 512) ga = 512;
-  k_sample_apply<<<dim3(ga, B), 256, 0, st>>>(z, n, Bc, part, G, norm_g, norm_b, eps);
-  CTN_COUNT_LAUNCH();
-  CTN_RETURN_IF_CUDA_ERR();
-  return CTN_OK;
+  CTN_TRY(ctn_sample_gln_stats(z, nullptr, n, B, part, G, st));
+  return ctn_sample_gln_apply(z, n, B, Bc, part, G, norm_g, norm_b, eps, st);
 }
 
 // ---- separator tail + decoder: PReLU -> map -> GTU1d -> mask nonlinearity -> w * mask -> ConvTranspose1d -> crop ----------------

@@ -99,6 +99,26 @@ struct PwArgs {
   float* dw_u_pre_out;
 };
 
+// gLN per sample over the n contiguous values of each of B samples (ctn_dptnet.cu): ctn_sample_gln_stats sums x = z + z2 (z2
+// nullable) in double over G = ctn_sample_gln_parts(n) slices per sample into part double[B][G][2] [1 launch, no atomics];
+// ctn_sample_gln_apply normalises z in place, f = i % F [1 launch].  Every reader of part sums the G partials in slice order
+// (sample_gln_mean_rstd), so repeated calls give the same bits.
+int ctn_sample_gln_parts(size_t n);
+int ctn_sample_gln_stats(const float* z, const float* z2, size_t n, int B, double* part, int G, cudaStream_t st);
+int ctn_sample_gln_apply(float* z, size_t n, int B, int F, const double* part, int G, const float* gamma, const float* beta, float eps,
+                         cudaStream_t st);
+// (mean, rstd) of sample b from its G partials, summed in slice order by thread 0 into st (shared, double[2]); the caller's
+// whole CTA must reach it (it holds a barrier)
+__device__ __forceinline__ float2 sample_gln_mean_rstd(const double* __restrict__ part, int G, int b, double n, float eps, double* st) {
+  if (threadIdx.x == 0) {
+    double s = 0.0, ss = 0.0;
+    for (int g = 0; g < G; ++g) { s += part[((size_t)b * G + g) * 2]; ss += part[((size_t)b * G + g) * 2 + 1]; }
+    st[0] = s; st[1] = ss;
+  }
+  __syncthreads();
+  return gln_mean_rstd(st, n, eps);
+}
+
 // One 1x1 contraction (ctn_wgmma.cu).  math is the model's mode: fp32 runs the FFMA kernel; the tensor-core modes run the wgmma
 // kernel, on fp16 pieces in the f16x3 mode exactly when the operand has a static bound (a.act_scale), on tf32 pieces otherwise.
 // wimg_scratch == nullptr: a.wimg already holds the weight image (ctn_pw_prepare / ctn_pw_prepare_batch with the same

@@ -189,6 +189,13 @@ ctn_tas_lstm_fwd = _sig("ctn_tas_lstm_fwd", _i, _fp, C.POINTER(_fp), _fp, _fp, _
 ctn_tas_tail_workspace_bytes = _sig("ctn_tas_tail_workspace_bytes", _sz, _i, _i, _i, _i)
 ctn_tas_tail_fwd = _sig("ctn_tas_tail_fwd", _i, _fp, _fp, _fp, _fp, _fp, _fp, _fp, _fp, _i, _i, _i, _i, _i, _i, _i, _i, _i, _i, _i, _i,
                         _fp, _sz, _fp)
+# GALRNet: the separator head (pad + segment + gLN, no bottleneck) and the low-dimension globally attentive block
+ctn_galr_head_workspace_bytes = _sig("ctn_galr_head_workspace_bytes", _sz, _i, _i, _i, _i)
+ctn_galr_head_fwd = _sig("ctn_galr_head_fwd", _i, _fp, _fp, _fp, _fp, _i, _i, _i, _i, _i, _i, _i, _i, _f, _fp, _sz, _fp)
+ctn_galr_supported = _sig("ctn_galr_supported", _i, _i, _i, _i, _i)
+ctn_galr_inter_workspace_bytes = _sig("ctn_galr_inter_workspace_bytes", _sz, _i, _i, _i, _i, _i)
+ctn_galr_inter_fwd = _sig("ctn_galr_inter_fwd", _i, _fp, _fp, _fp, _fp, _fp, _fp, _i, _fp, _fp, _fp, _fp, _fp, _fp, _fp, _fp, _fp, _i, _i,
+                          _i, _i, _i, _f, _f, _fp, _sz, _fp)
 ctn_clip_adam_chunks = _sig("ctn_clip_adam_chunks", _i, C.POINTER(_i), _i, C.POINTER(_i), C.POINTER(_i), _i)
 ctn_clip_adam_step = _sig("ctn_clip_adam_step", _i, _fp, _i, _fp, _fp, _fp, _i, _fp, _sz, _fp, _fp, _fp, _fp, _fp, _f, _f, _f, _f, _f, _fp, _fp)
 ctn_depthwise_conv1d_fwd = _sig("ctn_depthwise_conv1d_fwd", _i, _fp, _fp, _fp, _fp, _i, _i, _i, _i, _i, _i, _i, _i, _fp)
@@ -256,6 +263,7 @@ EXPORTED = [
     "ctn_sfm_tail_workspace_bytes", "ctn_sfm_tail_fwd",
     "ctn_tas_enc_gated_fwd", "ctn_tas_frame_norm_fwd", "ctn_tas_lstm_max_hidden", "ctn_tas_lstm_supported", "ctn_tas_lstm_group",
     "ctn_tas_lstm_workspace_bytes", "ctn_tas_lstm_fwd", "ctn_tas_tail_workspace_bytes", "ctn_tas_tail_fwd",
+    "ctn_galr_head_workspace_bytes", "ctn_galr_head_fwd", "ctn_galr_supported", "ctn_galr_inter_workspace_bytes", "ctn_galr_inter_fwd",
 ]
 
 

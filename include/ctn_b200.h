@@ -449,6 +449,34 @@ int ctn_tas_tail_fwd(const float* skip, const float* w, const float* fc_w, const
                      float* what, int B, int N, int Hd, int S, int frames, int pitch, int L, int stride, int crop_left, int T, int softmax,
                      int math, void* workspace, size_t workspace_bytes, ctn_stream_t stream);
 
+/* ---- GALRNet path (src/models/galrnet.py, src/models/galr.py, csrc/ctn_galr.cu) ----
+ *
+ * The dual-path state is channels-last, (B,S,K,F); the intra-chunk block is ctn_bilstm_proj_fwd + ctn_dprnn_norm_res2_fwd with
+ * swap = 0, and the tail is ctn_dpt_tail_fwd with Bc = N.
+ *
+ * Separator head, galrnet.py:233-239: z (B,S,chunk,F) = gLN(Segment1d(pad(w))) with the gLN per sample over the segmented tensor
+ * (overlap duplicates and padding zeros included), no bottleneck.  w (B,F,pitch) with `frames` valid columns; S = (frames +
+ * pad_left + pad_right - chunk) / hop + 1.  workspace >= ctn_galr_head_workspace_bytes(B,S,chunk,F), 256-byte aligned.  Every
+ * refusal comes before the first launch.  3 launches. */
+size_t ctn_galr_head_workspace_bytes(int B, int S, int chunk_size, int F);
+int ctn_galr_head_fwd(const float* w, const float* norm_g, const float* norm_b, float* z, int B, int F, int frames, int pitch, int chunk_size,
+                      int hop_size, int pad_left, int pad_right, float eps, void* workspace, size_t workspace_bytes, ctn_stream_t stream);
+/* LowDimensionGloballyAttentiveBlock.forward, galr.py:161-197, on x (B,S,K,F) channels-last -> out (B,S,K,F); out may alias x.
+ * zt = LN_F(fc_map(x) along K) + pe, then y = MultiheadAttention(zt) over the S chunks of each of the B*Q down-sampled frames,
+ * out = fc_inv(gLN(y + zt)) along Q + x with the gLN per sample over (Q,S,F).  map_w (Q,K), map_b (Q); ln_g, ln_b (F) of
+ * norm2d_in (eps ln_eps); in_w, in_b, out_w, out_b as ctn_mha_fwd; gn_g, gn_b (F) of norm2d_out (eps gn_eps); inv_w (K,Q),
+ * inv_b (K).  pe_div (F/2): the divisors 10000^(j/F) of the positional encoding, formed as the reference forms them (fp32); the
+ * encoding of position p = s*Q + q is sin(p / pe_div[f]) for f < F/2 and cos(p / pe_div[f - F/2]) above.  LayerNorm and gLN
+ * statistics are summed in double in a fixed order: repeated calls give the same bits.  Envelope (ctn_galr_supported): F in
+ * {32,64,128}, 1 <= Q <= K, F/heads in ctn_mha_supported's; B, S <= 65535, B*Q <= 65535, S*Q <= 2^24.  workspace >=
+ * ctn_galr_inter_workspace_bytes(B,S,K,Q,F), 256-byte aligned.  Every refusal comes before the first launch.  6 launches. */
+int ctn_galr_supported(int F, int K, int Q, int heads);
+size_t ctn_galr_inter_workspace_bytes(int B, int S, int K, int Q, int F);
+int ctn_galr_inter_fwd(const float* x, const float* map_w, const float* map_b, const float* ln_g, const float* ln_b, const float* pe_div,
+                       int heads, const float* in_w, const float* in_b, const float* out_w, const float* out_b, const float* gn_g,
+                       const float* gn_b, const float* inv_w, const float* inv_b, float* out, int B, int S, int K, int Q, int F, float ln_eps,
+                       float gn_eps, void* workspace, size_t workspace_bytes, ctn_stream_t stream);
+
 /* modules.conv.DepthwiseSeparableConv1d.forward, src/modules/conv.py:24-28 (not on Conv-TasNet's path; API completeness).
  * Depthwise stage: x (B,C,T) contiguous, w (C,1,K), bias nullable -> y (B,C,y_pitch) with T_out = (T + 2 padding - dilation (K-1) - 1)
  * / stride + 1 valid columns, the rest zero.  Pointwise stage: x (B,K,pitch) padded layout with `frames` valid columns, W (M,K,1),
