@@ -51,13 +51,14 @@ __global__ void __launch_bounds__(128) k_rowproj(const float* __restrict__ X, co
 }
 
 // O[seq][t][h D + c] = sum_j softmax_j(q_t . k_j / sqrt(D)) v_j[c] for head h, qkv (NSEQ, T, 3F) = [q | k | v] per token.
-// grid (ceil(T / 64), heads, NSEQ), block 64: one query per thread, q and the running output in registers; keys and values of
-// a 64-key tile in shared memory (every thread reads the same key: broadcast).  Per 16 keys the running max m and sum l are
+// grid (NSEQ, ceil(T / 64), heads), block 64: one query per thread, q and the running output in registers; keys and values of
+// a 64-key tile in shared memory (every thread reads the same key: broadcast).  The sequences are on x, whose limit is 2^31 - 1,
+// so a batch of any size runs (DPTNet's inter path has B * chunk_size sequences).  Per 16 keys the running max m and sum l are
 // updated: the old terms are rescaled by exp(m_old - m_new), exactly as in a one-pass softmax.
 template <int D>
 __global__ void __launch_bounds__(ATT_Q) k_attn(const float* __restrict__ qkv, float* __restrict__ O, int T, int F, float scale) {
   __shared__ float ks[ATT_KT][D], vs[ATT_KT][D];
-  const int seq = blockIdx.z, hd = blockIdx.y, t = blockIdx.x * ATT_Q + threadIdx.x;
+  const int seq = blockIdx.x, hd = blockIdx.z, t = blockIdx.y * ATT_Q + threadIdx.x;
   const size_t base = (size_t)seq * T;
   const int F3 = 3 * F;
   float q[D], acc[D];
@@ -266,7 +267,7 @@ extern "C" int ctn_mha_fwd(const float* z, int NSEQ, int T, int F, int heads, co
                            const float* out_b, float* y, void* workspace, size_t workspace_bytes, ctn_stream_t stream) {
   LaunchScope scope(z);
   if (!z || !in_w || !in_b || !out_w || !out_b || !y || !workspace || NSEQ <= 0 || T <= 0 || F <= 0 || heads <= 0) return CTN_EINVAL;
-  if (!mha_ok(F, heads) || NSEQ > 65535) return CTN_EUNSUPPORTED;
+  if (!mha_ok(F, heads) || (T + ATT_Q - 1) / ATT_Q > 65535) return CTN_EUNSUPPORTED;
   if (((uintptr_t)workspace) & 255) return CTN_EALIGN;
   if (workspace_bytes < ctn_mha_workspace_bytes(NSEQ, T, F)) return CTN_EWORKSPACE;
   cudaStream_t st = (cudaStream_t)stream;
@@ -278,7 +279,7 @@ extern "C" int ctn_mha_fwd(const float* z, int NSEQ, int T, int F, int heads, co
   CTN_COUNT_LAUNCH();
   const int D = F / heads;
   const float scale = (float)(1.0 / sqrt((double)D));
-  const dim3 ga((T + ATT_Q - 1) / ATT_Q, heads, NSEQ);
+  const dim3 ga(NSEQ, (T + ATT_Q - 1) / ATT_Q, heads);
   if (D == 8) k_attn<8><<<ga, ATT_Q, 0, st>>>(qkv, o, T, F, scale);
   if (D == 16) k_attn<16><<<ga, ATT_Q, 0, st>>>(qkv, o, T, F, scale);
   if (D == 32) k_attn<32><<<ga, ATT_Q, 0, st>>>(qkv, o, T, F, scale);

@@ -171,8 +171,8 @@ extern "C" int ctn_galr_inter_fwd(const float* x, const float* map_w, const floa
       !out || !workspace || B <= 0 || S <= 0 || K <= 0 || Q <= 0 || F <= 0 || heads <= 0)
     return CTN_EINVAL;
   if (!ctn_galr_supported(F, K, Q, heads)) return CTN_EUNSUPPORTED;
-  // grid limits, the attention's sequence count, and positions s Q + q exact in fp32
-  if (B > 65535 || S > 65535 || (long long)B * Q > 65535 || (long long)S * Q > (1LL << 24)) return CTN_EUNSUPPORTED;
+  // the grids of the down- and up-map and of the gLN statistics, and positions s Q + q exact in fp32
+  if (B > 65535 || S > 65535 || (long long)S * Q > (1LL << 24)) return CTN_EUNSUPPORTED;
   if (((uintptr_t)workspace) & 255) return CTN_EALIGN;
   if (workspace_bytes < ctn_galr_inter_workspace_bytes(B, S, K, Q, F)) return CTN_EWORKSPACE;
   cudaStream_t st = (cudaStream_t)stream;

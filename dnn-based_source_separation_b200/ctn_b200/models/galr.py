@@ -143,9 +143,9 @@ class LowDimensionGloballyAttentiveBlock(GloballyAttentiveBlockBase):
         if K != self.chunk_size or F != self.norm2d_in.num_features:
             raise ValueError("chunk_size={}, num_features={} given to a block built for {}, {}".format(K, F, self.chunk_size,
                                                                                                    self.norm2d_in.num_features))
-        if B > 65535 or S > 65535 or B * Q > 65535 or S * Q > 1 << 24:
+        if B > 65535 or S > 65535 or S * Q > 1 << 24:
             raise NotImplementedError("batch_size={}, S={} with down_chunk_size={} are outside the globally attentive block's launch "
-                                      "limits (batch_size, S, batch_size * down_chunk_size <= 65535; S * down_chunk_size <= 2^24)"
+                                      "limits (batch_size, S <= 65535; S * down_chunk_size <= 2^24)"
                                       .format(B, S, Q))
 
     def _divisors(self, F, dev):

@@ -309,8 +309,8 @@ int ctn_bilstm_relu_proj_fwd(const float* z, int NSEQ, int T, int F, int H, cons
                              float* hout, void* workspace, size_t workspace_bytes, ctn_stream_t stream);
 /* nn.MultiheadAttention(F, heads)(z, z, z) without mask (dptnet.py:512), on channels-last sequences: z (NSEQ,T,F) -> y (NSEQ,T,F) =
  * out_proj(attention) + out_b, no residual.  in_w (3F,F), in_b (3F), out_w (F,F), out_b (F); scale 1/sqrt(F/heads).  fp32 FMAs, keys
- * streamed through an online softmax: any T.  Envelope (ctn_mha_supported): F <= 128, F % 4 == 0, F/heads in {8,16,32,64};
- * NSEQ <= 65535.  workspace >= ctn_mha_workspace_bytes(NSEQ,T,F), 256-byte aligned.  3 launches. */
+ * streamed through an online softmax: any T up to 65535 tiles of 64.  Envelope (ctn_mha_supported): F <= 128, F % 4 == 0,
+ * F/heads in {8,16,32,64}; any NSEQ (the sequences are the grid's x).  workspace >= ctn_mha_workspace_bytes(NSEQ,T,F), 256-byte aligned.  3 launches. */
 int ctn_mha_supported(int F, int heads);
 size_t ctn_mha_workspace_bytes(int NSEQ, int T, int F);
 int ctn_mha_fwd(const float* z, int NSEQ, int T, int F, int heads, const float* in_w, const float* in_b, const float* out_w,
@@ -394,7 +394,7 @@ int ctn_sfm_pos_enc_fwd(const float* X, const float* pe, float* out, int B, int 
  * norm2.weight, norm2.bias; then the positional-encoding buffer and the final gLN's weight and bias.  The four contractions of a
  * layer run through ctn_pw in the numeric mode `math`; every weight image of the call is built in one batch first.  Sequences
  * longer than 5000 tokens: CTN_EINVAL.  workspace >= ctn_sfm_transformer_workspace_bytes(), 256-byte aligned.
- * Launches: 7*layers + 2, plus ceil(4*layers / 48) weight-image launches outside the fp32 mode. */
+ * Launches: 7*layers + 2, plus, outside the fp32 mode, ceil(4*n / 48) weight-image launches for each batch of n <= 64 layers. */
 size_t ctn_sfm_transformer_workspace_bytes(int B, int F, int d_ff, int layers, int pitch, int math);
 int ctn_sfm_transformer_fwd(const float* X, float* out, const float* const* w, int B, int F, int heads, int d_ff, int layers, int S, int C,
                             int pitch, int intra, float eps, int math, void* workspace, size_t workspace_bytes, ctn_stream_t stream);
@@ -468,7 +468,7 @@ int ctn_galr_head_fwd(const float* w, const float* norm_g, const float* norm_b, 
  * inv_b (K).  pe_div (F/2): the divisors 10000^(j/F) of the positional encoding, formed as the reference forms them (fp32); the
  * encoding of position p = s*Q + q is sin(p / pe_div[f]) for f < F/2 and cos(p / pe_div[f - F/2]) above.  LayerNorm and gLN
  * statistics are summed in double in a fixed order: repeated calls give the same bits.  Envelope (ctn_galr_supported): F in
- * {32,64,128}, 1 <= Q <= K, F/heads in ctn_mha_supported's; B, S <= 65535, B*Q <= 65535, S*Q <= 2^24.  workspace >=
+ * {32,64,128}, 1 <= Q <= K, F/heads in ctn_mha_supported's; B, S <= 65535, S*Q <= 2^24.  workspace >=
  * ctn_galr_inter_workspace_bytes(B,S,K,Q,F), 256-byte aligned.  Every refusal comes before the first launch.  6 launches. */
 int ctn_galr_supported(int F, int K, int Q, int heads);
 size_t ctn_galr_inter_workspace_bytes(int B, int S, int K, int Q, int F);

@@ -107,7 +107,7 @@ def test_features_outside_kernel_envelope_refused():
         G.GloballyAttentiveBlock(32, num_heads=4)
 
 
-def test_forward_refusals_before_cuda():
+def test_forward_and_launch_limit_refusals_before_cuda():
     g = GOLD["tiny"]
     m = make(g["cfg"]).eval()
     x = g["x"]  # CPU tensors: every refusal must fire before the CUDA check
@@ -140,7 +140,10 @@ def test_forward_refusals_before_cuda():
             blk.inter_chunk_block.norm2d_in(z)
     m.eval()
     with torch.no_grad(), pytest.raises(NotImplementedError, match="launch limits"):
-        blk.inter_chunk_block.check_shape((16385, 3, 16, 32))  # batch_size * down_chunk_size > 65535
+        blk.inter_chunk_block.check_shape((65536, 3, 16, 32))  # batch_size > 65535: the grids of the down- and up-map
+    with torch.no_grad(), pytest.raises(NotImplementedError, match="launch limits"):
+        blk.inter_chunk_block.check_shape((2, 65536, 16, 32))    # S > 65535
+    blk.inter_chunk_block.check_shape((16385, 3, 16, 32))  # batch_size * down_chunk_size > 65535: the attention takes any count
     with torch.no_grad(), pytest.raises(ValueError):
         blk.inter_chunk_block(torch.randn(2, 32, 3, 15))       # not the chunk size the block was built for
 

@@ -114,7 +114,7 @@ def test_inter_block_silence_and_scaled_inputs(scale):
     check(out, inter_ref(x, sd, heads, Q))
 
 
-def test_inter_block_refusals_before_launch():
+def test_inter_block_grid_limit_refusals_before_launch():
     F, K, Q = 64, 100, 32
     sd = inter_weights(F, K, Q, 1)
     x = torch.randn(1, 3, K, F).to(DEV)
@@ -132,7 +132,9 @@ def test_inter_block_refusals_before_launch():
 
     assert call(Q_=K + 1) == N.CTN_EUNSUPPORTED
     assert call(heads=16) == N.CTN_EUNSUPPORTED          # head dimension 4
-    assert call(B=2049) == N.CTN_EUNSUPPORTED            # B Q > 65535
+    assert call(B=65536) == N.CTN_EUNSUPPORTED           # B > 65535: the grids of the down- and up-map
+    assert call(S=65536) == N.CTN_EUNSUPPORTED           # S > 65535
+    assert call(B=2049) == N.CTN_EWORKSPACE              # B Q = 65568 attention sequences are inside the envelope
     assert call(nb=nbytes // 2) == N.CTN_EWORKSPACE
     assert N.ctn_last_launch_count() == 0
 
