@@ -204,6 +204,36 @@ struct SkipJob { const float* r; const float* v1; const float* v2; const double*
 struct SkipJobs { SkipJob j[CTN_MAX_BLOCKS]; int n; };
 int ctn_skip_reduce(const SkipJobs& jobs, double n2, float eps, float* skip, int B, int Sc, int frames, int pitch, cudaStream_t st);
 
+// Online (chunk-by-chunk) inference, shared by causal Conv-TasNet (ctn_online.cu) and causal LSTM-TasNet (ctn_tasnet.cu).  The
+// state's header holds T0, the samples pushed since the reset.  Every kernel of a push reads it; the decoder, the push's last
+// kernel, advances it once all its CTAs have read it (ticket).
+struct OnlineHdr {
+  long long T0;     // samples pushed since the reset
+  unsigned ticket;  // CTAs of the decoder that have finished reading T0
+  unsigned pad;
+};
+struct OnlineFrames { long long T0, F0; int nv; };
+// frames done before this push (F0) and completed by it (nv), from the device counter
+__device__ __forceinline__ OnlineFrames push_frames(const OnlineHdr* hdr, int L, int S, int n) {
+  OnlineFrames f;
+  f.T0 = *(const volatile long long*)&hdr->T0;
+  const long long T1 = f.T0 + n;
+  f.F0 = f.T0 >= L ? (f.T0 - L) / S + 1 : 0;
+  const long long F1 = T1 >= L ? (T1 - L) / S + 1 : 0;
+  f.nv = (int)(F1 - f.F0);
+  return f;
+}
+// Encoder over [carry | chunk] of B streams (k_online_enc, ctn_encoder_fwd's order): w (B, N, pitch), columns [nv, pitch) zero;
+// carry [B][L - S] takes the last L - S samples.  Shared memory (L - S + n) floats, at most 200 KB.  1 launch.
+size_t ctn_online_enc_smem(int L, int S, int n);
+int ctn_online_enc(const float* x, const float* W, float* carry, float* w, const OnlineHdr* hdr, int B, int N, int L, int S, int n,
+                   int pitch, int relu, cudaStream_t st);
+// Decoder over [history | chunk] of BS rows (k_online_dec, ctn_decoder_fwd's summation order) with the offline crop.  push = 1:
+// y (BS, n), the history [BS][N][L/S - 1] takes the last frames and the decoder advances T0 by n; push = 0 (flush): y (BS, D)
+// from the history alone, nothing advanced.  N (L/S - 1) floats of shared memory, at most 48 KB.  1 launch.
+int ctn_online_dec(const float* what, const float* Wd, float* hist, float* y, OnlineHdr* hdr, int BS, int N, int L, int S, int n, int pitch,
+                   int push, cudaStream_t st);
+
 // the refusals of ctn_decoder_fwd, for callers that must refuse before their own launches (ctn_sep_tail_fwd)
 int ctn_decoder_check(int BS, int N, int frames, int in_pitch, int L, int stride, int crop_left, int T_out);
 

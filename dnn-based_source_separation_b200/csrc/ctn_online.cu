@@ -16,7 +16,8 @@
 // frame of the chunk, and one CTA does it with __syncthreads alone.  The chunk is walked in tiles of 32 frames (lane =
 // frame, warp = channel group), the scan carried from tile to tile.  With B streams the grid is B CTAs.
 //
-// Counters: the state's header holds T0, the samples pushed since the reset.  Every kernel of a push reads it; the decoder,
+// Counters (OnlineHdr, push_frames in ctn_internal.h, shared with the online LSTM-TasNet): the state's header holds T0, the
+// samples pushed since the reset.  Every kernel of a push reads it; the decoder,
 // the push's last kernel, advances it once all its CTAs have read it (ticket).  Frames done before the push:
 // F0 = T0 >= L ? (T0 - L) / S + 1 : 0; the push completes F1 - F0 of its n / S columns.
 #include <string.h>
@@ -28,12 +29,6 @@ namespace {
 constexpr int OT = 512;          // threads of the per-stream cLN kernels
 constexpr int NW = OT / 32;      // channel groups
 constexpr int TF = 32;           // frames per tile
-
-struct OnlineHdr {
-  long long T0;     // samples pushed since the reset
-  unsigned ticket;  // CTAs of the decoder that have finished reading T0
-  unsigned pad;
-};
 
 struct OnlineState {
   OnlineHdr* hdr;
@@ -105,19 +100,6 @@ int check_cfg(const ctn_config_t* c) {
   return CTN_OK;
 }
 
-struct Frames { long long T0, F0; int nv; };
-
-// frames done before this push (F0) and completed by it (nv), from the device counter
-__device__ __forceinline__ Frames push_frames(const OnlineHdr* hdr, int L, int S, int n) {
-  Frames f;
-  f.T0 = *(const volatile long long*)&hdr->T0;
-  const long long T1 = f.T0 + n;
-  f.F0 = f.T0 >= L ? (f.T0 - L) / S + 1 : 0;
-  const long long F1 = T1 >= L ? (T1 - L) / S + 1 : 0;
-  f.nv = (int)(F1 - f.F0);
-  return f;
-}
-
 // Encoder over [carry | chunk]: w[b][c][f] = sum_k W[c][k] xcat[base + f S + k] (k ascending, as k_encoder), f < nv; zero up to pitch.
 // One CTA per stream: the carry is read into shared memory before it is overwritten.
 __global__ void __launch_bounds__(256) k_online_enc(const float* __restrict__ x, const float* __restrict__ W, float* __restrict__ carry,
@@ -125,7 +107,7 @@ __global__ void __launch_bounds__(256) k_online_enc(const float* __restrict__ x,
                                                     int pitch, int relu) {
   extern __shared__ float xs[];  // [D + n]
   const int b = blockIdx.x, D = L - S;
-  const Frames fr = push_frames(hdr, L, S, n);
+  const OnlineFrames fr = push_frames(hdr, L, S, n);
   float* cb = carry + (size_t)b * D;
   for (int i = threadIdx.x; i < D; i += 256) xs[i] = cb[i];
   for (int i = threadIdx.x; i < n; i += 256) xs[D + i] = x[(size_t)b * n + i];
@@ -198,7 +180,7 @@ __global__ void __launch_bounds__(OT) k_online_cln(const float* __restrict__ w, 
   __shared__ float2 mi[TF];
   __shared__ double run[2];
   const int b = blockIdx.x;
-  const Frames fr = push_frames(hdr, L, S, n);
+  const OnlineFrames fr = push_frames(hdr, L, S, n);
   double* rg = run_g + (size_t)b * rstride;
   if (threadIdx.x < 2) run[threadIdx.x] = rg[threadIdx.x];
   __syncthreads();
@@ -226,7 +208,7 @@ __global__ void __launch_bounds__(OT) k_online_block(float* __restrict__ h, floa
   __shared__ double run[4];
   const int b = blockIdx.x, lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
   const int Rd = (P - 1) * dil;
-  const Frames fr = push_frames(hdr, L, S, n);
+  const OnlineFrames fr = push_frames(hdr, L, S, n);
   double* rg = run_g + (size_t)b * rstride;
   if (threadIdx.x < 4) run[threadIdx.x] = rg[threadIdx.x];
   __syncthreads();
@@ -279,7 +261,7 @@ __global__ void __launch_bounds__(256) k_online_dec(const float* __restrict__ wh
                                                     int nout, int pitch, int split, int push) {
   extern __shared__ float hs[];  // [N][R-1] new history
   const int bs = blockIdx.x, R = L / S, D = L - S;
-  const Frames fr = push_frames(hdr, L, S, push ? n : 0);
+  const OnlineFrames fr = push_frames(hdr, L, S, push ? n : 0);
   const long long F1 = fr.F0 + fr.nv, Fh = fr.F0 - (R - 1);  // frames [Fh, F0) in the history
   const float* wb = what + (size_t)bs * N * pitch;
   float* hist = hist_g + (size_t)bs * N * (R - 1);
@@ -348,16 +330,39 @@ __global__ void __launch_bounds__(256) k_online_dec(const float* __restrict__ wh
   }
 }
 
-size_t enc_smem(const ctn_config_t* c, int n) { return sizeof(float) * ((size_t)c->kernel_size - c->stride + n); }
-
 bool decoder_split(int L, int S) { return L == 2 * S && (S == 8 || S == 1 || S == 10 || S == 2); }  // ctn_decoder_fwd's k_decoder cases
 
 }  // namespace
 
+size_t ctn_online_enc_smem(int L, int S, int n) { return sizeof(float) * ((size_t)L - S + n); }
+
+int ctn_online_enc(const float* x, const float* W, float* carry, float* w, const OnlineHdr* hdr, int B, int N, int L, int S, int n,
+                   int pitch, int relu, cudaStream_t st) {
+  const size_t smem = ctn_online_enc_smem(L, S, n);
+  if (smem > 48 * 1024) {
+    cudaError_t e = cudaFuncSetAttribute(k_online_enc, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+    if (e != cudaSuccess) return (int)e;
+  }
+  k_online_enc<<<B, 256, smem, st>>>(x, W, carry, w, hdr, N, L, S, n, pitch, relu);
+  CTN_COUNT_LAUNCH();
+  CTN_RETURN_IF_CUDA_ERR();
+  return CTN_OK;
+}
+
+int ctn_online_dec(const float* what, const float* Wd, float* hist, float* y, OnlineHdr* hdr, int BS, int N, int L, int S, int n, int pitch,
+                   int push, cudaStream_t st) {
+  const int R = L / S;
+  k_online_dec<<<BS, 256, sizeof(float) * (size_t)N * (R - 1), st>>>(what, Wd, hist, y, hdr, N, L, S, push ? n : 0, push ? n : L - S,
+                                                                     pitch, decoder_split(L, S) ? 1 : 0, push);
+  CTN_COUNT_LAUNCH();
+  CTN_RETURN_IF_CUDA_ERR();
+  return CTN_OK;
+}
+
 extern "C" int ctn_online_state_bytes(const ctn_config_t* cfg, int B, int max_chunk_frames, size_t* bytes) {
   CTN_TRY(check_cfg(cfg));
   if (B <= 0 || max_chunk_frames <= 0 || !bytes) return CTN_EINVAL;
-  if (enc_smem(cfg, max_chunk_frames * cfg->stride) > 200 * 1024) return CTN_EUNSUPPORTED;
+  if (ctn_online_enc_smem(cfg->kernel_size, cfg->stride, max_chunk_frames * cfg->stride) > 200 * 1024) return CTN_EUNSUPPORTED;
   Carver cv(nullptr);
   OnlineState s;
   carve(cv, cfg, B, ctn_pitch(max_chunk_frames), &s);
@@ -437,15 +442,7 @@ extern "C" int ctn_online_push(const ctn_config_t* cfg, const ctn_params_t* para
   const int rstride = (1 + 2 * RX) * 2;
   {
     StageTimer tm(CTN_ST_ENC, st);
-    const size_t smem = enc_smem(cfg, n);
-    if (smem > 48 * 1024) {
-      cudaError_t e = cudaFuncSetAttribute(k_online_enc, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-      if (e != cudaSuccess) return (int)e;
-    }
-    k_online_enc<<<B, 256, smem, st>>>(x, params->enc_w, s.enc_carry, s.w, s.hdr, N, L, S, n, pitch,
-                                                                       cfg->enc_relu);
-    CTN_COUNT_LAUNCH();
-    CTN_RETURN_IF_CUDA_ERR();
+    CTN_TRY(ctn_online_enc(x, params->enc_w, s.enc_carry, s.w, s.hdr, B, N, L, S, n, pitch, cfg->enc_relu, st));
   }
   {
     StageTimer tm(CTN_ST_HEAD, st);
@@ -492,18 +489,14 @@ extern "C" int ctn_online_push(const ctn_config_t* cfg, const ctn_params_t* para
   }
   {
     StageTimer tm(CTN_ST_DEC, st);
-    const int R = L / S;
-    k_online_dec<<<B * Ns, 256, sizeof(float) * (size_t)N * (R - 1), st>>>(s.what, s.dec_w, s.dec_hist, y, s.hdr, N, L, S, n, n,
-                                                                           pitch, decoder_split(L, S) ? 1 : 0, 1);
-    CTN_COUNT_LAUNCH();
-    CTN_RETURN_IF_CUDA_ERR();
+    CTN_TRY(ctn_online_dec(s.what, s.dec_w, s.dec_hist, y, s.hdr, B * Ns, N, L, S, n, pitch, 1, st));
   }
   return CTN_OK;
 }
 
 extern "C" int ctn_online_flush(const ctn_config_t* cfg, void* state, int B, float* y_tail, ctn_stream_t stream) {
   CTN_TRY(check_cfg(cfg));
-  const int L = cfg->kernel_size, S = cfg->stride, D = L - S, N = cfg->n_basis, R = L / S;
+  const int L = cfg->kernel_size, S = cfg->stride, D = L - S, N = cfg->n_basis;
   // a zero-delay model (kernel_size == stride) has no tail: y_tail holds 0 samples and may be null
   if (!state || (D > 0 && !y_tail) || B <= 0) return CTN_EINVAL;
   if (((uintptr_t)state) & 255) return CTN_EALIGN;
@@ -519,10 +512,5 @@ extern "C" int ctn_online_flush(const ctn_config_t* cfg, void* state, int B, flo
   if (T0 < L) return CTN_EINVAL;  // no frame yet: the offline model needs T >= kernel_size
   if (D == 0) return CTN_OK;
   // the tail segments read the history only; `what` is not touched (pitch is unused)
-  k_online_dec<<<B * cfg->n_sources, 256, sizeof(float) * (size_t)N * (R - 1), st>>>(s.what, s.dec_w, s.dec_hist,
-                                                                                     y_tail, s.hdr, N, L, S, 0, D, CTN_TILE_T,
-                                                                                     decoder_split(L, S) ? 1 : 0, 0);
-  CTN_COUNT_LAUNCH();
-  CTN_RETURN_IF_CUDA_ERR();
-  return CTN_OK;
+  return ctn_online_dec(s.what, s.dec_w, s.dec_hist, y_tail, s.hdr, B * cfg->n_sources, N, L, S, 0, CTN_TILE_T, 0, st);
 }

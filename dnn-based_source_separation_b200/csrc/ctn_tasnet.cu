@@ -14,8 +14,12 @@
 //     wait for each other.  Every sum has a fixed order: a repeated call gives the same bits.
 //   * the tail: fc as ctn_pw with the sigmoid mask and w * mask in its epilogue, or its logits and a softmax over the SOURCES
 //     (tasnet.py:312-316, nn.Softmax(dim=1) of (B, S, N, T')), then the transposed-conv decoder with the crop.
+//   * online inference of the causal model (ctn_tas_online_*, at the end of this file): the same stages on one chunk's columns, the
+//     recurrence carrying (h, c) in the caller's state (k_tas_lstm<true>), the filter banks those of the Conv-TasNet online path.
 #include <math.h>
 #include <string.h>
+
+#include <vector>
 
 #include "ctn_internal.h"
 
@@ -114,12 +118,15 @@ __global__ void __launch_bounds__(TAS_THREADS) k_tas_enc_gated(const float* __re
   tas_frame_norm_tile(wt, gamma, beta, xn + (size_t)b * N * pitch, N, f0, frames, pitch, eps);
 }
 
-// the frame norm alone, from w (B, N, pitch) (the plain Encoder's output).  grid (pitch / TAS_TF, B), dynamic smem wt[N][TAS_TF]
+// the frame norm alone, from w (B, N, pitch) (the plain Encoder's output).  grid (pitch / TAS_TF, B), dynamic smem wt[N][TAS_TF].
+// hdr (nullable, online push of n samples): `frames` is the push's completed-frame count, read from the device counter.
 __global__ void __launch_bounds__(TAS_THREADS) k_tas_frame_norm(const float* __restrict__ w, const float* __restrict__ gamma,
                                                                 const float* __restrict__ beta, float* __restrict__ xn, int N,
-                                                                int frames, int pitch, float eps) {
+                                                                int frames, int pitch, float eps, const OnlineHdr* __restrict__ hdr,
+                                                                int L, int S, int n) {
   extern __shared__ float wt[];
   const int b = blockIdx.y, f0 = blockIdx.x * TAS_TF;
+  if (hdr) frames = push_frames(hdr, L, S, n).nv;
   const float* wb = w + (size_t)b * N * pitch;
   for (int idx = threadIdx.x; idx < N * TAS_TF; idx += TAS_THREADS) {
     const int n = idx / TAS_TF, t = f0 + idx % TAS_TF;
@@ -154,6 +161,11 @@ struct LstmArgs {
   float* hbuf;          // [dirs][2][gmax][H]
   unsigned* bar;        // dirs counters, 32 words apart
   int B, H, T, pitch, dirs, U, cpd, gmax, Hs;
+  // carry mode (online push of n samples, dirs = 1): T is the push's completed-frame count from hdr; the state starts from and
+  // ends in hc [B][2][H] (h, then c, of each stream)
+  float* hc;
+  const OnlineHdr* hdr;
+  int L, S, n;
 };
 
 __device__ __forceinline__ void cp_async4(float* s, const float* g) {
@@ -168,10 +180,14 @@ size_t lstm_smem_bytes(int H, int U, int gmax) {
   return sizeof(float) * (4 * U * Hs + gmax * Hs + (size_t)4 * U * gmax + (size_t)2 * 4 * U * gmax * TAS_PF);
 }
 
+// CARRY: step 0 reads h_0 from a.hc and the owner of (sequence, unit) its c_0; after the last step's barrier the owner writes (h, c)
+// back.  That store cannot race a slower CTA's step-0 read of a.hc: a CTA passes the barrier of step T - 1 only once every CTA of
+// its direction has arrived there, and a CTA arrives at any barrier only after its step-0 read (DESIGN.md section 18).
+template <bool CARRY>
 __global__ void __launch_bounds__(TAS_THREADS, 1) k_tas_lstm(const LstmArgs a) {
   extern __shared__ __align__(16) float sm[];
   const int d = blockIdx.x / a.cpd, c = blockIdx.x % a.cpd;
-  const int H = a.H, T = a.T, Hs = a.Hs, gmax = a.gmax;
+  const int H = a.H, T = CARRY ? push_frames(a.hdr, a.L, a.S, a.n).nv : a.T, Hs = a.Hs, gmax = a.gmax;
   const int j0 = c * a.U, nu = min(a.U, H - j0), R = 4 * nu;
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
   float* ws = sm;                          // local row r = g nu + u  <->  W_hh row g H + j0 + u
@@ -199,7 +215,8 @@ __global__ void __launch_bounds__(TAS_THREADS, 1) k_tas_lstm(const LstmArgs a) {
     const int nb = min(gmax, a.B - b0);
     const bool owner = tid < nu * nb;
     const int uo = owner ? tid % nu : 0, bo = owner ? tid / nu : 0;
-    float cst = 0.f;
+    float cst = 0.f, hlast = 0.f;
+    if (CARRY && owner && T > 0) cst = a.hc[((size_t)(b0 + bo) * 2 + 1) * H + j0 + uo];
     // input projections of steps [tile PF, tile PF + PF) into prefetch buffer tile & 1: pre[buf][(r nb + b) PF + p]
     auto prefetch = [&](int tile) {
       float* dst = pre + (size_t)(tile & 1) * 4 * a.U * gmax * TAS_PF;
@@ -225,7 +242,7 @@ __global__ void __launch_bounds__(TAS_THREADS, 1) k_tas_lstm(const LstmArgs a) {
       const float* hprev = hb + (size_t)((s + 1) & 1) * gmax * H;
       for (int i = tid; i < nb * H; i += TAS_THREADS) {
         const int bb = i / H, k = i % H;
-        hs[bb * Hs + k] = s ? __ldcg(hprev + (size_t)bb * H + k) : 0.f;
+        hs[bb * Hs + k] = s ? __ldcg(hprev + (size_t)bb * H + k) : (CARRY ? a.hc[(size_t)(b0 + bb) * 2 * H + k] : 0.f);
       }
       __syncthreads();
       // gate rows: warp tiles of TAS_RB rows x TAS_SB sequences, lanes stride k, then a fixed shuffle tree
@@ -274,6 +291,7 @@ __global__ void __launch_bounds__(TAS_THREADS, 1) k_tas_lstm(const LstmArgs a) {
         }
         cst = fmaf(sigm(gv[1]), cst, sigm(gv[0]) * tanhf(gv[2]));
         const float h = sigm(gv[3]) * tanhf(cst);
+        hlast = h;
         const size_t o = ((size_t)(b0 + bo) * a.dirs * H + (size_t)d * H + j0 + uo) * a.pitch + t;
         a.out[o] = h;
         if (a.skip_out) a.skip_out[o] = h + a.skip_in[o];
@@ -293,6 +311,10 @@ __global__ void __launch_bounds__(TAS_THREADS, 1) k_tas_lstm(const LstmArgs a) {
         __threadfence();
       }
       __syncthreads();
+    }
+    if (CARRY && owner && T > 0) {  // after the barrier of step T - 1
+      a.hc[(size_t)(b0 + bo) * 2 * H + j0 + uo] = hlast;
+      a.hc[((size_t)(b0 + bo) * 2 + 1) * H + j0 + uo] = cst;
     }
   }
 }
@@ -419,7 +441,8 @@ extern "C" int ctn_tas_frame_norm_fwd(const float* w, const float* gamma, const 
   const size_t smem = sizeof(float) * (size_t)N * TAS_TF;
   if (smem > (size_t)(smem_optin > 48 * 1024 ? smem_optin : 48 * 1024)) return CTN_EUNSUPPORTED;
   CTN_TRY(set_smem((const void*)k_tas_frame_norm, smem));
-  k_tas_frame_norm<<<dim3(pitch / TAS_TF, B), TAS_THREADS, smem, (cudaStream_t)stream>>>(w, gamma, beta, xn, N, frames, pitch, eps);
+  k_tas_frame_norm<<<dim3(pitch / TAS_TF, B), TAS_THREADS, smem, (cudaStream_t)stream>>>(w, gamma, beta, xn, N, frames, pitch, eps, nullptr,
+                                                                                         0, 0, 0);
   CTN_COUNT_LAUNCH();
   CTN_RETURN_IF_CUDA_ERR();
   return CTN_OK;
@@ -476,9 +499,9 @@ extern "C" int ctn_tas_lstm_fwd(const float* x, const float* const* w, float* ou
   if (!one) return CTN_ENOTBUILT;
   int occ = 0, nsm = 0, smem_optin = 0;
   device_limits(&nsm, &smem_optin);
-  cudaError_t e = cudaFuncSetAttribute((const void*)k_tas_lstm, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)geo.smem);
+  cudaError_t e = cudaFuncSetAttribute((const void*)k_tas_lstm<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)geo.smem);
   if (e != cudaSuccess) return (int)e;
-  if ((e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, k_tas_lstm, TAS_THREADS, geo.smem)) != cudaSuccess) return (int)e;
+  if ((e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, k_tas_lstm<false>, TAS_THREADS, geo.smem)) != cudaSuccess) return (int)e;
   if ((long long)occ * nsm < (long long)dirs * geo.cpd) return CTN_EUNSUPPORTED;  // the spinning CTAs could not all be resident
   cudaStream_t st = (cudaStream_t)stream;
   const int M = dirs * 4 * H;
@@ -516,6 +539,7 @@ extern "C" int ctn_tas_lstm_fwd(const float* x, const float* const* w, float* ou
   }
   CTN_TRY(ctn_pw(a, PRO_NONE, EPI_H, math, nullptr, st));
   LstmArgs la;
+  memset(&la, 0, sizeof(la));
   la.G = G;
   la.whh[0] = w[1];
   la.whh[1] = dirs == 2 ? w[5] : w[1];
@@ -534,7 +558,7 @@ extern "C" int ctn_tas_lstm_fwd(const float* x, const float* const* w, float* ou
   attr[0].val.cooperative = 1;
   cfg.attrs = attr;
   cfg.numAttrs = 1;
-  if ((e = cudaLaunchKernelEx(&cfg, k_tas_lstm, la)) != cudaSuccess) {
+  if ((e = cudaLaunchKernelEx(&cfg, k_tas_lstm<false>, la)) != cudaSuccess) {
     cudaGetLastError();
     return (int)e;
   }
@@ -586,4 +610,277 @@ extern "C" int ctn_tas_tail_fwd(const float* skip, const float* w, const float* 
   CTN_TRY(ctn_decoder_fwd(what, dec_w, out, B * S, N, frames, pitch, L, stride, crop_left, T, stream));
   if (latent) CTN_TRY(ctn_copy_from_pitch(what, latent, B * S * N, frames, pitch, st));
   return CTN_OK;
+}
+
+// ---- online (chunk-by-chunk) inference of the causal model (DESIGN.md section 18) ------------------------------------------------
+// Per push: k_online_enc (the Conv-TasNet online encoder and its carry) -> the frame norm of the chunk's columns -> per layer the
+// stacked-W_ih projection (ctn_pw, image built at init) and the carrying recurrence, skip = x + skip on the last layer of every
+// block after the first -> fc with the mask (+ the softmax over the sources) -> k_online_dec, which advances T0.  Every kernel
+// derives the push's frame count from the device counter, so the launch sequence depends on the config alone.
+namespace {
+
+struct TasOnline {
+  OnlineHdr* hdr;
+  float* enc_carry;          // [B][L - S]
+  float* dec_hist;           // [B S][N][L/S - 1]
+  float* hc;                 // [X R][B][2][H]: (h, c) of every layer
+  double* dummy;             // [B][2] sink of the projections' unused EPI_H statistics
+  size_t carry_bytes;        // the bytes above: zeroed by init and reset
+  std::vector<float*> wcat, bcat, img;  // per layer: W_ih (4H, F), b_ih + b_hh (4H), its image (tensor-core modes)
+  float* fc_img;
+  float* dec_w;              // (N, L): the flush has no parameter argument
+  // one chunk, (B, rows, pitch)
+  float *w, *xn, *G, *z0, *z1, *sk, *what;
+  float* hbuf;               // [2][TAS_GMAX][H]
+  unsigned* bar;             // [X R][32] barrier counters, zeroed by every push
+};
+
+int tas_layers(const ctn_tas_config_t* c) { return c->num_blocks * c->num_layers; }
+
+void tas_carve(Carver& cv, const ctn_tas_config_t* c, int B, int pitch, TasOnline* s) {
+  const int XR = tas_layers(c), H = c->hidden, N = c->n_basis, S = c->n_sources, L = c->kernel_size, St = c->stride;
+  s->hdr = cv.take<OnlineHdr>(1);
+  s->enc_carry = cv.take<float>((size_t)B * (L - St));
+  s->dec_hist = cv.take<float>((size_t)B * S * N * (L / St - 1));
+  s->hc = cv.take<float>((size_t)XR * B * 2 * H);
+  s->dummy = cv.take<double>((size_t)B * 2);
+  cv.off = (cv.off + 255) & ~(size_t)255;
+  s->carry_bytes = cv.off;
+  s->wcat.assign(XR, nullptr);
+  s->bcat.assign(XR, nullptr);
+  s->img.assign(XR, nullptr);
+  for (int i = 0; i < XR; ++i) {
+    const int F = i == 0 ? N : H;
+    s->wcat[i] = cv.take<float>((size_t)4 * H * F);
+    s->bcat[i] = cv.take<float>((size_t)4 * H);
+    if (c->math != CTN_MATH_FP32) s->img[i] = cv.take<float>(ctn_pw_wimg_bytes(4 * H, F, c->math) / sizeof(float));
+  }
+  s->fc_img = c->math != CTN_MATH_FP32 ? cv.take<float>(ctn_pw_wimg_bytes(S * N, H, c->math) / sizeof(float)) : nullptr;
+  s->dec_w = cv.take<float>((size_t)N * L);
+  const size_t bp = (size_t)B * pitch;
+  s->w = cv.take<float>(bp * N);
+  s->xn = cv.take<float>(bp * N);
+  s->G = cv.take<float>(bp * 4 * H);
+  s->z0 = cv.take<float>(bp * H);
+  s->z1 = cv.take<float>(bp * H);
+  s->sk = cv.take<float>(bp * H);
+  s->what = cv.take<float>(bp * S * N);
+  s->hbuf = cv.take<float>((size_t)2 * TAS_GMAX * H);
+  s->bar = cv.take<unsigned>((size_t)XR * 32);
+}
+
+// the config refusals, before any CUDA call
+int tas_online_check(const ctn_tas_config_t* c) {
+  if (!c) return CTN_EINVAL;
+  if (c->causal != 1) return CTN_EUNSUPPORTED;  // a non-causal model is bidirectional: its reverse pass needs the whole signal
+  if (c->gated) return CTN_EUNSUPPORTED;        // the gated encoder divides by the norm of the whole signal
+  if (c->n_basis <= 0 || c->kernel_size <= 0 || c->stride <= 0 || c->kernel_size % c->stride != 0 || c->hidden <= 0 ||
+      c->num_blocks <= 0 || c->num_layers <= 0 || c->n_sources <= 0 || !math_ok(c->math))
+    return CTN_EINVAL;
+  if ((size_t)c->n_basis * (c->kernel_size / c->stride - 1) * sizeof(float) > 48 * 1024) return CTN_EUNSUPPORTED;  // decoder history
+  return CTN_OK;
+}
+
+// the device's refusals (after LaunchScope: they query the current device): the recurrence geometry, its co-residency, the
+// frame norm's shared memory
+int tas_online_device_check(const ctn_tas_config_t* c, int B, int max_chunk_frames, LstmGeo* geo) {
+  if (!lstm_geo_here(c->hidden, 1, geo)) return CTN_EUNSUPPORTED;
+  const long long ngroups = (B + geo->gmax - 1) / geo->gmax;
+  if (ngroups * max_chunk_frames * geo->cpd >= 0x7fffffffLL) return CTN_EUNSUPPORTED;  // the barrier counters are 32-bit
+  int nsm = 0, smem_optin = 0, occ = 0;
+  device_limits(&nsm, &smem_optin);
+  if (sizeof(float) * (size_t)c->n_basis * TAS_TF > (size_t)(smem_optin > 48 * 1024 ? smem_optin : 48 * 1024)) return CTN_EUNSUPPORTED;
+  cudaError_t e = cudaFuncSetAttribute((const void*)k_tas_lstm<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)geo->smem);
+  if (e != cudaSuccess) return (int)e;
+  if ((e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, k_tas_lstm<true>, TAS_THREADS, geo->smem)) != cudaSuccess) return (int)e;
+  if ((long long)occ * nsm < geo->cpd) return CTN_EUNSUPPORTED;
+  return CTN_OK;
+}
+
+}  // namespace
+
+extern "C" int ctn_tas_online_state_bytes(const ctn_tas_config_t* cfg, int B, int max_chunk_frames, size_t* bytes) {
+  CTN_TRY(tas_online_check(cfg));
+  if (B <= 0 || max_chunk_frames <= 0 || !bytes) return CTN_EINVAL;
+  if (B > 65535) return CTN_EUNSUPPORTED;
+  if (ctn_online_enc_smem(cfg->kernel_size, cfg->stride, max_chunk_frames * cfg->stride) > 200 * 1024) return CTN_EUNSUPPORTED;
+  Carver cv(nullptr);
+  TasOnline s;
+  tas_carve(cv, cfg, B, ctn_pitch(max_chunk_frames), &s);
+  *bytes = cv.off + 256;
+  return CTN_OK;
+}
+
+extern "C" int ctn_tas_online_init(const ctn_tas_config_t* cfg, const ctn_tas_params_t* params, int B, int max_chunk_frames, void* state,
+                                   size_t state_bytes, ctn_stream_t stream) {
+  CTN_TRY(tas_online_check(cfg));
+  if (!params || !params->lstm || !params->fc_w || !params->dec_w || !state || B <= 0 || max_chunk_frames <= 0) return CTN_EINVAL;
+  const int XR = tas_layers(cfg), H = cfg->hidden, N = cfg->n_basis, S = cfg->n_sources;
+  for (int i = 0; i < 4 * XR; ++i)
+    if (!params->lstm[i]) return CTN_EINVAL;
+  if (((uintptr_t)state) & 255) return CTN_EALIGN;
+  size_t need = 0;
+  CTN_TRY(ctn_tas_online_state_bytes(cfg, B, max_chunk_frames, &need));
+  if (state_bytes < need) return CTN_EWORKSPACE;
+  LaunchScope scope(state);
+  LstmGeo geo;
+  CTN_TRY(tas_online_device_check(cfg, B, max_chunk_frames, &geo));
+  cudaStream_t st = (cudaStream_t)stream;
+  Carver cv(state);
+  TasOnline s;
+  tas_carve(cv, cfg, B, ctn_pitch(max_chunk_frames), &s);
+  cudaError_t e = cudaMemsetAsync(state, 0, s.carry_bytes, st);
+  if (e != cudaSuccess) return (int)e;
+  // the offline layer stacks W_ih, sums the biases and builds the image on every call; here once
+  std::vector<WimgJob> jobs;
+  for (int i = 0; i < XR; ++i) {
+    const int F = i == 0 ? N : H;
+    TasW p;
+    p.w_ih[0] = p.w_ih[1] = params->lstm[4 * i];
+    p.b_ih[0] = p.b_ih[1] = params->lstm[4 * i + 2];
+    p.b_hh[0] = p.b_hh[1] = params->lstm[4 * i + 3];
+    int gp = (int)(((size_t)4 * H * F + 255) / 256);
+    if (gp > 1024) gp = 1024;
+    k_tas_lstm_prep<<<gp, 256, 0, st>>>(p, s.wcat[i], s.bcat[i], F, 4 * H, 1);
+    CTN_COUNT_LAUNCH();
+    CTN_RETURN_IF_CUDA_ERR();
+    if (s.img[i]) jobs.push_back(WimgJob{s.wcat[i], s.img[i], 4 * H, F});
+  }
+  if (s.fc_img) jobs.push_back(WimgJob{params->fc_w, s.fc_img, S * N, H});
+  for (const WimgJob& j : jobs) CTN_TRY(ctn_pw_prepare_batch(&j, 1, cfg->math, false, st));  // as the offline layer and tail build them
+  e = cudaMemcpyAsync(s.dec_w, params->dec_w, sizeof(float) * (size_t)N * cfg->kernel_size, cudaMemcpyDeviceToDevice, st);
+  return e == cudaSuccess ? CTN_OK : (int)e;
+}
+
+extern "C" int ctn_tas_online_reset(const ctn_tas_config_t* cfg, void* state, int B, ctn_stream_t stream) {
+  CTN_TRY(tas_online_check(cfg));
+  if (!state || B <= 0) return CTN_EINVAL;
+  if (((uintptr_t)state) & 255) return CTN_EALIGN;
+  LaunchScope scope(state);
+  Carver cv(nullptr);
+  TasOnline s;
+  tas_carve(cv, cfg, B, CTN_TILE_T, &s);
+  cudaError_t e = cudaMemsetAsync(state, 0, s.carry_bytes, (cudaStream_t)stream);
+  return e == cudaSuccess ? CTN_OK : (int)e;
+}
+
+extern "C" int ctn_tas_online_push(const ctn_tas_config_t* cfg, const ctn_tas_params_t* params, void* state, const float* x, int B,
+                                   int max_chunk_frames, int n, float* y, ctn_stream_t stream) {
+  CTN_TRY(tas_online_check(cfg));
+  if (!params || !params->lstm || !params->enc_w || !params->gamma || !params->beta || !params->fc_w || !params->fc_b || !state || !x ||
+      !y || B <= 0 || max_chunk_frames <= 0)
+    return CTN_EINVAL;
+  const int L = cfg->kernel_size, S = cfg->stride, XR = tas_layers(cfg), H = cfg->hidden, N = cfg->n_basis, Ns = cfg->n_sources;
+  if (n <= 0 || n % S != 0 || n / S > max_chunk_frames) return CTN_EINVAL;
+  for (int i = 0; i < 4 * XR; ++i)
+    if (!params->lstm[i]) return CTN_EINVAL;
+  if (((uintptr_t)state) & 255) return CTN_EALIGN;
+  if (B > 65535) return CTN_EUNSUPPORTED;
+  LaunchScope scope(state);
+  LstmGeo geo;
+  CTN_TRY(tas_online_device_check(cfg, B, max_chunk_frames, &geo));
+  const float* one = one_ptr();
+  if (!one) return CTN_ENOTBUILT;
+  cudaStream_t st = (cudaStream_t)stream;
+  const int F = n / S, pitch = ctn_pitch(F);  // the chunk's layout: every scratch tensor is rewritten by each push
+  Carver cv(state);
+  TasOnline s;
+  tas_carve(cv, cfg, B, pitch, &s);
+  cudaError_t e = cudaMemsetAsync(s.bar, 0, sizeof(unsigned) * 32 * XR, st);
+  if (e != cudaSuccess) return (int)e;
+  {
+    StageTimer tm(CTN_ST_ENC, st);
+    CTN_TRY(ctn_online_enc(x, params->enc_w, s.enc_carry, s.w, s.hdr, B, N, L, S, n, pitch, cfg->enc_relu, st));
+  }
+  {
+    StageTimer tm(CTN_ST_HEAD, st);
+    const size_t smem = sizeof(float) * (size_t)N * TAS_TF;
+    CTN_TRY(set_smem((const void*)k_tas_frame_norm, smem));
+    k_tas_frame_norm<<<dim3(pitch / TAS_TF, B), TAS_THREADS, smem, st>>>(s.w, params->gamma, params->beta, s.xn, N, F, pitch, cfg->eps,
+                                                                         s.hdr, L, S, n);
+    CTN_COUNT_LAUNCH();
+    CTN_RETURN_IF_CUDA_ERR();
+  }
+  const float* in = s.xn;
+  for (int blk = 0, i = 0; blk < cfg->num_blocks; ++blk) {
+    for (int r = 0; r < cfg->num_layers; ++r, ++i) {
+      const bool last = r == cfg->num_layers - 1;
+      float* out = blk == 0 && last ? s.sk : (i & 1 ? s.z1 : s.z0);  // never the layer's input
+      {
+        StageTimer tm(CTN_ST_PW1, st);
+        PwArgs a;
+        memset(&a, 0, sizeof(a));
+        a.A = in; a.W = s.wcat[i]; a.D = s.G; a.B = B; a.M = 4 * H; a.K = i == 0 ? N : H; a.frames = F; a.pitch = pitch;
+        a.bias = s.bcat[i]; a.slope = one; a.stats_out = s.dummy; a.wimg = s.img[i];
+        CTN_TRY(ctn_pw(a, PRO_NONE, EPI_H, cfg->math, nullptr, st));
+      }
+      StageTimer tm(CTN_ST_DW, st);
+      LstmArgs la;
+      memset(&la, 0, sizeof(la));
+      la.G = s.G;
+      la.whh[0] = la.whh[1] = params->lstm[4 * i + 1];
+      la.out = out;
+      if (blk > 0 && last) la.skip_in = la.skip_out = s.sk;  // skip = x + skip (tasnet.py:369), in place
+      la.hbuf = s.hbuf; la.bar = s.bar + 32 * i;
+      la.B = B; la.H = H; la.T = F; la.pitch = pitch; la.dirs = 1; la.U = geo.U; la.cpd = geo.cpd; la.gmax = geo.gmax;
+      la.Hs = (H + 3) & ~3;
+      la.hc = s.hc + (size_t)i * B * 2 * H; la.hdr = s.hdr; la.L = L; la.S = S; la.n = n;
+      cudaLaunchConfig_t lc;
+      memset(&lc, 0, sizeof(lc));
+      lc.gridDim = dim3(geo.cpd);
+      lc.blockDim = dim3(TAS_THREADS);
+      lc.dynamicSmemBytes = geo.smem;
+      lc.stream = st;
+      cudaLaunchAttribute attr[1];
+      attr[0].id = cudaLaunchAttributeCooperative;
+      attr[0].val.cooperative = 1;
+      lc.attrs = attr;
+      lc.numAttrs = 1;
+      if ((e = cudaLaunchKernelEx(&lc, k_tas_lstm<true>, la)) != cudaSuccess) {
+        cudaGetLastError();
+        return (int)e;
+      }
+      CTN_COUNT_LAUNCH();
+      CTN_RETURN_IF_CUDA_ERR();
+      in = out;
+    }
+  }
+  {
+    StageTimer tm(CTN_ST_MASK, st);
+    PwArgs m;
+    memset(&m, 0, sizeof(m));
+    m.A = s.sk; m.W = params->fc_w; m.D = s.what; m.B = B; m.M = Ns * N; m.K = H; m.frames = F; m.pitch = pitch;
+    m.pro_slope = one; m.bias = params->fc_b; m.wenc = s.w; m.Nb = N; m.mask_logits = cfg->mask_softmax ? 1 : 0; m.wimg = s.fc_img;
+    CTN_TRY(ctn_pw(m, PRO_PRELU, EPI_MASK, cfg->math, nullptr, st));
+    if (cfg->mask_softmax) {
+      int gx = (int)(((size_t)N * pitch + 255) / 256);
+      if (gx > 256) gx = 256;
+      k_tas_softmax_src<<<dim3(gx, B), 256, 0, st>>>(s.what, s.w, Ns, N, F, pitch);
+      CTN_COUNT_LAUNCH();
+      CTN_RETURN_IF_CUDA_ERR();
+    }
+  }
+  StageTimer tm(CTN_ST_DEC, st);
+  return ctn_online_dec(s.what, s.dec_w, s.dec_hist, y, s.hdr, B * Ns, N, L, S, n, pitch, 1, st);
+}
+
+extern "C" int ctn_tas_online_flush(const ctn_tas_config_t* cfg, void* state, int B, float* y_tail, ctn_stream_t stream) {
+  CTN_TRY(tas_online_check(cfg));
+  const int L = cfg->kernel_size, S = cfg->stride, D = L - S;
+  // a zero-delay model (kernel_size == stride) has no tail: y_tail holds 0 samples and may be null
+  if (!state || (D > 0 && !y_tail) || B <= 0) return CTN_EINVAL;
+  if (((uintptr_t)state) & 255) return CTN_EALIGN;
+  LaunchScope scope(state);
+  cudaStream_t st = (cudaStream_t)stream;
+  Carver cv(state);
+  TasOnline s;
+  tas_carve(cv, cfg, B, CTN_TILE_T, &s);
+  long long T0 = 0;
+  cudaError_t e = cudaMemcpyAsync(&T0, &s.hdr->T0, sizeof(T0), cudaMemcpyDeviceToHost, st);
+  if (e == cudaSuccess) e = cudaStreamSynchronize(st);
+  if (e != cudaSuccess) return (int)e;
+  if (T0 < L) return CTN_EINVAL;  // no frame yet: the offline model needs T >= kernel_size
+  if (D == 0) return CTN_OK;
+  // the tail segments read the history only; `what` is not touched (pitch is unused)
+  return ctn_online_dec(s.what, s.dec_w, s.dec_hist, y_tail, s.hdr, B * cfg->n_sources, cfg->n_basis, L, S, 0, CTN_TILE_T, 0, st);
 }

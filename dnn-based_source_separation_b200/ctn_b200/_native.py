@@ -51,6 +51,18 @@ class Params(C.Structure):
 TOP_FIELDS = tuple(n for n, _ in Params._fields_ if n != "blocks")
 
 
+class TasConfig(C.Structure):
+    """ctn_tas_config_t: the online LSTM-TasNet's config"""
+    _fields_ = [(n, C.c_int32) for n in (
+        "n_basis", "kernel_size", "stride", "hidden", "num_blocks", "num_layers", "n_sources", "causal", "gated", "enc_relu",
+        "mask_softmax", "math")] + [("eps", C.c_float)]
+
+
+class TasParams(C.Structure):
+    """ctn_tas_params_t: lstm is a host array of 4 per layer (weight_ih, weight_hh, bias_ih, bias_hh), block-major"""
+    _fields_ = [("enc_w", _fp), ("gamma", _fp), ("beta", _fp), ("lstm", C.POINTER(_fp)), ("fc_w", _fp), ("fc_b", _fp), ("dec_w", _fp)]
+
+
 def build_params(slots, dev):
     """ctn_params_t over [(slot, tensor-or-None)], slot = a top-level field name or (block index, block field name); the block
     array spans the highest block index.  Every tensor must be float32 on `dev`; a non-contiguous one is passed as a contiguous
@@ -205,6 +217,11 @@ ctn_online_init = _sig("ctn_online_init", _i, C.POINTER(Config), C.POINTER(Param
 ctn_online_reset = _sig("ctn_online_reset", _i, C.POINTER(Config), _fp, _i, _fp)
 ctn_online_push = _sig("ctn_online_push", _i, C.POINTER(Config), C.POINTER(Params), _fp, _fp, _i, _i, _i, _fp, _fp)
 ctn_online_flush = _sig("ctn_online_flush", _i, C.POINTER(Config), _fp, _i, _fp, _fp)
+ctn_tas_online_state_bytes = _sig("ctn_tas_online_state_bytes", _i, C.POINTER(TasConfig), _i, _i, C.POINTER(_sz))
+ctn_tas_online_init = _sig("ctn_tas_online_init", _i, C.POINTER(TasConfig), C.POINTER(TasParams), _i, _i, _fp, _sz, _fp)
+ctn_tas_online_reset = _sig("ctn_tas_online_reset", _i, C.POINTER(TasConfig), _fp, _i, _fp)
+ctn_tas_online_push = _sig("ctn_tas_online_push", _i, C.POINTER(TasConfig), C.POINTER(TasParams), _fp, _fp, _i, _i, _i, _fp, _fp)
+ctn_tas_online_flush = _sig("ctn_tas_online_flush", _i, C.POINTER(TasConfig), _fp, _i, _fp, _fp)
 # recordings of any length: chunk plan, gather, permutation alignment, overlap-add, and the call around ctn_convtasnet_fwd
 ctn_chunk_plan = _sig("ctn_chunk_plan", _i, _i, _i, _i, C.POINTER(_i), _i)
 ctn_chunk_gather = _sig("ctn_chunk_gather", _i, _fp, _i, _i, _i, _i, _i, _i, _fp, _fp)
@@ -263,6 +280,7 @@ EXPORTED = [
     "ctn_sfm_tail_workspace_bytes", "ctn_sfm_tail_fwd",
     "ctn_tas_enc_gated_fwd", "ctn_tas_frame_norm_fwd", "ctn_tas_lstm_max_hidden", "ctn_tas_lstm_supported", "ctn_tas_lstm_group",
     "ctn_tas_lstm_workspace_bytes", "ctn_tas_lstm_fwd", "ctn_tas_tail_workspace_bytes", "ctn_tas_tail_fwd",
+    "ctn_tas_online_state_bytes", "ctn_tas_online_init", "ctn_tas_online_reset", "ctn_tas_online_push", "ctn_tas_online_flush",
     "ctn_galr_head_workspace_bytes", "ctn_galr_head_fwd", "ctn_galr_supported", "ctn_galr_inter_workspace_bytes", "ctn_galr_inter_fwd",
 ]
 

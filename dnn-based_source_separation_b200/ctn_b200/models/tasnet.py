@@ -9,6 +9,7 @@ so its checkpoints load with ``load_state_dict(strict=True)``.  Forward:
   * fc, the mask (sigmoid, or softmax over the sources), w * mask and the decoder -> ``ctn_tas_tail_fwd``.
 Everything stays channel-first and pitched, (B, C, ctn_pitch(T')), between the stages.
 Envelope: rnn_type='lstm', monaural 3-D input, sep_hidden_channels up to ``ctn_tas_lstm_max_hidden`` of the device; forward only.
+A causal model with the plain encoder also streams: ``model.online(batch_size, max_chunk)`` (models/online.py).
 """
 import os
 
@@ -226,6 +227,12 @@ class TasNet(nn.Module):
                                    self.decoder.conv_transpose1d.weight.data_ptr(), out.data_ptr(), N.ptr(latent), what.data_ptr(), B, Nb, Hd,
                                    S, frames, pitch, L, stride, pl, T, int(sep.mask_softmax), math, base, nbytes, st), "ctn_tas_tail_fwd")
         return out, latent
+
+    def online(self, batch_size=1, max_chunk=320):
+        """-> a streaming separator of a causal, plain-encoder model for ``batch_size`` streams and pushes of up to ``max_chunk``
+        samples (a multiple of the stride): see ``ctn_b200.models.online.TasOnlineSeparator``.  The numeric mode is fixed here."""
+        from .online import TasOnlineSeparator
+        return TasOnlineSeparator(self, batch_size, max_chunk)
 
     @classmethod
     def build_model(cls, model_path, load_state_dict=False):

@@ -449,6 +449,53 @@ int ctn_tas_tail_fwd(const float* skip, const float* w, const float* fc_w, const
                      float* what, int B, int N, int Hd, int S, int frames, int pitch, int L, int stride, int crop_left, int T, int softmax,
                      int math, void* workspace, size_t workspace_bytes, ctn_stream_t stream);
 
+/* Online (chunk-by-chunk) inference of the causal LSTM-TasNet, with the contract of ctn_online_*: B streams advance together; a push
+ * of n samples per stream returns n samples per source, delayed by D = kernel_size - stride.  With x = everything pushed since the last
+ * init / reset (T samples, T % stride == 0), Y = the concatenated push outputs and Z = the flush output: Y[..., :D] == 0 and
+ * cat(Y[..., D:], Z) == TasNet.forward(x).  Envelope: causal = 1 and gated = 0 (else CTN_EUNSUPPORTED: a non-causal model is
+ * bidirectional, and the gated encoder divides by the norm of the whole signal); rnn_type 'lstm', monaural; sigmoid or softmax mask;
+ * every math mode; hidden within ctn_tas_lstm_supported(F, hidden, 1).
+ * `state`: one device buffer of ctn_tas_online_state_bytes(cfg, B, max_chunk_frames) bytes, 256-byte aligned, owned by the caller: the
+ * sample counter, the encoder's input carry, the decoder's history, (h, c) of every LSTM layer, the stacked input weights, summed biases
+ * and weight images (built by ctn_tas_online_init, kept by ctn_tas_online_reset) and the scratch of one chunk.  Pushes read the counter
+ * from the state on the device, so a captured push replays.  The weights must not change after init.
+ * Push launches: 4 + 2 num_blocks num_layers (+ 1 with the softmax mask).  Every refusal comes before the first CUDA call, except the
+ * device envelope of the recurrence, which init and push check before their first launch. */
+typedef struct ctn_tas_config {
+  int32_t n_basis;      /* N */
+  int32_t kernel_size;  /* L */
+  int32_t stride;       /* L/2 by default */
+  int32_t hidden;       /* H (sep_hidden_channels) */
+  int32_t num_blocks;   /* sep_num_blocks */
+  int32_t num_layers;   /* sep_num_layers */
+  int32_t n_sources;    /* S */
+  int32_t causal;       /* must be 1 */
+  int32_t gated;        /* enc_basis == 'trainableGated': CTN_EUNSUPPORTED */
+  int32_t enc_relu;     /* enc_nonlinear == 'relu' */
+  int32_t mask_softmax; /* mask_nonlinear == 'softmax' (over the sources); else sigmoid */
+  int32_t math;         /* enum ctn_math of the input projections and fc */
+  float eps;            /* the Separator's frame-norm eps */
+} ctn_tas_config_t;
+
+typedef struct ctn_tas_params {
+  const float* enc_w;        /* encoder.conv1d.weight (N,1,L) */
+  const float* gamma;        /* separator.gamma (1,N,1) */
+  const float* beta;         /* separator.beta  (1,N,1) */
+  const float* const* lstm;  /* HOST array of 4 num_blocks num_layers device pointers, block-major, in torch order per layer k of
+                                separator.rnn.{block}: weight_ih_l{k} (4H,F), weight_hh_l{k} (4H,H), bias_ih_l{k}, bias_hh_l{k} (4H) */
+  const float* fc_w;         /* separator.fc.weight (S*N,H) */
+  const float* fc_b;         /* separator.fc.bias   (S*N) */
+  const float* dec_w;        /* decoder.conv_transpose1d.weight (N,1,L) */
+} ctn_tas_params_t;
+
+int ctn_tas_online_state_bytes(const ctn_tas_config_t* cfg, int B, int max_chunk_frames, size_t* bytes);
+int ctn_tas_online_init(const ctn_tas_config_t* cfg, const ctn_tas_params_t* params, int B, int max_chunk_frames, void* state,
+                        size_t state_bytes, ctn_stream_t stream);
+int ctn_tas_online_reset(const ctn_tas_config_t* cfg, void* state, int B, ctn_stream_t stream);
+int ctn_tas_online_push(const ctn_tas_config_t* cfg, const ctn_tas_params_t* params, void* state, const float* x, int B, int max_chunk_frames,
+                        int n, float* y, ctn_stream_t stream);
+int ctn_tas_online_flush(const ctn_tas_config_t* cfg, void* state, int B, float* y_tail, ctn_stream_t stream);
+
 /* ---- GALRNet path (src/models/galrnet.py, src/models/galr.py, csrc/ctn_galr.cu) ----
  *
  * The dual-path state is channels-last, (B,S,K,F); the intra-chunk block is ctn_bilstm_proj_fwd + ctn_dprnn_norm_res2_fwd with

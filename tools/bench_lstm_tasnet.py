@@ -104,7 +104,7 @@ def split(fn):
     tot = {"input_projections": 0.0, "recurrence": 0.0, "rest": 0.0}
     for i, e in enumerate(ks):
         ms = e.time_range.elapsed_us() / 1e3
-        if "k_tas_lstm(" in e.name or e.name.endswith("k_tas_lstm"):
+        if "k_tas_lstm(" in e.name or "k_tas_lstm<" in e.name or e.name.endswith("k_tas_lstm"):
             tot["recurrence"] += ms
         elif ("k_pw" in e.name and i != pw[-1]) or "k_tas_lstm_prep" in e.name or ("k_build_wimg" in e.name and i < pw[-1] - 1):
             tot["input_projections"] += ms
