@@ -15,6 +15,22 @@ from dptnet_ref import bilstm, bound, mha, segment_geometry, synth_state_dict  #
 
 DEFECTS = ("interleaved_encoding", "exponent_2f", "encoding_before_ln", "ln_over_tokens", "attention_within_chunk", "gln_per_sequence",
            "residual_after_gln", "fc_inv_bias_dropped", "outer_residual_omitted")
+# mistakes at the kernels' own edges, planted by tests/tas_galr_edges_ref.py: the gLN eps outside its sqrt, and the down- or
+# up-map skipping its last pass of PASS_ELEMS / F rows (the rows keep 0, or the block input where the block runs in place)
+EDGE_DEFECTS = ("galr_gln_eps_placement", "galr_down_last_pass_dropped", "galr_up_last_pass_dropped")
+PASS_ELEMS = 2048  # k_galr_down / k_galr_up: (256 / F) threads per row x 8 rows, so 2048 / F rows per pass
+MHA_ELEMS = 1 << 24  # scores per attention slice: long sequences go through mha in slices of sequences, to bound the memory
+
+
+def last_pass_start(rows, F):
+    return (rows - 1) // (PASS_ELEMS // F) * (PASS_ELEMS // F)
+
+
+def mha_sliced(z, sd, p, heads):
+    """mha over z (n, T, F) in slices of sequences (each sequence is independent)"""
+    n, T, _ = z.shape
+    step = max(1, MHA_ELEMS // (heads * T * T))
+    return torch.cat([mha(z[i:i + step], sd, p, heads) for i in range(0, n, step)])
 
 
 def pe_table(length, F, defect=None):
@@ -40,11 +56,12 @@ def intra_block(z, sd, p, eps):
     return (y - m) / torch.sqrt(v + eps) * sd[p + "norm1d.norm.weight"].double() + sd[p + "norm1d.norm.bias"].double() + z
 
 
-def inter_block(x, sd, p, heads, Q, eps, pe=None, defect=None):
+def inter_block(x, sd, p, heads, Q, eps, pe=None, defect=None, gn_eps=None):
     """LowDimensionGloballyAttentiveBlock (galr.py:161-197) on x (B, S, K, F) channels-last.  pe: (S*Q, F) encoding (fp64 of
-    the fp32 table), formed here when None."""
+    the fp32 table), formed here when None.  eps is the LayerNorm's; gn_eps the gLN's (eps when None)."""
     d = lambda k: sd[p + k].double()  # noqa: E731
     B, S, K, F = x.shape
+    gn_eps = eps if gn_eps is None else gn_eps
     if pe is None:
         pe = pe_table(S * Q, F, defect)
     pe = pe.reshape(S, Q, F)
@@ -57,20 +74,25 @@ def inter_block(x, sd, p, heads, Q, eps, pe=None, defect=None):
     z = (z - m) / torch.sqrt(v + eps) * d("norm2d_in.norm.weight") + d("norm2d_in.norm.bias")
     if defect != "encoding_before_ln":
         z = z + pe
+    if defect == "galr_down_last_pass_dropped":
+        z[:, :, last_pass_start(Q, F):] = 0
     if defect == "attention_within_chunk":
-        y = mha(z.reshape(B * S, Q, F), sd, p + "multihead_attn.", heads).reshape(B, S, Q, F)
+        y = mha_sliced(z.reshape(B * S, Q, F), sd, p + "multihead_attn.", heads).reshape(B, S, Q, F)
     else:
-        y = mha(z.permute(0, 2, 1, 3).reshape(B * Q, S, F), sd, p + "multihead_attn.", heads).reshape(B, Q, S, F).permute(0, 2, 1, 3)
+        y = mha_sliced(z.permute(0, 2, 1, 3).reshape(B * Q, S, F), sd, p + "multihead_attn.", heads).reshape(B, Q, S, F).permute(0, 2, 1, 3)
     u = y if defect == "residual_after_gln" else y + z
     dims = (1, 3) if defect == "gln_per_sequence" else (1, 2, 3)
     m = u.mean(dim=dims, keepdim=True)
     v = ((u - m) ** 2).mean(dim=dims, keepdim=True)
-    g = (u - m) / torch.sqrt(v + eps) * d("norm2d_out.norm.weight") + d("norm2d_out.norm.bias")
+    sd_ = torch.sqrt(v) + gn_eps if defect == "galr_gln_eps_placement" else torch.sqrt(v + gn_eps)
+    g = (u - m) / sd_ * d("norm2d_out.norm.weight") + d("norm2d_out.norm.bias")
     if defect == "residual_after_gln":
         g = g + z
     out = torch.einsum("bsqf,kq->bskf", g, d("fc_inv.weight"))
     if defect != "fc_inv_bias_dropped":
         out = out + d("fc_inv.bias").view(1, 1, K, 1)
+    if defect == "galr_up_last_pass_dropped":
+        out[:, :, last_pass_start(K, F):] = 0
     if defect != "outer_residual_omitted":
         out = out + x
     return out
