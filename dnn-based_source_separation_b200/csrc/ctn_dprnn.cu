@@ -105,18 +105,18 @@ __global__ void __launch_bounds__(256) k_sample_stats(const float* __restrict__ 
   // 128-bit loads only when every sample starts 16-byte aligned (Y is; sample b sits b*n floats further): else all scalar
   const size_t n4 = (n & 3) ? 0 : n / 4;
   double s = 0.0, ss = 0.0;
+  // every element in double before it is added: fp32 partials lose the variance under a DC offset
   for (size_t i0 = (size_t)blockIdx.x * blockDim.x; i0 < n4; i0 += (size_t)gridDim.x * blockDim.x * 4) {
-    float ls = 0.f, lss = 0.f;
 #pragma unroll
     for (int u = 0; u < 4; ++u) {
       const size_t i = i0 + (size_t)u * gridDim.x * blockDim.x + threadIdx.x;
       if (i < n4) {
         const float4 v = __ldg(p + i);
-        ls += (v.x + v.y) + (v.z + v.w);
-        lss = fmaf(v.x, v.x, fmaf(v.y, v.y, fmaf(v.z, v.z, fmaf(v.w, v.w, lss))));
+        const double x = v.x, y = v.y, z = v.z, w = v.w;
+        s += (x + y) + (z + w);
+        ss = fma(x, x, fma(y, y, fma(z, z, fma(w, w, ss))));
       }
     }
-    s += ls; ss += lss;
   }
   for (size_t i = n4 * 4 + (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (size_t)gridDim.x * blockDim.x) {
     const float v = Y[(size_t)b * n + i];
@@ -166,6 +166,7 @@ extern "C" int ctn_segment_fwd(const float* x, float* Z, int B, int F, int frame
     return CTN_EINVAL;
   const int Tp = frames + pad_left + pad_right;
   if (Tp < chunk_size) return CTN_EINVAL;
+  if (B > 65535) return CTN_EUNSUPPORTED;  // the batch is the grid's z (y) axis
   const int S = (Tp - chunk_size) / hop_size + 1;  // F.unfold drops a ragged tail (transform.py:21)
   cudaStream_t st = (cudaStream_t)stream;
   if (channels_last) {
@@ -191,6 +192,7 @@ extern "C" int ctn_overlap_add_fwd(const float* Z, float* y, int B, int F, int S
   if (!Z || !y || B <= 0 || F <= 0 || S <= 0 || chunk_size <= 0 || hop_size <= 0 || crop_left < 0 || T_out <= 0 || out_pitch < T_out)
     return CTN_EINVAL;
   if (crop_left + T_out > (S - 1) * hop_size + chunk_size) return CTN_EINVAL;
+  if (B > 65535) return CTN_EUNSUPPORTED;  // the batch is the grid's z (y) axis
   cudaStream_t st = (cudaStream_t)stream;
   if (channels_last) {
     k_overlap_add_cl<<<dim3((out_pitch + 31) / 32, (F + 31) / 32, B), dim3(32, 8), 0, st>>>(Z, y, F, S, chunk_size, hop_size, crop_left, T_out,
@@ -209,6 +211,7 @@ extern "C" int ctn_dprnn_norm_res_fwd(const float* Y, const float* R, const floa
                                       int D2, int F, float eps, int swap, double* scratch, ctn_stream_t stream) {
   LaunchScope scope(Y);
   if (!Y || !R || !gamma || !beta || !out || !scratch || B <= 0 || D1 <= 0 || D2 <= 0 || F <= 0) return CTN_EINVAL;
+  if (B > 65535) return CTN_EUNSUPPORTED;  // the batch is the grid's y axis
   if (swap && (out == Y || out == R)) return CTN_EINVAL;  // the path swap cannot run in place
   if ((((uintptr_t)Y) | ((uintptr_t)R) | ((uintptr_t)out) | ((uintptr_t)gamma) | ((uintptr_t)beta)) & 15) return CTN_EALIGN;
   cudaStream_t st = (cudaStream_t)stream;

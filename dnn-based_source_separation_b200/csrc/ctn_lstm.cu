@@ -223,6 +223,8 @@ int launch_bilstm(const LstmArgs& a, size_t smem, cudaStream_t st) {
 }
 
 // Y = P0 + P1 + bias (the Linear of dprnn.py:87 / 139 split over the two directions): gLN statistics of it ...
+// Every element goes into double before it is added (as k_sample_part of ctn_dptnet.cu): fp32 runs of 16 values lose the
+// variance under a DC offset far above the spread (DESIGN 19 gives the rows that failed on an H100 before this).
 __global__ void __launch_bounds__(256) k_sample_stats2(const float* __restrict__ P0, const float* __restrict__ P1,
                                                        const float* __restrict__ bias, size_t n, int F, double* __restrict__ stats) {
   __shared__ double red[64];
@@ -232,19 +234,16 @@ __global__ void __launch_bounds__(256) k_sample_stats2(const float* __restrict__
   const size_t n4 = n / 4;  // F % 4 == 0
   double s = 0.0, ss = 0.0;
   for (size_t i0 = (size_t)blockIdx.x * blockDim.x * 4; i0 < n4; i0 += (size_t)gridDim.x * blockDim.x * 4) {
-    float ls = 0.f, lss = 0.f;
 #pragma unroll
     for (int u = 0; u < 4; ++u) {
       const size_t i = i0 + (size_t)u * blockDim.x + threadIdx.x;
       if (i < n4) {
         const float4 a = __ldg(p0 + i), c = __ldg(p1 + i), bb = __ldg(reinterpret_cast<const float4*>(bias + (i * 4) % F));
-        const float x = a.x + c.x + bb.x, y = a.y + c.y + bb.y, z = a.z + c.z + bb.z, w = a.w + c.w + bb.w;
-        ls += (x + y) + (z + w);
-        lss = fmaf(x, x, fmaf(y, y, fmaf(z, z, fmaf(w, w, lss))));
+        const double x = a.x + c.x + bb.x, y = a.y + c.y + bb.y, z = a.z + c.z + bb.z, w = a.w + c.w + bb.w;
+        s += (x + y) + (z + w);
+        ss = fma(x, x, fma(y, y, fma(z, z, fma(w, w, ss))));
       }
     }
-    s += ls;
-    ss += lss;
   }
   block_sum2_d(s, ss, red);
   if (threadIdx.x == 0) { atomicAdd(&stats[2 * b], s); atomicAdd(&stats[2 * b + 1], ss); }
@@ -328,7 +327,8 @@ int bilstm_proj(const float* z, int NSEQ, int T, int F, int H, const float* cons
   if ((w_fc == nullptr) != (P == nullptr)) return CTN_EINVAL;
   if (!w_fc && !hout) return CTN_EINVAL;
   const int Fp = w_fc ? Fo : 0;
-  if (!lstm_supported(F, H, Fp)) return CTN_EUNSUPPORTED;
+  // Fo = 0 names the envelope without a projection: with w_fc the image would hold projection slabs the workspace size omits
+  if (!lstm_supported(F, H, Fp) || (w_fc && Fp == 0)) return CTN_EUNSUPPORTED;
   if (workspace_bytes < lstm_ws_bytes(F, H, Fp)) return CTN_EWORKSPACE;
   if ((((uintptr_t)z) | ((uintptr_t)P) | ((uintptr_t)hout) | ((uintptr_t)workspace)) & 15) return CTN_EALIGN;
   const size_t fixed = lstm_fixed_smem(F, H);

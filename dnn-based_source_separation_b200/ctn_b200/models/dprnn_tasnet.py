@@ -133,8 +133,10 @@ class DPRNNTasNet(nn.Module):
         if torch.is_grad_enabled() and any(p.requires_grad for p in self.parameters()):
             raise NotImplementedError("the DPRNN-TasNet path is forward-only: call under torch.no_grad()")
         x = input.contiguous()
-        dev = N.require_cuda(x)
         B, _, T = x.shape
+        if B > 65535:  # segmentation, overlap-add and the gLN + residual put the batch on a grid axis of at most 65535 blocks
+            raise NotImplementedError("batch_size={} is outside the DPRNN-TasNet kernels' launch limit (batch_size <= 65535)".format(B))
+        dev = N.require_cuda(x)
         sep = self.separator
         sep.math = self.math if self.math is not None else sep.math
         frames, pl, pr = N.frames_of(T, self.kernel_size, self.stride)

@@ -272,6 +272,8 @@ int ctn_separator_fwd(const ctn_config_t* cfg, const ctn_params_t* params, const
  * `hop_size` of the padded sequence, S = (frames + pad_left + pad_right - chunk_size) / hop_size + 1.
  * channels_last = 0: Z (B,F,S,chunk) -- the reference layout;  1: Z (B,S,chunk,F) -- the batch_first layout the intra-chunk
  * LSTM consumes, i.e. the permute of src/models/dprnn.py:83-84 folded in. */
+/* B <= 65535 (the batch is a grid axis): larger batches are refused with CTN_EUNSUPPORTED before any launch, here and in
+ * ctn_overlap_add_fwd and ctn_dprnn_norm_res_fwd. */
 int ctn_segment_fwd(const float* x, float* Z, int B, int F, int frames, int pitch, int chunk_size, int hop_size, int pad_left,
                     int pad_right, int channels_last, ctn_stream_t stream);
 /* OverlapAdd1d.forward, src/models/transform.py:46-62, fused with the crop of dprnn_tasnet.py:347: y (B,F,out_pitch),
@@ -281,7 +283,9 @@ int ctn_overlap_add_fwd(const float* Z, float* y, int B, int F, int S, int chunk
                         int out_pitch, int channels_last, ctn_stream_t stream);
 /* Tail of IntraChunkRNN / InterChunkRNN.forward, src/models/dprnn.py:87-94 / 140-148: out = gLN(Y; gamma, beta) + R on
  * channels-last tensors (B,D1,D2,F) (gLN = GroupNorm(1,F): per-sample statistics over D1*D2*F values).  swap = 1 stores out as
- * (B,D2,D1,F) -- the layout of the other path (the permutes of dprnn.py:83, 91, 136, 144-146).  scratch: double[B][2]. */
+ * (B,D2,D1,F) -- the layout of the other path (the permutes of dprnn.py:83, 91, 136, 144-146).  scratch: double[B][2].  The
+ * statistics add every element in double (one partial per CTA, added with atomics), so a DC offset far above the spread keeps its
+ * variance.  B <= 65535; every refusal comes before the first launch.  2 launches. */
 int ctn_dprnn_norm_res_fwd(const float* Y, const float* R, const float* gamma, const float* beta, float* out, int B, int D1, int D2,
                            int F, float eps, int swap, double* scratch, ctn_stream_t stream);
 /* Bidirectional LSTM + the 2H -> F Linear of a dual-path block, src/models/dprnn.py:85-87 / 138-139 (nn.LSTM(batch_first,
@@ -291,14 +295,16 @@ int ctn_dprnn_norm_res_fwd(const float* Y, const float* R, const float* gamma, c
  * w_fc (Fo,2H) nullable.  P (2,NSEQ,T,Fo): partial projections W_fc[:, dir*H:(dir+1)*H] h_dir WITHOUT the Linear's bias -- the
  * Linear output is P[0] + P[1] + bias (ctn_dprnn_norm_res2_fwd consumes it in that form).  hout (NSEQ,T,2H) nullable: the LSTM
  * output itself (forward direction in [:H], reverse in [H:]).  Envelope: F, H in {32,64,128}, Fo in {32,64,96,128}
- * (ctn_bilstm_supported); workspace >= ctn_bilstm_workspace_bytes(F,H,Fo), 256-byte aligned.  z_absmax (nullable): device word holding
+ * (ctn_bilstm_supported; Fo = 0 only without w_fc); workspace >= ctn_bilstm_workspace_bytes(F,H,Fo), 16-byte aligned.  z_absmax (nullable): device word holding
  * the bit pattern of max|z| (the fp16 operand scale of x is derived from it); null = measured here with one more pass over z. */
 int ctn_bilstm_supported(int F, int H, int Fo);
 size_t ctn_bilstm_workspace_bytes(int F, int H, int Fo);
 int ctn_bilstm_proj_fwd(const float* z, int NSEQ, int T, int F, int H, const float* const* w, const float* w_fc, int Fo, float* P,
                         float* hout, const unsigned* z_absmax, void* workspace, size_t workspace_bytes, ctn_stream_t stream);
 /* ctn_dprnn_norm_res_fwd with Y = P[0] + P[1] + fc_bias, P (2,B,D1,D2,F) as ctn_bilstm_proj_fwd leaves it (F % 4 == 0).
- * out_absmax (nullable): receives the bit pattern of max|out| -- the z_absmax of the next ctn_bilstm_proj_fwd. */
+ * out_absmax (nullable): receives the bit pattern of max|out| -- the z_absmax of the next ctn_bilstm_proj_fwd.  Statistics as
+ * above, each element of P[0] + P[1] + fc_bias in double.  F <= 1024, B <= 65535; every refusal comes before the first launch.
+ * 2 launches. */
 int ctn_dprnn_norm_res2_fwd(const float* P, const float* fc_bias, const float* R, const float* gamma, const float* beta, float* out,
                             int B, int D1, int D2, int F, float eps, int swap, double* scratch, unsigned* out_absmax, ctn_stream_t stream);
 /* ---- DPTNet path: the dual-path transformer (src/models/dptnet.py) ----
