@@ -55,21 +55,19 @@ extern "C" int ctn_pointwise_conv1d_fwd(const float* x, const float* W, const fl
   if (((uintptr_t)x) & 15) return CTN_EALIGN;  // 128-bit operand loads
   const size_t ybytes = ((size_t)B * M * pitch * sizeof(float) + 255) & ~(size_t)255;
   const size_t wbytes = math != CTN_MATH_FP32 ? ctn_pw_wimg_bytes(M, K, math) + 256 : 0;
-  if (workspace_bytes < ybytes + wbytes + (size_t)B * 2 * sizeof(double) + 64 * sizeof(float) + 512) return CTN_EWORKSPACE;
+  if (workspace_bytes < ybytes + wbytes + (size_t)B * 2 * sizeof(double) + 512) return CTN_EWORKSPACE;
   cudaStream_t st = (cudaStream_t)stream;
   float* yp = (float*)workspace;
   float* wimg = (float*)((char*)workspace + ybytes);
   double* stats = (double*)((char*)workspace + ybytes + ((wbytes + 255) & ~(size_t)255));
-  float* one = (float*)(stats + 2 * B);
   PwArgs a;
   memset(&a, 0, sizeof(a));
   a.A = x; a.W = W; a.D = yp; a.B = B; a.M = M; a.K = K; a.frames = frames; a.pitch = pitch;
   int epi = EPI_RAW;
   if (bias) {  // bias add = the EPI_H epilogue with a PReLU slope of 1 (identity); its statistics go to scratch
-    const float onev = 1.f;
-    cudaError_t e = cudaMemcpyAsync(one, &onev, sizeof(float), cudaMemcpyHostToDevice, st);
-    if (e != cudaSuccess) return (int)e;
-    e = cudaMemsetAsync(stats, 0, sizeof(double) * 2 * B, st);
+    const float* one = ctn_device_one();
+    if (!one) return CTN_ENOTBUILT;
+    cudaError_t e = cudaMemsetAsync(stats, 0, sizeof(double) * 2 * B, st);
     if (e != cudaSuccess) return (int)e;
     a.bias = bias; a.slope = one; a.stats_out = stats;
     epi = EPI_H;

@@ -14,7 +14,7 @@ namespace {
 
 // ---- segmentation ---------------------------------------------------------------------------------------------------
 // xp = zero-pad(x, pad_left, .) (dprnn_tasnet.py:339-345); chunk s covers padded frames [s*P, s*P + K) (transform.py:25).
-// layout 1 (channels-last): Z[b][s][k][f];  layout 0 (reference): Z[b][f][s][k].
+// channels-last (layout 1): Z[b][s][k][f].
 // grid (ceil(Tp/32), ceil(F/32), B), block (32, 8): a 32 (frames) x 32 (channels) tile is transposed through shared memory
 // so that both the reads (frames contiguous) and the channels-last writes (channels contiguous) are coalesced.
 __global__ void __launch_bounds__(256) k_segment_cl(const float* __restrict__ x, float* __restrict__ Z, int F, int frames, int pitch,
@@ -36,17 +36,19 @@ __global__ void __launch_bounds__(256) k_segment_cl(const float* __restrict__ x,
     for (int s = s_hi; s >= 0 && s * P + K > tp; --s) Z[(((size_t)b * S + s) * K + (tp - s * P)) * F + f] = v;
   }
 }
-__global__ void __launch_bounds__(256) k_segment_ref(const float* __restrict__ x, float* __restrict__ Z, int F, int frames, int pitch,
-                                                     int pad_left, int S, int K, int P) {
-  // one thread per output element, k fastest (reads are contiguous along k)
-  const size_t n = (size_t)F * S * K;
-  const int b = blockIdx.y;
-  for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (size_t)gridDim.x * blockDim.x) {
-    const int k = (int)(i % K);
-    const int s = (int)((i / K) % S);
-    const int f = (int)(i / ((size_t)K * S));
-    const int t = s * P + k - pad_left;
-    Z[(size_t)b * n + i] = (t >= 0 && t < frames) ? x[((size_t)b * F + f) * pitch + t] : 0.f;
+// channel-first (rows of z_pitch >= S K): Z[b][f][s K + k] = xp[b][f][s P + k], columns [S K, z_pitch) = 0.  grid
+// (ceil(z_pitch / 256), min(B F, 65535)), the (b, f) rows strided over y, so no channel count is refused.
+__global__ void __launch_bounds__(256) k_segment_cf(const float* __restrict__ x, float* __restrict__ Z, long long BF, int frames, int pitch,
+                                                    int pad_left, int S, int K, int P, long long z_pitch) {
+  const long long i = (long long)blockIdx.x * 256 + threadIdx.x;
+  if (i >= z_pitch) return;
+  for (long long bf = blockIdx.y; bf < BF; bf += gridDim.y) {
+    float v = 0.f;
+    if (i < (long long)S * K) {
+      const int s = (int)(i / K), k = (int)(i % K), tt = s * P + k - pad_left;
+      if (tt >= 0 && tt < frames) v = __ldg(x + bf * pitch + tt);
+    }
+    Z[bf * z_pitch + i] = v;
   }
 }
 
@@ -76,21 +78,22 @@ __global__ void __launch_bounds__(256) k_overlap_add_cl(const float* __restrict_
     if (f < F && t < out_pitch) y[((size_t)b * F + f) * out_pitch + t] = t < T_out ? tile[threadIdx.x][j] : 0.f;
   }
 }
-__global__ void __launch_bounds__(256) k_overlap_add_ref(const float* __restrict__ Z, float* __restrict__ y, int F, int S, int K, int P,
-                                                         int crop_left, int T_out, int out_pitch) {
-  const int b = blockIdx.y;
-  const size_t n = (size_t)F * out_pitch;
-  for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (size_t)gridDim.x * blockDim.x) {
-    const int t = (int)(i % out_pitch), f = (int)(i / out_pitch);
+// channel-first: chunk s of row (b, f) at Z[b][f][s K .. s K + K) of a z_pitch row; grid as k_segment_cf over out_pitch
+__global__ void __launch_bounds__(256) k_overlap_add_cf(const float* __restrict__ Z, float* __restrict__ y, long long BF, int S, int K, int P,
+                                                        long long z_pitch, int crop_left, int T_out, int out_pitch) {
+  const int t = blockIdx.x * 256 + threadIdx.x;
+  if (t >= out_pitch) return;
+  for (long long bf = blockIdx.y; bf < BF; bf += gridDim.y) {
     float acc = 0.f;
     if (t < T_out) {
       const int tp = t + crop_left;
       int s_lo = (tp - K + 1 <= 0) ? 0 : (tp - K + P) / P;
       int s_hi = tp / P;
       if (s_hi > S - 1) s_hi = S - 1;
-      for (int s = s_lo; s <= s_hi; ++s) acc += Z[(((size_t)b * F + f) * S + s) * K + (tp - s * P)];
+      const float* z = Z + bf * z_pitch;
+      for (int s = s_lo; s <= s_hi; ++s) acc += __ldg(z + (size_t)s * K + tp - s * P);
     }
-    y[(size_t)b * n + i] = acc;
+    y[bf * out_pitch + t] = acc;
   }
 }
 
@@ -159,17 +162,31 @@ __global__ void __launch_bounds__(256) k_norm_res(const float* __restrict__ Y, c
 
 }  // namespace
 
+// rows of the channel-first grid: (b, f) strided over at most 65535 CTAs of y
+static unsigned cf_rows(long long BF) { return (unsigned)(BF < 65535 ? BF : 65535); }
+
+// the row pitch a layout argument selects for S chunks of K frames: 0 for channels-last (1), S K for the dense channel-first
+// layout (0), the argument itself from S K on; -1 for any other value
+static long long row_pitch(int layout, int S, int K) {
+  const long long n = (long long)S * K;
+  if (layout == 1) return 0;
+  if (layout == 0) return n;
+  return layout >= n ? layout : -1;
+}
+
 extern "C" int ctn_segment_fwd(const float* x, float* Z, int B, int F, int frames, int pitch, int chunk_size, int hop_size,
-                               int pad_left, int pad_right, int channels_last, ctn_stream_t stream) {
+                               int pad_left, int pad_right, int layout, ctn_stream_t stream) {
   LaunchScope scope(x);
   if (!x || !Z || B <= 0 || F <= 0 || frames <= 0 || pitch < frames || chunk_size <= 0 || hop_size <= 0 || pad_left < 0 || pad_right < 0)
     return CTN_EINVAL;
   const int Tp = frames + pad_left + pad_right;
   if (Tp < chunk_size) return CTN_EINVAL;
-  if (B > 65535) return CTN_EUNSUPPORTED;  // the batch is the grid's z (y) axis
   const int S = (Tp - chunk_size) / hop_size + 1;  // F.unfold drops a ragged tail (transform.py:21)
+  const long long z_pitch = row_pitch(layout, S, chunk_size);
+  if (z_pitch < 0) return CTN_EINVAL;
+  if (B > 65535) return CTN_EUNSUPPORTED;  // the batch is the channels-last grid's z axis
   cudaStream_t st = (cudaStream_t)stream;
-  if (channels_last) {
+  if (!z_pitch) {
     const int Tc = (S - 1) * hop_size + chunk_size;  // frames that land in some chunk
     if (hop_size > chunk_size) {  // gaps between chunks: not every cell is written by the scatter below
       cudaError_t e = cudaMemsetAsync(Z, 0, sizeof(float) * (size_t)B * S * chunk_size * F, st);
@@ -177,9 +194,9 @@ extern "C" int ctn_segment_fwd(const float* x, float* Z, int B, int F, int frame
     }
     k_segment_cl<<<dim3((Tc + 31) / 32, (F + 31) / 32, B), dim3(32, 8), 0, st>>>(x, Z, F, frames, pitch, pad_left, S, chunk_size, hop_size, Tc);
   } else {
-    const size_t n = (size_t)F * S * chunk_size;
-    k_segment_ref<<<dim3((unsigned)((n + 1023) / 1024 < 4096 ? (n + 1023) / 1024 : 4096), B), 256, 0, st>>>(x, Z, F, frames, pitch, pad_left, S,
-                                                                                                         chunk_size, hop_size);
+    const long long BF = (long long)B * F;
+    k_segment_cf<<<dim3((unsigned)((z_pitch + 255) / 256), cf_rows(BF)), 256, 0, st>>>(x, Z, BF, frames, pitch, pad_left, S, chunk_size, hop_size,
+                                                                            z_pitch);
   }
   CTN_COUNT_LAUNCH();
   CTN_RETURN_IF_CUDA_ERR();
@@ -187,20 +204,22 @@ extern "C" int ctn_segment_fwd(const float* x, float* Z, int B, int F, int frame
 }
 
 extern "C" int ctn_overlap_add_fwd(const float* Z, float* y, int B, int F, int S, int chunk_size, int hop_size, int crop_left,
-                                   int T_out, int out_pitch, int channels_last, ctn_stream_t stream) {
+                                   int T_out, int out_pitch, int layout, ctn_stream_t stream) {
   LaunchScope scope(Z);
   if (!Z || !y || B <= 0 || F <= 0 || S <= 0 || chunk_size <= 0 || hop_size <= 0 || crop_left < 0 || T_out <= 0 || out_pitch < T_out)
     return CTN_EINVAL;
   if (crop_left + T_out > (S - 1) * hop_size + chunk_size) return CTN_EINVAL;
-  if (B > 65535) return CTN_EUNSUPPORTED;  // the batch is the grid's z (y) axis
+  const long long z_pitch = row_pitch(layout, S, chunk_size);
+  if (z_pitch < 0) return CTN_EINVAL;
+  if (B > 65535) return CTN_EUNSUPPORTED;  // the batch is the channels-last grid's z axis
   cudaStream_t st = (cudaStream_t)stream;
-  if (channels_last) {
+  if (!z_pitch) {
     k_overlap_add_cl<<<dim3((out_pitch + 31) / 32, (F + 31) / 32, B), dim3(32, 8), 0, st>>>(Z, y, F, S, chunk_size, hop_size, crop_left, T_out,
                                                                                         out_pitch);
   } else {
-    const size_t n = (size_t)F * out_pitch;
-    k_overlap_add_ref<<<dim3((unsigned)((n + 255) / 256 < 8192 ? (n + 255) / 256 : 8192), B), 256, 0, st>>>(Z, y, F, S, chunk_size, hop_size,
-                                                                                                         crop_left, T_out, out_pitch);
+    const long long BF = (long long)B * F;
+    k_overlap_add_cf<<<dim3((out_pitch + 255) / 256, cf_rows(BF)), 256, 0, st>>>(Z, y, BF, S, chunk_size, hop_size, z_pitch, crop_left, T_out,
+                                                                                 out_pitch);
   }
   CTN_COUNT_LAUNCH();
   CTN_RETURN_IF_CUDA_ERR();

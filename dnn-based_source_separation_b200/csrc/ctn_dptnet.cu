@@ -10,9 +10,10 @@
 //     one CTA per (b, d1) row sums the row in double in a fixed order (no atomics: repeated calls give the same bits), then
 //     normalises it, storing the intra <-> inter swap on the way out.
 //   * the head's gLN (dptnet.py:337) is per SAMPLE over the segmented tensor, duplicated overlap frames and padding zeros included.
-//   * the tail is PReLU -> map 1x1 -> GTU1d (map and map_gate in one 1x1 of 2N rows) -> mask nonlinearity -> w * mask -> decoder.
+//   * the head (bottleneck 1x1, optional: GALRNet has none) and the tail are shared by DPTNet, GALRNet and SepFormer.  The tail is
+//     PReLU -> map 1x1 -> GTU1d (map and map_gate in one 1x1 of 2N rows) [-> bottleneck_conv1d_out, SepFormer] -> mask
+//     nonlinearity -> w * mask -> decoder; all weight images of a call are built in one batch.
 #include <math.h>
-#include <string.h>
 
 #include "ctn_internal.h"
 
@@ -183,22 +184,40 @@ __global__ void __launch_bounds__(256) k_sample_apply(float* __restrict__ z, siz
   }
 }
 
-// GTU1d + mask nonlinearity + w * mask: g (B*S, 2N, pitch) = [map; map_gate] (x) + bias, w (B, N, pitch) ->
-// what[b s][n][t] = act(tanh(g[n]) sigmoid(g[N + n])) w[b][n][t], act = ReLU or sigmoid; columns [frames, pitch) = 0.
-__global__ void __launch_bounds__(256) k_gtu_mask(const float* __restrict__ g, const float* __restrict__ w, float* __restrict__ what,
-                                                  int S, int N, int frames, int pitch, int mask_relu) {
-  const int bs = blockIdx.y, b = bs / S;
+// GTU1d and the mask, one or both per launch, on the (R = B S, ., pitch) layout, columns [frames, pitch) = 0:
+//   GTU:  v = tanh(g[n]) sigmoid(g[N + n]) from g (R, 2N, pitch) = [map; map_gate] (x) + bias;  otherwise v = x (R, N, pitch);
+//   MASK: out[r][n][t] = act(v) w[r / S][n][t], act = ReLU (mask_relu) or sigmoid;  otherwise out = v.
+// grid (<= 256, R), block 256.
+template <bool GTU, bool MASK>
+__global__ void __launch_bounds__(256) k_gtu_mask(const float* __restrict__ x, const float* __restrict__ w, float* __restrict__ out, int S,
+                                                  int N, int frames, int pitch, int mask_relu) {
+  const int r = blockIdx.y, b = r / S;
   for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < (size_t)N * pitch; i += (size_t)gridDim.x * blockDim.x) {
     const int n = (int)(i / pitch), t = (int)(i % pitch);
     float v = 0.f;
     if (t < frames) {
-      const float a = g[((size_t)bs * 2 * N + n) * pitch + t], gt = g[((size_t)bs * 2 * N + N + n) * pitch + t];
-      const float u = tanhf(a) * (1.f / (1.f + expf(-gt)));
-      const float mk = mask_relu ? fmaxf(u, 0.f) : 1.f / (1.f + expf(-u));
-      v = mk * w[((size_t)b * N + n) * pitch + t];
+      if (GTU) {
+        const float a = x[((size_t)r * 2 * N + n) * pitch + t], gt = x[((size_t)r * 2 * N + N + n) * pitch + t];
+        v = tanhf(a) * (1.f / (1.f + expf(-gt)));
+      } else {
+        v = x[(size_t)r * N * pitch + i];
+      }
+      if (MASK) {
+        const float mk = mask_relu ? fmaxf(v, 0.f) : 1.f / (1.f + expf(-v));
+        v = mk * w[((size_t)b * N + n) * pitch + t];
+      }
     }
-    what[(size_t)bs * N * pitch + i] = v;
+    out[(size_t)r * N * pitch + i] = v;
   }
+}
+template <bool GTU, bool MASK>
+int launch_gtu_mask(const float* x, const float* w, float* out, int R, int S, int N, int frames, int pitch, int mask_relu, cudaStream_t st) {
+  int gx = (int)(((size_t)N * pitch + 255) / 256);
+  if (gx > 256) gx = 256;
+  k_gtu_mask<GTU, MASK><<<dim3(gx, R), 256, 0, st>>>(x, w, out, S, N, frames, pitch, mask_relu);
+  CTN_COUNT_LAUNCH();
+  CTN_RETURN_IF_CUDA_ERR();
+  return CTN_OK;
 }
 
 bool mha_ok(int F, int heads) {
@@ -207,26 +226,46 @@ bool mha_ok(int F, int heads) {
   return D == 8 || D == 16 || D == 32 || D == 64;
 }
 
-size_t up256(size_t b) { return (b + 255) & ~(size_t)255; }
-
-// device scalar 1.0: the PReLU slope that turns the EPI_H epilogue of ctn_pw into a plain bias add.  The source has static
-// storage: a CUDA graph that captures this copy reads it again at every replay.
-int put_one(float* one, cudaStream_t st) {
-  static const float onev = 1.f;
-  cudaError_t e = cudaMemcpyAsync(one, &onev, sizeof(float), cudaMemcpyHostToDevice, st);
-  return e == cudaSuccess ? CTN_OK : (int)e;
+struct MhaWs { float *qkv, *o; };
+void carve_mha(Carver& cv, int NSEQ, int T, int F, MhaWs* ws) {
+  const size_t tok = (size_t)NSEQ * T;
+  ws->qkv = cv.take<float>(tok * 3 * F);
+  ws->o = cv.take<float>(tok * F);
 }
 
-// 1x1 with bias on the pitched layout through ctn_pw (EPI_H, slope 1); stats: double[2 B] scratch the epilogue writes
-int pw_bias(const float* A, const float* W, const float* bias, float* D, int B, int M, int K, int frames, int pitch, const float* one,
-            double* stats, int math, float* wimg, cudaStream_t st) {
-  cudaError_t e = cudaMemsetAsync(stats, 0, sizeof(double) * 2 * B, st);
-  if (e != cudaSuccess) return (int)e;
-  PwArgs a;
-  memset(&a, 0, sizeof(a));
-  a.A = A; a.W = W; a.D = D; a.B = B; a.M = M; a.K = K; a.frames = frames; a.pitch = pitch;
-  a.bias = bias; a.slope = one; a.stats_out = stats;
-  return ctn_pw(a, PRO_NONE, EPI_H, math, wimg, st);
+// the head's workspace: the bottleneck's output, its weight image (tf32x3-sized: any mode fits) and statistics, the gLN partials
+struct HeadWs {
+  float *x0, *wimg;
+  double *stats, *part;
+};
+void carve_head(Carver& cv, int B, int N, int Bc, int pitch, int S, int K, HeadWs* ws) {
+  ws->x0 = cv.take<float>((size_t)B * Bc * pitch);
+  ws->wimg = cv.take<float>(ctn_pw_wimg_bytes(Bc, N, CTN_MATH_TF32X3) / sizeof(float));
+  ws->stats = cv.take<double>(2 * (size_t)B);
+  ws->part = cv.take<double>((size_t)B * ctn_sample_gln_parts((size_t)S * K * Bc) * 2);
+}
+
+// the tail's workspace; u and img_out only with bottleneck_conv1d_out
+struct TailWs {
+  float *yp, *m, *u, *g, *wcat, *bcat, *img_map, *img_gtu, *img_out;
+  double* stats;
+};
+void carve_tail(Carver& cv, int B, int N, int Bc, int S, int pitch, bool bout, TailWs* ws) {
+  const size_t R = (size_t)B * S;
+  ws->yp = cv.take<float>((size_t)B * Bc * pitch);
+  ws->m = cv.take<float>(R * N * pitch);
+  ws->u = bout ? cv.take<float>(R * N * pitch) : nullptr;
+  ws->g = cv.take<float>(R * 2 * N * pitch);
+  ws->wcat = cv.take<float>((size_t)2 * N * N);
+  ws->bcat = cv.take<float>((size_t)2 * N);
+  ws->img_map = cv.take<float>(ctn_pw_wimg_bytes(S * N, Bc, CTN_MATH_TF32X3) / sizeof(float));
+  ws->img_gtu = cv.take<float>(ctn_pw_wimg_bytes(2 * N, N, CTN_MATH_TF32X3) / sizeof(float));
+  ws->img_out = bout ? cv.take<float>(ctn_pw_wimg_bytes(N, N, CTN_MATH_TF32X3) / sizeof(float)) : nullptr;
+  ws->stats = cv.take<double>(2 * R);
+}
+
+bool math_ok(int math) {
+  return math == CTN_MATH_FP32 || math == CTN_MATH_TF32 || math == CTN_MATH_TF32X3 || math == CTN_MATH_F16X3;
 }
 
 }  // namespace
@@ -259,8 +298,10 @@ extern "C" int ctn_mha_supported(int F, int heads) { return mha_ok(F, heads) ? 1
 
 extern "C" size_t ctn_mha_workspace_bytes(int NSEQ, int T, int F) {
   if (NSEQ <= 0 || T <= 0 || F <= 0) return 0;
-  const size_t tok = (size_t)NSEQ * T;
-  return up256(tok * 3 * F * sizeof(float)) + up256(tok * F * sizeof(float)) + 256;
+  Carver cv(nullptr);
+  MhaWs ws;
+  carve_mha(cv, NSEQ, T, F, &ws);
+  return cv.off + 256;
 }
 
 extern "C" int ctn_mha_fwd(const float* z, int NSEQ, int T, int F, int heads, const float* in_w, const float* in_b, const float* out_w,
@@ -272,8 +313,10 @@ extern "C" int ctn_mha_fwd(const float* z, int NSEQ, int T, int F, int heads, co
   if (workspace_bytes < ctn_mha_workspace_bytes(NSEQ, T, F)) return CTN_EWORKSPACE;
   cudaStream_t st = (cudaStream_t)stream;
   const long long tok = (long long)NSEQ * T;
-  float* qkv = static_cast<float*>(workspace);
-  float* o = reinterpret_cast<float*>(static_cast<char*>(workspace) + up256((size_t)tok * 3 * F * sizeof(float)));
+  Carver cv(workspace);
+  MhaWs ws;
+  carve_mha(cv, NSEQ, T, F, &ws);
+  float *qkv = ws.qkv, *o = ws.o;
   const unsigned gproj = (unsigned)((tok + PROJ_ROWS - 1) / PROJ_ROWS);
   k_rowproj<<<gproj, 128, 0, st>>>(z, in_w, in_b, qkv, tok, F, 3 * F);
   CTN_COUNT_LAUNCH();
@@ -304,94 +347,106 @@ extern "C" int ctn_seq_norm_fwd(const float* Y0, const float* Y1, const float* b
   return CTN_OK;
 }
 
-// ---- separator head: bottleneck 1x1 -> pad + segment (channels-last) -> gLN over the segmented tensor ---------------------------
+// ---- separator head: [bottleneck 1x1 ->] pad + segment (channels-last) -> gLN over the segmented tensor --------------------------
 extern "C" size_t ctn_dpt_head_workspace_bytes(int B, int N, int Bc, int pitch, int S, int K) {
   if (B <= 0 || N <= 0 || Bc <= 0 || pitch <= 0 || S <= 0 || K <= 0) return 0;
-  const size_t n = (size_t)S * K * Bc;
-  return up256((size_t)B * Bc * pitch * sizeof(float)) + up256(ctn_pw_wimg_bytes(Bc, N, CTN_MATH_TF32X3)) + up256(2 * B * sizeof(double)) +
-         up256(sizeof(float)) + up256((size_t)B * ctn_sample_gln_parts(n) * 2 * sizeof(double)) + 256;
+  Carver cv(nullptr);
+  HeadWs ws;
+  carve_head(cv, B, N, Bc, pitch, S, K, &ws);
+  return cv.off + 256;
 }
 
 extern "C" int ctn_dpt_head_fwd(const float* w, const float* bn_w, const float* bn_b, const float* norm_g, const float* norm_b, float* z,
                                 int B, int N, int Bc, int frames, int pitch, int chunk_size, int hop_size, int pad_left, int pad_right,
                                 float eps, int math, void* workspace, size_t workspace_bytes, ctn_stream_t stream) {
   LaunchScope scope(w);
-  if (!w || !bn_w || !bn_b || !norm_g || !norm_b || !z || !workspace || B <= 0 || N <= 0 || Bc <= 0 || frames <= 0 || chunk_size <= 0 ||
-      hop_size <= 0 || pad_left < 0 || pad_right < 0)
+  if (!w || !norm_g || !norm_b || !z || !workspace || B <= 0 || N <= 0 || Bc <= 0 || frames <= 0 || chunk_size <= 0 || hop_size <= 0 ||
+      pad_left < 0 || pad_right < 0)
     return CTN_EINVAL;
+  if (!bn_w != !bn_b || (!bn_w && Bc != N) || !math_ok(math)) return CTN_EINVAL;
   if (pitch < frames || pitch % CTN_TILE_T != 0 || (((uintptr_t)workspace) & 255) || (((uintptr_t)w) & 15)) return CTN_EALIGN;
   const int Tp = frames + pad_left + pad_right;
   if (Tp < chunk_size) return CTN_EINVAL;
+  if (B > 65535) return CTN_EUNSUPPORTED;  // the grids of the segmentation and the gLN
   const int S = (Tp - chunk_size) / hop_size + 1;
   if (workspace_bytes < ctn_dpt_head_workspace_bytes(B, N, Bc, pitch, S, chunk_size)) return CTN_EWORKSPACE;
   cudaStream_t st = (cudaStream_t)stream;
   const size_t n = (size_t)S * chunk_size * Bc;
   const int G = ctn_sample_gln_parts(n);
   Carver cv(workspace);
-  float* x0 = cv.take<float>((size_t)B * Bc * pitch);
-  float* wimg = cv.take<float>(ctn_pw_wimg_bytes(Bc, N, CTN_MATH_TF32X3) / sizeof(float));
-  double* stats = cv.take<double>(2 * B);
-  float* one = cv.take<float>(1);
-  double* part = cv.take<double>((size_t)B * G * 2);
-  CTN_TRY(put_one(one, st));
-  CTN_TRY(pw_bias(w, bn_w, bn_b, x0, B, Bc, N, frames, pitch, one, stats, math, math != CTN_MATH_FP32 ? wimg : nullptr, st));
-  CTN_TRY(ctn_segment_fwd(x0, z, B, Bc, frames, pitch, chunk_size, hop_size, pad_left, pad_right, 1, stream));
-  CTN_TRY(ctn_sample_gln_stats(z, nullptr, n, B, part, G, st));
-  return ctn_sample_gln_apply(z, n, B, Bc, part, G, norm_g, norm_b, eps, st);
+  HeadWs ws;
+  carve_head(cv, B, N, Bc, pitch, S, chunk_size, &ws);
+  const float* x = w;
+  if (bn_w) {
+    const float* one = ctn_device_one();
+    if (!one) return CTN_ENOTBUILT;
+    cudaError_t e = cudaMemsetAsync(ws.stats, 0, sizeof(double) * 2 * B, st);
+    if (e != cudaSuccess) return (int)e;
+    const WimgJob job{bn_w, ws.wimg, Bc, N};
+    CTN_TRY(ctn_pw_prepare_batch(&job, 1, math, false, st));
+    CTN_TRY(ctn_pw_run(w, bn_w, ws.wimg, ws.x0, B, Bc, N, frames, pitch, math, bn_b, one, ws.stats, st));
+    x = ws.x0;
+  }
+  CTN_TRY(ctn_segment_fwd(x, z, B, Bc, frames, pitch, chunk_size, hop_size, pad_left, pad_right, 1, stream));
+  CTN_TRY(ctn_sample_gln_stats(z, nullptr, n, B, ws.part, G, st));
+  return ctn_sample_gln_apply(z, n, B, Bc, ws.part, G, norm_g, norm_b, eps, st);
 }
 
-// ---- separator tail + decoder: PReLU -> map -> GTU1d -> mask nonlinearity -> w * mask -> ConvTranspose1d -> crop ----------------
-extern "C" size_t ctn_dpt_tail_workspace_bytes(int B, int N, int Bc, int S, int pitch) {
+// ---- separator tail + decoder: PReLU -> map -> GTU1d [-> bottleneck_conv1d_out] -> mask nonlinearity -> w * mask -> decoder ------
+extern "C" size_t ctn_dpt_tail_workspace_bytes(int B, int N, int Bc, int S, int pitch, int bout) {
   if (B <= 0 || N <= 0 || Bc <= 0 || S <= 0 || pitch <= 0) return 0;
-  size_t wimg = ctn_pw_wimg_bytes(S * N, Bc, CTN_MATH_TF32X3), w2 = ctn_pw_wimg_bytes(2 * N, N, CTN_MATH_TF32X3);
-  if (w2 > wimg) wimg = w2;
-  return up256((size_t)B * Bc * pitch * 4) + up256((size_t)B * S * N * pitch * 4) + up256((size_t)B * S * 2 * N * pitch * 4) +
-         up256((size_t)2 * N * N * 4) + up256((size_t)2 * N * 4) + up256(wimg) + up256((size_t)2 * B * S * 8) + up256(4) + 256;
+  Carver cv(nullptr);
+  TailWs ws;
+  carve_tail(cv, B, N, Bc, S, pitch, bout != 0, &ws);
+  return cv.off + 256;
 }
 
 extern "C" int ctn_dpt_tail_fwd(const float* y, const float* w, const float* prelu, const float* map_w, const float* map_b,
-                                const float* gtu_w, const float* gtu_b, const float* gate_w, const float* gate_b, const float* dec_w,
-                                float* out, float* latent, float* what, int B, int N, int Bc, int S, int frames, int pitch, int L,
-                                int stride, int crop_left, int T, int mask_relu, int math, void* workspace, size_t workspace_bytes,
-                                ctn_stream_t stream) {
+                                const float* gtu_w, const float* gtu_b, const float* gate_w, const float* gate_b, const float* bout_w,
+                                const float* bout_b, const float* dec_w, float* out, float* latent, float* what, int B, int N, int Bc,
+                                int S, int frames, int pitch, int L, int stride, int crop_left, int T, int mask_relu, int math,
+                                void* workspace, size_t workspace_bytes, ctn_stream_t stream) {
   LaunchScope scope(y);
   if (!y || !w || !prelu || !map_w || !map_b || !gtu_w || !gtu_b || !gate_w || !gate_b || !dec_w || !out || !what || !workspace || B <= 0 ||
       N <= 0 || Bc <= 0 || S <= 0 || frames <= 0)
     return CTN_EINVAL;
+  if (!bout_w != !bout_b || !math_ok(math)) return CTN_EINVAL;
+  const bool bout = bout_w != nullptr;
   if (pitch < frames || pitch % CTN_TILE_T != 0 || (((uintptr_t)workspace) & 255)) return CTN_EALIGN;
   if ((((uintptr_t)y) | ((uintptr_t)w) | ((uintptr_t)what)) & 15) return CTN_EALIGN;
-  if (workspace_bytes < ctn_dpt_tail_workspace_bytes(B, N, Bc, S, pitch)) return CTN_EWORKSPACE;
+  if (workspace_bytes < ctn_dpt_tail_workspace_bytes(B, N, Bc, S, pitch, bout)) return CTN_EWORKSPACE;
   if ((long long)B * S > 65535) return CTN_EUNSUPPORTED;
   CTN_TRY(ctn_decoder_check(B * S, N, frames, pitch, L, stride, crop_left, T));
+  const float* one = ctn_device_one();
+  if (!one) return CTN_ENOTBUILT;
   cudaStream_t st = (cudaStream_t)stream;
-  size_t wimg_bytes = ctn_pw_wimg_bytes(S * N, Bc, CTN_MATH_TF32X3), w2 = ctn_pw_wimg_bytes(2 * N, N, CTN_MATH_TF32X3);
-  if (w2 > wimg_bytes) wimg_bytes = w2;
+  const int R = B * S;
   Carver cv(workspace);
-  float* yp = cv.take<float>((size_t)B * Bc * pitch);
-  float* m = cv.take<float>((size_t)B * S * N * pitch);
-  float* g = cv.take<float>((size_t)B * S * 2 * N * pitch);
-  float* wcat = cv.take<float>((size_t)2 * N * N);
-  float* bcat = cv.take<float>((size_t)2 * N);
-  float* wimg = cv.take<float>(wimg_bytes / sizeof(float));
-  double* stats = cv.take<double>((size_t)2 * B * S);
-  float* one = cv.take<float>(1);
-  float* wi = math != CTN_MATH_FP32 ? wimg : nullptr;
+  TailWs ws;
+  carve_tail(cv, B, N, Bc, S, pitch, bout, &ws);
+  const bool tc = math != CTN_MATH_FP32;
   cudaError_t e;
   // [map; map_gate] as one 2N x N contraction
-  if ((e = cudaMemcpyAsync(wcat, gtu_w, sizeof(float) * N * N, cudaMemcpyDeviceToDevice, st)) != cudaSuccess) return (int)e;
-  if ((e = cudaMemcpyAsync(wcat + (size_t)N * N, gate_w, sizeof(float) * N * N, cudaMemcpyDeviceToDevice, st)) != cudaSuccess) return (int)e;
-  if ((e = cudaMemcpyAsync(bcat, gtu_b, sizeof(float) * N, cudaMemcpyDeviceToDevice, st)) != cudaSuccess) return (int)e;
-  if ((e = cudaMemcpyAsync(bcat + N, gate_b, sizeof(float) * N, cudaMemcpyDeviceToDevice, st)) != cudaSuccess) return (int)e;
-  CTN_TRY(put_one(one, st));
-  CTN_TRY(ctn_prelu_apply(y, yp, prelu, B, Bc, frames, pitch, st));
-  CTN_TRY(pw_bias(yp, map_w, map_b, m, B, S * N, Bc, frames, pitch, one, stats, math, wi, st));
-  CTN_TRY(pw_bias(m, wcat, bcat, g, B * S, 2 * N, N, frames, pitch, one, stats, math, wi, st));
-  int gx = (int)(((size_t)N * pitch + 255) / 256);
-  if (gx > 256) gx = 256;
-  k_gtu_mask<<<dim3(gx, B * S), 256, 0, st>>>(g, w, what, S, N, frames, pitch, mask_relu);
-  CTN_COUNT_LAUNCH();
-  CTN_RETURN_IF_CUDA_ERR();
-  CTN_TRY(ctn_decoder_fwd(what, dec_w, out, B * S, N, frames, pitch, L, stride, crop_left, T, stream));
-  if (latent) CTN_TRY(ctn_copy_from_pitch(what, latent, B * S * N, frames, pitch, st));
+  if ((e = cudaMemcpyAsync(ws.wcat, gtu_w, sizeof(float) * N * N, cudaMemcpyDeviceToDevice, st)) != cudaSuccess) return (int)e;
+  if ((e = cudaMemcpyAsync(ws.wcat + (size_t)N * N, gate_w, sizeof(float) * N * N, cudaMemcpyDeviceToDevice, st)) != cudaSuccess) return (int)e;
+  if ((e = cudaMemcpyAsync(ws.bcat, gtu_b, sizeof(float) * N, cudaMemcpyDeviceToDevice, st)) != cudaSuccess) return (int)e;
+  if ((e = cudaMemcpyAsync(ws.bcat + N, gate_b, sizeof(float) * N, cudaMemcpyDeviceToDevice, st)) != cudaSuccess) return (int)e;
+  if ((e = cudaMemsetAsync(ws.stats, 0, sizeof(double) * 2 * R, st)) != cudaSuccess) return (int)e;
+  if (tc) {  // every weight image of the call in one batch
+    const WimgJob jobs[3] = {{map_w, ws.img_map, S * N, Bc}, {ws.wcat, ws.img_gtu, 2 * N, N}, {bout_w, ws.img_out, N, N}};
+    CTN_TRY(ctn_pw_prepare_batch(jobs, bout ? 3 : 2, math, false, st));
+  }
+  CTN_TRY(ctn_prelu_apply(y, ws.yp, prelu, B, Bc, frames, pitch, st));
+  CTN_TRY(ctn_pw_run(ws.yp, map_w, ws.img_map, ws.m, B, S * N, Bc, frames, pitch, math, map_b, one, ws.stats, st));
+  CTN_TRY(ctn_pw_run(ws.m, ws.wcat, ws.img_gtu, ws.g, R, 2 * N, N, frames, pitch, math, ws.bcat, one, ws.stats, st));
+  if (bout) {
+    CTN_TRY((launch_gtu_mask<true, false>(ws.g, nullptr, ws.u, R, S, N, frames, pitch, mask_relu, st)));
+    CTN_TRY(ctn_pw_run(ws.u, bout_w, ws.img_out, ws.m, R, N, N, frames, pitch, math, bout_b, one, ws.stats, st));
+    CTN_TRY((launch_gtu_mask<false, true>(ws.m, w, what, R, S, N, frames, pitch, mask_relu, st)));
+  } else {
+    CTN_TRY((launch_gtu_mask<true, true>(ws.g, w, what, R, S, N, frames, pitch, mask_relu, st)));
+  }
+  CTN_TRY(ctn_decoder_fwd(what, dec_w, out, R, N, frames, pitch, L, stride, crop_left, T, stream));
+  if (latent) CTN_TRY(ctn_copy_from_pitch(what, latent, R * N, frames, pitch, st));
   return CTN_OK;
 }

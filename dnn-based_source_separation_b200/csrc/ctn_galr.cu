@@ -1,8 +1,8 @@
-// GALRNet stages.  Reference: src/models/galr.py:135-197 (LowDimensionGloballyAttentiveBlock), src/models/galrnet.py:222-240
-// (Separator head).
+// GALRNet stages.  Reference: src/models/galr.py:135-197 (LowDimensionGloballyAttentiveBlock).
 //
 // The dual-path state is channels-last, X (B, S, K, F), as on the DPTNet path; the intra-chunk block is the DPRNN one unchanged
-// (ctn_bilstm_proj_fwd + ctn_dprnn_norm_res2_fwd, swap = 0).  One LowDimensionGloballyAttentiveBlock is
+// (ctn_bilstm_proj_fwd + ctn_dprnn_norm_res2_fwd, swap = 0), and the head and tail are DPTNet's (ctn_dpt_head_fwd without a
+// bottleneck, ctn_dpt_tail_fwd without bottleneck_conv1d_out).  One LowDimensionGloballyAttentiveBlock is
 //   * down-map (k_galr_down, one CTA per (b, s)): fc_map along the chunk axis, K -> Q, in fp32 FMAs; LayerNorm over the F channels
 //     of each of the Q tokens, mean then centred variance in double; plus the sinusoidal encoding of position p = s Q + q, feature
 //     f < F/2: sin(p / d[f]), else cos(p / d[f - F/2]) (concatenated, not interleaved).  The divisors d = 10000^(j / F) come from
@@ -25,8 +25,6 @@ constexpr int GMAX_F = 128;
 constexpr int GROWS = GT / 32 * GR;  // most output rows per pass (F = 32)
 
 bool galr_ok(int F, int K, int Q) { return (F == 32 || F == 64 || F == 128) && K >= 1 && Q >= 1 && Q <= K; }
-
-size_t up256(size_t b) { return (b + 255) & ~(size_t)255; }
 
 // x (B, S, K, F) -> zt (B, Q, S, F) = LN_F(fc_map(x) along K) + pe.  grid (S, B), block 256.  Thread (grp, f): grp = tid / F,
 // rows grp + r (256 / F) of each pass of (256 / F) * 8 tokens; the K reduction runs over tiles of 32 rows of x and of fc_map in
@@ -149,6 +147,19 @@ __global__ void __launch_bounds__(GT) k_galr_up(const float* __restrict__ Y, con
   }
 }
 
+struct GalrWs {
+  float *zt, *y;
+  void* mha;
+  double* part;
+};
+void carve_galr(Carver& cv, int B, int S, int Q, int F, GalrWs* ws) {
+  const size_t n = (size_t)Q * S * F;
+  ws->zt = cv.take<float>((size_t)B * n);
+  ws->y = cv.take<float>((size_t)B * n);
+  ws->mha = cv.take<char>(ctn_mha_workspace_bytes(B * Q, S, F));
+  ws->part = cv.take<double>((size_t)B * ctn_sample_gln_parts(n) * 2);
+}
+
 }  // namespace
 
 // ---- one LowDimensionGloballyAttentiveBlock -----------------------------------------------------------------------------------
@@ -156,9 +167,10 @@ extern "C" int ctn_galr_supported(int F, int K, int Q, int heads) { return galr_
 
 extern "C" size_t ctn_galr_inter_workspace_bytes(int B, int S, int K, int Q, int F) {
   if (B <= 0 || S <= 0 || K <= 0 || Q <= 0 || F <= 0) return 0;
-  const size_t n = (size_t)Q * S * F;
-  return 2 * up256((size_t)B * n * sizeof(float)) + up256(ctn_mha_workspace_bytes(B * Q, S, F)) +
-         up256((size_t)B * ctn_sample_gln_parts(n) * 2 * sizeof(double)) + 256;
+  Carver cv(nullptr);
+  GalrWs ws;
+  carve_galr(cv, B, S, Q, F, &ws);
+  return cv.off + 256;
 }
 
 extern "C" int ctn_galr_inter_fwd(const float* x, const float* map_w, const float* map_b, const float* ln_g, const float* ln_b,
@@ -179,46 +191,17 @@ extern "C" int ctn_galr_inter_fwd(const float* x, const float* map_w, const floa
   const size_t n = (size_t)Q * S * F;
   const int G = ctn_sample_gln_parts(n);
   Carver cv(workspace);
-  float* zt = cv.take<float>((size_t)B * n);
-  float* y = cv.take<float>((size_t)B * n);
-  const size_t mha_bytes = ctn_mha_workspace_bytes(B * Q, S, F);
-  void* mha_ws = cv.take<char>(mha_bytes);
-  double* part = cv.take<double>((size_t)B * G * 2);
+  GalrWs ws;
+  carve_galr(cv, B, S, Q, F, &ws);
+  float *zt = ws.zt, *y = ws.y;
+  double* part = ws.part;
   k_galr_down<<<dim3(S, B), GT, 0, st>>>(x, map_w, map_b, ln_g, ln_b, pe_div, zt, S, K, Q, F, ln_eps);
   CTN_COUNT_LAUNCH();
   CTN_RETURN_IF_CUDA_ERR();
-  CTN_TRY(ctn_mha_fwd(zt, B * Q, S, F, heads, in_w, in_b, out_w, out_b, y, mha_ws, mha_bytes, stream));
+  CTN_TRY(ctn_mha_fwd(zt, B * Q, S, F, heads, in_w, in_b, out_w, out_b, y, ws.mha, ctn_mha_workspace_bytes(B * Q, S, F), stream));
   CTN_TRY(ctn_sample_gln_stats(y, zt, n, B, part, G, st));
   k_galr_up<<<dim3(S, B), GT, 0, st>>>(y, zt, part, G, gn_g, gn_b, inv_w, inv_b, x, out, S, K, Q, F, gn_eps);
   CTN_COUNT_LAUNCH();
   CTN_RETURN_IF_CUDA_ERR();
   return CTN_OK;
-}
-
-// ---- separator head: pad + Segment1d (channels-last) + gLN over the segmented tensor, no bottleneck -----------------------------
-extern "C" size_t ctn_galr_head_workspace_bytes(int B, int S, int K, int F) {
-  if (B <= 0 || S <= 0 || K <= 0 || F <= 0) return 0;
-  return up256((size_t)B * ctn_sample_gln_parts((size_t)S * K * F) * 2 * sizeof(double)) + 256;
-}
-
-extern "C" int ctn_galr_head_fwd(const float* w, const float* norm_g, const float* norm_b, float* z, int B, int F, int frames, int pitch,
-                                 int chunk_size, int hop_size, int pad_left, int pad_right, float eps, void* workspace,
-                                 size_t workspace_bytes, ctn_stream_t stream) {
-  LaunchScope scope(w);
-  if (!w || !norm_g || !norm_b || !z || !workspace || B <= 0 || F <= 0 || frames <= 0 || pitch < frames || chunk_size <= 0 ||
-      hop_size <= 0 || pad_left < 0 || pad_right < 0)
-    return CTN_EINVAL;
-  const int Tp = frames + pad_left + pad_right;
-  if (Tp < chunk_size) return CTN_EINVAL;
-  if (B > 65535) return CTN_EUNSUPPORTED;
-  if (((uintptr_t)workspace) & 255) return CTN_EALIGN;
-  const int S = (Tp - chunk_size) / hop_size + 1;
-  if (workspace_bytes < ctn_galr_head_workspace_bytes(B, S, chunk_size, F)) return CTN_EWORKSPACE;
-  cudaStream_t st = (cudaStream_t)stream;
-  const size_t n = (size_t)S * chunk_size * F;
-  const int G = ctn_sample_gln_parts(n);
-  double* part = Carver(workspace).take<double>((size_t)B * G * 2);
-  CTN_TRY(ctn_segment_fwd(w, z, B, F, frames, pitch, chunk_size, hop_size, pad_left, pad_right, 1, stream));
-  CTN_TRY(ctn_sample_gln_stats(z, nullptr, n, B, part, G, st));
-  return ctn_sample_gln_apply(z, n, B, F, part, G, norm_g, norm_b, eps, st);
 }

@@ -13,14 +13,17 @@ struct FoldedConv {
               // of the gLN group) >= max |normalised value|  (activation envelope of the fp16-piece mode)
 };
 
-// Workspace carving: 256-byte aligned sub-buffers of one allocation.  base == nullptr only measures (off = bytes needed).
+inline size_t up256(size_t b) { return (b + 255) & ~(size_t)255; }
+
+// Workspace carving: 256-byte aligned sub-buffers of one allocation.  base == nullptr only measures (off = bytes needed), so an
+// entry's workspace query is its carve run on Carver(nullptr) and cannot drift from the carve itself.
 struct Carver {
   char* base;
   size_t off;
   explicit Carver(void* b) : base((char*)b), off(0) {}
   template <typename T>
   T* take(size_t count) {
-    off = (off + 255) & ~(size_t)255;
+    off = up256(off);
     T* p = base ? (T*)(base + off) : nullptr;
     off += count * sizeof(T);
     return p;
@@ -127,6 +130,14 @@ int ctn_pw(const PwArgs& a, int pro, int epi, int math, float* wimg_scratch, cud
 size_t ctn_pw_wimg_bytes(int M, int K, int math);
 // weight image of a.W (a.M, a.K) for ctn_pw(a, .., math, nullptr, ..); nothing to do in the fp32 mode
 int ctn_pw_prepare(const PwArgs& a, int math, float* wimg, cudaStream_t st);
+// device scalar 1.0 of the current device (one __device__ constant, ctn_wgmma.cu): the PReLU slope that turns the PReLU of the
+// EPI_H epilogue or the PRO_PRELU prologue into an identity.  nullptr when the symbol cannot be resolved.
+const float* ctn_device_one();
+// One 1x1 contraction of a pitched (B, K, pitch) operand from a prebuilt weight image (wimg; none in the fp32 mode): EPI_RAW
+// without bias; with bias, EPI_H with the PReLU slope (ctn_device_one(): a plain bias add) and its statistics in stats (double[2 B],
+// accumulated, never read back by the callers).
+int ctn_pw_run(const float* A, const float* W, const float* wimg, float* D, int B, int M, int K, int frames, int pitch, int math,
+               const float* bias, const float* slope, double* stats, cudaStream_t st);
 // EPI_MASKDEC (PRO_PRELU) applies to this contraction: fp16-piece mode, n_basis a multiple of 128, K <= 128 (the operand stays
 // resident in shared memory), decoder kernel 16 / stride 8 (caller)
 int ctn_pw_maskdec_supported(const PwArgs& a, int math);

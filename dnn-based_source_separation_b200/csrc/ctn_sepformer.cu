@@ -14,9 +14,9 @@
 //     centred variance in double (two passes), so a token whose features are all equal comes out exactly beta.
 //   * the end of each Intra/InterTransformer: GroupNorm(1, F) per SEQUENCE (F x len values, summed in double in a fixed order,
 //     no atomics) plus the outer residual, the block input without the positional encoding (sepformer.py:468, 476).
-//   * the tail: PReLU -> map -> GTU1d -> bottleneck_conv1d_out -> ReLU / sigmoid -> w * mask -> decoder.
+//   * segmentation, overlap-add (ctn_segment_fwd / ctn_overlap_add_fwd with z_pitch) and the tail (ctn_dpt_tail_fwd with
+//     bottleneck_conv1d_out) are the shared entries.
 #include <math.h>
-#include <string.h>
 
 #include "ctn_internal.h"
 
@@ -188,78 +188,6 @@ __global__ void __launch_bounds__(128) k_sfm_pos_enc(const float* __restrict__ X
   out[i] = x + (x + __ldg(pe + (size_t)pos * F + f));
 }
 
-// segmentation into the pitched channel-first layout: Z[b][f][s C + k] = xpad[b][f][s P + k] (xpad = x zero-padded by pad_left on
-// the left), columns [S C, z_pitch) = 0.  grid (ceil(z_pitch / 256), F, B)
-__global__ void __launch_bounds__(256) k_sfm_segment(const float* __restrict__ x, float* __restrict__ Z, int F, int frames, int pitch,
-                                                     int pad_left, int S, int C, int P, int z_pitch) {
-  const int f = blockIdx.y, b = blockIdx.z, i = blockIdx.x * 256 + threadIdx.x;
-  if (i >= z_pitch) return;
-  float v = 0.f;
-  if (i < S * C) {
-    const int s = i / C, k = i % C, tt = s * P + k - pad_left;
-    if (tt >= 0 && tt < frames) v = __ldg(x + ((size_t)b * F + f) * pitch + tt);
-  }
-  Z[((size_t)b * F + f) * z_pitch + i] = v;
-}
-
-// overlap-add + crop from the pitched layout: y[b][f][t] = sum over the chunks s covering padded frame tp = t + crop_left, s
-// ascending, of Z[b][f][s C + tp - s P]; columns [T_out, out_pitch) = 0.  grid (ceil(out_pitch / 256), F, B)
-__global__ void __launch_bounds__(256) k_sfm_overlap_add(const float* __restrict__ Z, float* __restrict__ y, int F, int S, int C, int P,
-                                                         int z_pitch, int crop_left, int T_out, int out_pitch) {
-  const int f = blockIdx.y, b = blockIdx.z, t = blockIdx.x * 256 + threadIdx.x;
-  if (t >= out_pitch) return;
-  float acc = 0.f;
-  if (t < T_out) {
-    const int tp = t + crop_left;
-    int s_lo = (tp - C + 1 <= 0) ? 0 : (tp - C + P) / P;
-    int s_hi = tp / P;
-    if (s_hi > S - 1) s_hi = S - 1;
-    const float* z = Z + ((size_t)b * F + f) * z_pitch;
-    for (int s = s_lo; s <= s_hi; ++s) acc += __ldg(z + (size_t)s * C + tp - s * P);
-  }
-  y[((size_t)b * F + f) * out_pitch + t] = acc;
-}
-
-// PReLU on the (B, C, pitch) layout (columns [frames, pitch) = 0); thread 0 of CTA 0 also stores the device scalar 1.0 the
-// bias-only contractions of the tail take as their PReLU slope
-__global__ void __launch_bounds__(256) k_sfm_prelu(const float* __restrict__ x, float* __restrict__ y, const float* __restrict__ slope,
-                                                   size_t n, int frames, int pitch, float* one) {
-  if (blockIdx.x == 0 && threadIdx.x == 0) *one = 1.f;
-  const float a = __ldg(slope);
-  for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (size_t)gridDim.x * blockDim.x)
-    y[i] = (int)(i % pitch) < frames ? prelu_f(x[i], a) : 0.f;
-}
-
-// GTU1d: g (R, 2N, pitch) = [map; map_gate] m + bias -> u (R, N, pitch) = tanh(g[n]) sigmoid(g[N + n]); columns [frames, pitch) = 0
-__global__ void __launch_bounds__(256) k_sfm_gtu(const float* __restrict__ g, float* __restrict__ u, int N, int frames, int pitch) {
-  const int r = blockIdx.y;
-  for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < (size_t)N * pitch; i += (size_t)gridDim.x * blockDim.x) {
-    const int n = (int)(i / pitch), t = (int)(i % pitch);
-    float v = 0.f;
-    if (t < frames) {
-      const float a = g[((size_t)r * 2 * N + n) * pitch + t], gt = g[((size_t)r * 2 * N + N + n) * pitch + t];
-      v = tanhf(a) * (1.f / (1.f + expf(-gt)));
-    }
-    u[(size_t)r * N * pitch + i] = v;
-  }
-}
-
-// what[b s][n][t] = act(v[b s][n][t]) w[b][n][t], act = ReLU (mask_relu) or sigmoid; columns [frames, pitch) = 0
-__global__ void __launch_bounds__(256) k_sfm_mask(const float* __restrict__ v, const float* __restrict__ w, float* __restrict__ what, int S,
-                                                  int N, int frames, int pitch, int mask_relu) {
-  const int bs = blockIdx.y, b = bs / S;
-  for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < (size_t)N * pitch; i += (size_t)gridDim.x * blockDim.x) {
-    const int n = (int)(i / pitch), t = (int)(i % pitch);
-    float o = 0.f;
-    if (t < frames) {
-      const float x = v[(size_t)bs * N * pitch + i];
-      const float mk = mask_relu ? fmaxf(x, 0.f) : 1.f / (1.f + expf(-x));
-      o = mk * w[((size_t)b * N + n) * pitch + t];
-    }
-    what[(size_t)bs * N * pitch + i] = o;
-  }
-}
-
 bool attn_ok(int F, int heads) {
   if (F <= 0 || heads <= 0 || F % heads) return false;
   const int D = F / heads;
@@ -311,24 +239,29 @@ int launch_seq_norm(const float* X, const float* R, const float* gamma, const fl
   return CTN_OK;
 }
 
-// one 1x1 contraction of the pitched state through ctn_pw from a prebuilt weight image (none in the fp32 mode): EPI_RAW, or
-// EPI_H with the PReLU slope and the statistics scratch the caller passes (ReLU: a device slope of 0)
-int pw_run(const float* A, const float* W, const float* wimg, float* D, int B, int M, int K, int frames, int pitch, int math,
-           const float* bias, const float* slope, double* stats, cudaStream_t st) {
-  PwArgs a;
-  memset(&a, 0, sizeof(a));
-  a.A = A; a.W = W; a.D = D; a.B = B; a.M = M; a.K = K; a.frames = frames; a.pitch = pitch;
-  a.wimg = wimg;
-  if (bias) { a.bias = bias; a.slope = slope; a.stats_out = stats; }
-  return ctn_pw(a, PRO_NONE, bias ? EPI_H : EPI_RAW, math, nullptr, st);
-}
-
-size_t up256(size_t b) { return (b + 255) & ~(size_t)255; }
-
 size_t tf_img_bytes(int F, int d_ff, int math, int k) {  // image of contraction k of a layer: QKV, out_proj, linear1, linear2
   if (math == CTN_MATH_FP32) return 0;
   const int shapes[4][2] = {{3 * F, F}, {F, F}, {d_ff, F}, {F, d_ff}};
   return up256(ctn_pw_wimg_bytes(shapes[k][0], shapes[k][1], math));
+}
+
+// the workspace of ctn_sfm_transformer_fwd; every layer's four images lie back to back in imgs, per_layer bytes apart
+struct TfWs {
+  float *x, *o, *g, *imgs;
+  double* stats;
+  float* zero;
+  size_t per_layer;
+};
+void carve_tf(Carver& cv, int B, int F, int d_ff, int layers, int pitch, int math, TfWs* ws) {
+  const size_t big = (size_t)(3 * F > d_ff ? 3 * F : d_ff);
+  ws->x = cv.take<float>((size_t)B * F * pitch);    // the residual stream of the layers
+  ws->o = cv.take<float>((size_t)B * F * pitch);    // attention output, then linear2's output
+  ws->g = cv.take<float>((size_t)B * big * pitch);  // QKV, then out_proj's output, then linear1's
+  ws->per_layer = 0;
+  for (int k = 0; k < 4; ++k) ws->per_layer += tf_img_bytes(F, d_ff, math, k);
+  ws->imgs = ws->per_layer ? cv.take<float>(ws->per_layer * layers / sizeof(float)) : nullptr;
+  ws->stats = cv.take<double>((size_t)2 * B);
+  ws->zero = cv.take<float>(1);
 }
 
 }  // namespace
@@ -380,46 +313,13 @@ extern "C" int ctn_sfm_pos_enc_fwd(const float* X, const float* pe, float* out, 
   return CTN_OK;
 }
 
-// ---- segmentation / overlap-add on the pitched channel-first layout -------------------------------------------------------------
-extern "C" int ctn_sfm_segment_fwd(const float* x, float* Z, int B, int F, int frames, int pitch, int chunk_size, int hop_size, int pad_left,
-                                   int pad_right, int z_pitch, ctn_stream_t stream) {
-  LaunchScope scope(x);
-  if (!x || !Z || B <= 0 || F <= 0 || frames <= 0 || pitch < frames || chunk_size <= 0 || hop_size <= 0 || pad_left < 0 || pad_right < 0)
-    return CTN_EINVAL;
-  const int Tp = frames + pad_left + pad_right;
-  if (Tp < chunk_size) return CTN_EINVAL;
-  const int S = (Tp - chunk_size) / hop_size + 1;
-  if ((long long)S * chunk_size > z_pitch) return CTN_EINVAL;
-  if (B > 65535 || F > 65535) return CTN_EUNSUPPORTED;
-  k_sfm_segment<<<dim3((z_pitch + 255) / 256, F, B), 256, 0, (cudaStream_t)stream>>>(x, Z, F, frames, pitch, pad_left, S, chunk_size, hop_size,
-                                                                                  z_pitch);
-  CTN_COUNT_LAUNCH();
-  CTN_RETURN_IF_CUDA_ERR();
-  return CTN_OK;
-}
-
-extern "C" int ctn_sfm_overlap_add_fwd(const float* Z, float* y, int B, int F, int S, int chunk_size, int hop_size, int z_pitch,
-                                       int crop_left, int T_out, int out_pitch, ctn_stream_t stream) {
-  LaunchScope scope(Z);
-  if (!Z || !y || B <= 0 || F <= 0 || S <= 0 || chunk_size <= 0 || hop_size <= 0 || crop_left < 0 || T_out <= 0 || out_pitch < T_out)
-    return CTN_EINVAL;
-  if ((long long)S * chunk_size > z_pitch || crop_left + T_out > (S - 1) * hop_size + chunk_size) return CTN_EINVAL;
-  if (B > 65535 || F > 65535) return CTN_EUNSUPPORTED;
-  k_sfm_overlap_add<<<dim3((out_pitch + 255) / 256, F, B), 256, 0, (cudaStream_t)stream>>>(Z, y, F, S, chunk_size, hop_size, z_pitch,
-                                                                                        crop_left, T_out, out_pitch);
-  CTN_COUNT_LAUNCH();
-  CTN_RETURN_IF_CUDA_ERR();
-  return CTN_OK;
-}
-
 // ---- one IntraTransformer / InterTransformer ---------------------------------------------------------------------------------------
 extern "C" size_t ctn_sfm_transformer_workspace_bytes(int B, int F, int d_ff, int layers, int pitch, int math) {
   if (B <= 0 || F <= 0 || d_ff <= 0 || layers <= 0 || pitch <= 0) return 0;
-  const size_t big = (size_t)(3 * F > d_ff ? 3 * F : d_ff);
-  size_t img = 0;
-  for (int k = 0; k < 4; ++k) img += tf_img_bytes(F, d_ff, math, k);
-  return up256((size_t)B * F * pitch * 4) * 2 + up256((size_t)B * big * pitch * 4) + img * layers + up256((size_t)2 * B * 8) + up256(4) +
-         256;
+  Carver cv(nullptr);
+  TfWs ws;
+  carve_tf(cv, B, F, d_ff, layers, pitch, math, &ws);
+  return cv.off + 256;
 }
 
 extern "C" int ctn_sfm_transformer_fwd(const float* X, float* out, const float* const* w, int B, int F, int heads, int d_ff, int layers,
@@ -440,20 +340,14 @@ extern "C" int ctn_sfm_transformer_fwd(const float* X, float* out, const float* 
   if (workspace_bytes < ctn_sfm_transformer_workspace_bytes(B, F, d_ff, layers, pitch, math)) return CTN_EWORKSPACE;
   cudaStream_t st = (cudaStream_t)stream;
   const int ntok = S * C;
-  const size_t big = (size_t)(3 * F > d_ff ? 3 * F : d_ff);
   Carver cv(workspace);
-  float* x = cv.take<float>((size_t)B * F * pitch);   // the residual stream of the layers
-  float* o = cv.take<float>((size_t)B * F * pitch);   // attention output, then linear2's output
-  float* g = cv.take<float>((size_t)B * big * pitch); // QKV, then out_proj's output, then linear1's
-  float* imgs = nullptr;
-  size_t per_layer = 0;
-  for (int k = 0; k < 4; ++k) per_layer += tf_img_bytes(F, d_ff, math, k);
-  if (per_layer) imgs = cv.take<float>(per_layer * layers / sizeof(float));
-  double* stats = cv.take<double>((size_t)2 * B);
-  float* zero = cv.take<float>(1);
+  TfWs ws;
+  carve_tf(cv, B, F, d_ff, layers, pitch, math, &ws);
+  float *x = ws.x, *o = ws.o, *g = ws.g, *imgs = ws.imgs, *zero = ws.zero;
+  double* stats = ws.stats;
   auto img = [&](int l, int k) -> float* {
     if (!imgs) return nullptr;
-    size_t off = per_layer * l;
+    size_t off = ws.per_layer * l;
     for (int i = 0; i < k; ++i) off += tf_img_bytes(F, d_ff, math, i);
     return reinterpret_cast<float*>(reinterpret_cast<char*>(imgs) + off);
   };
@@ -482,86 +376,14 @@ extern "C" int ctn_sfm_transformer_fwd(const float* X, float* out, const float* 
   for (int l = 0; l < layers; ++l) {
     const float* const* p = w + SFM_LAYER_PTRS * l;
     // x = norm1(x + out_proj(attention(in_proj(x))))
-    CTN_TRY(pw_run(x, p[0], img(l, 0), g, B, 3 * F, F, ntok, pitch, math, nullptr, nullptr, nullptr, st));
+    CTN_TRY(ctn_pw_run(x, p[0], img(l, 0), g, B, 3 * F, F, ntok, pitch, math, nullptr, nullptr, nullptr, st));
     CTN_TRY(launch_attn(g, p[1], o, B, F, heads, pitch, q, st));
-    CTN_TRY(pw_run(o, p[2], img(l, 1), g, B, F, F, ntok, pitch, math, nullptr, nullptr, nullptr, st));
+    CTN_TRY(ctn_pw_run(o, p[2], img(l, 1), g, B, F, F, ntok, pitch, math, nullptr, nullptr, nullptr, st));
     CTN_TRY(launch_token_ln(x, g, p[3], p[8], p[9], x, B, F, ntok, pitch, eps, st));
     // x = norm2(x + linear2(relu(linear1(x))))
-    CTN_TRY(pw_run(x, p[4], img(l, 2), g, B, d_ff, F, ntok, pitch, math, p[5], zero, stats, st));
-    CTN_TRY(pw_run(g, p[6], img(l, 3), o, B, F, d_ff, ntok, pitch, math, nullptr, nullptr, nullptr, st));
+    CTN_TRY(ctn_pw_run(x, p[4], img(l, 2), g, B, d_ff, F, ntok, pitch, math, p[5], zero, stats, st));
+    CTN_TRY(ctn_pw_run(g, p[6], img(l, 3), o, B, F, d_ff, ntok, pitch, math, nullptr, nullptr, nullptr, st));
     CTN_TRY(launch_token_ln(x, o, p[7], p[10], p[11], x, B, F, ntok, pitch, eps, st));
   }
   return launch_seq_norm(x, X, fin[1], fin[2], out, B, F, pitch, ntok, q, eps, st);
-}
-
-// ---- separator tail + decoder ----------------------------------------------------------------------------------------------------
-extern "C" size_t ctn_sfm_tail_workspace_bytes(int B, int N, int Bc, int S, int pitch) {
-  if (B <= 0 || N <= 0 || Bc <= 0 || S <= 0 || pitch <= 0) return 0;
-  const size_t R = (size_t)B * S;
-  return up256((size_t)B * Bc * pitch * 4) + up256(R * N * pitch * 4) * 2 + up256(R * 2 * N * pitch * 4) + up256((size_t)2 * N * N * 4) +
-         up256((size_t)2 * N * 4) + up256(ctn_pw_wimg_bytes(S * N, Bc, CTN_MATH_TF32X3)) + up256(ctn_pw_wimg_bytes(2 * N, N, CTN_MATH_TF32X3)) +
-         up256(ctn_pw_wimg_bytes(N, N, CTN_MATH_TF32X3)) + up256(2 * R * 8) + up256(4) + 256;
-}
-
-extern "C" int ctn_sfm_tail_fwd(const float* y, const float* w, const float* prelu, const float* map_w, const float* map_b,
-                                const float* gtu_w, const float* gtu_b, const float* gate_w, const float* gate_b, const float* bout_w,
-                                const float* bout_b, const float* dec_w, float* out, float* latent, float* what, int B, int N, int Bc,
-                                int S, int frames, int pitch, int L, int stride, int crop_left, int T, int mask_relu, int math,
-                                void* workspace, size_t workspace_bytes, ctn_stream_t stream) {
-  LaunchScope scope(y);
-  if (!y || !w || !prelu || !map_w || !map_b || !gtu_w || !gtu_b || !gate_w || !gate_b || !bout_w || !bout_b || !dec_w || !out || !what ||
-      !workspace || B <= 0 || N <= 0 || Bc <= 0 || S <= 0 || frames <= 0)
-    return CTN_EINVAL;
-  if (math != CTN_MATH_FP32 && math != CTN_MATH_TF32 && math != CTN_MATH_TF32X3 && math != CTN_MATH_F16X3) return CTN_EINVAL;
-  if (pitch < frames || pitch % CTN_TILE_T != 0 || (((uintptr_t)workspace) & 255)) return CTN_EALIGN;
-  if ((((uintptr_t)y) | ((uintptr_t)w) | ((uintptr_t)what)) & 15) return CTN_EALIGN;
-  if (workspace_bytes < ctn_sfm_tail_workspace_bytes(B, N, Bc, S, pitch)) return CTN_EWORKSPACE;
-  if ((long long)B * S > 65535) return CTN_EUNSUPPORTED;
-  CTN_TRY(ctn_decoder_check(B * S, N, frames, pitch, L, stride, crop_left, T));
-  cudaStream_t st = (cudaStream_t)stream;
-  const int R = B * S;
-  Carver cv(workspace);
-  float* yp = cv.take<float>((size_t)B * Bc * pitch);
-  float* m = cv.take<float>((size_t)R * N * pitch);
-  float* u = cv.take<float>((size_t)R * N * pitch);
-  float* g = cv.take<float>((size_t)R * 2 * N * pitch);
-  float* wcat = cv.take<float>((size_t)2 * N * N);
-  float* bcat = cv.take<float>((size_t)2 * N);
-  float* img_map = cv.take<float>(ctn_pw_wimg_bytes(S * N, Bc, CTN_MATH_TF32X3) / 4);
-  float* img_gtu = cv.take<float>(ctn_pw_wimg_bytes(2 * N, N, CTN_MATH_TF32X3) / 4);
-  float* img_out = cv.take<float>(ctn_pw_wimg_bytes(N, N, CTN_MATH_TF32X3) / 4);
-  double* stats = cv.take<double>((size_t)2 * R);
-  float* one = cv.take<float>(1);
-  const bool tc = math != CTN_MATH_FP32;
-  cudaError_t e;
-  // [map; map_gate] as one 2N x N contraction
-  if ((e = cudaMemcpyAsync(wcat, gtu_w, sizeof(float) * N * N, cudaMemcpyDeviceToDevice, st)) != cudaSuccess) return (int)e;
-  if ((e = cudaMemcpyAsync(wcat + (size_t)N * N, gate_w, sizeof(float) * N * N, cudaMemcpyDeviceToDevice, st)) != cudaSuccess) return (int)e;
-  if ((e = cudaMemcpyAsync(bcat, gtu_b, sizeof(float) * N, cudaMemcpyDeviceToDevice, st)) != cudaSuccess) return (int)e;
-  if ((e = cudaMemcpyAsync(bcat + N, gate_b, sizeof(float) * N, cudaMemcpyDeviceToDevice, st)) != cudaSuccess) return (int)e;
-  if ((e = cudaMemsetAsync(stats, 0, sizeof(double) * 2 * R, st)) != cudaSuccess) return (int)e;
-  if (tc) {
-    const WimgJob jobs[3] = {{map_w, img_map, S * N, Bc}, {wcat, img_gtu, 2 * N, N}, {bout_w, img_out, N, N}};
-    CTN_TRY(ctn_pw_prepare_batch(jobs, 3, math, false, st));
-  }
-  const size_t n = (size_t)B * Bc * pitch;
-  int gp = (int)((n + 255) / 256);
-  if (gp > 1024) gp = 1024;
-  k_sfm_prelu<<<gp, 256, 0, st>>>(y, yp, prelu, n, frames, pitch, one);
-  CTN_COUNT_LAUNCH();
-  CTN_RETURN_IF_CUDA_ERR();
-  CTN_TRY(pw_run(yp, map_w, tc ? img_map : nullptr, m, B, S * N, Bc, frames, pitch, math, map_b, one, stats, st));
-  CTN_TRY(pw_run(m, wcat, tc ? img_gtu : nullptr, g, R, 2 * N, N, frames, pitch, math, bcat, one, stats, st));
-  int gx = (int)(((size_t)N * pitch + 255) / 256);
-  if (gx > 256) gx = 256;
-  k_sfm_gtu<<<dim3(gx, R), 256, 0, st>>>(g, u, N, frames, pitch);
-  CTN_COUNT_LAUNCH();
-  CTN_RETURN_IF_CUDA_ERR();
-  CTN_TRY(pw_run(u, bout_w, tc ? img_out : nullptr, m, R, N, N, frames, pitch, math, bout_b, one, stats, st));
-  k_sfm_mask<<<dim3(gx, R), 256, 0, st>>>(m, w, what, S, N, frames, pitch, mask_relu);
-  CTN_COUNT_LAUNCH();
-  CTN_RETURN_IF_CUDA_ERR();
-  CTN_TRY(ctn_decoder_fwd(what, dec_w, out, R, N, frames, pitch, L, stride, crop_left, T, stream));
-  if (latent) CTN_TRY(ctn_copy_from_pitch(what, latent, R * N, frames, pitch, st));
-  return CTN_OK;
 }

@@ -31,8 +31,6 @@ constexpr int TAS_PF = 16;       // steps of input projection prefetched per til
 constexpr int TAS_GMAX = 16;     // most sequences one pass of the recurrence carries
 constexpr int TAS_RB = 4, TAS_SB = 4;  // gate rows x sequences per warp register tile
 
-__device__ const float k_tas_one = 1.f;  // the PReLU slope that makes the pro/epilogue PReLU of ctn_pw an identity
-
 // ---- encoder ------------------------------------------------------------------------------------------------------------------
 // nrm[b] = ||x_b||_2 over the T samples (zero padding adds nothing), summed in double, fixed reduction tree.  grid B, block 256.
 __global__ void __launch_bounds__(256) k_tas_sig_norm(const float* __restrict__ x, double* __restrict__ nrm, int T) {
@@ -355,16 +353,8 @@ bool lstm_geo_here(int H, int dirs, LstmGeo* g) {
   return lstm_geo(H, dirs, nsm, smem, g);
 }
 
-size_t up256(size_t b) { return (b + 255) & ~(size_t)255; }
-
 bool math_ok(int math) {
   return math == CTN_MATH_FP32 || math == CTN_MATH_TF32 || math == CTN_MATH_TF32X3 || math == CTN_MATH_F16X3;
-}
-
-const float* one_ptr() {
-  void* p = nullptr;
-  if (cudaGetSymbolAddress(&p, k_tas_one) != cudaSuccess) return nullptr;
-  return (const float*)p;
 }
 
 size_t enc_smem_bytes(int N, int L, int stride) {
@@ -495,7 +485,7 @@ extern "C" int ctn_tas_lstm_fwd(const float* x, const float* const* w, float* ou
   if (!lstm_geo_here(H, dirs, &geo)) return CTN_EUNSUPPORTED;
   const long long ngroups = (B + geo.gmax - 1) / geo.gmax;
   if (ngroups * frames * geo.cpd >= 0x7fffffffLL) return CTN_EUNSUPPORTED;  // the barrier counters are 32-bit
-  const float* one = one_ptr();
+  const float* one = ctn_device_one();
   if (!one) return CTN_ENOTBUILT;
   int occ = 0, nsm = 0, smem_optin = 0;
   device_limits(&nsm, &smem_optin);
@@ -585,7 +575,7 @@ extern "C" int ctn_tas_tail_fwd(const float* skip, const float* w, const float* 
   if (workspace_bytes < ctn_tas_tail_workspace_bytes(N, Hd, S, math)) return CTN_EWORKSPACE;
   if ((long long)B * S > 65535) return CTN_EUNSUPPORTED;
   CTN_TRY(ctn_decoder_check(B * S, N, frames, pitch, L, stride, crop_left, T));
-  const float* one = one_ptr();
+  const float* one = ctn_device_one();
   if (!one) return CTN_ENOTBUILT;
   cudaStream_t st = (cudaStream_t)stream;
   PwArgs m;
@@ -779,7 +769,7 @@ extern "C" int ctn_tas_online_push(const ctn_tas_config_t* cfg, const ctn_tas_pa
   LaunchScope scope(state);
   LstmGeo geo;
   CTN_TRY(tas_online_device_check(cfg, B, max_chunk_frames, &geo));
-  const float* one = one_ptr();
+  const float* one = ctn_device_one();
   if (!one) return CTN_ENOTBUILT;
   cudaStream_t st = (cudaStream_t)stream;
   const int F = n / S, pitch = ctn_pitch(F);  // the chunk's layout: every scratch tensor is rewritten by each push

@@ -1060,6 +1060,26 @@ int ctn_pw_prepare_batch(const WimgJob* jobs, int n, int math, bool bounded, cud
   return CTN_OK;
 }
 
+namespace {
+__device__ const float k_one = 1.f;
+}  // namespace
+
+const float* ctn_device_one() {
+  void* p = nullptr;
+  if (cudaGetSymbolAddress(&p, k_one) != cudaSuccess) return nullptr;
+  return (const float*)p;
+}
+
+int ctn_pw_run(const float* A, const float* W, const float* wimg, float* D, int B, int M, int K, int frames, int pitch, int math,
+               const float* bias, const float* slope, double* stats, cudaStream_t st) {
+  PwArgs a;
+  memset(&a, 0, sizeof(a));
+  a.A = A; a.W = W; a.D = D; a.B = B; a.M = M; a.K = K; a.frames = frames; a.pitch = pitch;
+  a.wimg = wimg;
+  if (bias) { a.bias = bias; a.slope = slope; a.stats_out = stats; }
+  return ctn_pw(a, PRO_NONE, bias ? EPI_H : EPI_RAW, math, nullptr, st);
+}
+
 int ctn_pw_maskdec_supported(const PwArgs& a, int math) { return maskdec_ok(a, piece_math(math, a.act_scale != nullptr)); }
 
 int ctn_pw(const PwArgs& a, int pro, int epi, int math, float* wimg_scratch, cudaStream_t st) {

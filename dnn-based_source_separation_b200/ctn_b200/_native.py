@@ -172,12 +172,10 @@ ctn_mha_fwd = _sig("ctn_mha_fwd", _i, _fp, _i, _i, _i, _i, _fp, _fp, _fp, _fp, _
 ctn_seq_norm_fwd = _sig("ctn_seq_norm_fwd", _i, _fp, _fp, _fp, _fp, _fp, _fp, _fp, _i, _i, _i, _i, _f, _i, _fp)
 ctn_dpt_head_workspace_bytes = _sig("ctn_dpt_head_workspace_bytes", _sz, _i, _i, _i, _i, _i, _i)
 ctn_dpt_head_fwd = _sig("ctn_dpt_head_fwd", _i, _fp, _fp, _fp, _fp, _fp, _fp, _i, _i, _i, _i, _i, _i, _i, _i, _i, _f, _i, _fp, _sz, _fp)
-ctn_dpt_tail_workspace_bytes = _sig("ctn_dpt_tail_workspace_bytes", _sz, _i, _i, _i, _i, _i)
-ctn_dpt_tail_fwd = _sig("ctn_dpt_tail_fwd", _i, _fp, _fp, _fp, _fp, _fp, _fp, _fp, _fp, _fp, _fp, _fp, _fp, _fp, _i, _i, _i, _i, _i, _i, _i,
-                        _i, _i, _i, _i, _i, _fp, _sz, _fp)
-# SepFormer path: pitched channel-first dual-path state, strided attention, token LayerNorm, per-sequence gLN + residual, encoder, tail
-ctn_sfm_segment_fwd = _sig("ctn_sfm_segment_fwd", _i, _fp, _fp, _i, _i, _i, _i, _i, _i, _i, _i, _i, _fp)
-ctn_sfm_overlap_add_fwd = _sig("ctn_sfm_overlap_add_fwd", _i, _fp, _fp, _i, _i, _i, _i, _i, _i, _i, _i, _i, _fp)
+ctn_dpt_tail_workspace_bytes = _sig("ctn_dpt_tail_workspace_bytes", _sz, _i, _i, _i, _i, _i, _i)
+ctn_dpt_tail_fwd = _sig("ctn_dpt_tail_fwd", _i, _fp, _fp, _fp, _fp, _fp, _fp, _fp, _fp, _fp, _fp, _fp, _fp, _fp, _fp, _fp, _i, _i, _i, _i,
+                        _i, _i, _i, _i, _i, _i, _i, _i, _fp, _sz, _fp)
+# SepFormer path: strided attention, token LayerNorm, per-sequence gLN + residual, encoder
 ctn_sfm_attn_supported = _sig("ctn_sfm_attn_supported", _i, _i, _i)
 ctn_sfm_attn_fwd = _sig("ctn_sfm_attn_fwd", _i, _fp, _fp, _fp, _i, _i, _i, _i, _i, _i, _i, _fp)
 ctn_sfm_token_ln_fwd = _sig("ctn_sfm_token_ln_fwd", _i, _fp, _fp, _fp, _fp, _fp, _fp, _i, _i, _i, _i, _f, _fp)
@@ -186,9 +184,6 @@ ctn_sfm_pos_enc_fwd = _sig("ctn_sfm_pos_enc_fwd", _i, _fp, _fp, _fp, _i, _i, _i,
 ctn_sfm_transformer_workspace_bytes = _sig("ctn_sfm_transformer_workspace_bytes", _sz, _i, _i, _i, _i, _i, _i)
 ctn_sfm_transformer_fwd = _sig("ctn_sfm_transformer_fwd", _i, _fp, _fp, C.POINTER(_fp), _i, _i, _i, _i, _i, _i, _i, _i, _i, _f, _i, _fp,
                                _sz, _fp)
-ctn_sfm_tail_workspace_bytes = _sig("ctn_sfm_tail_workspace_bytes", _sz, _i, _i, _i, _i, _i)
-ctn_sfm_tail_fwd = _sig("ctn_sfm_tail_fwd", _i, _fp, _fp, _fp, _fp, _fp, _fp, _fp, _fp, _fp, _fp, _fp, _fp, _fp, _fp, _fp, _i, _i, _i, _i,
-                        _i, _i, _i, _i, _i, _i, _i, _i, _fp, _sz, _fp)
 # LSTM-TasNet: gated encoder + frame norm, the persistent (bi-)LSTM layer, and the fc / mask / decoder tail
 ctn_tas_enc_gated_fwd = _sig("ctn_tas_enc_gated_fwd", _i, _fp, _fp, _fp, _fp, _fp, _fp, _fp, _fp, _i, _i, _i, _i, _i, _i, _i, _i, _f, _f,
                              _fp)
@@ -201,9 +196,7 @@ ctn_tas_lstm_fwd = _sig("ctn_tas_lstm_fwd", _i, _fp, C.POINTER(_fp), _fp, _fp, _
 ctn_tas_tail_workspace_bytes = _sig("ctn_tas_tail_workspace_bytes", _sz, _i, _i, _i, _i)
 ctn_tas_tail_fwd = _sig("ctn_tas_tail_fwd", _i, _fp, _fp, _fp, _fp, _fp, _fp, _fp, _fp, _i, _i, _i, _i, _i, _i, _i, _i, _i, _i, _i, _i,
                         _fp, _sz, _fp)
-# GALRNet: the separator head (pad + segment + gLN, no bottleneck) and the low-dimension globally attentive block
-ctn_galr_head_workspace_bytes = _sig("ctn_galr_head_workspace_bytes", _sz, _i, _i, _i, _i)
-ctn_galr_head_fwd = _sig("ctn_galr_head_fwd", _i, _fp, _fp, _fp, _fp, _i, _i, _i, _i, _i, _i, _i, _i, _f, _fp, _sz, _fp)
+# GALRNet: the low-dimension globally attentive block
 ctn_galr_supported = _sig("ctn_galr_supported", _i, _i, _i, _i, _i)
 ctn_galr_inter_workspace_bytes = _sig("ctn_galr_inter_workspace_bytes", _sz, _i, _i, _i, _i, _i)
 ctn_galr_inter_fwd = _sig("ctn_galr_inter_fwd", _i, _fp, _fp, _fp, _fp, _fp, _fp, _i, _fp, _fp, _fp, _fp, _fp, _fp, _fp, _fp, _fp, _i, _i,
@@ -275,13 +268,12 @@ EXPORTED = [
     "ctn_bss_workspace_bytes", "ctn_bss_eval_sources", "ctn_bss_images_workspace_bytes", "ctn_bss_eval_images",
     "ctn_bilstm_relu_proj_fwd", "ctn_mha_supported", "ctn_mha_workspace_bytes", "ctn_mha_fwd", "ctn_seq_norm_fwd",
     "ctn_dpt_head_workspace_bytes", "ctn_dpt_head_fwd", "ctn_dpt_tail_workspace_bytes", "ctn_dpt_tail_fwd",
-    "ctn_sfm_segment_fwd", "ctn_sfm_overlap_add_fwd", "ctn_sfm_attn_supported", "ctn_sfm_attn_fwd", "ctn_sfm_token_ln_fwd",
+    "ctn_sfm_attn_supported", "ctn_sfm_attn_fwd", "ctn_sfm_token_ln_fwd",
     "ctn_sfm_seq_norm_res_fwd", "ctn_sfm_pos_enc_fwd", "ctn_sfm_transformer_workspace_bytes", "ctn_sfm_transformer_fwd",
-    "ctn_sfm_tail_workspace_bytes", "ctn_sfm_tail_fwd",
     "ctn_tas_enc_gated_fwd", "ctn_tas_frame_norm_fwd", "ctn_tas_lstm_max_hidden", "ctn_tas_lstm_supported", "ctn_tas_lstm_group",
     "ctn_tas_lstm_workspace_bytes", "ctn_tas_lstm_fwd", "ctn_tas_tail_workspace_bytes", "ctn_tas_tail_fwd",
     "ctn_tas_online_state_bytes", "ctn_tas_online_init", "ctn_tas_online_reset", "ctn_tas_online_push", "ctn_tas_online_flush",
-    "ctn_galr_head_workspace_bytes", "ctn_galr_head_fwd", "ctn_galr_supported", "ctn_galr_inter_workspace_bytes", "ctn_galr_inter_fwd",
+    "ctn_galr_supported", "ctn_galr_inter_workspace_bytes", "ctn_galr_inter_fwd",
 ]
 
 

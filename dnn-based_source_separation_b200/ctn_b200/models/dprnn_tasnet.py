@@ -15,9 +15,8 @@ import torch.nn as nn
 from .. import _native as N
 from ..utils.filterbank import choose_filterbank
 from ..utils.tasnet import choose_layer_norm
+from ._dual_path import forward_only, math_of, segment_geometry
 from .dprnn import DPRNN
-from .tdcn import resolve_math
-from . import tdcn as _tdcn
 from .transform import (Segment1d, OverlapAdd1d, ctn_segment_fwd, ctn_overlap_add_fwd, ctn_stage_workspace_bytes, ctn_sep_head_fwd,
                         ctn_sep_tail_fwd)
 
@@ -49,18 +48,9 @@ class Separator(nn.Module):
             raise ValueError("Cannot support {}".format(mask_nonlinear))
         self.math = None
 
-    def _math(self):
-        return resolve_math(self.math if self.math is not None else _tdcn.DEFAULT_MATH)
-
     def segment_geometry(self, n_frames):
         """padding rule of dprnn_tasnet.py:339-341 -> (pad_left, pad_right, S)"""
-        K, P = self.chunk_size, self.hop_size
-        padding = (P - (n_frames - K) % P) % P
-        pl = padding // 2
-        pr = padding - pl
-        if n_frames + padding < K:
-            raise ValueError("n_frames={} is too short for chunk_size={}".format(n_frames, K))
-        return pl, pr, (n_frames + padding - K) // P + 1
+        return segment_geometry(n_frames, self.chunk_size, self.hop_size)
 
     def run_pitched(self, w, stats0, frames, pitch, dev):
         """w (B, N, pitch) pitched encoder output (+ its statistics) -> y (B, Bc, pitch): everything between the encoder and the
@@ -73,7 +63,7 @@ class Separator(nn.Module):
         x0 = torch.empty(B, Bc, pitch, dtype=torch.float32, device=dev)
         g0, b0 = self.norm1d.norm.weight, self.norm1d.norm.bias
         N.check(ctn_sep_head_fwd(w.data_ptr(), stats0.data_ptr(), g0.data_ptr(), b0.data_ptr(), self.bottleneck_conv1d.weight.data_ptr(),
-                                 self.bottleneck_conv1d.bias.data_ptr(), x0.data_ptr(), B, Nf, Bc, frames, pitch, float(self.eps), self._math(),
+                                 self.bottleneck_conv1d.bias.data_ptr(), x0.data_ptr(), B, Nf, Bc, frames, pitch, float(self.eps), math_of(self.math),
                                  base, nbytes, st), "ctn_sep_head_fwd")
         pl, pr, S = self.segment_geometry(frames)
         z = torch.empty(B, S, K, Bc, dtype=torch.float32, device=dev)
@@ -130,8 +120,7 @@ class DPRNNTasNet(nn.Module):
             raise NotImplementedError("multichannel (4-D) input is outside the sm_90a kernel envelope")
         else:
             raise ValueError("Not support {} dimension input".format(n_dim))
-        if torch.is_grad_enabled() and any(p.requires_grad for p in self.parameters()):
-            raise NotImplementedError("the DPRNN-TasNet path is forward-only: call under torch.no_grad()")
+        forward_only(self, input)
         x = input.contiguous()
         B, _, T = x.shape
         if B > 65535:  # segmentation, overlap-add and the gLN + residual put the batch on a grid axis of at most 65535 blocks
@@ -154,7 +143,7 @@ class DPRNNTasNet(nn.Module):
         N.check(ctn_sep_tail_fwd(y.data_ptr(), w.data_ptr(), sep.prelu.weight.data_ptr(), sep.mask_conv1d.weight.data_ptr(),
                                  sep.mask_conv1d.bias.data_ptr(), self.decoder.conv_transpose1d.weight.data_ptr(), out.data_ptr(),
                                  N.ptr(latent), what.data_ptr(), B, Nb, sep.bottleneck_channels, S, frames, pitch, self.kernel_size,
-                                 self.stride, pl, T, sep._math(), base, ws_bytes, st), "ctn_sep_tail_fwd")
+                                 self.stride, pl, T, math_of(sep.math), base, ws_bytes, st), "ctn_sep_tail_fwd")
         return out, latent
 
     def get_config(self):

@@ -12,8 +12,6 @@ The dual-path state stays channels-last, (batch, D1, D2, F), as on the DPRNN-Tas
 Envelope: trainable bases, monaural 3-D input, non-causal, sep_norm=True, sep_nonlinear='relu', mask 'relu' or 'sigmoid',
 num_features and hidden_channels inside the native LSTM's sizes, head dimension F / heads in {8, 16, 32, 64}; forward only.
 """
-import os
-
 import torch
 import torch.nn as nn
 
@@ -21,24 +19,13 @@ from .. import _native as N
 from ..utils.filterbank import choose_filterbank
 from ..utils.model import choose_nonlinear
 from ..utils.tasnet import choose_layer_norm
+from ._dual_path import GTUTailModel, build_from_pretrained, eval_dropout, forward_only, math_of, segment_geometry
 from .conv_tasnet import _load_checkpoint
 from .dprnn import choose_rnn
 from .gtu import GTU1d
-from .tdcn import resolve_math
-from . import tdcn as _tdcn
 from .transform import Segment1d, OverlapAdd1d
 
 EPS = 1e-12
-
-
-def _no_grad_check(module):
-    if torch.is_grad_enabled() and any(p.requires_grad for p in module.parameters()):
-        raise NotImplementedError("the DPTNet path is forward-only: call under torch.no_grad()")
-
-
-def _dropout_check(module, dropout):
-    if module.training and dropout > 0:
-        raise NotImplementedError("dropout > 0 in training mode is outside the sm_90a path: call model.eval()")
 
 
 class MultiheadAttentionBlock(nn.Module):
@@ -62,12 +49,12 @@ class MultiheadAttentionBlock(nn.Module):
 
     def forward(self, input):
         """input, output (T, batch_size, embed_dim) (dptnet.py:502-525)"""
-        _no_grad_check(self)
+        forward_only(self, input)
         return self._step(input.permute(1, 0, 2).unsqueeze(0).contiguous(), False)[0].permute(1, 0, 2).contiguous()
 
     def _step(self, z, swap):
         """z (B, D1, D2, F) channels-last -> GroupNorm over each (b, d1) sequence of z + MHA(z), (B, D2, D1, F) when swap"""
-        _dropout_check(self, self.dropout_p)
+        eval_dropout(self, self.dropout_p)
         B, D1, D2, F = z.shape
         dev = N.require_cuda(z)
         st = N.stream_ptr(dev)
@@ -105,7 +92,7 @@ class FeedForwardBlock(nn.Module):
 
     def forward(self, input):
         """input, output (T, batch_size, num_features) (dptnet.py:548-572)"""
-        _no_grad_check(self)
+        forward_only(self, input)
         return self._step(input.permute(1, 0, 2).unsqueeze(0).contiguous(), False)[0].permute(1, 0, 2).contiguous()
 
     def _step(self, z, swap):
@@ -136,7 +123,7 @@ class ImprovedTransformer(nn.Module):
 
     def forward(self, input):
         """input, output (T, batch_size, num_features)"""
-        _no_grad_check(self)
+        forward_only(self, input)
         return self._step(input.permute(1, 0, 2).unsqueeze(0).contiguous(), False)[0].permute(1, 0, 2).contiguous()
 
     def _step(self, z, swap):
@@ -152,7 +139,7 @@ class IntraChunkTransformer(nn.Module):
 
     def forward(self, input):
         """input, output (batch_size, num_features, S, chunk_size) (dptnet.py:414-430)"""
-        _no_grad_check(self)
+        forward_only(self, input)
         return self.transformer._step(input.permute(0, 2, 3, 1).contiguous(), False).permute(0, 3, 1, 2).contiguous()
 
 
@@ -165,7 +152,7 @@ class InterChunkTransformer(nn.Module):
 
     def forward(self, input):
         """input, output (batch_size, num_features, S, chunk_size) (dptnet.py:445-461)"""
-        _no_grad_check(self)
+        forward_only(self, input)
         return self.transformer._step(input.permute(0, 3, 2, 1).contiguous(), False).permute(0, 3, 2, 1).contiguous()
 
 
@@ -179,7 +166,7 @@ class DualPathTransformerBlock(nn.Module):
 
     def forward(self, input):
         """input, output (batch_size, num_features, S, chunk_size)"""
-        _no_grad_check(self)
+        forward_only(self, input)
         return self.forward_channels_last(input.permute(0, 2, 3, 1).contiguous()).permute(0, 3, 1, 2).contiguous()
 
     def forward_channels_last(self, z):
@@ -199,7 +186,7 @@ class DualPathTransformer(nn.Module):
 
     def forward(self, input):
         """input, output (batch_size, num_features, S, chunk_size)"""
-        _no_grad_check(self)
+        forward_only(self, input)
         return self.forward_channels_last(input.permute(0, 2, 3, 1).contiguous()).permute(0, 3, 1, 2).contiguous()
 
     def forward_channels_last(self, z):
@@ -237,23 +224,16 @@ class Separator(nn.Module):
         self.mask_relu = mask_nonlinear == 'relu'
         self.math = None
 
-    def _math(self):
-        return resolve_math(self.math if self.math is not None else _tdcn.DEFAULT_MATH)
+    folds_gln = False
 
-    def segment_geometry(self, n_frames):
-        """padding rule of dptnet.py:330-332 -> (pad_left, pad_right, S)"""
-        K, P = self.chunk_size, self.hop_size
-        padding = (P - (n_frames - K) % P) % P
-        pl = padding // 2
-        if n_frames + padding < K:
-            raise ValueError("n_frames={} is too short for chunk_size={}".format(n_frames, K))
-        return pl, padding - pl, (n_frames + padding - K) // P + 1
+    def check(self, B, n_frames):
+        segment_geometry(n_frames, self.chunk_size, self.hop_size)
 
-    def run_pitched(self, w, frames, pitch, dev):
+    def run_pitched(self, w, stats0, frames, pitch, dev):
         """w (B, N, pitch) pitched encoder output -> y (B, Bc, pitch): everything between the encoder and the PReLU of dptnet.py:341"""
         B = w.shape[0]
         Nf, Bc, K, P = self.num_features, self.bottleneck_channels, self.chunk_size, self.hop_size
-        pl, pr, S = self.segment_geometry(frames)
+        pl, pr, S = segment_geometry(frames, K, P)
         st = N.stream_ptr(dev)
         z = torch.empty(B, S, K, Bc, dtype=torch.float32, device=dev)
         nws = N.ctn_dpt_head_workspace_bytes(B, Nf, Bc, pitch, S, K)
@@ -261,7 +241,7 @@ class Separator(nn.Module):
         g, b = self.norm2d.norm.weight, self.norm2d.norm.bias
         N.check(N.ctn_dpt_head_fwd(w.data_ptr(), self.bottleneck_conv1d.weight.data_ptr(), self.bottleneck_conv1d.bias.data_ptr(),
                                    g.data_ptr(), b.data_ptr(), z.data_ptr(), B, Nf, Bc, frames, pitch, K, P, pl, pr, float(self.eps),
-                                   self._math(), base, nbytes, st), "ctn_dpt_head_fwd")
+                                   math_of(self.math), base, nbytes, st), "ctn_dpt_head_fwd")
         z = self.dptransformer.forward_channels_last(z)
         y = torch.empty(B, Bc, pitch, dtype=torch.float32, device=dev)
         N.check(N.ctn_overlap_add_fwd(z.data_ptr(), y.data_ptr(), B, Bc, S, K, P, pl, frames, pitch, 1, st), "ctn_overlap_add_fwd")
@@ -272,7 +252,7 @@ class Separator(nn.Module):
         raise NotImplementedError("the stand-alone DPTNet Separator.forward (materialised mask) is not built; use DPTNet")
 
 
-class DPTNet(nn.Module):
+class DPTNet(GTUTailModel):
     """Dual-path transformer based network"""
     pretrained_model_ids = {
         "wsj0-mix": {
@@ -319,45 +299,6 @@ class DPTNet(nn.Module):
         self.decoder = decoder
         self.math = None
 
-    def forward(self, input):
-        output, _ = self._run(input, want_latent=False)
-        return output
-
-    def extract_latent(self, input):
-        """input (batch_size, 1, T) -> output (batch_size, n_sources, T), latent (batch_size, n_sources, n_basis, T')"""
-        return self._run(input, want_latent=True)
-
-    def _run(self, input, want_latent):
-        if input.dim() != 3:
-            raise ValueError("input.size() is expected (?, 1, ?), but given {}".format(tuple(input.size())))
-        assert input.size(1) == 1, "input.size() is expected (?, 1, ?), but given {}".format(input.size())
-        _no_grad_check(self)
-        _dropout_check(self, self.sep_dropout)
-        x = input.contiguous()
-        dev = N.require_cuda(x)
-        B, _, T = x.shape
-        sep = self.separator
-        sep.math = self.math if self.math is not None else sep.math
-        frames, pl, pr = N.frames_of(T, self.kernel_size, self.stride)
-        pitch = N.ctn_pitch(frames)
-        st = N.stream_ptr(dev)
-        Nb, S = self.n_basis, self.n_sources
-        w = torch.empty(B, Nb, pitch, dtype=torch.float32, device=dev)
-        N.check(N.ctn_encoder_fwd(x.data_ptr(), self.encoder.conv1d.weight.data_ptr(), w.data_ptr(), B, T, pl, pr, Nb, self.kernel_size,
-                                  self.stride, int(self.encoder.nonlinear), pitch, None, st), "ctn_encoder_fwd")
-        y = sep.run_pitched(w, frames, pitch, dev)
-        out = torch.empty(B, S, T, dtype=torch.float32, device=dev)
-        latent = torch.empty(B, S, Nb, frames, dtype=torch.float32, device=dev) if want_latent else None
-        what = torch.empty(B, S * Nb, pitch, dtype=torch.float32, device=dev)
-        nws = N.ctn_dpt_tail_workspace_bytes(B, Nb, sep.bottleneck_channels, S, pitch)
-        base, nbytes = N.aligned(N.workspace(dev, nws + 256, tag="dpt_tail"))
-        N.check(N.ctn_dpt_tail_fwd(y.data_ptr(), w.data_ptr(), sep.prelu.weight.data_ptr(), sep.map.weight.data_ptr(), sep.map.bias.data_ptr(),
-                                   sep.gtu.map.weight.data_ptr(), sep.gtu.map.bias.data_ptr(), sep.gtu.map_gate.weight.data_ptr(),
-                                   sep.gtu.map_gate.bias.data_ptr(), self.decoder.conv_transpose1d.weight.data_ptr(), out.data_ptr(),
-                                   N.ptr(latent), what.data_ptr(), B, Nb, sep.bottleneck_channels, S, frames, pitch, self.kernel_size,
-                                   self.stride, pl, T, int(sep.mask_relu), sep._math(), base, nbytes, st), "ctn_dpt_tail_fwd")
-        return out, latent
-
     def get_config(self):
         return {
             'n_basis': self.n_basis, 'kernel_size': self.kernel_size, 'stride': self.stride, 'enc_basis': self.enc_basis,
@@ -390,32 +331,5 @@ class DPTNet(nn.Module):
 
     @classmethod
     def build_from_pretrained(cls, root="./pretrained", quiet=False, load_state_dict=True, **kwargs):
-        """dptnet.py:219-259: resolve <root>/DPTNet/wsj0-mix/sr<rate>/<n>speakers/model/<choice>.pth like the reference and build the
-        model from it.  The download step is the reference's own helper; when the file is not there and that helper is not
-        importable, FileNotFoundError names the expected path."""
-        task = kwargs.get('task')
-        if task not in cls.pretrained_model_ids:
-            raise KeyError("Invalid task ({}) is specified.".format(task))
-        if task not in ['wsj0-mix', 'wsj0']:
-            raise NotImplementedError("Not support task={}.".format(task))
-        sample_rate = kwargs.get('sample_rate') or 8000
-        n_sources = kwargs.get('n_sources') or 2
-        model_choice = kwargs.get('model_choice') or 'best'
-        model_id = cls.pretrained_model_ids[task][sample_rate][n_sources]
-        download_dir = os.path.join(root, cls.__name__, task, "sr{}/{}speakers".format(sample_rate, n_sources))
-        model_path = os.path.join(download_dir, "model", "{}.pth".format(model_choice))
-        if not os.path.exists(model_path):
-            try:
-                from utils.utils import download_pretrained_model_from_google_drive  # the reference's helper, when src/ is on the path
-            except Exception:
-                raise FileNotFoundError("{} not found (Google-Drive id {!r}); place the reference checkpoint there -- this path loads "
-                                        "checkpoints, it does not download them".format(model_path, model_id))
-            download_pretrained_model_from_google_drive(model_id, download_dir, quiet=quiet)
-        model = cls.build_model(model_path, load_state_dict=load_state_dict)
-        for key, value in {'n_sources': n_sources, 'sample_rate': sample_rate}.items():
-            setattr(model, key, value)
-        return model
-
-    @property
-    def num_parameters(self):
-        return sum(p.numel() for p in self.parameters() if p.requires_grad)
+        """dptnet.py:219-259: <root>/DPTNet/wsj0-mix/sr<rate>/<n>speakers/model/<choice>.pth, loaded, never downloaded"""
+        return build_from_pretrained(cls, root, load_state_dict, **kwargs)

@@ -16,19 +16,10 @@ import torch.nn as nn
 
 from .. import _native as N
 from ..utils.tasnet import choose_layer_norm
+from ._dual_path import eval_dropout, forward_only
 from .dprnn import IntraChunkRNN as LocallyRecurrentBlock
 
 EPS = 1e-12
-
-
-def _no_grad_check(module, *inputs):
-    if torch.is_grad_enabled() and (any(p.requires_grad for p in module.parameters()) or any(t.requires_grad for t in inputs)):
-        raise NotImplementedError("the GALRNet path is forward-only: call under torch.no_grad()")
-
-
-def _dropout_check(module, dropout):
-    if module.training and dropout is not None and dropout > 0:
-        raise NotImplementedError("dropout > 0 in training mode is outside the sm_90a path: call model.eval()")
 
 
 class GALR(nn.Module):
@@ -40,7 +31,7 @@ class GALR(nn.Module):
 
     def forward(self, input):
         """input, output (batch_size, num_features, S, chunk_size)"""
-        _no_grad_check(self, input)
+        forward_only(self, input)
         return self.forward_channels_last(input.permute(0, 2, 3, 1).contiguous()).permute(0, 3, 1, 2).contiguous()
 
     def forward_channels_last(self, z):
@@ -67,13 +58,13 @@ class GALRBlock(nn.Module):
 
     def forward(self, input):
         """input, output (batch_size, num_features, S, chunk_size)"""
-        _no_grad_check(self, input)
+        forward_only(self, input)
         return self.forward_channels_last(input.permute(0, 2, 3, 1).contiguous()).permute(0, 3, 1, 2).contiguous()
 
     def forward_channels_last(self, z):
         """z (B, S, K, F) -> (B, S, K, F): the bi-LSTM over the K frames of each chunk, then the attention over the S chunks"""
         self.inter_chunk_block.check_shape(z.shape)
-        _dropout_check(self.inter_chunk_block, self.inter_chunk_block.dropout_p)
+        eval_dropout(self.inter_chunk_block, self.inter_chunk_block.dropout_p)
         return self.inter_chunk_block._step(self.intra_chunk_block._step(z, swap=False))
 
 
@@ -128,8 +119,8 @@ class LowDimensionGloballyAttentiveBlock(GloballyAttentiveBlockBase):
 
     def forward(self, input):
         """input, output (batch_size, num_features, S, K) (galr.py:161-197)"""
-        _no_grad_check(self, input)
-        _dropout_check(self, self.dropout_p)
+        forward_only(self, input)
+        eval_dropout(self, self.dropout_p)
         z = input.permute(0, 2, 3, 1).contiguous()
         self.check_shape(z.shape)
         return self._step(z).permute(0, 3, 1, 2).contiguous()

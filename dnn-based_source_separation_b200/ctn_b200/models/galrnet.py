@@ -3,8 +3,8 @@
 Same constructor, module tree, ``state_dict`` keys, ``get_config`` and ``num_parameters`` as the reference, so a checkpoint the
 recipe's trainer saves (its ``get_config()`` plus ``'state_dict'``) loads with ``GALRNet(**config)`` and
 ``load_state_dict(strict=True)``.  Forward = encoder kernel -> pad + Segment1d (channels-last) + gLN over the segmented tensor
-(``ctn_galr_head_fwd``) -> N x GALRBlock (models/galr.py) -> OverlapAdd1d + crop -> PReLU + map 1x1 + GTU1d + mask nonlinearity +
-w * mask + transposed-conv decoder (``ctn_dpt_tail_fwd`` with the bottleneck width equal to n_basis: GALRNet has no bottleneck).
+(``ctn_dpt_head_fwd`` without a bottleneck) -> N x GALRBlock (models/galr.py) -> OverlapAdd1d + crop -> PReLU + map 1x1 + GTU1d +
+mask nonlinearity + w * mask + transposed-conv decoder (``ctn_dpt_tail_fwd`` with the bottleneck width equal to n_basis).
 Envelope: trainable bases, monaural 3-D input, non-causal, sep_norm=True, low_dimension=True, mask 'relu' or 'sigmoid', the GALR
 blocks' sizes (models/galr.py); forward only, dropout only in eval mode.
 """
@@ -15,16 +15,15 @@ from .. import _native as N
 from ..utils.filterbank import choose_filterbank
 from ..utils.model import choose_nonlinear
 from ..utils.tasnet import choose_layer_norm
-from .galr import GALR, _dropout_check, _no_grad_check
+from ._dual_path import GTUTailModel, math_of, segment_geometry
+from .galr import GALR
 from .gtu import GTU1d
-from .tdcn import resolve_math
-from . import tdcn as _tdcn
 from .transform import Segment1d, OverlapAdd1d
 
 EPS = 1e-12
 
 
-class GALRNet(nn.Module):
+class GALRNet(GTUTailModel):
     def __init__(self, n_basis, kernel_size, stride=None, enc_basis=None, dec_basis=None, sep_hidden_channels=128, sep_chunk_size=100,
                  sep_hop_size=50, sep_down_chunk_size=None, sep_num_blocks=6, sep_num_heads=8, sep_norm=True, sep_dropout=0.1,
                  mask_nonlinear='relu', causal=True, n_sources=2, low_dimension=True, eps=EPS, **kwargs):
@@ -58,48 +57,6 @@ class GALRNet(nn.Module):
         self.decoder = decoder
         self.math = None
 
-    def forward(self, input):
-        output, _ = self._run(input, want_latent=False)
-        return output
-
-    def extract_latent(self, input):
-        """input (batch_size, 1, T) -> output (batch_size, n_sources, T), latent (batch_size, n_sources, n_basis, T')"""
-        return self._run(input, want_latent=True)
-
-    def _run(self, input, want_latent):
-        if input.dim() != 3:
-            raise ValueError("input.size() is expected (?, 1, ?), but given {}".format(tuple(input.size())))
-        assert input.size(1) == 1, "input.size() is expected (?, 1, ?), but given {}".format(input.size())
-        _no_grad_check(self, input)
-        _dropout_check(self, self.sep_dropout)
-        x = input.contiguous()
-        B, _, T = x.shape
-        sep = self.separator
-        sep.math = self.math if self.math is not None else sep.math
-        frames, pl, pr = N.frames_of(T, self.kernel_size, self.stride)
-        _, _, S_chunks = sep.segment_geometry(frames)
-        for blk in sep.galr.net:
-            blk.inter_chunk_block.check_shape((B, S_chunks, sep.chunk_size, self.n_basis))
-        dev = N.require_cuda(x)
-        pitch = N.ctn_pitch(frames)
-        st = N.stream_ptr(dev)
-        Nb, S = self.n_basis, self.n_sources
-        w = torch.empty(B, Nb, pitch, dtype=torch.float32, device=dev)
-        N.check(N.ctn_encoder_fwd(x.data_ptr(), self.encoder.conv1d.weight.data_ptr(), w.data_ptr(), B, T, pl, pr, Nb, self.kernel_size,
-                                  self.stride, int(self.encoder.nonlinear), pitch, None, st), "ctn_encoder_fwd")
-        y = sep.run_pitched(w, frames, pitch, dev)
-        out = torch.empty(B, S, T, dtype=torch.float32, device=dev)
-        latent = torch.empty(B, S, Nb, frames, dtype=torch.float32, device=dev) if want_latent else None
-        what = torch.empty(B, S * Nb, pitch, dtype=torch.float32, device=dev)
-        nws = N.ctn_dpt_tail_workspace_bytes(B, Nb, Nb, S, pitch)
-        base, nbytes = N.aligned(N.workspace(dev, nws + 256, tag="galr_tail"))
-        N.check(N.ctn_dpt_tail_fwd(y.data_ptr(), w.data_ptr(), sep.prelu.weight.data_ptr(), sep.map.weight.data_ptr(), sep.map.bias.data_ptr(),
-                                   sep.gtu.map.weight.data_ptr(), sep.gtu.map.bias.data_ptr(), sep.gtu.map_gate.weight.data_ptr(),
-                                   sep.gtu.map_gate.bias.data_ptr(), self.decoder.conv_transpose1d.weight.data_ptr(), out.data_ptr(),
-                                   N.ptr(latent), what.data_ptr(), B, Nb, Nb, S, frames, pitch, self.kernel_size, self.stride, pl, T,
-                                   int(sep.mask_relu), sep._math(), base, nbytes, st), "ctn_dpt_tail_fwd")
-        return out, latent
-
     def get_config(self):
         return {
             'n_basis': self.n_basis, 'kernel_size': self.kernel_size, 'stride': self.stride, 'enc_basis': self.enc_basis,
@@ -110,10 +67,6 @@ class GALRNet(nn.Module):
             'sep_norm': self.sep_norm, 'sep_dropout': self.sep_dropout, 'low_dimension': self.low_dimension,
             'mask_nonlinear': self.mask_nonlinear, 'causal': self.causal, 'n_sources': self.n_sources, 'eps': self.eps,
         }
-
-    @property
-    def num_parameters(self):
-        return sum(p.numel() for p in self.parameters() if p.requires_grad)
 
 
 class Separator(nn.Module):
@@ -147,30 +100,26 @@ class Separator(nn.Module):
         self.mask_relu = mask_nonlinear == 'relu'
         self.math = None
 
-    def _math(self):
-        return resolve_math(self.math if self.math is not None else _tdcn.DEFAULT_MATH)
+    folds_gln = False
 
-    def segment_geometry(self, n_frames):
-        """padding rule of galrnet.py:233-235 -> (pad_left, pad_right, S)"""
-        K, P = self.chunk_size, self.hop_size
-        padding = (P - (n_frames - K) % P) % P
-        pl = padding // 2
-        if n_frames + padding < K:
-            raise ValueError("n_frames={} is too short for chunk_size={}".format(n_frames, K))
-        return pl, padding - pl, (n_frames + padding - K) // P + 1
+    def check(self, B, n_frames):
+        """the padding rule of galrnet.py:233-235, and every GALR block's launch limits"""
+        S = segment_geometry(n_frames, self.chunk_size, self.hop_size)[2]
+        for blk in self.galr.net:
+            blk.inter_chunk_block.check_shape((B, S, self.chunk_size, self.num_features))
 
-    def run_pitched(self, w, frames, pitch, dev):
+    def run_pitched(self, w, stats0, frames, pitch, dev):
         """w (B, N, pitch) pitched encoder output -> y (B, N, pitch): everything between the encoder and the PReLU of galrnet.py:243"""
         B = w.shape[0]
         Nf, K, P = self.num_features, self.chunk_size, self.hop_size
-        pl, pr, S = self.segment_geometry(frames)
+        pl, pr, S = segment_geometry(frames, K, P)
         st = N.stream_ptr(dev)
         z = torch.empty(B, S, K, Nf, dtype=torch.float32, device=dev)
-        nws = N.ctn_galr_head_workspace_bytes(B, S, K, Nf)
+        nws = N.ctn_dpt_head_workspace_bytes(B, Nf, Nf, pitch, S, K)
         base, nbytes = N.aligned(N.workspace(dev, nws + 256, tag="galr_head"))
         g, b = self.norm2d.norm.weight, self.norm2d.norm.bias
-        N.check(N.ctn_galr_head_fwd(w.data_ptr(), g.data_ptr(), b.data_ptr(), z.data_ptr(), B, Nf, frames, pitch, K, P, pl, pr,
-                                    float(self.eps), base, nbytes, st), "ctn_galr_head_fwd")
+        N.check(N.ctn_dpt_head_fwd(w.data_ptr(), None, None, g.data_ptr(), b.data_ptr(), z.data_ptr(), B, Nf, Nf, frames, pitch, K, P, pl, pr,
+                                   float(self.eps), math_of(self.math), base, nbytes, st), "ctn_dpt_head_fwd")
         z = self.galr.forward_channels_last(z)
         y = torch.empty(B, Nf, pitch, dtype=torch.float32, device=dev)
         N.check(N.ctn_overlap_add_fwd(z.data_ptr(), y.data_ptr(), B, Nf, S, K, P, pl, frames, pitch, 1, st), "ctn_overlap_add_fwd")

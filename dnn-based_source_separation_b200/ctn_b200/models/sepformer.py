@@ -3,9 +3,10 @@
 Same constructors, module tree and ``state_dict`` keys as the reference (torch's own ``nn.TransformerEncoder`` /
 ``nn.TransformerEncoderLayer`` hold the layer parameters), so its checkpoints load with ``load_state_dict(strict=True)``.
 Forward = encoder kernel (+ the gLN statistics of w) -> gLN + bottleneck_conv1d_in (``ctn_sep_head_fwd``) -> pad + Segment1d
-into the pitched channel-first state (``ctn_sfm_segment_fwd``) -> per SepFormerBlock one IntraTransformer and one
-InterTransformer (``ctn_sfm_transformer_fwd`` each) -> OverlapAdd1d + crop (``ctn_sfm_overlap_add_fwd``) -> PReLU, map, GTU1d,
-bottleneck_conv1d_out, mask nonlinearity, w * mask and the transposed-conv decoder (``ctn_sfm_tail_fwd``).
+into the pitched channel-first state (``ctn_segment_fwd`` with a row pitch) -> per SepFormerBlock one IntraTransformer and one
+InterTransformer (``ctn_sfm_transformer_fwd`` each) -> OverlapAdd1d + crop (``ctn_overlap_add_fwd``) -> PReLU, map, GTU1d,
+bottleneck_conv1d_out, mask nonlinearity, w * mask and the transposed-conv decoder (``ctn_dpt_tail_fwd`` with
+bottleneck_conv1d_out).
 
 The dual-path state stays (B, F, pitch) with token s*C + k for chunk s and frame k (csrc/ctn_sepformer.cu): the four Linear
 layers of every encoder layer are ctn_pw contractions in the model's numeric mode, and the two paths differ only in the token
@@ -14,8 +15,6 @@ residual is the block input itself.
 Envelope: trainable bases, monaural 3-D input, causal=False, sep_norm=True, sep_nonlinear='relu', mask 'relu' or 'sigmoid',
 head dimensions F / heads in {8, 16, 32, 64} for the intra and the inter heads; forward only (sep_dropout acts as in eval()).
 """
-import os
-
 import torch
 import torch.nn as nn
 
@@ -23,29 +22,14 @@ from .. import _native as N
 from ..utils.filterbank import choose_filterbank
 from ..utils.model import choose_nonlinear
 from ..utils.tasnet import choose_layer_norm
+from ._dual_path import GTUTailModel, build_from_pretrained, eval_dropout, forward_only, math_of, segment_geometry
 from .conv_tasnet import _load_checkpoint
 from .gtu import GTU1d
-from .tdcn import resolve_math
-from . import tdcn as _tdcn
 from .transform import Segment1d, OverlapAdd1d
 from .transformer import PositionalEncoding
 
 EPS = 1e-12
 PE_ROWS = 5000  # rows of PositionalEncoding's buffer (transformer.py:8): the longest sequence either path can take
-
-
-def _no_grad_check(module):
-    if torch.is_grad_enabled() and any(p.requires_grad for p in module.parameters()):
-        raise NotImplementedError("the SepFormer path is forward-only: call under torch.no_grad()")
-
-
-def _dropout_check(module, dropout):
-    if module.training and dropout > 0:
-        raise NotImplementedError("dropout > 0 in training mode is outside the sm_90a path: call model.eval()")
-
-
-def _math_of(math):
-    return resolve_math(math if math is not None else _tdcn.DEFAULT_MATH)
 
 
 class LayerNormWrapper(nn.Module):
@@ -104,7 +88,7 @@ class _PathTransformer(nn.Module):
 
     def run_pitched(self, z, S, C, math):
         """z (B, F, pitch) pitched state, token s*C + k -> a new (B, F, pitch) tensor"""
-        _dropout_check(self, self.dropout_p)
+        eval_dropout(self, self.dropout_p)
         B, F, pitch = z.shape
         dev = N.require_cuda(z)
         out = torch.empty_like(z)
@@ -117,8 +101,8 @@ class _PathTransformer(nn.Module):
 
     def forward(self, input):
         """input, output (batch_size, num_features, S, chunk_size)"""
-        _no_grad_check(self)
-        return _on_pitched(lambda z, S, C: self.run_pitched(z, S, C, _math_of(None)), input)
+        forward_only(self, input)
+        return _on_pitched(lambda z, S, C: self.run_pitched(z, S, C, math_of(None)), input)
 
 
 def _on_pitched(fn, input):
@@ -168,8 +152,8 @@ class SepFormerBlock(nn.Module):
 
     def forward(self, input):
         """input, output (batch_size, num_features, S, chunk_size)"""
-        _no_grad_check(self)
-        return _on_pitched(lambda z, S, C: self.run_pitched(z, S, C, _math_of(None)), input)
+        forward_only(self, input)
+        return _on_pitched(lambda z, S, C: self.run_pitched(z, S, C, math_of(None)), input)
 
 
 class SepFormerBackbone(nn.Module):
@@ -189,8 +173,8 @@ class SepFormerBackbone(nn.Module):
 
     def forward(self, input):
         """input, output (batch_size, num_features, S, chunk_size)"""
-        _no_grad_check(self)
-        return _on_pitched(lambda z, S, C: self.run_pitched(z, S, C, _math_of(None)), input)
+        forward_only(self, input)
+        return _on_pitched(lambda z, S, C: self.run_pitched(z, S, C, math_of(None)), input)
 
 
 class Separator(nn.Module):
@@ -225,27 +209,19 @@ class Separator(nn.Module):
         self.mask_relu = mask_nonlinear == 'relu'
         self.math = None
 
-    def _math(self):
-        return _math_of(self.math)
+    folds_gln = True
 
-    def segment_geometry(self, n_frames):
-        """padding rule of sepformer.py:342-344 -> (pad_left, pad_right, S)"""
-        K, P = self.chunk_size, self.hop_size
-        padding = (P - (n_frames - K) % P) % P
-        pl = padding // 2
-        if n_frames + padding < K:
-            raise ValueError("n_frames={} is too short for chunk_size={}".format(n_frames, K))
-        S = (n_frames + padding - K) // P + 1
-        _check_lengths(S, K)
-        return pl, padding - pl, S
+    def check(self, B, n_frames):
+        """the padding rule of sepformer.py:342-344, and sequences within the positional encoding's rows"""
+        _check_lengths(segment_geometry(n_frames, self.chunk_size, self.hop_size)[2], self.chunk_size)
 
     def run_pitched(self, w, stats0, frames, pitch, dev):
         """w (B, N, pitch) pitched encoder output (+ its statistics) -> y (B, Bc, pitch): everything between the encoder and the
         PReLU of sepformer.py:353"""
         B = w.shape[0]
         Nf, Bc, K, P = self.num_features, self.bottleneck_channels, self.chunk_size, self.hop_size
-        pl, pr, S = self.segment_geometry(frames)
-        math = self._math()
+        pl, pr, S = segment_geometry(frames, K, P)
+        math = math_of(self.math)
         st = N.stream_ptr(dev)
         base, nbytes = N.aligned(N.workspace(dev, N.ctn_stage_workspace_bytes(Bc, Nf) + 256, tag="sfm_head"))
         x0 = torch.empty(B, Bc, pitch, dtype=torch.float32, device=dev)
@@ -255,10 +231,10 @@ class Separator(nn.Module):
                                    base, nbytes, st), "ctn_sep_head_fwd")
         zp = N.ctn_pitch(S * K)
         z = torch.empty(B, Bc, zp, dtype=torch.float32, device=dev)
-        N.check(N.ctn_sfm_segment_fwd(x0.data_ptr(), z.data_ptr(), B, Bc, frames, pitch, K, P, pl, pr, zp, st), "ctn_sfm_segment_fwd")
+        N.check(N.ctn_segment_fwd(x0.data_ptr(), z.data_ptr(), B, Bc, frames, pitch, K, P, pl, pr, zp, st), "ctn_segment_fwd")
         z = self.dptransformer.run_pitched(z, S, K, math)
         y = torch.empty(B, Bc, pitch, dtype=torch.float32, device=dev)
-        N.check(N.ctn_sfm_overlap_add_fwd(z.data_ptr(), y.data_ptr(), B, Bc, S, K, P, zp, pl, frames, pitch, st), "ctn_sfm_overlap_add_fwd")
+        N.check(N.ctn_overlap_add_fwd(z.data_ptr(), y.data_ptr(), B, Bc, S, K, P, pl, frames, pitch, zp, st), "ctn_overlap_add_fwd")
         return y
 
     def forward(self, input):
@@ -266,7 +242,7 @@ class Separator(nn.Module):
         raise NotImplementedError("the stand-alone SepFormer Separator.forward (materialised mask) is not built; use SepFormer")
 
 
-class SepFormer(nn.Module):
+class SepFormer(GTUTailModel):
     pretrained_model_ids = {
         "wsj0-mix": {
             8000: {
@@ -324,48 +300,6 @@ class SepFormer(nn.Module):
         self.decoder = decoder
         self.math = None
 
-    def forward(self, input):
-        output, _ = self._run(input, want_latent=False)
-        return output
-
-    def extract_latent(self, input):
-        """input (batch_size, 1, T) -> output (batch_size, n_sources, T), latent (batch_size, n_sources, n_basis, T')"""
-        return self._run(input, want_latent=True)
-
-    def _run(self, input, want_latent):
-        if input.dim() != 3:
-            raise ValueError("input.size() is expected (?, 1, ?), but given {}".format(tuple(input.size())))
-        assert input.size(1) == 1, "input.size() is expected (?, 1, ?), but given {}".format(input.size())
-        _no_grad_check(self)
-        _dropout_check(self, self.sep_dropout)
-        sep = self.separator
-        B, _, T = input.shape
-        frames, pl, pr = N.frames_of(T, self.kernel_size, self.stride)
-        sep.segment_geometry(frames)  # too short / too long: ValueError before any device work
-        x = input.contiguous()
-        dev = N.require_cuda(x)
-        sep.math = self.math if self.math is not None else sep.math
-        pitch = N.ctn_pitch(frames)
-        st = N.stream_ptr(dev)
-        Nb, S = self.n_basis, self.n_sources
-        w = torch.empty(B, Nb, pitch, dtype=torch.float32, device=dev)
-        stats0 = torch.zeros(2 * B, dtype=torch.float64, device=dev)
-        N.check(N.ctn_encoder_fwd(x.data_ptr(), self.encoder.conv1d.weight.data_ptr(), w.data_ptr(), B, T, pl, pr, Nb, self.kernel_size,
-                                  self.stride, int(self.encoder.nonlinear), pitch, stats0.data_ptr(), st), "ctn_encoder_fwd")
-        y = sep.run_pitched(w, stats0, frames, pitch, dev)
-        out = torch.empty(B, S, T, dtype=torch.float32, device=dev)
-        latent = torch.empty(B, S, Nb, frames, dtype=torch.float32, device=dev) if want_latent else None
-        what = torch.empty(B, S * Nb, pitch, dtype=torch.float32, device=dev)
-        nws = N.ctn_sfm_tail_workspace_bytes(B, Nb, sep.bottleneck_channels, S, pitch)
-        base, nbytes = N.aligned(N.workspace(dev, nws + 256, tag="sfm_tail"))
-        N.check(N.ctn_sfm_tail_fwd(y.data_ptr(), w.data_ptr(), sep.prelu.weight.data_ptr(), sep.map.weight.data_ptr(), sep.map.bias.data_ptr(),
-                                   sep.gtu.map.weight.data_ptr(), sep.gtu.map.bias.data_ptr(), sep.gtu.map_gate.weight.data_ptr(),
-                                   sep.gtu.map_gate.bias.data_ptr(), sep.bottleneck_conv1d_out.weight.data_ptr(),
-                                   sep.bottleneck_conv1d_out.bias.data_ptr(), self.decoder.conv_transpose1d.weight.data_ptr(), out.data_ptr(),
-                                   N.ptr(latent), what.data_ptr(), B, Nb, sep.bottleneck_channels, S, frames, pitch, self.kernel_size,
-                                   self.stride, pl, T, int(sep.mask_relu), sep._math(), base, nbytes, st), "ctn_sfm_tail_fwd")
-        return out, latent
-
     def get_config(self):
         return {
             'in_channels': self.in_channels, 'n_basis': self.n_basis, 'kernel_size': self.kernel_size, 'stride': self.stride,
@@ -400,27 +334,5 @@ class SepFormer(nn.Module):
 
     @classmethod
     def build_from_pretrained(cls, root="./pretrained", quiet=False, load_state_dict=True, **kwargs):
-        """sepformer.py:229-269: resolve <root>/SepFormer/wsj0-mix/sr<rate>/<n>speakers/model/<choice>.pth like the reference and build
-        the model from it.  Nothing is downloaded: a missing file raises FileNotFoundError naming the expected path."""
-        task = kwargs.get('task')
-        if task not in cls.pretrained_model_ids:
-            raise KeyError("Invalid task ({}) is specified.".format(task))
-        if task not in ['wsj0-mix', 'wsj0']:
-            raise NotImplementedError("Not support task={}.".format(task))
-        sample_rate = kwargs.get('sample_rate') or 8000
-        n_sources = kwargs.get('n_sources') or 2
-        model_choice = kwargs.get('model_choice') or 'best'
-        model_id = cls.pretrained_model_ids[task][sample_rate][n_sources]
-        download_dir = os.path.join(root, cls.__name__, task, "sr{}/{}speakers".format(sample_rate, n_sources))
-        model_path = os.path.join(download_dir, "model", "{}.pth".format(model_choice))
-        if not os.path.exists(model_path):
-            raise FileNotFoundError("{} not found (Google-Drive id {!r}); place the reference checkpoint there -- this path loads "
-                                    "checkpoints, it does not download them".format(model_path, model_id))
-        model = cls.build_model(model_path, load_state_dict=load_state_dict)
-        for key, value in {'n_sources': n_sources, 'sample_rate': sample_rate}.items():
-            setattr(model, key, value)
-        return model
-
-    @property
-    def num_parameters(self):
-        return sum(p.numel() for p in self.parameters() if p.requires_grad)
+        """sepformer.py:229-269: <root>/SepFormer/wsj0-mix/sr<rate>/<n>speakers/model/<choice>.pth, loaded, never downloaded"""
+        return build_from_pretrained(cls, root, load_state_dict, **kwargs)

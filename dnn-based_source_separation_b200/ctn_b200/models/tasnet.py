@@ -11,18 +11,15 @@ Everything stays channel-first and pitched, (B, C, ctn_pitch(T')), between the s
 Envelope: rnn_type='lstm', monaural 3-D input, sep_hidden_channels up to ``ctn_tas_lstm_max_hidden`` of the device; forward only.
 A causal model with the plain encoder also streams: ``model.online(batch_size, max_chunk)`` (models/online.py).
 """
-import os
-
 import torch
 import torch.nn as nn
 
 from .. import _native as N
 from ..utils.filterbank import choose_filterbank
 from ..utils.model import choose_nonlinear
+from ._dual_path import build_from_pretrained, forward_only, math_of
 from .conv_tasnet import _load_checkpoint
 from .filterbank import GatedEncoder
-from .tdcn import resolve_math
-from . import tdcn as _tdcn
 
 EPS = 1e-12
 
@@ -188,8 +185,7 @@ class TasNet(nn.Module):
             raise NotImplementedError("in_channels={} (multichannel) is outside the sm_90a LSTM-TasNet path".format(self.in_channels))
         sep = self.separator
         sep.check_envelope()
-        if torch.is_grad_enabled() and (input.requires_grad or any(p.requires_grad for p in self.parameters())):
-            raise NotImplementedError("the LSTM-TasNet path is forward-only: call under torch.no_grad()")
+        forward_only(self, input)
         B, _, T = input.shape
         L, stride = self.kernel_size, self.stride
         padding = (stride - (T - L) % stride) % stride
@@ -200,7 +196,7 @@ class TasNet(nn.Module):
         sep.check_hidden()
         frames, pl, pr = N.frames_of(T, L, stride)
         pitch = N.ctn_pitch(frames)
-        math = resolve_math(self.math if self.math is not None else _tdcn.DEFAULT_MATH)
+        math = math_of(self.math)
         st = N.stream_ptr(dev)
         Nb, S = self.n_basis, self.n_sources
         w = torch.empty(B, Nb, pitch, dtype=torch.float32, device=dev)
@@ -260,26 +256,8 @@ class TasNet(nn.Module):
 
     @classmethod
     def build_from_pretrained(cls, root="./pretrained", quiet=False, load_state_dict=True, **kwargs):
-        """tasnet.py:227-267: resolve <root>/<class>/wsj0-mix/sr<rate>/<n>speakers/model/<choice>.pth like the reference and build the
-        model from it.  Nothing is downloaded: a missing file raises FileNotFoundError naming the expected path."""
-        task = kwargs.get('task')
-        if task not in cls.pretrained_model_ids:
-            raise KeyError("Invalid task ({}) is specified.".format(task))
-        if task not in ['wsj0-mix', 'wsj0']:
-            raise NotImplementedError("Not support task={}.".format(task))
-        sample_rate = kwargs.get('sample_rate') or 8000
-        n_sources = kwargs.get('n_sources') or 2
-        model_choice = kwargs.get('model_choice') or 'best'
-        model_id = cls.pretrained_model_ids[task][sample_rate][n_sources]
-        download_dir = os.path.join(root, cls.__name__, task, "sr{}/{}speakers".format(sample_rate, n_sources))
-        model_path = os.path.join(download_dir, "model", "{}.pth".format(model_choice))
-        if not os.path.exists(model_path):
-            raise FileNotFoundError("{} not found (Google-Drive id {!r}); place the reference checkpoint there -- this path loads "
-                                    "checkpoints, it does not download them".format(model_path, model_id))
-        model = cls.build_model(model_path, load_state_dict=load_state_dict)
-        for key, value in {'n_sources': n_sources, 'sample_rate': sample_rate}.items():
-            setattr(model, key, value)
-        return model
+        """tasnet.py:227-267: <root>/<class>/wsj0-mix/sr<rate>/<n>speakers/model/<choice>.pth, loaded, never downloaded"""
+        return build_from_pretrained(cls, root, load_state_dict, **kwargs)
 
     @property
     def num_parameters(self):

@@ -3,7 +3,8 @@
 Mirrors src/models/transform.py:6-65 of the reference (same constructors, same shapes): ``Segment1d`` turns
 (batch, features, frames) into (batch, features, S, chunk_size) with S = (frames - chunk_size) // hop_size + 1,
 ``OverlapAdd1d`` sums the overlapping chunks back into (batch, features, (S - 1) * hop_size + chunk_size).
-The DPRNN separator uses the same kernels with ``channels_last=1`` and the padding / crop fused in.
+The dual-path separators use the same entries with the padding / crop fused in: channels-last (``layout=1``: DPRNN, DPTNet,
+GALRNet) or channel-first with padded rows (``layout`` = the row pitch: SepFormer).
 """
 import torch
 import torch.nn as nn

@@ -270,17 +270,20 @@ int ctn_separator_fwd(const ctn_config_t* cfg, const ctn_params_t* params, const
  * Segment1d.forward, src/models/transform.py:15-29, fused with the zero padding of src/models/dprnn_tasnet.py:339-345:
  * x (B,F,pitch) with `frames` valid columns (pitch == frames for a contiguous tensor) -> chunks of `chunk_size` frames every
  * `hop_size` of the padded sequence, S = (frames + pad_left + pad_right - chunk_size) / hop_size + 1.
- * channels_last = 0: Z (B,F,S,chunk) -- the reference layout;  1: Z (B,S,chunk,F) -- the batch_first layout the intra-chunk
- * LSTM consumes, i.e. the permute of src/models/dprnn.py:83-84 folded in. */
-/* B <= 65535 (the batch is a grid axis): larger batches are refused with CTN_EUNSUPPORTED before any launch, here and in
- * ctn_overlap_add_fwd and ctn_dprnn_norm_res_fwd. */
+ * layout selects Z:  1 -- channels-last (B,S,chunk,F), the batch_first layout the intra-chunk LSTM consumes, i.e. the permute of
+ * src/models/dprnn.py:83-84 folded in;  0 -- the reference's (B,F,S,chunk);  any value >= S*chunk -- channel-first with padded rows,
+ * (B,F,layout) with token s*chunk + k for chunk s and frame k and columns [S*chunk, layout) written as 0 (SepFormer's dual-path state,
+ * layout = ctn_pitch(S*chunk)).  Every other value: CTN_EINVAL.  (With S*chunk = 1, 1 names both channels-last and rows of 1: the
+ * same memory.) */
+/* B <= 65535 (the batch is a grid axis of the channels-last kernels): larger batches are refused with CTN_EUNSUPPORTED before any
+ * launch, here and in ctn_overlap_add_fwd and ctn_dprnn_norm_res_fwd.  Any F.  1 launch. */
 int ctn_segment_fwd(const float* x, float* Z, int B, int F, int frames, int pitch, int chunk_size, int hop_size, int pad_left,
-                    int pad_right, int channels_last, ctn_stream_t stream);
+                    int pad_right, int layout, ctn_stream_t stream);
 /* OverlapAdd1d.forward, src/models/transform.py:46-62, fused with the crop of dprnn_tasnet.py:347: y (B,F,out_pitch),
- * y[..][t] = sum of the chunks covering padded frame t + crop_left, t < T_out; columns [T_out,out_pitch) = 0.
- * Z laid out as above (channels_last). */
+ * y[..][t] = sum of the chunks covering padded frame t + crop_left in ascending chunk order, t < T_out; columns [T_out,out_pitch) = 0.
+ * Z laid out as above (layout); the columns of a padded row past S*chunk are not read.  1 launch. */
 int ctn_overlap_add_fwd(const float* Z, float* y, int B, int F, int S, int chunk_size, int hop_size, int crop_left, int T_out,
-                        int out_pitch, int channels_last, ctn_stream_t stream);
+                        int out_pitch, int layout, ctn_stream_t stream);
 /* Tail of IntraChunkRNN / InterChunkRNN.forward, src/models/dprnn.py:87-94 / 140-148: out = gLN(Y; gamma, beta) + R on
  * channels-last tensors (B,D1,D2,F) (gLN = GroupNorm(1,F): per-sample statistics over D1*D2*F values).  swap = 1 stores out as
  * (B,D2,D1,F) -- the layout of the other path (the permutes of dprnn.py:83, 91, 136, 144-146).  scratch: double[B][2].  The
@@ -327,23 +330,30 @@ int ctn_mha_fwd(const float* z, int NSEQ, int T, int F, int heads, const float* 
  * fixed order: repeated calls give the same bits.  1 launch. */
 int ctn_seq_norm_fwd(const float* Y0, const float* Y1, const float* bias, const float* R, const float* gamma, const float* beta,
                      float* out, int B, int D1, int D2, int F, float eps, int swap, ctn_stream_t stream);
-/* Separator head, dptnet.py:334-337: z (B,S,chunk,Bc) = gLN(Segment1d(pad(Wb w + bb))) with the gLN per sample over the segmented
- * tensor (overlap duplicates and padding zeros included).  w (B,N,pitch) pitched, 16-byte aligned; S = (frames + pad_left +
- * pad_right - chunk) / hop + 1.  The 1x1 follows ctn_pw's numeric mode `math`.  workspace >= ctn_dpt_head_workspace_bytes(B, N, Bc,
- * pitch, S, chunk), 256-byte aligned.  Every refusal comes before the first launch. */
+/* Separator head, dptnet.py:334-337 and galrnet.py:233-239: z (B,S,chunk,Bc) = gLN(Segment1d(pad(Wb w + bb))) with the gLN per sample
+ * over the segmented tensor (overlap duplicates and padding zeros included).  bn_w = bn_b = NULL: no bottleneck (GALRNet), w itself is
+ * segmented and Bc must equal N.  w (B,N,pitch) pitched, 16-byte aligned; S = (frames + pad_left + pad_right - chunk) / hop + 1;
+ * B <= 65535.  The 1x1 follows ctn_pw's numeric mode `math`.  workspace >= ctn_dpt_head_workspace_bytes(B, N, Bc, pitch, S, chunk)
+ * (either case), 256-byte aligned.  Every refusal comes before the first launch.  Launches: 3, + 1 for the bottleneck (+ 1 weight-image
+ * launch outside the fp32 mode). */
 size_t ctn_dpt_head_workspace_bytes(int B, int N, int Bc, int pitch, int S, int chunk_size);
 int ctn_dpt_head_fwd(const float* w, const float* bn_w, const float* bn_b, const float* norm_g, const float* norm_b, float* z, int B,
                      int N, int Bc, int frames, int pitch, int chunk_size, int hop_size, int pad_left, int pad_right, float eps, int math,
                      void* workspace, size_t workspace_bytes, ctn_stream_t stream);
-/* Separator tail + decoder, dptnet.py:341-346 and 136-143: PReLU -> map 1x1 (Bc -> S*N) -> GTU1d per source (tanh(map) *
- * sigmoid(map_gate), N -> N, gtu.py:37-42) -> ReLU (mask_relu = 1) or sigmoid -> w * mask -> ConvTranspose1d -> crop.
- * y (B,Bc,pitch), w (B,N,pitch); out (B,S,T); latent nullable (B,S,N,frames); what (B,S*N,pitch) scratch; B*S <= 65535.
- * workspace >= ctn_dpt_tail_workspace_bytes(B,N,Bc,S,pitch), 256-byte aligned.  Every refusal comes before the first launch. */
-size_t ctn_dpt_tail_workspace_bytes(int B, int N, int Bc, int S, int pitch);
+/* Separator tail + decoder of DPTNet, GALRNet and SepFormer, dptnet.py:341-346, sepformer.py:353-359 and 136-143: PReLU -> map 1x1
+ * (Bc -> S*N) -> GTU1d per source (tanh(map) * sigmoid(map_gate), N -> N, gtu.py:37-42) [-> bottleneck_conv1d_out (N -> N, bias),
+ * SepFormer] -> ReLU (mask_relu = 1) or sigmoid -> w * mask -> ConvTranspose1d -> crop.  bout_w, bout_b: both or neither; without them
+ * the GTU, the mask and w * mask are one kernel.  y (B,Bc,pitch), w (B,N,pitch); out (B,S,T); latent nullable (B,S,N,frames);
+ * what (B,S*N,pitch) scratch; B*S <= 65535.  The weight images are built in one batch.  workspace >=
+ * ctn_dpt_tail_workspace_bytes(B,N,Bc,S,pitch,bout) with bout = 1 when bout_w is given, 256-byte aligned.  Every refusal comes before
+ * the first launch.  Launches: 4 + the decoder's without bout, 6 + the decoder's with it (+ 1 weight-image launch outside the fp32
+ * mode, + 1 with latent). */
+size_t ctn_dpt_tail_workspace_bytes(int B, int N, int Bc, int S, int pitch, int bout);
 int ctn_dpt_tail_fwd(const float* y, const float* w, const float* prelu, const float* map_w, const float* map_b, const float* gtu_w,
-                     const float* gtu_b, const float* gate_w, const float* gate_b, const float* dec_w, float* out, float* latent, float* what,
-                     int B, int N, int Bc, int S, int frames, int pitch, int L, int stride, int crop_left, int T, int mask_relu, int math,
-                     void* workspace, size_t workspace_bytes, ctn_stream_t stream);
+                     const float* gtu_b, const float* gate_w, const float* gate_b, const float* bout_w, const float* bout_b,
+                     const float* dec_w, float* out, float* latent, float* what, int B, int N, int Bc, int S, int frames, int pitch, int L,
+                     int stride, int crop_left, int T, int mask_relu, int math, void* workspace, size_t workspace_bytes,
+                     ctn_stream_t stream);
 /* Separator head on the padded layout, src/models/conv_tasnet.py:370-371 == src/models/dprnn_tasnet.py:335-336:
  * x0 (B,Bc,pitch) = Wb gLN(w) + bb; w (B,N,pitch), stats0 double[B][2] = (sum, sumsq) of w (as ctn_encoder_fwd leaves them).
  * workspace >= ctn_stage_workspace_bytes(Bc, N), 256-byte aligned; w and x0 16-byte aligned.  Every refusal comes before the first launch. */
@@ -365,14 +375,8 @@ int ctn_sep_tail_fwd(const float* y, const float* w, const float* prelu, const f
  * (ctn_pitch(S*C) in the model); columns [S*C, pitch) are zero wherever these entries write the state.  intra = 1 selects the
  * sequences of IntraTransformer (the C tokens of one chunk), intra = 0 those of InterTransformer (the S tokens of one frame, C apart).
  * Every entry refuses before its first launch and is CUDA-graph capturable.
- *
- * Segment1d / OverlapAdd1d on that layout (sepformer.py:348-352): Z (B,F,z_pitch), Z[b][f][s*C + k] = the zero-padded x at frame
- * s*hop + k - pad_left, columns [S*C, z_pitch) = 0; the overlap-add sums the chunks covering frame t + crop_left in ascending s into
- * y (B,F,out_pitch), columns [T_out, out_pitch) = 0.  1 launch each. */
-int ctn_sfm_segment_fwd(const float* x, float* Z, int B, int F, int frames, int pitch, int chunk_size, int hop_size, int pad_left,
-                        int pad_right, int z_pitch, ctn_stream_t stream);
-int ctn_sfm_overlap_add_fwd(const float* Z, float* y, int B, int F, int S, int chunk_size, int hop_size, int z_pitch, int crop_left,
-                            int T_out, int out_pitch, ctn_stream_t stream);
+ * Segmentation and overlap-add on that layout (sepformer.py:348-352) are ctn_segment_fwd / ctn_overlap_add_fwd with layout =
+ * ctn_pitch(S*C); the tail is ctn_dpt_tail_fwd with bottleneck_conv1d_out. */
 /* Scaled dot-product attention of nn.MultiheadAttention(F, heads) over every sequence of the path: qkv (B,3F,pitch) = the
  * in-projection WITHOUT its bias (as ctn_pw leaves it, channel-first), in_b (3F) added on load; O (B,F,pitch) receives the
  * concatenated heads before out_proj; its columns outside the sequences are not written.  Scale 1/sqrt(F/heads), online softmax
@@ -404,18 +408,6 @@ int ctn_sfm_pos_enc_fwd(const float* X, const float* pe, float* out, int B, int 
 size_t ctn_sfm_transformer_workspace_bytes(int B, int F, int d_ff, int layers, int pitch, int math);
 int ctn_sfm_transformer_fwd(const float* X, float* out, const float* const* w, int B, int F, int heads, int d_ff, int layers, int S, int C,
                             int pitch, int intra, float eps, int math, void* workspace, size_t workspace_bytes, ctn_stream_t stream);
-/* Separator tail + decoder, sepformer.py:353-359 and 142-155: PReLU -> map 1x1 (Bc -> S*N) -> GTU1d per source -> bottleneck_conv1d_out
- * (N -> N, bias) -> ReLU (mask_relu = 1) or sigmoid -> w * mask -> ConvTranspose1d -> crop.  y (B,Bc,pitch), w (B,N,pitch);
- * out (B,S,T); latent nullable (B,S,N,frames); what (B,S*N,pitch) scratch; B*S <= 65535.  The three weight images are built in one
- * batch.  workspace >= ctn_sfm_tail_workspace_bytes(B,N,Bc,S,pitch), 256-byte aligned.  Launches: 6 + the decoder's (+ 1 weight-image
- * launch outside the fp32 mode, + 1 with latent). */
-size_t ctn_sfm_tail_workspace_bytes(int B, int N, int Bc, int S, int pitch);
-int ctn_sfm_tail_fwd(const float* y, const float* w, const float* prelu, const float* map_w, const float* map_b, const float* gtu_w,
-                     const float* gtu_b, const float* gate_w, const float* gate_b, const float* bout_w, const float* bout_b,
-                     const float* dec_w, float* out, float* latent, float* what, int B, int N, int Bc, int S, int frames, int pitch, int L,
-                     int stride, int crop_left, int T, int mask_relu, int math, void* workspace, size_t workspace_bytes,
-                     ctn_stream_t stream);
-
 /* ---- LSTM-TasNet path (src/models/tasnet.py, csrc/ctn_tasnet.cu) ----
  *
  * GatedEncoder (filterbank.py:325-346) + the Separator's frame norm (tasnet.py:356-359): x (B,1,T) -> w (B,N,pitch) =
@@ -505,15 +497,8 @@ int ctn_tas_online_flush(const ctn_tas_config_t* cfg, void* state, int B, float*
 /* ---- GALRNet path (src/models/galrnet.py, src/models/galr.py, csrc/ctn_galr.cu) ----
  *
  * The dual-path state is channels-last, (B,S,K,F); the intra-chunk block is ctn_bilstm_proj_fwd + ctn_dprnn_norm_res2_fwd with
- * swap = 0, and the tail is ctn_dpt_tail_fwd with Bc = N.
- *
- * Separator head, galrnet.py:233-239: z (B,S,chunk,F) = gLN(Segment1d(pad(w))) with the gLN per sample over the segmented tensor
- * (overlap duplicates and padding zeros included), no bottleneck.  w (B,F,pitch) with `frames` valid columns; S = (frames +
- * pad_left + pad_right - chunk) / hop + 1.  workspace >= ctn_galr_head_workspace_bytes(B,S,chunk,F), 256-byte aligned.  Every
- * refusal comes before the first launch.  3 launches. */
-size_t ctn_galr_head_workspace_bytes(int B, int S, int chunk_size, int F);
-int ctn_galr_head_fwd(const float* w, const float* norm_g, const float* norm_b, float* z, int B, int F, int frames, int pitch, int chunk_size,
-                      int hop_size, int pad_left, int pad_right, float eps, void* workspace, size_t workspace_bytes, ctn_stream_t stream);
+ * swap = 0; the head is ctn_dpt_head_fwd without a bottleneck and the tail ctn_dpt_tail_fwd with Bc = N and without bout.
+ */
 /* LowDimensionGloballyAttentiveBlock.forward, galr.py:161-197, on x (B,S,K,F) channels-last -> out (B,S,K,F); out may alias x.
  * zt = LN_F(fc_map(x) along K) + pe, then y = MultiheadAttention(zt) over the S chunks of each of the B*Q down-sampled frames,
  * out = fc_inv(gLN(y + zt)) along Q + x with the gLN per sample over (Q,S,F).  map_w (Q,K), map_b (Q); ln_g, ln_b (F) of

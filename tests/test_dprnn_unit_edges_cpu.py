@@ -10,7 +10,7 @@ import torch
 import convtasnet_oracle as O
 import dprnn_oracle as DO
 import dprnn_unit_edges_ref as E
-from ctn_b200.models.dprnn_tasnet import Separator
+from ctn_b200.models.dprnn_tasnet import DPRNNTasNet, Separator
 
 GOLDEN = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden")
 
@@ -100,6 +100,14 @@ def test_segment_geometry_is_the_models():
     for K, P in ((12, 5), (250, 125)):
         assert {(r[2] - K) % P for r in rows.values() if (r[3], r[4]) == (K, P)} == set(range(P))
     assert E.segment_geometry(479999, 250, 125)[2] == 3839 and E.segment_geometry(79999, 250, 125)[2] == 639
+
+
+def test_forward_refusal_before_cuda():
+    """frozen weights and a CPU input that requires grad, under grad mode: the forward would record no graph, so it is refused"""
+    m = DPRNNTasNet(16, 4, enc_basis="trainable", dec_basis="trainable", enc_nonlinear=None, sep_hidden_channels=32,
+                    sep_bottleneck_channels=32, sep_chunk_size=8, sep_hop_size=4, sep_num_blocks=1, causal=False).requires_grad_(False)
+    with pytest.raises(NotImplementedError, match="forward-only"):
+        m(torch.randn(1, 1, 64, requires_grad=True))
 
 
 def test_model_rows_cover_every_padding_remainder():

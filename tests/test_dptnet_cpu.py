@@ -1,6 +1,8 @@
 """DPTNet without a GPU: the fp64 restatement against the reference's goldens, the module tree and state_dict keys, the
 config round trip, every envelope refusal (before any CUDA check), and the planted defects the GPU bound must reject."""
 import os
+import sys
+import types
 
 import pytest
 import torch
@@ -62,6 +64,19 @@ def test_build_model_round_trip(tmp_path):
         DPTNet.build_from_pretrained(root=str(tmp_path), task="musdb18")
 
 
+def test_build_from_pretrained_never_downloads(tmp_path, monkeypatch):
+    """a missing checkpoint names its path even where the reference's downloader is importable, and the downloader is not called"""
+    def download(*args, **kwargs):
+        pytest.fail("build_from_pretrained called a downloader")
+    utils = types.ModuleType("utils")
+    utils.utils = types.ModuleType("utils.utils")
+    utils.utils.download_pretrained_model_from_google_drive = download
+    monkeypatch.setitem(sys.modules, "utils", utils)
+    monkeypatch.setitem(sys.modules, "utils.utils", utils.utils)
+    with pytest.raises(FileNotFoundError, match=os.path.join("DPTNet", "wsj0-mix", "sr8000", "2speakers", "model", "best.pth")):
+        DPTNet.build_from_pretrained(root=str(tmp_path), task="wsj0-mix", n_sources=2)
+
+
 @pytest.mark.parametrize("over,exc", [
     (dict(causal=True), NotImplementedError),
     (dict(mask_nonlinear="softmax"), NotImplementedError),
@@ -94,6 +109,9 @@ def test_forward_refusals_before_cuda():
     x = g["x"]  # a CPU tensor: the refusals must fire before the CUDA check
     with pytest.raises(NotImplementedError, match="forward-only"):
         m(x)
+    frozen = make(g["cfg"]).requires_grad_(False)             # no parameter requires grad, the input does
+    with pytest.raises(NotImplementedError, match="forward-only"):
+        frozen(x.clone().requires_grad_())
     with torch.no_grad():
         with pytest.raises(ValueError):
             m(x[:, 0])

@@ -176,12 +176,12 @@ def test_model_scaled_inputs(scale):
     check(out, R.dptnet_fwd(x, sd, c))
 
 
-def test_model_launches():
+def test_model_launches_with_batched_tail_images():
     """per call: encoder 1; head 1x1 (+ its weight image outside fp32) + segment + 2; per block 2 x (3 + 1 + 2 + 1); overlap-add 1;
-    tail: PReLU 1, two 1x1 (+ weight images), GTU 1, decoder 1"""
+    tail: (its two weight images in one launch outside fp32) PReLU 1, two 1x1, GTU + mask 1, decoder 1"""
     m, sd, c = model_of("recipe_2spk")
     x = torch.randn(1, 1, 800, generator=torch.Generator().manual_seed(2)).to(DEV)
-    for math, pw in (("fp32", 1), ("tf32x3", 2)):
+    for math, img in (("fp32", 0), ("tf32x3", 1)):
         m.math = math
         with torch.no_grad():
             m(x)
@@ -189,5 +189,5 @@ def test_model_launches():
             m(x)
             n = N.ctn_total_launch_count() - n0
         dec = 1
-        expect = 1 + (pw + 1 + 2) + c["sep_num_blocks"] * 14 + 1 + (1 + 2 * pw + 1 + dec)
+        expect = 1 + (img + 1 + 1 + 2) + c["sep_num_blocks"] * 14 + 1 + (img + 1 + 2 + 1 + dec)
         assert n == expect, (math, n, expect)

@@ -97,7 +97,7 @@ TAIL = [(n_src, MODES[i], (n_src + i) % 2, i % 2) for n_src in (1, 2, 3, 4) for 
 
 
 @pytest.mark.parametrize("n_src,mode,mask_relu,latent", TAIL)
-def test_dpt_tail_against_fp64(n_src, mode, mask_relu, latent):
+def test_gtu_tail_without_bout_against_fp64(n_src, mode, mask_relu, latent):
     B, Nb, Bc, frames, L, stride, crop = 2, 64, 32, 37, 4, 2, 1
     pitch = N.ctn_pitch(frames)
     T = (frames - 1) * stride + L - 3                          # odd, and cropped on both sides
@@ -109,10 +109,11 @@ def test_dpt_tail_against_fp64(n_src, mode, mask_relu, latent):
     shapes = [(B, n_src, T), (B, n_src * Nb, pitch)] + ([(B, n_src, Nb, frames)] if latent else [])
 
     def run(o, base, nb):
-        return N.ctn_dpt_tail_fwd(yd.data_ptr(), wd.data_ptr(), *[d[k].data_ptr() for k in R.DPT_TAIL_ORDER], o[0].data_ptr(),
+        return N.ctn_dpt_tail_fwd(yd.data_ptr(), wd.data_ptr(), *[d[k].data_ptr() for k in R.DPT_TAIL_ORDER[:7]], None, None,
+                                  d["dec_w"].data_ptr(), o[0].data_ptr(),
                                   o[2].data_ptr() if latent else None, o[1].data_ptr(), B, Nb, Bc, n_src, frames, pitch, L, stride, crop,
                                   T, mask_relu, N.MATH_NAMES[mode], base, nb, st())
-    outs, _ = twice(run, shapes, N.ctn_dpt_tail_workspace_bytes(B, Nb, Bc, n_src, pitch))
+    outs, _ = twice(run, shapes, N.ctn_dpt_tail_workspace_bytes(B, Nb, Bc, n_src, pitch, 0))
     ref_out, ref_what = R.dpt_tail(y, w, p, n_src, mask_relu, stride, crop, T, frames)
     what = outs[1].reshape(B, n_src, Nb, pitch)
     assert not what[..., frames:].any()
@@ -123,24 +124,25 @@ def test_dpt_tail_against_fp64(n_src, mode, mask_relu, latent):
         assert torch.equal(outs[2], what[..., :frames])
 
 
-def test_dpt_tail_refuses_too_many_rows_before_launch():
+def test_gtu_tail_refuses_too_many_rows_before_launch():
     B, n_src, Nb, Bc, frames, L, stride = 16384, 4, 8, 8, 8, 2, 1  # B * n_src = 65536
     pitch = N.ctn_pitch(frames)
     T = (frames - 1) * stride + L
     y, w = torch.zeros(B, Bc, pitch, device=DEV), torch.zeros(B, Nb, pitch, device=DEV)
     out, what = torch.zeros(B, n_src, T, device=DEV), torch.zeros(B, n_src * Nb, pitch, device=DEV)
     p = {k: dev(v) for k, v in R.dpt_tail_params(Nb, Bc, n_src, L, 1).items()}
-    ws = torch.empty(N.ctn_dpt_tail_workspace_bytes(B, Nb, Bc, n_src, pitch) + 256, dtype=torch.uint8, device=DEV)
+    ws = torch.empty(N.ctn_dpt_tail_workspace_bytes(B, Nb, Bc, n_src, pitch, 0) + 256, dtype=torch.uint8, device=DEV)
     base, nb = N.aligned(ws)
     torch.cuda.synchronize()
     n0 = N.ctn_total_launch_count()
-    rc = N.ctn_dpt_tail_fwd(y.data_ptr(), w.data_ptr(), *[p[k].data_ptr() for k in R.DPT_TAIL_ORDER], out.data_ptr(), None, what.data_ptr(),
+    rc = N.ctn_dpt_tail_fwd(y.data_ptr(), w.data_ptr(), *[p[k].data_ptr() for k in R.DPT_TAIL_ORDER[:7]], None, None, p["dec_w"].data_ptr(),
+                            out.data_ptr(), None, what.data_ptr(),
                             B, Nb, Bc, n_src, frames, pitch, L, stride, 0, T, 1, N.MATH_NAMES["fp32"], base, nb, st())
     assert rc == N.CTN_EUNSUPPORTED
     assert N.ctn_total_launch_count() == n0
 
 
-# ---- ctn_sfm_segment_fwd / ctn_sfm_overlap_add_fwd ----------------------------------------------------------------------------------
+# ---- ctn_segment_fwd / ctn_overlap_add_fwd on SepFormer's pitched channel-first layout -----------------------------------------------
 def _ola_cases():
     cases = []
     for K, P in ((16, 8), (16, 16), (16, 5), (16, 24)):
@@ -149,7 +151,7 @@ def _ola_cases():
 
 
 @pytest.mark.parametrize("K,P,frames", _ola_cases())
-def test_sfm_segment_and_overlap_add_exact(K, P, frames):
+def test_pitched_segment_and_overlap_add_exact(K, P, frames):
     """segmentation is a copy: bit for bit; the overlap-add is the fp32 sum of the covering chunks in ascending s, from 0, which a
     CPU fp32 loop in the same order reproduces bit for bit"""
     B, Fc = 2, 8
@@ -158,15 +160,15 @@ def test_sfm_segment_and_overlap_add_exact(K, P, frames):
     zp = N.ctn_pitch(S * K)
     x = R.pitched(B, Fc, frames, pitch, frames, pad="random")    # the pad columns of x must not reach Z
     xd = dev(x)
-    (Z,), n = twice(lambda o, base, nb: N.ctn_sfm_segment_fwd(xd.data_ptr(), o[0].data_ptr(), B, Fc, frames, pitch, K, P, pl, pr, zp, st()),
+    (Z,), n = twice(lambda o, base, nb: N.ctn_segment_fwd(xd.data_ptr(), o[0].data_ptr(), B, Fc, frames, pitch, K, P, pl, pr, zp, st()),
                     [(B, Fc, zp)], 0)
     assert n == 1
     assert torch.equal(Z, R.sfm_segment(x[..., :frames], K, P, pl, pr, zp))
     Zin = torch.randn(B, Fc, zp, generator=torch.Generator().manual_seed(K + P))
     Zin[..., S * K:] = float("nan")                              # past the chunks: must not be read
     Zd = dev(Zin)
-    (y,), n = twice(lambda o, base, nb: N.ctn_sfm_overlap_add_fwd(Zd.data_ptr(), o[0].data_ptr(), B, Fc, S, K, P, zp, pl, frames, pitch,
-                                                                  st()), [(B, Fc, pitch)], 0)
+    (y,), n = twice(lambda o, base, nb: N.ctn_overlap_add_fwd(Zd.data_ptr(), o[0].data_ptr(), B, Fc, S, K, P, pl, frames, pitch, zp,
+                                                              st()), [(B, Fc, pitch)], 0)
     assert n == 1
     assert torch.equal(y, R.sfm_overlap_add(Zin, S, K, P, pl, frames, pitch))
 

@@ -1,5 +1,5 @@
 """GALRNet on the GPU against fp64 (tests/galrnet_ref.py) and the reference's goldens: the globally attentive block
-(``ctn_galr_inter_fwd``) and the separator head (``ctn_galr_head_fwd``) on their own, with outputs and workspaces pre-filled with
+(``ctn_galr_inter_fwd``) and the separator head (``ctn_dpt_head_fwd`` without a bottleneck) on their own, with outputs and workspaces pre-filled with
 NaN, across K, Q, S, F and B; digital silence; inputs scaled by 1e-3 and 1e3; the whole model in every 1x1 numeric mode at every
 padding remainder of the hop; a repeated call bit for bit; a CUDA-graph replay; the launches each call makes."""
 import os
@@ -141,7 +141,7 @@ def test_inter_block_grid_limit_refusals_before_launch():
 
 @pytest.mark.parametrize("B,F,frames,K,P", [(1, 64, 499, 100, 50), (3, 32, 16, 16, 8), (1, 128, 3999, 100, 50), (3, 64, 1000, 250, 125),
                                             (2, 64, 101, 100, 50)])
-def test_head_against_fp64(B, F, frames, K, P):
+def test_head_without_bottleneck_against_fp64(B, F, frames, K, P):
     pitch = N.ctn_pitch(frames)
     g = torch.Generator().manual_seed(frames)
     w = torch.zeros(B, F, pitch)
@@ -154,9 +154,9 @@ def test_head_against_fp64(B, F, frames, K, P):
     outs = []
     for _ in range(2):
         z = nan(B, S, K, F)
-        (base, nbytes), keep = nan_ws(N.ctn_galr_head_workspace_bytes(B, S, K, F))
-        N.check(N.ctn_galr_head_fwd(w.data_ptr(), gm.data_ptr(), bt.data_ptr(), z.data_ptr(), B, F, frames, pitch, K, P, pl, pr, EPS, base,
-                                    nbytes, st()), "ctn_galr_head_fwd")
+        (base, nbytes), keep = nan_ws(N.ctn_dpt_head_workspace_bytes(B, F, F, pitch, S, K))
+        N.check(N.ctn_dpt_head_fwd(w.data_ptr(), None, None, gm.data_ptr(), bt.data_ptr(), z.data_ptr(), B, F, F, frames, pitch, K, P, pl, pr,
+                                   EPS, N.MATH_NAMES["fp32"], base, nbytes, st()), "ctn_dpt_head_fwd")
         assert N.ctn_last_launch_count() == 3
         outs.append(z)
     torch.cuda.synchronize()
@@ -256,19 +256,19 @@ def test_repeated_call_is_bit_identical():
     assert torch.equal(a, b)
 
 
-def test_model_launches():
-    """per call: encoder 1; head 3; per block: intra bi-LSTM 2 + gLN and residual 2, inter 6; overlap-add 1; tail: PReLU 1, two 1x1
-    (+ their weight images outside fp32), GTU + mask 1, decoder 1"""
+def test_model_launches_with_batched_tail_images():
+    """per call: encoder 1; head 3; per block: intra bi-LSTM 2 + gLN and residual 2, inter 6; overlap-add 1; tail: (its two weight
+    images in one launch outside fp32) PReLU 1, two 1x1, GTU + mask 1, decoder 1"""
     m, _, c = model_of("recipe_2spk")
     x = torch.randn(1, 1, 4000, generator=torch.Generator().manual_seed(2)).to(DEV)
-    for math_, pw in (("fp32", 1), ("tf32x3", 2)):
+    for math_, img in (("fp32", 0), ("tf32x3", 1)):
         m.math = math_
         with torch.no_grad():
             m(x)
             n0 = N.ctn_total_launch_count()
             m(x)
             n = N.ctn_total_launch_count() - n0
-        expect = 1 + 3 + c["sep_num_blocks"] * (2 + 2 + 6) + 1 + (1 + 2 * pw + 1 + 1)
+        expect = 1 + 3 + c["sep_num_blocks"] * (2 + 2 + 6) + 1 + (img + 1 + 2 + 1 + 1)
         assert n == expect, (math_, n, expect)
 
 

@@ -120,6 +120,9 @@ def test_forward_refusals_before_cuda():
     x = g["x"]  # a CPU tensor: the refusals must fire before the CUDA check
     with pytest.raises(NotImplementedError, match="forward-only"):
         m(x)
+    frozen = make(g["cfg"]).eval().requires_grad_(False)      # no parameter requires grad, the input does
+    with pytest.raises(NotImplementedError, match="forward-only"):
+        frozen(x.clone().requires_grad_())
     with torch.no_grad():
         with pytest.raises(ValueError):
             m(x[:, 0])

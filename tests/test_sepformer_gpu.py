@@ -135,7 +135,7 @@ def test_seq_norm_residual_against_fp64(B, F, S, C, intra):
 
 
 @pytest.mark.parametrize("mask_relu,math_", [(1, "tf32x3"), (0, "fp32"), (1, "fp32")])
-def test_tail_against_fp64(mask_relu, math_):
+def test_gtu_tail_with_bout_against_fp64(mask_relu, math_):
     B, Nb, Bc, S, frames, L, stride = 2, 256, 256, 3, 300, 16, 8
     pitch = N.ctn_pitch(frames)
     keys = [("prelu", (1,)), ("map_w", (S * Nb, Bc)), ("map_b", (S * Nb,)), ("gtu_w", (Nb, Nb)), ("gtu_b", (Nb,)), ("gate_w", (Nb, Nb)),
@@ -146,10 +146,10 @@ def test_tail_against_fp64(mask_relu, math_):
     w = torch.relu(torch.randn(B, Nb, pitch, generator=g)).to(DEV)
     T = (frames - 1) * stride + L - 6
     out, latent, what = nan(B, S, T), nan(B, S, Nb, frames), nan(B, S * Nb, pitch)
-    (base, nbytes), keep = nan_ws(N.ctn_sfm_tail_workspace_bytes(B, Nb, Bc, S, pitch))
-    N.check(N.ctn_sfm_tail_fwd(y.data_ptr(), w.data_ptr(), *[p[k].data_ptr() for k, _ in keys], out.data_ptr(), latent.data_ptr(),
+    (base, nbytes), keep = nan_ws(N.ctn_dpt_tail_workspace_bytes(B, Nb, Bc, S, pitch, 1))
+    N.check(N.ctn_dpt_tail_fwd(y.data_ptr(), w.data_ptr(), *[p[k].data_ptr() for k, _ in keys], out.data_ptr(), latent.data_ptr(),
                                what.data_ptr(), B, Nb, Bc, S, frames, pitch, L, stride, 3, T, mask_relu, _mode(math_), base, nbytes, st()),
-            "ctn_sfm_tail_fwd")
+            "ctn_dpt_tail_fwd")
     assert N.ctn_last_launch_count() == (1 if math_ != "fp32" else 0) + 6 + 1 + 1
     torch.cuda.synchronize()
     d = {k: v.double().cpu() for k, v in p.items()}

@@ -439,12 +439,12 @@ def test_galr_inter_refusals_before_launch():
         assert N.ctn_last_launch_count() == 0
 
 
-# ---- the separator head (ctn_galr_head_fwd) ---------------------------------------------------------------------------------------------
+# ---- the separator head (ctn_dpt_head_fwd without a bottleneck) --------------------------------------------------------------------------
 HEAD_ROWS = E.head_rows()
 
 
 @pytest.mark.parametrize("name", list(HEAD_ROWS))
-def test_galr_head_entry(name):
+def test_galr_head_without_bottleneck_entry(name):
     r = HEAD_ROWS[name]
     B, F, frames, K, P = r["B"], r["F"], r["frames"], r["K"], r["P"]
     pitch = N.ctn_pitch(frames)
@@ -454,26 +454,26 @@ def test_galr_head_entry(name):
     sd = E.head_params(F, F + K)
     pl, pr, S = GR.segment_geometry(frames, K, P)
     wd, g, b = dev(w), dev(sd["separator.norm2d.norm.weight"]), dev(sd["separator.norm2d.norm.bias"])
-    (z,), n = twice(lambda o, base, nb: N.ctn_galr_head_fwd(wd.data_ptr(), g.data_ptr(), b.data_ptr(), o[0].data_ptr(), B, F, frames, pitch,
-                                                            K, P, pl, pr, 1e-12, base, nb, st()), [((B, S, K, F),)],
-                    N.ctn_galr_head_workspace_bytes(B, S, K, F))
+    (z,), n = twice(lambda o, base, nb: N.ctn_dpt_head_fwd(wd.data_ptr(), None, None, g.data_ptr(), b.data_ptr(), o[0].data_ptr(), B, F, F,
+                                                           frames, pitch, K, P, pl, pr, 1e-12, N.MATH_NAMES["fp32"], base, nb, st()),
+                    [((B, S, K, F),)], N.ctn_dpt_head_workspace_bytes(B, F, F, pitch, S, K))
     assert n == 3
     ref = GR.head(w[..., :frames].double(), sd, dict(sep_chunk_size=K, sep_hop_size=P, eps=1e-12))
     report("galr head", name, check(z, ref, 1))
 
 
-def test_galr_head_refuses_fewer_frames_than_the_chunk_before_launch():
+def test_head_without_bottleneck_refuses_fewer_frames_before_launch():
     """with a hop of 1 the padding rule adds nothing, so 11 frames cannot fill a chunk of 16"""
     B, F, frames, K, P = 1, 32, 11, 16, 1
     assert GR.segment_geometry(frames, K, P)[:2] == (0, 0)
     pitch = N.ctn_pitch(frames)
     w, z = torch.zeros(B, F, pitch, device=DEV), torch.zeros(B, 1, K, F, device=DEV)
     g = torch.ones(F, device=DEV)
-    ws = torch.empty(N.ctn_galr_head_workspace_bytes(B, 1, K, F) + 256, dtype=torch.uint8, device=DEV)
+    ws = torch.empty(N.ctn_dpt_head_workspace_bytes(B, F, F, pitch, 1, K) + 256, dtype=torch.uint8, device=DEV)
     base, nb = N.aligned(ws)
     torch.cuda.synchronize()
-    assert N.ctn_galr_head_fwd(w.data_ptr(), g.data_ptr(), g.data_ptr(), z.data_ptr(), B, F, frames, pitch, K, P, 0, 0, 1e-12, base, nb,
-                               st()) == N.CTN_EINVAL
+    assert N.ctn_dpt_head_fwd(w.data_ptr(), None, None, g.data_ptr(), g.data_ptr(), z.data_ptr(), B, F, F, frames, pitch, K, P, 0, 0, 1e-12,
+                              N.MATH_NAMES["fp32"], base, nb, st()) == N.CTN_EINVAL
     assert N.ctn_last_launch_count() == 0
 
 
